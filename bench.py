@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — headline benchmark of the GRU/BiLSTM hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]                  # this repo's CUDA path
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]  # this repo's CUDA path
     python bench.py --impl reference [--gpus N] [--steps K] [--warmup W]  # reference CPU path (oracle port)
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...      # one rank per GPU, NCCL
 
@@ -13,7 +13,7 @@ Workload (config.workload): ONE fuse_net_whole train step, reference semantics (
 
 One JSON line on stdout (rank 0): metric/value = sequences/s with inputs resident in HBM (CUDA-graph replay, CUDA
 events, max over ranks); e2e = same metric through the public API from pinned HOST buffers (H2D inside the timed
-region, loss read back); roofline = dominant kernel (GRU forward recurrence) vs the measured HBM peak;
+region, loss read back); roofline = dominant kernel (GRU forward recurrence) vs the HBM peak;
 cpu_baseline = the oracle port of the reference on this box's host cores; extra = fwd+bwd ms/batch of the
 BASELINE c2 / c3 module configs and the end-to-end fine-tune variant of the fuse step.
 """
@@ -52,9 +52,8 @@ def usable_cores() -> int:
 
 # The OpenMP pool must be sized BEFORE torch is imported: a plain `python bench.py` on the GPU box would otherwise
 # start os.cpu_count() = 128 intra-op threads inside a 16-core cgroup quota; after the first parallel host copy they
-# spin, the cgroup throttles the whole process and the launching thread with it (round-1 N=1 e2e: 1.21-1.36 ms/step
-# against 0.90 with OMP_NUM_THREADS=1, profiles/README.md). torchrun sets OMP_NUM_THREADS=1 itself, which is why
-# only the N=1 line showed it.
+# spin, and the cgroup throttles the whole process and the launching thread with it. torchrun sets OMP_NUM_THREADS=1
+# itself, which is why only single-process runs showed it.
 os.environ.setdefault("OMP_NUM_THREADS", str(usable_cores()))
 
 import torch  # noqa: E402
@@ -68,7 +67,7 @@ T_TEXT, E_TEXT, H_TEXT = 30, 1024, 128
 FUSE_ARGS = dict(text_embed_size=E_TEXT, text_hidden_dims=H_TEXT, rnn_layers=2, dropout=0.3, num_classes=2,
                  audio_hidden_dims=H_AUDIO, audio_embed_size=E_AUDIO)   # fuse_net_whole.py:398-414
 LR = 8e-6                                                               # fuse_net_whole.py:406, 416
-N_ROTATE = 4  # distinct resident input batches; 4 x 31.5 MB of inputs + per-step intermediates > 126 MB L2
+N_ROTATE = 4  # distinct resident input batches; 4 x 31.5 MB of inputs + per-step intermediates > 50 MB L2 (H100)
 
 
 _REAL_STDOUT_FD = None
@@ -100,7 +99,7 @@ def _peaks():
             p = json.load(fh)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+        return 3350.0, "NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
 
 
 def _config(n_gpus: int) -> dict:
@@ -112,7 +111,7 @@ def _config(n_gpus: int) -> dict:
         "global_batch": B_PER_GPU * n_gpus,
         "parallelism": f"dp{n_gpus}",
         "allreduce_bytes": 2 * (H_TEXT + H_AUDIO) * 4,
-        "l2": f"inputs rotate over {N_ROTATE} resident batches (working set > 126 MB L2); no explicit flush",
+        "l2": f"inputs rotate over {N_ROTATE} resident batches (working set > 50 MB L2); no explicit flush",
     }
 
 
@@ -532,13 +531,14 @@ def run_ours(args) -> None:
 
     # ---- capture one CUDA graph per resident input batch ---------------------------------------------
     graphs, use_graph = [], not args.no_graph
+    graph_out = []   # logits tensor of each captured step (lives in the graph pool, rewritten by every replay)
     if use_graph:
         try:
             pool = None
             for i in range(N_ROTATE):
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g, pool=pool):
-                    train_step(*dev_in[i])
+                    graph_out.append(train_step(*dev_in[i]))
                 pool = g.pool()
                 graphs.append(g)
         except Exception as exc:  # e.g. NCCL capture unsupported: fall back to eager launches
@@ -550,8 +550,8 @@ def run_ours(args) -> None:
     def run_step(i: int):
         if use_graph:
             graphs[i % N_ROTATE].replay()
-        else:
-            train_step(*dev_in[i % N_ROTATE])
+            return graph_out[i % N_ROTATE]
+        return train_step(*dev_in[i % N_ROTATE])
 
     _log(f"graphs captured: {use_graph}; launches/step {launches_per_step}")
     # ---- (A) device-resident throughput: W warm-up + exactly K timed steps ----------------------------
@@ -566,10 +566,12 @@ def run_ours(args) -> None:
     _barrier()
     e0.record()
     for i in range(K):
-        run_step(W + i)
+        last_out = run_step(W + i)
     e1.record()
     _barrier()
     ms_total = _max_over_ranks(e0.elapsed_time(e1), dev)
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(args.dump_outputs, {"logits": last_out, "loss": loss_buf})
     clocks = sampler.stop() if rank == 0 else None
     ms_per_step = ms_total / K
     value = B_PER_GPU * n_gpus * K / (ms_total * 1e-3)
@@ -762,26 +764,17 @@ def run_ours(args) -> None:
         alg_flops = 2 * B * T * 3 * H * H                       # recurrent contraction of this launch
         t_launch = rec_ms / max(rec_n, 1) * 1e-3
         achieved = alg_bytes / t_launch / 1e9
-        traffic = None   # dram bytes per launch from the committed ncu --set full capture of this kernel
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")) as fh:
-                traffic = json.load(fh)["r02_ncu_rec_fwd.csv"]["dram_bytes_per_launch"]
-        except Exception:
-            pass
         line["roofline"] = {
             "bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-            "traffic": traffic, "traffic_source": "profiles/r02_ncu_rec_fwd.csv (one ncu --set full capture of this kernel, "
-                                                  "cold L2: includes the x-projection read that is an L2 hit in the real "
-                                                  "step; a constant from that capture, not measured by this run)",
             "peak_source": peak_src,
             "kernel": "rec_fwd_kernel<GRU,H=256> (persistent cluster recurrence, one launch per layer)",
             "launch_ms": t_launch * 1e3, "launches_timed": rec_n,
             "algorithmic_bytes_per_launch": alg_bytes,
             "share_of_step": 2 * t_launch * 1e3 / ms_per_step,
             "note": "the recurrence is FFMA/shared-memory bound, not HBM bound (SURVEY.md §7): see ffma",
-            "ffma": {"achieved_tflops": alg_flops / t_launch / 1e12, "peak_tflops": 74.5,
-                     "frac": alg_flops / t_launch / 1e12 / 74.5,
-                     "peak_source": "148 SMs x 128 FMA x 2 x 1.965 GHz (nominal fp32)"},
+            "ffma": {"achieved_tflops": alg_flops / t_launch / 1e12, "peak_tflops": 67.0,
+                     "frac": alg_flops / t_launch / 1e12 / 67.0,
+                     "peak_source": "NVIDIA H100 SXM data sheet: 67 TFLOP/s fp32 at 700 W (not measured)"},
             "gemm_ms_per_launch": gemm_ms / max(gemm_n, 1),
         }
         # ---- secondary module configs (fwd+bwd ms/batch) and the end-to-end fine-tune variant -----------
@@ -808,6 +801,18 @@ def run_ours(args) -> None:
         _emit(line)
     pf_graphs.clear()
     _teardown(graphs, e2e_graphs, world, fused)
+
+
+def _dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write each tensor as out_dir/<name>.npy in float32, so that two builds can be compared output for output (the
+    inputs, weights and dropout streams of a run depend only on the fixed seeds above)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+    _log(f"outputs of the last timed step written to {out_dir}: {sorted(arrays)}")
 
 
 def _teardown(graphs, e2e_graphs, world: int, fused=None) -> None:
@@ -887,7 +892,7 @@ def _finetune_variant(dev, world: int, iters: int = 20, warmup: int = 5) -> dict
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=200, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--no-graph", action="store_true", help="launch every step eagerly (no CUDA graph)")
@@ -903,7 +908,11 @@ def main() -> None:
                     help="data-parallel gradient exchange of the fused step: in-kernel NVLink peer stores (peer: wait at "
                          "the end of the step; peer_async: send now, sum + Adam at the start of the next step beside "
                          "the encoders, flushed after the last step) or NCCL")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (logits, loss) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     _protect_stdout()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-"""b200rnn — B200-native (sm_100a) GRU / BiLSTM sequence encoders behind the torch.nn.GRU / nn.LSTM API.
+"""b200rnn — H100-native (sm_90a) GRU / BiLSTM sequence encoders behind the torch.nn.GRU / nn.LSTM API.
 
 The one hot path of speechandlanguageprocessing/ICASSP2022-Depression (SURVEY.md §8), rebuilt from scratch:
 PyTorch host code -> C-ABI shared library (include/b200rnn.h) -> hand-written CUDA kernels.

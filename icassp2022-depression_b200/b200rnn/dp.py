@@ -3,9 +3,9 @@ sequences sharded over ranks, and exactly ONE all-reduce per step over a single 
 
 The reference has no distributed code at all; this is the one parallel axis the hot path offers (independent
 sequences). Gradients of every trainable parameter are views into one contiguous buffer: the wgrad GEMMs of the
-B200 GRU/LSTM write straight into those views (``B200RNN_FLAG_ACCUMULATE_GRADS``), PyTorch's autograd accumulates
+b200rnn GRU/LSTM write straight into those views (``B200RNN_FLAG_ACCUMULATE_GRADS``), PyTorch's autograd accumulates
 the dense shells' gradients into them in place, and ``all_reduce`` consumes the buffer as is — no pack kernel.
-Backend: NCCL over NVLink 5 / NVSwitch on the GPU box, gloo in the CPU tests.
+Backend: NCCL over NVLink / NVSwitch between the GPUs of one machine, gloo in the CPU tests.
 """
 from __future__ import annotations
 

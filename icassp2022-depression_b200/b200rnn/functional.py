@@ -31,7 +31,7 @@ class RNNConfig:
 def _require_cuda_f32(t: torch.Tensor, name: str) -> None:
     if not t.is_cuda:
         raise _lib.B200RNNError(
-            f"b200rnn: {name} is on {t.device}; this library runs on CUDA (sm_100a) only and has no CPU path"
+            f"b200rnn: {name} is on {t.device}; this library runs on CUDA (sm_90a) only and has no CPU path"
         )
     if t.dtype != torch.float32:
         raise _lib.B200RNNError(f"b200rnn: {name} must be float32 (got {t.dtype})")

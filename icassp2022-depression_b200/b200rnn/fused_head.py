@@ -256,7 +256,7 @@ class FusedFuseStep:
         """The two independent encoder branches (fuse_net_whole.py:347 text BiLSTM, :361 audio GRU). With
         ``concurrent_branches`` the audio branch - the critical path, 2 x 120 serial steps - is enqueued on a second,
         high-priority stream (fork / join by events, captured as parallel branches of the CUDA graph): its persistent
-        recurrence occupies 128 of the 148 SMs for most of the step, the text kernels fill the rest instead of
+        recurrence occupies most of the 132 SMs for most of the step, the text kernels fill the rest instead of
         waiting behind it. ``text_stage(seq, h_n)`` (the text half of the head kernel) runs on the text stream before
         the join, i.e. off the critical path."""
         dev = batch.text.device

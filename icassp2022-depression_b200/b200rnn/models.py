@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's model classes for the hot path, built on the B200 GRU / LSTM.
+"""Host-side mirror of the reference's model classes for the hot path, built on the b200rnn GRU / LSTM.
 
 Same class names, constructor arguments, attribute / state-dict key names and ``forward`` semantics as
 

@@ -1,4 +1,4 @@
-"""Drop-in ``nn.Module`` mirrors of ``torch.nn.GRU`` / ``torch.nn.LSTM`` backed by the sm_100a kernels.
+"""Drop-in ``nn.Module`` mirrors of ``torch.nn.GRU`` / ``torch.nn.LSTM`` backed by the sm_90a kernels.
 
 They keep the constructor signature, parameter names / shapes / registration order
 (``weight_ih_l{k}[_reverse]``, ``weight_hh_...``, ``bias_ih_...``, ``bias_hh_...``; torch rnn.py:171-216), the
@@ -213,7 +213,7 @@ class _B200RNNBase(nn.Module):
 
 
 class GRU(_B200RNNBase):
-    """``torch.nn.GRU`` (gate order r,z,n; rnn.py:1221-1224) on hand-written sm_100a kernels."""
+    """``torch.nn.GRU`` (gate order r,z,n; rnn.py:1221-1224) on hand-written sm_90a kernels."""
 
     _mode = _lib.GRU
     _gates = 3
@@ -224,7 +224,7 @@ class GRU(_B200RNNBase):
 
 
 class LSTM(_B200RNNBase):
-    """``torch.nn.LSTM`` (gate order i,f,g,o; rnn.py:842-847) on hand-written sm_100a kernels."""
+    """``torch.nn.LSTM`` (gate order i,f,g,o; rnn.py:842-847) on hand-written sm_90a kernels."""
 
     _mode = _lib.LSTM
     _gates = 4
@@ -235,7 +235,7 @@ class LSTM(_B200RNNBase):
 
 
 def install() -> None:
-    """Rebind ``torch.nn.GRU`` / ``torch.nn.LSTM`` so unmodified reference code builds the B200 modules."""
+    """Rebind ``torch.nn.GRU`` / ``torch.nn.LSTM`` so unmodified reference code builds the b200rnn modules."""
     nn.GRU = GRU
     nn.LSTM = LSTM
     torch.nn.modules.GRU = GRU
@@ -250,7 +250,7 @@ def uninstall() -> None:
 
 
 def from_torch(module: nn.Module) -> _B200RNNBase:
-    """Build the B200 twin of a stock ``nn.GRU`` / ``nn.LSTM`` and copy its parameters."""
+    """Build the b200rnn twin of a stock ``nn.GRU`` / ``nn.LSTM`` and copy its parameters."""
     if isinstance(module, _TORCH_GRU):
         cls = GRU
     elif isinstance(module, _TORCH_LSTM):

@@ -10,7 +10,7 @@ with ``criterion = nn.CrossEntropyLoss()`` applied to the model's *Softmax outpu
 :class:`TrainStep` runs exactly that sequence - gradient zeroing, forward, loss, backward (dx included: the loops set
 ``requires_grad`` on the input), one gradient all-reduce when data parallel, AdamW - as ONE CUDA graph:
 
-* the encoders are the B200 GRU / LSTM kernels (forward + BPTT), their weight gradients land directly in the flat
+* the encoders are the b200rnn GRU / LSTM kernels (forward + BPTT), their weight gradients land directly in the flat
   gradient bucket of :class:`b200rnn.FlatAdamW`;
 * Softmax + CrossEntropyLoss and its gradient are one kernel (``b200rnn_softmax_ce``) fed with the model's pre-softmax
   logits (``forward_logits``);

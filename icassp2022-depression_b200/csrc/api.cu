@@ -56,7 +56,7 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
     return B200RNN_ERR_INVALID;
   }
   if (d->hidden_size != 128 && d->hidden_size != 256) {
-    set_error("hidden_size %d unsupported: the sm_100a persistent kernels are built for 128 and 256",
+    set_error("hidden_size %d unsupported: the sm_90a persistent kernels are built for 128 and 256",
               d->hidden_size);
     return B200RNN_ERR_UNSUPPORTED;
   }
@@ -124,7 +124,7 @@ struct ScratchLayout {
   // backward
   size_t b_dgates[2], b_dghn[2], b_wt[2], b_bpart[2], b_dy, b_gemm;
   size_t b_gemm_bytes;
-  // tcgen05 backward GEMMs: dense TF32 hi/lo splits of the operands (hi at the offset, lo right behind it); the names
+  // tensor-core backward GEMMs: dense TF32 hi/lo splits of the operands (hi at the offset, lo right behind it); the names
   // keep their round-1 "T" although nothing is transposed any more (MN-major operands, gemm_tc.cu)
   size_t b_tc_dg, b_tc_dgT, b_tc_hnT, b_tc_xT, b_tc_yT, b_tc_wT, b_tc_part;
   size_t b_tc_part_bytes;
@@ -143,7 +143,7 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
     s->f_y[k] = off;
     off += align_up(d.TB * d.DH, ALIGN_F);
   }
-  // split operands (hi/lo) of the tcgen05 3xTF32 input projection
+  // split operands (hi/lo) of the tensor-core 3xTF32 input projection
   {
     const int Kmax = d.I > (int)d.DH ? d.I : (int)d.DH;
     s->f_tc = off;
@@ -565,7 +565,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
     // with the fused LayerNorm the layer-0 dgrad is d/dLN(x): it goes to scratch and through the LN backward below
     const bool ln_l0 = (l == 0) && fused_ln;
     const bool want_dx = (l > 0) || (dx != nullptr) || (ln_l0 && (dln_gamma || dln_beta));
-    // ---- tcgen05 3xTF32 path for the wgrad / dgrad GEMMs (falls back to the FFMA kernel per GEMM) -------------
+    // ---- tensor-core 3xTF32 path for the wgrad / dgrad GEMMs (falls back to the FFMA kernel per GEMM) -------------
     const long long ldk = sl.b_ldk;
     const bool tc_l = tc_available() && (Il % 128 == 0);
     // Operands whose contraction index (t,b) is their ROW index - X_l, dG, h_prev, dn*r - go to the tensor cores as
@@ -592,7 +592,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
         float* dGs = S + sl.b_tc_dg;   // [TB][GH] hi, then lo: MN-major A of the wgrads AND K-major A of the dgrad
         float* hnS = S + sl.b_tc_hnT;  // [TB][H]   (GRU: dn * r)
         const TcOperand opX{xS, xS + d.TB * (size_t)Il, (long long)Il, true};
-        // the tcgen05 epilogue stores float4: a gradient target that is not 16-byte aligned (a view into a caller's
+        // the tensor-core path needs 16-byte aligned outputs: a gradient target that is not 16-byte aligned (a view into a caller's
         // flat bucket behind an odd-sized tensor) takes the FFMA GEMM below instead of failing
         const bool tc_wih = dw_ih && aligned_to(dw_ih, 16), tc_whh = dw_hh && aligned_to(dw_hh, 16) && d.T > 1;
         float* Cx = nullptr;
@@ -765,7 +765,7 @@ B200RNN_API int b200rnn_gemm_f32(int M, int N, int K, const float* A, int64_t ld
   g.M = M; g.N = N; g.K = K;
   g.bias1 = bias;
   g.accumulate = accumulate;
-  g.tc_ws = scratch;  // used by the tcgen05 3xTF32 path when the problem is eligible and the buffer is large enough
+  g.tc_ws = scratch;  // used by the tensor-core 3xTF32 path when the problem is eligible and the buffer is large enough
   g.tc_ws_bytes = scratch_bytes;
   return launch_gemm(g, scratch, scratch_bytes, static_cast<cudaStream_t>(stream_));
 }

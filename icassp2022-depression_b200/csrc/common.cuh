@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for the b200rnn sm_100a kernels.
+// common.cuh — shared device/host helpers for the b200rnn sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,6 +26,8 @@ void count_launch(int n = 1);  // bumps the counter behind b200rnn_launch_count(
 // the CURRENT device ordinal, so a process that drives several GPUs (or a module living on cuda:1 while cuda:0 is the
 // process default) sets the attributes on each of them. The Python bridge makes the tensor's device current first.
 constexpr int MAX_DEVICES = 64;
+// SMs of an H100 SXM: sizes the grid-stride launches (one or a few waves) and fixed-order partial-sum buffers
+constexpr int NUM_SMS = 132;
 inline int current_device() {
   int d = 0;
   if (cudaGetDevice(&d) != cudaSuccess) {

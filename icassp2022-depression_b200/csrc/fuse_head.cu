@@ -8,10 +8,9 @@
 //   [data parallel] sum of that gradient over the ranks: one-shot NVLink exchange, peer stores + flags (below)
 //   torch.optim.Adam step on fc_final.0.weight                                          :416, 456
 //
-// Round 1 ran this as 7 launches (attention_pool, rng_next, 2x mlp_dropout, fuse_loss_grad, adam, adam_step) plus a
-// 3 KB ncclAllReduce and a 1/world scaling launch between the loss and Adam: ~135 us of latency-bound dwarfs per
-// step cold, ~105 us of NCCL launch latency at 8 GPUs (profiles/README.md). Here a CTA owns ROWS batch rows from the
-// LSTM output to its rows' loss and gradient contribution; the last CTA to finish (ticket counter) reduces the
+// As separate kernels this is 7 launches (attention_pool, rng_next, 2x mlp_dropout, fuse_loss_grad, adam, adam_step)
+// plus a 3 KB ncclAllReduce and a 1/world scaling launch between the loss and Adam, all latency-bound. Here a CTA owns
+// ROWS batch rows from the LSTM output to its rows' loss and gradient contribution; the last CTA to finish (ticket counter) reduces the
 // contributions in a fixed order, exchanges the 768-float gradient with the peer GPUs, and applies Adam.
 //
 // Peer exchange (world > 1): every rank owns a small receive buffer (b200rnn_comm_create) that its peers map through

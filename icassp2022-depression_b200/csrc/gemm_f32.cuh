@@ -19,7 +19,7 @@ struct GemmParams {
   const float* bias2;
   int bias2_n;
   int accumulate;
-  // optional workspace for the tcgen05 3xTF32 path (gemm_tc.cu); NULL => fp32 FFMA path
+  // optional workspace for the tensor-core 3xTF32 path (gemm_tc.cu); NULL => fp32 FFMA path
   void* tc_ws;
   size_t tc_ws_bytes;
   int tc_a_presplit;  // the A operand's hi/lo halves already sit at tc_ws (see tc_a_hi / tc_a_lo)
@@ -43,12 +43,12 @@ int launch_layernorm_bwd(const float* x, const RowMap& x_rows, const float* dy, 
                          float eps, float* dx, const RowMap& dx_rows, float* dgamma, float* dbeta, int accumulate,
                          float* part, cudaStream_t stream);
 
-// tcgen05 3xTF32 path: C = A[M,K] * B[N,K]^T + biases (both operands k-contiguous, K % 32 == 0, N % 128 == 0)
+// tensor-core (wgmma) 3xTF32 path: C = A[M,K] * B[N,K]^T + biases (both operands k-contiguous, K % 32 == 0, N % 128 == 0)
 size_t gemm_tc_scratch_bytes(int M, int N, int K);
 bool gemm_tc_eligible(const GemmParams& p, size_t ws_bytes);
 int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t stream);
 
-// Building blocks of the tcgen05 path for callers that manage the split operands themselves (backward pass).
+// Building blocks of the tensor-core path for callers that manage the split operands themselves (backward pass).
 struct TcOperand {
   const float* hi;
   const float* lo;

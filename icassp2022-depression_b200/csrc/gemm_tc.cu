@@ -1,25 +1,24 @@
-// gemm_tc.cu — tensor-core path of the time-parallel input projection (K1):
-//     C[M,N] = A[M,K] * W[N,K]^T + bias          fp32 in / fp32 out, 3xTF32 on tcgen05
+// gemm_tc.cu — tensor-core path of the time-parallel input projection (K1) and of the wgrad / dgrad GEMMs:
+//     C[M,N] = A[M,K] * W[N,K]^T + bias          fp32 in / fp32 out, 3xTF32 on Hopper wgmma
 //
 // The hidden x input gate contraction over ALL time steps at once is the one genuinely dense GEMM of the path
-// (M = B*T up to 15360, N = G*H, K = I), so it goes to the 5th-generation tensor cores — but the reference
-// arithmetic is fp32 (torch rnn.py:1221-1224 / :842-847) and parity is judged at 1e-5, which plain TF32
-// (10-bit mantissa) cannot hold. Each operand is therefore split x = hi + lo with hi = rna_tf32(x),
-// lo = x - hi (exact), and three MMAs accumulate hi*hi + lo*hi + hi*lo in the fp32 TMEM accumulator
-// (the dropped lo*lo term is ~2^-22 relative).
-// The tensor core adds into the fp32 TMEM accumulator with truncation (round toward zero), a bias of about half an
-// ulp per MMA that grows linearly with the number of MMAs chained on one accumulator (measured: 1.5e-5 abs at
-// K=1024 with a single accumulator). So the chain is cut: k-blocks go round-robin to NMAIN=3 accumulators for
-// hi*hi, the small cross terms get their own, and the epilogue adds the four with ordinary round-to-nearest fp32.
+// (M = B*T up to 15360, N = G*H, K = I), so it goes to the tensor cores — but the reference arithmetic is fp32
+// (torch rnn.py:1221-1224 / :842-847) and parity is judged at 1e-5, which plain TF32 (10-bit mantissa) cannot hold.
+// Each operand is therefore split x = hi + lo with hi = rna_tf32(x), lo = x - hi (exact), and three MMAs accumulate
+// hi*hi + lo*hi + hi*lo (the dropped lo*lo term is ~2^-22 relative).
+// The tensor core adds into its fp32 accumulator with truncation rather than round-to-nearest, a bias that grows with
+// the number of MMAs chained on one accumulator. So the chain is cut after every k-block (12 MMAs): the wgmma
+// accumulator restarts from zero and is added into a second register accumulator with ordinary round-to-nearest fp32.
 // Resulting error ~1e-6 relative to the largest output, same order as fp32 FFMA.
 //
-// Kernel anatomy (one 128x128 output tile per CTA, 256 threads):
-//   warp 0   : TMA producer  — cp.async.bulk.tensor 2-D tiles (128 rows x 32 fp32 = 128-byte swizzled rows) of
-//              A_hi, A_lo, W_hi, W_lo into a 3-stage shared-memory ring, mbarrier complete_tx
-//   warp 1   : MMA issuer    — one elected lane issues tcgen05.mma.cta_group::1.kind::tf32 (M128 N128 K8), 12 per
-//              stage, accumulator in TMEM; tcgen05.commit releases the stage / signals the epilogue
-//   warp 2   : TMEM allocator (128 columns) / deallocator
-//   warps 4-7: epilogue      — tcgen05.ld 32x32b.x16 -> registers, + folded biases, coalesced-per-row stores
+// Kernel anatomy (one 128x128 output tile per CTA and work item, 384 threads, persistent over the tiles):
+//   warpgroup 0   : producer — K-major operands (contraction index contiguous) arrive by TMA, 2-D tiles of
+//                   128 rows x 32 fp32 in the 128-byte swizzle wgmma reads; MN-major operands (contraction index = the
+//                   source's row index: dG, X, h_prev in the wgrads) are read with coalesced loads and written
+//                   transposed into the same swizzled K-major layout, since wgmma takes tf32 operands K-major only.
+//                   A 3-stage shared-memory ring (A_hi, A_lo, W_hi, W_lo per stage), mbarrier full/empty.
+//   warpgroups 1-2: consumers — 64 rows of the tile each: wgmma.m64n128k8.tf32 from shared-memory descriptors,
+//                   12 per stage, then the round-to-nearest flush and finally the epilogue (+ folded biases).
 #include <cuda.h>  // CUtensorMap types only; the encoder is fetched through cudaGetDriverEntryPoint
 #include <mutex>
 
@@ -32,13 +31,11 @@ namespace b200rnn {
 namespace {
 
 constexpr int BM = 128, BN = 128, BK = 32, STAGES = 3;
-constexpr int LNB_BLOCKS = 148 * 2;  // CTAs of the LayerNorm backward (per-CTA column partials, reduced in fixed order)
+constexpr int LNB_BLOCKS = NUM_SMS * 2;  // CTAs of the LayerNorm backward (per-CTA column partials, reduced in fixed order)
 constexpr int TILE_BYTES = BM * BK * 4;        // 16 KB, both A and W tiles (BM == BN)
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;    // A_hi, A_lo, W_hi, W_lo
-constexpr int TC_THREADS = 256;
-constexpr int TC_SMEM = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 128 /*barriers*/ + 2 * BN * 4 /*bias*/ + 64;
-constexpr int NMAIN = 3;                       // hi*hi accumulators (k-blocks round-robin), + 1 for the cross terms
-constexpr int TMEM_COLS = (NMAIN + 1) * BN;    // 512: the whole TMEM of the SM
+constexpr int TC_THREADS = 384;
+constexpr int TC_SMEM = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 128 /*barriers*/;
 
 // ---- PTX wrappers specific to this kernel -----------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
@@ -51,69 +48,48 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   ptx::smem_u32(bar))
+// raise the expected transaction bytes of the current phase without arriving
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(ptx::smem_u32(bar)), "r"(bytes)
                : "memory");
 }
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld_x16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 
-// shared-memory matrix descriptor: K-major tile, 128-byte swizzle, rows of 128 B, 8-row groups 1024 B apart
+// shared-memory matrix descriptor (sm_90): K-major tile, 128-byte swizzle, rows of 128 B, 8-row groups 1024 B apart
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address   [0,14)
-  d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major) = 1
-  d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                             // descriptor version 1 (sm_100)
-  d |= (uint64_t)2 << 61;                             // layout type: SWIZZLE_128B
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);  // start address        [0,14)
+  d |= (uint64_t)1 << 16;                       // leading byte offset  (unused for swizzled K-major)
+  d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset: 8 rows * 128 B
+  d |= (uint64_t)1 << 62;                       // layout type: SWIZZLE_128B
   return d;
 }
 
-// MN-major tile (the contraction index is the ROW index of the source matrix, e.g. dG [T*B, G*H] as the A operand of
-// dW = dG^T X). For 32-bit operands the only MN-major shared-memory layout tcgen05 accepts is "128-byte swizzle with
-// 32-byte atoms" (descriptor layout type 1; CUTLASS: Layout_MN_SW128_32B_Atom = Swizzle<2,5,2> on byte addresses):
-// rows of 32 floats of M/N (128 B), FOUR K rows per 512-byte atom, inside an atom the 32-byte chunks of a row are
-// XOR-ed with (row & 3) - exactly what a TMA box {32 floats, 32 rows} with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
-// deposits. Atoms along K are 512 B apart (SBO), the four 32-wide column blocks of a 128-wide tile 4 KB apart (LBO).
-// One MMA (K = 8) consumes two atoms along K; the next K step starts 1 KB further.
-__device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(4096 >> 4) << 16;  // leading byte offset: next 32-wide block along M/N
-  d |= (uint64_t)(512 >> 4) << 32;   // stride byte offset: next 4 K rows
-  d |= (uint64_t)1 << 46;            // descriptor version 1 (sm_100)
-  d |= (uint64_t)1 << 61;            // layout type: SWIZZLE_128B_BASE32B
-  return d;
+#define B200_ACC8(i) "+f"(d[i + 0]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                     "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64x128] (+)= A[64x8] * B[128x8]^T, tf32 operands from shared memory, fp32 accumulator in registers
+__device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t adesc, uint64_t bdesc, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : B200_ACC8(0), B200_ACC8(8), B200_ACC8(16), B200_ACC8(24), B200_ACC8(32), B200_ACC8(40), B200_ACC8(48),
+        B200_ACC8(56)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-
-// instruction descriptor: D=f32, A=B=tf32, both K-major, M=128, N=128, dense, no negate
-constexpr uint32_t IDESC_TF32_128x128 =
-    (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+#undef B200_ACC8
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accesses of the accumulator across the asynchronous MMA
+__device__ __forceinline__ void reg_fence(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 struct TcArgs {
   float* C;
@@ -123,18 +99,34 @@ struct TcArgs {
   const float* bias2;
   int bias2_n;
   int tiles_m, tiles_n;
-  int nmain;  // hi*hi accumulators in use (1..NMAIN): k-blocks go round-robin over them
-  int nsets;  // TMEM accumulator sets (2 when (nmain+1)*BN*2 <= 512: epilogue of tile i overlaps mainloop of i+1)
   int accumulate;   // C += result (splitk == 1 only)
   int a_mn, b_mn;   // operand is MN-major: source matrix [K rows][M or N contiguous] (wgrad / dgrad without transposes)
+  const float *a_hi, *a_lo, *b_hi, *b_lo;  // MN-major operands are read through these (K-major ones through TMA)
+  long long lda, ldb;
   int splitk;       // > 1: work item = (k-split, tile); raw partial sums go to partial[ks][M][N]
   int kb_per_split; // k-blocks per split
   float* partial;
 };
 
-// Persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ... (m fastest, so consecutive tiles of a CTA mostly
-// share their W tile rows in L2). Warp roles loop independently over the same tile sequence and meet only through
-// mbarriers: smem ring full/empty (TMA <-> MMA), TMEM set full/empty (MMA <-> epilogue).
+// One 128 x BK tile of an MN-major operand (src: [K rows][ext columns], leading dimension ld) into the K-major
+// 128-byte-swizzled layout: thread t owns tile row t (= source column c0 + t), its 32 k values go out as 8 float4
+// chunks, chunk j at ((j ^ (t & 7)) * 16) inside the 128-byte row. Rows / columns past the source read as zero.
+__device__ __forceinline__ void load_mn_tile(unsigned char* tile, const float* __restrict__ src, long long ld, int ext,
+                                             int K, int c0, int k0, int t) {
+  const int c = c0 + t;
+  float v[BK];
+#pragma unroll
+  for (int kk = 0; kk < BK; ++kk)
+    v[kk] = (c < ext && k0 + kk < K) ? __ldg(src + (long long)(k0 + kk) * ld + c) : 0.f;
+  unsigned char* row = tile + (t >> 3) * 1024 + (t & 7) * 128;
+#pragma unroll
+  for (int j = 0; j < BK / 4; ++j)
+    *reinterpret_cast<float4*>(row + ((j ^ (t & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+}
+
+// Persistent: each CTA walks work items blockIdx.x, +gridDim.x, ... (m fastest, so consecutive tiles of a CTA mostly
+// share their W tile rows in L2). Producer and consumers loop independently over the same item sequence and meet only
+// through the full / empty mbarriers of the shared-memory ring.
 __global__ void __launch_bounds__(TC_THREADS, 1)
     gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                        const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
@@ -144,189 +136,135 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   unsigned char* base = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * STAGE_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;   // [2]
-  uint64_t* tempty = tfull + 2;       // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 4);  // [2][BN] folded bias of the tile, per TMEM set
 
-  // canonical warp index: the shuffle makes it warp-uniform for the compiler, so the single-thread TMA / MMA issue
-  // loops below stay on the uniform datapath (no per-instruction R2UR broadcast loop around UTMALDG / UTCHMMA)
+  // canonical warp index: the shuffle makes it warp-uniform for the compiler, so the single-thread TMA issue stays on
+  // the uniform datapath (no per-instruction R2UR broadcast loop around UTMALDG)
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  const int nkb_total = (args.K + BK - 1) / BK;  // TMA zero-fills the K tail
+  const int nkb_total = (args.K + BK - 1) / BK;  // the K tail reads as zero
   const int ntiles = args.tiles_m * args.tiles_n;
   const int nitems = ntiles * args.splitk;
-  const int set_cols = (args.nmain + 1) * BN;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      ptx::mbar_init(&full[s], 1);
-      ptx::mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      ptx::mbar_init(&tfull[s], 1);
-      ptx::mbar_init(&tempty[s], 4);  // one arrival per epilogue warp
+      ptx::mbar_init(&full[s], 128);  // every producer thread, after its own stores
+      ptx::mbar_init(&empty[s], 8);   // one arrival per consumer warp
     }
     ptx::fence_mbar_init();
-    prefetch_tmap(&map_a_hi);
-    prefetch_tmap(&map_a_lo);
-    prefetch_tmap(&map_b_hi);
-    prefetch_tmap(&map_b_lo);
+    if (!args.a_mn) {
+      prefetch_tmap(&map_a_hi);
+      prefetch_tmap(&map_a_lo);
+    }
+    if (!args.b_mn) {
+      prefetch_tmap(&map_b_hi);
+      prefetch_tmap(&map_b_lo);
+    }
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(ptx::smem_u32(tmem_slot)),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
 
-  if (warp == 0) {
-    if (ptx::elect_one_sync()) {
-      int it = 0;  // running k-block counter across tiles (ring position)
-      for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-        const int tile = item % ntiles, ks = item / ntiles;
-        const int m0 = (tile % args.tiles_m) * BM, n0 = (tile / args.tiles_m) * BN;
-        const int kb0 = ks * args.kb_per_split;
-        const int kb1 = min(nkb_total, kb0 + args.kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          ptx::mbar_wait(&empty[s], ph ^ 1);
-          unsigned char* st = base + s * STAGE_BYTES;
-          ptx::mbar_arrive_expect_tx(&full[s], STAGE_BYTES);
-          if (args.a_mn) {  // four {32 floats of M, BK rows of K} boxes per split half
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              tma_load_2d(st + 0 * TILE_BYTES + j * 4096, &map_a_hi, m0 + 32 * j, kb * BK, &full[s]);
-              tma_load_2d(st + 1 * TILE_BYTES + j * 4096, &map_a_lo, m0 + 32 * j, kb * BK, &full[s]);
+  if (warp < 4) {
+    const int t = threadIdx.x;
+    const uint32_t tx = (args.a_mn ? 0u : 2u * TILE_BYTES) + (args.b_mn ? 0u : 2u * TILE_BYTES);
+    int it = 0;  // running k-block counter across items (ring position)
+    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+      const int tile = item % ntiles, ks = item / ntiles;
+      const int m0 = (tile % args.tiles_m) * BM, n0 = (tile / args.tiles_m) * BN;
+      const int kb0 = ks * args.kb_per_split;
+      const int kb1 = min(nkb_total, kb0 + args.kb_per_split);
+      for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        ptx::mbar_wait(&empty[s], ph ^ 1);
+        unsigned char* st = base + s * STAGE_BYTES;
+        if (warp == 0 && tx) {
+          if (ptx::elect_one_sync()) {
+            mbar_expect_tx(&full[s], tx);
+            if (!args.a_mn) {
+              tma_load_2d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0, &full[s]);
+              tma_load_2d(st + 1 * TILE_BYTES, &map_a_lo, kb * BK, m0, &full[s]);
             }
-          } else {
-            tma_load_2d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0, &full[s]);
-            tma_load_2d(st + 1 * TILE_BYTES, &map_a_lo, kb * BK, m0, &full[s]);
-          }
-          if (args.b_mn) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              tma_load_2d(st + 2 * TILE_BYTES + j * 4096, &map_b_hi, n0 + 32 * j, kb * BK, &full[s]);
-              tma_load_2d(st + 3 * TILE_BYTES + j * 4096, &map_b_lo, n0 + 32 * j, kb * BK, &full[s]);
+            if (!args.b_mn) {
+              tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * BK, n0, &full[s]);
+              tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
             }
-          } else {
-            tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * BK, n0, &full[s]);
-            tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
           }
+          __syncwarp();
         }
+        if (args.a_mn) {
+          load_mn_tile(st + 0 * TILE_BYTES, args.a_hi, args.lda, args.M, args.K, m0, kb * BK, t);
+          load_mn_tile(st + 1 * TILE_BYTES, args.a_lo, args.lda, args.M, args.K, m0, kb * BK, t);
+        }
+        if (args.b_mn) {
+          load_mn_tile(st + 2 * TILE_BYTES, args.b_hi, args.ldb, args.N, args.K, n0, kb * BK, t);
+          load_mn_tile(st + 3 * TILE_BYTES, args.b_lo, args.ldb, args.N, args.K, n0, kb * BK, t);
+        }
+        if (args.a_mn || args.b_mn) ptx::fence_proxy_async();  // generic stores -> visible to wgmma (async proxy)
+        ptx::mbar_arrive(&full[s]);
       }
     }
-  } else if (warp == 1) {
-    if (ptx::elect_one_sync()) {
-      int it = 0, ti = 0;
-      // instruction descriptor with the operands' major-ness (bit 15: A is MN-major, bit 16: B is MN-major)
-      const uint32_t idesc = IDESC_TF32_128x128 | (args.a_mn ? (1u << 15) : 0u) | (args.b_mn ? (1u << 16) : 0u);
-      for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++ti) {
-        const int nkb = min(nkb_total, (item / ntiles + 1) * args.kb_per_split) - (item / ntiles) * args.kb_per_split;
-        const int set = ti % args.nsets;
-        const uint32_t use = (uint32_t)(ti / args.nsets);  // how often this set has been used before
-        ptx::mbar_wait(&tempty[set], (use & 1) ^ 1);       // the epilogue has drained this set
-        tc_fence_after();
-        const uint32_t acc_set = tmem_base + (uint32_t)(set * set_cols);
-        const uint32_t acc_cross = acc_set + (uint32_t)(args.nmain * BN);
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          ptx::mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t st = ptx::smem_u32(base + s * STAGE_BYTES);
-          const uint64_t a_hi = args.a_mn ? make_mnmajor_sw128_desc(st + 0 * TILE_BYTES) : make_kmajor_sw128_desc(st + 0 * TILE_BYTES);
-          const uint64_t a_lo = args.a_mn ? make_mnmajor_sw128_desc(st + 1 * TILE_BYTES) : make_kmajor_sw128_desc(st + 1 * TILE_BYTES);
-          const uint64_t b_hi = args.b_mn ? make_mnmajor_sw128_desc(st + 2 * TILE_BYTES) : make_kmajor_sw128_desc(st + 2 * TILE_BYTES);
-          const uint64_t b_lo = args.b_mn ? make_mnmajor_sw128_desc(st + 3 * TILE_BYTES) : make_kmajor_sw128_desc(st + 3 * TILE_BYTES);
-          const uint32_t acc_main = acc_set + (uint32_t)((kb % args.nmain) * BN);
-          // K step of 8: K-major = 32 bytes further inside the swizzle atom; MN-major = the next 1 KB atom
-          const uint32_t a_step = args.a_mn ? (1024u >> 4) : (32u >> 4), b_step = args.b_mn ? (1024u >> 4) : (32u >> 4);
-#pragma unroll
-          for (int k = 0; k < BK / 8; ++k) {
-            const uint64_t adva = (uint64_t)(k * a_step), advb = (uint64_t)(k * b_step);
-            tc_mma_tf32(acc_cross, a_lo + adva, b_hi + advb, idesc, (kb | k) != 0 ? 1u : 0u);
-            tc_mma_tf32(acc_cross, a_hi + adva, b_lo + advb, idesc, 1u);
-            tc_mma_tf32(acc_main, a_hi + adva, b_hi + advb, idesc, (kb >= args.nmain || k != 0) ? 1u : 0u);
-          }
-          tc_commit(&empty[s]);  // implies tcgen05.fence::before_thread_sync
-        }
-        tc_commit(&tfull[set]);
-      }
-    }
-  } else if (warp >= 4) {
-    const int wq = warp & 3;  // TMEM lane quarter this warp may read
-    const int et = threadIdx.x - 128;  // 0..127
-    int ti = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++ti) {
+  } else {
+    const int wg = (threadIdx.x >> 7) - 1;   // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+    const int wq = warp & 3;                 // warp within the warpgroup: 16 accumulator rows each
+    int it = 0;
+    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       const int tile = item % ntiles, ks = item / ntiles;
       const int nkb = min(nkb_total, (ks + 1) * args.kb_per_split) - ks * args.kb_per_split;
       const int m0 = (tile % args.tiles_m) * BM, n0 = (tile / args.tiles_m) * BN;
-      const int set = ti % args.nsets;
-      const uint32_t use = (uint32_t)(ti / args.nsets);
-      // folded bias of this tile's columns -> smem (issued before waiting for the accumulator)
-      {
-        const int n = n0 + et;
-        float bv = 0.f;
-        if (args.splitk == 1) {
-          if (args.bias1) bv += __ldg(args.bias1 + n);
-          if (args.bias2 && n < args.bias2_n) bv += __ldg(args.bias2 + n);
+      float total[64], acc[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) total[i] = 0.f;
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        ptx::mbar_wait(&full[s], ph);
+        const uint32_t st = ptx::smem_u32(base + s * STAGE_BYTES);
+        const uint64_t a_hi = make_kmajor_sw128_desc(st + 0 * TILE_BYTES + wg * 8192);
+        const uint64_t a_lo = make_kmajor_sw128_desc(st + 1 * TILE_BYTES + wg * 8192);
+        const uint64_t b_hi = make_kmajor_sw128_desc(st + 2 * TILE_BYTES);
+        const uint64_t b_lo = make_kmajor_sw128_desc(st + 3 * TILE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 8; ++k) {
+          const uint64_t adv = (uint64_t)(k * (32 >> 4));  // K step of 8 tf32 = 32 bytes inside the swizzle atom
+          wgmma_tf32_m64n128k8(acc, a_lo + adv, b_hi + adv, k != 0);
+          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_lo + adv, 1);
+          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_hi + adv, 1);
         }
-        bias_s[set * BN + et] = bv;
+        wgmma_commit();
+        wgmma_wait0();
+        reg_fence(acc);
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty[s]);  // this warp's share of the stage has been read
+#pragma unroll
+        for (int i = 0; i < 64; ++i) total[i] += acc[i];
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // epilogue warps only
-      ptx::mbar_wait(&tfull[set], use & 1);
-      tc_fence_after();
-      const int row = m0 + wq * 32 + lane;
-      float* crow = (args.splitk > 1)
-                        ? args.partial + ((size_t)ks * args.M + (row < args.M ? row : 0)) * args.N + n0
-                        : args.C + args.c_rows.off(row < args.M ? row : 0) + n0;
-      const uint32_t lane_base = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(set * set_cols);
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        float v[16];
-        tc_ld_x16(lane_base + (uint32_t)(args.nmain * BN + c0), v);  // cross terms
-        for (int a = 0; a < args.nmain; ++a) {
-          if (a < nkb) {  // accumulator a was written (uniform condition)
-            float m[16];
-            tc_ld_x16(lane_base + (uint32_t)(a * BN + c0), m);
+      // accumulator fragment: element i sits at row 16 wq + lane/4 + 8 ((i/2) & 1), column 8 (i/4) + 2 (lane%4) + i%2
+      const int r0 = m0 + wg * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-            for (int e = 0; e < 16; ++e) v[e] += m[e];
-          }
-        }
-        if (row < args.M) {
-          const float4* bs = reinterpret_cast<const float4*>(&bias_s[set * BN + c0]);
-          float4* dst = reinterpret_cast<float4*>(crow + c0);
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (row >= args.M) continue;
+        float* crow = (args.splitk > 1) ? args.partial + ((size_t)ks * args.M + row) * args.N + n0
+                                        : args.C + args.c_rows.off(row) + n0;
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 bq = bs[q];
-            float4 o = make_float4(v[4 * q + 0] + bq.x, v[4 * q + 1] + bq.y, v[4 * q + 2] + bq.z, v[4 * q + 3] + bq.w);
-            if (args.accumulate && args.splitk == 1) {
-              const float4 old = dst[q];
-              o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
+        for (int q = 0; q < 16; ++q) {
+          const int col = 8 * q + 2 * (lane & 3);
+          float2 o = make_float2(total[4 * q + 2 * h], total[4 * q + 2 * h + 1]);
+          if (args.splitk == 1) {
+            const int n = n0 + col;
+            if (args.bias1) { o.x += __ldg(args.bias1 + n); o.y += __ldg(args.bias1 + n + 1); }
+            if (args.bias2) {
+              if (n < args.bias2_n) o.x += __ldg(args.bias2 + n);
+              if (n + 1 < args.bias2_n) o.y += __ldg(args.bias2 + n + 1);
             }
-            dst[q] = o;
+            if (args.accumulate) {
+              const float2 old = *reinterpret_cast<const float2*>(crow + col);
+              o.x += old.x; o.y += old.y;
+            }
           }
+          *reinterpret_cast<float2*>(crow + col) = o;
         }
-      }
-      // this warp is done reading the set: release it to the MMA issuer
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(ptx::smem_u32(&tempty[set])) : "memory");
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                 : "memory");
   }
 }
 
@@ -544,21 +482,6 @@ bool make_map(CUtensorMap* map, const float* ptr, int rows, int K, long long ld 
   return r == CUDA_SUCCESS;
 }
 
-// MN-major operand: dense row-major [Krows, MN] fp32 matrix (the contraction index is the row), box = [32 K rows,
-// 32 floats of M/N], 128-byte swizzle; rows beyond Krows and columns beyond MN read as zero
-bool make_map_mn(CUtensorMap* map, const float* ptr, int Krows, int MN, long long ld) {
-  EncodeTiledFn enc = get_encoder();
-  if (!enc) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)MN, (cuuint64_t)Krows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(float)};
-  cuuint32_t box[2] = {32u, (cuuint32_t)BK};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
-}
-
 bool tc_disabled() {
   static const bool off = getenv("B200RNN_NO_TC") != nullptr;
   return off;
@@ -583,7 +506,7 @@ int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, flo
   const bool vec = (reinterpret_cast<uintptr_t>(src) & 15u) == 0 && rows.s_outer % 4 == 0 && rows.s_inner % 4 == 0;
   size_t nv = (size_t)R * (Cc / 4);
   int blocks = (int)((nv + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
   if (blocks < 1) blocks = 1;
   ProfScope prof(PROF_MISC, stream);
   split_tf32_kernel<<<blocks, 256, 0, stream>>>(src, rows, R, Cc, hi, lo, vec ? 1 : 0);
@@ -606,7 +529,7 @@ int tc_layernorm_split(const float* src, const RowMap& rows, int R, int Cc, cons
     return B200RNN_ERR_UNSUPPORTED;
   }
   int blocks = (R + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
   ProfScope prof(PROF_MISC, stream);
   switch (Cc / 128) {  // instantiated widths: 128, 256, 512, 1024 (the reference normalises 256-d audio features)
     case 1: layernorm_split_kernel<1><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, hi, lo, out); break;
@@ -658,7 +581,7 @@ int launch_layernorm_bwd(const float* x, const RowMap& x_rows, const float* dy, 
   return B200RNN_OK;
 }
 
-// C[M,N] (+)= A[M,K] * B[N,K]^T (+ biases), operands already split into hi/lo K-major matrices.
+// C[M,N] (+)= A[M,K] * B[N,K]^T (+ biases), operands already split into hi/lo matrices (K- or MN-major).
 int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
                      const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
                      size_t splitk_ws_bytes, cudaStream_t stream) {
@@ -670,11 +593,10 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
     set_error("tc_gemm: output must be 16-byte aligned with row strides that are multiples of 4 floats");
     return B200RNN_ERR_UNSUPPORTED;
   }
-  CUtensorMap m_ahi, m_alo, m_bhi, m_blo;
-  const bool ok_a = A.mn ? (make_map_mn(&m_ahi, A.hi, K, M, A.ld) && make_map_mn(&m_alo, A.lo, K, M, A.ld))
-                         : (make_map(&m_ahi, A.hi, M, K, A.ld) && make_map(&m_alo, A.lo, M, K, A.ld));
-  const bool ok_b = B.mn ? (make_map_mn(&m_bhi, B.hi, K, N, B.ld) && make_map_mn(&m_blo, B.lo, K, N, B.ld))
-                         : (make_map(&m_bhi, B.hi, N, K, B.ld) && make_map(&m_blo, B.lo, N, K, B.ld));
+  // MN-major operands are read by the kernel's own loads: their tensor maps stay zero and unused
+  CUtensorMap m_ahi{}, m_alo{}, m_bhi{}, m_blo{};
+  const bool ok_a = A.mn || (make_map(&m_ahi, A.hi, M, K, A.ld) && make_map(&m_alo, A.lo, M, K, A.ld));
+  const bool ok_b = B.mn || (make_map(&m_bhi, B.hi, N, K, B.ld) && make_map(&m_blo, B.lo, N, K, B.ld));
   if (!ok_a || !ok_b) {
     set_error("tc_gemm: cuTensorMapEncodeTiled failed (operands must be 16-byte aligned, ld %% 4 == 0)");
     return B200RNN_ERR_CUDA;
@@ -689,7 +611,7 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
       attr_done[dev] = true;
     }
   }
-  int sms = 148;
+  int sms = NUM_SMS;
   {
     int dev = 0;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -701,6 +623,8 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
   a.accumulate = accumulate;
   a.a_mn = A.mn ? 1 : 0;
   a.b_mn = B.mn ? 1 : 0;
+  a.a_hi = A.hi; a.a_lo = A.lo; a.lda = A.ld;
+  a.b_hi = B.hi; a.b_lo = B.lo; a.ldb = B.ld;
   a.tiles_m = (M + BM - 1) / BM;
   a.tiles_n = N / BN;
   const int ntiles = a.tiles_m * a.tiles_n;
@@ -717,10 +641,6 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
   a.kb_per_split = (nkb + splitk - 1) / splitk;
   a.splitk = (nkb + a.kb_per_split - 1) / a.kb_per_split;
   a.partial = static_cast<float*>(splitk_ws);
-  a.nmain = (a.kb_per_split + 11) / 12;  // <= 12 k-blocks (48 hi*hi MMAs) chained per accumulator
-  if (a.nmain < 1) a.nmain = 1;
-  if (a.nmain > NMAIN) a.nmain = NMAIN;
-  a.nsets = ((a.nmain + 1) * BN * 2 <= TMEM_COLS) ? 2 : 1;
   const int nitems = ntiles * a.splitk;
   dim3 grid(nitems < sms ? nitems : sms, 1, 1);
   {
@@ -736,7 +656,7 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
 
 int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t stream) {
   if (!gemm_tc_eligible(p, ws_bytes)) {
-    set_error("gemm_tc: problem not eligible for the tcgen05 path");
+    set_error("gemm_tc: problem not eligible for the tensor-core path");
     return B200RNN_ERR_UNSUPPORTED;
   }
   float* a_hi = tc_a_hi(ws);

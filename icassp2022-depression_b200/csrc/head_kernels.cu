@@ -581,7 +581,7 @@ B200RNN_API int b200rnn_adamw(float* p, const float* g, float* m, float* v, floa
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (n > 0) {
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
     adam_kernel<<<blocks, 256, 0, st>>>(p, g, m, v, step, n, lr, beta1, beta2, eps, weight_decay, grad_scale);
     B200_CUDA_CHECK(cudaGetLastError());
     count_launch();

@@ -6,7 +6,6 @@ namespace b200rnn {
 
 namespace {
 
-constexpr int SMS = 148;
 
 // Inter-layer dropout, nn.GRU/nn.LSTM semantics (rnn.py:857-860, :1233-1236): Bernoulli(1-p) keep mask,
 // kept values scaled by 1/(1-p). One Philox call yields the mask of 4 consecutive elements.
@@ -120,7 +119,7 @@ int launch_dropout(const float* in, float* out, size_t n, float p, const uint64_
   const float scale = p < 1.f ? 1.f / (1.f - p) : 0.f;
   size_t nquad = (n + 3) / 4;
   int blocks = (int)((nquad + 255) / 256);
-  if (blocks > SMS * 8) blocks = SMS * 8;
+  if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
   dropout_kernel<<<blocks, 256, 0, stream>>>(in, out, n, p, scale, hdr, stream_id);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
@@ -137,7 +136,7 @@ int launch_dropout_split(const float* in, float* out, float* hi, float* lo, size
   const float scale = p < 1.f ? 1.f / (1.f - p) : 0.f;
   size_t nquad = n / 4;
   int blocks = (int)((nquad + 255) / 256);
-  if (blocks > SMS * 8) blocks = SMS * 8;
+  if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
   dropout_split_kernel<<<blocks, 256, 0, stream>>>(in, out, hi, lo, n, p, scale, hdr, stream_id);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();

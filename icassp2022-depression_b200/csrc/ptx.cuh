@@ -1,4 +1,4 @@
-// ptx.cuh — thin inline-PTX wrappers (sm_100a): mbarrier, TMA bulk copy, cluster barrier, DSMEM.
+// ptx.cuh — thin inline-PTX wrappers (sm_90a): mbarrier, TMA bulk copy, cluster barrier, DSMEM.
 #pragma once
 #include <stdint.h>
 
@@ -45,7 +45,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // one lane of the (fully converged) warp returns true; unlike `lane == 0` the compiler keeps the enclosed code on
-// the uniform datapath (tcgen05.mma / commit operands in uniform registers, no per-instruction broadcast loop)
+// the uniform datapath (TMA operands in uniform registers, no per-instruction broadcast loop)
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred = 0;
   asm volatile(

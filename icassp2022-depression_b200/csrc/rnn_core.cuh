@@ -124,10 +124,15 @@ __device__ __forceinline__ void dots_chunk(const float* __restrict__ W_s, int gr
   }
 }
 
-// Same chunk contraction on the packed-fp32 pipe of sm_100 (FFMA2, PTX fma.rn.f32x2): the accumulator of every
-// (row, batch) is a float2 holding the even-k and odd-k partial sums, so one instruction retires two FMAs and the
-// operands are the naturally 64-bit aligned halves of the 16-byte shared-memory loads. Halves the FMA issue slots
-// of the time loop; fold_pairs() adds the two halves before the butterfly.
+// Two independent round-to-nearest FMAs on the halves of a float2. sm_90 has no packed fp32 FMA, so this is two FFMA;
+// each half rounds exactly like fma.rn.f32, so the paired contractions below give the same bits as scalar FMA chains.
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+
+// Same chunk contraction with a float2 accumulator per (row, batch) holding the even-k and odd-k partial sums (two
+// independent FMA chains, operands are the naturally 64-bit aligned halves of the 16-byte shared-memory loads);
+// fold_pairs() adds the two halves before the butterfly.
 template <int NR, int RG, int KL, int UPL, int BS, int KLEN, int VSTRIDE>
 __device__ __forceinline__ void dots_chunk2(const float* __restrict__ W_s, int group_stride, int row0,
                                             const float (&wreg)[RG > 0 ? RG : 1][UPL][KLEN / KL],
@@ -155,8 +160,8 @@ __device__ __forceinline__ void dots_chunk2(const float* __restrict__ W_s, int g
 #pragma unroll
       for (int ab = 0; ab < BS; ++ab) {
         float2 a = acc[r][au][ab];
-        a = __ffma2_rn(make_float2(wv.x, wv.y), make_float2(hv[ab].x, hv[ab].y), a);
-        a = __ffma2_rn(make_float2(wv.z, wv.w), make_float2(hv[ab].z, hv[ab].w), a);
+        a = fma2_rn(make_float2(wv.x, wv.y), make_float2(hv[ab].x, hv[ab].y), a);
+        a = fma2_rn(make_float2(wv.z, wv.w), make_float2(hv[ab].z, hv[ab].w), a);
         acc[r][au][ab] = a;
       }
     }
@@ -174,11 +179,11 @@ __device__ __forceinline__ void fold_pairs(const float2 (&acc2)[NR][UPL][BS], fl
 }
 
 // ---- batch-paired packed contraction (forward GRU) --------------------------------------------------------------
-// dots_chunk2 pairs two k of ONE (row, batch) in an FFMA2, which costs a float2 accumulator per (row, batch) (96
-// registers for the GRU) and a pair fold before the butterfly. Pairing two BATCH rows instead makes both halves of the
-// float2 final outputs: half the accumulator registers, no fold, and the weight becomes a 32-bit operand broadcast to
-// both halves (ptxas emits `FFMA2 Rd, Rw.F32, Rh.F32x2, Rd.F32x2`). For that the two batch values of one k must be an
-// aligned 64-bit word in shared memory, so the state vector is kept in a paired layout:
+// dots_chunk2 pairs two k of ONE (row, batch), which costs a float2 accumulator per (row, batch) (96 registers for the
+// GRU) and a pair fold before the butterfly. Pairing two BATCH rows instead makes both halves of the float2 final
+// outputs: half the accumulator registers, no fold, and one weight serves both halves. For that the two batch values
+// of one k must be an aligned 64-bit word in shared memory (one 8-byte load), so the state vector is kept in a paired
+// layout:
 //   index(j, b) = ((((j / CW) * 4 + j % 4) * (BS/2) + b / 2) * KL + (j % CW) / 4) * 2 + b % 2,   CW = 4*KL
 // i.e. for a fixed (chunk, e = k % 4, batch pair) the KL k-lanes read KL consecutive 8-byte words (conflict free).
 // Slot am of a lane holds batch pair am ^ (q >> 1); the low bit of q is resolved by the last butterfly stage.
@@ -219,10 +224,10 @@ __device__ __forceinline__ void dots_chunk2b(const float* __restrict__ W_s, int 
 #pragma unroll
       for (int am = 0; am < NP; ++am) {
         float2 a = acc[r][au][am];
-        a = __ffma2_rn(make_float2(wv.x, wv.x), hp[0][am], a);
-        a = __ffma2_rn(make_float2(wv.y, wv.y), hp[1][am], a);
-        a = __ffma2_rn(make_float2(wv.z, wv.z), hp[2][am], a);
-        a = __ffma2_rn(make_float2(wv.w, wv.w), hp[3][am], a);
+        a = fma2_rn(make_float2(wv.x, wv.x), hp[0][am], a);
+        a = fma2_rn(make_float2(wv.y, wv.y), hp[1][am], a);
+        a = fma2_rn(make_float2(wv.z, wv.z), hp[2][am], a);
+        a = fma2_rn(make_float2(wv.w, wv.w), hp[3][am], a);
         acc[r][au][am] = a;
       }
     }

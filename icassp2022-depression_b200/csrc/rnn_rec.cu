@@ -1,4 +1,4 @@
-// rnn_rec.cu — persistent recurrence kernels for sm_100a (K2/K3 forward, K4/K5 backward).
+// rnn_rec.cu — persistent recurrence kernels for sm_90a (K2/K3 forward, K4/K5 backward).
 //
 // Replaces the T-serial inner loop the reference reaches through torch.nn.GRU / torch.nn.LSTM
 // (GRU cell equations torch/nn/modules/rnn.py:1221-1224, LSTM cell :842-847; call sites
@@ -18,7 +18,7 @@
 //   * batch slices are independent clusters: no grid-wide synchronisation anywhere.
 //
 // fp32 FFMA by choice: the per-step contraction is [BS x H] x [H x G*HS] with BS = 4..8 rows per CTA —
-// far too skinny for tcgen05 tiles, and parity is judged at 1e-5 against an fp32 reference.
+// far too skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference.
 #include <mutex>
 #include <stdlib.h>
 
@@ -31,12 +31,12 @@ namespace b200rnn {
 
 namespace {
 
-constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_100
+constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_90
 // The CTA's own state slice is delivered locally (st.shared + mbarrier.arrive per warp). -DB200RNN_SELF_VIA_CLUSTER
 // builds the round-1 behaviour (own slice through st.async like the peers'): compute-sanitizer's racecheck does not
 // model the ordering that inline-PTX mbarrier.arrive / try_wait give to ordinary shared-memory stores and flags every
 // local store / LDS pair of the default build, so the race-free evidence of the REST of the kernel is taken on that
-// build (profiles/README.md); the ordering argument for the local path is in allgather_units' comment.
+// build; the ordering argument for the local path is in allgather_units' comment.
 #ifdef B200RNN_SELF_VIA_CLUSTER
 constexpr bool kLocalSelf = false;
 #else
@@ -135,8 +135,7 @@ __device__ __forceinline__ void allgather_units(float val, float* vec_local, int
 // forward
 // =================================================================================================
 // VL = true: per-sequence lengths (PackedSequence semantics): past its length a sequence keeps its state and emits 0
-// PB = true: batch-paired FFMA2 contraction and state layout (rnn_core.cuh, dots_chunk2b); used where it measured
-// faster (GRU H=256 4-row clusters, LSTM H=256), see launch_rec_fwd
+// PB = true: batch-paired contraction and state layout (rnn_core.cuh, dots_chunk2b), see launch_rec_fwd
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false, bool PB = false>
 __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     rec_fwd_kernel(const RecFwdParams p, const int nslices) {
@@ -238,11 +237,9 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     long long* trow = p.trace + ((size_t)step * 8 + (w & 7)) * 8;
     if (tr) trow[0] = clock64();
 
-    // FFMA2 (two fp32 FMAs per issue slot) for the GRU only: k-paired (PACK2: float2 = even-k / odd-k partial sums of
-    // one output, folded before the butterfly) or batch-paired (PACKB: float2 = two batch rows of one unit, weight as
-    // a broadcast 32-bit operand, state kept in the paired shared-memory layout). Measured on the LSTM H=128 forward (same box, round 2):
-    // FFMA2 53.6 us vs scalar FFMA 49.5 us per layer - with three distinct 64-bit register operands an FFMA2 issues
-    // every 3 cycles (register-file bandwidth), and the 4-gate packed accumulators leave the scheduler less room
+    // float2 accumulators for the GRU only: k-paired (PACK2: float2 = even-k / odd-k partial sums of one output,
+    // folded before the butterfly) or batch-paired (PACKB: float2 = two batch rows of one unit, one weight for both,
+    // state kept in the paired shared-memory layout); the LSTM keeps scalar accumulators
     constexpr bool PACKB = PB;
     constexpr bool PACK2 = !PACKB && (MODE == B200RNN_GRU) && RG < 2;
     float2 acc2[PACK2 ? G : 1][UPL][BS];
@@ -553,8 +550,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     const uint32_t par = (step >> 1) & 1;
 
     // ---- dh_{prev}[b][j] = direct + sum_col dgh[b][col] * W_hh[col][j], one gate block of columns at a time ----
-    // FFMA2: even-k / odd-k partial sums in one float2 accumulator (one issue slot per two FMAs), folded before the
-    // butterfly - the scalar FFMA pipe retires one warp instruction per two cycles and SMSP
+    // even-k / odd-k partial sums in one float2 accumulator (two independent FMA chains), folded before the butterfly
     float2 acc2[1][UPL][BS];
     float acc[1][UPL][BS];
 #pragma unroll
@@ -664,7 +660,7 @@ int max_active_clusters(K kernel, int C, int NT, size_t smem) {
   }
   if (prepare_kernel(kernel, smem) != B200RNN_OK) return 0;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(C * 148), 1, 1);
+  cfg.gridDim = dim3((unsigned)(C * NUM_SMS), 1, 1);
   cfg.blockDim = dim3((unsigned)NT, 1, 1);
   cfg.dynamicSmemBytes = smem;
   cudaLaunchAttribute attr[1];
@@ -711,7 +707,7 @@ bool try_bwd(RecBwdParams& p, cudaStream_t s, bool force, int* rc) {
   if (!force && nclusters > max_active_clusters(k, C, Cfg::NT, Cfg::BWD_SMEM)) return false;
   // transposed, per-CTA contiguous copy of W_hh for this cluster width
   for (int d = 0; d < p.D; ++d) {
-    whh_prep_kernel<<<148, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], Cfg::G, H, C);
+    whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], Cfg::G, H, C);
     if (cudaGetLastError() != cudaSuccess) {
       set_error("whh_prep launch failed");
       *rc = B200RNN_ERR_CUDA;
@@ -729,13 +725,6 @@ int env_variant(const char* name, int dflt) {
   return v ? atoi(v) : dflt;
 }
 
-// Batch-size-aware dispatch (measured on one box, GRU H=256, T=120, per layer launch; profiles/README.md):
-//   B = 128 : FFMA <C=4,BS=4> 222 us (215 us with the batch-paired FFMA2 form) | tcgen05 recurrence 354 us
-//   B =  64 : FFMA <C=4,BS=4> 215 us (64 CTAs: 43 % of the chip) | FFMA <C=4,BS=2> 175 us (128 CTAs, half the FFMA per step)
-//   B <= 48 : FFMA <C=4,BS=4> 209 us | tcgen05 ~205-215 us | FFMA <C=4,BS=2> 170 us
-// so: clusters of 2 batch rows whenever they fit one wave (B <= ~72), clusters of 4 above, and the tensor-core
-// recurrence only when forced (B200RNN_REC_TC=1) - it is bound by the 8-CTA all-to-all of the state, not by math.
-bool rec_tc_preferred(const RecFwdParams&) { return false; }
 }  // namespace
 
 // smallest BS any backward config uses is 2
@@ -747,20 +736,15 @@ int rec_bwd_max_slices(int B) { return (B + 1) / 2; }
 int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
   int rc = B200RNN_OK;
   if (p.B <= 0 || p.T <= 0) return rc;
-  // The tcgen05 recurrence (rnn_rec_tc.cu) is parity-green but never the fastest choice any more (rec_tc_preferred());
-  // B200RNN_REC_TC=1 forces it (A/B runs, tests/test_gpu_tc_rec.py).
-  static const int rec_tc = env_variant("B200RNN_REC_TC", -1);
-  if ((rec_tc == 1 || (rec_tc < 0 && rec_tc_preferred(p))) && launch_rec_fwd_tc(p, s, &rc)) return rc;
-  // One tuned config per shape (B200, round-1/2 A/B runs in profiles/README.md) plus a wider-batch fallback that runs
-  // in several waves when the batch needs more clusters than fit the chip.
+  // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
+  // than fit the chip.
   if (p.mode == B200RNN_GRU && p.H == 256) {
-    // half-filled chip (B <= 74, e.g. BASELINE c2 with B = 64): clusters of 2 batch rows use twice the SMs with half the
-    // FFMA work per step (all three gate blocks in shared memory, 4 warps per CTA)
+    // half-filled chip (e.g. BASELINE c2 with B = 64): clusters of 2 batch rows use twice the SMs with half the FFMA
+    // work per step (all three gate blocks in shared memory, 4 warps per CTA); taken only while every cluster is
+    // co-resident (try_fwd checks the occupancy)
     static const int bs2 = env_variant("B200RNN_GRU_BS2", 1);  // =0: A/B switch
-    if (bs2 && p.B <= 74 && try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
-    // batch-paired FFMA2 (rnn_core.cuh dots_chunk2b): 215 us at B=128, T=120 against 222 us for the k-paired form on
-    // the same box. The same change measured SLOWER for the 2-row clusters (0.408 vs 0.397 ms per 2-layer forward at
-    // B=64) and with two gate blocks in registers (0.549 vs 0.539 ms), so only this config uses it.
+    if (bs2 && p.B <= 2 * (NUM_SMS / 4) && try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
+    // batch-paired contraction (rnn_core.cuh dots_chunk2b): half the accumulator registers of the k-paired form
     if (try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, false, &rc)) return rc;
     try_fwd<B200RNN_GRU, 256, 8, 8, 32, 4, 1>(p, s, true, &rc);
     return rc;
@@ -771,13 +755,13 @@ int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
     return rc;
   }
   if (p.mode == B200RNN_LSTM && p.H == 256) {
-    // batch-paired FFMA2: 0.238 vs 0.242 ms per 2-layer BiLSTM forward (B=64, T=30) for the scalar-FFMA form
-    if (try_fwd<B200RNN_LSTM, 256, 4, 4, 16, 4, 1, true>(p, s, false, &rc)) return rc;
+    // scalar FFMA: the batch-paired form needs more registers than sm_90 leaves this config (it spills)
+    if (try_fwd<B200RNN_LSTM, 256, 4, 4, 16, 4, 1>(p, s, false, &rc)) return rc;
     try_fwd<B200RNN_LSTM, 256, 8, 8, 16, 2, 1>(p, s, true, &rc);
     return rc;
   }
   if (p.mode == B200RNN_LSTM && p.H == 128) {
-    // scalar FFMA: the batch-paired FFMA2 form measured 0.185 vs 0.180 ms per 2-layer BiLSTM forward (B=128, T=30)
+    // scalar FFMA
     if (try_fwd<B200RNN_LSTM, 128, 2, 4, 16, 4, 1>(p, s, false, &rc)) return rc;
     try_fwd<B200RNN_LSTM, 128, 4, 8, 16, 2, 1>(p, s, true, &rc);
     return rc;
@@ -791,10 +775,10 @@ int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
   int rc = B200RNN_OK;
   if (p.B <= 0 || p.T <= 0) return rc;
   // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
-  // (not the weights) dominates the shared-memory traffic of the backward contraction: 303 -> 278 us (GRU H=256)
+  // (not the weights) dominates the shared-memory traffic of the backward contraction
   if (p.mode == B200RNN_GRU && p.H == 256) {
     static const int bs2 = env_variant("B200RNN_GRU_BS2", 1);
-    if (bs2 && p.B <= 74 && try_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
+    if (bs2 && p.B <= 2 * (NUM_SMS / 4) && try_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
     if (try_bwd<B200RNN_GRU, 256, 4, 4, 32, 8, 1>(p, s, false, &rc)) return rc;
     try_bwd<B200RNN_GRU, 256, 8, 8, 32, 4, 1>(p, s, true, &rc);
     return rc;

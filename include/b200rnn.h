@@ -1,5 +1,5 @@
 /*
- * b200rnn.h — C-ABI of the B200-native GRU / (Bi)LSTM sequence-encoder library.
+ * b200rnn.h — C-ABI of the H100-native GRU / (Bi)LSTM sequence-encoder library.
  *
  * This is the drop-in boundary for the ONE hot path of
  * speechandlanguageprocessing/ICASSP2022-Depression: the multi-layer torch.nn.GRU /
@@ -45,7 +45,7 @@ enum { B200RNN_GRU = 0, B200RNN_LSTM = 1 };
 enum {
   B200RNN_OK = 0,
   B200RNN_ERR_INVALID = -1,     /* bad descriptor / null pointer / misaligned buffer        */
-  B200RNN_ERR_UNSUPPORTED = -2, /* shape outside what the sm_100a kernels are built for     */
+  B200RNN_ERR_UNSUPPORTED = -2, /* shape outside what the sm_90a kernels are built for      */
   B200RNN_ERR_CUDA = -3         /* a CUDA runtime call failed (message has cudaGetErrorString) */
 };
 
@@ -82,7 +82,7 @@ B200RNN_API const char* b200rnn_last_error(void);
 /* Kernels this library has launched in this process so far (captured launches count once per capture). */
 B200RNN_API unsigned long long b200rnn_launch_count(void);
 
-/* Number of SMs of the current device as seen by the library (148 on B200); <0 on error. */
+/* Number of SMs of the current device as seen by the library (132 on H100 SXM); <0 on error. */
 B200RNN_API int b200rnn_sm_count(void);
 
 /*

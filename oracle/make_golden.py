@@ -1,6 +1,6 @@
-"""ORACLE tooling — generates tests/golden/*.npz from the REFERENCE's own classes (run in the build container).
+"""ORACLE tooling — generates tests/golden/*.npz from the REFERENCE's own classes.
 
-    python oracle/make_golden.py            # needs /root/reference; writes tests/golden/
+    python oracle/make_golden.py            # needs the reference checkout (oracle/ast_loader.py); writes tests/golden/
 
 Each fixture is produced by executing the reference ``ClassDef``s (oracle/ast_loader.py) on CPU with torch
 {torch_version}; weights and inputs are regenerated from names (oracle/params.py), so a fixture holds only small
@@ -133,9 +133,33 @@ def fuse(case: str, key: str, regression: bool, B: int, T: int) -> None:
                              torch=torch.__version__))
 
 
+# classes compared by tests/test_oracle.py::test_ref_models_match_reference_live: (key, class, cfg, input shape)
+LIVE = {
+    "audio_clf": ("AudioBiLSTM", AUDIO_CLF, (4, 6, 256)),
+    "text_clf": ("TextBiLSTM", TEXT_CLF, (4, 6, 1024)),
+    "audio_reg": ("AudioBiLSTM", AUDIO_REG, (4, 3, 256)),
+    "text_reg": ("TextBiLSTM", TEXT_REG, (4, 3, 1024)),
+}
+
+
+def live_outputs(case: str = "ref_live_outputs") -> None:
+    """Parameter names and eval() outputs of the reference classes on name-keyed weights and inputs (one fixture)."""
+    arrays, names = {}, {}
+    for key, (cls_name, cfg, shape) in LIVE.items():
+        model = ast_loader.load_classes(key, [cls_name])[cls_name](cfg)
+        params.fill_module(model)
+        model.eval()
+        with torch.no_grad():
+            arrays["out:" + key] = model(params.inputs_for("live:" + key, shape)).numpy()
+        names[key] = [n for n, _ in model.named_parameters()]
+    _save(case, arrays, dict(case=case, names=names, classes={k: v[0] for k, v in LIVE.items()},
+                             refs={k: ast_loader.FILES[k] for k in LIVE},
+                             torch=torch.__version__))
+
+
 def main() -> None:
     if not ast_loader.available():
-        raise SystemExit("reference tree not found; fixtures can only be generated in the build container")
+        raise SystemExit("reference tree not found: set B200RNN_REFERENCE_ROOT to its DepressionCollected directory")
     torch.set_num_threads(1)
     single_modal("audio_clf_b3_t5", "audio_clf", "AudioBiLSTM", AUDIO_CLF, (3, 5, 256), "ce")
     single_modal("text_clf_b3_t6", "text_clf", "TextBiLSTM", TEXT_CLF, (3, 6, 1024), "ce")
@@ -147,6 +171,7 @@ def main() -> None:
     rnn_boundary("lstm_boundary_b5_t17", "text_clf", "TextBiLSTM", TEXT_CLF, "lstm_net", (5, 17, 1024), True)
     fuse("fuse_clf_b3_t3", "fuse_clf", False, 3, 3)
     fuse("fuse_reg_b3_t3", "fuse_reg", True, 3, 3)
+    live_outputs()
 
 
 if __name__ == "__main__":

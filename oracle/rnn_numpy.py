@@ -2,8 +2,8 @@
 
 A numpy restatement, in float64 by default, of the multi-layer GRU / bidirectional LSTM the reference reaches
 through ``torch.nn.GRU`` / ``torch.nn.LSTM`` (call sites audio_gru_whole.py:59-60,105; text_bilstm_whole.py:54-56,105;
-fuse_net_whole.py:266-268,281-286,347,361). The arithmetic itself lives in a third-party dependency that is not under
-/root/reference — PyTorch (the reference pins no version; the oracle version is the installed torch 2.11.0) — so this
+fuse_net_whole.py:266-268,281-286,347,361). The arithmetic itself lives in a third-party dependency that is not part
+of the reference — PyTorch (the reference pins no version; the oracle version is the installed torch 2.11.0) — so this
 file restates the published equations:
 
   GRU  (torch/nn/modules/rnn.py:1221-1224), gate order r,z,n:

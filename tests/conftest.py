@@ -13,12 +13,12 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session", autouse=True)
 def _built_library():
-    """Every test run starts from a built C-ABI library (nvcc cross-compiles sm_100a without a GPU)."""
+    """Every test run starts from a built C-ABI library (nvcc cross-compiles sm_90a without a GPU)."""
     # build() unconditionally (an incremental `make`: seconds when nothing changed), so the tests always run the
     # binary the tree's sources produce - never a stale pre-built one that merely travelled with the snapshot
     import __graft_entry__

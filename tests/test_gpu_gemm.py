@@ -23,8 +23,8 @@ def test_gemm_layouts(M, N, K, a_kc, b_kc):
     torch.cuda.synchronize()
     err = (out.cpu() - ref).abs().max().item()
     scale = ref.abs().max().item()
-    # 4e-6 of the largest output: fp32 FFMA sits near 1e-6, the tcgen05 3xTF32 path (truncating fp32 accumulate
-    # in TMEM) near 2.5e-6; plain TF32 would be ~1e-3
+    # 4e-6 of the largest output: fp32 FFMA sits near 1e-6, the tensor-core 3xTF32 path (truncating fp32 accumulate
+    # inside each k-block) a little above; plain TF32 would be ~1e-3
     assert err <= 4e-6 * scale * max(1.0, (K / 256) ** 0.5) + 1e-5, (err, scale)
 
 
@@ -46,7 +46,7 @@ def test_gemm_accumulate_and_no_splitk():
 
 @pytest.mark.parametrize("M,N,K", [(15360, 768, 256), (3840, 512, 1024), (130, 384, 512), (1, 128, 32), (257, 1024, 256)])
 def test_tcgen05_3xtf32_input_projection(M, N, K):
-    """Eligible shapes (A, W k-contiguous, K % 32 == 0, N % 128 == 0) run on tcgen05 with the 3xTF32 split; the
+    """Eligible shapes (A, W k-contiguous, K % 32 == 0, N % 128 == 0) run on wgmma with the 3xTF32 split; the
     result must stay within fp32-FFMA-like error of the float64 product (plain TF32 would be ~1e-3 relative)."""
     import b200rnn
 

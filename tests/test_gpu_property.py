@@ -1,5 +1,5 @@
 """Property test (hypothesis) over the nn.GRU / nn.LSTM argument space the drop-in supports (SURVEY.md §4):
-random B in [1,130], T in [1,40], input widths that hit both GEMM paths (tcgen05: I % 32 == 0; FFMA: anything else),
+random B in [1,130], T in [1,40], input widths that hit both GEMM paths (tensor cores: I % 32 == 0; FFMA: anything else),
 H in {128, 256}, 1-2 layers, 1-2 directions, batch_first or not, ragged batch tails, B=1, T=1 — forward outputs and
 all gradients against stock torch on CPU."""
 import pytest

@@ -1,12 +1,11 @@
 """CPU tests pinning the ORACLE: numpy restatement vs the executed dependency (torch.nn.GRU / nn.LSTM), restated
-model shells vs the golden fixtures recorded from the reference's own classes, and — where /root/reference
-exists — vs those classes executed live."""
+model shells vs the golden fixtures recorded from the reference's own classes (oracle/make_golden.py)."""
 import numpy as np
 import pytest
 import torch
 
 from conftest import load_golden
-from oracle import ast_loader, params, ref_models
+from oracle import params, ref_models
 from oracle.rnn_numpy import NumpyRNN
 
 FUSE_CFG = dict(text_embed_size=1024, text_hidden_dims=128, rnn_layers=2, dropout=0.3, num_classes=2,
@@ -170,7 +169,6 @@ def test_numpy_oracle_reproduces_reference_rnn_boundary(case, kind):
         _close(arrays["grad:" + n], torch.from_numpy(g), 1e-5, n)
 
 
-@pytest.mark.skipif(not ast_loader.available(), reason="/root/reference only exists in the build container")
 @pytest.mark.parametrize("key,name,cls,regression,shape", [
     ("audio_clf", "AudioBiLSTM", ref_models.RefAudio, False, (4, 6, 256)),
     ("text_clf", "TextBiLSTM", ref_models.RefText, False, (4, 6, 1024)),
@@ -178,13 +176,18 @@ def test_numpy_oracle_reproduces_reference_rnn_boundary(case, kind):
     ("text_reg", "TextBiLSTM", ref_models.RefText, True, (4, 3, 1024)),
 ])
 def test_ref_models_match_reference_live(key, name, cls, regression, shape):
+    """The restated classes against the reference's own ones: same parameter names, same eval() output on the same
+    name-keyed weights and inputs (tests/golden/ref_live_outputs.npz, recorded from the reference's classes by
+    oracle/make_golden.py)."""
     from oracle import make_golden as mg
 
-    cfg = {"audio_clf": mg.AUDIO_CLF, "text_clf": mg.TEXT_CLF, "audio_reg": mg.AUDIO_REG, "text_reg": mg.TEXT_REG}[key]
-    theirs = ast_loader.load_classes(key, [name])[name](cfg)
+    arrays, meta = load_golden("ref_live_outputs")
+    assert meta["classes"][key] == name and tuple(mg.LIVE[key][2]) == shape
+    cfg = mg.LIVE[key][1]
     mine = cls(cfg, regression=regression)
-    assert [n for n, _ in theirs.named_parameters()] == [n for n, _ in mine.named_parameters()]
-    mine.load_state_dict(theirs.state_dict())
-    theirs.eval(), mine.eval()
-    x = torch.randn(*shape)
-    assert torch.allclose(theirs(x), mine(x), atol=1e-6)
+    assert [n for n, _ in mine.named_parameters()] == meta["names"][key]
+    params.fill_module(mine)
+    mine.eval()
+    with torch.no_grad():
+        out = mine(params.inputs_for("live:" + key, shape))
+    assert np.abs(out.numpy() - arrays["out:" + key]).max() < 1e-6

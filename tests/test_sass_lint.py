@@ -1,11 +1,10 @@
 """Static checks on the SASS of the built library (cuobjdump, no GPU).
 
-* the Blackwell instructions the design claims are really there (tcgen05 MMA / TMEM load+store / commit, TMA tensor
-  and bulk copies, st.async, packed FFMA2);
-* two code-generation pitfalls found with the profiler in round 1 stay fixed:
-    - a tcgen05.mma / TMA issue whose operands the compiler cannot prove warp-uniform is wrapped in an
-      ELECT + R2UR.BROADCAST + BRA.U.ANY loop (~55 cycles per MMA instead of ~16): kernels that issue UTCHMMA or
-      UTMALDG must contain no BRA.U.ANY;
+* the Hopper instructions the design claims are really there (wgmma, TMA tensor and bulk copies, st.async,
+  mbarrier);
+* two code-generation pitfalls stay fixed:
+    - a TMA issue whose operands the compiler cannot prove warp-uniform is wrapped in an
+      ELECT + R2UR.BROADCAST + BRA.U.ANY loop: kernels that issue HGMMA or UTMALDG must contain no BRA.U.ANY;
     - a shared-memory pointer aligned through an integer round trip becomes generic (LD.E / ST.E instead of
       LDS / STS) and its loads queue behind outstanding global loads: the tensor-core kernels must not contain
       generic loads/stores at all (their global traffic is LDG/STG).
@@ -43,24 +42,24 @@ def _has(ops, prefix):
     return any(o.startswith(prefix) for o in ops)
 
 
-def test_expected_blackwell_instructions_are_present(functions):
+def test_expected_hopper_instructions_are_present(functions):
     all_ops = [o for ops in functions.values() for o in ops]
-    for prefix, what in [("UTCHMMA", "tcgen05.mma"), ("LDTM", "tcgen05.ld"), ("STTM", "tcgen05.st"),
-                         ("UTCBAR", "tcgen05.commit"), ("UTMALDG", "TMA tensor load"), ("UBLKCP", "TMA bulk copy"),
-                         ("STAS", "st.async"), ("FFMA2", "packed fp32 FMA"), ("SYNCS", "mbarrier")]:
+    for prefix, what in [("HGMMA", "wgmma.mma_async"), ("WARPGROUP", "wgmma fence / commit / wait"),
+                         ("UTMALDG", "TMA tensor load"), ("UBLKCP", "TMA bulk copy"), ("STAS", "st.async"),
+                         ("SYNCS", "mbarrier")]:
         assert _has(all_ops, prefix), f"no {prefix} ({what}) in the library"
 
 
 def test_tensor_core_issue_stays_on_the_uniform_datapath(functions):
-    tc = {n: ops for n, ops in functions.items() if _has(ops, "UTCHMMA") or _has(ops, "UTMALDG")}
-    assert len(tc) >= 4, sorted(tc)   # GEMM + three tensor-core recurrence instantiations
+    tc = {n: ops for n, ops in functions.items() if _has(ops, "HGMMA") or _has(ops, "UTMALDG")}
+    assert len(tc) >= 1, sorted(tc)   # the 3xTF32 GEMM
     for name, ops in tc.items():
-        assert not _has(ops, "BRA.U.ANY"), f"{name}: tcgen05 / TMA issue inside a register-broadcast loop"
+        assert not _has(ops, "BRA.U.ANY"), f"{name}: wgmma / TMA issue inside a register-broadcast loop"
 
 
 def test_tensor_core_kernels_keep_the_shared_state_space(functions):
     for name, ops in functions.items():
-        if _has(ops, "UTCHMMA"):
+        if _has(ops, "HGMMA"):
             generic = [o for o in ops if re.fullmatch(r"(LD|ST)(\.E)?(\.\d+)?", o)]
             assert not generic, f"{name}: generic loads/stores {sorted(set(generic))}"
             assert _has(ops, "LDS") or _has(ops, "STS"), name

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """Small shapes through every recurrence variant, for compute-sanitizer (memcheck / racecheck):
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py
-    B200RNN_REC_TC=1 compute-sanitizer --tool racecheck python tools/sanitize_paths.py
     B200RNN_GRU_BS2=0 compute-sanitizer --tool memcheck python tools/sanitize_paths.py rnn   # recurrence only, 4-row GRU clusters
 """
 import os, sys
