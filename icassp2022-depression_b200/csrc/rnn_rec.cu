@@ -21,6 +21,7 @@
 // far too skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference.
 #include <mutex>
 #include <stdlib.h>
+#include <string.h>
 
 #include "profile.cuh"
 #include "ptx.cuh"
@@ -44,13 +45,14 @@ constexpr bool kLocalSelf = true;
 #endif
 constexpr unsigned FULLMASK = 0xffffffffu;
 
-template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
+// NG: unit groups per warp (forward): a warp contracts NG groups of UPW units against the same state loads
+template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, int NG = 1>
 struct RecCfg {
   static constexpr int G = (MODE == B200RNN_GRU) ? 3 : 4;
   static constexpr int GH = G * H;
   static constexpr int HS = H / C;
-  static constexpr int UPW = (32 / KL) * UPL;
-  static constexpr int NW = HS / UPW;
+  static constexpr int UPW = (32 / KL) * UPL;  // units per warp and unit group
+  static constexpr int NW = HS / (UPW * NG);
   static constexpr int NT = NW * 32;
   static constexpr int NSM = G - RG;  // gate blocks held in shared memory
   static constexpr int CW = 4 * KL;   // floats of the contraction dimension per chunk
@@ -66,7 +68,7 @@ struct RecCfg {
   static_assert(NBAR * 8 <= (int)BAR_BYTES, "barrier block too small");
   static_assert(ROT ? (HS % CW == 0) : (CW % HS == 0), "chunks must tile the per-CTA slices");
   static_assert(RG >= 0 && RG <= 2, "at most two register-resident gate blocks");
-  static_assert(HS * C == H && NW * UPW == HS && NW >= 1, "bad split");
+  static_assert(HS * C == H && NW * UPW * NG == HS && NW >= 1, "bad split");
   static_assert(UPW % 4 == 0, "the exchange packs 4 units per 16-byte store");
   static_assert(NT <= 1024, "too many threads");
 };
@@ -136,10 +138,13 @@ __device__ __forceinline__ void allgather_units(float val, float* vec_local, int
 // =================================================================================================
 // VL = true: per-sequence lengths (PackedSequence semantics): past its length a sequence keeps its state and emits 0
 // PB = true: batch-paired contraction and state layout (rnn_core.cuh, dots_chunk2b), see launch_rec_fwd
-template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false, bool PB = false>
-__global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
+// NG = 2: every warp owns two groups of UPW units (rnn_core.cuh, dots_chunk_ng): half the warps, each state load serves
+// both groups, and every lane applies the gate math to two (unit, batch) outputs
+template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false, bool PB = false, int NG = 1>
+__global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1)
     rec_fwd_kernel(const RecFwdParams p, const int nslices) {
-  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
+  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>;
+  static_assert(NG == 1 || (MODE == B200RNN_GRU && RG == 0 && !PB), "NG = 2: GRU, scalar FFMA, RG = 0");
   using LM = LaneMap<KL, UPL, BS>;
   constexpr int G = Cfg::G, HS = Cfg::HS, NT = Cfg::NT, UPW = Cfg::UPW, NSM = Cfg::NSM, GH = Cfg::GH;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -160,9 +165,11 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 
   if (tid == 0) {
     // [0]: weights (tx bytes). [1 + buf*C + src]: slice of source CTA `src` - remote sources complete tx bytes
-    // (one arrive.expect_tx by thread 0 per phase), the CTA's OWN slice is published by one plain arrive per warp
+    // (one arrive.expect_tx by thread 0 per phase), the CTA's OWN slice is published by one plain arrive per warp and
+    // unit group
     for (int i = 0; i < Cfg::NBAR; ++i)
-      ptx::mbar_init(&bars[i], (kLocalSelf && i >= 1 && (uint32_t)((i - 1) % C) == rank) ? (uint32_t)Cfg::NW : 1u);
+      ptx::mbar_init(&bars[i],
+                     (kLocalSelf && i >= 1 && (uint32_t)((i - 1) % C) == rank) ? (uint32_t)(Cfg::NW * NG) : 1u);
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -177,48 +184,58 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
   for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
   const int rot = Cfg::ROT ? (int)rank * CPS : 0;
   float wreg[RG > 0 ? RG : 1][UPL][H / KL];
-  load_resident<RG, KL, UPL, BS, H>(w_hh, H, (long long)NSM * H + j0 + w * UPW, rot, lane, wreg);
+  load_resident<RG, KL, UPL, BS, H>(w_hh, H, (long long)NSM * H + j0 + w * UPW * NG, rot, lane, wreg);
   ptx::mbar_wait(&bars[0], 0);
   __syncthreads();
   ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
 
-  // ---- lane identity: after the butterfly this lane owns (unit, batch) ------------------------------
+  // ---- lane identity: after the butterfly this lane owns (unit, batch) of each unit group ----------------
   const int uw = LM::unit(lane), qb = LM::q(lane);
-  const int j = j0 + w * UPW + uw;  // hidden unit
-  const int b = b0 + qb;            // batch row
+  const int ju = j0 + w * UPW * NG + uw;  // hidden unit of group 0; group ug owns ju + ug * UPW
+  const int b = b0 + qb;                  // batch row
   const bool valid = b < B;
   float* gates = p.gates[dir];
   float* extra = p.extra[dir];
-  const float bhn = (MODE == B200RNN_GRU) ? p.b_hh[dir][2 * H + j] : 0.f;
+  float bhn[NG];
+#pragma unroll
+  for (int ug = 0; ug < NG; ++ug) bhn[ug] = (MODE == B200RNN_GRU) ? p.b_hh[dir][2 * H + ju + ug * UPW] : 0.f;
 
-  float h_prev = 0.f, c_prev = 0.f, h_sum = 0.f;
+  float h_prev[NG], c_prev[NG], h_sum[NG];
+#pragma unroll
+  for (int ug = 0; ug < NG; ++ug) h_prev[ug] = c_prev[ug] = h_sum[ug] = 0.f;
   int len_b = T;
   if constexpr (VL) {
     if (valid) len_b = p.lengths[b];
   }
-  float gi[G];
+  float gi[NG][G];
 #pragma unroll
-  for (int g = 0; g < G; ++g) gi[g] = 0.f;
+  for (int ug = 0; ug < NG; ++ug)
+#pragma unroll
+    for (int g = 0; g < G; ++g) gi[ug][g] = 0.f;
   if (valid && T > 0) {
     const int t0 = dir ? T - 1 : 0;
-    const float* gp = gates + ((size_t)t0 * B + b) * GH + j;
+    const float* gp = gates + ((size_t)t0 * B + b) * GH + ju;
 #pragma unroll
-    for (int g = 0; g < G; ++g) gi[g] = gp[g * H];
+    for (int ug = 0; ug < NG; ++ug)
+#pragma unroll
+      for (int g = 0; g < G; ++g) gi[ug][g] = gp[g * H + ug * UPW];
   }
 
   // Global stores of a step (output, saved gates) are DEFERRED into the next step, behind its first chunk: they used to
   // sit between the exchange and the next contraction, i.e. on the serial path of every step (225 cycles).
-  float pend_y = 0.f, pend_s0 = 0.f, pend_s1 = 0.f, pend_s2 = 0.f, pend_s3 = 0.f, pend_sx = 0.f;
+  float pend_y[NG], pend_s[NG][4], pend_sx[NG];
   auto flush_pending = [&](int tp) {
     if (valid) {
-      if (p.y) p.y[(long long)tp * p.y_st + (long long)b * p.y_sb + dir * H + j] = pend_y;
-      if (p.training) {
-        float* gp = gates + ((size_t)tp * B + b) * GH + j;
-        gp[0] = pend_s0;
-        gp[H] = pend_s1;
-        gp[2 * H] = pend_s2;
-        if (G == 4) gp[3 * H] = pend_s3;
-        extra[((size_t)tp * B + b) * H + j] = pend_sx;
+#pragma unroll
+      for (int ug = 0; ug < NG; ++ug) {
+        const int j = ju + ug * UPW;
+        if (p.y) p.y[(long long)tp * p.y_st + (long long)b * p.y_sb + dir * H + j] = pend_y[ug];
+        if (p.training) {
+          float* gp = gates + ((size_t)tp * B + b) * GH + j;
+#pragma unroll
+          for (int g = 0; g < G; ++g) gp[g * H] = pend_s[ug][g];
+          extra[((size_t)tp * B + b) * H + j] = pend_sx[ug];
+        }
       }
     }
   };
@@ -241,12 +258,12 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     // folded before the butterfly) or batch-paired (PACKB: float2 = two batch rows of one unit, one weight for both,
     // state kept in the paired shared-memory layout); the LSTM keeps scalar accumulators
     constexpr bool PACKB = PB;
-    constexpr bool PACK2 = !PACKB && (MODE == B200RNN_GRU) && RG < 2;
+    constexpr bool PACK2 = !PACKB && NG == 1 && (MODE == B200RNN_GRU) && RG < 2;
     float2 acc2[PACK2 ? G : 1][UPL][BS];
     float2 acc2b[PACKB ? G : 1][UPL][BS / 2];
-    float acc[G][UPL][BS];
+    float acc[NG * G][UPL][BS];  // [ug * G + g]
 #pragma unroll
-    for (int g = 0; g < G; ++g)
+    for (int g = 0; g < NG * G; ++g)
 #pragma unroll
       for (int au = 0; au < UPL; ++au)
 #pragma unroll
@@ -273,6 +290,8 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
         dots_chunk2b<G, RG, KL, UPL, BS, H>(W_s, HS, w * UPW, wreg, h_cur, c, ca, lane, acc2b);
       else if constexpr (PACK2)
         dots_chunk2<G, RG, KL, UPL, BS, H, H>(W_s, HS, w * UPW, wreg, h_cur, c, ca, lane, acc2);
+      else if constexpr (NG > 1)
+        dots_chunk_ng<NG, G, KL, UPL, BS, H, H>(W_s, HS, w * UPW * NG, h_cur, ca, lane, acc);
       else
         dots_chunk<G, RG, KL, UPL, BS, H, H>(W_s, HS, w * UPW, wreg, h_cur, c, ca, lane, acc);
       if (c == 0 && step > 0) flush_pending(dir ? (T - step) : (step - 1));  // the previous step's stores
@@ -291,65 +310,79 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       for (int g = 0; g < G; ++g) acc[g][0][0] = red[g];
     } else {
       if constexpr (PACK2) fold_pairs<G, UPL, BS>(acc2, acc);
-      warp_transpose_reduce<G, KL, UPL, BS>(acc);
+      warp_transpose_reduce<NG * G, KL, UPL, BS>(acc);
     }
     if (tr) trow[5] = clock64() + (long long)(acc[0][0][0] == 12345.678f);  // butterfly done (value dependence pins it)
 
-    float hnew, s0, s1, s2, s3 = 0.f, sx;
-    if (MODE == B200RNN_GRU) {
-      const float r = sigmoid_f(gi[0] + acc[0][0][0]);
-      const float z = sigmoid_f(gi[1] + acc[1][0][0]);
-      const float hn = acc[2][0][0] + bhn;
-      const float n = tanh_f(gi[2] + r * hn);
-      hnew = n + z * (h_prev - n);
-      if constexpr (VL) {
-        if (t >= len_b) hnew = h_prev;
-      }
-      s0 = r; s1 = z; s2 = n; sx = hn;
-    } else {
-      const float ig = sigmoid_f(gi[0] + acc[0][0][0]);
-      const float fg = sigmoid_f(gi[1] + acc[1][0][0]);
-      const float gg = tanh_f(gi[2] + acc[2][0][0]);
-      const float og = sigmoid_f(gi[G - 1] + acc[G - 1][0][0]);
-      float cnew = fg * c_prev + ig * gg;
-      hnew = og * tanh_f(cnew);
-      if constexpr (VL) {
-        if (t >= len_b) {
-          cnew = c_prev;
-          hnew = h_prev;
+    float hnew[NG];
+#pragma unroll
+    for (int ug = 0; ug < NG; ++ug) {
+      float s[4], sx;
+      if (MODE == B200RNN_GRU) {
+        const float r = sigmoid_f(gi[ug][0] + acc[ug * G][0][0]);
+        const float z = sigmoid_f(gi[ug][1] + acc[ug * G + 1][0][0]);
+        const float hn = acc[ug * G + 2][0][0] + bhn[ug];
+        const float n = tanh_f(gi[ug][2] + r * hn);
+        hnew[ug] = n + z * (h_prev[ug] - n);
+        if constexpr (VL) {
+          if (t >= len_b) hnew[ug] = h_prev[ug];
         }
+        s[0] = r; s[1] = z; s[2] = n; s[3] = 0.f; sx = hn;
+      } else {
+        const float ig = sigmoid_f(gi[ug][0] + acc[ug * G][0][0]);
+        const float fg = sigmoid_f(gi[ug][1] + acc[ug * G + 1][0][0]);
+        const float gg = tanh_f(gi[ug][2] + acc[ug * G + 2][0][0]);
+        const float og = sigmoid_f(gi[ug][G - 1] + acc[ug * G + G - 1][0][0]);
+        float cnew = fg * c_prev[ug] + ig * gg;
+        hnew[ug] = og * tanh_f(cnew);
+        if constexpr (VL) {
+          if (t >= len_b) {
+            cnew = c_prev[ug];
+            hnew[ug] = h_prev[ug];
+          }
+        }
+        c_prev[ug] = cnew;
+        s[0] = ig; s[1] = fg; s[2] = gg; s[3] = og; sx = cnew;
       }
-      c_prev = cnew;
-      s0 = ig; s1 = fg; s2 = gg; s3 = og; sx = cnew;
+      h_prev[ug] = hnew[ug];
+      float yv = hnew[ug];  // what the caller sees at this step
+      if constexpr (VL) {
+        if (t >= len_b) yv = 0.f;
+      }
+      h_sum[ug] += yv;
+      // this step's global stores wait in registers until the next step's first chunk has been issued
+      pend_y[ug] = yv;
+#pragma unroll
+      for (int g = 0; g < 4; ++g) pend_s[ug][g] = s[g];
+      pend_sx[ug] = sx;
     }
-    h_prev = hnew;
-    float yv = hnew;  // what the caller sees at this step
-    if constexpr (VL) {
-      if (t >= len_b) yv = 0.f;
-    }
-    h_sum += yv;
-    if (tr) trow[6] = clock64() + (long long)(hnew == 12345.678f);          // gate math done
+    if (tr) trow[6] = clock64() + (long long)(hnew[0] == 12345.678f);       // gate math done
 
-    if (step + 1 < T)
-      allgather_units<C, KL, UPL, BS, kLocalSelf, PACKB>(hnew, h_nxt, H, j0 + w * UPW, &bars[1 + nxt * C + rank], lane,
-                                                         rank);
+    if (step + 1 < T) {
+#pragma unroll
+      for (int ug = 0; ug < NG; ++ug)
+        allgather_units<C, KL, UPL, BS, kLocalSelf, PACKB>(hnew[ug], h_nxt, H, j0 + (w * NG + ug) * UPW,
+                                                           &bars[1 + nxt * C + rank], lane, rank);
+    }
     if (tr) trow[7] = clock64();                                            // exchange issued
 
-    // prefetch of the next step's x-projection (long latency, consumed at the next gate math); this step's global
-    // stores wait in registers until the next step's first chunk has been issued
-    pend_y = yv; pend_s0 = s0; pend_s1 = s1; pend_s2 = s2; pend_s3 = s3; pend_sx = sx;
+    // prefetch of the next step's x-projection (long latency, consumed at the next gate math)
     if (step == T - 1) flush_pending(t);
     if (valid) {
-      if (step == T - 1) {
-        p.h_n[((size_t)dir * B + b) * H + j] = hnew;
-        if (p.y_pool) p.y_pool[(size_t)b * p.D * H + dir * H + j] = h_sum;
-        if (MODE == B200RNN_LSTM && p.c_n) p.c_n[((size_t)dir * B + b) * H + j] = c_prev;
-      }
-      if (step + 1 < T) {
-        const int tn = dir ? (T - 2 - step) : (step + 1);
-        const float* gp = gates + ((size_t)tn * B + b) * GH + j;
 #pragma unroll
-        for (int g = 0; g < G; ++g) gi[g] = gp[g * H];
+      for (int ug = 0; ug < NG; ++ug) {
+        const int j = ju + ug * UPW;
+        if (step == T - 1) {
+          p.h_n[((size_t)dir * B + b) * H + j] = hnew[ug];
+          if (p.y_pool) p.y_pool[(size_t)b * p.D * H + dir * H + j] = h_sum[ug];
+          if (MODE == B200RNN_LSTM && p.c_n) p.c_n[((size_t)dir * B + b) * H + j] = c_prev[ug];
+        }
+        if (step + 1 < T) {
+          const int tn = dir ? (T - 2 - step) : (step + 1);
+          const float* gp = gates + ((size_t)tn * B + b) * GH + j;
+#pragma unroll
+          for (int g = 0; g < G; ++g) gi[ug][g] = gp[g * H];
+        }
       }
     }
   }
@@ -680,18 +713,19 @@ int max_active_clusters(K kernel, int C, int NT, size_t smem) {
   return n;
 }
 
-template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool PB = false>
+template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool PB = false, int NG = 1>
 bool try_fwd(const RecFwdParams& p, cudaStream_t s, bool force, int* rc) {
-  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
+  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>;
   static_assert(Cfg::FWD_SMEM <= MAX_SMEM, "forward config does not fit an SM");
-  auto k = p.lengths ? rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, true, PB>
-                     : rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, false, PB>;
+  auto k = p.lengths ? rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, true, PB, NG>
+                     : rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, false, PB, NG>;
   const int nslices = (p.B + BS - 1) / BS;
   const int nclusters = nslices * p.D;
   static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
   if (debug)
-    fprintf(stderr, "[b200rnn] fwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d: need %d clusters, capacity %d, smem %zu\n", C, BS,
-            KL, UPL, RG, nclusters, max_active_clusters(k, C, Cfg::NT, Cfg::FWD_SMEM), (size_t)Cfg::FWD_SMEM);
+    fprintf(stderr, "[b200rnn] fwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d PB=%d NG=%d: need %d clusters, capacity %d, smem %zu\n",
+            C, BS, KL, UPL, RG, (int)PB, NG, nclusters, max_active_clusters(k, C, Cfg::NT, Cfg::FWD_SMEM),
+            (size_t)Cfg::FWD_SMEM);
   if (!force && nclusters > max_active_clusters(k, C, Cfg::NT, Cfg::FWD_SMEM)) return false;
   *rc = launch_clustered(k, p, nslices, nclusters, C, Cfg::NT, Cfg::FWD_SMEM, s, PROF_REC_FWD);
   return true;
@@ -739,14 +773,32 @@ int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
   if (p.mode == B200RNN_GRU && p.H == 256) {
-    // half-filled chip (e.g. BASELINE c2 with B = 64): clusters of 2 batch rows use twice the SMs with half the FFMA
-    // work per step (all three gate blocks in shared memory, 4 warps per CTA); taken only while every cluster is
-    // co-resident (try_fwd checks the occupancy)
+    // 4-CTA clusters of 2, 4 or 8 batch rows; each takes 4 * ceil(B / BS) SMs:
+    //   bs2 <4,2,16,8,0>: all three gate blocks in shared memory, 4 warps per CTA
+    //   bs4 <4,4,16,4,1> batch-paired (rnn_core.cuh dots_chunk2b): two gate blocks in shared memory, one in registers,
+    //       8 warps per CTA
+    //   bs8 <4,8,16,2,0> two unit groups per warp (NG = 2, rnn_core.cuh dots_chunk_ng): all three gate blocks in
+    //       shared memory (213 KB), 8 warps per CTA; twice the FFMA work per CTA and step of bs4 on half the SMs
+    // A cluster cannot span GPCs, and H100 SXM GPCs are floor-swept unevenly, so the number of co-resident 4-CTA clusters
+    // (30 on a 132-SM card measured) comes from the driver (try_fwd), never from the SM count. Measured per layer launch
+    // at T = 120 (DESIGN.md): a config in one wave beats the next wider one, and bs8 in one wave beats bs4 in two.
+    // B200RNN_GRU_FWD=bs2|bs4|bs8 forces one config (A/B runs).
+    static const char* forced = getenv("B200RNN_GRU_FWD");
+    if (forced) {
+      if (!strcmp(forced, "bs2")) try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, true, &rc);
+      else if (!strcmp(forced, "bs4")) try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, true, &rc);
+      else if (!strcmp(forced, "bs8")) try_fwd<B200RNN_GRU, 256, 4, 8, 16, 2, 0, false, 2>(p, s, true, &rc);
+      else {
+        set_error("B200RNN_GRU_FWD=%s: expected bs2, bs4 or bs8", forced);
+        rc = B200RNN_ERR_INVALID;
+      }
+      return rc;
+    }
     static const int bs2 = env_variant("B200RNN_GRU_BS2", 1);  // =0: A/B switch
-    if (bs2 && p.B <= 2 * (NUM_SMS / 4) && try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
-    // batch-paired contraction (rnn_core.cuh dots_chunk2b): half the accumulator registers of the k-paired form
+    if (bs2 && try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
     if (try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, false, &rc)) return rc;
-    try_fwd<B200RNN_GRU, 256, 8, 8, 32, 4, 1>(p, s, true, &rc);
+    // the widest clusters: one wave up to B = 8 x the 4-CTA cluster capacity, several waves beyond
+    try_fwd<B200RNN_GRU, 256, 4, 8, 16, 2, 0, false, 2>(p, s, true, &rc);
     return rc;
   }
   if (p.mode == B200RNN_GRU && p.H == 128) {
@@ -777,8 +829,9 @@ int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
   // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
   // (not the weights) dominates the shared-memory traffic of the backward contraction
   if (p.mode == B200RNN_GRU && p.H == 256) {
+    // as in the forward: a config is taken only when the driver reports all its clusters co-resident
     static const int bs2 = env_variant("B200RNN_GRU_BS2", 1);
-    if (bs2 && p.B <= 2 * (NUM_SMS / 4) && try_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
+    if (bs2 && try_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
     if (try_bwd<B200RNN_GRU, 256, 4, 4, 32, 8, 1>(p, s, false, &rc)) return rc;
     try_bwd<B200RNN_GRU, 256, 8, 8, 32, 4, 1>(p, s, true, &rc);
     return rc;
