@@ -67,6 +67,11 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
       : "memory");
 }
 
+// named CTA barrier `id` (1..15; 0 is __syncthreads) over `nthreads` threads, a multiple of 32
+__device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 // ---- thread-block cluster -----------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -107,6 +112,25 @@ __device__ __forceinline__ void st_async_v4(uint32_t cluster_addr, float4 v, uin
           cluster_addr),
       "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"(cluster_mbar)
       : "memory");
+}
+
+// ---- warp-level tensor-core MMA (SASS: HMMA.1688.F32.TF32) ----------------------------------------
+// x = hi + lo with hi = x truncated to TF32 (its 13 low mantissa bits cleared, in a 32-bit container) and lo = x - hi
+// (exact in fp32, |lo| < 2^-10 |x|). The MMA reads only the TF32 bits of lo, so hi*hi + lo*hi + hi*lo carries ~2^-20
+// relative error per product (3xTF32). Two ops per value: cvt.rna.tf32.f32 (the round-to-nearest split of gemm_tc.cu)
+// is five in SASS and made the recurrence measurably slower at no measurable gain in accuracy (DESIGN.md).
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+  hi = __float_as_uint(x) & 0xffffe000u;
+  lo = __float_as_uint(x - __uint_as_float(hi));
+}
+// D[16x8] += A[16x8] * B[8x8], fragments as in the PTX ISA (g = lane / 4, t = lane % 4):
+//   a = {A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]}, b = {B[t][g], B[t+4][g]},
+//   d = {D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]}
+__device__ __forceinline__ void mma_tf32_m16n8k8(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
 }  // namespace ptx

@@ -17,8 +17,9 @@
 //     consumer waits on a local mbarrier, double buffered. No cluster barrier, fence or L1 flush in the loop.
 //   * batch slices are independent clusters: no grid-wide synchronisation anywhere.
 //
-// fp32 FFMA by choice: the per-step contraction is [BS x H] x [H x G*HS] with BS = 4..8 rows per CTA —
-// far too skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference.
+// fp32 FFMA for most configs: the per-step contraction is [BS x H] x [H x G*HS] with BS = 2..8 rows per CTA — far too
+// skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference. The GRU H=256 8-row config runs it
+// on the tensor cores with warp-level mma.sync (N = 8) in 3xTF32 instead (rec_fwd_tc_kernel).
 #include <mutex>
 #include <stdlib.h>
 #include <string.h>
@@ -390,6 +391,280 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1
 }
 
 // =================================================================================================
+// forward, GRU H = 256 on the tensor cores (config tc8)
+// =================================================================================================
+// The cluster design of rec_fwd_kernel at C = 4, BS = 8 (weights staged once, per-source mbarriers, double-buffered
+// state, st.async all-gather with the own slice delivered locally, own slice first, deferred global stores, x-projection
+// prefetched one step ahead), but the per-step contraction [192 gate rows of the CTA] x [K = 256] x [8 batch rows] runs
+// on the tensor cores as mma.sync m16n8k8 in 3xTF32 (ptx.cuh split_tf32), at fp32-level error:
+//   * unit group ug (16 units of the CTA's slice) has three gate tiles (r, z, n): three M = 16 tiles of W_hh rows,
+//     N = the 8 batch rows, K in 32 k-steps of 8. Two warps share a unit group and split K: warp (ug, kh) takes k-steps
+//     kh*4 .. kh*4+3 of every source slice, so each scheduler runs two warps and hides the other's MMA and shared-memory
+//     latency (one warp per group was measured slower).
+//   * the accumulator fragment leaves lane (g, t) = (lane / 4, lane % 4) units g, g+8 of the group for batch rows 2t,
+//     2t+1 of all three gates. Warp kh finishes units g + 8*kh: it swaps the other half's partial sums with its partner
+//     through shared memory, and the gate math stays in the lane (2 outputs each), with no butterfly.
+//   * weights in A-fragment order: a lane's four values of one (tile, k-step) are one conflict-free LDS.128.
+//   * state in B-fragment order (tc_state_index): a lane's two values of one k-step are one conflict-free LDS.64, and
+//     the 8 units a warp finishes are one whole k-step, i.e. 64 contiguous floats: the all-gather is one float4 per lane
+//     of the first half-warp.
+//   * per tile, hi*hi and the two cross terms (lo*hi + hi*lo) have their own accumulators, restarted for each source
+//     slice (at most 8 MMAs) and added round-to-nearest into the fp32 sum: six independent MMA chains per warp, and the
+//     truncating tensor-core accumulation never runs longer than in gemm_tc.cu (12 MMAs).
+struct TcFwdCfg {
+  static constexpr int H = 256, C = 4, BS = 8, G = 3, GH = G * H;
+  static constexpr int HS = H / C;        // units per CTA
+  static constexpr int NUG = HS / 16;     // unit groups
+  static constexpr int NW = 2 * NUG;      // warps: (k half, unit group)
+  static constexpr int NT = NW * 32;
+  static constexpr int KS = H / 8;        // k-steps of the contraction
+  static constexpr int KSC = HS / 8;      // k-steps per source slice
+  static constexpr size_t W_BYTES = (size_t)G * HS * H * sizeof(float);
+  static constexpr size_t RED_BYTES = (size_t)NW * 2 * G * 32 * sizeof(float);  // partial sums swapped between halves
+  static constexpr size_t SMEM = W_BYTES + (size_t)2 * BS * H * sizeof(float) + RED_BYTES + 2 * C * sizeof(uint64_t);
+};
+
+// position of state element (k, batch row b) in the B-fragment-ordered buffer: lane (g, t) of k-step ks reads
+// {h[g][ks*8 + t], h[g][ks*8 + t + 4]} as the float2 at ks*64 + lane*2
+__device__ __forceinline__ int tc_state_index(int k, int b) {
+  return ((k >> 3) * 8 + b) * 8 + (k & 3) * 2 + ((k >> 2) & 1);
+}
+
+template <bool VL>
+__global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFwdParams p, const int nslices) {
+  using Cfg = TcFwdCfg;
+  constexpr int H = Cfg::H, C = Cfg::C, BS = Cfg::BS, G = Cfg::G, GH = Cfg::GH, HS = Cfg::HS, NUG = Cfg::NUG,
+                NW = Cfg::NW, NT = Cfg::NT, KS = Cfg::KS, KSC = Cfg::KSC;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  float4* W_f = reinterpret_cast<float4*>(smem_raw);                  // [NUG][G][KS][32 lanes] A fragments
+  float* h_s = reinterpret_cast<float*>(smem_raw + Cfg::W_BYTES);     // [2][BS * H] B-fragment order
+  float* red = h_s + 2 * BS * H;                                       // [NW][2 * G][32 lanes]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(red + NW * 2 * G * 32);  // [buf * C + src] state slices
+
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int ug = w % NUG, kh = w / NUG;
+  const uint32_t rank = ptx::cluster_ctarank();
+  const int cid = blockIdx.x / C;
+  const int dir = cid / nslices;
+  const int slice = cid - dir * nslices;
+  const int b0 = slice * BS;
+  const int j0 = (int)rank * HS;
+  const int B = p.B, T = p.T;
+  const float* w_hh = p.w_hh[dir];
+
+  if (tid == 0) {
+    // remote sources complete tx bytes (one arrive.expect_tx by thread 0 per phase), the own slice is published by one
+    // plain arrive per warp
+    for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], (uint32_t)(i % C) == rank ? (uint32_t)NW : 1u);
+    ptx::fence_mbar_init();
+  }
+  // this CTA's rows of the three gate blocks, read as coalesced float4 and scattered into A-fragment order: row u of
+  // gate block g goes to unit group u / 16, tile g, fragment row u % 16; k0..k0+3 are the lanes t = 0..3 of one k-step
+  // half
+#pragma unroll 8
+  for (int i = tid; i < G * HS * H / 4; i += NT) {
+    const int rr = i / (H / 4), k0 = (i % (H / 4)) * 4;
+    const int g = rr / HS, u = rr % HS;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(w_hh + ((size_t)g * H + j0 + u) * H + k0));
+    float* dst = reinterpret_cast<float*>(W_f + (((u / 16) * G + g) * KS + k0 / 8) * 32 + (u % 8) * 4) +
+                 (u % 16) / 8 + 2 * ((k0 / 4) & 1);
+    dst[0] = v.x;
+    dst[4] = v.y;
+    dst[8] = v.z;
+    dst[12] = v.w;
+  }
+  for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
+  __syncthreads();
+  ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
+
+  // ---- lane identity: output jb is unit ju, batch row bb + jb (accumulator fragment elements 2*kh + jb) ----------
+  const int fg = lane >> 2, ft = lane & 3;
+  const int u0 = ug * 16 + kh * 8;  // first unit (within the CTA's slice) this warp finishes
+  const int ju = j0 + u0 + fg;
+  const int bb = b0 + 2 * ft;
+  bool valid[2];
+  int len_b[2];
+#pragma unroll
+  for (int jb = 0; jb < 2; ++jb) {
+    valid[jb] = bb + jb < B;
+    len_b[jb] = T;
+    if constexpr (VL) {
+      if (valid[jb]) len_b[jb] = p.lengths[bb + jb];
+    }
+  }
+  float* gates = p.gates[dir];
+  float* extra = p.extra[dir];
+  const float bhn = p.b_hh[dir][2 * H + ju];
+
+  float h_prev[2], h_sum[2], gi[2][G];
+#pragma unroll
+  for (int jb = 0; jb < 2; ++jb) {
+    h_prev[jb] = h_sum[jb] = 0.f;
+#pragma unroll
+    for (int g = 0; g < G; ++g) gi[jb][g] = 0.f;
+  }
+  auto load_gi = [&](int tn) {
+#pragma unroll
+    for (int jb = 0; jb < 2; ++jb)
+      if (valid[jb]) {
+        const float* gp = gates + ((size_t)tn * B + bb + jb) * GH + ju;
+#pragma unroll
+        for (int g = 0; g < G; ++g) gi[jb][g] = gp[g * H];
+      }
+  };
+  if (T > 0) load_gi(dir ? T - 1 : 0);
+
+  // a step's global stores (output, saved gates) wait in registers until the next step's first slice is contracted
+  float pend_y[2], pend_s[2][G], pend_sx[2];
+  auto flush_pending = [&](int tp) {
+#pragma unroll
+    for (int jb = 0; jb < 2; ++jb) {
+      if (!valid[jb]) continue;
+      const int b = bb + jb;
+      if (p.y) p.y[(long long)tp * p.y_st + (long long)b * p.y_sb + dir * H + ju] = pend_y[jb];
+      if (p.training) {
+        float* gp = gates + ((size_t)tp * B + b) * GH + ju;
+#pragma unroll
+        for (int g = 0; g < G; ++g) gp[g * H] = pend_s[jb][g];
+        extra[((size_t)tp * B + b) * H + ju] = pend_sx[jb];
+      }
+    }
+  };
+
+  const float4* W_w = W_f + (size_t)ug * G * KS * 32 + lane;
+  float* red_mine = red + w * 2 * G * 32 + lane;                         // written by this warp
+  const float* red_partner = red + (w ^ NUG) * 2 * G * 32 + lane;        // written by the other k half
+  for (int step = 0; step < T; ++step) {
+    const int t = dir ? (T - 1 - step) : step;
+    const int cur = step & 1, nxt = cur ^ 1;
+    const float2* h_cur = reinterpret_cast<const float2*>(h_s + cur * BS * H) + lane;
+    const uint32_t par = ((step - 1) >> 1) & 1;
+
+    float acc[G][4];
+#pragma unroll
+    for (int g = 0; g < G; ++g)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[g][i] = 0.f;
+    // one source slice at a time, starting with the slice this CTA produced itself
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      const int src = (c + (int)rank) % C;
+      if (step > 0) ptx::mbar_wait(&bars[cur * C + src], par);
+      float d[G][2][4];  // [gate tile][lo*hi + hi*lo, hi*hi]
+#pragma unroll
+      for (int g = 0; g < G; ++g)
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) d[g][m][i] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < KSC / 2; ++kk) {
+        const int ks = src * KSC + kh * (KSC / 2) + kk;
+        const float2 hv = h_cur[ks * 32];
+        uint32_t bh[2], bl[2];
+        ptx::split_tf32(hv.x, bh[0], bl[0]);
+        ptx::split_tf32(hv.y, bh[1], bl[1]);
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+          const float4 wv = W_w[(g * KS + ks) * 32];
+          uint32_t ah[4], al[4];
+          ptx::split_tf32(wv.x, ah[0], al[0]);
+          ptx::split_tf32(wv.y, ah[1], al[1]);
+          ptx::split_tf32(wv.z, ah[2], al[2]);
+          ptx::split_tf32(wv.w, ah[3], al[3]);
+          ptx::mma_tf32_m16n8k8(d[g][0], al, bh);
+          ptx::mma_tf32_m16n8k8(d[g][0], ah, bl);
+          ptx::mma_tf32_m16n8k8(d[g][1], ah, bh);
+        }
+      }
+#pragma unroll
+      for (int g = 0; g < G; ++g)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[g][i] += d[g][0][i] + d[g][1][i];
+      if (c == 0 && step > 0) flush_pending(dir ? (T - step) : (step - 1));  // the previous step's stores
+    }
+    // every slice of h_step has been consumed by this thread => the barriers of the other buffer are re-armed
+    if (tid == 0 && step + 1 < T) {
+#pragma unroll
+      for (int src = 0; src < C; ++src)
+        if ((uint32_t)src != rank) ptx::mbar_arrive_expect_tx(&bars[nxt * C + src], (uint32_t)(BS * HS * sizeof(float)));
+    }
+    // swap halves with the partner warp: it finishes the other 8 units. WAR on `red`: the partner overwrites it only
+    // after its next step's own-slice wait, which needs this warp's arrive below (after the read).
+#pragma unroll
+    for (int g = 0; g < G; ++g)
+#pragma unroll
+      for (int jb = 0; jb < 2; ++jb) red_mine[(g * 2 + jb) * 32] = kh ? acc[g][jb] : acc[g][2 + jb];
+    ptx::named_barrier_sync(1 + ug, 64);
+    float pre[G][2];  // recurrent pre-activations of this lane's two outputs
+#pragma unroll
+    for (int g = 0; g < G; ++g)
+#pragma unroll
+      for (int jb = 0; jb < 2; ++jb) {
+        pre[g][jb] = (kh ? acc[g][2 + jb] : acc[g][jb]) + red_partner[(g * 2 + jb) * 32];
+      }
+
+    float hnew[2];
+#pragma unroll
+    for (int jb = 0; jb < 2; ++jb) {
+      const float r = sigmoid_f(gi[jb][0] + pre[0][jb]);
+      const float z = sigmoid_f(gi[jb][1] + pre[1][jb]);
+      const float hn = pre[2][jb] + bhn;
+      const float n = tanh_f(gi[jb][2] + r * hn);
+      hnew[jb] = n + z * (h_prev[jb] - n);
+      float yv = hnew[jb];  // what the caller sees at this step
+      if constexpr (VL) {
+        if (t >= len_b[jb]) {
+          hnew[jb] = h_prev[jb];
+          yv = 0.f;
+        }
+      }
+      h_prev[jb] = hnew[jb];
+      h_sum[jb] += yv;
+      pend_y[jb] = yv;
+      pend_s[jb][0] = r;
+      pend_s[jb][1] = z;
+      pend_s[jb][2] = n;
+      pend_sx[jb] = hn;
+    }
+
+    if (step + 1 < T) {
+      // own copy with ordinary stores; after __syncwarp the warp's k-step is 16 contiguous float4 that go to the peers
+      // with st.async (ordering of the local path: allgather_units)
+      float* h_nxt = h_s + nxt * BS * H;
+#pragma unroll
+      for (int jb = 0; jb < 2; ++jb) h_nxt[tc_state_index(ju, 2 * ft + jb)] = hnew[jb];
+      __syncwarp();
+      if (lane < 16) {
+        float* mine = h_nxt + (j0 + u0) / 8 * 64 + lane * 4;
+        const float4 v = *reinterpret_cast<const float4*>(mine);
+        const uint32_t dst = ptx::smem_u32(mine), bar = ptx::smem_u32(&bars[nxt * C + rank]);
+#pragma unroll
+        for (int r = 1; r < C; ++r) {
+          const uint32_t peer = (rank + r) % C;
+          ptx::st_async_v4(ptx::mapa(dst, peer), v, ptx::mapa(bar, peer));
+        }
+      }
+      if (lane == 0) ptx::mbar_arrive(&bars[nxt * C + rank]);
+    }
+
+    if (step == T - 1) {
+      flush_pending(t);
+#pragma unroll
+      for (int jb = 0; jb < 2; ++jb) {
+        if (!valid[jb]) continue;
+        const int b = bb + jb;
+        p.h_n[((size_t)dir * B + b) * H + ju] = hnew[jb];
+        if (p.y_pool) p.y_pool[(size_t)b * p.D * H + dir * H + ju] = h_sum[jb];
+      }
+    } else {
+      load_gi(dir ? (T - 2 - step) : (step + 1));  // consumed at the next gate math
+    }
+  }
+  ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
+}
+
+// =================================================================================================
 // backward (BPTT)
 // =================================================================================================
 // w_prep layout (written by whh_prep_kernel): [C ranks][G][HS][H],
@@ -731,6 +1006,20 @@ bool try_fwd(const RecFwdParams& p, cudaStream_t s, bool force, int* rc) {
   return true;
 }
 
+// the tensor-core config is the widest-cluster one: it always launches (several waves when its clusters do not all fit)
+int run_fwd_tc(const RecFwdParams& p, cudaStream_t s) {
+  using Cfg = TcFwdCfg;
+  static_assert(Cfg::SMEM <= MAX_SMEM, "forward config does not fit an SM");
+  auto k = p.lengths ? rec_fwd_tc_kernel<true> : rec_fwd_tc_kernel<false>;
+  const int nslices = (p.B + Cfg::BS - 1) / Cfg::BS;
+  const int nclusters = nslices * p.D;
+  static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
+  if (debug)
+    fprintf(stderr, "[b200rnn] fwd cfg tc8 C=%d BS=%d mma.sync 3xTF32: need %d clusters, capacity %d, smem %zu\n", Cfg::C,
+            Cfg::BS, nclusters, max_active_clusters(k, Cfg::C, Cfg::NT, Cfg::SMEM), (size_t)Cfg::SMEM);
+  return launch_clustered(k, p, nslices, nclusters, Cfg::C, Cfg::NT, Cfg::SMEM, s, PROF_REC_FWD);
+}
+
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
 bool try_bwd(RecBwdParams& p, cudaStream_t s, bool force, int* rc) {
   using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
@@ -779,17 +1068,20 @@ int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
     //       8 warps per CTA
     //   bs8 <4,8,16,2,0> two unit groups per warp (NG = 2, rnn_core.cuh dots_chunk_ng): all three gate blocks in
     //       shared memory (213 KB), 8 warps per CTA; twice the FFMA work per CTA and step of bs4 on half the SMs
+    //   tc8 8 batch rows, the contraction on the tensor cores (rec_fwd_tc_kernel, mma.sync 3xTF32), 8 warps per CTA
     // A cluster cannot span GPCs, and H100 SXM GPCs are floor-swept unevenly, so the number of co-resident 4-CTA clusters
     // (30 on a 132-SM card measured) comes from the driver (try_fwd), never from the SM count. Measured per layer launch
-    // at T = 120 (DESIGN.md): a config in one wave beats the next wider one, and bs8 in one wave beats bs4 in two.
-    // B200RNN_GRU_FWD=bs2|bs4|bs8 forces one config (A/B runs).
+    // at T = 120 (DESIGN.md): a config in one wave beats the next wider one, and tc8 in one wave beats bs4 in two; bs8
+    // (slower than tc8 at every B) only runs when forced.
+    // B200RNN_GRU_FWD=bs2|bs4|bs8|tc8 forces one config (A/B runs).
     static const char* forced = getenv("B200RNN_GRU_FWD");
     if (forced) {
       if (!strcmp(forced, "bs2")) try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, true, &rc);
       else if (!strcmp(forced, "bs4")) try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, true, &rc);
       else if (!strcmp(forced, "bs8")) try_fwd<B200RNN_GRU, 256, 4, 8, 16, 2, 0, false, 2>(p, s, true, &rc);
+      else if (!strcmp(forced, "tc8")) rc = run_fwd_tc(p, s);
       else {
-        set_error("B200RNN_GRU_FWD=%s: expected bs2, bs4 or bs8", forced);
+        set_error("B200RNN_GRU_FWD=%s: expected bs2, bs4, bs8 or tc8", forced);
         rc = B200RNN_ERR_INVALID;
       }
       return rc;
@@ -797,9 +1089,9 @@ int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
     static const int bs2 = env_variant("B200RNN_GRU_BS2", 1);  // =0: A/B switch
     if (bs2 && try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
     if (try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, false, &rc)) return rc;
-    // the widest clusters: one wave up to B = 8 x the 4-CTA cluster capacity, several waves beyond
-    try_fwd<B200RNN_GRU, 256, 4, 8, 16, 2, 0, false, 2>(p, s, true, &rc);
-    return rc;
+    // the widest clusters, on the tensor cores (rec_fwd_tc_kernel; 0.32 ms per launch at T = 120 against 0.40 for
+    // bs8): one wave up to B = 8 x the 4-CTA cluster capacity, several waves beyond
+    return run_fwd_tc(p, s);
   }
   if (p.mode == B200RNN_GRU && p.H == 128) {
     if (try_fwd<B200RNN_GRU, 128, 2, 4, 16, 4, 1>(p, s, false, &rc)) return rc;
