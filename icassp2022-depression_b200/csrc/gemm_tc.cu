@@ -482,17 +482,11 @@ bool make_map(CUtensorMap* map, const float* ptr, int rows, int K, long long ld 
   return r == CUDA_SUCCESS;
 }
 
-bool tc_disabled() {
-  static const bool off = getenv("B200RNN_NO_TC") != nullptr;
-  return off;
-}
-
 }  // namespace
 
 size_t gemm_tc_scratch_bytes(int M, int N, int K) { return (size_t)2 * ((size_t)M + N) * K * sizeof(float) + 1024; }
 
 bool gemm_tc_eligible(const GemmParams& p, size_t ws_bytes) {
-  if (tc_disabled()) return false;
   if (p.accumulate) return false;
   if (p.M < 1 || p.K < BK || p.K % BK != 0 || p.N % BN != 0) return false;
   if (!p.a_kcontig && p.M % 4 != 0) return false;  // MN-major split copies are dense [K][M]: rows must stay 16-byte aligned
@@ -515,7 +509,7 @@ int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, flo
   return B200RNN_OK;
 }
 
-bool tc_available() { return !tc_disabled() && get_encoder() != nullptr; }
+bool tc_available() { return get_encoder() != nullptr; }
 
 float* tc_a_hi(void* ws) { return reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255); }
 float* tc_a_lo(void* ws, int M, int K) { return tc_a_hi(ws) + (size_t)M * K; }

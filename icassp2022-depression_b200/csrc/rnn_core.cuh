@@ -124,40 +124,6 @@ __device__ __forceinline__ void dots_chunk(const float* __restrict__ W_s, int gr
   }
 }
 
-// Same chunk contraction for NG groups of UPW units per warp (group ug = rows row0 + ug*UPW ..): the BS state loads of
-// a chunk serve all NG groups, so a CTA with NG = 2 reads the state half as often per FFMA as one with a warp per group.
-// Every weight row lives in shared memory. acc[ug * NRG + r] accumulates gate block r of group ug.
-template <int NG, int NRG, int KL, int UPL, int BS, int KLEN, int VSTRIDE>
-__device__ __forceinline__ void dots_chunk_ng(const float* __restrict__ W_s, int group_stride, int row0,
-                                              const float* __restrict__ vec_s, int ca, int lane,
-                                              float (&acc)[NG * NRG][UPL][BS]) {
-  using LM = LaneMap<KL, UPL, BS>;
-  static_assert(KLEN % (4 * KL) == 0, "contraction length must be a multiple of 4*KL");
-  const int kl = LM::kl(lane), p = LM::p(lane), q = LM::q(lane), cgrp = LM::cl(lane);
-  const int koff = ca * 4 * KL + kl * 4;
-  float4 hv[BS];
-#pragma unroll
-  for (int ab = 0; ab < BS; ++ab) hv[ab] = *reinterpret_cast<const float4*>(&vec_s[(ab ^ q) * VSTRIDE + koff]);
-#pragma unroll
-  for (int ug = 0; ug < NG; ++ug)
-#pragma unroll
-    for (int r = 0; r < NRG; ++r)
-#pragma unroll
-      for (int au = 0; au < UPL; ++au) {
-        const int row = r * group_stride + row0 + ug * LM::UPW + cgrp * UPL + (au ^ p);
-        const float4 wv = *reinterpret_cast<const float4*>(&W_s[row * KLEN + koff]);
-#pragma unroll
-        for (int ab = 0; ab < BS; ++ab) {
-          float a = acc[ug * NRG + r][au][ab];
-          a = fmaf(wv.x, hv[ab].x, a);
-          a = fmaf(wv.y, hv[ab].y, a);
-          a = fmaf(wv.z, hv[ab].z, a);
-          a = fmaf(wv.w, hv[ab].w, a);
-          acc[ug * NRG + r][au][ab] = a;
-        }
-      }
-}
-
 // Two independent round-to-nearest FMAs on the halves of a float2. sm_90 has no packed fp32 FMA, so this is two FFMA;
 // each half rounds exactly like fma.rn.f32, so the paired contractions below give the same bits as scalar FMA chains.
 __device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {

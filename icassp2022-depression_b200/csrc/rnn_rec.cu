@@ -20,9 +20,10 @@
 // fp32 FFMA for most configs: the per-step contraction is [BS x H] x [H x G*HS] with BS = 2..8 rows per CTA — far too
 // skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference. The GRU H=256 8-row config runs it
 // on the tensor cores with warp-level mma.sync (N = 8) in 3xTF32 instead (rec_fwd_tc_kernel).
+#include <map>
 #include <mutex>
 #include <stdlib.h>
-#include <string.h>
+#include <utility>
 
 #include "profile.cuh"
 #include "ptx.cuh"
@@ -46,14 +47,13 @@ constexpr bool kLocalSelf = true;
 #endif
 constexpr unsigned FULLMASK = 0xffffffffu;
 
-// NG: unit groups per warp (forward): a warp contracts NG groups of UPW units against the same state loads
-template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, int NG = 1>
+template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
 struct RecCfg {
   static constexpr int G = (MODE == B200RNN_GRU) ? 3 : 4;
   static constexpr int GH = G * H;
   static constexpr int HS = H / C;
-  static constexpr int UPW = (32 / KL) * UPL;  // units per warp and unit group
-  static constexpr int NW = HS / (UPW * NG);
+  static constexpr int UPW = (32 / KL) * UPL;  // units per warp
+  static constexpr int NW = HS / UPW;
   static constexpr int NT = NW * 32;
   static constexpr int NSM = G - RG;  // gate blocks held in shared memory
   static constexpr int CW = 4 * KL;   // floats of the contraction dimension per chunk
@@ -69,7 +69,7 @@ struct RecCfg {
   static_assert(NBAR * 8 <= (int)BAR_BYTES, "barrier block too small");
   static_assert(ROT ? (HS % CW == 0) : (CW % HS == 0), "chunks must tile the per-CTA slices");
   static_assert(RG >= 0 && RG <= 2, "at most two register-resident gate blocks");
-  static_assert(HS * C == H && NW * UPW * NG == HS && NW >= 1, "bad split");
+  static_assert(HS * C == H && NW * UPW == HS && NW >= 1, "bad split");
   static_assert(UPW % 4 == 0, "the exchange packs 4 units per 16-byte store");
   static_assert(NT <= 1024, "too many threads");
 };
@@ -137,17 +137,116 @@ __device__ __forceinline__ void allgather_units(float val, float* vec_local, int
 // =================================================================================================
 // forward
 // =================================================================================================
-// VL = true: per-sequence lengths (PackedSequence semantics): past its length a sequence keeps its state and emits 0
+// One (unit j, batch row b) output of a forward lane, everything it does outside the contraction: the x-projection
+// prefetched one step ahead, the gate math and state update, the step's global stores, and the final h_n / c_n / y_pool
+// stores. VL: past its length a sequence keeps its state and emits 0 (PackedSequence semantics). A row past the batch
+// (!valid) computes on zeros and stores nothing.
+// The stores of a step are held in registers until flush(), which the kernels call behind the next step's first chunk:
+// between the exchange and the next contraction they sat on the serial path of every step (225 cycles).
+// Saved for the backward, in the format rec_bwd_kernel's load_step reads: gates[t][b][g*H + j] (the x-projection on
+// entry) is overwritten with the activated gate g (GRU r, z, n; LSTM i, f, g, o), and extra[t][b][j] holds
+// hn = (W_hn h_{t-1})_j + b_hn (GRU) or c_t (LSTM).
+template <int MODE, int H, bool VL>
+struct FwdCell {
+  static constexpr int G = (MODE == B200RNN_GRU) ? 3 : 4;
+  float* gates;
+  float* extra;
+  int j, b, len;
+  bool valid;
+  float bhn, h = 0.f, c = 0.f, h_sum = 0.f;
+  float gi[G];                       // x-projection of the step update() computes next
+  float pend_y, pend_s[G], pend_sx;  // stores of the last step update() computed
+
+  __device__ __forceinline__ FwdCell(const RecFwdParams& p, int dir, int j_, int b_)
+      : gates(p.gates[dir]), extra(p.extra[dir]), j(j_), b(b_), len(p.T), valid(b_ < p.B) {
+    bhn = (MODE == B200RNN_GRU) ? p.b_hh[dir][2 * H + j] : 0.f;
+    if constexpr (VL) {
+      if (valid) len = p.lengths[b];
+    }
+#pragma unroll
+    for (int g = 0; g < G; ++g) gi[g] = 0.f;
+  }
+
+  __device__ __forceinline__ void load_gi(const RecFwdParams& p, int t) {
+    if (valid) {
+      const float* gp = gates + ((size_t)t * p.B + b) * (G * H) + j;
+#pragma unroll
+      for (int g = 0; g < G; ++g) gi[g] = gp[g * H];
+    }
+  }
+
+  // step at time t from the recurrent pre-activations pre[g] = (W_hh h_{t-1})[g*H + j]; returns the new state
+  __device__ __forceinline__ float update(int t, const float (&pre)[G]) {
+    float hnew, s[G], sx;
+    if constexpr (MODE == B200RNN_GRU) {
+      const float r = sigmoid_f(gi[0] + pre[0]);
+      const float z = sigmoid_f(gi[1] + pre[1]);
+      const float hn = pre[2] + bhn;
+      const float n = tanh_f(gi[2] + r * hn);
+      hnew = n + z * (h - n);
+      if constexpr (VL) {
+        if (t >= len) hnew = h;
+      }
+      s[0] = r; s[1] = z; s[2] = n; sx = hn;
+    } else {
+      const float ig = sigmoid_f(gi[0] + pre[0]);
+      const float fg = sigmoid_f(gi[1] + pre[1]);
+      const float gg = tanh_f(gi[2] + pre[2]);
+      const float og = sigmoid_f(gi[3] + pre[3]);
+      float cnew = fmaf(fg, c, ig * gg);  // spelled out: which product is fused must not be left to the compiler
+      hnew = og * tanh_f(cnew);
+      if constexpr (VL) {
+        if (t >= len) {
+          cnew = c;
+          hnew = h;
+        }
+      }
+      c = cnew;
+      s[0] = ig; s[1] = fg; s[2] = gg; s[3] = og; sx = cnew;
+    }
+    h = hnew;
+    float yv = hnew;  // what the caller sees at this step
+    if constexpr (VL) {
+      if (t >= len) yv = 0.f;
+    }
+    h_sum += yv;
+    pend_y = yv;
+#pragma unroll
+    for (int g = 0; g < G; ++g) pend_s[g] = s[g];
+    pend_sx = sx;
+    return hnew;
+  }
+
+  // the stores of the last update(), which computed time t
+  __device__ __forceinline__ void flush(const RecFwdParams& p, int dir, int t) {
+    if (valid) {
+      if (p.y) p.y[(long long)t * p.y_st + (long long)b * p.y_sb + dir * H + j] = pend_y;
+      if (p.training) {
+        float* gp = gates + ((size_t)t * p.B + b) * (G * H) + j;
+#pragma unroll
+        for (int g = 0; g < G; ++g) gp[g * H] = pend_s[g];
+        extra[((size_t)t * p.B + b) * H + j] = pend_sx;
+      }
+    }
+  }
+
+  // after the last step: the final state and the sum over time of the output
+  __device__ __forceinline__ void finish(const RecFwdParams& p, int dir) {
+    if (valid) {
+      p.h_n[((size_t)dir * p.B + b) * H + j] = h;
+      if (p.y_pool) p.y_pool[(size_t)b * p.D * H + dir * H + j] = h_sum;
+      if (MODE == B200RNN_LSTM && p.c_n) p.c_n[((size_t)dir * p.B + b) * H + j] = c;
+    }
+  }
+};
+
 // PB = true: batch-paired contraction and state layout (rnn_core.cuh, dots_chunk2b), see launch_rec_fwd
-// NG = 2: every warp owns two groups of UPW units (rnn_core.cuh, dots_chunk_ng): half the warps, each state load serves
-// both groups, and every lane applies the gate math to two (unit, batch) outputs
-template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false, bool PB = false, int NG = 1>
-__global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1)
+template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false, bool PB = false>
+__global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     rec_fwd_kernel(const RecFwdParams p, const int nslices) {
-  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>;
-  static_assert(NG == 1 || (MODE == B200RNN_GRU && RG == 0 && !PB), "NG = 2: GRU, scalar FFMA, RG = 0");
+  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
   using LM = LaneMap<KL, UPL, BS>;
-  constexpr int G = Cfg::G, HS = Cfg::HS, NT = Cfg::NT, UPW = Cfg::UPW, NSM = Cfg::NSM, GH = Cfg::GH;
+  constexpr int G = Cfg::G, HS = Cfg::HS, NT = Cfg::NT, UPW = Cfg::UPW, NSM = Cfg::NSM;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* W_s = reinterpret_cast<float*>(smem_raw);                 // [NSM*HS][H]
   float* h_s = W_s + (size_t)NSM * HS * H;                         // [2][BS][H]
@@ -161,16 +260,14 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1
   const int slice = cid - dir * nslices;
   const int b0 = slice * BS;
   const int j0 = (int)rank * HS;
-  const int B = p.B, T = p.T;
+  const int T = p.T;
   const float* w_hh = p.w_hh[dir];
 
   if (tid == 0) {
     // [0]: weights (tx bytes). [1 + buf*C + src]: slice of source CTA `src` - remote sources complete tx bytes
-    // (one arrive.expect_tx by thread 0 per phase), the CTA's OWN slice is published by one plain arrive per warp and
-    // unit group
+    // (one arrive.expect_tx by thread 0 per phase), the CTA's OWN slice is published by one plain arrive per warp
     for (int i = 0; i < Cfg::NBAR; ++i)
-      ptx::mbar_init(&bars[i],
-                     (kLocalSelf && i >= 1 && (uint32_t)((i - 1) % C) == rank) ? (uint32_t)(Cfg::NW * NG) : 1u);
+      ptx::mbar_init(&bars[i], (kLocalSelf && i >= 1 && (uint32_t)((i - 1) % C) == rank) ? (uint32_t)Cfg::NW : 1u);
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -185,61 +282,14 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1
   for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
   const int rot = Cfg::ROT ? (int)rank * CPS : 0;
   float wreg[RG > 0 ? RG : 1][UPL][H / KL];
-  load_resident<RG, KL, UPL, BS, H>(w_hh, H, (long long)NSM * H + j0 + w * UPW * NG, rot, lane, wreg);
+  load_resident<RG, KL, UPL, BS, H>(w_hh, H, (long long)NSM * H + j0 + w * UPW, rot, lane, wreg);
   ptx::mbar_wait(&bars[0], 0);
   __syncthreads();
   ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
 
-  // ---- lane identity: after the butterfly this lane owns (unit, batch) of each unit group ----------------
-  const int uw = LM::unit(lane), qb = LM::q(lane);
-  const int ju = j0 + w * UPW * NG + uw;  // hidden unit of group 0; group ug owns ju + ug * UPW
-  const int b = b0 + qb;                  // batch row
-  const bool valid = b < B;
-  float* gates = p.gates[dir];
-  float* extra = p.extra[dir];
-  float bhn[NG];
-#pragma unroll
-  for (int ug = 0; ug < NG; ++ug) bhn[ug] = (MODE == B200RNN_GRU) ? p.b_hh[dir][2 * H + ju + ug * UPW] : 0.f;
-
-  float h_prev[NG], c_prev[NG], h_sum[NG];
-#pragma unroll
-  for (int ug = 0; ug < NG; ++ug) h_prev[ug] = c_prev[ug] = h_sum[ug] = 0.f;
-  int len_b = T;
-  if constexpr (VL) {
-    if (valid) len_b = p.lengths[b];
-  }
-  float gi[NG][G];
-#pragma unroll
-  for (int ug = 0; ug < NG; ++ug)
-#pragma unroll
-    for (int g = 0; g < G; ++g) gi[ug][g] = 0.f;
-  if (valid && T > 0) {
-    const int t0 = dir ? T - 1 : 0;
-    const float* gp = gates + ((size_t)t0 * B + b) * GH + ju;
-#pragma unroll
-    for (int ug = 0; ug < NG; ++ug)
-#pragma unroll
-      for (int g = 0; g < G; ++g) gi[ug][g] = gp[g * H + ug * UPW];
-  }
-
-  // Global stores of a step (output, saved gates) are DEFERRED into the next step, behind its first chunk: they used to
-  // sit between the exchange and the next contraction, i.e. on the serial path of every step (225 cycles).
-  float pend_y[NG], pend_s[NG][4], pend_sx[NG];
-  auto flush_pending = [&](int tp) {
-    if (valid) {
-#pragma unroll
-      for (int ug = 0; ug < NG; ++ug) {
-        const int j = ju + ug * UPW;
-        if (p.y) p.y[(long long)tp * p.y_st + (long long)b * p.y_sb + dir * H + j] = pend_y[ug];
-        if (p.training) {
-          float* gp = gates + ((size_t)tp * B + b) * GH + j;
-#pragma unroll
-          for (int g = 0; g < G; ++g) gp[g * H] = pend_s[ug][g];
-          extra[((size_t)tp * B + b) * H + j] = pend_sx[ug];
-        }
-      }
-    }
-  };
+  // ---- lane identity: after the butterfly this lane owns (unit, batch) ------------------------------
+  FwdCell<MODE, H, VL> cell(p, dir, j0 + w * UPW + LM::unit(lane), b0 + LM::q(lane));
+  if (T > 0) cell.load_gi(p, dir ? T - 1 : 0);
 
   for (int step = 0; step < T; ++step) {
     const int t = dir ? (T - 1 - step) : step;
@@ -259,12 +309,12 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1
     // folded before the butterfly) or batch-paired (PACKB: float2 = two batch rows of one unit, one weight for both,
     // state kept in the paired shared-memory layout); the LSTM keeps scalar accumulators
     constexpr bool PACKB = PB;
-    constexpr bool PACK2 = !PACKB && NG == 1 && (MODE == B200RNN_GRU) && RG < 2;
+    constexpr bool PACK2 = !PACKB && (MODE == B200RNN_GRU) && RG < 2;
     float2 acc2[PACK2 ? G : 1][UPL][BS];
     float2 acc2b[PACKB ? G : 1][UPL][BS / 2];
-    float acc[NG * G][UPL][BS];  // [ug * G + g]
+    float acc[G][UPL][BS];
 #pragma unroll
-    for (int g = 0; g < NG * G; ++g)
+    for (int g = 0; g < G; ++g)
 #pragma unroll
       for (int au = 0; au < UPL; ++au)
 #pragma unroll
@@ -291,11 +341,9 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1
         dots_chunk2b<G, RG, KL, UPL, BS, H>(W_s, HS, w * UPW, wreg, h_cur, c, ca, lane, acc2b);
       else if constexpr (PACK2)
         dots_chunk2<G, RG, KL, UPL, BS, H, H>(W_s, HS, w * UPW, wreg, h_cur, c, ca, lane, acc2);
-      else if constexpr (NG > 1)
-        dots_chunk_ng<NG, G, KL, UPL, BS, H, H>(W_s, HS, w * UPW * NG, h_cur, ca, lane, acc);
       else
         dots_chunk<G, RG, KL, UPL, BS, H, H>(W_s, HS, w * UPW, wreg, h_cur, c, ca, lane, acc);
-      if (c == 0 && step > 0) flush_pending(dir ? (T - step) : (step - 1));  // the previous step's stores
+      if (c == 0 && step > 0) cell.flush(p, dir, dir ? (T - step) : (step - 1));  // the previous step's stores
     }
     // every slice of h_step has been consumed by this thread => the barriers of the other buffer are re-armed
     if (tid == 0 && step + 1 < T) {
@@ -311,81 +359,26 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>::NT, 1
       for (int g = 0; g < G; ++g) acc[g][0][0] = red[g];
     } else {
       if constexpr (PACK2) fold_pairs<G, UPL, BS>(acc2, acc);
-      warp_transpose_reduce<NG * G, KL, UPL, BS>(acc);
+      warp_transpose_reduce<G, KL, UPL, BS>(acc);
     }
     if (tr) trow[5] = clock64() + (long long)(acc[0][0][0] == 12345.678f);  // butterfly done (value dependence pins it)
 
-    float hnew[NG];
+    float pre[G];
 #pragma unroll
-    for (int ug = 0; ug < NG; ++ug) {
-      float s[4], sx;
-      if (MODE == B200RNN_GRU) {
-        const float r = sigmoid_f(gi[ug][0] + acc[ug * G][0][0]);
-        const float z = sigmoid_f(gi[ug][1] + acc[ug * G + 1][0][0]);
-        const float hn = acc[ug * G + 2][0][0] + bhn[ug];
-        const float n = tanh_f(gi[ug][2] + r * hn);
-        hnew[ug] = n + z * (h_prev[ug] - n);
-        if constexpr (VL) {
-          if (t >= len_b) hnew[ug] = h_prev[ug];
-        }
-        s[0] = r; s[1] = z; s[2] = n; s[3] = 0.f; sx = hn;
-      } else {
-        const float ig = sigmoid_f(gi[ug][0] + acc[ug * G][0][0]);
-        const float fg = sigmoid_f(gi[ug][1] + acc[ug * G + 1][0][0]);
-        const float gg = tanh_f(gi[ug][2] + acc[ug * G + 2][0][0]);
-        const float og = sigmoid_f(gi[ug][G - 1] + acc[ug * G + G - 1][0][0]);
-        float cnew = fg * c_prev[ug] + ig * gg;
-        hnew[ug] = og * tanh_f(cnew);
-        if constexpr (VL) {
-          if (t >= len_b) {
-            cnew = c_prev[ug];
-            hnew[ug] = h_prev[ug];
-          }
-        }
-        c_prev[ug] = cnew;
-        s[0] = ig; s[1] = fg; s[2] = gg; s[3] = og; sx = cnew;
-      }
-      h_prev[ug] = hnew[ug];
-      float yv = hnew[ug];  // what the caller sees at this step
-      if constexpr (VL) {
-        if (t >= len_b) yv = 0.f;
-      }
-      h_sum[ug] += yv;
-      // this step's global stores wait in registers until the next step's first chunk has been issued
-      pend_y[ug] = yv;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) pend_s[ug][g] = s[g];
-      pend_sx[ug] = sx;
-    }
-    if (tr) trow[6] = clock64() + (long long)(hnew[0] == 12345.678f);       // gate math done
+    for (int g = 0; g < G; ++g) pre[g] = acc[g][0][0];
+    const float hnew = cell.update(t, pre);
+    if (tr) trow[6] = clock64() + (long long)(hnew == 12345.678f);          // gate math done
 
-    if (step + 1 < T) {
-#pragma unroll
-      for (int ug = 0; ug < NG; ++ug)
-        allgather_units<C, KL, UPL, BS, kLocalSelf, PACKB>(hnew[ug], h_nxt, H, j0 + (w * NG + ug) * UPW,
-                                                           &bars[1 + nxt * C + rank], lane, rank);
-    }
+    if (step + 1 < T)
+      allgather_units<C, KL, UPL, BS, kLocalSelf, PACKB>(hnew, h_nxt, H, j0 + w * UPW, &bars[1 + nxt * C + rank], lane,
+                                                         rank);
     if (tr) trow[7] = clock64();                                            // exchange issued
 
-    // prefetch of the next step's x-projection (long latency, consumed at the next gate math)
-    if (step == T - 1) flush_pending(t);
-    if (valid) {
-#pragma unroll
-      for (int ug = 0; ug < NG; ++ug) {
-        const int j = ju + ug * UPW;
-        if (step == T - 1) {
-          p.h_n[((size_t)dir * B + b) * H + j] = hnew[ug];
-          if (p.y_pool) p.y_pool[(size_t)b * p.D * H + dir * H + j] = h_sum[ug];
-          if (MODE == B200RNN_LSTM && p.c_n) p.c_n[((size_t)dir * B + b) * H + j] = c_prev[ug];
-        }
-        if (step + 1 < T) {
-          const int tn = dir ? (T - 2 - step) : (step + 1);
-          const float* gp = gates + ((size_t)tn * B + b) * GH + j;
-#pragma unroll
-          for (int g = 0; g < G; ++g) gi[ug][g] = gp[g * H];
-        }
-      }
+    if (step == T - 1) {
+      cell.flush(p, dir, t);
+      cell.finish(p, dir);
     }
+    if (step + 1 < T) cell.load_gi(p, dir ? (T - 2 - step) : (step + 1));  // long latency, consumed at the next gate math
   }
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
 }
@@ -433,8 +426,8 @@ __device__ __forceinline__ int tc_state_index(int k, int b) {
 template <bool VL>
 __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFwdParams p, const int nslices) {
   using Cfg = TcFwdCfg;
-  constexpr int H = Cfg::H, C = Cfg::C, BS = Cfg::BS, G = Cfg::G, GH = Cfg::GH, HS = Cfg::HS, NUG = Cfg::NUG,
-                NW = Cfg::NW, NT = Cfg::NT, KS = Cfg::KS, KSC = Cfg::KSC;
+  constexpr int H = Cfg::H, C = Cfg::C, BS = Cfg::BS, G = Cfg::G, HS = Cfg::HS, NUG = Cfg::NUG, NW = Cfg::NW,
+                NT = Cfg::NT, KS = Cfg::KS, KSC = Cfg::KSC;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float4* W_f = reinterpret_cast<float4*>(smem_raw);                  // [NUG][G][KS][32 lanes] A fragments
   float* h_s = reinterpret_cast<float*>(smem_raw + Cfg::W_BYTES);     // [2][BS * H] B-fragment order
@@ -449,7 +442,7 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
   const int slice = cid - dir * nslices;
   const int b0 = slice * BS;
   const int j0 = (int)rank * HS;
-  const int B = p.B, T = p.T;
+  const int T = p.T;
   const float* w_hh = p.w_hh[dir];
 
   if (tid == 0) {
@@ -477,59 +470,15 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
   __syncthreads();
   ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
 
-  // ---- lane identity: output jb is unit ju, batch row bb + jb (accumulator fragment elements 2*kh + jb) ----------
+  // ---- lane identity: output jb is unit ju, batch row b0 + 2 * ft + jb (accumulator fragment elements 2*kh + jb) ---
   const int fg = lane >> 2, ft = lane & 3;
   const int u0 = ug * 16 + kh * 8;  // first unit (within the CTA's slice) this warp finishes
   const int ju = j0 + u0 + fg;
-  const int bb = b0 + 2 * ft;
-  bool valid[2];
-  int len_b[2];
+  FwdCell<B200RNN_GRU, H, VL> cell[2] = {{p, dir, ju, b0 + 2 * ft}, {p, dir, ju, b0 + 2 * ft + 1}};
+  if (T > 0) {
 #pragma unroll
-  for (int jb = 0; jb < 2; ++jb) {
-    valid[jb] = bb + jb < B;
-    len_b[jb] = T;
-    if constexpr (VL) {
-      if (valid[jb]) len_b[jb] = p.lengths[bb + jb];
-    }
+    for (int jb = 0; jb < 2; ++jb) cell[jb].load_gi(p, dir ? T - 1 : 0);
   }
-  float* gates = p.gates[dir];
-  float* extra = p.extra[dir];
-  const float bhn = p.b_hh[dir][2 * H + ju];
-
-  float h_prev[2], h_sum[2], gi[2][G];
-#pragma unroll
-  for (int jb = 0; jb < 2; ++jb) {
-    h_prev[jb] = h_sum[jb] = 0.f;
-#pragma unroll
-    for (int g = 0; g < G; ++g) gi[jb][g] = 0.f;
-  }
-  auto load_gi = [&](int tn) {
-#pragma unroll
-    for (int jb = 0; jb < 2; ++jb)
-      if (valid[jb]) {
-        const float* gp = gates + ((size_t)tn * B + bb + jb) * GH + ju;
-#pragma unroll
-        for (int g = 0; g < G; ++g) gi[jb][g] = gp[g * H];
-      }
-  };
-  if (T > 0) load_gi(dir ? T - 1 : 0);
-
-  // a step's global stores (output, saved gates) wait in registers until the next step's first slice is contracted
-  float pend_y[2], pend_s[2][G], pend_sx[2];
-  auto flush_pending = [&](int tp) {
-#pragma unroll
-    for (int jb = 0; jb < 2; ++jb) {
-      if (!valid[jb]) continue;
-      const int b = bb + jb;
-      if (p.y) p.y[(long long)tp * p.y_st + (long long)b * p.y_sb + dir * H + ju] = pend_y[jb];
-      if (p.training) {
-        float* gp = gates + ((size_t)tp * B + b) * GH + ju;
-#pragma unroll
-        for (int g = 0; g < G; ++g) gp[g * H] = pend_s[jb][g];
-        extra[((size_t)tp * B + b) * H + ju] = pend_sx[jb];
-      }
-    }
-  };
 
   const float4* W_w = W_f + (size_t)ug * G * KS * 32 + lane;
   float* red_mine = red + w * 2 * G * 32 + lane;                         // written by this warp
@@ -581,7 +530,10 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
       for (int g = 0; g < G; ++g)
 #pragma unroll
         for (int i = 0; i < 4; ++i) acc[g][i] += d[g][0][i] + d[g][1][i];
-      if (c == 0 && step > 0) flush_pending(dir ? (T - step) : (step - 1));  // the previous step's stores
+      if (c == 0 && step > 0) {  // the previous step's stores
+#pragma unroll
+        for (int jb = 0; jb < 2; ++jb) cell[jb].flush(p, dir, dir ? (T - step) : (step - 1));
+      }
     }
     // every slice of h_step has been consumed by this thread => the barriers of the other buffer are re-armed
     if (tid == 0 && step + 1 < T) {
@@ -596,37 +548,16 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
 #pragma unroll
       for (int jb = 0; jb < 2; ++jb) red_mine[(g * 2 + jb) * 32] = kh ? acc[g][jb] : acc[g][2 + jb];
     ptx::named_barrier_sync(1 + ug, 64);
-    float pre[G][2];  // recurrent pre-activations of this lane's two outputs
+    float pre[2][G];  // recurrent pre-activations of this lane's two outputs
 #pragma unroll
     for (int g = 0; g < G; ++g)
 #pragma unroll
       for (int jb = 0; jb < 2; ++jb) {
-        pre[g][jb] = (kh ? acc[g][2 + jb] : acc[g][jb]) + red_partner[(g * 2 + jb) * 32];
+        pre[jb][g] = (kh ? acc[g][2 + jb] : acc[g][jb]) + red_partner[(g * 2 + jb) * 32];
       }
-
     float hnew[2];
 #pragma unroll
-    for (int jb = 0; jb < 2; ++jb) {
-      const float r = sigmoid_f(gi[jb][0] + pre[0][jb]);
-      const float z = sigmoid_f(gi[jb][1] + pre[1][jb]);
-      const float hn = pre[2][jb] + bhn;
-      const float n = tanh_f(gi[jb][2] + r * hn);
-      hnew[jb] = n + z * (h_prev[jb] - n);
-      float yv = hnew[jb];  // what the caller sees at this step
-      if constexpr (VL) {
-        if (t >= len_b[jb]) {
-          hnew[jb] = h_prev[jb];
-          yv = 0.f;
-        }
-      }
-      h_prev[jb] = hnew[jb];
-      h_sum[jb] += yv;
-      pend_y[jb] = yv;
-      pend_s[jb][0] = r;
-      pend_s[jb][1] = z;
-      pend_s[jb][2] = n;
-      pend_sx[jb] = hn;
-    }
+    for (int jb = 0; jb < 2; ++jb) hnew[jb] = cell[jb].update(t, pre[jb]);
 
     if (step + 1 < T) {
       // own copy with ordinary stores; after __syncwarp the warp's k-step is 16 contiguous float4 that go to the peers
@@ -649,16 +580,14 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
     }
 
     if (step == T - 1) {
-      flush_pending(t);
 #pragma unroll
-      for (int jb = 0; jb < 2; ++jb) {
-        if (!valid[jb]) continue;
-        const int b = bb + jb;
-        p.h_n[((size_t)dir * B + b) * H + ju] = hnew[jb];
-        if (p.y_pool) p.y_pool[(size_t)b * p.D * H + dir * H + ju] = h_sum[jb];
-      }
-    } else {
-      load_gi(dir ? (T - 2 - step) : (step + 1));  // consumed at the next gate math
+      for (int jb = 0; jb < 2; ++jb) cell[jb].flush(p, dir, t);
+#pragma unroll
+      for (int jb = 0; jb < 2; ++jb) cell[jb].finish(p, dir);
+    }
+    if (step + 1 < T) {
+#pragma unroll
+      for (int jb = 0; jb < 2; ++jb) cell[jb].load_gi(p, dir ? (T - 2 - step) : (step + 1));
     }
   }
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
@@ -909,101 +838,89 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 // =================================================================================================
 // launchers
 // =================================================================================================
-template <typename K>
-int prepare_kernel(K kernel, size_t smem) {
-  struct Done {
-    const void* k;
-    int dev;
-  };
-  static std::mutex mu;  // forward and autograd-backward threads both launch
-  static Done done[256];
-  static int ndone = 0;
-  const int dev = current_device();
-  std::lock_guard<std::mutex> lk(mu);
-  for (int i = 0; i < ndone; ++i)
-    if (done[i].k == (const void*)kernel && done[i].dev == dev) return B200RNN_OK;
-  B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  if (ndone < 256) done[ndone++] = Done{(const void*)kernel, dev};
-  return B200RNN_OK;
-}
-
-template <typename K, typename P>
-int launch_clustered(K kernel, const P& params, int nslices, int nclusters, int C, int NT, size_t smem,
-                     cudaStream_t stream, int prof_kind) {
-  int rc = prepare_kernel(kernel, smem);
-  if (rc) return rc;
-  ProfScope prof(prof_kind, stream);
+// Launch config of `nclusters` clusters of C CTAs; `attr` is the storage of the cluster dimension it points to.
+cudaLaunchConfig_t cluster_config(int nclusters, int C, int NT, size_t smem, cudaStream_t s, cudaLaunchAttribute* attr) {
+  attr->id = cudaLaunchAttributeClusterDimension;
+  attr->val.clusterDim.x = (unsigned)C;
+  attr->val.clusterDim.y = 1;
+  attr->val.clusterDim.z = 1;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(nclusters * C), 1, 1);
   cfg.blockDim = dim3((unsigned)NT, 1, 1);
   cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
+  cfg.stream = s;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, params, nslices));
-  count_launch();
+  return cfg;
+}
+
+// Once per (kernel, device): opt the kernel in to `smem` bytes of dynamic shared memory and ask the driver how many of
+// its clusters can be resident at once (0 when the query fails).
+int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capacity) {
+  static std::mutex mu;  // forward and autograd-backward threads both launch
+  static std::map<std::pair<const void*, int>, int> cache;
+  const std::pair<const void*, int> key(kernel, current_device());
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = cache.find(key);
+  if (it == cache.end()) {
+    B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = cluster_config(NUM_SMS, C, NT, smem, 0, &attr);
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) {
+      cudaGetLastError();
+      n = 0;
+    }
+    it = cache.emplace(key, n).first;
+  }
+  *capacity = it->second;
   return B200RNN_OK;
 }
 
-// how many clusters of this kernel can be resident at once (cached per kernel)
-template <typename K>
-int max_active_clusters(K kernel, int C, int NT, size_t smem) {
-  struct Entry {
-    const void* k;
-    int dev, n;
-  };
-  static std::mutex mu;
-  static Entry cache[256];
-  static int ncache = 0;
-  const int dev = current_device();
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    for (int i = 0; i < ncache; ++i)
-      if (cache[i].k == (const void*)kernel && cache[i].dev == dev) return cache[i].n;
-  }
-  if (prepare_kernel(kernel, smem) != B200RNN_OK) return 0;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(C * NUM_SMS), 1, 1);
-  cfg.blockDim = dim3((unsigned)NT, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)C;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) {
-    cudaGetLastError();
-    n = 0;
-  }
-  std::lock_guard<std::mutex> lk(mu);
-  if (ncache < 256) cache[ncache++] = Entry{(const void*)kernel, dev, n};
-  return n;
-}
+int no_prep(int) { return B200RNN_OK; }
 
-template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool PB = false, int NG = 1>
-bool try_fwd(const RecFwdParams& p, cudaStream_t s, bool force, int* rc) {
-  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG, NG>;
-  static_assert(Cfg::FWD_SMEM <= MAX_SMEM, "forward config does not fit an SM");
-  auto k = p.lengths ? rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, true, PB, NG>
-                     : rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, false, PB, NG>;
+// Launches `kernel` as D * ceil(B / BS) clusters of C CTAs if the driver reports them all co-resident, or regardless
+// when `force` (then in several waves if they do not fit). Returns false, having launched nothing, when the config is
+// not taken. Otherwise prep(nslices) runs first, and *rc is its status or the launch's. B200RNN_DEBUG prints one line
+// per config considered: "[b200rnn] <desc>: need N clusters, capacity M, smem S".
+template <typename K, typename P, typename Prep, typename... Args>
+bool try_clustered(K kernel, P& p, int C, int BS, int NT, size_t smem, int prof_kind, bool force, cudaStream_t s,
+                   int* rc, Prep prep, const char* desc, Args... desc_args) {
   const int nslices = (p.B + BS - 1) / BS;
   const int nclusters = nslices * p.D;
+  int capacity = 0;
+  *rc = cluster_capacity((const void*)kernel, C, NT, smem, &capacity);
+  if (*rc != B200RNN_OK) return true;
   static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
-  if (debug)
-    fprintf(stderr, "[b200rnn] fwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d PB=%d NG=%d: need %d clusters, capacity %d, smem %zu\n",
-            C, BS, KL, UPL, RG, (int)PB, NG, nclusters, max_active_clusters(k, C, Cfg::NT, Cfg::FWD_SMEM),
-            (size_t)Cfg::FWD_SMEM);
-  if (!force && nclusters > max_active_clusters(k, C, Cfg::NT, Cfg::FWD_SMEM)) return false;
-  *rc = launch_clustered(k, p, nslices, nclusters, C, Cfg::NT, Cfg::FWD_SMEM, s, PROF_REC_FWD);
+  if (debug) {
+    char what[96];
+    snprintf(what, sizeof(what), desc, desc_args...);
+    fprintf(stderr, "[b200rnn] %s: need %d clusters, capacity %d, smem %zu\n", what, nclusters, capacity, smem);
+  }
+  if (!force && nclusters > capacity) return false;
+  *rc = prep(nslices);
+  if (*rc != B200RNN_OK) return true;
+  ProfScope prof(prof_kind, s);
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = cluster_config(nclusters, C, NT, smem, s, &attr);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p, nslices);
+  if (e != cudaSuccess) {
+    set_error("cudaLaunchKernelEx of a recurrence kernel failed: %s", cudaGetErrorString(e));
+    *rc = B200RNN_ERR_CUDA;
+    return true;
+  }
+  count_launch();
   return true;
+}
+
+template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool PB = false>
+bool try_fwd(const RecFwdParams& p, cudaStream_t s, bool force, int* rc) {
+  using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
+  static_assert(Cfg::FWD_SMEM <= MAX_SMEM, "forward config does not fit an SM");
+  auto k = p.lengths ? rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, true, PB>
+                     : rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, false, PB>;
+  return try_clustered(k, p, C, BS, Cfg::NT, Cfg::FWD_SMEM, PROF_REC_FWD, force, s, rc, no_prep,
+                       "fwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d PB=%d", C, BS, KL, UPL, RG, (int)PB);
 }
 
 // the tensor-core config is the widest-cluster one: it always launches (several waves when its clusters do not all fit)
@@ -1011,13 +928,10 @@ int run_fwd_tc(const RecFwdParams& p, cudaStream_t s) {
   using Cfg = TcFwdCfg;
   static_assert(Cfg::SMEM <= MAX_SMEM, "forward config does not fit an SM");
   auto k = p.lengths ? rec_fwd_tc_kernel<true> : rec_fwd_tc_kernel<false>;
-  const int nslices = (p.B + Cfg::BS - 1) / Cfg::BS;
-  const int nclusters = nslices * p.D;
-  static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
-  if (debug)
-    fprintf(stderr, "[b200rnn] fwd cfg tc8 C=%d BS=%d mma.sync 3xTF32: need %d clusters, capacity %d, smem %zu\n", Cfg::C,
-            Cfg::BS, nclusters, max_active_clusters(k, Cfg::C, Cfg::NT, Cfg::SMEM), (size_t)Cfg::SMEM);
-  return launch_clustered(k, p, nslices, nclusters, Cfg::C, Cfg::NT, Cfg::SMEM, s, PROF_REC_FWD);
+  int rc = B200RNN_OK;
+  try_clustered(k, p, Cfg::C, Cfg::BS, Cfg::NT, Cfg::SMEM, PROF_REC_FWD, true, s, &rc, no_prep,
+                "fwd cfg tc8 C=%d BS=%d mma.sync 3xTF32", Cfg::C, Cfg::BS);
+  return rc;
 }
 
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
@@ -1025,27 +939,21 @@ bool try_bwd(RecBwdParams& p, cudaStream_t s, bool force, int* rc) {
   using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
   static_assert(Cfg::BWD_SMEM <= MAX_SMEM, "backward config does not fit an SM");
   auto k = p.lengths ? rec_bwd_kernel<MODE, H, C, BS, KL, UPL, RG, true> : rec_bwd_kernel<MODE, H, C, BS, KL, UPL, RG, false>;
-  const int nslices = (p.B + BS - 1) / BS;
-  const int nclusters = nslices * p.D;
-  if (!force && nclusters > max_active_clusters(k, C, Cfg::NT, Cfg::BWD_SMEM)) return false;
   // transposed, per-CTA contiguous copy of W_hh for this cluster width
-  for (int d = 0; d < p.D; ++d) {
-    whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], Cfg::G, H, C);
-    if (cudaGetLastError() != cudaSuccess) {
-      set_error("whh_prep launch failed");
-      *rc = B200RNN_ERR_CUDA;
-      return true;
+  auto prep = [&](int nslices) -> int {
+    for (int d = 0; d < p.D; ++d) {
+      whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], Cfg::G, H, C);
+      if (cudaGetLastError() != cudaSuccess) {
+        set_error("whh_prep launch failed");
+        return B200RNN_ERR_CUDA;
+      }
+      count_launch();
     }
-    count_launch();
-  }
-  p.nslices_out = nslices;
-  *rc = launch_clustered(k, p, nslices, nclusters, C, Cfg::NT, Cfg::BWD_SMEM, s, PROF_REC_BWD);
-  return true;
-}
-
-int env_variant(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
+    p.nslices_out = nslices;
+    return B200RNN_OK;
+  };
+  return try_clustered(k, p, C, BS, Cfg::NT, Cfg::BWD_SMEM, PROF_REC_BWD, force, s, rc, prep,
+                       "bwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d", C, BS, KL, UPL, RG);
 }
 
 }  // namespace
@@ -1066,31 +974,13 @@ int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
     //   bs2 <4,2,16,8,0>: all three gate blocks in shared memory, 4 warps per CTA
     //   bs4 <4,4,16,4,1> batch-paired (rnn_core.cuh dots_chunk2b): two gate blocks in shared memory, one in registers,
     //       8 warps per CTA
-    //   bs8 <4,8,16,2,0> two unit groups per warp (NG = 2, rnn_core.cuh dots_chunk_ng): all three gate blocks in
-    //       shared memory (213 KB), 8 warps per CTA; twice the FFMA work per CTA and step of bs4 on half the SMs
     //   tc8 8 batch rows, the contraction on the tensor cores (rec_fwd_tc_kernel, mma.sync 3xTF32), 8 warps per CTA
     // A cluster cannot span GPCs, and H100 SXM GPCs are floor-swept unevenly, so the number of co-resident 4-CTA clusters
-    // (30 on a 132-SM card measured) comes from the driver (try_fwd), never from the SM count. Measured per layer launch
-    // at T = 120 (DESIGN.md): a config in one wave beats the next wider one, and tc8 in one wave beats bs4 in two; bs8
-    // (slower than tc8 at every B) only runs when forced.
-    // B200RNN_GRU_FWD=bs2|bs4|bs8|tc8 forces one config (A/B runs).
-    static const char* forced = getenv("B200RNN_GRU_FWD");
-    if (forced) {
-      if (!strcmp(forced, "bs2")) try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, true, &rc);
-      else if (!strcmp(forced, "bs4")) try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, true, &rc);
-      else if (!strcmp(forced, "bs8")) try_fwd<B200RNN_GRU, 256, 4, 8, 16, 2, 0, false, 2>(p, s, true, &rc);
-      else if (!strcmp(forced, "tc8")) rc = run_fwd_tc(p, s);
-      else {
-        set_error("B200RNN_GRU_FWD=%s: expected bs2, bs4, bs8 or tc8", forced);
-        rc = B200RNN_ERR_INVALID;
-      }
-      return rc;
-    }
-    static const int bs2 = env_variant("B200RNN_GRU_BS2", 1);  // =0: A/B switch
-    if (bs2 && try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
+    // (30 on a 132-SM card measured) comes from the driver (try_clustered), never from the SM count. Measured per layer
+    // launch at T = 120 (DESIGN.md): a config in one wave beats the next wider one, and tc8 in one wave beats bs4 in two.
+    if (try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
     if (try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, false, &rc)) return rc;
-    // the widest clusters, on the tensor cores (rec_fwd_tc_kernel; 0.32 ms per launch at T = 120 against 0.40 for
-    // bs8): one wave up to B = 8 x the 4-CTA cluster capacity, several waves beyond
+    // the widest clusters: one wave up to B = 8 x the 4-CTA cluster capacity, several waves beyond
     return run_fwd_tc(p, s);
   }
   if (p.mode == B200RNN_GRU && p.H == 128) {
@@ -1122,8 +1012,7 @@ int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
   // (not the weights) dominates the shared-memory traffic of the backward contraction
   if (p.mode == B200RNN_GRU && p.H == 256) {
     // as in the forward: a config is taken only when the driver reports all its clusters co-resident
-    static const int bs2 = env_variant("B200RNN_GRU_BS2", 1);
-    if (bs2 && try_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
+    if (try_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
     if (try_bwd<B200RNN_GRU, 256, 4, 4, 32, 8, 1>(p, s, false, &rc)) return rc;
     try_bwd<B200RNN_GRU, 256, 8, 8, 32, 4, 1>(p, s, true, &rc);
     return rc;

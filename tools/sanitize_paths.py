@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Small shapes through every recurrence variant, for compute-sanitizer (memcheck / racecheck):
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py
-    B200RNN_GRU_BS2=0 compute-sanitizer --tool memcheck python tools/sanitize_paths.py rnn   # recurrence only, 4-row GRU clusters
+    compute-sanitizer --tool memcheck python tools/sanitize_paths.py rnn   # recurrence only
+The GRU H=256 layer also runs at B = 96, which needs the 4-row clusters (bs4: the 2-row ones do not all fit at once).
 """
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -13,18 +14,19 @@ torch.manual_seed(0)
 for kind, I, H, L, bi in (("gru", 64, 256, 2, False), ("lstm", 64, 128, 2, True), ("gru", 32, 128, 1, True), ("lstm", 32, 256, 1, False)):
     cls = b200rnn.GRU if kind == "gru" else b200rnn.LSTM
     m = cls(I, H, num_layers=L, bidirectional=bi, batch_first=True, dropout=0.3 if L > 1 else 0.0).to(dev).train()
-    B, T = 9, 6
-    x = torch.randn(B, T, I, device=dev, requires_grad=True)
-    y = m(x)[0]
-    y.sum().backward()
-    lengths = torch.tensor([6, 1, 3, 6, 2, 5, 4, 6, 1])
-    xp = pack_padded_sequence(x.detach().requires_grad_(True), lengths, batch_first=True, enforce_sorted=False)
-    yp = m(xp)[0]
-    yp.data.sum().backward()
-    with torch.no_grad():
-        m.eval()(x)
-    torch.cuda.synchronize()
-    print(kind, H, "ok", flush=True)
+    T = 6
+    for B in (9, 96) if (kind, H) == ("gru", 256) else (9,):
+        x = torch.randn(B, T, I, device=dev, requires_grad=True)
+        y = m.train()(x)[0]
+        y.sum().backward()
+        lengths = torch.tensor([6, 1, 3, 6, 2, 5, 4, 6, 1] * (B // 9) + [6] * (B % 9))
+        xp = pack_padded_sequence(x.detach().requires_grad_(True), lengths, batch_first=True, enforce_sorted=False)
+        yp = m(xp)[0]
+        yp.data.sum().backward()
+        with torch.no_grad():
+            m.eval()(x)
+        torch.cuda.synchronize()
+        print(kind, H, B, "ok", flush=True)
 if sys.argv[1:] == ["rnn"]:
     sys.exit(0)
 # round 2: the fused shells (LayerNorm prologue + pooled gradient under autograd, attention pooling fwd/bwd, Softmax+CE,

@@ -2,7 +2,8 @@
 """Debug: per-step, per-warp timeline (SM clock cycles) of the forward recurrence, CTA 0, lane 0 of each warp.
 Needs the -DB200RNN_TRACE build:  make -C icassp2022-depression_b200 trace
     B200RNN_LIB=$PWD/icassp2022-depression_b200/lib_trace/libb200rnn.so python tools/trace_rec.py [gru|lstm]
-Stamps per (step, warp): 0 step top | 1-4 wait for chunk 0..3 passed | 5 butterfly done | 6 gates done | 7 exchange issued."""
+Stamps per (step, warp): 0 step top | 1-4 wait for chunk 0..3 passed | 5 butterfly done | 6 gates done | 7 exchange issued.
+The GRU runs at B = 96, which takes the 4-row FFMA config (bs4); the tensor-core config (B > 120) has no stamps."""
 import ctypes, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "icassp2022-depression_b200"))
@@ -13,7 +14,7 @@ lib.b200rnn_debug_set_trace.argtypes = [ctypes.c_void_p]
 kind = sys.argv[1] if len(sys.argv) > 1 else "gru"
 dev = torch.device("cuda:0")
 if kind == "gru":
-    m = b200rnn.GRU(256, 256, num_layers=1, batch_first=True).to(dev).eval(); x = torch.randn(128, 120, 256, device=dev); T = 120; nch = 4
+    m = b200rnn.GRU(256, 256, num_layers=1, batch_first=True).to(dev).eval(); x = torch.randn(96, 120, 256, device=dev); T = 120; nch = 4
 else:
     m = b200rnn.LSTM(1024, 128, num_layers=1, bidirectional=True).to(dev).eval(); x = torch.randn(30, 128, 1024, device=dev); T = 30; nch = 2
 with torch.no_grad():
