@@ -120,6 +120,7 @@ struct ScratchLayout {
   // forward
   size_t f_gates[2], f_y[2], f_tc;
   size_t f_tc_bytes;
+  size_t f_ready;  // int per TC_TILE_M-row tile of the input projection: its finished column tiles (streamed GEMM)
   size_t f_total;
   // backward
   size_t b_dgates[2], b_dghn[2], b_wt[2], b_bpart[2], b_dy, b_gemm;
@@ -150,6 +151,8 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
     s->f_tc_bytes = gemm_tc_scratch_bytes((int)d.TB, (int)d.GH, Kmax);
     off += align_up(s->f_tc_bytes / sizeof(float) + 1, ALIGN_F);
   }
+  s->f_ready = off;
+  off += align_up((d.TB + TC_TILE_M - 1) / TC_TILE_M, ALIGN_F);
   s->f_total = off;
 
   off = 0;
@@ -320,6 +323,15 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
   }
 
   const bool tc = tc_available();
+  int sms = NUM_SMS;
+  {
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  // ready counters of a streamed input projection; every kernel that writes the GEMM's A operand zeroes them, so each
+  // layer (and each CUDA-graph replay) starts from zero without a launch of its own
+  int* ready = reinterpret_cast<int*>(S + sl.f_ready);
+  const int tiles_m = (int)((d.TB + TC_TILE_M - 1) / TC_TILE_M);
   bool a_ready = false;  // the next layer's A operand (hi/lo) was already produced by this layer's dropout pass
   for (int l = 0; l < d.L; ++l) {
     const int Il = l == 0 ? d.I : (int)d.DH;
@@ -336,27 +348,40 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
         in = S + sl.f_y[(l - 1) & 1];
       in_rows = simple_rows((long long)d.DH);
     }
-    // ---- A operand of the tensor-core input projection, prepared once per layer (shared by the directions)
     const bool tc_layer = tc && (Il % 32 == 0) && (d.GH % 128 == 0);
+    // ---- the recurrence config, chosen before anything of the layer is enqueued
+    RecFwdParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.mode = d.mode; rp.B = d.B; rp.T = d.T; rp.H = d.H; rp.D = d.D;
+    rp.training = save ? 1 : 0;
+    rp.lengths = lengths;
+    RecFwdLaunch rec;
+    rc = plan_rec_fwd(rp, &rec);
+    if (rc) return rc;
+    // Stream the input projection into the recurrence (DESIGN.md §4): the GEMM runs beside the recurrence and publishes
+    // its row tiles in time order, the recurrence starts while it runs and waits per step for the tiles it reads. Only
+    // when the recurrence is unidirectional (it walks t upwards), fits one wave of 4-CTA clusters and takes at most half
+    // of the SMs; the GEMM runs as 4-CTA clusters in the cluster slots the recurrence leaves free. Otherwise GEMM and
+    // recurrence run one after the other.
+    const int gemm_clusters = rec.capacity - rec.nclusters;
+    const bool stream_xproj = d.D == 1 && tc_layer && rec.C == 4 && rec.one_wave() && 2 * rec.ctas() <= sms &&
+                              gemm_clusters > 0;
+    // ---- A operand of the tensor-core input projection, prepared once per layer (shared by the directions)
     void* tc_ws = S + sl.f_tc;
     if (tc_layer) {
       float* a_hi = tc_a_hi(tc_ws);
       float* a_lo = tc_a_lo(tc_ws, (int)d.TB, Il);
       if (l == 0 && ln_gamma)
         rc = tc_layernorm_split(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, a_hi, a_lo, st,
-                                (save && fused_ln) ? R + rl.xln : nullptr);
+                                (save && fused_ln) ? R + rl.xln : nullptr, ready, tiles_m);
       else if (!a_ready)
-        rc = tc_split(in, in_rows, (int)d.TB, Il, a_hi, a_lo, st);
+        rc = tc_split(in, in_rows, (int)d.TB, Il, a_hi, a_lo, st, ready, tiles_m);
       if (rc) return rc;
     } else if (l == 0 && ln_gamma) {
       set_error("forward: the fused LayerNorm prologue needs the tensor-core input projection (input_size %% 32 == 0)");
       return B200RNN_ERR_UNSUPPORTED;
     }
     a_ready = false;
-    RecFwdParams rp;
-    memset(&rp, 0, sizeof(rp));
-    rp.mode = d.mode; rp.B = d.B; rp.T = d.T; rp.H = d.H; rp.D = d.D;
-    rp.training = save ? 1 : 0;
     for (int k = 0; k < d.D; ++k) {
       const float* const* pp = params + (size_t)(l * d.D + k) * 4;
       const float *w_ih = pp[0], *w_hh = pp[1], *b_ih = pp[2], *b_hh = pp[3];
@@ -386,6 +411,12 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
           g.tc_b_hi = WC + wl.hi[l][k];
           g.tc_b_lo = WC + wl.lo[l][k];
         }
+        if (stream_xproj && gemm_tc_eligible(g, g.tc_ws_bytes)) {
+          g.tc_ready = ready;
+          g.tc_stream_clusters = gemm_clusters;
+          rp.ready = ready;
+          rp.tiles_n = (int)d.GH / TC_TILE_N;
+        }
       }
       rc = launch_gemm(g, nullptr, 0, st);
       if (rc) return rc;
@@ -406,14 +437,15 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     rp.h_n = h_n + (size_t)l * d.D * d.B * d.H;
     rp.c_n = c_n ? c_n + (size_t)l * d.D * d.B * d.H : nullptr;
     rp.trace = g_trace;
-    rp.lengths = lengths;
-    rc = launch_rec_fwd(rp, st);
+    // Streamed, this launch directly follows the GEMM in the stream (nothing may be enqueued between them) and never
+    // comes first: launched after the GEMM, the recurrence waits only on a kernel whose CTAs have all started.
+    rc = launch_rec_fwd(rec, rp, st);
     if (rc) return rc;
     if (drop && l + 1 < d.L) {  // K7; keeps the raw output when it is needed by backward, else in place
       float* dropped = save ? R + rl.ydrop[l] : ylay;
       if (tc) {  // also emit the hi/lo split the next layer's tensor-core GEMM consumes (one pass instead of two)
         rc = launch_dropout_split(ylay, dropped, tc_a_hi(tc_ws), tc_a_lo(tc_ws, (int)d.TB, (int)d.DH), d.TB * d.DH, d.p, hdr,
-                                  (uint32_t)l, st);
+                                  (uint32_t)l, st, ready, tiles_m);
         a_ready = true;
       } else {
         rc = launch_dropout(ylay, dropped, d.TB * d.DH, d.p, hdr, (uint32_t)l, st);

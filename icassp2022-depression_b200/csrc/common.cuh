@@ -28,6 +28,9 @@ void count_launch(int n = 1);  // bumps the counter behind b200rnn_launch_count(
 constexpr int MAX_DEVICES = 64;
 // SMs of an H100 SXM: sizes the grid-stride launches (one or a few waves) and fixed-order partial-sum buffers
 constexpr int NUM_SMS = 132;
+// output tile of the tensor-core GEMM (gemm_tc.cu): a streamed input projection counts the finished TC_TILE_N-column
+// tiles of every TC_TILE_M-row tile of its output, and the forward recurrence waits on those counters (api.cu)
+constexpr int TC_TILE_M = 128, TC_TILE_N = 128;
 inline int current_device() {
   int d = 0;
   if (cudaGetDevice(&d) != cudaSuccess) {

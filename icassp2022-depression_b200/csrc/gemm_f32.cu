@@ -282,6 +282,10 @@ int launch_gemm(const GemmParams& p, void* scratch, size_t scratch_bytes, cudaSt
     return B200RNN_ERR_INVALID;
   }
   if (p.tc_ws && gemm_tc_eligible(p, p.tc_ws_bytes)) return launch_gemm_tc(p, p.tc_ws, p.tc_ws_bytes, stream);
+  if (p.tc_ready) {
+    set_error("gemm: a streamed launch needs the tensor-core path");
+    return B200RNN_ERR_INVALID;
+  }
   GemmDev d;
   d.A = p.A; d.a_rows = p.a_rows;
   d.B = p.B; d.b_rows = p.b_rows;

@@ -27,6 +27,12 @@ struct GemmParams {
   // (b200rnn_prepare_weights: frozen encoders split their W_ih once, not once per step)
   const float* tc_b_hi;
   const float* tc_b_lo;
+  // optional, tensor-core path only: streamed launch. ready[m] counts the finished n-tiles of row tile m (TC_TILE_M
+  // rows); the tiles are walked time-major by tc_stream_clusters 4-CTA clusters, and the launch lets the next kernel
+  // in the stream start early (the forward recurrence, which waits on these counters). The counters must be zero on
+  // entry.
+  int* tc_ready;
+  int tc_stream_clusters;
 };
 
 // where launch_gemm_tc expects / puts the split A operand inside its workspace
@@ -34,8 +40,10 @@ float* tc_a_hi(void* ws);
 float* tc_a_lo(void* ws, int M, int K);
 // LayerNorm over the last dimension fused with the TF32 split: hi/lo <- split(LN(src row) * gamma + beta)
 // `out` (optional): dense [R][Cc] copy of LN(src) kept for the backward pass (layer-0 wgrad operand)
+// `clear` (optional): nclear ints zeroed by the same launch (the ready counters of a streamed GEMM that reads hi / lo)
 int tc_layernorm_split(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta,
-                       float eps, float* hi, float* lo, cudaStream_t stream, float* out = nullptr);
+                       float eps, float* hi, float* lo, cudaStream_t stream, float* out = nullptr,
+                       int* clear = nullptr, int nclear = 0);
 // backward of that prologue: dx (strided like x) from dy = d/dLN(x) (dense), dgamma / dbeta (+)=; part = scratch of
 // layernorm_bwd_scratch_floats(Cc) floats
 size_t layernorm_bwd_scratch_floats(int Cc);
@@ -57,10 +65,12 @@ struct TcOperand {
                     // for operands whose contraction index is their row index: dG, X, h_prev in the wgrad GEMMs)
 };
 bool tc_available();
-int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream);
+int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream,
+             int* clear = nullptr, int nclear = 0);
+// ready: streamed launch of stream_clusters 4-CTA clusters (GemmParams::tc_ready); needs splitk_ws == NULL
 int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
                      const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
-                     size_t splitk_ws_bytes, cudaStream_t stream);
+                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready = nullptr, int stream_clusters = 0);
 // C(m,n) (+)= sum_z partial[z][m][n] (+ biases), fixed order (deterministic)
 int launch_splitk_reduce(const float* partial, int splitk, int M, int N, float* C, const RowMap& c_rows,
                          const float* bias1, const float* bias2, int bias2_n, int accumulate, cudaStream_t stream);

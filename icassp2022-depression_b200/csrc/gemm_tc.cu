@@ -21,6 +21,7 @@
 //                   12 per stage, then the round-to-nearest flush and finally the epilogue (+ folded biases).
 #include <cuda.h>  // CUtensorMap types only; the encoder is fetched through cudaGetDriverEntryPoint
 #include <mutex>
+#include <stdlib.h>
 
 #include "gemm_f32.cuh"
 #include "profile.cuh"
@@ -30,7 +31,7 @@ namespace b200rnn {
 
 namespace {
 
-constexpr int BM = 128, BN = 128, BK = 32, STAGES = 3;
+constexpr int BM = TC_TILE_M, BN = TC_TILE_N, BK = 32, STAGES = 3;
 constexpr int LNB_BLOCKS = NUM_SMS * 2;  // CTAs of the LayerNorm backward (per-CTA column partials, reduced in fixed order)
 constexpr int TILE_BYTES = BM * BK * 4;        // 16 KB, both A and W tiles (BM == BN)
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;    // A_hi, A_lo, W_hi, W_lo
@@ -106,7 +107,20 @@ struct TcArgs {
   int splitk;       // > 1: work item = (k-split, tile); raw partial sums go to partial[ks][M][N]
   int kb_per_split; // k-blocks per split
   float* partial;
+  int* ready;       // streamed (splitk == 1): tiles walked time-major, ready[m] += 1 per finished tile of row tile m
 };
+
+// work item -> output tile origin: m fastest (consecutive tiles of a CTA mostly share their W tile rows in L2), or
+// time-major when streamed (the consumer reads row tile m after m - 1)
+__device__ __forceinline__ void tile_origin(const TcArgs& a, int tile, int& m0, int& n0) {
+  if (a.ready) {
+    m0 = (tile / a.tiles_n) * BM;
+    n0 = (tile % a.tiles_n) * BN;
+  } else {
+    m0 = (tile % a.tiles_m) * BM;
+    n0 = (tile / a.tiles_m) * BN;
+  }
+}
 
 // One 128 x BK tile of an MN-major operand (src: [K rows][ext columns], leading dimension ld) into the K-major
 // 128-byte-swizzled layout: thread t owns tile row t (= source column c0 + t), its 32 k values go out as 8 float4
@@ -124,9 +138,12 @@ __device__ __forceinline__ void load_mn_tile(unsigned char* tile, const float* _
     *reinterpret_cast<float4*>(row + ((j ^ (t & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
 }
 
-// Persistent: each CTA walks work items blockIdx.x, +gridDim.x, ... (m fastest, so consecutive tiles of a CTA mostly
-// share their W tile rows in L2). Producer and consumers loop independently over the same item sequence and meet only
-// through the full / empty mbarriers of the shared-memory ring.
+// Persistent: each CTA walks work items blockIdx.x, +gridDim.x, ... (tile_origin). Producer and consumers loop
+// independently over the same item sequence and meet only through the full / empty mbarriers of the shared-memory ring.
+// Streamed (args.ready, api.cu): the kernel lets the next kernel of the stream launch at once (griddepcontrol), and
+// after a tile's stores the consumer warpgroups publish it with one release increment of ready[m]. Every read of the
+// A operand of a tile precedes that increment (the consumers have drained the ring stages of the tile), and the kernel
+// itself never waits on anything outside its CTA.
 __global__ void __launch_bounds__(TC_THREADS, 1)
     gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                        const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
@@ -143,6 +160,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   const int nkb_total = (args.K + BK - 1) / BK;  // the K tail reads as zero
   const int ntiles = args.tiles_m * args.tiles_n;
   const int nitems = ntiles * args.splitk;
+  if (args.ready) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
@@ -167,7 +185,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     int it = 0;  // running k-block counter across items (ring position)
     for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       const int tile = item % ntiles, ks = item / ntiles;
-      const int m0 = (tile % args.tiles_m) * BM, n0 = (tile / args.tiles_m) * BN;
+      int m0, n0;
+      tile_origin(args, tile, m0, n0);
       const int kb0 = ks * args.kb_per_split;
       const int kb1 = min(nkb_total, kb0 + args.kb_per_split);
       for (int kb = kb0; kb < kb1; ++kb, ++it) {
@@ -208,7 +227,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       const int tile = item % ntiles, ks = item / ntiles;
       const int nkb = min(nkb_total, (ks + 1) * args.kb_per_split) - ks * args.kb_per_split;
-      const int m0 = (tile % args.tiles_m) * BM, n0 = (tile / args.tiles_m) * BN;
+      int m0, n0;
+      tile_origin(args, tile, m0, n0);
       float total[64], acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) total[i] = 0.f;
@@ -264,6 +284,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           *reinterpret_cast<float2*>(crow + col) = o;
         }
       }
+      if (args.ready) {  // publish the tile: every storing thread fences, the 256 consumer threads meet, one releases
+        __threadfence();
+        ptx::named_barrier_sync(1, 256);
+        if (threadIdx.x == 128)
+          asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(args.ready + m0 / BM) : "memory");
+      }
     }
   }
 }
@@ -271,7 +297,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 // x = hi + lo with hi = round-to-nearest TF32 (kept in a 32-bit container), lo = x - hi (exact in fp32).
 // Reads rows through a RowMap (batch_first / permuted inputs), writes two dense [M,K] matrices.
 __global__ void split_tf32_kernel(const float* __restrict__ src, RowMap rows, int M, int K, float* __restrict__ hi,
-                                  float* __restrict__ lo, int vec_ok) {
+                                  float* __restrict__ lo, int vec_ok, int* __restrict__ clear, int nclear) {
+  if (blockIdx.x == 0)
+    for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
   const size_t nvec = (size_t)M * (K / 4);
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nvec; i += (size_t)gridDim.x * blockDim.x) {
     const int m = (int)(i / (K / 4));
@@ -299,7 +327,10 @@ __global__ void split_tf32_kernel(const float* __restrict__ src, RowMap rows, in
 template <int NV>  // float4 per lane
 __global__ void layernorm_split_kernel(const float* __restrict__ src, RowMap rows, int R, int Cc,
                                        const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                                       float* __restrict__ hi, float* __restrict__ lo, float* __restrict__ out) {
+                                       float* __restrict__ hi, float* __restrict__ lo, float* __restrict__ out,
+                                       int* __restrict__ clear, int nclear) {
+  if (blockIdx.x == 0)
+    for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
   for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < R; r += gridDim.x * wpb) {
@@ -496,14 +527,15 @@ bool gemm_tc_eligible(const GemmParams& p, size_t ws_bytes) {
   return get_encoder() != nullptr;
 }
 
-int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream) {
+int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream,
+             int* clear, int nclear) {
   const bool vec = (reinterpret_cast<uintptr_t>(src) & 15u) == 0 && rows.s_outer % 4 == 0 && rows.s_inner % 4 == 0;
   size_t nv = (size_t)R * (Cc / 4);
   int blocks = (int)((nv + 255) / 256);
   if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
   if (blocks < 1) blocks = 1;
   ProfScope prof(PROF_MISC, stream);
-  split_tf32_kernel<<<blocks, 256, 0, stream>>>(src, rows, R, Cc, hi, lo, vec ? 1 : 0);
+  split_tf32_kernel<<<blocks, 256, 0, stream>>>(src, rows, R, Cc, hi, lo, vec ? 1 : 0, clear, clear ? nclear : 0);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;
@@ -515,7 +547,7 @@ float* tc_a_hi(void* ws) { return reinterpret_cast<float*>((reinterpret_cast<uin
 float* tc_a_lo(void* ws, int M, int K) { return tc_a_hi(ws) + (size_t)M * K; }
 
 int tc_layernorm_split(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta,
-                       float eps, float* hi, float* lo, cudaStream_t stream, float* out) {
+                       float eps, float* hi, float* lo, cudaStream_t stream, float* out, int* clear, int nclear) {
   const bool vec = (reinterpret_cast<uintptr_t>(src) & 15u) == 0 && rows.s_outer % 4 == 0 && rows.s_inner % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0 && (reinterpret_cast<uintptr_t>(beta) & 15u) == 0;
   if (!vec || !(Cc == 128 || Cc == 256 || Cc == 512 || Cc == 1024)) {
@@ -525,12 +557,16 @@ int tc_layernorm_split(const float* src, const RowMap& rows, int R, int Cc, cons
   int blocks = (R + 7) / 8;
   if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
   ProfScope prof(PROF_MISC, stream);
+  if (!clear) nclear = 0;
+#define B200_LNS(NV_) \
+  layernorm_split_kernel<NV_><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, hi, lo, out, clear, nclear)
   switch (Cc / 128) {  // instantiated widths: 128, 256, 512, 1024 (the reference normalises 256-d audio features)
-    case 1: layernorm_split_kernel<1><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, hi, lo, out); break;
-    case 2: layernorm_split_kernel<2><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, hi, lo, out); break;
-    case 4: layernorm_split_kernel<4><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, hi, lo, out); break;
-    default: layernorm_split_kernel<8><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, hi, lo, out); break;
+    case 1: B200_LNS(1); break;
+    case 2: B200_LNS(2); break;
+    case 4: B200_LNS(4); break;
+    default: B200_LNS(8); break;
   }
+#undef B200_LNS
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;
@@ -578,7 +614,11 @@ int launch_layernorm_bwd(const float* x, const RowMap& x_rows, const float* dy, 
 // C[M,N] (+)= A[M,K] * B[N,K]^T (+ biases), operands already split into hi/lo matrices (K- or MN-major).
 int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
                      const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
-                     size_t splitk_ws_bytes, cudaStream_t stream) {
+                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready, int stream_clusters) {
+  if (ready && (splitk_ws || stream_clusters < 1)) {
+    set_error("tc_gemm: a streamed launch publishes whole tiles and takes no split-K workspace");
+    return B200RNN_ERR_INVALID;
+  }
   if (M < 1 || N % BN != 0 || K < 1) {
     set_error("tc_gemm: unsupported shape M=%d N=%d K=%d", M, N, K);
     return B200RNN_ERR_UNSUPPORTED;
@@ -635,12 +675,38 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
   a.kb_per_split = (nkb + splitk - 1) / splitk;
   a.splitk = (nkb + a.kb_per_split - 1) / a.kb_per_split;
   a.partial = static_cast<float*>(splitk_ws);
+  a.ready = ready;
   const int nitems = ntiles * a.splitk;
   dim3 grid(nitems < sms ? nitems : sms, 1, 1);
-  {
+  if (!ready) {
     ProfScope prof(PROF_GEMM, stream);
     gemm_tf32x3_kernel<<<grid, TC_THREADS, TC_SMEM, stream>>>(m_ahi, m_alo, m_bhi, m_blo, a);
     B200_CUDA_CHECK(cudaGetLastError());
+    count_launch();
+  } else {
+    // Streamed: 4-CTA clusters (no cluster feature is used). A GPC holds floor(SMs / 4) of them whatever else runs
+    // in it, so the GEMM takes exactly `stream_clusters` of the 4-CTA cluster slots and leaves the others to the
+    // recurrence's 4-CTA clusters (api.cu); single CTAs spread over the GPCs would fragment them.
+    const int want = (nitems + 3) / 4;
+    grid.x = 4 * (want < stream_clusters ? want : stream_clusters);
+    static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
+    if (debug)
+      fprintf(stderr, "[b200rnn] streamed x-projection: gemm grid %u (4-CTA clusters) of %d SMs, %d row tiles x %d column tiles\n",
+              grid.x, sms, a.tiles_m, a.tiles_n);
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 4;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = dim3(TC_THREADS, 1, 1);
+    cfg.dynamicSmemBytes = TC_SMEM;
+    cfg.stream = stream;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    ProfScope prof(PROF_GEMM, stream);
+    B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tf32x3_kernel, m_ahi, m_alo, m_bhi, m_blo, a));
     count_launch();
   }
   if (a.splitk > 1)
@@ -673,7 +739,8 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
     b_lo = w_lo;
   }
   TcOperand A{a_hi, a_lo, p.a_kcontig ? p.K : p.M, !p.a_kcontig}, B{b_hi, b_lo, p.b_kcontig ? p.K : p.N, !p.b_kcontig};
-  return tc_gemm_presplit(A, B, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, 0, nullptr, 0, stream);
+  return tc_gemm_presplit(A, B, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, 0, nullptr, 0, stream,
+                          p.tc_ready, p.tc_stream_clusters);
 }
 
 }  // namespace b200rnn

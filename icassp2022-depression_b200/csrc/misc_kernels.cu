@@ -48,7 +48,10 @@ __global__ void dropout_kernel(const float* __restrict__ in, float* __restrict__
 
 __global__ void dropout_split_kernel(const float* __restrict__ in, float* __restrict__ out, float* __restrict__ hi,
                                      float* __restrict__ lo, size_t n, float p, float scale,
-                                     const uint64_t* __restrict__ hdr, uint32_t stream_id) {
+                                     const uint64_t* __restrict__ hdr, uint32_t stream_id, int* __restrict__ clear,
+                                     int nclear) {
+  if (blockIdx.x == 0)
+    for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
   const uint64_t seed = hdr[0], offset = hdr[1];
   const size_t nquad = n / 4;
   const uint32_t thr = (uint32_t)fminf(p * 4294967296.0f, 4294967295.0f);
@@ -127,7 +130,7 @@ int launch_dropout(const float* in, float* out, size_t n, float p, const uint64_
 }
 
 int launch_dropout_split(const float* in, float* out, float* hi, float* lo, size_t n, float p, const uint64_t* hdr,
-                         uint32_t stream_id, cudaStream_t stream) {
+                         uint32_t stream_id, cudaStream_t stream, int* clear, int nclear) {
   if (n == 0) return B200RNN_OK;
   if (n % 4 != 0) {
     set_error("dropout_split: element count must be a multiple of 4");
@@ -137,7 +140,8 @@ int launch_dropout_split(const float* in, float* out, float* hi, float* lo, size
   size_t nquad = n / 4;
   int blocks = (int)((nquad + 255) / 256);
   if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-  dropout_split_kernel<<<blocks, 256, 0, stream>>>(in, out, hi, lo, n, p, scale, hdr, stream_id);
+  dropout_split_kernel<<<blocks, 256, 0, stream>>>(in, out, hi, lo, n, p, scale, hdr, stream_id, clear,
+                                                   clear ? nclear : 0);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;

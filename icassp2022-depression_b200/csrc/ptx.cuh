@@ -114,6 +114,13 @@ __device__ __forceinline__ void st_async_v4(uint32_t cluster_addr, float4 v, uin
       : "memory");
 }
 
+// ---- global-memory flags --------------------------------------------------------------------------
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
 // ---- warp-level tensor-core MMA (SASS: HMMA.1688.F32.TF32) ----------------------------------------
 // x = hi + lo with hi = x truncated to TF32 (its 13 low mantissa bits cleared, in a 32-bit container) and lo = x - hi
 // (exact in fp32, |lo| < 2^-10 |x|). The MMA reads only the TF32 bits of lo, so hi*hi + lo*hi + hi*lo carries ~2^-20

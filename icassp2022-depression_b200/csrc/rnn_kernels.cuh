@@ -19,7 +19,24 @@ struct RecFwdParams {
   float* c_n;                // [D,B,H] of this layer (LSTM) or NULL
   long long* trace;          // debug: per-step phase timestamps of CTA 0 / warp 0 (NULL = off), [T][8]
   const int* lengths;        // optional [B]: valid steps per sequence (PackedSequence semantics); NULL = all T
+  // streamed x-projection (D = 1 only): the GEMM writing gates[0] may still run. The x-projection of step t is read
+  // only once ready[m] >= tiles_n for the row tiles m holding rows [t*B, (t+1)*B) (TC_TILE_M rows each). NULL = the
+  // gates are complete at launch.
+  const int* ready;
+  int tiles_n;
 };
+
+// A recurrence launch chosen for a shape, before anything is enqueued: `nclusters` clusters of C CTAs, of which
+// `capacity` can be co-resident (cudaOccupancyMaxActiveClusters).
+template <typename P>
+struct ClusterLaunch {
+  void (*kernel)(P, int);
+  int C, NT, nslices, nclusters, capacity;
+  size_t smem;
+  int ctas() const { return nclusters * C; }
+  bool one_wave() const { return nclusters <= capacity; }
+};
+using RecFwdLaunch = ClusterLaunch<RecFwdParams>;
 
 struct RecBwdParams {
   int mode, B, T, H, D;
@@ -45,7 +62,10 @@ struct RecBwdParams {
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)
 int rec_bwd_max_slices(int B);
 
-int launch_rec_fwd(const RecFwdParams& p, cudaStream_t stream);
+// forward: choose the config for p's shape (mode, H, B, D, lengths or not), then launch it; p.ready != NULL launches
+// it with programmatic stream serialization, so that it may start while the GEMM before it still runs
+int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* out);
+int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t stream);
 int launch_rec_bwd(RecBwdParams& p, cudaStream_t stream);
 
 }  // namespace b200rnn

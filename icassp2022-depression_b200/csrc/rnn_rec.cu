@@ -240,6 +240,28 @@ struct FwdCell {
   }
 };
 
+// Streamed x-projection (RecFwdParams::ready, api.cu): before a warp reads the x-projection of step t, it waits until
+// the GEMM has published every row tile that holds rows [t*B, (t+1)*B). The whole warp polls the counter with acquire
+// semantics (one broadcast load; a poll loop run by one lane alone made ptxas spill the FFMA configs' registers), and
+// the loads of `gates` that follow stay ordinary loads. `upto`, the last row tile this warp has seen complete, makes a
+// step whose tiles are already known complete cost one compare. Steps are visited in increasing t: only
+// unidirectional layers are streamed.
+// The wait always ends: the GEMM never waits on anything, and the programmatic launch starts this kernel only after
+// every GEMM CTA has started. It is bounded all the same (trap after 4M polls, seconds, like the peer exchange in
+// fuse_head.cu), so that a protocol bug is a CUDA error, not a hung GPU.
+struct GiReady {
+  int upto = -1;
+  __device__ __forceinline__ void wait(const RecFwdParams& p, int t) {
+    if (p.ready == nullptr) return;
+    const int last = ((t + 1) * p.B - 1) / TC_TILE_M;
+    if (last <= upto) return;
+    for (int m = max(upto + 1, t * p.B / TC_TILE_M); m <= last; ++m)
+      for (int n = 0; ptx::ld_acquire_gpu(p.ready + m) < p.tiles_n; ++n)
+        if (n > (1 << 22)) __trap();
+    upto = last;
+  }
+};
+
 // PB = true: batch-paired contraction and state layout (rnn_core.cuh, dots_chunk2b), see launch_rec_fwd
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false, bool PB = false>
 __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
@@ -289,7 +311,11 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 
   // ---- lane identity: after the butterfly this lane owns (unit, batch) ------------------------------
   FwdCell<MODE, H, VL> cell(p, dir, j0 + w * UPW + LM::unit(lane), b0 + LM::q(lane));
-  if (T > 0) cell.load_gi(p, dir ? T - 1 : 0);
+  GiReady gi_ready;
+  if (T > 0) {
+    gi_ready.wait(p, dir ? T - 1 : 0);
+    cell.load_gi(p, dir ? T - 1 : 0);
+  }
 
   for (int step = 0; step < T; ++step) {
     const int t = dir ? (T - 1 - step) : step;
@@ -378,7 +404,10 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       cell.flush(p, dir, t);
       cell.finish(p, dir);
     }
-    if (step + 1 < T) cell.load_gi(p, dir ? (T - 2 - step) : (step + 1));  // long latency, consumed at the next gate math
+    if (step + 1 < T) {  // long latency, consumed at the next gate math
+      gi_ready.wait(p, dir ? (T - 2 - step) : (step + 1));
+      cell.load_gi(p, dir ? (T - 2 - step) : (step + 1));
+    }
   }
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
 }
@@ -475,7 +504,9 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
   const int u0 = ug * 16 + kh * 8;  // first unit (within the CTA's slice) this warp finishes
   const int ju = j0 + u0 + fg;
   FwdCell<B200RNN_GRU, H, VL> cell[2] = {{p, dir, ju, b0 + 2 * ft}, {p, dir, ju, b0 + 2 * ft + 1}};
+  GiReady gi_ready;
   if (T > 0) {
+    gi_ready.wait(p, dir ? T - 1 : 0);
 #pragma unroll
     for (int jb = 0; jb < 2; ++jb) cell[jb].load_gi(p, dir ? T - 1 : 0);
   }
@@ -586,6 +617,7 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
       for (int jb = 0; jb < 2; ++jb) cell[jb].finish(p, dir);
     }
     if (step + 1 < T) {
+      gi_ready.wait(p, dir ? (T - 2 - step) : (step + 1));
 #pragma unroll
       for (int jb = 0; jb < 2; ++jb) cell[jb].load_gi(p, dir ? (T - 2 - step) : (step + 1));
     }
@@ -838,19 +870,24 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 // =================================================================================================
 // launchers
 // =================================================================================================
-// Launch config of `nclusters` clusters of C CTAs; `attr` is the storage of the cluster dimension it points to.
-cudaLaunchConfig_t cluster_config(int nclusters, int C, int NT, size_t smem, cudaStream_t s, cudaLaunchAttribute* attr) {
-  attr->id = cudaLaunchAttributeClusterDimension;
-  attr->val.clusterDim.x = (unsigned)C;
-  attr->val.clusterDim.y = 1;
-  attr->val.clusterDim.z = 1;
+// Launch config of `nclusters` clusters of C CTAs; `attr` is the storage of the attributes it points to: the cluster
+// dimension and, when `programmatic`, programmatic stream serialization (the launch may start while the kernel before
+// it in the stream still runs, once every CTA of that kernel has executed griddepcontrol.launch_dependents).
+cudaLaunchConfig_t cluster_config(int nclusters, int C, int NT, size_t smem, cudaStream_t s,
+                                  cudaLaunchAttribute (&attr)[2], bool programmatic = false) {
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = (unsigned)C;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(nclusters * C), 1, 1);
   cfg.blockDim = dim3((unsigned)NT, 1, 1);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = programmatic ? 2 : 1;
   return cfg;
 }
 
@@ -864,8 +901,8 @@ int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capaci
   auto it = cache.find(key);
   if (it == cache.end()) {
     B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchAttribute attr;
-    const cudaLaunchConfig_t cfg = cluster_config(NUM_SMS, C, NT, smem, 0, &attr);
+    cudaLaunchAttribute attr[2];
+    const cudaLaunchConfig_t cfg = cluster_config(NUM_SMS, C, NT, smem, 0, attr);
     int n = 0;
     if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) {
       cudaGetLastError();
@@ -877,15 +914,13 @@ int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capaci
   return B200RNN_OK;
 }
 
-int no_prep(int) { return B200RNN_OK; }
-
-// Launches `kernel` as D * ceil(B / BS) clusters of C CTAs if the driver reports them all co-resident, or regardless
-// when `force` (then in several waves if they do not fit). Returns false, having launched nothing, when the config is
-// not taken. Otherwise prep(nslices) runs first, and *rc is its status or the launch's. B200RNN_DEBUG prints one line
-// per config considered: "[b200rnn] <desc>: need N clusters, capacity M, smem S".
-template <typename K, typename P, typename Prep, typename... Args>
-bool try_clustered(K kernel, P& p, int C, int BS, int NT, size_t smem, int prof_kind, bool force, cudaStream_t s,
-                   int* rc, Prep prep, const char* desc, Args... desc_args) {
+// Chooses `kernel` as D * ceil(B / BS) clusters of C CTAs if the driver reports them all co-resident, or regardless
+// when `force` (then in several waves if they do not fit). Returns false when the config is not taken; true when it is
+// (*L describes it, nothing is enqueued yet) or when the capacity query failed (*rc). B200RNN_DEBUG prints one line per
+// config considered: "[b200rnn] <desc>: need N clusters, capacity M, smem S".
+template <typename P, typename... Args>
+bool pick_clustered(void (*kernel)(P, int), const P& p, int C, int BS, int NT, size_t smem, bool force,
+                    ClusterLaunch<P>* L, int* rc, const char* desc, Args... desc_args) {
   const int nslices = (p.B + BS - 1) / BS;
   const int nclusters = nslices * p.D;
   int capacity = 0;
@@ -898,39 +933,42 @@ bool try_clustered(K kernel, P& p, int C, int BS, int NT, size_t smem, int prof_
     fprintf(stderr, "[b200rnn] %s: need %d clusters, capacity %d, smem %zu\n", what, nclusters, capacity, smem);
   }
   if (!force && nclusters > capacity) return false;
-  *rc = prep(nslices);
-  if (*rc != B200RNN_OK) return true;
-  ProfScope prof(prof_kind, s);
-  cudaLaunchAttribute attr;
-  const cudaLaunchConfig_t cfg = cluster_config(nclusters, C, NT, smem, s, &attr);
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p, nslices);
-  if (e != cudaSuccess) {
-    set_error("cudaLaunchKernelEx of a recurrence kernel failed: %s", cudaGetErrorString(e));
-    *rc = B200RNN_ERR_CUDA;
-    return true;
-  }
-  count_launch();
+  *L = ClusterLaunch<P>{kernel, C, NT, nslices, nclusters, capacity, smem};
   return true;
 }
 
+template <typename P>
+int launch_clustered(const ClusterLaunch<P>& L, const P& p, int prof_kind, bool programmatic, cudaStream_t s) {
+  ProfScope prof(prof_kind, s);
+  cudaLaunchAttribute attr[2];
+  const cudaLaunchConfig_t cfg = cluster_config(L.nclusters, L.C, L.NT, L.smem, s, attr, programmatic);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, L.kernel, p, L.nslices);
+  if (e != cudaSuccess) {
+    set_error("cudaLaunchKernelEx of a recurrence kernel failed: %s", cudaGetErrorString(e));
+    return B200RNN_ERR_CUDA;
+  }
+  count_launch();
+  return B200RNN_OK;
+}
+
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool PB = false>
-bool try_fwd(const RecFwdParams& p, cudaStream_t s, bool force, int* rc) {
+bool pick_fwd(const RecFwdParams& p, bool force, RecFwdLaunch* L, int* rc) {
   using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
   static_assert(Cfg::FWD_SMEM <= MAX_SMEM, "forward config does not fit an SM");
   auto k = p.lengths ? rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, true, PB>
                      : rec_fwd_kernel<MODE, H, C, BS, KL, UPL, RG, false, PB>;
-  return try_clustered(k, p, C, BS, Cfg::NT, Cfg::FWD_SMEM, PROF_REC_FWD, force, s, rc, no_prep,
-                       "fwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d PB=%d", C, BS, KL, UPL, RG, (int)PB);
+  return pick_clustered(k, p, C, BS, Cfg::NT, Cfg::FWD_SMEM, force, L, rc,
+                        "fwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d PB=%d", C, BS, KL, UPL, RG, (int)PB);
 }
 
-// the tensor-core config is the widest-cluster one: it always launches (several waves when its clusters do not all fit)
-int run_fwd_tc(const RecFwdParams& p, cudaStream_t s) {
+// the tensor-core config is the widest-cluster one: it is always taken (several waves when its clusters do not all fit)
+int pick_fwd_tc(const RecFwdParams& p, RecFwdLaunch* L) {
   using Cfg = TcFwdCfg;
   static_assert(Cfg::SMEM <= MAX_SMEM, "forward config does not fit an SM");
   auto k = p.lengths ? rec_fwd_tc_kernel<true> : rec_fwd_tc_kernel<false>;
   int rc = B200RNN_OK;
-  try_clustered(k, p, Cfg::C, Cfg::BS, Cfg::NT, Cfg::SMEM, PROF_REC_FWD, true, s, &rc, no_prep,
-                "fwd cfg tc8 C=%d BS=%d mma.sync 3xTF32", Cfg::C, Cfg::BS);
+  pick_clustered(k, p, Cfg::C, Cfg::BS, Cfg::NT, Cfg::SMEM, true, L, &rc, "fwd cfg tc8 C=%d BS=%d mma.sync 3xTF32",
+                 Cfg::C, Cfg::BS);
   return rc;
 }
 
@@ -939,21 +977,24 @@ bool try_bwd(RecBwdParams& p, cudaStream_t s, bool force, int* rc) {
   using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
   static_assert(Cfg::BWD_SMEM <= MAX_SMEM, "backward config does not fit an SM");
   auto k = p.lengths ? rec_bwd_kernel<MODE, H, C, BS, KL, UPL, RG, true> : rec_bwd_kernel<MODE, H, C, BS, KL, UPL, RG, false>;
+  ClusterLaunch<RecBwdParams> L;
+  if (!pick_clustered(k, p, C, BS, Cfg::NT, Cfg::BWD_SMEM, force, &L, rc,
+                      "bwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d", C, BS, KL, UPL, RG))
+    return false;
+  if (*rc != B200RNN_OK) return true;
   // transposed, per-CTA contiguous copy of W_hh for this cluster width
-  auto prep = [&](int nslices) -> int {
-    for (int d = 0; d < p.D; ++d) {
-      whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], Cfg::G, H, C);
-      if (cudaGetLastError() != cudaSuccess) {
-        set_error("whh_prep launch failed");
-        return B200RNN_ERR_CUDA;
-      }
-      count_launch();
+  for (int d = 0; d < p.D; ++d) {
+    whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], Cfg::G, H, C);
+    if (cudaGetLastError() != cudaSuccess) {
+      set_error("whh_prep launch failed");
+      *rc = B200RNN_ERR_CUDA;
+      return true;
     }
-    p.nslices_out = nslices;
-    return B200RNN_OK;
-  };
-  return try_clustered(k, p, C, BS, Cfg::NT, Cfg::BWD_SMEM, PROF_REC_BWD, force, s, rc, prep,
-                       "bwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d", C, BS, KL, UPL, RG);
+    count_launch();
+  }
+  p.nslices_out = L.nslices;
+  *rc = launch_clustered(L, p, PROF_REC_BWD, false, s);
+  return true;
 }
 
 }  // namespace
@@ -964,8 +1005,9 @@ int rec_bwd_max_slices(int B) { return (B + 1) / 2; }
 // Candidates are ordered by batch rows per cluster; the first one whose clusters are all co-resident
 // (one wave => every sequence advances in lock step) wins, else the widest one runs in several waves.
 // Template arguments: <MODE, H, C, BS, KL, UPL, RG>.
-int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
+int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
   int rc = B200RNN_OK;
+  L->kernel = nullptr;
   if (p.B <= 0 || p.T <= 0) return rc;
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
@@ -976,33 +1018,42 @@ int launch_rec_fwd(const RecFwdParams& p, cudaStream_t s) {
     //       8 warps per CTA
     //   tc8 8 batch rows, the contraction on the tensor cores (rec_fwd_tc_kernel, mma.sync 3xTF32), 8 warps per CTA
     // A cluster cannot span GPCs, and H100 SXM GPCs are floor-swept unevenly, so the number of co-resident 4-CTA clusters
-    // (30 on a 132-SM card measured) comes from the driver (try_clustered), never from the SM count. Measured per layer
+    // (30 on a 132-SM card measured) comes from the driver (pick_clustered), never from the SM count. Measured per layer
     // launch at T = 120 (DESIGN.md): a config in one wave beats the next wider one, and tc8 in one wave beats bs4 in two.
-    if (try_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
-    if (try_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, s, false, &rc)) return rc;
+    if (pick_fwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, false, L, &rc)) return rc;
+    if (pick_fwd<B200RNN_GRU, 256, 4, 4, 16, 4, 1, true>(p, false, L, &rc)) return rc;
     // the widest clusters: one wave up to B = 8 x the 4-CTA cluster capacity, several waves beyond
-    return run_fwd_tc(p, s);
+    return pick_fwd_tc(p, L);
   }
   if (p.mode == B200RNN_GRU && p.H == 128) {
-    if (try_fwd<B200RNN_GRU, 128, 2, 4, 16, 4, 1>(p, s, false, &rc)) return rc;
-    try_fwd<B200RNN_GRU, 128, 4, 8, 32, 4, 1>(p, s, true, &rc);
+    if (pick_fwd<B200RNN_GRU, 128, 2, 4, 16, 4, 1>(p, false, L, &rc)) return rc;
+    pick_fwd<B200RNN_GRU, 128, 4, 8, 32, 4, 1>(p, true, L, &rc);
     return rc;
   }
   if (p.mode == B200RNN_LSTM && p.H == 256) {
     // scalar FFMA: the batch-paired form needs more registers than sm_90 leaves this config (it spills)
-    if (try_fwd<B200RNN_LSTM, 256, 4, 4, 16, 4, 1>(p, s, false, &rc)) return rc;
-    try_fwd<B200RNN_LSTM, 256, 8, 8, 16, 2, 1>(p, s, true, &rc);
+    if (pick_fwd<B200RNN_LSTM, 256, 4, 4, 16, 4, 1>(p, false, L, &rc)) return rc;
+    pick_fwd<B200RNN_LSTM, 256, 8, 8, 16, 2, 1>(p, true, L, &rc);
     return rc;
   }
   if (p.mode == B200RNN_LSTM && p.H == 128) {
     // scalar FFMA
-    if (try_fwd<B200RNN_LSTM, 128, 2, 4, 16, 4, 1>(p, s, false, &rc)) return rc;
-    try_fwd<B200RNN_LSTM, 128, 4, 8, 16, 2, 1>(p, s, true, &rc);
+    if (pick_fwd<B200RNN_LSTM, 128, 2, 4, 16, 4, 1>(p, false, L, &rc)) return rc;
+    pick_fwd<B200RNN_LSTM, 128, 4, 8, 16, 2, 1>(p, true, L, &rc);
     return rc;
   }
   set_error("recurrence: unsupported (mode=%d, hidden_size=%d); built for hidden_size 128 and 256", p.mode,
             p.H);
   return B200RNN_ERR_UNSUPPORTED;
+}
+
+int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s) {
+  if (p.B <= 0 || p.T <= 0) return B200RNN_OK;
+  if (p.ready && p.D != 1) {  // GiReady walks the row tiles in increasing t
+    set_error("recurrence: a streamed x-projection needs a unidirectional layer");
+    return B200RNN_ERR_INVALID;
+  }
+  return launch_clustered(L, p, PROF_REC_FWD, p.ready != nullptr, s);
 }
 
 int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
