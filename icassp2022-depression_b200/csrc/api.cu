@@ -328,11 +328,12 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     int dev = 0;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   }
-  // ready counters of a streamed input projection; every kernel that writes the GEMM's A operand zeroes them, so each
-  // layer (and each CUDA-graph replay) starts from zero without a launch of its own
+  // ready counters of a streamed input projection; a kernel that writes the GEMM's A operand (LayerNorm, dense copy,
+  // dropout) zeroes them, so each layer (and each CUDA-graph replay) starts from zero; an A operand read straight from
+  // the caller's tensor or the previous layer's output takes a memset
   int* ready = reinterpret_cast<int*>(S + sl.f_ready);
   const int tiles_m = (int)((d.TB + TC_TILE_M - 1) / TC_TILE_M);
-  bool a_ready = false;  // the next layer's A operand (hi/lo) was already produced by this layer's dropout pass
+  bool ready_zeroed = false;  // this layer's dropout pass zeroed the counters for the next layer
   for (int l = 0; l < d.L; ++l) {
     const int Il = l == 0 ? d.I : (int)d.DH;
     // ---- layer input ---------------------------------------------------------------------------
@@ -366,22 +367,31 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     const int gemm_clusters = rec.capacity - rec.nclusters;
     const bool stream_xproj = d.D == 1 && tc_layer && rec.C == 4 && rec.one_wave() && 2 * rec.ctas() <= sms &&
                               gemm_clusters > 0;
-    // ---- A operand of the tensor-core input projection, prepared once per layer (shared by the directions)
+    // ---- A operand of the tensor-core input projection (fp32, split on chip by the GEMM), shared by the directions:
+    // the layer input itself when the GEMM can read it in place, else a dense copy in the GEMM's workspace
     void* tc_ws = S + sl.f_tc;
+    const float* a_in = in;
+    RowMap a_rows = in_rows;
     if (tc_layer) {
-      float* a_hi = tc_a_hi(tc_ws);
-      float* a_lo = tc_a_lo(tc_ws, (int)d.TB, Il);
-      if (l == 0 && ln_gamma)
-        rc = tc_layernorm_split(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, a_hi, a_lo, st,
-                                (save && fused_ln) ? R + rl.xln : nullptr, ready, tiles_m);
-      else if (!a_ready)
-        rc = tc_split(in, in_rows, (int)d.TB, Il, a_hi, a_lo, st, ready, tiles_m);
+      float* a_dense = tc_a_hi(tc_ws);
+      if (l == 0 && ln_gamma) {
+        float* out = (save && fused_ln) ? R + rl.xln : a_dense;
+        rc = tc_layernorm(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, out, st, ready, tiles_m);
+        a_in = out;
+        a_rows = simple_rows(Il);
+      } else if (!tc_a_f32_in_place(in, in_rows, (int)d.TB, Il)) {
+        rc = tc_gather_rows(in, in_rows, (int)d.TB, Il, a_dense, st, ready, tiles_m);
+        a_in = a_dense;
+        a_rows = simple_rows(Il);
+      } else if (stream_xproj && !ready_zeroed) {
+        B200_CUDA_CHECK(cudaMemsetAsync(ready, 0, tiles_m * sizeof(int), st));
+      }
       if (rc) return rc;
     } else if (l == 0 && ln_gamma) {
       set_error("forward: the fused LayerNorm prologue needs the tensor-core input projection (input_size %% 32 == 0)");
       return B200RNN_ERR_UNSUPPORTED;
     }
-    a_ready = false;
+    ready_zeroed = false;
     for (int k = 0; k < d.D; ++k) {
       const float* const* pp = params + (size_t)(l * d.D + k) * 4;
       const float *w_ih = pp[0], *w_hh = pp[1], *b_ih = pp[2], *b_hh = pp[3];
@@ -397,7 +407,7 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
       // K1: x-projection of every time step at once, biases folded (GRU: b_hh only for r,z)
       GemmParams g;
       memset(&g, 0, sizeof(g));
-      g.A = in; g.a_rows = in_rows; g.a_kcontig = 1;
+      g.A = a_in; g.a_rows = a_rows; g.a_kcontig = 1;
       g.B = w_ih; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
       g.C = gates; g.c_rows = simple_rows((long long)d.GH);
       g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
@@ -406,7 +416,7 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
       if (tc_layer) {
         g.tc_ws = tc_ws;
         g.tc_ws_bytes = sl.f_tc_bytes;
-        g.tc_a_presplit = 1;
+        g.tc_a_f32 = 1;
         if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders)
           g.tc_b_hi = WC + wl.hi[l][k];
           g.tc_b_lo = WC + wl.lo[l][k];
@@ -443,13 +453,9 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     if (rc) return rc;
     if (drop && l + 1 < d.L) {  // K7; keeps the raw output when it is needed by backward, else in place
       float* dropped = save ? R + rl.ydrop[l] : ylay;
-      if (tc) {  // also emit the hi/lo split the next layer's tensor-core GEMM consumes (one pass instead of two)
-        rc = launch_dropout_split(ylay, dropped, tc_a_hi(tc_ws), tc_a_lo(tc_ws, (int)d.TB, (int)d.DH), d.TB * d.DH, d.p, hdr,
-                                  (uint32_t)l, st, ready, tiles_m);
-        a_ready = true;
-      } else {
-        rc = launch_dropout(ylay, dropped, d.TB * d.DH, d.p, hdr, (uint32_t)l, st);
-      }
+      // the next layer's GEMM reads `dropped` in place; the same launch zeroes its ready counters
+      rc = launch_dropout(ylay, dropped, d.TB * d.DH, d.p, hdr, (uint32_t)l, st, ready, tiles_m);
+      ready_zeroed = true;
       if (rc) return rc;
     }
   }
@@ -800,6 +806,30 @@ B200RNN_API int b200rnn_gemm_f32(int M, int N, int K, const float* A, int64_t ld
   g.tc_ws = scratch;  // used by the tensor-core 3xTF32 path when the problem is eligible and the buffer is large enough
   g.tc_ws_bytes = scratch_bytes;
   return launch_gemm(g, scratch, scratch_bytes, static_cast<cudaStream_t>(stream_));
+}
+
+/* test only (not declared in the public header): the input projection's fp32-A tensor-core GEMM as the forward runs
+   it, C[M][N] = A W^T + bias. Row m = t * a_batch + b of A sits at A + t * a_st + b * a_sb (a_batch = 0: dense rows,
+   a_st floats apart) and is read in place; W [N][K] is split into `scratch` per call. ready != NULL: streamed launch
+   on stream_clusters 4-CTA clusters, the M / 128 counters must be zero on entry. */
+B200RNN_API int b200rnn_debug_gemm_f32a(int M, int N, int K, const float* A, int64_t a_st, int64_t a_sb, int a_batch,
+                                        const float* W, float* C, const float* bias, int* ready, int stream_clusters,
+                                        void* scratch, size_t scratch_bytes, void* stream_) {
+  GemmParams g;
+  memset(&g, 0, sizeof(g));
+  g.A = A; g.a_rows = a_batch > 0 ? tb_rows(a_st, a_sb, a_batch) : simple_rows(a_st); g.a_kcontig = 1;
+  g.B = W; g.b_rows = simple_rows(K); g.b_kcontig = 1;
+  g.C = C; g.c_rows = simple_rows(N);
+  g.M = M; g.N = N; g.K = K;
+  g.bias1 = bias;
+  g.tc_a_f32 = 1;
+  g.tc_ready = ready;
+  g.tc_stream_clusters = stream_clusters;
+  if (!gemm_tc_eligible(g, scratch_bytes) || !tc_a_f32_in_place(A, g.a_rows, M, K)) {
+    set_error("debug_gemm_f32a: problem not eligible for the fp32-A tensor-core path");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  return launch_gemm_tc(g, scratch, scratch_bytes, static_cast<cudaStream_t>(stream_));
 }
 
 }  // extern "C"

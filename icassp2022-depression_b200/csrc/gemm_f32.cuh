@@ -22,7 +22,7 @@ struct GemmParams {
   // optional workspace for the tensor-core 3xTF32 path (gemm_tc.cu); NULL => fp32 FFMA path
   void* tc_ws;
   size_t tc_ws_bytes;
-  int tc_a_presplit;  // the A operand's hi/lo halves already sit at tc_ws (see tc_a_hi / tc_a_lo)
+  int tc_a_f32;  // A (k-contiguous) is read in fp32 through a_rows and split on chip; needs tc_a_f32_in_place
   // optional: the B operand (a weight matrix) already split into dense [N,K] hi / lo matrices by an earlier call
   // (b200rnn_prepare_weights: frozen encoders split their W_ih once, not once per step)
   const float* tc_b_hi;
@@ -35,15 +35,21 @@ struct GemmParams {
   int tc_stream_clusters;
 };
 
-// where launch_gemm_tc expects / puts the split A operand inside its workspace
+// where launch_gemm_tc puts the split A operand inside its workspace (tc_a_hi: also room for a dense fp32 [M][K] A)
 float* tc_a_hi(void* ws);
 float* tc_a_lo(void* ws, int M, int K);
-// LayerNorm over the last dimension fused with the TF32 split: hi/lo <- split(LN(src row) * gamma + beta)
-// `out` (optional): dense [R][Cc] copy of LN(src) kept for the backward pass (layer-0 wgrad operand)
-// `clear` (optional): nclear ints zeroed by the same launch (the ready counters of a streamed GEMM that reads hi / lo)
-int tc_layernorm_split(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta,
-                       float eps, float* hi, float* lo, cudaStream_t stream, float* out = nullptr,
-                       int* clear = nullptr, int nclear = 0);
+// whether the fp32-A GEMM can read A[M][K] in place through `rows` (dense, or a [T][B] view with B dividing 128 or a
+// multiple of it; 16-byte aligned base and strides)
+bool tc_a_f32_in_place(const float* A, const RowMap& rows, int M, int K);
+// dense fp32 copy dst[R][Cc] <- rows of src, for an A operand that cannot be read in place
+// `clear` (optional): nclear ints zeroed by the same launch (the ready counters of a streamed GEMM that reads dst)
+int tc_gather_rows(const float* src, const RowMap& rows, int R, int Cc, float* dst, cudaStream_t stream,
+                   int* clear = nullptr, int nclear = 0);
+// LayerNorm over the last dimension: out[R][Cc] <- LN(src row) * gamma + beta (dense fp32: the A operand of the
+// input projection, and when kept, the layer-0 wgrad operand of the backward pass)
+// `clear` (optional): nclear ints zeroed by the same launch (the ready counters of a streamed GEMM that reads out)
+int tc_layernorm(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta, float eps,
+                 float* out, cudaStream_t stream, int* clear = nullptr, int nclear = 0);
 // backward of that prologue: dx (strided like x) from dy = d/dLN(x) (dense), dgamma / dbeta (+)=; part = scratch of
 // layernorm_bwd_scratch_floats(Cc) floats
 size_t layernorm_bwd_scratch_floats(int Cc);
@@ -65,12 +71,16 @@ struct TcOperand {
                     // for operands whose contraction index is their row index: dG, X, h_prev in the wgrad GEMMs)
 };
 bool tc_available();
-int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream,
-             int* clear = nullptr, int nclear = 0);
+int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream);
 // ready: streamed launch of stream_clusters 4-CTA clusters (GemmParams::tc_ready); needs splitk_ws == NULL
 int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
                      const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
                      size_t splitk_ws_bytes, cudaStream_t stream, int* ready = nullptr, int stream_clusters = 0);
+// C = A[M,K] * B[N,K]^T + biases, A fp32 read in place through a_rows (tc_a_f32_in_place) and split in registers,
+// B K-major presplit; bit-identical to tc_gemm_presplit on the split of A. ready / stream_clusters as above.
+int tc_gemm_f32a(const float* A, const RowMap& a_rows, const TcOperand& B, int M, int N, int K, float* C,
+                 const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
+                 int* ready = nullptr, int stream_clusters = 0);
 // C(m,n) (+)= sum_z partial[z][m][n] (+ biases), fixed order (deterministic)
 int launch_splitk_reduce(const float* partial, int splitk, int M, int N, float* C, const RowMap& c_rows,
                          const float* bias1, const float* bias2, int bias2_n, int accumulate, cudaStream_t stream);

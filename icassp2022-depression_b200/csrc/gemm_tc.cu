@@ -17,11 +17,22 @@
 //                   source's row index: dG, X, h_prev in the wgrads) are read with coalesced loads and written
 //                   transposed into the same swizzled K-major layout, since wgmma takes tf32 operands K-major only.
 //                   A 3-stage shared-memory ring (A_hi, A_lo, W_hi, W_lo per stage), mbarrier full/empty.
-//   warpgroups 1-2: consumers — 64 rows of the tile each: wgmma.m64n128k8.tf32 from shared-memory descriptors,
-//                   12 per stage, then the round-to-nearest flush and finally the epilogue (+ folded biases).
+//                   fp32 A mode (the forward input projection): A arrives unsplit, 16 KB of fp32 per stage (the A_lo
+//                   slot stays unused), by a 3-D TMA that reads the layer input in place (batch-first / permuted views
+//                   included); one thread issues it with the W tiles.
+//   warpgroups 1-2: consumers — 64 rows of the tile each: wgmma.m64n128k8.tf32, 12 per stage, then the
+//                   round-to-nearest flush and finally the epilogue (+ folded biases, loaded before the first store).
+//                   Presplit A: both operands from shared-memory descriptors. fp32 A: each thread loads its A fragment
+//                   (16 floats per k-block), splits it in registers with the rounding of split_tf32_kernel and issues
+//                   the MMAs with A from registers; the next k-block's fragment is loaded while the current MMAs run.
+//                   The MMAs see exactly the operands of the presplit path, so C is bit-identical, while A is read
+//                   from HBM / L2 in fp32 (half the bytes), never written back split, and read from shared memory
+//                   once instead of three times per k-step. setmaxnreg moves registers from the producer (40) to the
+//                   consumers (232) for the two fragment buffers.
 #include <cuda.h>  // CUtensorMap types only; the encoder is fetched through cudaGetDriverEntryPoint
 #include <mutex>
 #include <stdlib.h>
+#include <string.h>
 
 #include "gemm_f32.cuh"
 #include "profile.cuh"
@@ -44,6 +55,15 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
           ptx::smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+// box of a 3-D map: coordinates (k, inner row, outer row)
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2,
+                                            uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+          ptx::smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
@@ -82,6 +102,23 @@ __device__ __forceinline__ void wgmma_tf32_m64n128k8(float (&d)[64], uint64_t ad
         B200_ACC8(56)
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// the same with A from registers: a[0..3] = A(g, t), A(g + 8, t), A(g, t + 4), A(g + 8, t + 4) of the warp's 16 rows,
+// g = lane / 4, t = lane % 4 (tf32 bit patterns)
+__device__ __forceinline__ void wgmma_tf32_m64n128k8_ra(float (&d)[64], const uint32_t* a, uint64_t bdesc,
+                                                        int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : B200_ACC8(0), B200_ACC8(8), B200_ACC8(16), B200_ACC8(24), B200_ACC8(32), B200_ACC8(40), B200_ACC8(48),
+        B200_ACC8(56)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
 #undef B200_ACC8
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -108,7 +145,11 @@ struct TcArgs {
   int kb_per_split; // k-blocks per split
   float* partial;
   int* ready;       // streamed (splitk == 1): tiles walked time-major, ready[m] += 1 per finished tile of row tile m
+  int a_f32;        // A is fp32 (map_a_hi, 3-D), split in registers by the consumers; W K-major presplit
+  int a_inner;      // fp32 A: rows per outer index of the 3-D map (tile m0 sits at (m0 % a_inner, m0 / a_inner))
 };
+
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64K registers of the SM
 
 // work item -> output tile origin: m fastest (consecutive tiles of a CTA mostly share their W tile rows in L2), or
 // time-major when streamed (the consumer reads row tile m after m - 1)
@@ -144,6 +185,11 @@ __device__ __forceinline__ void load_mn_tile(unsigned char* tile, const float* _
 // after a tile's stores the consumer warpgroups publish it with one release increment of ready[m]. Every read of the
 // A operand of a tile precedes that increment (the consumers have drained the ring stages of the tile), and the kernel
 // itself never waits on anything outside its CTA.
+// MN: some operand is MN-major (backward wgrad / dgrad). Its producer keeps 32 loads per thread in flight and needs
+// the default register budget, so that instantiation has no setmaxnreg; in the K-major one (every operand by TMA, one
+// thread issues) the producer gives registers to the consumers, whose fp32-A path holds the running sum, the wgmma
+// accumulator and two A fragments (4 x 64 registers).
+template <bool MN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                        const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
@@ -164,13 +210,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      ptx::mbar_init(&full[s], 128);  // every producer thread, after its own stores
-      ptx::mbar_init(&empty[s], 8);   // one arrival per consumer warp
+      ptx::mbar_init(&full[s], args.a_f32 ? 1 : 128);  // the TMA issuer (fp32 A) / every producer thread
+      ptx::mbar_init(&empty[s], 8);                     // one arrival per consumer warp
     }
     ptx::fence_mbar_init();
     if (!args.a_mn) {
       prefetch_tmap(&map_a_hi);
-      prefetch_tmap(&map_a_lo);
+      if (!args.a_f32) prefetch_tmap(&map_a_lo);
     }
     if (!args.b_mn) {
       prefetch_tmap(&map_b_hi);
@@ -180,85 +226,194 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   __syncthreads();
 
   if (warp < 4) {
+    if constexpr (!MN) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
     const int t = threadIdx.x;
-    const uint32_t tx = (args.a_mn ? 0u : 2u * TILE_BYTES) + (args.b_mn ? 0u : 2u * TILE_BYTES);
-    int it = 0;  // running k-block counter across items (ring position)
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int tile = item % ntiles, ks = item / ntiles;
-      int m0, n0;
-      tile_origin(args, tile, m0, n0);
-      const int kb0 = ks * args.kb_per_split;
-      const int kb1 = min(nkb_total, kb0 + args.kb_per_split);
-      for (int kb = kb0; kb < kb1; ++kb, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        ptx::mbar_wait(&empty[s], ph ^ 1);
-        unsigned char* st = base + s * STAGE_BYTES;
-        if (warp == 0 && tx) {
-          if (ptx::elect_one_sync()) {
-            mbar_expect_tx(&full[s], tx);
-            if (!args.a_mn) {
-              tma_load_2d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0, &full[s]);
-              tma_load_2d(st + 1 * TILE_BYTES, &map_a_lo, kb * BK, m0, &full[s]);
-            }
-            if (!args.b_mn) {
+    if (!MN && args.a_f32) {  // one thread issues the fp32 A tile and the W tiles; the consumers split A
+      if (warp == 0) {
+        int it = 0;  // running k-block counter across items (ring position)
+        for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+          int m0, n0;
+          tile_origin(args, item % ntiles, m0, n0);
+          for (int kb = 0; kb < nkb_total; ++kb, ++it) {
+            const int s = it % STAGES;
+            ptx::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+            unsigned char* st = base + s * STAGE_BYTES;
+            if (ptx::elect_one_sync()) {  // the A_lo slot stays unused: the consumers split A in registers
+              ptx::mbar_arrive_expect_tx(&full[s], 3u * TILE_BYTES);
+              tma_load_3d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0 % args.a_inner, m0 / args.a_inner, &full[s]);
               tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * BK, n0, &full[s]);
               tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
             }
+            __syncwarp();
           }
-          __syncwarp();
         }
-        if (args.a_mn) {
-          load_mn_tile(st + 0 * TILE_BYTES, args.a_hi, args.lda, args.M, args.K, m0, kb * BK, t);
-          load_mn_tile(st + 1 * TILE_BYTES, args.a_lo, args.lda, args.M, args.K, m0, kb * BK, t);
+      }
+    } else {
+      const bool a_mn = MN && args.a_mn, b_mn = MN && args.b_mn;
+      const uint32_t tx = (a_mn ? 0u : 2u * TILE_BYTES) + (b_mn ? 0u : 2u * TILE_BYTES);
+      int it = 0;  // running k-block counter across items (ring position)
+      for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
+        const int tile = item % ntiles, ks = item / ntiles;
+        int m0, n0;
+        tile_origin(args, tile, m0, n0);
+        const int kb0 = ks * args.kb_per_split;
+        const int kb1 = min(nkb_total, kb0 + args.kb_per_split);
+        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+          const int s = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          ptx::mbar_wait(&empty[s], ph ^ 1);
+          unsigned char* st = base + s * STAGE_BYTES;
+          if (warp == 0 && tx) {
+            if (ptx::elect_one_sync()) {
+              mbar_expect_tx(&full[s], tx);
+              if (!a_mn) {
+                tma_load_2d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0, &full[s]);
+                tma_load_2d(st + 1 * TILE_BYTES, &map_a_lo, kb * BK, m0, &full[s]);
+              }
+              if (!b_mn) {
+                tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * BK, n0, &full[s]);
+                tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
+              }
+            }
+            __syncwarp();
+          }
+          if (a_mn) {
+            load_mn_tile(st + 0 * TILE_BYTES, args.a_hi, args.lda, args.M, args.K, m0, kb * BK, t);
+            load_mn_tile(st + 1 * TILE_BYTES, args.a_lo, args.lda, args.M, args.K, m0, kb * BK, t);
+          }
+          if (b_mn) {
+            load_mn_tile(st + 2 * TILE_BYTES, args.b_hi, args.ldb, args.N, args.K, n0, kb * BK, t);
+            load_mn_tile(st + 3 * TILE_BYTES, args.b_lo, args.ldb, args.N, args.K, n0, kb * BK, t);
+          }
+          if (a_mn || b_mn) ptx::fence_proxy_async();  // generic stores -> visible to wgmma (async proxy)
+          ptx::mbar_arrive(&full[s]);
         }
-        if (args.b_mn) {
-          load_mn_tile(st + 2 * TILE_BYTES, args.b_hi, args.ldb, args.N, args.K, n0, kb * BK, t);
-          load_mn_tile(st + 3 * TILE_BYTES, args.b_lo, args.ldb, args.N, args.K, n0, kb * BK, t);
-        }
-        if (args.a_mn || args.b_mn) ptx::fence_proxy_async();  // generic stores -> visible to wgmma (async proxy)
-        ptx::mbar_arrive(&full[s]);
       }
     }
   } else {
+    if constexpr (!MN) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
     const int wg = (threadIdx.x >> 7) - 1;   // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
     const int wq = warp & 3;                 // warp within the warpgroup: 16 accumulator rows each
+    // the 12 MMAs of the k-block in ring position `pos` into acc, which restarts from zero; committed as one group
+    auto issue = [&](float (&acc)[64], int pos) {
+      ptx::mbar_wait(&full[pos % STAGES], (pos / STAGES) & 1);
+      const uint32_t st = ptx::smem_u32(base + (pos % STAGES) * STAGE_BYTES);
+      const uint64_t a_hi = make_kmajor_sw128_desc(st + 0 * TILE_BYTES + wg * 8192);
+      const uint64_t a_lo = make_kmajor_sw128_desc(st + 1 * TILE_BYTES + wg * 8192);
+      const uint64_t b_hi = make_kmajor_sw128_desc(st + 2 * TILE_BYTES);
+      const uint64_t b_lo = make_kmajor_sw128_desc(st + 3 * TILE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 8; ++k) {
+        const uint64_t adv = (uint64_t)(k * (32 >> 4));  // K step of 8 tf32 = 32 bytes inside the swizzle atom
+        wgmma_tf32_m64n128k8(acc, a_lo + adv, b_hi + adv, k != 0);
+        wgmma_tf32_m64n128k8(acc, a_hi + adv, b_lo + adv, 1);
+        wgmma_tf32_m64n128k8(acc, a_hi + adv, b_hi + adv, 1);
+      }
+      wgmma_commit();
+    };
+    // k-block `pos` has completed: hand its stage back and add it into total (round-to-nearest, increasing kb)
+    auto drain = [&](float (&total)[64], float (&acc)[64], int pos) {
+      reg_fence(acc);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&empty[pos % STAGES]);  // this warp's share of the stage has been read
+#pragma unroll
+      for (int i = 0; i < 64; ++i) total[i] += acc[i];
+    };
+    // fp32 A: this thread's A fragment of the k-block in ring position `pos` (rows g and g + 8 of the warp's 16, k = t + 4j
+    // of the 32; conflict-free under the 128-byte swizzle since row & 7 == g), split as split_tf32_kernel does:
+    // fa[8 s + i] = hi of a_i at k-step s, fa[8 s + 4 + i] = lo
+    const int g = lane >> 2, tq = lane & 3;
+    const uint32_t a_row = (uint32_t)(wg * 64 + wq * 16 + g) * 128u + tq * 4u;
+    auto load_a = [&](uint32_t (&fa)[32], int pos) {
+      ptx::mbar_wait(&full[pos % STAGES], (pos / STAGES) & 1);
+      const unsigned char* at = base + (pos % STAGES) * STAGE_BYTES + a_row;
+#pragma unroll
+      for (int s4 = 0; s4 < BK / 8; ++s4) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float x = *reinterpret_cast<const float*>(at + (i & 1) * 1024 + ((((2 * s4 + (i >> 1)) ^ g)) << 4));
+          uint32_t h;
+          asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
+          fa[8 * s4 + i] = h;
+          fa[8 * s4 + 4 + i] = __float_as_uint(x - __uint_as_float(h));
+        }
+      }
+    };
+    // the 12 MMAs of a k-block with A from registers: same products, same order as `issue`
+    auto issue_ra = [&](float (&acc)[64], const uint32_t (&fa)[32], int pos) {
+      const uint32_t st = ptx::smem_u32(base + (pos % STAGES) * STAGE_BYTES);
+      const uint64_t b_hi = make_kmajor_sw128_desc(st + 2 * TILE_BYTES);
+      const uint64_t b_lo = make_kmajor_sw128_desc(st + 3 * TILE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 8; ++k) {
+        const uint64_t adv = (uint64_t)(k * (32 >> 4));
+        wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k + 4], b_hi + adv, k != 0);
+        wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k], b_lo + adv, 1);
+        wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k], b_hi + adv, 1);
+      }
+      wgmma_commit();
+    };
     int it = 0;
     for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       const int tile = item % ntiles, ks = item / ntiles;
       const int nkb = min(nkb_total, (ks + 1) * args.kb_per_split) - ks * args.kb_per_split;
       int m0, n0;
       tile_origin(args, tile, m0, n0);
-      float total[64], acc[64];
+      float total[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) total[i] = 0.f;
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        ptx::mbar_wait(&full[s], ph);
-        const uint32_t st = ptx::smem_u32(base + s * STAGE_BYTES);
-        const uint64_t a_hi = make_kmajor_sw128_desc(st + 0 * TILE_BYTES + wg * 8192);
-        const uint64_t a_lo = make_kmajor_sw128_desc(st + 1 * TILE_BYTES + wg * 8192);
-        const uint64_t b_hi = make_kmajor_sw128_desc(st + 2 * TILE_BYTES);
-        const uint64_t b_lo = make_kmajor_sw128_desc(st + 3 * TILE_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 8; ++k) {
-          const uint64_t adv = (uint64_t)(k * (32 >> 4));  // K step of 8 tf32 = 32 bytes inside the swizzle atom
-          wgmma_tf32_m64n128k8(acc, a_lo + adv, b_hi + adv, k != 0);
-          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_lo + adv, 1);
-          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_hi + adv, 1);
+      float acc[64];
+      if (!MN && args.a_f32) {
+        // A from registers: the k-block's fp32 fragment is loaded and split here; the next k-block's is loaded while
+        // the current MMAs run. Fragments alternate between fa0 and fa1; the loop body is unconditional and the tail
+        // peeled, so no branch merges registers a wgmma in flight reads.
+        uint32_t fa0[32], fa1[32];
+        load_a(fa0, it);
+        int kb = 0;
+        for (; kb + 2 < nkb; kb += 2) {
+          issue_ra(acc, fa0, it + kb);
+          load_a(fa1, it + kb + 1);
+          wgmma_wait0();
+          drain(total, acc, it + kb);
+          issue_ra(acc, fa1, it + kb + 1);
+          load_a(fa0, it + kb + 2);
+          wgmma_wait0();
+          drain(total, acc, it + kb + 1);
         }
-        wgmma_commit();
+        issue_ra(acc, fa0, it + kb);
+        if (kb + 1 < nkb) load_a(fa1, it + kb + 1);
         wgmma_wait0();
-        reg_fence(acc);
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&empty[s]);  // this warp's share of the stage has been read
-#pragma unroll
-        for (int i = 0; i < 64; ++i) total[i] += acc[i];
+        drain(total, acc, it + kb);
+        if (kb + 1 < nkb) {
+          issue_ra(acc, fa1, it + kb + 1);
+          wgmma_wait0();
+          drain(total, acc, it + kb + 1);
+        }
+      } else {
+        for (int kb = 0; kb < nkb; ++kb) {
+          issue(acc, it + kb);
+          wgmma_wait0();
+          drain(total, acc, it + kb);
+        }
       }
+      it += nkb;
       // accumulator fragment: element i sits at row 16 wq + lane/4 + 8 ((i/2) & 1), column 8 (i/4) + 2 (lane%4) + i%2
       const int r0 = m0 + wg * 64 + wq * 16 + (lane >> 2);
+      // the biases of this thread's 32 columns, loaded before the first store: loads placed after a store of C would
+      // each wait a full load latency (the compiler cannot move them across a store that might alias)
+      float b1v[32], b2v[32];
+#pragma unroll
+      for (int q = 0; q < 16; ++q) {
+        const int n = n0 + 8 * q + 2 * (lane & 3);
+        b1v[2 * q] = b1v[2 * q + 1] = b2v[2 * q] = b2v[2 * q + 1] = 0.f;
+        if (args.splitk == 1 && args.bias1) { b1v[2 * q] = __ldg(args.bias1 + n); b1v[2 * q + 1] = __ldg(args.bias1 + n + 1); }
+        if (args.splitk == 1 && args.bias2) {
+          if (n < args.bias2_n) b2v[2 * q] = __ldg(args.bias2 + n);
+          if (n + 1 < args.bias2_n) b2v[2 * q + 1] = __ldg(args.bias2 + n + 1);
+        }
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = r0 + 8 * h;
@@ -271,10 +426,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           float2 o = make_float2(total[4 * q + 2 * h], total[4 * q + 2 * h + 1]);
           if (args.splitk == 1) {
             const int n = n0 + col;
-            if (args.bias1) { o.x += __ldg(args.bias1 + n); o.y += __ldg(args.bias1 + n + 1); }
+            if (args.bias1) { o.x += b1v[2 * q]; o.y += b1v[2 * q + 1]; }
             if (args.bias2) {
-              if (n < args.bias2_n) o.x += __ldg(args.bias2 + n);
-              if (n + 1 < args.bias2_n) o.y += __ldg(args.bias2 + n + 1);
+              if (n < args.bias2_n) o.x += b2v[2 * q];
+              if (n + 1 < args.bias2_n) o.y += b2v[2 * q + 1];
             }
             if (args.accumulate) {
               const float2 old = *reinterpret_cast<const float2*>(crow + col);
@@ -297,9 +452,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 // x = hi + lo with hi = round-to-nearest TF32 (kept in a 32-bit container), lo = x - hi (exact in fp32).
 // Reads rows through a RowMap (batch_first / permuted inputs), writes two dense [M,K] matrices.
 __global__ void split_tf32_kernel(const float* __restrict__ src, RowMap rows, int M, int K, float* __restrict__ hi,
-                                  float* __restrict__ lo, int vec_ok, int* __restrict__ clear, int nclear) {
-  if (blockIdx.x == 0)
-    for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
+                                  float* __restrict__ lo, int vec_ok) {
   const size_t nvec = (size_t)M * (K / 4);
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nvec; i += (size_t)gridDim.x * blockDim.x) {
     const int m = (int)(i / (K / 4));
@@ -322,13 +475,29 @@ __global__ void split_tf32_kernel(const float* __restrict__ src, RowMap rows, in
   }
 }
 
-// LayerNorm(row) * gamma + beta, then the TF32 split — the prologue of audio_gru_whole.py:104 / fuse_net_whole.py:360
-// folded into the operand preparation of K1 (SURVEY.md 8f rank 1). One warp per row; Cc % 128 == 0, Cc <= 1024.
+// Dense fp32 copy of a layer input whose rows the fp32-A GEMM cannot read in place (a batch size that neither divides
+// 128 nor is a multiple of it, or misaligned strides); also zeroes `clear` (ready counters of a streamed GEMM).
+__global__ void gather_rows_kernel(const float* __restrict__ src, RowMap rows, int M, int K, float* __restrict__ dst,
+                                   int vec_ok, int* __restrict__ clear, int nclear) {
+  if (blockIdx.x == 0)
+    for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
+  const size_t nvec = (size_t)M * (K / 4);
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nvec; i += (size_t)gridDim.x * blockDim.x) {
+    const int m = (int)(i / (K / 4));
+    const int k = (int)(i - (size_t)m * (K / 4)) * 4;
+    const float* p = src + rows.off(m) + k;
+    const float4 x = vec_ok ? __ldg(reinterpret_cast<const float4*>(p)) : make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3));
+    *reinterpret_cast<float4*>(dst + (size_t)m * K + k) = x;
+  }
+}
+
+// LayerNorm(row) * gamma + beta — the prologue of audio_gru_whole.py:104 / fuse_net_whole.py:360, written dense in fp32
+// as the A operand of K1 (which splits it on chip) and, when saved, of the layer-0 wgrad. One warp per row;
+// Cc % 128 == 0, Cc <= 1024.
 template <int NV>  // float4 per lane
-__global__ void layernorm_split_kernel(const float* __restrict__ src, RowMap rows, int R, int Cc,
-                                       const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                                       float* __restrict__ hi, float* __restrict__ lo, float* __restrict__ out,
-                                       int* __restrict__ clear, int nclear) {
+__global__ void layernorm_kernel(const float* __restrict__ src, RowMap rows, int R, int Cc,
+                                 const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                                 float* __restrict__ out, int* __restrict__ clear, int nclear) {
   if (blockIdx.x == 0)
     for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
   const int lane = threadIdx.x & 31;
@@ -359,19 +528,9 @@ __global__ void layernorm_split_kernel(const float* __restrict__ src, RowMap row
       const int k = i * 128 + lane * 4;
       const float4 g = __ldg(reinterpret_cast<const float4*>(gamma + k));
       const float4 bt = __ldg(reinterpret_cast<const float4*>(beta + k));
-      float y[4] = {(x[i].x - mean) * rstd * g.x + bt.x, (x[i].y - mean) * rstd * g.y + bt.y,
-                    (x[i].z - mean) * rstd * g.z + bt.z, (x[i].w - mean) * rstd * g.w + bt.w};
-      float h[4], l[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        uint32_t t;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(y[e]));
-        h[e] = __uint_as_float(t);
-        l[e] = y[e] - h[e];
-      }
-      *reinterpret_cast<float4*>(hi + (size_t)r * Cc + k) = make_float4(h[0], h[1], h[2], h[3]);
-      *reinterpret_cast<float4*>(lo + (size_t)r * Cc + k) = make_float4(l[0], l[1], l[2], l[3]);
-      if (out) *reinterpret_cast<float4*>(out + (size_t)r * Cc + k) = make_float4(y[0], y[1], y[2], y[3]);  // for backward
+      const float4 y = make_float4((x[i].x - mean) * rstd * g.x + bt.x, (x[i].y - mean) * rstd * g.y + bt.y,
+                                   (x[i].z - mean) * rstd * g.z + bt.z, (x[i].w - mean) * rstd * g.w + bt.w);
+      *reinterpret_cast<float4*>(out + (size_t)r * Cc + k) = y;
     }
   }
 }
@@ -513,6 +672,30 @@ bool make_map(CUtensorMap* map, const float* ptr, int rows, int K, long long ld 
   return r == CUDA_SUCCESS;
 }
 
+// fp32 A operand read in place through its row map: 3-D map {K, inner rows, outer rows} with box {32, bi, 128 / bi},
+// so a 128-row tile is one box. Dense rows (inner_n >= M): {K, M, 1}. Rows r = t * B + b of a [T][B] view (tb_rows):
+// {K, B, T}, which tiles when B divides 128 or is a multiple of it. Strides must be multiples of 16 bytes.
+bool make_a_f32_map(CUtensorMap* map, const float* ptr, const RowMap& rows, int M, int K, int* inner) {
+  EncodeTiledFn enc = get_encoder();
+  if (!enc || (reinterpret_cast<uintptr_t>(ptr) & 15u) || K % 4 != 0) return false;
+  const bool dense = rows.inner_n >= M;
+  const long long ni = dense ? M : rows.inner_n;
+  const long long no = dense ? 1 : (M + ni - 1) / ni;
+  const long long si = rows.s_inner, so = dense ? (long long)M * rows.s_inner : rows.s_outer;
+  if (!dense && (M % ni != 0 || !(ni % BM == 0 || BM % ni == 0))) return false;
+  if (si < K || si % 4 != 0 || so < 1 || so % 4 != 0) return false;
+  const cuuint32_t bi = (cuuint32_t)(dense || ni >= BM ? BM : ni);
+  cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)ni, (cuuint64_t)no};
+  cuuint64_t strides[2] = {(cuuint64_t)si * sizeof(float), (cuuint64_t)so * sizeof(float)};
+  cuuint32_t box[3] = {(cuuint32_t)BK, bi, (cuuint32_t)BM / bi};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  *inner = (int)ni;
+  return r == CUDA_SUCCESS;
+}
+
 }  // namespace
 
 size_t gemm_tc_scratch_bytes(int M, int N, int K) { return (size_t)2 * ((size_t)M + N) * K * sizeof(float) + 1024; }
@@ -527,15 +710,38 @@ bool gemm_tc_eligible(const GemmParams& p, size_t ws_bytes) {
   return get_encoder() != nullptr;
 }
 
-int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream,
-             int* clear, int nclear) {
+int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream) {
   const bool vec = (reinterpret_cast<uintptr_t>(src) & 15u) == 0 && rows.s_outer % 4 == 0 && rows.s_inner % 4 == 0;
   size_t nv = (size_t)R * (Cc / 4);
   int blocks = (int)((nv + 255) / 256);
   if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
   if (blocks < 1) blocks = 1;
   ProfScope prof(PROF_MISC, stream);
-  split_tf32_kernel<<<blocks, 256, 0, stream>>>(src, rows, R, Cc, hi, lo, vec ? 1 : 0, clear, clear ? nclear : 0);
+  split_tf32_kernel<<<blocks, 256, 0, stream>>>(src, rows, R, Cc, hi, lo, vec ? 1 : 0);
+  B200_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return B200RNN_OK;
+}
+
+bool tc_a_f32_in_place(const float* A, const RowMap& rows, int M, int K) {
+  CUtensorMap m;
+  int inner = 0;
+  return make_a_f32_map(&m, A, rows, M, K, &inner);
+}
+
+int tc_gather_rows(const float* src, const RowMap& rows, int R, int Cc, float* dst, cudaStream_t stream, int* clear,
+                   int nclear) {
+  const bool vec = (reinterpret_cast<uintptr_t>(src) & 15u) == 0 && rows.s_outer % 4 == 0 && rows.s_inner % 4 == 0;
+  if (Cc % 4 != 0) {
+    set_error("gather_rows: the row width must be a multiple of 4");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  size_t nv = (size_t)R * (Cc / 4);
+  int blocks = (int)((nv + 255) / 256);
+  if (blocks > NUM_SMS * 16) blocks = NUM_SMS * 16;
+  if (blocks < 1) blocks = 1;
+  ProfScope prof(PROF_MISC, stream);
+  gather_rows_kernel<<<blocks, 256, 0, stream>>>(src, rows, R, Cc, dst, vec ? 1 : 0, clear, clear ? nclear : 0);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;
@@ -546,12 +752,12 @@ bool tc_available() { return get_encoder() != nullptr; }
 float* tc_a_hi(void* ws) { return reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255); }
 float* tc_a_lo(void* ws, int M, int K) { return tc_a_hi(ws) + (size_t)M * K; }
 
-int tc_layernorm_split(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta,
-                       float eps, float* hi, float* lo, cudaStream_t stream, float* out, int* clear, int nclear) {
+int tc_layernorm(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta, float eps,
+                 float* out, cudaStream_t stream, int* clear, int nclear) {
   const bool vec = (reinterpret_cast<uintptr_t>(src) & 15u) == 0 && rows.s_outer % 4 == 0 && rows.s_inner % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0 && (reinterpret_cast<uintptr_t>(beta) & 15u) == 0;
   if (!vec || !(Cc == 128 || Cc == 256 || Cc == 512 || Cc == 1024)) {
-    set_error("layernorm_split: needs 16-byte aligned rows and a feature width of 128, 256, 512 or 1024");
+    set_error("layernorm: needs 16-byte aligned rows and a feature width of 128, 256, 512 or 1024");
     return B200RNN_ERR_UNSUPPORTED;
   }
   int blocks = (R + 7) / 8;
@@ -559,7 +765,7 @@ int tc_layernorm_split(const float* src, const RowMap& rows, int R, int Cc, cons
   ProfScope prof(PROF_MISC, stream);
   if (!clear) nclear = 0;
 #define B200_LNS(NV_) \
-  layernorm_split_kernel<NV_><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, hi, lo, out, clear, nclear)
+  layernorm_kernel<NV_><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, out, clear, nclear)
   switch (Cc / 128) {  // instantiated widths: 128, 256, 512, 1024 (the reference normalises 256-d audio features)
     case 1: B200_LNS(1); break;
     case 2: B200_LNS(2); break;
@@ -611,11 +817,33 @@ int launch_layernorm_bwd(const float* x, const RowMap& x_rows, const float* dy, 
   return B200RNN_OK;
 }
 
-// C[M,N] (+)= A[M,K] * B[N,K]^T (+ biases), operands already split into hi/lo matrices (K- or MN-major).
-int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
-                     const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
-                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready, int stream_clusters) {
-  if (ready && (splitk_ws || stream_clusters < 1)) {
+namespace {
+
+int num_sms() {
+  int sms = NUM_SMS, dev = 0;
+  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
+}
+
+TcArgs tc_args(int M, int N, int K, float* C, const RowMap& c_rows, const float* bias1, const float* bias2,
+               int bias2_n, int accumulate, int* ready) {
+  TcArgs a;
+  memset(&a, 0, sizeof(a));
+  a.C = C; a.c_rows = c_rows;
+  a.M = M; a.N = N; a.K = K;
+  a.bias1 = bias1; a.bias2 = bias2; a.bias2_n = bias2_n;
+  a.accumulate = accumulate;
+  a.tiles_m = (M + BM - 1) / BM;
+  a.tiles_n = N / BN;
+  a.splitk = 1;
+  a.kb_per_split = (K + BK - 1) / BK;
+  a.ready = ready;
+  return a;
+}
+
+int check_tc_shape(int M, int N, int K, const float* C, const RowMap& c_rows, int* ready, bool splitk,
+                   int stream_clusters) {
+  if (ready && (splitk || stream_clusters < 1)) {
     set_error("tc_gemm: a streamed launch publishes whole tiles and takes no split-K workspace");
     return B200RNN_ERR_INVALID;
   }
@@ -627,42 +855,84 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
     set_error("tc_gemm: output must be 16-byte aligned with row strides that are multiples of 4 floats");
     return B200RNN_ERR_UNSUPPORTED;
   }
-  // MN-major operands are read by the kernel's own loads: their tensor maps stay zero and unused
-  CUtensorMap m_ahi{}, m_alo{}, m_bhi{}, m_blo{};
-  const bool ok_a = A.mn || (make_map(&m_ahi, A.hi, M, K, A.ld) && make_map(&m_alo, A.lo, M, K, A.ld));
-  const bool ok_b = B.mn || (make_map(&m_bhi, B.hi, N, K, B.ld) && make_map(&m_blo, B.lo, N, K, B.ld));
-  if (!ok_a || !ok_b) {
-    set_error("tc_gemm: cuTensorMapEncodeTiled failed (operands must be 16-byte aligned, ld %% 4 == 0)");
-    return B200RNN_ERR_CUDA;
-  }
+  return B200RNN_OK;
+}
+
+// one launch of gemm_tf32x3_kernel over a.tiles_m x a.tiles_n x a.splitk work items (args complete)
+int launch_tc(const CUtensorMap (&m)[4], const TcArgs& a, int stream_clusters, cudaStream_t stream) {
   static std::mutex mu;
   static bool attr_done[MAX_DEVICES] = {false};
   {
     const int dev = current_device();
     std::lock_guard<std::mutex> lk(mu);
     if (!attr_done[dev]) {
-      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       attr_done[dev] = true;
     }
   }
-  int sms = NUM_SMS;
-  {
-    int dev = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = num_sms();
+  const int nitems = a.tiles_m * a.tiles_n * a.splitk;
+  auto kernel = (a.a_mn || a.b_mn) ? gemm_tf32x3_kernel<true> : gemm_tf32x3_kernel<false>;
+  dim3 grid(nitems < sms ? nitems : sms, 1, 1);
+  if (!a.ready) {
+    ProfScope prof(PROF_GEMM, stream);
+    kernel<<<grid, TC_THREADS, TC_SMEM, stream>>>(m[0], m[1], m[2], m[3], a);
+    B200_CUDA_CHECK(cudaGetLastError());
+    count_launch();
+    return B200RNN_OK;
   }
-  TcArgs a;
-  a.C = C; a.c_rows = c_rows;
-  a.M = M; a.N = N; a.K = K;
-  a.bias1 = bias1; a.bias2 = bias2; a.bias2_n = bias2_n;
-  a.accumulate = accumulate;
+  // Streamed: 4-CTA clusters (no cluster feature is used). A GPC holds floor(SMs / 4) of them whatever else runs
+  // in it, so the GEMM takes exactly `stream_clusters` of the 4-CTA cluster slots and leaves the others to the
+  // recurrence's 4-CTA clusters (api.cu); single CTAs spread over the GPCs would fragment them.
+  const int want = (nitems + 3) / 4;
+  grid.x = 4 * (want < stream_clusters ? want : stream_clusters);
+  static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
+  if (debug)
+    fprintf(stderr, "[b200rnn] streamed x-projection: gemm grid %u (4-CTA clusters) of %d SMs, %d row tiles x %d column tiles\n",
+            grid.x, sms, a.tiles_m, a.tiles_n);
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 4;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(TC_THREADS, 1, 1);
+  cfg.dynamicSmemBytes = TC_SMEM;
+  cfg.stream = stream;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  ProfScope prof(PROF_GEMM, stream);
+  B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, m[0], m[1], m[2], m[3], a));
+  count_launch();
+  return B200RNN_OK;
+}
+
+}  // namespace
+
+// C[M,N] (+)= A[M,K] * B[N,K]^T (+ biases), operands already split into hi/lo matrices (K- or MN-major).
+int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
+                     const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
+                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready, int stream_clusters) {
+  int rc = check_tc_shape(M, N, K, C, c_rows, ready, splitk_ws != nullptr, stream_clusters);
+  if (rc) return rc;
+  // MN-major operands are read by the kernel's own loads: their tensor maps stay zero and unused
+  CUtensorMap m[4] = {};
+  const bool ok_a = A.mn || (make_map(&m[0], A.hi, M, K, A.ld) && make_map(&m[1], A.lo, M, K, A.ld));
+  const bool ok_b = B.mn || (make_map(&m[2], B.hi, N, K, B.ld) && make_map(&m[3], B.lo, N, K, B.ld));
+  if (!ok_a || !ok_b) {
+    set_error("tc_gemm: cuTensorMapEncodeTiled failed (operands must be 16-byte aligned, ld %% 4 == 0)");
+    return B200RNN_ERR_CUDA;
+  }
+  TcArgs a = tc_args(M, N, K, C, c_rows, bias1, bias2, bias2_n, accumulate, ready);
   a.a_mn = A.mn ? 1 : 0;
   a.b_mn = B.mn ? 1 : 0;
   a.a_hi = A.hi; a.a_lo = A.lo; a.lda = A.ld;
   a.b_hi = B.hi; a.b_lo = B.lo; a.ldb = B.ld;
-  a.tiles_m = (M + BM - 1) / BM;
-  a.tiles_n = N / BN;
   const int ntiles = a.tiles_m * a.tiles_n;
   const int nkb = (K + BK - 1) / BK;
+  const int sms = num_sms();
   // split-K when the tile count cannot fill the chip and K is long (the wgrad shapes: K = T*B)
   int splitk = 1;
   if (splitk_ws && ntiles * 2 <= sms && nkb >= 16) {
@@ -675,43 +945,39 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
   a.kb_per_split = (nkb + splitk - 1) / splitk;
   a.splitk = (nkb + a.kb_per_split - 1) / a.kb_per_split;
   a.partial = static_cast<float*>(splitk_ws);
-  a.ready = ready;
-  const int nitems = ntiles * a.splitk;
-  dim3 grid(nitems < sms ? nitems : sms, 1, 1);
-  if (!ready) {
-    ProfScope prof(PROF_GEMM, stream);
-    gemm_tf32x3_kernel<<<grid, TC_THREADS, TC_SMEM, stream>>>(m_ahi, m_alo, m_bhi, m_blo, a);
-    B200_CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  } else {
-    // Streamed: 4-CTA clusters (no cluster feature is used). A GPC holds floor(SMs / 4) of them whatever else runs
-    // in it, so the GEMM takes exactly `stream_clusters` of the 4-CTA cluster slots and leaves the others to the
-    // recurrence's 4-CTA clusters (api.cu); single CTAs spread over the GPCs would fragment them.
-    const int want = (nitems + 3) / 4;
-    grid.x = 4 * (want < stream_clusters ? want : stream_clusters);
-    static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
-    if (debug)
-      fprintf(stderr, "[b200rnn] streamed x-projection: gemm grid %u (4-CTA clusters) of %d SMs, %d row tiles x %d column tiles\n",
-              grid.x, sms, a.tiles_m, a.tiles_n);
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = 4;
-    attr.val.clusterDim.y = 1;
-    attr.val.clusterDim.z = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(TC_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = TC_SMEM;
-    cfg.stream = stream;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    ProfScope prof(PROF_GEMM, stream);
-    B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemm_tf32x3_kernel, m_ahi, m_alo, m_bhi, m_blo, a));
-    count_launch();
-  }
+  rc = launch_tc(m, a, stream_clusters, stream);
+  if (rc) return rc;
   if (a.splitk > 1)
     return launch_splitk_reduce(a.partial, a.splitk, M, N, C, c_rows, bias1, bias2, bias2_n, accumulate, stream);
   return B200RNN_OK;
+}
+
+// C[M,N] = A[M,K] * B[N,K]^T + biases with A in fp32, read in place through its row map and split on chip; B K-major
+// presplit. Same operands, same MMAs, same sums as tc_gemm_presplit on split(A), so C is bit-identical.
+int tc_gemm_f32a(const float* A, const RowMap& a_rows, const TcOperand& B, int M, int N, int K, float* C,
+                 const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
+                 int* ready, int stream_clusters) {
+  int rc = check_tc_shape(M, N, K, C, c_rows, ready, false, stream_clusters);
+  if (rc) return rc;
+  if (B.mn || K % BK != 0) {
+    set_error("tc_gemm: the fp32-A path takes a K-major presplit B and K %% 32 == 0");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  CUtensorMap m[4] = {};
+  int inner = 0;
+  if (!make_a_f32_map(&m[0], A, a_rows, M, K, &inner)) {
+    set_error("tc_gemm: the fp32 A operand cannot be read in place (16-byte aligned rows; batch dividing 128 or a "
+              "multiple of it)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  if (!make_map(&m[2], B.hi, N, K, B.ld) || !make_map(&m[3], B.lo, N, K, B.ld)) {
+    set_error("tc_gemm: cuTensorMapEncodeTiled failed (operands must be 16-byte aligned, ld %% 4 == 0)");
+    return B200RNN_ERR_CUDA;
+  }
+  TcArgs a = tc_args(M, N, K, C, c_rows, bias1, bias2, bias2_n, 0, ready);
+  a.a_f32 = 1;
+  a.a_inner = inner;
+  return launch_tc(m, a, stream_clusters, stream);
 }
 
 int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t stream) {
@@ -725,7 +991,7 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
   const float* b_lo = p.tc_b_lo;
   int rc = B200RNN_OK;
   // a_kcontig: A is [M rows][K]; else A is [K rows][M] (MN-major): the split copy keeps the source's orientation
-  if (!p.tc_a_presplit)
+  if (!p.tc_a_f32)
     rc = p.a_kcontig ? tc_split(p.A, p.a_rows, p.M, p.K, a_hi, a_lo, stream)
                      : tc_split(p.A, p.a_rows, p.K, p.M, a_hi, a_lo, stream);
   if (rc) return rc;
@@ -738,7 +1004,11 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
     b_hi = w_hi;
     b_lo = w_lo;
   }
-  TcOperand A{a_hi, a_lo, p.a_kcontig ? p.K : p.M, !p.a_kcontig}, B{b_hi, b_lo, p.b_kcontig ? p.K : p.N, !p.b_kcontig};
+  TcOperand B{b_hi, b_lo, p.b_kcontig ? p.K : p.N, !p.b_kcontig};
+  if (p.tc_a_f32)
+    return tc_gemm_f32a(p.A, p.a_rows, B, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, stream,
+                        p.tc_ready, p.tc_stream_clusters);
+  TcOperand A{a_hi, a_lo, p.a_kcontig ? p.K : p.M, !p.a_kcontig};
   return tc_gemm_presplit(A, B, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, 0, nullptr, 0, stream,
                           p.tc_ready, p.tc_stream_clusters);
 }

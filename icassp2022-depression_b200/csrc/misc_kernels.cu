@@ -23,7 +23,10 @@ __global__ void rng_setup_kernel(uint64_t* hdr, uint64_t seed, uint64_t offset, 
 }
 
 __global__ void dropout_kernel(const float* __restrict__ in, float* __restrict__ out, size_t n, float p,
-                               float scale, const uint64_t* __restrict__ hdr, uint32_t stream_id) {
+                               float scale, const uint64_t* __restrict__ hdr, uint32_t stream_id,
+                               int* __restrict__ clear, int nclear) {
+  if (blockIdx.x == 0)
+    for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
   const uint64_t seed = hdr[0], offset = hdr[1];
   const size_t nquad = (n + 3) / 4;
   // keep iff u >= p where u = x * 2^-32 in [0,1)
@@ -43,35 +46,6 @@ __global__ void dropout_kernel(const float* __restrict__ in, float* __restrict__
     } else {
       for (int e = 0; e < 4 && i0 + e < n; ++e) out[i0 + e] = rr[e] >= thr ? in[i0 + e] * scale : 0.f;
     }
-  }
-}
-
-__global__ void dropout_split_kernel(const float* __restrict__ in, float* __restrict__ out, float* __restrict__ hi,
-                                     float* __restrict__ lo, size_t n, float p, float scale,
-                                     const uint64_t* __restrict__ hdr, uint32_t stream_id, int* __restrict__ clear,
-                                     int nclear) {
-  if (blockIdx.x == 0)
-    for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
-  const uint64_t seed = hdr[0], offset = hdr[1];
-  const size_t nquad = n / 4;
-  const uint32_t thr = (uint32_t)fminf(p * 4294967296.0f, 4294967295.0f);
-  for (size_t qd = blockIdx.x * (size_t)blockDim.x + threadIdx.x; qd < nquad;
-       qd += (size_t)gridDim.x * blockDim.x) {
-    Philox4 r = philox4x32_10(seed, offset + qd, (uint64_t)stream_id);  // same stream as dropout_kernel
-    float4 v = *reinterpret_cast<const float4*>(in + qd * 4);
-    v.x = r.x >= thr ? v.x * scale : 0.f;
-    v.y = r.y >= thr ? v.y * scale : 0.f;
-    v.z = r.z >= thr ? v.z * scale : 0.f;
-    v.w = r.w >= thr ? v.w * scale : 0.f;
-    if (out) *reinterpret_cast<float4*>(out + qd * 4) = v;
-    float4 h, l;
-    uint32_t t;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(v.x)); h.x = __uint_as_float(t); l.x = v.x - h.x;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(v.y)); h.y = __uint_as_float(t); l.y = v.y - h.y;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(v.z)); h.z = __uint_as_float(t); l.z = v.z - h.z;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(v.w)); h.w = __uint_as_float(t); l.w = v.w - h.w;
-    *reinterpret_cast<float4*>(hi + qd * 4) = h;
-    *reinterpret_cast<float4*>(lo + qd * 4) = l;
   }
 }
 
@@ -117,36 +91,17 @@ int launch_rng_setup(uint64_t* hdr, uint64_t seed, uint64_t offset, uint64_t* st
 }
 
 int launch_dropout(const float* in, float* out, size_t n, float p, const uint64_t* hdr, uint32_t stream_id,
-                   cudaStream_t stream) {
+                   cudaStream_t stream, int* clear, int nclear) {
   if (n == 0) return B200RNN_OK;
   const float scale = p < 1.f ? 1.f / (1.f - p) : 0.f;
   size_t nquad = (n + 3) / 4;
   int blocks = (int)((nquad + 255) / 256);
   if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-  dropout_kernel<<<blocks, 256, 0, stream>>>(in, out, n, p, scale, hdr, stream_id);
+  dropout_kernel<<<blocks, 256, 0, stream>>>(in, out, n, p, scale, hdr, stream_id, clear, clear ? nclear : 0);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;
 }
-
-int launch_dropout_split(const float* in, float* out, float* hi, float* lo, size_t n, float p, const uint64_t* hdr,
-                         uint32_t stream_id, cudaStream_t stream, int* clear, int nclear) {
-  if (n == 0) return B200RNN_OK;
-  if (n % 4 != 0) {
-    set_error("dropout_split: element count must be a multiple of 4");
-    return B200RNN_ERR_INVALID;
-  }
-  const float scale = p < 1.f ? 1.f / (1.f - p) : 0.f;
-  size_t nquad = n / 4;
-  int blocks = (int)((nquad + 255) / 256);
-  if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
-  dropout_split_kernel<<<blocks, 256, 0, stream>>>(in, out, hi, lo, n, p, scale, hdr, stream_id, clear,
-                                                   clear ? nclear : 0);
-  B200_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return B200RNN_OK;
-}
-
 
 int launch_bias_reduce(const float* part, int nslices, int mode, int H, float* db_ih, float* db_hh,
                        int accumulate, cudaStream_t stream) {

@@ -12,14 +12,9 @@ int launch_rng_setup(uint64_t* hdr, uint64_t seed, uint64_t offset, uint64_t* st
 
 // out[i] = in[i] * mask(i) / (1-p) over n dense elements; mask is Philox4x32-10 keyed by hdr = {seed, offset}
 // and the per-layer stream id; in == out is allowed (in place).
+// `clear` (optional): nclear ints zeroed by the same launch (the ready counters of a streamed GEMM that reads out).
 int launch_dropout(const float* in, float* out, size_t n, float p, const uint64_t* hdr, uint32_t stream_id,
-                   cudaStream_t stream);
-
-// Same, and additionally emits the TF32 hi/lo split of the dropped values (operand of the next layer's K1 GEMM),
-// saving a separate pass over the layer output. n must be a multiple of 4, all pointers 16-byte aligned.
-// `clear` (optional): nclear ints zeroed by the same launch (the ready counters of a streamed GEMM that reads hi / lo).
-int launch_dropout_split(const float* in, float* out, float* hi, float* lo, size_t n, float p, const uint64_t* hdr,
-                         uint32_t stream_id, cudaStream_t stream, int* clear = nullptr, int nclear = 0);
+                   cudaStream_t stream, int* clear = nullptr, int nclear = 0);
 
 // db_ih / db_hh from the per-slice partial sums written by the backward recurrence:
 //   part [nslices][(G+1)*H]  (first G*H: sum of dGi columns; tail H: GRU sum of dn*r)
