@@ -17,7 +17,7 @@ GRU, LSTM = 0, 1
 FLAG_ACCUMULATE_GRADS = 1
 FLAG_SAVE_FOR_BACKWARD = 2
 FLAG_FUSED_LN = 4
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)
 SYMBOLS = (
@@ -150,7 +150,7 @@ def load() -> ctypes.CDLL:
     ]
     lib.b200rnn_forward_fused.restype = c_int
     lib.b200rnn_forward_fused.argtypes = lib.b200rnn_forward.argtypes[:-1] + [c_void_p, c_void_p, c_float, c_void_p,
-                                                                              c_void_p, c_void_p, c_void_p]
+                                                                              c_void_p, c_void_p, c_void_p, c_void_p]
     lib.b200rnn_wcache_bytes.restype = c_int
     lib.b200rnn_wcache_bytes.argtypes = [POINTER(Desc), POINTER(c_size_t)]
     lib.b200rnn_prepare_weights.restype = c_int

@@ -102,7 +102,7 @@ class _RNNFunction(torch.autograd.Function):
                     y.data_ptr(), ys_t, ys_b, h_n.data_ptr(), c_n.data_ptr() if c_n is not None else None,
                     reserve.data_ptr() if save else None, scratch.data_ptr(),
                     0, 0, rng_state.data_ptr() if rng_state is not None else None, None, None, 0.0, None,
-                    lengths.data_ptr() if lengths is not None else None, None, _stream_ptr(dev))
+                    lengths.data_ptr() if lengths is not None else None, None, None, _stream_ptr(dev))
             _lib.check(rc, "b200rnn_forward")
         else:
             h_n.zero_()
@@ -225,7 +225,7 @@ class _LNRNNPoolFunction(torch.autograd.Function):
                 reserve.data_ptr(), scratch.data_ptr(), 0, 0,
                 rng_state.data_ptr() if rng_state is not None else None,
                 ln_w.data_ptr() if fused_ln else None, ln_b.data_ptr() if fused_ln else None, float(ln_eps),
-                pooled.data_ptr(), None, None, _stream_ptr(dev))
+                pooled.data_ptr(), None, None, None, _stream_ptr(dev))
         _lib.check(rc, "b200rnn_forward_fused")
         ctx.cfg, ctx.grad_sink, ctx.ln_eps, ctx.fused_ln = cfg, grad_sink, float(ln_eps), fused_ln
         ctx.save_for_backward(x_tm, y, reserve, ln_w if fused_ln else x_tm.new_empty(0), *weights)
@@ -331,9 +331,10 @@ def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig
 def rnn_forward_fused(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig,
                       rng_state: Optional[torch.Tensor] = None, ln_weight: Optional[torch.Tensor] = None,
                       ln_bias: Optional[torch.Tensor] = None, ln_eps: float = 1e-5, pool_sum: bool = False,
-                      wcache: Optional[torch.Tensor] = None):
+                      wcache: Optional[torch.Tensor] = None, prologue_done: Optional[torch.cuda.Event] = None):
     """No-grad forward with the shell fusions of ``b200rnn_forward_fused``: optional LayerNorm prologue on ``x``
     and, with ``pool_sum``, the sum over time of the output instead of the sequence (``[B, D*H]``).
+    ``prologue_done`` is recorded on the current stream after the layer-0 operand preparation, before the first GEMM.
 
     Mirrors ``x = ln(x); x, _ = gru(x); x = x.sum(dim=1)`` (fuse_net_whole.py:360-362). Returns ``(out, h_n[, c_n])``.
     """
@@ -358,6 +359,8 @@ def rnn_forward_fused(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNN
     h_n = torch.empty(L * D, B, H, dtype=torch.float32, device=dev)
     c_n = torch.empty(L * D, B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
     params = _lib.ptr_array([w.data_ptr() for w in weights])
+    if prologue_done is not None and not prologue_done.cuda_event:
+        prologue_done.record()      # torch creates the CUDA event at its first record
     with _on(dev):
         rc = lib.b200rnn_forward_fused(
             ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params, y_ptr, ys_t, ys_b,
@@ -365,7 +368,8 @@ def rnn_forward_fused(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNN
             rng_state.data_ptr() if rng_state is not None else None,
             ln_weight.data_ptr() if ln_weight is not None else None,
             ln_bias.data_ptr() if ln_bias is not None else None,
-            float(ln_eps), pool_ptr, None, wcache.data_ptr() if wcache is not None else None, _stream_ptr(dev))
+            float(ln_eps), pool_ptr, None, wcache.data_ptr() if wcache is not None else None,
+            prologue_done.cuda_event if prologue_done is not None else None, _stream_ptr(dev))
     _lib.check(rc, "b200rnn_forward_fused")
     return (out, h_n) if c_n is None else (out, h_n, c_n)
 

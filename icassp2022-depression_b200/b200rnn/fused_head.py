@@ -157,6 +157,7 @@ class FusedFuseStep:
         self.concurrent_branches = bool(concurrent_branches)
         self.split_head = bool(concurrent_branches)   # text half of the head on the text stream, before the join
         self._side = None
+        self._prologue_done = None
         self.regression = bool(getattr(model, "regression", False))
         self.C = 1 if self.regression else 2
         if model.num_classes != self.C:
@@ -248,17 +249,20 @@ class FusedFuseStep:
                                         m.lstm_net._rng_state, wcache=m.lstm_net.frozen_weight_cache())
         return seq, h_n.contiguous()
 
-    def _audio_branch(self, batch: FuseBatch):
+    def _audio_branch(self, batch: FuseBatch, prologue_done=None):
         m = self.model
-        return m.lstm_net_audio.forward_ln_sum(batch.audio, None if self.regression else m.ln)
+        return m.lstm_net_audio.forward_ln_sum(batch.audio, None if self.regression else m.ln, prologue_done)
 
     def _encoders(self, batch: FuseBatch, text_stage=None):
         """The two independent encoder branches (fuse_net_whole.py:347 text BiLSTM, :361 audio GRU). With
         ``concurrent_branches`` the audio branch - the critical path, 2 x 120 serial steps - is enqueued on a second,
         high-priority stream (fork / join by events, captured as parallel branches of the CUDA graph): its persistent
         recurrence occupies most of the 132 SMs for most of the step, the text kernels fill the rest instead of
-        waiting behind it. ``text_stage(seq, h_n)`` (the text half of the head kernel) runs on the text stream before
-        the join, i.e. off the critical path."""
+        waiting behind it. The text stream is gated on the audio prologue (LayerNorm): CTAs cannot be pre-empted, and
+        text GEMM CTAs that are pending while the LayerNorm runs take the SMs it frees and hold them for tens of µs,
+        so the audio GEMM and recurrence would start late. Gated, the audio kernels become pending no later than the
+        text ones, at higher priority. ``text_stage(seq, h_n)`` (the text half of the head kernel) runs on the text
+        stream before the join, i.e. off the critical path."""
         dev = batch.text.device
         if not self.concurrent_branches:
             seq, h_n = self._text_branch(batch)
@@ -266,10 +270,12 @@ class FusedFuseStep:
             return seq, h_n, self._audio_branch(batch), extra
         if self._side is None:
             self._side = torch.cuda.Stream(dev, priority=-1)
+            self._prologue_done = torch.cuda.Event()
         main = torch.cuda.current_stream(dev)
         self._side.wait_stream(main)
         with torch.cuda.stream(self._side):
-            pooled = self._audio_branch(batch)
+            pooled = self._audio_branch(batch, self._prologue_done)
+        main.wait_event(self._prologue_done)
         seq, h_n = self._text_branch(batch)
         extra = text_stage(seq, h_n) if text_stage is not None else None
         main.wait_stream(self._side)

@@ -180,7 +180,8 @@ class _B200RNNBase(nn.Module):
             raise NotImplementedError("b200rnn: unbatched 2-D input is not implemented")
         return rnn_forward(input, self._flat_weights, self._config(), self._rng_state, self._grad_sink)
 
-    def forward_ln_sum(self, input: torch.Tensor, ln: Optional[nn.LayerNorm] = None) -> torch.Tensor:
+    def forward_ln_sum(self, input: torch.Tensor, ln: Optional[nn.LayerNorm] = None,
+                       prologue_done: Optional[torch.cuda.Event] = None) -> torch.Tensor:
         """``self(ln(input))[0].sum(dim=time)`` — the audio branch of fuse_net_whole.py:360-362 / fuse_net.py:338-339.
 
         For widths the tensor-core projection takes, LayerNorm is folded into the layer-0 operand preparation and the
@@ -189,24 +190,29 @@ class _B200RNNBase(nn.Module):
         autograd (audio_gru_whole.py:103-108 + loss.backward()) the same fusions run in both directions
         (``b200rnn_backward_fused``: LayerNorm backward, pooled-gradient broadcast inside the BPTT kernel). Otherwise
         the same value is computed unfused.
+
+        ``prologue_done`` (no-grad fused path): recorded on the current stream once the LayerNorm prologue is
+        enqueued, before the first GEMM; on every other path, recorded before anything is enqueued.
         """
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
         shape_ok = (input.is_cuda and input.dim() == 3 and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and
                                     ln.bias is not None)))
+        fusable = not need_grad and shape_ok
+        if prologue_done is not None and not fusable:
+            prologue_done.record()
         if need_grad and shape_ok and not isinstance(input, nn.utils.rnn.PackedSequence):
             # training graph: LayerNorm forward+backward folded around the layer-0 GEMMs, pooled gradient broadcast
             # inside the BPTT kernel (no [T,B,H] output gradient, no LN(x) autograd tensor)
             return rnn_ln_pool_sum(input, self._flat_weights, self._config(), self._rng_state, self._grad_sink,
                                    ln.weight if ln is not None else None, ln.bias if ln is not None else None,
                                    ln.eps if ln is not None else 1e-5)
-        fusable = not need_grad and shape_ok
         if fusable:
             out = rnn_forward_fused(input, self._flat_weights, self._config(), self._rng_state,
                                     ln.weight if ln is not None else None, ln.bias if ln is not None else None,
                                     ln.eps if ln is not None else 1e-5, pool_sum=True,
-                                    wcache=self.frozen_weight_cache())
+                                    wcache=self.frozen_weight_cache(), prologue_done=prologue_done)
             return out[0]
         seq = self(ln(input) if ln is not None else input)[0]
         return seq.sum(dim=1 if self.batch_first else 0)

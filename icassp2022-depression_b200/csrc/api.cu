@@ -265,12 +265,17 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
                                       const float* const* params, float* y, int64_t ys_t, int64_t ys_b, float* h_n,
                                       float* c_n, void* reserve, void* scratch, uint64_t seed, uint64_t offset,
                                       uint64_t* rng_state, const float* ln_gamma, const float* ln_beta, float ln_eps,
-                                      float* y_pool, const int32_t* lengths, const void* wcache, void* stream_) {
+                                      float* y_pool, const int32_t* lengths, const void* wcache,
+                                      void* prologue_done, void* stream_) {
   Dims d;
   int rc = check_desc(desc, &d);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
-  if (d.B == 0 || d.T == 0) return B200RNN_OK;
+  cudaEvent_t prologue_ev = static_cast<cudaEvent_t>(prologue_done);
+  if (d.B == 0 || d.T == 0) {
+    if (prologue_ev) B200_CUDA_CHECK(cudaEventRecord(prologue_ev, st));
+    return B200RNN_OK;
+  }
   if (wcache && !aligned_to(wcache, 256)) {
     set_error("forward: the weight cache must be 256-byte aligned");
     return B200RNN_ERR_INVALID;
@@ -391,6 +396,9 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
       set_error("forward: the fused LayerNorm prologue needs the tensor-core input projection (input_size %% 32 == 0)");
       return B200RNN_ERR_UNSUPPORTED;
     }
+    // everything before the first GEMM is enqueued: kernels of a stream gated on this event become pending no earlier
+    // than the layer-0 GEMM, which then wins the SMs on this stream's priority
+    if (l == 0 && prologue_ev) B200_CUDA_CHECK(cudaEventRecord(prologue_ev, st));
     ready_zeroed = false;
     for (int k = 0; k < d.D; ++k) {
       const float* const* pp = params + (size_t)(l * d.D + k) * 4;
@@ -467,7 +475,7 @@ B200RNN_API int b200rnn_forward(const b200rnn_desc* desc, const float* x, int64_
                                 float* c_n, void* reserve, void* scratch, uint64_t seed, uint64_t offset,
                                 uint64_t* rng_state, void* stream_) {
   return b200rnn_forward_fused(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset,
-                               rng_state, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, stream_);
+                               rng_state, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr, stream_);
 }
 
 B200RNN_API int b200rnn_wcache_bytes(const b200rnn_desc* desc, size_t* bytes) {

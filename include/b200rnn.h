@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define B200RNN_ABI_VERSION 2
+#define B200RNN_ABI_VERSION 3
 
 #if defined(__GNUC__)
 #define B200RNN_API __attribute__((visibility("default")))
@@ -136,14 +136,20 @@ B200RNN_API int b200rnn_forward(const b200rnn_desc* desc, const float* x, int64_
  *                             TF32 hi/lo split of every weight_ih, so that frozen encoders (fuse_net_whole.py:590-593:
  *                             only fc_final.0.weight trains) do not re-split their weights at every step. NULL = split on
  *                             the fly. The caller owns it and must refresh it whenever a weight_ih changes.
- * Everything else as b200rnn_forward (which is this call with the six extra arguments zero).
+ *   prologue_done           : optional cudaEvent_t, recorded on `stream` once the layer-0 operand preparation (RNG
+ *                             setup, LayerNorm or input copy) is enqueued, before the first input projection. A
+ *                             concurrent stream that waits on it enqueues its own kernels only after that point, so the
+ *                             GPU's block scheduler sees this call's first GEMM and recurrence before them (the fuse
+ *                             step gates its text branch on it). NULL = not recorded.
+ * Everything else as b200rnn_forward (which is this call with the seven extra arguments zero).
  */
 B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, int64_t x_stride_t,
                                       int64_t x_stride_b, const float* const* params, float* y, int64_t y_stride_t,
                                       int64_t y_stride_b, float* h_n, float* c_n, void* reserve, void* scratch,
                                       uint64_t dropout_seed, uint64_t dropout_offset, uint64_t* rng_state,
                                       const float* ln_gamma, const float* ln_beta, float ln_eps, float* y_pool,
-                                      const int32_t* lengths, const void* wcache, void* stream /* cudaStream_t */);
+                                      const int32_t* lengths, const void* wcache, void* prologue_done,
+                                      void* stream /* cudaStream_t */);
 
 /* Weight cache of b200rnn_forward_fused: size for this descriptor (batch / seq_len are ignored), and the pass that
  * fills it (one small launch per weight_ih; 256-byte aligned caller-owned buffer). */
