@@ -132,6 +132,9 @@ struct ScratchLayout {
   long long b_ldk;  // leading dimension of the transposed operands: T*B rounded up to a multiple of 4
   size_t b_dxln, b_lnpart;  // fused LayerNorm backward: dense d/dLN(x) [TB][I], per-CTA column partials
   size_t b_total;
+  // both passes, past both layouts: int [B], the batch-slot order of a ragged batch (launch_length_order); the forward
+  // and the backward each compute it from `lengths`
+  size_t order;
 };
 
 void make_scratch(const Dims& d, ScratchLayout* s) {
@@ -197,6 +200,9 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
   s->b_lnpart = off;
   off += align_up(layernorm_bwd_scratch_floats(d.I), ALIGN_F);
   s->b_total = off;
+
+  s->order = s->f_total > s->b_total ? s->f_total : s->b_total;
+  s->f_total = s->b_total = s->order + align_up((size_t)d.B, ALIGN_F);
 }
 
 // ---- weight cache layout (floats): per (layer, direction) the TF32 hi then lo split of weight_ih [G*H, I_l] -------
@@ -326,6 +332,12 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     rc = launch_rng_setup(hdr, seed, offset, rng_state, drop ? (uint64_t)((d.TB * d.DH + 3) / 4) : 0, st);
     if (rc) return rc;
   }
+  int* order = nullptr;  // ragged batch: rows sorted into batch slots by length, shared by every layer
+  if (lengths) {
+    order = reinterpret_cast<int*>(S + sl.order);
+    rc = launch_length_order(lengths, d.B, order, st);
+    if (rc) return rc;
+  }
 
   const bool tc = tc_available();
   int sms = NUM_SMS;
@@ -361,6 +373,7 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     rp.mode = d.mode; rp.B = d.B; rp.T = d.T; rp.H = d.H; rp.D = d.D;
     rp.training = save ? 1 : 0;
     rp.lengths = lengths;
+    rp.order = order;
     RecFwdLaunch rec;
     rc = plan_rec_fwd(rp, &rec);
     if (rc) return rc;
@@ -561,6 +574,12 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
   const uint64_t* hdr = reinterpret_cast<const uint64_t*>(R);  // dropout seed/offset used by the forward
   const int accumulate = (desc->flags & B200RNN_FLAG_ACCUMULATE_GRADS) ? 1 : 0;
   void* gemm_ws = sl.b_gemm_bytes ? (void*)(S + sl.b_gemm) : nullptr;
+  int* order = nullptr;  // the forward's slot order, recomputed from the same lengths (nothing of it is in the reserve)
+  if (lengths) {
+    order = reinterpret_cast<int*>(S + sl.order);
+    rc = launch_length_order(lengths, d.B, order, st);
+    if (rc) return rc;
+  }
 
   for (int l = d.L - 1; l >= 0; --l) {
     const int Il = l == 0 ? d.I : (int)d.DH;
@@ -592,6 +611,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
       bp.dbias_part[k] = S + sl.b_bpart[k];
     }
     bp.lengths = lengths;
+    bp.order = order;
     rc = launch_rec_bwd(bp, st);
     if (rc) return rc;
 

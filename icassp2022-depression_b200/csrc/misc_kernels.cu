@@ -1,5 +1,5 @@
 // misc_kernels.cu — dropout (K7), weight transpose, bias-gradient reduction. All HBM-bound, coalesced,
-// grid sized in multiples of the SM count.
+// grid sized in multiples of the SM count. Plus the one-CTA batch-slot order of a ragged batch.
 #include "misc_kernels.cuh"
 
 namespace b200rnn {
@@ -46,6 +46,30 @@ __global__ void dropout_kernel(const float* __restrict__ in, float* __restrict__
     } else {
       for (int e = 0; e < 4 && i0 + e < n; ++e) out[i0 + e] = rr[e] >= thr ? in[i0 + e] * scale : 0.f;
     }
+  }
+}
+
+// Rank of row i = #{j : len_j > len_i} + #{j < i : len_j == len_i}: a permutation, deterministic, no atomics. The
+// lengths go through shared memory in tiles of ORDER_TILE; B^2 compares in all (16K at B = 128).
+constexpr int ORDER_TILE = 1024;
+
+__global__ void length_order_kernel(const int* __restrict__ lengths, int B, int* __restrict__ order) {
+  __shared__ int tile[ORDER_TILE];
+  for (int i0 = 0; i0 < B; i0 += blockDim.x) {  // every thread runs every iteration (the barriers below)
+    const int i = i0 + threadIdx.x;
+    const int li = i < B ? lengths[i] : 0;
+    int rank = 0;
+    for (int j0 = 0; j0 < B; j0 += ORDER_TILE) {
+      const int n = min(ORDER_TILE, B - j0);
+      __syncthreads();
+      for (int k = threadIdx.x; k < n; k += blockDim.x) tile[k] = lengths[j0 + k];
+      __syncthreads();
+      for (int k = 0; k < n; ++k) {
+        const int lj = tile[k];
+        rank += (lj > li || (lj == li && j0 + k < i)) ? 1 : 0;
+      }
+    }
+    if (i < B) order[rank] = i;
   }
 }
 
@@ -98,6 +122,15 @@ int launch_dropout(const float* in, float* out, size_t n, float p, const uint64_
   int blocks = (int)((nquad + 255) / 256);
   if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
   dropout_kernel<<<blocks, 256, 0, stream>>>(in, out, n, p, scale, hdr, stream_id, clear, clear ? nclear : 0);
+  B200_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return B200RNN_OK;
+}
+
+int launch_length_order(const int* lengths, int B, int* order, cudaStream_t stream) {
+  if (B <= 0) return B200RNN_OK;
+  const int threads = B < ORDER_TILE ? (B + 31) / 32 * 32 : ORDER_TILE;
+  length_order_kernel<<<1, threads, 0, stream>>>(lengths, B, order);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;

@@ -16,6 +16,10 @@ int launch_rng_setup(uint64_t* hdr, uint64_t seed, uint64_t offset, uint64_t* st
 int launch_dropout(const float* in, float* out, size_t n, float p, const uint64_t* hdr, uint32_t stream_id,
                    cudaStream_t stream, int* clear = nullptr, int nclear = 0);
 
+// Batch-slot order of a ragged batch: order[slot] = the row of rank `slot` when the B rows are sorted by descending
+// lengths[row], ties by row index (a stable sort: non-increasing lengths give the identity). One CTA.
+int launch_length_order(const int* lengths, int B, int* order, cudaStream_t stream);
+
 // db_ih / db_hh from the per-slice partial sums written by the backward recurrence:
 //   part [nslices][(G+1)*H]  (first G*H: sum of dGi columns; tail H: GRU sum of dn*r)
 //   GRU : db_ih = sum(part[:, :3H]);  db_hh = (sum part[:, :2H], sum part[:, 3H:4H])

@@ -5,6 +5,9 @@
 namespace b200rnn {
 
 // One launch runs ALL directions of one layer: grid = D * nslices clusters of C CTAs.
+// Ragged batches (lengths != NULL, the VL instantiations): batch slot q of slice s holds row order[s*BS + q], so a
+// cluster holds sequences of similar length, and it runs only as many steps as its longest one; the outputs and gate
+// gradients of the steps it skips are written as zeros, like those of every step past a sequence's length.
 struct RecFwdParams {
   int mode, B, T, H, D;
   int training;              // save activated gates + hn/c for backward
@@ -19,6 +22,7 @@ struct RecFwdParams {
   float* c_n;                // [D,B,H] of this layer (LSTM) or NULL
   long long* trace;          // debug: per-step phase timestamps of CTA 0 / warp 0 (NULL = off), [T][8]
   const int* lengths;        // optional [B]: valid steps per sequence (PackedSequence semantics); NULL = all T
+  const int* order;          // with lengths: [B] row of each batch slot, by descending length (launch_length_order)
   // streamed x-projection (D = 1 only): the GEMM writing gates[0] may still run. The x-projection of step t is read
   // only once ready[m] >= tiles_n for the row tiles m holding rows [t*B, (t+1)*B) (TC_TILE_M rows each). NULL = the
   // gates are complete at launch.
@@ -57,6 +61,7 @@ struct RecBwdParams {
   float* dbias_part[2];      // out: [nslices][(G+1)*H] per-slice column sums (rows 0..G*H: dGi; GRU tail H: dghn)
   int nslices_out;           // filled by the launcher
   const int* lengths;        // optional [B], as in the forward
+  const int* order;          // with lengths: [B] row of each batch slot, as in the forward
 };
 
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)

@@ -16,6 +16,9 @@
 //     transaction bytes on an mbarrier in the destination CTA): data and "ready" signal travel together, the
 //     consumer waits on a local mbarrier, double buffered. No cluster barrier, fence or L1 flush in the loop.
 //   * batch slices are independent clusters: no grid-wide synchronisation anywhere.
+//   * ragged batches (the VL instantiations): the batch slots hold the rows sorted by descending length
+//     (RecFwdParams::order), and a cluster runs only the steps of its longest sequence; the skipped steps' outputs and
+//     gate gradients are written as zeros after the loop.
 //
 // fp32 FFMA for most configs: the per-step contraction is [BS x H] x [H x G*HS] with BS = 2..8 rows per CTA — far too
 // skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference. The GRU H=256 8-row config runs it
@@ -139,8 +142,8 @@ __device__ __forceinline__ void allgather_units(float val, float* vec_local, int
 // =================================================================================================
 // One (unit j, batch row b) output of a forward lane, everything it does outside the contraction: the x-projection
 // prefetched one step ahead, the gate math and state update, the step's global stores, and the final h_n / c_n / y_pool
-// stores. VL: past its length a sequence keeps its state and emits 0 (PackedSequence semantics). A row past the batch
-// (!valid) computes on zeros and stores nothing.
+// stores. VL: past its length a sequence keeps its state and emits 0 (PackedSequence semantics), and batch slot `slot`
+// holds row order[slot]. A slot past the batch (!valid) computes on zeros and stores nothing.
 // The stores of a step are held in registers until flush(), which the kernels call behind the next step's first chunk:
 // between the exchange and the next contraction they sat on the serial path of every step (225 cycles).
 // Saved for the backward, in the format rec_bwd_kernel's load_step reads: gates[t][b][g*H + j] (the x-projection on
@@ -157,11 +160,14 @@ struct FwdCell {
   float gi[G];                       // x-projection of the step update() computes next
   float pend_y, pend_s[G], pend_sx;  // stores of the last step update() computed
 
-  __device__ __forceinline__ FwdCell(const RecFwdParams& p, int dir, int j_, int b_)
-      : gates(p.gates[dir]), extra(p.extra[dir]), j(j_), b(b_), len(p.T), valid(b_ < p.B) {
+  __device__ __forceinline__ FwdCell(const RecFwdParams& p, int dir, int j_, int slot)
+      : gates(p.gates[dir]), extra(p.extra[dir]), j(j_), b(slot), len(p.T), valid(slot < p.B) {
     bhn = (MODE == B200RNN_GRU) ? p.b_hh[dir][2 * H + j] : 0.f;
     if constexpr (VL) {
-      if (valid) len = p.lengths[b];
+      if (valid) {
+        b = p.order[slot];
+        len = p.lengths[b];
+      }
     }
 #pragma unroll
     for (int g = 0; g < G; ++g) gi[g] = 0.f;
@@ -238,7 +244,20 @@ struct FwdCell {
       if (MODE == B200RNN_LSTM && p.c_n) p.c_n[((size_t)dir * p.B + b) * H + j] = c;
     }
   }
+
+  // VL, after the cluster's Ts steps: the outputs of the steps [Ts, T) it skipped are 0, as past any sequence's length
+  // (the caller and the W_hh gradient GEMM read them). A cluster of empty sequences never reached finish().
+  __device__ __forceinline__ void skip_tail(const RecFwdParams& p, int dir, int Ts) {
+    if (Ts == 0) finish(p, dir);
+    if (valid && p.y)
+      for (int t = Ts; t < p.T; ++t) p.y[(long long)t * p.y_st + (long long)b * p.y_sb + dir * H + j] = 0.f;
+  }
 };
+
+// VL: the steps a cluster runs, the length of its first batch slot (the longest: order sorts by descending length)
+__device__ __forceinline__ int slice_steps(const int* lengths, const int* order, int b0, int T) {
+  return min(max(lengths[order[b0]], 0), T);
+}
 
 // Streamed x-projection (RecFwdParams::ready, api.cu): before a warp reads the x-projection of step t, it waits until
 // the GEMM has published every row tile that holds rows [t*B, (t+1)*B). The whole warp polls the counter with acquire
@@ -282,7 +301,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
   const int slice = cid - dir * nslices;
   const int b0 = slice * BS;
   const int j0 = (int)rank * HS;
-  const int T = p.T;
+  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
   const float* w_hh = p.w_hh[dir];
 
   if (tid == 0) {
@@ -409,6 +428,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       cell.load_gi(p, dir ? (T - 2 - step) : (step + 1));
     }
   }
+  if constexpr (VL) cell.skip_tail(p, dir, T);
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
 }
 
@@ -471,7 +491,7 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
   const int slice = cid - dir * nslices;
   const int b0 = slice * BS;
   const int j0 = (int)rank * HS;
-  const int T = p.T;
+  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
   const float* w_hh = p.w_hh[dir];
 
   if (tid == 0) {
@@ -622,6 +642,10 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
       for (int jb = 0; jb < 2; ++jb) cell[jb].load_gi(p, dir ? (T - 2 - step) : (step + 1));
     }
   }
+  if constexpr (VL) {
+#pragma unroll
+    for (int jb = 0; jb < 2; ++jb) cell[jb].skip_tail(p, dir, T);
+  }
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
 }
 
@@ -670,7 +694,8 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
   const int slice = cid - dir * nslices;
   const int b0 = slice * BS;
   const int j0 = (int)rank * HS;
-  const int B = p.B, T = p.T;
+  const int B = p.B;
+  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
   const float* w_prep = p.w_prep[dir] + (size_t)rank * G * HS * H;
 
   if (tid == 0) {
@@ -697,8 +722,8 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 
   const int uw = LM::unit(lane), qb = LM::q(lane);
   const int j = j0 + w * UPW + uw;
-  const int b = b0 + qb;
-  const bool valid = b < B;
+  const bool valid = b0 + qb < B;
+  const int b = (VL && valid) ? p.order[b0 + qb] : b0 + qb;  // VL: batch slot b0 + qb holds row order[b0 + qb]
   const float* gates = p.gates[dir];
   const float* extra = p.extra[dir];
   float* dgates = p.dgates[dir];
@@ -848,6 +873,17 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     fold_pairs<1, UPL, BS>(acc2, acc);
     warp_transpose_reduce<1, KL, UPL, BS>(acc);
     dh_carry = direct + acc[0][0][0];
+  }
+  if constexpr (VL) {
+    // the steps [T, p.T) the cluster skipped: their gate gradients are 0, as past any sequence's length (the wgrad and
+    // dgrad GEMMs sum over every step)
+    if (valid)
+      for (int t = T; t < p.T; ++t) {
+        float* gp = dgates + ((size_t)t * B + b) * GH + j;
+#pragma unroll
+        for (int g = 0; g < G; ++g) gp[g * H] = 0.f;
+        if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + b) * H + j] = 0.f;
+      }
   }
 
   // ---- per-slice bias-gradient partials: sum over this slice's batch rows (the low lane bits) -------------
