@@ -17,6 +17,7 @@ GRU, LSTM = 0, 1
 FLAG_ACCUMULATE_GRADS = 1
 FLAG_SAVE_FOR_BACKWARD = 2
 FLAG_FUSED_LN = 4
+FLAG_TF32 = 8
 ABI_VERSION = 3
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)

@@ -26,6 +26,19 @@ class RNNConfig:
     dropout: float
     training: bool
     batch_first: bool
+    tf32: bool = False   # single-pass TF32 tensor-core GEMMs / tc8 recurrence (tf32_enabled()), else 3xTF32
+
+
+def tf32_enabled() -> bool:
+    """Whether torch's fp32 matmul precision asks for TF32: ``torch.backends.cuda.matmul.fp32_precision``, or, while
+    that is ``"none"``, the global ``torch.backends.fp32_precision``. ``torch.set_float32_matmul_precision("high")``
+    sets the former to ``"tf32"``, ``"highest"`` to ``"ieee"``; the default ``"none"`` / ``"ieee"`` keeps 3xTF32.
+    (``torch.get_float32_matmul_precision()`` is not used: it raises once both the legacy and the new API have been
+    used in a process.) The cuDNN RNN knob, which defaults to TF32, is deliberately not followed."""
+    mode = torch.backends.cuda.matmul.fp32_precision
+    if mode == "none":
+        mode = torch.backends.fp32_precision
+    return mode == "tf32"
 
 
 def _require_cuda_f32(t: torch.Tensor, name: str) -> None:
@@ -53,6 +66,8 @@ def _make_desc(cfg: RNNConfig, B: int, T: int, save: bool, accumulate: bool = Fa
         flags |= _lib.FLAG_ACCUMULATE_GRADS
     if fused_ln:
         flags |= _lib.FLAG_FUSED_LN
+    if cfg.tf32:
+        flags |= _lib.FLAG_TF32
     return _lib.Desc(cfg.mode, B, T, cfg.input_size, cfg.hidden_size, cfg.num_layers, cfg.num_dirs,
                      1 if cfg.training else 0, float(cfg.dropout), flags)
 

@@ -147,6 +147,10 @@ class FusedFuseStep:
     step's update only once the next step has begun or :meth:`flush` was called; ``exchange="nccl"`` keeps the separate
     ``all_reduce`` + ``b200rnn_adamw`` launches;
     ``exchange="none"`` runs a single-replica step even when a process group exists.
+
+    The encoders follow torch's fp32 matmul precision (``functional.tf32_enabled``: single-pass TF32 GEMMs and tc8
+    recurrence). A captured step keeps the mode that was active at capture; changing the setting later does not change
+    a replay.
     """
 
     def __init__(self, model, lr: float = 8e-6, betas=(0.9, 0.999), eps: float = 1e-8, bucket=None,

@@ -23,7 +23,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .functional import RNNConfig, prepare_weights, rnn_forward, rnn_forward_fused, rnn_ln_pool_sum
+from .functional import (RNNConfig, prepare_weights, rnn_forward, rnn_forward_fused, rnn_ln_pool_sum,
+                         tf32_enabled)
 
 _TORCH_GRU = nn.GRU
 _TORCH_LSTM = nn.LSTM
@@ -148,9 +149,12 @@ class _B200RNNBase(nn.Module):
         return self._wcache[1]
 
     def _config(self) -> RNNConfig:
+        """The call's configuration, built per forward call: the TF32 mode follows torch's fp32 matmul precision at
+        that moment (``functional.tf32_enabled``), and the backward of the call reuses it."""
         return RNNConfig(mode=self._mode, input_size=self.input_size, hidden_size=self.hidden_size,
                          num_layers=self.num_layers, num_dirs=2 if self.bidirectional else 1,
-                         dropout=self.dropout, training=self.training, batch_first=self.batch_first)
+                         dropout=self.dropout, training=self.training, batch_first=self.batch_first,
+                         tf32=tf32_enabled())
 
     def _run_packed(self, packed):
         """PackedSequence path (ragged DAIC-style sequences): pad, run with per-sequence lengths, re-pack exactly like

@@ -72,6 +72,8 @@ class TrainStep:
     ``loss(output, y) -> scalar`` applied to ``model(x)`` (regression scripts).
     ``step(x, y)`` copies the batch into the graph's static buffers, replays, and returns ``(output, loss)`` tensors
     that are overwritten by the next call.
+    The TF32 mode (torch's fp32 matmul precision, ``functional.tf32_enabled``) is the one active when the graph is
+    captured; changing the setting later does not change a replay (``use_graph=False`` follows it per step).
     """
 
     def __init__(self, model: torch.nn.Module, optimizer: FlatAdamW, x_shape, y_shape=None,
@@ -153,6 +155,7 @@ class FuseFineTuneStep(TrainStep):
     fuse_net_whole.py:421-465 / the all-``requires_grad`` setting of Regression/fuse_net.py:578-583 with the encoders
     inside autograd): BiLSTM + GRU forward and BPTT, attention, both heads, ``MyLoss``, ONE all-reduce over the
     10.46 MB gradient bucket, Adam (``FlatAdamW`` with weight decay 0) - captured as one CUDA graph.
+    Like :class:`TrainStep`, it keeps the TF32 mode that was active at capture.
     """
 
     def __init__(self, model, optimizer: FlatAdamW, batch: int, t_audio: int, t_text: int, criterion=None,

@@ -340,6 +340,7 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
   }
 
   const bool tc = tc_available();
+  const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0;  // single-pass TF32 GEMMs and tc8 recurrence
   int sms = NUM_SMS;
   {
     int dev = 0;
@@ -374,6 +375,7 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     rp.training = save ? 1 : 0;
     rp.lengths = lengths;
     rp.order = order;
+    rp.tf32 = tf32 ? 1 : 0;
     RecFwdLaunch rec;
     rc = plan_rec_fwd(rp, &rec);
     if (rc) return rc;
@@ -438,9 +440,10 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
         g.tc_ws = tc_ws;
         g.tc_ws_bytes = sl.f_tc_bytes;
         g.tc_a_f32 = 1;
-        if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders)
+        g.tc_tf32 = tf32 ? 1 : 0;
+        if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders); TF32 reads only hi
           g.tc_b_hi = WC + wl.hi[l][k];
-          g.tc_b_lo = WC + wl.lo[l][k];
+          g.tc_b_lo = tf32 ? nullptr : WC + wl.lo[l][k];
         }
         if (stream_xproj && gemm_tc_eligible(g, g.tc_ws_bytes)) {
           g.tc_ready = ready;
@@ -573,6 +576,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
   const bool drop = d.training && d.p > 0.f && d.L > 1;
   const uint64_t* hdr = reinterpret_cast<const uint64_t*>(R);  // dropout seed/offset used by the forward
   const int accumulate = (desc->flags & B200RNN_FLAG_ACCUMULATE_GRADS) ? 1 : 0;
+  const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0;  // single-pass TF32 tensor-core GEMMs: hi operands only
   void* gemm_ws = sl.b_gemm_bytes ? (void*)(S + sl.b_gemm) : nullptr;
   int* order = nullptr;  // the forward's slot order, recomputed from the same lengths (nothing of it is in the reserve)
   if (lengths) {
@@ -631,15 +635,18 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
     // with the fused LayerNorm the layer-0 dgrad is d/dLN(x): it goes to scratch and through the LN backward below
     const bool ln_l0 = (l == 0) && fused_ln;
     const bool want_dx = (l > 0) || (dx != nullptr) || (ln_l0 && (dln_gamma || dln_beta));
-    // ---- tensor-core 3xTF32 path for the wgrad / dgrad GEMMs (falls back to the FFMA kernel per GEMM) -------------
+    // ---- tensor-core 3xTF32 (single-pass TF32) path for the wgrad / dgrad GEMMs (falls back to the FFMA kernel per
+    // GEMM) ---------------------------------------------------------------------------------------------------------
     const long long ldk = sl.b_ldk;
     const bool tc_l = tc_available() && (Il % 128 == 0);
     // Operands whose contraction index (t,b) is their ROW index - X_l, dG, h_prev, dn*r - go to the tensor cores as
     // MN-major tiles (gemm_tc.cu): they only need the dense TF32 hi/lo split, no transposing pass (round 1 transposed
     // every one of them: 10 passes, 8 % of the c2 train step).
+    // lo(p): the lo half of a split operand whose hi is at p, or NULL in single-pass TF32 mode (neither written nor read)
+    auto lo = [&](float* hi, size_t n) -> float* { return tf32 ? nullptr : hi + n; };
     float* xS = S + sl.b_tc_xT;  // [TB][Il] hi, then lo
     if (tc_l) {  // X_l, shared by both directions
-      rc = tc_split(in, in_rows, (int)d.TB, Il, xS, xS + d.TB * (size_t)Il, st);
+      rc = tc_split(in, in_rows, (int)d.TB, Il, xS, lo(xS, d.TB * (size_t)Il), st);
       if (rc) return rc;
     }
     (void)ldk;
@@ -657,7 +664,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
       if (tc_l) {
         float* dGs = S + sl.b_tc_dg;   // [TB][GH] hi, then lo: MN-major A of the wgrads AND K-major A of the dgrad
         float* hnS = S + sl.b_tc_hnT;  // [TB][H]   (GRU: dn * r)
-        const TcOperand opX{xS, xS + d.TB * (size_t)Il, (long long)Il, true};
+        const TcOperand opX{xS, lo(xS, d.TB * (size_t)Il), (long long)Il, true};
         // the tensor-core path needs 16-byte aligned outputs: a gradient target that is not 16-byte aligned (a view into a caller's
         // flat bucket behind an odd-sized tensor) takes the FFMA GEMM below instead of failing
         const bool tc_wih = dw_ih && aligned_to(dw_ih, 16), tc_whh = dw_hh && aligned_to(dw_hh, 16) && d.T > 1;
@@ -675,13 +682,13 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
           tc_dx = (reinterpret_cast<uintptr_t>(Cx) % 16 == 0) && cx_rows.s_outer % 4 == 0 && cx_rows.s_inner % 4 == 0;
         }
         if (tc_wih || tc_whh || tc_dx) {
-          rc = tc_split(dG, simple_rows((long long)d.GH), (int)d.TB, (int)d.GH, dGs, dGs + d.TB * d.GH, st);
+          rc = tc_split(dG, simple_rows((long long)d.GH), (int)d.TB, (int)d.GH, dGs, lo(dGs, d.TB * d.GH), st);
           if (rc) return rc;
         }
         if (tc_wih) {  // dW_ih[GH, Il] = sum_tb dG[tb, :]^T X_l[tb, :]
-          const TcOperand opA{dGs, dGs + d.TB * d.GH, (long long)d.GH, true};
+          const TcOperand opA{dGs, lo(dGs, d.TB * d.GH), (long long)d.GH, true};
           rc = tc_gemm_presplit(opA, opX, (int)d.GH, Il, (int)d.TB, dw_ih, simple_rows(Il), nullptr, nullptr, 0,
-                                accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st);
+                                accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
           if (rc) return rc;
           done_dwih = true;
         }
@@ -690,39 +697,41 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
           // offset of B (forward: dG[t] with y[t-1]; reverse: dG[t] with y[t+1]); rows beyond Kp read as zero (TMA)
           float* yS = S + sl.b_tc_yT;  // [TB][H]
           rc = tc_split(bp.y + (long long)k * d.H, tb_rows(bp.y_st, bp.y_sb, d.B), (int)d.TB, d.H, yS,
-                        yS + d.TB * (size_t)d.H, st);
+                        lo(yS, d.TB * (size_t)d.H), st);
           if (rc) return rc;
           const int Kp = (d.T - 1) * d.B;
           const size_t rowA = (k == 0) ? (size_t)d.B : 0, rowY = (k == 0) ? 0 : (size_t)d.B;
-          const TcOperand opY{yS + rowY * d.H, yS + d.TB * (size_t)d.H + rowY * d.H, (long long)d.H, true};
+          const TcOperand opY{yS + rowY * d.H, tf32 ? nullptr : yS + d.TB * (size_t)d.H + rowY * d.H, (long long)d.H, true};
           if (d.mode == B200RNN_LSTM) {
-            const TcOperand opA{dGs + rowA * d.GH, dGs + d.TB * d.GH + rowA * d.GH, (long long)d.GH, true};
+            const TcOperand opA{dGs + rowA * d.GH, tf32 ? nullptr : dGs + d.TB * d.GH + rowA * d.GH, (long long)d.GH, true};
             rc = tc_gemm_presplit(opA, opY, (int)d.GH, d.H, Kp, dw_hh, simple_rows(d.H), nullptr, nullptr, 0,
-                                  accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st);
+                                  accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
             if (rc) return rc;
           } else {
-            rc = tc_split(dHN, simple_rows((long long)d.H), (int)d.TB, d.H, hnS, hnS + d.TB * (size_t)d.H, st);
+            rc = tc_split(dHN, simple_rows((long long)d.H), (int)d.TB, d.H, hnS, lo(hnS, d.TB * (size_t)d.H), st);
             if (rc) return rc;
             // columns [0, 2H) of dG: r and z gates
-            const TcOperand opRZ{dGs + rowA * d.GH, dGs + d.TB * d.GH + rowA * d.GH, (long long)d.GH, true};
+            const TcOperand opRZ{dGs + rowA * d.GH, tf32 ? nullptr : dGs + d.TB * d.GH + rowA * d.GH, (long long)d.GH,
+                                 true};
             rc = tc_gemm_presplit(opRZ, opY, 2 * d.H, d.H, Kp, dw_hh, simple_rows(d.H), nullptr, nullptr, 0,
-                                  accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st);
+                                  accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
             if (rc) return rc;
-            const TcOperand opN{hnS + rowA * d.H, hnS + d.TB * (size_t)d.H + rowA * d.H, (long long)d.H, true};  // n rows: dn * r
+            const TcOperand opN{hnS + rowA * d.H, tf32 ? nullptr : hnS + d.TB * (size_t)d.H + rowA * d.H, (long long)d.H,
+                                true};  // n rows: dn * r
             rc = tc_gemm_presplit(opN, opY, d.H, d.H, Kp, dw_hh + (size_t)2 * d.H * d.H, simple_rows(d.H), nullptr,
-                                  nullptr, 0, accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st);
+                                  nullptr, 0, accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
             if (rc) return rc;
           }
           done_dwhh = true;
         }
         if (tc_dx) {  // dX_l (+)= dG[TB, GH] * W_ih[GH, Il]: A K-major (the same split of dG), B = W_ih as it lies (MN-major)
           float* wS = S + sl.b_tc_wT;   // [GH][Il] hi, then lo
-          rc = tc_split(pp[0], simple_rows(Il), (int)d.GH, Il, wS, wS + d.GH * (size_t)Il, st);
+          rc = tc_split(pp[0], simple_rows(Il), (int)d.GH, Il, wS, lo(wS, d.GH * (size_t)Il), st);
           if (rc) return rc;
-          const TcOperand opA{dGs, dGs + d.TB * d.GH, (long long)d.GH, false};
-          const TcOperand opB{wS, wS + d.GH * (size_t)Il, (long long)Il, true};
+          const TcOperand opA{dGs, lo(dGs, d.TB * d.GH), (long long)d.GH, false};
+          const TcOperand opB{wS, lo(wS, d.GH * (size_t)Il), (long long)Il, true};
           rc = tc_gemm_presplit(opA, opB, (int)d.TB, Il, (int)d.GH, Cx, cx_rows, nullptr, nullptr, 0, (k > 0) ? 1 : 0,
-                                nullptr, 0, st);
+                                nullptr, 0, st, nullptr, 0, tf32);
           if (rc) return rc;
           done_dx = true;
         }

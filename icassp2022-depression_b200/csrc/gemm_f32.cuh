@@ -33,6 +33,9 @@ struct GemmParams {
   // entry.
   int* tc_ready;
   int tc_stream_clusters;
+  // tensor-core path only: single-pass TF32 (one MMA per k-step on operands rounded to TF32; B200RNN_FLAG_TF32)
+  // instead of 3xTF32. Only tc_b_hi of a presplit weight is read, and a per-call split writes hi only.
+  int tc_tf32;
 };
 
 // where launch_gemm_tc puts the split A operand inside its workspace (tc_a_hi: also room for a dense fp32 [M][K] A)
@@ -65,22 +68,25 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
 // Building blocks of the tensor-core path for callers that manage the split operands themselves (backward pass).
 struct TcOperand {
   const float* hi;
-  const float* lo;
+  const float* lo;  // NULL for the operands of a single-pass TF32 GEMM
   long long ld;  // floats between consecutive rows (multiple of 4)
   bool mn = false;  // false: K-major, dense [M or N rows][K]; true: MN-major, dense [K rows][M or N] (no transpose needed
                     // for operands whose contraction index is their row index: dG, X, h_prev in the wgrad GEMMs)
 };
 bool tc_available();
+// lo == NULL: hi only (the operand of a single-pass TF32 GEMM)
 int tc_split(const float* src, const RowMap& rows, int R, int Cc, float* hi, float* lo, cudaStream_t stream);
 // ready: streamed launch of stream_clusters 4-CTA clusters (GemmParams::tc_ready); needs splitk_ws == NULL
+// tf32: single-pass TF32 (GemmParams::tc_tf32), only the hi parts of A and B are read
 int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
                      const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
-                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready = nullptr, int stream_clusters = 0);
+                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready = nullptr, int stream_clusters = 0,
+                     bool tf32 = false);
 // C = A[M,K] * B[N,K]^T + biases, A fp32 read in place through a_rows (tc_a_f32_in_place) and split in registers,
 // B K-major presplit; bit-identical to tc_gemm_presplit on the split of A. ready / stream_clusters as above.
 int tc_gemm_f32a(const float* A, const RowMap& a_rows, const TcOperand& B, int M, int N, int K, float* C,
                  const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
-                 int* ready = nullptr, int stream_clusters = 0);
+                 int* ready = nullptr, int stream_clusters = 0, bool tf32 = false);
 // C(m,n) (+)= sum_z partial[z][m][n] (+ biases), fixed order (deterministic)
 int launch_splitk_reduce(const float* partial, int splitk, int M, int N, float* C, const RowMap& c_rows,
                          const float* bias1, const float* bias2, int bias2_n, int accumulate, cudaStream_t stream);

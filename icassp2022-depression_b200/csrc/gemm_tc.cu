@@ -29,6 +29,11 @@
 //                   from HBM / L2 in fp32 (half the bytes), never written back split, and read from shared memory
 //                   once instead of three times per k-step. setmaxnreg moves registers from the producer (40) to the
 //                   consumers (232) for the two fragment buffers.
+//
+// Single-pass TF32 (TF32 = true, B200RNN_FLAG_TF32: the caller follows torch's fp32 matmul precision "tf32"): one MMA
+// per k-step, hi * hi, with every operand rounded to TF32 (cvt.rna) exactly once. The W_lo / A_lo tiles are neither
+// written nor loaded (a stage carries 32 KB instead of 48 KB) and a k-block is 4 MMAs; the round-to-nearest flush after
+// every k-block, the streamed publication and the epilogue are those of the 3xTF32 kernel.
 #include <cuda.h>  // CUtensorMap types only; the encoder is fetched through cudaGetDriverEntryPoint
 #include <mutex>
 #include <stdlib.h>
@@ -147,6 +152,7 @@ struct TcArgs {
   int* ready;       // streamed (splitk == 1): tiles walked time-major, ready[m] += 1 per finished tile of row tile m
   int a_f32;        // A is fp32 (map_a_hi, 3-D), split in registers by the consumers; W K-major presplit
   int a_inner;      // fp32 A: rows per outer index of the 3-D map (tile m0 sits at (m0 % a_inner, m0 / a_inner))
+  int tf32;         // single-pass TF32: the lo operands are absent (host side only: selects the kernel instantiation)
 };
 
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64K registers of the SM
@@ -189,7 +195,7 @@ __device__ __forceinline__ void load_mn_tile(unsigned char* tile, const float* _
 // the default register budget, so that instantiation has no setmaxnreg; in the K-major one (every operand by TMA, one
 // thread issues) the producer gives registers to the consumers, whose fp32-A path holds the running sum, the wgmma
 // accumulator and two A fragments (4 x 64 registers).
-template <bool MN>
+template <bool MN, bool TF32>
 __global__ void __launch_bounds__(TC_THREADS, 1)
     gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                        const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
@@ -216,11 +222,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     ptx::fence_mbar_init();
     if (!args.a_mn) {
       prefetch_tmap(&map_a_hi);
-      if (!args.a_f32) prefetch_tmap(&map_a_lo);
+      if (!TF32 && !args.a_f32) prefetch_tmap(&map_a_lo);
     }
     if (!args.b_mn) {
       prefetch_tmap(&map_b_hi);
-      prefetch_tmap(&map_b_lo);
+      if (!TF32) prefetch_tmap(&map_b_lo);
     }
   }
   __syncthreads();
@@ -239,10 +245,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             ptx::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
             unsigned char* st = base + s * STAGE_BYTES;
             if (ptx::elect_one_sync()) {  // the A_lo slot stays unused: the consumers split A in registers
-              ptx::mbar_arrive_expect_tx(&full[s], 3u * TILE_BYTES);
+              ptx::mbar_arrive_expect_tx(&full[s], (TF32 ? 2u : 3u) * TILE_BYTES);
               tma_load_3d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0 % args.a_inner, m0 / args.a_inner, &full[s]);
               tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * BK, n0, &full[s]);
-              tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
+              if (!TF32) tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
             }
             __syncwarp();
           }
@@ -250,7 +256,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
     } else {
       const bool a_mn = MN && args.a_mn, b_mn = MN && args.b_mn;
-      const uint32_t tx = (a_mn ? 0u : 2u * TILE_BYTES) + (b_mn ? 0u : 2u * TILE_BYTES);
+      constexpr uint32_t parts = TF32 ? 1u : 2u;  // hi (and lo) tile per operand
+      const uint32_t tx = (a_mn ? 0u : parts * TILE_BYTES) + (b_mn ? 0u : parts * TILE_BYTES);
       int it = 0;  // running k-block counter across items (ring position)
       for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
         const int tile = item % ntiles, ks = item / ntiles;
@@ -268,22 +275,22 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
               mbar_expect_tx(&full[s], tx);
               if (!a_mn) {
                 tma_load_2d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0, &full[s]);
-                tma_load_2d(st + 1 * TILE_BYTES, &map_a_lo, kb * BK, m0, &full[s]);
+                if (!TF32) tma_load_2d(st + 1 * TILE_BYTES, &map_a_lo, kb * BK, m0, &full[s]);
               }
               if (!b_mn) {
                 tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * BK, n0, &full[s]);
-                tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
+                if (!TF32) tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
               }
             }
             __syncwarp();
           }
           if (a_mn) {
             load_mn_tile(st + 0 * TILE_BYTES, args.a_hi, args.lda, args.M, args.K, m0, kb * BK, t);
-            load_mn_tile(st + 1 * TILE_BYTES, args.a_lo, args.lda, args.M, args.K, m0, kb * BK, t);
+            if (!TF32) load_mn_tile(st + 1 * TILE_BYTES, args.a_lo, args.lda, args.M, args.K, m0, kb * BK, t);
           }
           if (b_mn) {
             load_mn_tile(st + 2 * TILE_BYTES, args.b_hi, args.ldb, args.N, args.K, n0, kb * BK, t);
-            load_mn_tile(st + 3 * TILE_BYTES, args.b_lo, args.ldb, args.N, args.K, n0, kb * BK, t);
+            if (!TF32) load_mn_tile(st + 3 * TILE_BYTES, args.b_lo, args.ldb, args.N, args.K, n0, kb * BK, t);
           }
           if (a_mn || b_mn) ptx::fence_proxy_async();  // generic stores -> visible to wgmma (async proxy)
           ptx::mbar_arrive(&full[s]);
@@ -294,7 +301,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     if constexpr (!MN) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
     const int wg = (threadIdx.x >> 7) - 1;   // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
     const int wq = warp & 3;                 // warp within the warpgroup: 16 accumulator rows each
-    // the 12 MMAs of the k-block in ring position `pos` into acc, which restarts from zero; committed as one group
+    // the 12 (TF32: 4) MMAs of the k-block in ring position `pos` into acc, which restarts from zero; committed as one
+    // group
     auto issue = [&](float (&acc)[64], int pos) {
       ptx::mbar_wait(&full[pos % STAGES], (pos / STAGES) & 1);
       const uint32_t st = ptx::smem_u32(base + (pos % STAGES) * STAGE_BYTES);
@@ -306,9 +314,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 #pragma unroll
       for (int k = 0; k < BK / 8; ++k) {
         const uint64_t adv = (uint64_t)(k * (32 >> 4));  // K step of 8 tf32 = 32 bytes inside the swizzle atom
-        wgmma_tf32_m64n128k8(acc, a_lo + adv, b_hi + adv, k != 0);
-        wgmma_tf32_m64n128k8(acc, a_hi + adv, b_lo + adv, 1);
-        wgmma_tf32_m64n128k8(acc, a_hi + adv, b_hi + adv, 1);
+        if constexpr (TF32) {
+          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_hi + adv, k != 0);
+        } else {
+          wgmma_tf32_m64n128k8(acc, a_lo + adv, b_hi + adv, k != 0);
+          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_lo + adv, 1);
+          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_hi + adv, 1);
+        }
       }
       wgmma_commit();
     };
@@ -322,7 +334,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
     };
     // fp32 A: this thread's A fragment of the k-block in ring position `pos` (rows g and g + 8 of the warp's 16, k = t + 4j
     // of the 32; conflict-free under the 128-byte swizzle since row & 7 == g), split as split_tf32_kernel does:
-    // fa[8 s + i] = hi of a_i at k-step s, fa[8 s + 4 + i] = lo
+    // fa[8 s + i] = hi of a_i at k-step s, fa[8 s + 4 + i] = lo; TF32: fa[4 s + i] = hi, the rest unused
     const int g = lane >> 2, tq = lane & 3;
     const uint32_t a_row = (uint32_t)(wg * 64 + wq * 16 + g) * 128u + tq * 4u;
     auto load_a = [&](uint32_t (&fa)[32], int pos) {
@@ -335,12 +347,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           const float x = *reinterpret_cast<const float*>(at + (i & 1) * 1024 + ((((2 * s4 + (i >> 1)) ^ g)) << 4));
           uint32_t h;
           asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
-          fa[8 * s4 + i] = h;
-          fa[8 * s4 + 4 + i] = __float_as_uint(x - __uint_as_float(h));
+          if constexpr (TF32) {
+            fa[4 * s4 + i] = h;
+          } else {
+            fa[8 * s4 + i] = h;
+            fa[8 * s4 + 4 + i] = __float_as_uint(x - __uint_as_float(h));
+          }
         }
       }
     };
-    // the 12 MMAs of a k-block with A from registers: same products, same order as `issue`
+    // the 12 (TF32: 4) MMAs of a k-block with A from registers: same products, same order as `issue`
     auto issue_ra = [&](float (&acc)[64], const uint32_t (&fa)[32], int pos) {
       const uint32_t st = ptx::smem_u32(base + (pos % STAGES) * STAGE_BYTES);
       const uint64_t b_hi = make_kmajor_sw128_desc(st + 2 * TILE_BYTES);
@@ -349,9 +365,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 #pragma unroll
       for (int k = 0; k < BK / 8; ++k) {
         const uint64_t adv = (uint64_t)(k * (32 >> 4));
-        wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k + 4], b_hi + adv, k != 0);
-        wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k], b_lo + adv, 1);
-        wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k], b_hi + adv, 1);
+        if constexpr (TF32) {
+          wgmma_tf32_m64n128k8_ra(acc, &fa[4 * k], b_hi + adv, k != 0);
+        } else {
+          wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k + 4], b_hi + adv, k != 0);
+          wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k], b_lo + adv, 1);
+          wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k], b_hi + adv, 1);
+        }
       }
       wgmma_commit();
     };
@@ -450,7 +470,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 }
 
 // x = hi + lo with hi = round-to-nearest TF32 (kept in a 32-bit container), lo = x - hi (exact in fp32).
-// Reads rows through a RowMap (batch_first / permuted inputs), writes two dense [M,K] matrices.
+// Reads rows through a RowMap (batch_first / permuted inputs), writes two dense [M,K] matrices (lo == NULL: hi only,
+// the operand of a single-pass TF32 GEMM).
 __global__ void split_tf32_kernel(const float* __restrict__ src, RowMap rows, int M, int K, float* __restrict__ hi,
                                   float* __restrict__ lo, int vec_ok) {
   const size_t nvec = (size_t)M * (K / 4);
@@ -471,7 +492,7 @@ __global__ void split_tf32_kernel(const float* __restrict__ src, RowMap rows, in
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(x.z)); h.z = __uint_as_float(t); l.z = x.z - h.z;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(x.w)); h.w = __uint_as_float(t); l.w = x.w - h.w;
     *reinterpret_cast<float4*>(hi + (size_t)m * K + k) = h;
-    *reinterpret_cast<float4*>(lo + (size_t)m * K + k) = l;
+    if (lo) *reinterpret_cast<float4*>(lo + (size_t)m * K + k) = l;
   }
 }
 
@@ -866,14 +887,18 @@ int launch_tc(const CUtensorMap (&m)[4], const TcArgs& a, int stream_clusters, c
     const int dev = current_device();
     std::lock_guard<std::mutex> lk(mu);
     if (!attr_done[dev]) {
-      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
-      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       attr_done[dev] = true;
     }
   }
   const int sms = num_sms();
   const int nitems = a.tiles_m * a.tiles_n * a.splitk;
-  auto kernel = (a.a_mn || a.b_mn) ? gemm_tf32x3_kernel<true> : gemm_tf32x3_kernel<false>;
+  const bool mn = a.a_mn || a.b_mn;
+  auto kernel = a.tf32 ? (mn ? gemm_tf32x3_kernel<true, true> : gemm_tf32x3_kernel<false, true>)
+                       : (mn ? gemm_tf32x3_kernel<true, false> : gemm_tf32x3_kernel<false, false>);
   dim3 grid(nitems < sms ? nitems : sms, 1, 1);
   if (!a.ready) {
     ProfScope prof(PROF_GEMM, stream);
@@ -914,13 +939,13 @@ int launch_tc(const CUtensorMap (&m)[4], const TcArgs& a, int stream_clusters, c
 // C[M,N] (+)= A[M,K] * B[N,K]^T (+ biases), operands already split into hi/lo matrices (K- or MN-major).
 int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
                      const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
-                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready, int stream_clusters) {
+                     size_t splitk_ws_bytes, cudaStream_t stream, int* ready, int stream_clusters, bool tf32) {
   int rc = check_tc_shape(M, N, K, C, c_rows, ready, splitk_ws != nullptr, stream_clusters);
   if (rc) return rc;
   // MN-major operands are read by the kernel's own loads: their tensor maps stay zero and unused
   CUtensorMap m[4] = {};
-  const bool ok_a = A.mn || (make_map(&m[0], A.hi, M, K, A.ld) && make_map(&m[1], A.lo, M, K, A.ld));
-  const bool ok_b = B.mn || (make_map(&m[2], B.hi, N, K, B.ld) && make_map(&m[3], B.lo, N, K, B.ld));
+  const bool ok_a = A.mn || (make_map(&m[0], A.hi, M, K, A.ld) && (tf32 || make_map(&m[1], A.lo, M, K, A.ld)));
+  const bool ok_b = B.mn || (make_map(&m[2], B.hi, N, K, B.ld) && (tf32 || make_map(&m[3], B.lo, N, K, B.ld)));
   if (!ok_a || !ok_b) {
     set_error("tc_gemm: cuTensorMapEncodeTiled failed (operands must be 16-byte aligned, ld %% 4 == 0)");
     return B200RNN_ERR_CUDA;
@@ -930,6 +955,7 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
   a.b_mn = B.mn ? 1 : 0;
   a.a_hi = A.hi; a.a_lo = A.lo; a.lda = A.ld;
   a.b_hi = B.hi; a.b_lo = B.lo; a.ldb = B.ld;
+  a.tf32 = tf32 ? 1 : 0;
   const int ntiles = a.tiles_m * a.tiles_n;
   const int nkb = (K + BK - 1) / BK;
   const int sms = num_sms();
@@ -956,7 +982,7 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
 // presplit. Same operands, same MMAs, same sums as tc_gemm_presplit on split(A), so C is bit-identical.
 int tc_gemm_f32a(const float* A, const RowMap& a_rows, const TcOperand& B, int M, int N, int K, float* C,
                  const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
-                 int* ready, int stream_clusters) {
+                 int* ready, int stream_clusters, bool tf32) {
   int rc = check_tc_shape(M, N, K, C, c_rows, ready, false, stream_clusters);
   if (rc) return rc;
   if (B.mn || K % BK != 0) {
@@ -970,13 +996,14 @@ int tc_gemm_f32a(const float* A, const RowMap& a_rows, const TcOperand& B, int M
               "multiple of it)");
     return B200RNN_ERR_UNSUPPORTED;
   }
-  if (!make_map(&m[2], B.hi, N, K, B.ld) || !make_map(&m[3], B.lo, N, K, B.ld)) {
+  if (!make_map(&m[2], B.hi, N, K, B.ld) || (!tf32 && !make_map(&m[3], B.lo, N, K, B.ld))) {
     set_error("tc_gemm: cuTensorMapEncodeTiled failed (operands must be 16-byte aligned, ld %% 4 == 0)");
     return B200RNN_ERR_CUDA;
   }
   TcArgs a = tc_args(M, N, K, C, c_rows, bias1, bias2, bias2_n, 0, ready);
   a.a_f32 = 1;
   a.a_inner = inner;
+  a.tf32 = tf32 ? 1 : 0;
   return launch_tc(m, a, stream_clusters, stream);
 }
 
@@ -985,6 +1012,7 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
     set_error("gemm_tc: problem not eligible for the tensor-core path");
     return B200RNN_ERR_UNSUPPORTED;
   }
+  const bool tf32 = p.tc_tf32 != 0;
   float* a_hi = tc_a_hi(ws);
   float* a_lo = tc_a_lo(ws, p.M, p.K);
   const float* b_hi = p.tc_b_hi;
@@ -992,12 +1020,12 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
   int rc = B200RNN_OK;
   // a_kcontig: A is [M rows][K]; else A is [K rows][M] (MN-major): the split copy keeps the source's orientation
   if (!p.tc_a_f32)
-    rc = p.a_kcontig ? tc_split(p.A, p.a_rows, p.M, p.K, a_hi, a_lo, stream)
-                     : tc_split(p.A, p.a_rows, p.K, p.M, a_hi, a_lo, stream);
+    rc = p.a_kcontig ? tc_split(p.A, p.a_rows, p.M, p.K, a_hi, tf32 ? nullptr : a_lo, stream)
+                     : tc_split(p.A, p.a_rows, p.K, p.M, a_hi, tf32 ? nullptr : a_lo, stream);
   if (rc) return rc;
-  if (!b_hi || !b_lo) {
+  if (!b_hi || (!b_lo && !tf32)) {  // single-pass TF32 reads and writes only hi
     float* w_hi = a_lo + (size_t)p.M * p.K;
-    float* w_lo = w_hi + (size_t)p.N * p.K;
+    float* w_lo = tf32 ? nullptr : w_hi + (size_t)p.N * p.K;
     rc = p.b_kcontig ? tc_split(p.B, p.b_rows, p.N, p.K, w_hi, w_lo, stream)
                      : tc_split(p.B, p.b_rows, p.K, p.N, w_hi, w_lo, stream);
     if (rc) return rc;
@@ -1007,10 +1035,10 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
   TcOperand B{b_hi, b_lo, p.b_kcontig ? p.K : p.N, !p.b_kcontig};
   if (p.tc_a_f32)
     return tc_gemm_f32a(p.A, p.a_rows, B, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, stream,
-                        p.tc_ready, p.tc_stream_clusters);
+                        p.tc_ready, p.tc_stream_clusters, tf32);
   TcOperand A{a_hi, a_lo, p.a_kcontig ? p.K : p.M, !p.a_kcontig};
   return tc_gemm_presplit(A, B, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, 0, nullptr, 0, stream,
-                          p.tc_ready, p.tc_stream_clusters);
+                          p.tc_ready, p.tc_stream_clusters, tf32);
 }
 
 }  // namespace b200rnn

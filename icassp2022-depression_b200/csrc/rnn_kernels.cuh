@@ -28,6 +28,8 @@ struct RecFwdParams {
   // gates are complete at launch.
   const int* ready;
   int tiles_n;
+  int tf32;                  // single-pass TF32 contraction in the tensor-core config tc8 (B200RNN_FLAG_TF32); every
+                             // other config is fp32 FFMA and ignores it
 };
 
 // A recurrence launch chosen for a shape, before anything is enqueued: `nclusters` clusters of C CTAs, of which

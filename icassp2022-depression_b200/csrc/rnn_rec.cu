@@ -453,6 +453,12 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 //   * per tile, hi*hi and the two cross terms (lo*hi + hi*lo) have their own accumulators, restarted for each source
 //     slice (at most 8 MMAs) and added round-to-nearest into the fp32 sum: six independent MMA chains per warp, and the
 //     truncating tensor-core accumulation never runs longer than in gemm_tc.cu (12 MMAs).
+// Single-pass TF32 (TF32 = true, B200RNN_FLAG_TF32; rec_fwd_tf32_kernel): W_hh is rounded to TF32 (cvt.rna) once as it
+// is staged, and the lane that produces h_t rounds the copy it hands to the contraction (its own buffer and the
+// st.async to the peers) while its FwdCell keeps the fp32 h for the update. The step loop then converts nothing and
+// runs one mma.sync per (gate tile, k-step): 384 per CTA and step instead of 1,152, one accumulator per tile and source
+// slice (4 MMAs). Round-to-nearest, not the truncation of split_tf32: without a lo term a truncated operand would bias
+// every product the same way.
 struct TcFwdCfg {
   static constexpr int H = 256, C = 4, BS = 8, G = 3, GH = G * H;
   static constexpr int HS = H / C;        // units per CTA
@@ -472,8 +478,14 @@ __device__ __forceinline__ int tc_state_index(int k, int b) {
   return ((k >> 3) * 8 + b) * 8 + (k & 3) * 2 + ((k >> 2) & 1);
 }
 
-template <bool VL>
-__global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFwdParams p, const int nslices) {
+__device__ __forceinline__ float round_tf32(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
+
+template <bool VL, bool TF32>
+__device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int nslices) {
   using Cfg = TcFwdCfg;
   constexpr int H = Cfg::H, C = Cfg::C, BS = Cfg::BS, G = Cfg::G, HS = Cfg::HS, NUG = Cfg::NUG, NW = Cfg::NW,
                 NT = Cfg::NT, KS = Cfg::KS, KSC = Cfg::KSC;
@@ -510,10 +522,10 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
     const float4 v = __ldg(reinterpret_cast<const float4*>(w_hh + ((size_t)g * H + j0 + u) * H + k0));
     float* dst = reinterpret_cast<float*>(W_f + (((u / 16) * G + g) * KS + k0 / 8) * 32 + (u % 8) * 4) +
                  (u % 16) / 8 + 2 * ((k0 / 4) & 1);
-    dst[0] = v.x;
-    dst[4] = v.y;
-    dst[8] = v.z;
-    dst[12] = v.w;
+    dst[0] = TF32 ? round_tf32(v.x) : v.x;
+    dst[4] = TF32 ? round_tf32(v.y) : v.y;
+    dst[8] = TF32 ? round_tf32(v.z) : v.z;
+    dst[12] = TF32 ? round_tf32(v.w) : v.w;
   }
   for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
   __syncthreads();
@@ -550,7 +562,7 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
     for (int c = 0; c < C; ++c) {
       const int src = (c + (int)rank) % C;
       if (step > 0) ptx::mbar_wait(&bars[cur * C + src], par);
-      float d[G][2][4];  // [gate tile][lo*hi + hi*lo, hi*hi]
+      float d[G][2][4];  // [gate tile][lo*hi + hi*lo, hi*hi]; TF32: [gate tile][-, the single product]
 #pragma unroll
       for (int g = 0; g < G; ++g)
 #pragma unroll
@@ -561,26 +573,37 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
       for (int kk = 0; kk < KSC / 2; ++kk) {
         const int ks = src * KSC + kh * (KSC / 2) + kk;
         const float2 hv = h_cur[ks * 32];
-        uint32_t bh[2], bl[2];
-        ptx::split_tf32(hv.x, bh[0], bl[0]);
-        ptx::split_tf32(hv.y, bh[1], bl[1]);
+        if constexpr (TF32) {  // both operands are TF32 already
+          const uint32_t b[2] = {__float_as_uint(hv.x), __float_as_uint(hv.y)};
 #pragma unroll
-        for (int g = 0; g < G; ++g) {
-          const float4 wv = W_w[(g * KS + ks) * 32];
-          uint32_t ah[4], al[4];
-          ptx::split_tf32(wv.x, ah[0], al[0]);
-          ptx::split_tf32(wv.y, ah[1], al[1]);
-          ptx::split_tf32(wv.z, ah[2], al[2]);
-          ptx::split_tf32(wv.w, ah[3], al[3]);
-          ptx::mma_tf32_m16n8k8(d[g][0], al, bh);
-          ptx::mma_tf32_m16n8k8(d[g][0], ah, bl);
-          ptx::mma_tf32_m16n8k8(d[g][1], ah, bh);
+          for (int g = 0; g < G; ++g) {
+            const float4 wv = W_w[(g * KS + ks) * 32];
+            const uint32_t a[4] = {__float_as_uint(wv.x), __float_as_uint(wv.y), __float_as_uint(wv.z),
+                                   __float_as_uint(wv.w)};
+            ptx::mma_tf32_m16n8k8(d[g][1], a, b);
+          }
+        } else {
+          uint32_t bh[2], bl[2];
+          ptx::split_tf32(hv.x, bh[0], bl[0]);
+          ptx::split_tf32(hv.y, bh[1], bl[1]);
+#pragma unroll
+          for (int g = 0; g < G; ++g) {
+            const float4 wv = W_w[(g * KS + ks) * 32];
+            uint32_t ah[4], al[4];
+            ptx::split_tf32(wv.x, ah[0], al[0]);
+            ptx::split_tf32(wv.y, ah[1], al[1]);
+            ptx::split_tf32(wv.z, ah[2], al[2]);
+            ptx::split_tf32(wv.w, ah[3], al[3]);
+            ptx::mma_tf32_m16n8k8(d[g][0], al, bh);
+            ptx::mma_tf32_m16n8k8(d[g][0], ah, bl);
+            ptx::mma_tf32_m16n8k8(d[g][1], ah, bh);
+          }
         }
       }
 #pragma unroll
       for (int g = 0; g < G; ++g)
 #pragma unroll
-        for (int i = 0; i < 4; ++i) acc[g][i] += d[g][0][i] + d[g][1][i];
+        for (int i = 0; i < 4; ++i) acc[g][i] += TF32 ? d[g][1][i] : d[g][0][i] + d[g][1][i];
       if (c == 0 && step > 0) {  // the previous step's stores
 #pragma unroll
         for (int jb = 0; jb < 2; ++jb) cell[jb].flush(p, dir, dir ? (T - step) : (step - 1));
@@ -615,7 +638,7 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
       // with st.async (ordering of the local path: allgather_units)
       float* h_nxt = h_s + nxt * BS * H;
 #pragma unroll
-      for (int jb = 0; jb < 2; ++jb) h_nxt[tc_state_index(ju, 2 * ft + jb)] = hnew[jb];
+      for (int jb = 0; jb < 2; ++jb) h_nxt[tc_state_index(ju, 2 * ft + jb)] = TF32 ? round_tf32(hnew[jb]) : hnew[jb];
       __syncwarp();
       if (lane < 16) {
         float* mine = h_nxt + (j0 + u0) / 8 * 64 + lane * 4;
@@ -647,6 +670,16 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFw
     for (int jb = 0; jb < 2; ++jb) cell[jb].skip_tail(p, dir, T);
   }
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
+}
+
+// 3xTF32 (the default) and single-pass TF32 instantiations, fixed-length and ragged
+template <bool VL>
+__global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFwdParams p, const int nslices) {
+  rec_fwd_tc_body<VL, false>(p, nslices);
+}
+template <bool VL>
+__global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tf32_kernel(const RecFwdParams p, const int nslices) {
+  rec_fwd_tc_body<VL, true>(p, nslices);
 }
 
 // =================================================================================================
@@ -1001,10 +1034,11 @@ bool pick_fwd(const RecFwdParams& p, bool force, RecFwdLaunch* L, int* rc) {
 int pick_fwd_tc(const RecFwdParams& p, RecFwdLaunch* L) {
   using Cfg = TcFwdCfg;
   static_assert(Cfg::SMEM <= MAX_SMEM, "forward config does not fit an SM");
-  auto k = p.lengths ? rec_fwd_tc_kernel<true> : rec_fwd_tc_kernel<false>;
+  auto k = p.tf32 ? (p.lengths ? rec_fwd_tf32_kernel<true> : rec_fwd_tf32_kernel<false>)
+                  : (p.lengths ? rec_fwd_tc_kernel<true> : rec_fwd_tc_kernel<false>);
   int rc = B200RNN_OK;
-  pick_clustered(k, p, Cfg::C, Cfg::BS, Cfg::NT, Cfg::SMEM, true, L, &rc, "fwd cfg tc8 C=%d BS=%d mma.sync 3xTF32",
-                 Cfg::C, Cfg::BS);
+  pick_clustered(k, p, Cfg::C, Cfg::BS, Cfg::NT, Cfg::SMEM, true, L, &rc, "fwd cfg tc8 C=%d BS=%d mma.sync %s",
+                 Cfg::C, Cfg::BS, p.tf32 ? "TF32" : "3xTF32");
   return rc;
 }
 

@@ -55,6 +55,13 @@ enum {
 #define B200RNN_FLAG_FUSED_LN 4u          /* the LayerNorm prologue is part of the differentiated graph: the forward keeps
                                              LN(x) in `reserve`, b200rnn_backward_fused runs the LayerNorm backward.
                                              Must be set identically for workspace_bytes / forward_fused / backward_fused */
+#define B200RNN_FLAG_TF32 8u              /* single-pass TF32 instead of 3xTF32 on the tensor cores: the input-projection,
+                                             weight-gradient and input-gradient GEMMs and the GRU-256 tc8 recurrence
+                                             round their operands to TF32 (round to nearest, ties away from zero) and
+                                             issue one MMA per product; every other kernel stays fp32. Honoured by
+                                             forward / forward_fused / backward / backward_fused (set it identically for
+                                             a forward and its backward); workspace_bytes and prepare_weights accept it.
+                                             b200rnn_gemm_f32 is always 3xTF32. */
 
 /*
  * Problem descriptor. Mirrors the constructor arguments of torch.nn.GRU / torch.nn.LSTM
