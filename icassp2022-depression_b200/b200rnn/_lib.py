@@ -18,7 +18,7 @@ FLAG_ACCUMULATE_GRADS = 1
 FLAG_SAVE_FOR_BACKWARD = 2
 FLAG_FUSED_LN = 4
 FLAG_TF32 = 8
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)
 SYMBOLS = (
@@ -29,8 +29,10 @@ SYMBOLS = (
     "b200rnn_workspace_bytes",
     "b200rnn_forward",
     "b200rnn_forward_fused",
+    "b200rnn_forward_hx",
     "b200rnn_backward",
     "b200rnn_backward_fused",
+    "b200rnn_backward_hx",
     "b200rnn_wcache_bytes",
     "b200rnn_prepare_weights",
     "b200rnn_gemm_f32",
@@ -111,6 +113,11 @@ class B200RNNError(RuntimeError):
     pass
 
 
+class NoCPUPathError(B200RNNError, NotImplementedError):
+    """A host tensor reached a CUDA-only entry point. Also a ``NotImplementedError``, which is how torch reports an
+    operator with no kernel for a tensor's backend."""
+
+
 _lib = None
 
 
@@ -152,6 +159,18 @@ def load() -> ctypes.CDLL:
     lib.b200rnn_forward_fused.restype = c_int
     lib.b200rnn_forward_fused.argtypes = lib.b200rnn_forward.argtypes[:-1] + [c_void_p, c_void_p, c_float, c_void_p,
                                                                               c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.b200rnn_forward_hx.restype = c_int
+    lib.b200rnn_forward_hx.argtypes = [
+        POINTER(Desc), c_void_p, c_int64, c_int64,  # desc, x, strides
+        POINTER(c_void_p),                           # params
+        c_void_p, c_int64, c_int64,                  # y, strides
+        c_void_p, c_void_p,                          # h_0, c_0
+        c_void_p, c_void_p,                          # h_n, c_n
+        c_void_p, c_void_p,                          # reserve, scratch
+        c_uint64, c_uint64, c_void_p,                # seed, offset, rng_state
+        c_void_p,                                    # lengths
+        c_void_p,                                    # stream
+    ]
     lib.b200rnn_wcache_bytes.restype = c_int
     lib.b200rnn_wcache_bytes.argtypes = [POINTER(Desc), POINTER(c_size_t)]
     lib.b200rnn_prepare_weights.restype = c_int
@@ -163,6 +182,20 @@ def load() -> ctypes.CDLL:
         c_void_p, c_int64, c_int64,                  # y
         c_void_p, c_int64, c_int64,                  # dy
         c_void_p, c_void_p,                          # dh_n, dc_n
+        c_void_p, c_void_p,                          # reserve, scratch
+        c_void_p, c_int64, c_int64,                  # dx
+        POINTER(c_void_p),                           # dparams
+        c_void_p,                                    # lengths
+        c_void_p,                                    # stream
+    ]
+    lib.b200rnn_backward_hx.restype = c_int
+    lib.b200rnn_backward_hx.argtypes = [
+        POINTER(Desc), c_void_p, c_int64, c_int64,   # desc, x, strides
+        POINTER(c_void_p),                           # params
+        c_void_p, c_int64, c_int64,                  # y
+        c_void_p, c_int64, c_int64,                  # dy
+        c_void_p, c_void_p,                          # dh_n, dc_n
+        c_void_p, c_void_p, c_void_p, c_void_p,      # h_0, c_0, dh_0, dc_0
         c_void_p, c_void_p,                          # reserve, scratch
         c_void_p, c_int64, c_int64,                  # dx
         POINTER(c_void_p),                           # dparams

@@ -43,7 +43,7 @@ def tf32_enabled() -> bool:
 
 def _require_cuda_f32(t: torch.Tensor, name: str) -> None:
     if not t.is_cuda:
-        raise _lib.B200RNNError(
+        raise _lib.NoCPUPathError(
             f"b200rnn: {name} is on {t.device}; this library runs on CUDA (sm_90a) only and has no CPU path"
         )
     if t.dtype != torch.float32:
@@ -85,11 +85,16 @@ def _on(device):
 
 
 class _RNNFunction(torch.autograd.Function):
-    """y, h_n[, c_n] = RNN(x, weights); x is the logical time-major view [T,B,I]."""
+    """y, h_n[, c_n] = RNN(x, weights, h_0[, c_0]); x is the logical time-major view [T,B,I], h_0 / c_0 are None
+    (zeros) or contiguous [L*D,B,H]."""
+
+    # position of the first weight among forward()'s inputs (after ctx)
+    _W0 = 8
 
     @staticmethod
     def forward(ctx, x_tm: torch.Tensor, cfg: RNNConfig, rng_state: Optional[torch.Tensor], grad_sink,
-                lengths: Optional[torch.Tensor], save: bool, *weights: torch.Tensor):
+                lengths: Optional[torch.Tensor], save: bool, h_0: Optional[torch.Tensor], c_0: Optional[torch.Tensor],
+                *weights: torch.Tensor):
         lib = _lib.load()
         T, B, _ = x_tm.shape
         H, L, D = cfg.hidden_size, cfg.num_layers, cfg.num_dirs
@@ -110,25 +115,34 @@ class _RNNFunction(torch.autograd.Function):
         h_n = torch.empty(L * D, B, H, dtype=torch.float32, device=dev)
         c_n = torch.empty(L * D, B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
         params = _lib.ptr_array([w.data_ptr() for w in weights])
+        rng_ptr = rng_state.data_ptr() if rng_state is not None else None
+        len_ptr = lengths.data_ptr() if lengths is not None else None
+        c_n_ptr = c_n.data_ptr() if c_n is not None else None
         if B > 0 and T > 0:
             with _on(dev):
-                rc = lib.b200rnn_forward_fused(
-                    ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
-                    y.data_ptr(), ys_t, ys_b, h_n.data_ptr(), c_n.data_ptr() if c_n is not None else None,
-                    reserve.data_ptr() if save else None, scratch.data_ptr(),
-                    0, 0, rng_state.data_ptr() if rng_state is not None else None, None, None, 0.0, None,
-                    lengths.data_ptr() if lengths is not None else None, None, None, _stream_ptr(dev))
+                if h_0 is None:
+                    rc = lib.b200rnn_forward_fused(
+                        ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+                        y.data_ptr(), ys_t, ys_b, h_n.data_ptr(), c_n_ptr,
+                        reserve.data_ptr() if save else None, scratch.data_ptr(),
+                        0, 0, rng_ptr, None, None, 0.0, None, len_ptr, None, None, _stream_ptr(dev))
+                else:
+                    rc = lib.b200rnn_forward_hx(
+                        ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+                        y.data_ptr(), ys_t, ys_b, h_0.data_ptr(), c_0.data_ptr() if c_0 is not None else None,
+                        h_n.data_ptr(), c_n_ptr, reserve.data_ptr() if save else None, scratch.data_ptr(),
+                        0, 0, rng_ptr, len_ptr, _stream_ptr(dev))
             _lib.check(rc, "b200rnn_forward")
-        else:
-            h_n.zero_()
+        else:   # no step: the final state is the initial one
+            h_n.copy_(h_0) if h_0 is not None else h_n.zero_()
             if c_n is not None:
-                c_n.zero_()
+                c_n.copy_(c_0) if c_0 is not None else c_n.zero_()
         if save:
             ctx.cfg = cfg
             ctx.grad_sink = grad_sink
             ctx.ys = (ys_t, ys_b)
             ctx.lengths = lengths
-            ctx.save_for_backward(x_tm, y, reserve, *weights)
+            ctx.save_for_backward(x_tm, y, reserve, h_0, c_0, *weights)
         if c_n is None:
             return y, h_n
         return y, h_n, c_n
@@ -137,11 +151,15 @@ class _RNNFunction(torch.autograd.Function):
     def backward(ctx, dy, dh_n, dc_n=None):
         lib = _lib.load()
         cfg: RNNConfig = ctx.cfg
-        x_tm, y, reserve, *weights = ctx.saved_tensors
+        x_tm, y, reserve, h_0, c_0, *weights = ctx.saved_tensors
         T, B, _ = x_tm.shape
         H, L, D = cfg.hidden_size, cfg.num_layers, cfg.num_dirs
         dev = x_tm.device
         ys_t, ys_b = ctx.ys
+        w0 = _RNNFunction._W0
+        # gradients w.r.t. the initial state only when autograd asks: dh_0 costs the last step's contraction
+        dh_0 = torch.empty_like(h_0) if h_0 is not None and ctx.needs_input_grad[w0 - 2] else None
+        dc_0 = torch.empty_like(c_0) if c_0 is not None and ctx.needs_input_grad[w0 - 1] else None
 
         if dy is None:
             dy = torch.zeros_like(y)
@@ -164,7 +182,7 @@ class _RNNFunction(torch.autograd.Function):
         # weight gradients: either straight into caller-provided views (a flat all-reduce bucket) or into one
         # fresh flat buffer that is returned to autograd as views
         sink = ctx.grad_sink
-        w_needed = [ctx.needs_input_grad[6 + i] for i in range(len(weights))]
+        w_needed = [ctx.needs_input_grad[w0 + i] for i in range(len(weights))]
         grads_out: list = [None] * len(weights)
         accumulate = False
         if sink is not None:
@@ -189,23 +207,27 @@ class _RNNFunction(torch.autograd.Function):
         scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
         params = _lib.ptr_array([w.data_ptr() for w in weights])
         dparams = _lib.ptr_array(dptrs)
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
         if B > 0 and T > 0:
             with _on(dev):
-                rc = lib.b200rnn_backward(
-                    ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
-                    y.data_ptr(), ys_t, ys_b, dy.data_ptr(), dys_t, dys_b,
-                    dh_n.data_ptr() if dh_n is not None else None,
-                    dc_n.data_ptr() if dc_n is not None else None,
-                    reserve.data_ptr(), scratch.data_ptr(),
-                    dx.data_ptr() if dx is not None else None,
-                    dx.stride(0) if dx is not None else 0, dx.stride(1) if dx is not None else 0,
-                    dparams, ctx.lengths.data_ptr() if ctx.lengths is not None else None, _stream_ptr(dev))
+                head = (ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+                        y.data_ptr(), ys_t, ys_b, dy.data_ptr(), dys_t, dys_b, ptr(dh_n), ptr(dc_n))
+                tail = (reserve.data_ptr(), scratch.data_ptr(), ptr(dx),
+                        dx.stride(0) if dx is not None else 0, dx.stride(1) if dx is not None else 0,
+                        dparams, ptr(ctx.lengths), _stream_ptr(dev))
+                if h_0 is None:
+                    rc = lib.b200rnn_backward(*head, *tail)
+                else:
+                    rc = lib.b200rnn_backward_hx(*head, ptr(h_0), ptr(c_0), ptr(dh_0), ptr(dc_0), *tail)
             _lib.check(rc, "b200rnn_backward")
-        else:
+        else:   # no step: parameters get nothing, the state gradients pass through
             for g in grads_out:
                 if g is not None:
                     g.zero_()
-        return (dx, None, None, None, None, None, *grads_out)
+            for d0, dn in ((dh_0, dh_n), (dc_0, dc_n)):
+                if d0 is not None:
+                    d0.copy_(dn) if dn is not None else d0.zero_()
+        return (dx, None, None, None, None, None, dh_0, dc_0, *grads_out)
 
 
 class _LNRNNPoolFunction(torch.autograd.Function):
@@ -316,12 +338,46 @@ def rnn_ln_pool_sum(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNCo
     return _LNRNNPoolFunction.apply(x_tm, cfg, rng_state, grad_sink, ln_weight, ln_bias, ln_eps, *weights)
 
 
+def _initial_state(hx, cfg: RNNConfig, x: torch.Tensor):
+    """(h_0, c_0) of ``hx`` - None, ``h_0`` (GRU) or ``(h_0, c_0)`` (LSTM) - checked as torch checks them (shapes:
+    ``RNNBase.check_forward_args``, with its messages; then device and dtype against the input), contiguous. c_0 is
+    None for the GRU; both are None without ``hx``."""
+    if hx is None:
+        return None, None
+    lstm = cfg.mode == _lib.LSTM
+    states = tuple(hx) if lstm else (hx,)
+    if len(states) != (2 if lstm else 1):
+        raise RuntimeError(f"b200rnn: LSTM hx must be a pair (h_0, c_0), got {len(states)} tensors")
+    batch = x.size(0 if cfg.batch_first else 1) if x.dim() == 3 else None
+    expected = (cfg.num_layers * cfg.num_dirs, batch, cfg.hidden_size)
+    msgs = (("Expected hidden[0] size {}, got {}", "Expected hidden[1] size {}, got {}") if lstm
+            else ("Expected hidden size {}, got {}",))
+    for s, msg in zip(states, msgs):
+        if s.size() != expected:
+            raise RuntimeError(msg.format(expected, list(s.size())))
+    for s in states:
+        if s.device != x.device:
+            raise RuntimeError("Input and hidden tensors are not at the same device, found input tensor at "
+                               f"{x.device} and hidden tensor at {s.device}")
+        if s.dtype != x.dtype:
+            raise RuntimeError("Input and hidden tensors are not the same dtype, found input tensor with "
+                               f"{x.dtype} and hidden tensor with {s.dtype}")
+    states = tuple(s.contiguous() for s in states)
+    return states[0], (states[1] if lstm else None)
+
+
 def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig,
-                rng_state: Optional[torch.Tensor] = None, grad_sink=None, lengths: Optional[torch.Tensor] = None):
+                rng_state: Optional[torch.Tensor] = None, grad_sink=None, lengths: Optional[torch.Tensor] = None,
+                hx=None):
     """Run the multi-layer GRU/LSTM. ``x`` is [T,B,I] (or [B,T,I] if ``cfg.batch_first``), any strides.
+
+    ``hx`` is the initial state as torch takes it: None (zeros), ``h_0`` (GRU) or ``(h_0, c_0)`` (LSTM), each
+    [L*D, B, H] with the rows in ``x``'s batch order (also with ``lengths``). It is differentiable: ``dh_0`` / ``dc_0``
+    are computed only when autograd asks for them.
 
     Returns ``(y, h_n)`` for GRU and ``(y, h_n, c_n)`` for LSTM, laid out like torch.nn.GRU/LSTM outputs.
     """
+    h_0, c_0 = _initial_state(hx, cfg, x)
     _require_cuda_f32(x, "input")
     if x.dim() != 3:
         raise NotImplementedError("b200rnn: only batched 3-D input is supported (the reference never uses 2-D)")
@@ -338,8 +394,9 @@ def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig
     for i, w in enumerate(weights):
         if w.device != x.device:
             raise _lib.B200RNNError(f"b200rnn: weight[{i}] is on {w.device} but the input is on {x.device}")
-    save = torch.is_grad_enabled() and (x.requires_grad or any(w.requires_grad for w in weights))
-    return _RNNFunction.apply(x_tm, cfg, rng_state, grad_sink, lengths, save, *weights)
+    states = [s for s in (h_0, c_0) if s is not None]
+    save = torch.is_grad_enabled() and (x.requires_grad or any(t.requires_grad for t in (*weights, *states)))
+    return _RNNFunction.apply(x_tm, cfg, rng_state, grad_sink, lengths, save, h_0, c_0, *weights)
 
 
 @torch.no_grad()

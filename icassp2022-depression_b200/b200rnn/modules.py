@@ -10,8 +10,10 @@ default init U(-1/sqrt(H), 1/sqrt(H)) (rnn.py:308-311) and the ``forward`` retur
   fuse_net_whole.py:266-268, 281-286) construct them unchanged once :func:`install` has rebound
   ``torch.nn.GRU`` / ``torch.nn.LSTM``.
 
-``PackedSequence`` input is supported (per-sequence lengths in the kernels). Unused-by-the-reference features that
-raise ``NotImplementedError``: proj_size, bias=False, non-None initial state, unbatched 2-D input.
+``PackedSequence`` input is supported (per-sequence lengths in the kernels), and so are an initial state ``hx``
+(checked as torch checks it, differentiable: streaming inference or truncated BPTT that chains ``h_n`` into the next
+call) and unbatched 2-D input. Unused-by-the-reference features that raise ``NotImplementedError``: proj_size,
+bias=False. A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
 """
 from __future__ import annotations
 
@@ -156,12 +158,14 @@ class _B200RNNBase(nn.Module):
                          dropout=self.dropout, training=self.training, batch_first=self.batch_first,
                          tf32=tf32_enabled())
 
-    def _run_packed(self, packed):
+    def _run_packed(self, packed, hx):
         """PackedSequence path (ragged DAIC-style sequences): pad, run with per-sequence lengths, re-pack exactly like
-        torch (same batch_sizes / sorted_indices; h_n, c_n in the caller's original batch order)."""
+        torch (same batch_sizes / sorted_indices; hx, h_n and c_n in the caller's original batch order: the padded
+        batch is in that order already)."""
         rnn_utils = nn.utils.rnn
         padded, lengths = rnn_utils.pad_packed_sequence(packed, batch_first=self.batch_first)
-        out = rnn_forward(padded, self._flat_weights, self._config(), self._rng_state, self._grad_sink, lengths=lengths)
+        out = rnn_forward(padded, self._flat_weights, self._config(), self._rng_state, self._grad_sink, lengths=lengths,
+                          hx=hx)
         y = out[0]
         bdim = 0 if self.batch_first else 1
         if packed.sorted_indices is not None:
@@ -174,15 +178,36 @@ class _B200RNNBase(nn.Module):
                                             packed.unsorted_indices)
         return (y_packed, *out[1:])
 
+    def _hx_dims_error(self, hx, want: int) -> Optional[str]:
+        """torch's message when the initial state's rank does not match the input's batchedness, else None"""
+        batched = "batched 3-D" if want == 3 else "unbatched 2-D"
+        if self._mode == _lib.LSTM:
+            if hx[0].dim() != want or hx[1].dim() != want:
+                return (f"For {batched} input, hx and cx should also be {want}-D but got ({hx[0].dim()}-D, "
+                        f"{hx[1].dim()}-D) tensors")
+        elif hx.dim() != want:
+            return f"For {batched} input, hx should also be {want}-D but got {hx.dim()}-D tensor"
+        return None
+
     def _run(self, input, hx):
-        if hx is not None:
-            raise NotImplementedError("b200rnn: a non-None initial state is not implemented (the reference "
-                                      "always starts from zeros, rnn.py:1432-1440)")
         if isinstance(input, nn.utils.rnn.PackedSequence):
-            return self._run_packed(input)
-        if input.dim() != 3:
-            raise NotImplementedError("b200rnn: unbatched 2-D input is not implemented")
-        return rnn_forward(input, self._flat_weights, self._config(), self._rng_state, self._grad_sink)
+            return self._run_packed(input, hx)
+        if input.dim() not in (2, 3):
+            raise ValueError(f"{type(self).__name__}: Expected input to be 2D or 3D, got {input.dim()}D instead")
+        batched = input.dim() == 3
+        if hx is not None:
+            msg = self._hx_dims_error(hx, 3 if batched else 2)
+            if msg:
+                raise RuntimeError(msg)
+        if batched:
+            return rnn_forward(input, self._flat_weights, self._config(), self._rng_state, self._grad_sink, hx=hx)
+        # unbatched [T, I] (and [L*D, H] states): one batch row, whatever batch_first says, as torch runs it
+        batch_dim = 0 if self.batch_first else 1
+        if hx is not None:
+            hx = tuple(s.unsqueeze(1) for s in hx) if self._mode == _lib.LSTM else hx.unsqueeze(1)
+        out = rnn_forward(input.unsqueeze(batch_dim), self._flat_weights, self._config(), self._rng_state,
+                          self._grad_sink, hx=hx)
+        return (out[0].squeeze(batch_dim), *(s.squeeze(1) for s in out[1:]))
 
     def forward_ln_sum(self, input: torch.Tensor, ln: Optional[nn.LayerNorm] = None,
                        prologue_done: Optional[torch.cuda.Event] = None) -> torch.Tensor:

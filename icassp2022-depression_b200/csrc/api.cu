@@ -131,6 +131,7 @@ struct ScratchLayout {
   size_t b_tc_part_bytes;
   long long b_ldk;  // leading dimension of the transposed operands: T*B rounded up to a multiple of 4
   size_t b_dxln, b_lnpart;  // fused LayerNorm backward: dense d/dLN(x) [TB][I], per-CTA column partials
+  size_t b_h0;              // [B][G*H]: gate gradients of each row's first step, paired with h_0 in dW_hh
   size_t b_total;
   // both passes, past both layouts: int [B], the batch-slot order of a ragged batch (launch_length_order); the forward
   // and the backward each compute it from `lengths`
@@ -199,6 +200,8 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
   off += align_up(d.TB * (size_t)d.I, ALIGN_F);
   s->b_lnpart = off;
   off += align_up(layernorm_bwd_scratch_floats(d.I), ALIGN_F);
+  s->b_h0 = off;
+  off += align_up((size_t)d.B * d.GH, ALIGN_F);
   s->b_total = off;
 
   s->order = s->f_total > s->b_total ? s->f_total : s->b_total;
@@ -267,12 +270,13 @@ B200RNN_API int b200rnn_workspace_bytes(const b200rnn_desc* desc, size_t* reserv
   return B200RNN_OK;
 }
 
-B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
-                                      const float* const* params, float* y, int64_t ys_t, int64_t ys_b, float* h_n,
-                                      float* c_n, void* reserve, void* scratch, uint64_t seed, uint64_t offset,
-                                      uint64_t* rng_state, const float* ln_gamma, const float* ln_beta, float ln_eps,
-                                      float* y_pool, const int32_t* lengths, const void* wcache,
-                                      void* prologue_done, void* stream_) {
+// The forward of every entry point; h_0 / c_0 NULL = zeros (b200rnn_forward_hx checked their consistency)
+static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
+                        const float* const* params, float* y, int64_t ys_t, int64_t ys_b, float* h_n, float* c_n,
+                        void* reserve, void* scratch, uint64_t seed, uint64_t offset, uint64_t* rng_state,
+                        const float* ln_gamma, const float* ln_beta, float ln_eps, float* y_pool,
+                        const int32_t* lengths, const void* wcache, void* prologue_done, const float* h_0,
+                        const float* c_0, void* stream_) {
   Dims d;
   int rc = check_desc(desc, &d);
   if (rc) return rc;
@@ -470,6 +474,8 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     }
     rp.h_n = h_n + (size_t)l * d.D * d.B * d.H;
     rp.c_n = c_n ? c_n + (size_t)l * d.D * d.B * d.H : nullptr;
+    rp.h_0 = h_0 ? h_0 + (size_t)l * d.D * d.B * d.H : nullptr;
+    rp.c_0 = c_0 ? c_0 + (size_t)l * d.D * d.B * d.H : nullptr;
     rp.trace = g_trace;
     // Streamed, this launch directly follows the GEMM in the stream (nothing may be enqueued between them) and never
     // comes first: launched after the GEMM, the recurrence waits only on a kernel whose CTAs have all started.
@@ -484,6 +490,54 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     }
   }
   return B200RNN_OK;
+}
+
+// h_0 / c_0 / dh_0 / dc_0 of the hx entry points: c_0 (dc_0) only for the LSTM, and there c_0 only together with h_0
+static int check_initial_state(const b200rnn_desc* desc, const float* h_0, const void* c_0, const void* dc_0,
+                               const char* what) {
+  if (desc && desc->mode == B200RNN_GRU && (c_0 || dc_0)) {
+    set_error("%s: a GRU has no cell state (c_0 / dc_0 must be NULL)", what);
+    return B200RNN_ERR_INVALID;
+  }
+  if (c_0 && !h_0) {
+    set_error("%s: c_0 without h_0 (pass both initial states, or neither)", what);
+    return B200RNN_ERR_INVALID;
+  }
+  return B200RNN_OK;
+}
+
+B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
+                                      const float* const* params, float* y, int64_t ys_t, int64_t ys_b, float* h_n,
+                                      float* c_n, void* reserve, void* scratch, uint64_t seed, uint64_t offset,
+                                      uint64_t* rng_state, const float* ln_gamma, const float* ln_beta, float ln_eps,
+                                      float* y_pool, const int32_t* lengths, const void* wcache,
+                                      void* prologue_done, void* stream_) {
+  return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
+                      ln_gamma, ln_beta, ln_eps, y_pool, lengths, wcache, prologue_done, nullptr, nullptr, stream_);
+}
+
+B200RNN_API int b200rnn_forward_hx(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
+                                   const float* const* params, float* y, int64_t ys_t, int64_t ys_b, const float* h_0,
+                                   const float* c_0, float* h_n, float* c_n, void* reserve, void* scratch,
+                                   uint64_t seed, uint64_t offset, uint64_t* rng_state, const int32_t* lengths,
+                                   void* stream_) {
+  Dims d;
+  int rc = check_desc(desc, &d);
+  if (rc) return rc;
+  rc = check_initial_state(desc, h_0, c_0, nullptr, "forward_hx");
+  if (rc) return rc;
+  if (d.B > 0 && d.T == 0 && h_n && h_0) {  // no step: the final state is the initial one
+    cudaStream_t st = static_cast<cudaStream_t>(stream_);
+    const size_t bytes = (size_t)d.L * d.D * d.B * d.H * sizeof(float);
+    B200_CUDA_CHECK(cudaMemcpyAsync(h_n, h_0, bytes, cudaMemcpyDeviceToDevice, st));
+    if (c_n) {
+      if (c_0) B200_CUDA_CHECK(cudaMemcpyAsync(c_n, c_0, bytes, cudaMemcpyDeviceToDevice, st));
+      else B200_CUDA_CHECK(cudaMemsetAsync(c_n, 0, bytes, st));
+    }
+    return B200RNN_OK;
+  }
+  return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
+                      nullptr, nullptr, 0.f, nullptr, lengths, nullptr, nullptr, h_0, c_0, stream_);
 }
 
 B200RNN_API int b200rnn_forward(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
@@ -537,13 +591,14 @@ B200RNN_API int b200rnn_prepare_weights(const b200rnn_desc* desc, const float* c
   return B200RNN_OK;
 }
 
-B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
-                                       const float* const* params, const float* y, int64_t ys_t, int64_t ys_b,
-                                       const float* dy, int64_t dys_t, int64_t dys_b, const float* dy_pool,
-                                       float dy_pool_scale, const float* dh_n, const float* dc_n, const void* reserve,
-                                       void* scratch, float* dx, int64_t dxs_t, int64_t dxs_b, float* const* dparams,
-                                       const int32_t* lengths, const float* ln_gamma, float ln_eps, float* dln_gamma,
-                                       float* dln_beta, void* stream_) {
+// The backward of every entry point; h_0 / c_0 NULL = zeros, dh_0 / dc_0 NULL = not computed
+static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
+                         const float* const* params, const float* y, int64_t ys_t, int64_t ys_b, const float* dy,
+                         int64_t dys_t, int64_t dys_b, const float* dy_pool, float dy_pool_scale, const float* dh_n,
+                         const float* dc_n, const void* reserve, void* scratch, float* dx, int64_t dxs_t,
+                         int64_t dxs_b, float* const* dparams, const int32_t* lengths, const float* ln_gamma,
+                         float ln_eps, float* dln_gamma, float* dln_beta, const float* h_0, const float* c_0,
+                         float* dh_0, float* dc_0, void* stream_) {
   Dims d;
   int rc = check_desc(desc, &d);
   if (rc) return rc;
@@ -598,8 +653,13 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
       bp.y = R + rl.ylayer[l]; bp.y_st = (long long)d.B * d.DH; bp.y_sb = (long long)d.DH;
       bp.dy = S + sl.b_dy; bp.dy_st = (long long)d.B * d.DH; bp.dy_sb = (long long)d.DH;
     }
-    bp.dh_n = dh_n ? dh_n + (size_t)l * d.D * d.B * d.H : nullptr;
-    bp.dc_n = dc_n ? dc_n + (size_t)l * d.D * d.B * d.H : nullptr;
+    const size_t lstate = (size_t)l * d.D * d.B * d.H;  // this layer's [D,B,H] slice of the [L*D,B,H] states
+    bp.dh_n = dh_n ? dh_n + lstate : nullptr;
+    bp.dc_n = dc_n ? dc_n + lstate : nullptr;
+    bp.h_0 = h_0 ? h_0 + lstate : nullptr;
+    bp.c_0 = c_0 ? c_0 + lstate : nullptr;
+    bp.dh_0 = dh_0 ? dh_0 + lstate : nullptr;
+    bp.dc_0 = dc_0 ? dc_0 + lstate : nullptr;
     for (int k = 0; k < d.D; ++k) {
       const float* const* pp = params + (size_t)(l * d.D + k) * 4;
       if (!pp[0] || !pp[1]) {
@@ -747,7 +807,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
         rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
         if (rc) return rc;
       }
-      if (!done_dwhh) {  // dW_hh = sum_t dGh[t]^T * h_{prev(t)}   (h_prev of the first scanned step is 0)
+      if (!done_dwhh) {  // dW_hh = sum_t dGh[t]^T * h_{prev(t)}   (the first scanned step's h_0 term follows below)
         const int Kp = (d.T - 1) * d.B;
         // forward direction: pairs (dG[t], y[t-1]) for t = 1..T-1 ; reverse: (dG[t], y[t+1]) for t = 0..T-2
         const size_t g_t0 = (k == 0) ? (size_t)d.B : 0;  // first dG row
@@ -780,6 +840,23 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
           if (rc) return rc;
         }
       }
+      if (dw_hh && bp.h_0) {
+        // the first scanned step's previous state is h_0: dW_hh += sum_b dGh[t_first(b), b]^T h_0[b]. The shifted GEMMs
+        // above never pair that step with anything but a zero (T = 1: K = 0; ragged reverse rows: the masked output at
+        // len_b), so nothing is counted twice. One fixed-order K = B FFMA GEMM: deterministic.
+        float* rows0 = S + sl.b_h0;  // [B][GH]
+        rc = launch_initial_state_rows(dG, dHN, d.mode, d.B, d.T, d.H, k == 1, lengths, rows0, st);
+        if (rc) return rc;
+        GemmParams g;
+        memset(&g, 0, sizeof(g));
+        g.A = rows0; g.a_rows = simple_rows((long long)d.GH); g.a_kcontig = 0;
+        g.B = bp.h_0 + (size_t)k * d.B * d.H; g.b_rows = simple_rows(d.H); g.b_kcontig = 0;
+        g.C = dw_hh; g.c_rows = simple_rows(d.H);
+        g.M = (int)d.GH; g.N = d.H; g.K = d.B;
+        g.accumulate = 1;
+        rc = launch_gemm(g, nullptr, 0, st);
+        if (rc) return rc;
+      }
       if (!done_dx) {  // dX_l (+)= dGi * W_ih
         GemmParams g;
         memset(&g, 0, sizeof(g));
@@ -809,6 +886,50 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
     }
   }
   return B200RNN_OK;
+}
+
+B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
+                                       const float* const* params, const float* y, int64_t ys_t, int64_t ys_b,
+                                       const float* dy, int64_t dys_t, int64_t dys_b, const float* dy_pool,
+                                       float dy_pool_scale, const float* dh_n, const float* dc_n, const void* reserve,
+                                       void* scratch, float* dx, int64_t dxs_t, int64_t dxs_b, float* const* dparams,
+                                       const int32_t* lengths, const float* ln_gamma, float ln_eps, float* dln_gamma,
+                                       float* dln_beta, void* stream_) {
+  return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, dy_pool, dy_pool_scale, dh_n,
+                       dc_n, reserve, scratch, dx, dxs_t, dxs_b, dparams, lengths, ln_gamma, ln_eps, dln_gamma,
+                       dln_beta, nullptr, nullptr, nullptr, nullptr, stream_);
+}
+
+B200RNN_API int b200rnn_backward_hx(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
+                                    const float* const* params, const float* y, int64_t ys_t, int64_t ys_b,
+                                    const float* dy, int64_t dys_t, int64_t dys_b, const float* dh_n,
+                                    const float* dc_n, const float* h_0, const float* c_0, float* dh_0, float* dc_0,
+                                    const void* reserve, void* scratch, float* dx, int64_t dxs_t, int64_t dxs_b,
+                                    float* const* dparams, const int32_t* lengths, void* stream_) {
+  Dims d;
+  int rc = check_desc(desc, &d);
+  if (rc) return rc;
+  rc = check_initial_state(desc, h_0, c_0, dc_0, "backward_hx");
+  if (rc) return rc;
+  if (!dy) {
+    set_error("backward: null pointer argument");
+    return B200RNN_ERR_INVALID;
+  }
+  if (d.B > 0 && d.T == 0) {  // no step: the gradients pass from the final state to the initial one
+    cudaStream_t st = static_cast<cudaStream_t>(stream_);
+    const size_t bytes = (size_t)d.L * d.D * d.B * d.H * sizeof(float);
+    const float* src[2] = {dh_n, dc_n};
+    float* dst[2] = {dh_0, dc_0};
+    for (int i = 0; i < 2; ++i) {
+      if (!dst[i]) continue;
+      if (src[i]) B200_CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], bytes, cudaMemcpyDeviceToDevice, st));
+      else B200_CUDA_CHECK(cudaMemsetAsync(dst[i], 0, bytes, st));
+    }
+    return B200RNN_OK;
+  }
+  return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, nullptr, 0.f, dh_n, dc_n, reserve,
+                       scratch, dx, dxs_t, dxs_b, dparams, lengths, nullptr, 0.f, nullptr, nullptr, h_0, c_0, dh_0, dc_0,
+                       stream_);
 }
 
 B200RNN_API int b200rnn_backward(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,

@@ -73,6 +73,23 @@ __global__ void length_order_kernel(const int* __restrict__ lengths, int B, int*
   }
 }
 
+__global__ void initial_state_rows_kernel(const float* __restrict__ dgates, const float* __restrict__ dghn, int mode,
+                                          int B, int T, int H, int reverse, const int* __restrict__ lengths,
+                                          float* __restrict__ out) {
+  const int GH = (mode == B200RNN_GRU ? 3 : 4) * H;
+  const size_t n = (size_t)B * GH;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int b = (int)(i / GH), c = (int)(i % GH);
+    const int t = reverse ? (lengths ? min(max(lengths[b], 0), T) : T) - 1 : 0;
+    float v = 0.f;
+    if (t >= 0) {
+      const size_t row = (size_t)t * B + b;
+      v = (mode == B200RNN_GRU && c >= 2 * H) ? dghn[row * H + (c - 2 * H)] : dgates[row * GH + c];
+    }
+    out[i] = v;
+  }
+}
+
 __global__ void bias_reduce_kernel(const float* __restrict__ part, int nslices, int mode, int H, float* db_ih,
                                    float* db_hh, int accumulate) {
   const int G = mode == B200RNN_GRU ? 3 : 4;
@@ -131,6 +148,18 @@ int launch_length_order(const int* lengths, int B, int* order, cudaStream_t stre
   if (B <= 0) return B200RNN_OK;
   const int threads = B < ORDER_TILE ? (B + 31) / 32 * 32 : ORDER_TILE;
   length_order_kernel<<<1, threads, 0, stream>>>(lengths, B, order);
+  B200_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return B200RNN_OK;
+}
+
+int launch_initial_state_rows(const float* dgates, const float* dghn, int mode, int B, int T, int H, bool reverse,
+                              const int* lengths, float* out, cudaStream_t stream) {
+  const size_t n = (size_t)B * (mode == B200RNN_GRU ? 3 : 4) * H;
+  if (n == 0) return B200RNN_OK;
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > NUM_SMS * 4) blocks = NUM_SMS * 4;
+  initial_state_rows_kernel<<<blocks, 256, 0, stream>>>(dgates, dghn, mode, B, T, H, reverse ? 1 : 0, lengths, out);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;

@@ -20,6 +20,12 @@ int launch_dropout(const float* in, float* out, size_t n, float p, const uint64_
 // lengths[row], ties by row index (a stable sort: non-increasing lengths give the identity). One CTA.
 int launch_length_order(const int* lengths, int B, int* order, cudaStream_t stream);
 
+// The recurrent-side gate gradient of each row's first scanned step, the rows the initial state's dW_hh term pairs
+// with h_0: out[b][c] = dGh[t_first(b)][b][c] over c < G*H, where dGh is dgates [T,B,G*H] (the GRU's n columns come
+// from dghn [T,B,H] instead). t_first = 0 forward; reverse: T - 1, or lengths[b] - 1 (a row of length 0: zeros).
+int launch_initial_state_rows(const float* dgates, const float* dghn, int mode, int B, int T, int H, bool reverse,
+                              const int* lengths, float* out, cudaStream_t stream);
+
 // db_ih / db_hh from the per-slice partial sums written by the backward recurrence:
 //   part [nslices][(G+1)*H]  (first G*H: sum of dGi columns; tail H: GRU sum of dn*r)
 //   GRU : db_ih = sum(part[:, :3H]);  db_hh = (sum part[:, :2H], sum part[:, 3H:4H])

@@ -30,6 +30,8 @@ struct RecFwdParams {
   int tiles_n;
   int tf32;                  // single-pass TF32 contraction in the tensor-core config tc8 (B200RNN_FLAG_TF32); every
                              // other config is fp32 FFMA and ignores it
+  const float* h_0;          // optional [D,B,H] initial state of this layer, caller's row order (NULL: zeros)
+  const float* c_0;          // optional [D,B,H] initial cell state (LSTM; NULL: zeros)
 };
 
 // A recurrence launch chosen for a shape, before anything is enqueued: `nclusters` clusters of C CTAs, of which
@@ -64,6 +66,10 @@ struct RecBwdParams {
   int nslices_out;           // filled by the launcher
   const int* lengths;        // optional [B], as in the forward
   const int* order;          // with lengths: [B] row of each batch slot, as in the forward
+  const float* h_0;          // the forward's initial state [D,B,H] or NULL (zeros): h_{prev} of the first step
+  const float* c_0;          // the forward's initial cell state [D,B,H] or NULL (LSTM)
+  float* dh_0;               // out, optional [D,B,H]: gradient w.r.t. h_0 (NULL: the last step's contraction is skipped)
+  float* dc_0;               // out, optional [D,B,H]: gradient w.r.t. c_0 (LSTM)
 };
 
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)

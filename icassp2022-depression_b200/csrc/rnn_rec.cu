@@ -173,6 +173,16 @@ struct FwdCell {
     for (int g = 0; g < G; ++g) gi[g] = 0.f;
   }
 
+  // The state starts at h_0 / c_0 (zeros when NULL); a ragged row keeps it until its first real step. Called right
+  // before the step loop: a state loaded earlier stays live through the prologue and changes how ptxas schedules the
+  // loop. Only the uniform pointer test branches (a per-lane branch costs the loop its warp-uniform barrier waits): a
+  // slot past the batch loads the last row and discards it.
+  __device__ __forceinline__ void start(const RecFwdParams& p, int dir) {
+    const size_t s0 = ((size_t)dir * p.B + min(b, p.B - 1)) * H + j;
+    if (p.h_0) h = valid ? p.h_0[s0] : 0.f;
+    if (MODE == B200RNN_LSTM && p.c_0) c = valid ? p.c_0[s0] : 0.f;
+  }
+
   __device__ __forceinline__ void load_gi(const RecFwdParams& p, int t) {
     if (valid) {
       const float* gp = gates + ((size_t)t * p.B + b) * (G * H) + j;
@@ -259,6 +269,19 @@ __device__ __forceinline__ int slice_steps(const int* lengths, const int* order,
   return min(max(lengths[order[b0]], 0), T);
 }
 
+// Initial value of element (unit k, batch slot q) of the shared state buffer the first step contracts against: h_0 of
+// the row in slot b0 + q (zero past the batch). Every CTA fills its whole buffer from global memory, so step 0 needs no
+// exchange; the caller tests p.h_0 (uniform) and zero-fills without it. Branch-free per lane, like FwdCell's load.
+// This runs in the prologue, which with the streamed x-projection (RecFwdParams::ready) may overlap the GEMM before the
+// kernel: h_0 is an input of the call, which that GEMM never writes, so reading it that early is safe.
+template <bool VL>
+__device__ __forceinline__ float initial_state(const RecFwdParams& p, int dir, int b0, int q, int k) {
+  const int slot = min(b0 + q, p.B - 1);
+  const int row = VL ? p.order[slot] : slot;
+  const float v = p.h_0[((size_t)dir * p.B + row) * p.H + k];
+  return b0 + q < p.B ? v : 0.f;
+}
+
 // Streamed x-projection (RecFwdParams::ready, api.cu): before a warp reads the x-projection of step t, it waits until
 // the GEMM has published every row tile that holds rows [t*B, (t+1)*B). The whole warp polls the counter with acquire
 // semantics (one broadcast load; a poll loop run by one lane alone made ptxas spill the FFMA configs' registers), and
@@ -320,7 +343,15 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       ptx::tma_bulk_g2s(W_s + (size_t)g * HS * H, w_hh + ((size_t)g * H + j0) * H,
                         (uint32_t)(HS * H * sizeof(float)), &bars[0]);
   }
-  for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
+  if (p.h_0) {  // buffer 0: the initial state of the cluster's batch slots, in the layout the all-gather writes
+    for (int i = tid; i < BS * H; i += NT) {
+      const int q = i / H, k = i - q * H;
+      h_s[PB ? paired_index<KL, BS>(k, q) : i] = initial_state<VL>(p, dir, b0, q, k);
+      h_s[BS * H + i] = 0.f;
+    }
+  } else {
+    for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
+  }
   const int rot = Cfg::ROT ? (int)rank * CPS : 0;
   float wreg[RG > 0 ? RG : 1][UPL][H / KL];
   load_resident<RG, KL, UPL, BS, H>(w_hh, H, (long long)NSM * H + j0 + w * UPW, rot, lane, wreg);
@@ -335,6 +366,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     gi_ready.wait(p, dir ? T - 1 : 0);
     cell.load_gi(p, dir ? T - 1 : 0);
   }
+  cell.start(p, dir);
 
   for (int step = 0; step < T; ++step) {
     const int t = dir ? (T - 1 - step) : step;
@@ -527,7 +559,16 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     dst[8] = TF32 ? round_tf32(v.z) : v.z;
     dst[12] = TF32 ? round_tf32(v.w) : v.w;
   }
-  for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
+  if (p.h_0) {  // buffer 0: the initial state in B-fragment order, rounded like the copies the lanes producing h_t hand over
+    for (int i = tid; i < BS * H; i += NT) {
+      const int q = i / H, k = i - q * H;
+      const float v = initial_state<VL>(p, dir, b0, q, k);
+      h_s[tc_state_index(k, q)] = TF32 ? round_tf32(v) : v;
+      h_s[BS * H + i] = 0.f;
+    }
+  } else {
+    for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
+  }
   __syncthreads();
   ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
 
@@ -546,6 +587,8 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   const float4* W_w = W_f + (size_t)ug * G * KS * 32 + lane;
   float* red_mine = red + w * 2 * G * 32 + lane;                         // written by this warp
   const float* red_partner = red + (w ^ NUG) * 2 * G * 32 + lane;        // written by the other k half
+#pragma unroll
+  for (int jb = 0; jb < 2; ++jb) cell[jb].start(p, dir);
   for (int step = 0; step < T; ++step) {
     const int t = dir ? (T - 1 - step) : step;
     const int cur = step & 1, nxt = cur ^ 1;
@@ -780,28 +823,40 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
   float sv[G], sx = 0.f, hp = 0.f, dyv = 0.f;  // saved gates, hn / c_t, h_{prev} / c_{prev}, dy
 #pragma unroll
   for (int g = 0; g < G; ++g) sv[g] = 0.f;
+  // the state before the first step: h_0 (GRU, feeds dz) or c_0 (LSTM, feeds df), zeros when NULL
+  const float* s0 = (MODE == B200RNN_GRU) ? p.h_0 : p.c_0;
   auto load_step = [&](int step) {
     const int t = dir ? step : (T - 1 - step);
-    const bool has_prev = step < T - 1;
+    bool has_prev = step < T - 1;
     const int tp = dir ? t + 1 : t - 1;
+    // GRU, VL: the forward output at tp >= len_b is the masked 0, not the state the row kept (h_0: the reverse
+    // direction's first real step t = len_b - 1 reads it). The LSTM reads c from `extra`, where frozen steps saved the
+    // kept state.
+    if (MODE == B200RNN_GRU && VL && tp >= len_b) has_prev = false;
     const float* gp = gates + ((size_t)t * B + b) * GH + j;
 #pragma unroll
     for (int g = 0; g < G; ++g) sv[g] = gp[g * H];
     sx = extra[((size_t)t * B + b) * H + j];
     dyv = p.dy ? p.dy[(long long)t * p.dy_st + (long long)b * p.dy_sb + dir * H + j] : dy_pooled;
-    if (MODE == B200RNN_GRU)
-      hp = has_prev ? p.y[(long long)tp * p.y_st + (long long)b * p.y_sb + dir * H + j] : 0.f;
+    if (!has_prev)
+      hp = s0 ? s0[((size_t)dir * B + b) * H + j] : 0.f;
+    else if (MODE == B200RNN_GRU)
+      hp = p.y[(long long)tp * p.y_st + (long long)b * p.y_sb + dir * H + j];
     else
-      hp = has_prev ? extra[((size_t)tp * B + b) * H + j] : 0.f;
+      hp = extra[((size_t)tp * B + b) * H + j];
   };
   if (valid && T > 0) load_step(0);
 
+  // dh_0 requested: the last step also runs the exchange and the contraction, whose result is dh_0 (the same phase
+  // bookkeeping as any other step); else it ends after its stores
+  const bool want_dh0 = p.dh_0 != nullptr;
   for (int step = 0; step < T; ++step) {
     const int t = dir ? step : (T - 1 - step);
     const int buf = step & 1;
     float* d_buf = d_s + buf * BS * GH;
     const bool last = (step == T - 1);
-    if (tid == 0 && !last) {
+    const bool contract = !last || want_dh0;
+    if (tid == 0 && contract) {
 #pragma unroll
       for (int src = 0; src < C; ++src)
         if (!kLocalSelf || (uint32_t)src != rank)
@@ -854,7 +909,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       bsum[G] += dhn;
     }
 
-    if (!last) {
+    if (contract) {
       // all-gather the recurrent-side gate gradient (GRU: n-gate part is dn*r) into every peer CTA
 #pragma unroll
       for (int g = 0; g < G; ++g) {
@@ -872,8 +927,8 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       for (int g = 0; g < G; ++g) gp[g * H] = dg[g];
       if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + b) * H + j] = dhn;
     }
-    if (last) break;
-    if (valid) load_step(step + 1);
+    if (!contract) break;
+    if (valid && !last) load_step(step + 1);
     const uint32_t par = (step >> 1) & 1;
 
     // ---- dh_{prev}[b][j] = direct + sum_col dgh[b][col] * W_hh[col][j], one gate block of columns at a time ----
@@ -906,6 +961,12 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     fold_pairs<1, UPL, BS>(acc2, acc);
     warp_transpose_reduce<1, KL, UPL, BS>(acc);
     dh_carry = direct + acc[0][0][0];
+  }
+  // gradients w.r.t. the initial state: what the scan carried past its first step (frozen steps pass dh / dc through,
+  // and a cluster that ran no step passes dh_n / dc_n on)
+  if (valid) {
+    if (want_dh0) p.dh_0[((size_t)dir * B + b) * H + j] = dh_carry;
+    if (MODE == B200RNN_LSTM && p.dc_0) p.dc_0[((size_t)dir * B + b) * H + j] = dc_carry;
   }
   if constexpr (VL) {
     // the steps [T, p.T) the cluster skipped: their gate gradients are 0, as past any sequence's length (the wgrad and

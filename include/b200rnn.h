@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define B200RNN_ABI_VERSION 3
+#define B200RNN_ABI_VERSION 4
 
 #if defined(__GNUC__)
 #define B200RNN_API __attribute__((visibility("default")))
@@ -102,7 +102,7 @@ B200RNN_API int b200rnn_workspace_bytes(const b200rnn_desc* desc, size_t* reserv
 
 /*
  * Forward pass: replaces `_VF.gru` / `_VF.lstm` behind nn.GRU.forward / nn.LSTM.forward
- * (rnn.py:1449 / :1169) with hx = None (h0 = c0 = 0, rnn.py:1432-1440).
+ * (rnn.py:1449 / :1169) with hx = None (h0 = c0 = 0, rnn.py:1432-1440; a given hx: b200rnn_forward_hx).
  *
  *   x         [T,B,I] addressed as x[t*x_stride_t + b*x_stride_b + i]  (feature stride 1), so both the
  *             batch_first layout of audio_gru_whole.py:60 and the permuted NON-contiguous view of
@@ -158,6 +158,22 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
                                       const int32_t* lengths, const void* wcache, void* prologue_done,
                                       void* stream /* cudaStream_t */);
 
+/*
+ * Forward from a given initial state: nn.GRU.forward(input, h_0) / nn.LSTM.forward(input, (h_0, c_0))
+ * (rnn.py:1449 / :1169 with a non-None hx), e.g. streaming inference or truncated BPTT that carries h_n of one chunk
+ * into the next call.
+ *   h_0, c_0  [L*D, B, H] contiguous, layout of h_n / c_n, batch rows in the caller's order (also with `lengths`).
+ *             NULL = zeros. c_0 is LSTM only (a GRU rejects it) and needs h_0. With `lengths`, a row keeps its initial
+ *             state until its first valid step (the reverse direction's is lengths[b]-1). T = 0: h_n = h_0, c_n = c_0.
+ * Everything else as b200rnn_forward_fused without the model-shell fusions (no LayerNorm, y_pool, wcache or event).
+ * h_0 / c_0 must be passed again to b200rnn_backward_hx.
+ */
+B200RNN_API int b200rnn_forward_hx(const b200rnn_desc* desc, const float* x, int64_t x_stride_t, int64_t x_stride_b,
+                                   const float* const* params, float* y, int64_t y_stride_t, int64_t y_stride_b,
+                                   const float* h_0, const float* c_0, float* h_n, float* c_n, void* reserve,
+                                   void* scratch, uint64_t dropout_seed, uint64_t dropout_offset, uint64_t* rng_state,
+                                   const int32_t* lengths, void* stream /* cudaStream_t */);
+
 /* Weight cache of b200rnn_forward_fused: size for this descriptor (batch / seq_len are ignored), and the pass that
  * fills it (one small launch per weight_ih; 256-byte aligned caller-owned buffer). */
 B200RNN_API int b200rnn_wcache_bytes(const b200rnn_desc* desc, size_t* bytes);
@@ -183,6 +199,21 @@ B200RNN_API int b200rnn_backward(const b200rnn_desc* desc, const float* x, int64
                                  int64_t dy_stride_b, const float* dh_n, const float* dc_n, const void* reserve,
                                  void* scratch, float* dx, int64_t dx_stride_t, int64_t dx_stride_b,
                                  float* const* dparams, const int32_t* lengths, void* stream /* cudaStream_t */);
+
+/*
+ * Backward of b200rnn_forward_hx: b200rnn_backward plus
+ *   h_0, c_0    the initial states given to the forward (NULL = zeros); the dW_hh term of the first step pairs its
+ *               gate gradient with h_0
+ *   dh_0, dc_0  out, [L*D, B, H] contiguous: gradients w.r.t. h_0 / c_0 (written, never accumulated), or NULL to skip;
+ *               dh_0 costs the last step's recurrent contraction, dc_0 nothing. dc_0 is LSTM only.
+ */
+B200RNN_API int b200rnn_backward_hx(const b200rnn_desc* desc, const float* x, int64_t x_stride_t, int64_t x_stride_b,
+                                    const float* const* params, const float* y, int64_t y_stride_t,
+                                    int64_t y_stride_b, const float* dy, int64_t dy_stride_t, int64_t dy_stride_b,
+                                    const float* dh_n, const float* dc_n, const float* h_0, const float* c_0,
+                                    float* dh_0, float* dc_0, const void* reserve, void* scratch, float* dx,
+                                    int64_t dx_stride_t, int64_t dx_stride_b, float* const* dparams,
+                                    const int32_t* lengths, void* stream /* cudaStream_t */);
 
 /*
  * Backward with the model-shell fusions of the TRAINING path (SURVEY.md 8f rank 1; audio_gru_whole.py:103-108 with
