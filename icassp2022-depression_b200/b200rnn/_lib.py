@@ -18,6 +18,7 @@ FLAG_ACCUMULATE_GRADS = 1
 FLAG_SAVE_FOR_BACKWARD = 2
 FLAG_FUSED_LN = 4
 FLAG_TF32 = 8
+FLAG_PROJ = 16      # the descriptor carries proj_size (read only with this flag)
 ABI_VERSION = 4
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)
@@ -60,7 +61,8 @@ IPC_HANDLE_BYTES = 64
 
 
 class Desc(ctypes.Structure):
-    """``b200rnn_desc`` (include/b200rnn.h)."""
+    """``b200rnn_desc`` (include/b200rnn.h). ``proj_size`` is last and read only with ``FLAG_PROJ``: positional
+    construction with the first ten fields means "no projection"."""
 
     _fields_ = [
         ("mode", c_int32),
@@ -73,6 +75,7 @@ class Desc(ctypes.Structure):
         ("training", c_int32),
         ("dropout_p", c_float),
         ("flags", c_uint32),
+        ("proj_size", c_int32),
     ]
 
 

@@ -27,6 +27,12 @@ class RNNConfig:
     training: bool
     batch_first: bool
     tf32: bool = False   # single-pass TF32 tensor-core GEMMs / tc8 recurrence (tf32_enabled()), else 3xTF32
+    proj_size: int = 0   # LSTM with projections: width P of h_t (0 = none)
+
+    @property
+    def out_size(self) -> int:
+        """width of h_t and of the output per direction: proj_size, or hidden_size without a projection"""
+        return self.proj_size if self.proj_size > 0 else self.hidden_size
 
 
 def tf32_enabled() -> bool:
@@ -68,8 +74,10 @@ def _make_desc(cfg: RNNConfig, B: int, T: int, save: bool, accumulate: bool = Fa
         flags |= _lib.FLAG_FUSED_LN
     if cfg.tf32:
         flags |= _lib.FLAG_TF32
+    if cfg.proj_size:
+        flags |= _lib.FLAG_PROJ
     return _lib.Desc(cfg.mode, B, T, cfg.input_size, cfg.hidden_size, cfg.num_layers, cfg.num_dirs,
-                     1 if cfg.training else 0, float(cfg.dropout), flags)
+                     1 if cfg.training else 0, float(cfg.dropout), flags, cfg.proj_size)
 
 
 def _stream_ptr(device=None) -> int:
@@ -86,7 +94,8 @@ def _on(device):
 
 class _RNNFunction(torch.autograd.Function):
     """y, h_n[, c_n] = RNN(x, weights, h_0[, c_0]); x is the logical time-major view [T,B,I], h_0 / c_0 are None
-    (zeros) or contiguous [L*D,B,H]."""
+    (zeros) or contiguous [L*D,B,HO] / [L*D,B,H] (HO = proj_size, or H without a projection). A projected LSTM always
+    goes through the _hx entry points (with NULL states when hx is None): the _fused ones do not take proj_size."""
 
     # position of the first weight among forward()'s inputs (after ctx)
     _W0 = 8
@@ -97,7 +106,7 @@ class _RNNFunction(torch.autograd.Function):
                 *weights: torch.Tensor):
         lib = _lib.load()
         T, B, _ = x_tm.shape
-        H, L, D = cfg.hidden_size, cfg.num_layers, cfg.num_dirs
+        H, L, D, HO = cfg.hidden_size, cfg.num_layers, cfg.num_dirs, cfg.out_size
         dev = x_tm.device
         # `save` is decided by the caller: grad mode is always off in here, and needs_input_grad is True for
         # requires_grad weights even under torch.no_grad() (it would allocate the reserve and store gates for nothing)
@@ -107,12 +116,12 @@ class _RNNFunction(torch.autograd.Function):
         reserve = torch.empty(rbytes if save else 0, dtype=torch.uint8, device=dev)
         scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
         if cfg.batch_first:
-            y = torch.empty(B, T, D * H, dtype=torch.float32, device=dev)
-            ys_t, ys_b = D * H, T * D * H
+            y = torch.empty(B, T, D * HO, dtype=torch.float32, device=dev)
+            ys_t, ys_b = D * HO, T * D * HO
         else:
-            y = torch.empty(T, B, D * H, dtype=torch.float32, device=dev)
-            ys_t, ys_b = B * D * H, D * H
-        h_n = torch.empty(L * D, B, H, dtype=torch.float32, device=dev)
+            y = torch.empty(T, B, D * HO, dtype=torch.float32, device=dev)
+            ys_t, ys_b = B * D * HO, D * HO
+        h_n = torch.empty(L * D, B, HO, dtype=torch.float32, device=dev)
         c_n = torch.empty(L * D, B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
         params = _lib.ptr_array([w.data_ptr() for w in weights])
         rng_ptr = rng_state.data_ptr() if rng_state is not None else None
@@ -120,7 +129,7 @@ class _RNNFunction(torch.autograd.Function):
         c_n_ptr = c_n.data_ptr() if c_n is not None else None
         if B > 0 and T > 0:
             with _on(dev):
-                if h_0 is None:
+                if h_0 is None and not cfg.proj_size:
                     rc = lib.b200rnn_forward_fused(
                         ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
                         y.data_ptr(), ys_t, ys_b, h_n.data_ptr(), c_n_ptr,
@@ -129,7 +138,8 @@ class _RNNFunction(torch.autograd.Function):
                 else:
                     rc = lib.b200rnn_forward_hx(
                         ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
-                        y.data_ptr(), ys_t, ys_b, h_0.data_ptr(), c_0.data_ptr() if c_0 is not None else None,
+                        y.data_ptr(), ys_t, ys_b, h_0.data_ptr() if h_0 is not None else None,
+                        c_0.data_ptr() if c_0 is not None else None,
                         h_n.data_ptr(), c_n_ptr, reserve.data_ptr() if save else None, scratch.data_ptr(),
                         0, 0, rng_ptr, len_ptr, _stream_ptr(dev))
             _lib.check(rc, "b200rnn_forward")
@@ -215,7 +225,7 @@ class _RNNFunction(torch.autograd.Function):
                 tail = (reserve.data_ptr(), scratch.data_ptr(), ptr(dx),
                         dx.stride(0) if dx is not None else 0, dx.stride(1) if dx is not None else 0,
                         dparams, ptr(ctx.lengths), _stream_ptr(dev))
-                if h_0 is None:
+                if h_0 is None and not cfg.proj_size:
                     rc = lib.b200rnn_backward(*head, *tail)
                 else:
                     rc = lib.b200rnn_backward_hx(*head, ptr(h_0), ptr(c_0), ptr(dh_0), ptr(dc_0), *tail)
@@ -334,6 +344,8 @@ def rnn_ln_pool_sum(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNCo
     _require_cuda_f32(x, "input")
     for i, w in enumerate(weights):
         _require_cuda_f32(w, f"weight[{i}]")
+    if cfg.proj_size:
+        raise NotImplementedError("b200rnn: the fused LayerNorm / time-sum path does not take proj_size")
     x_tm = _tm_view(x.transpose(0, 1) if cfg.batch_first else x)
     return _LNRNNPoolFunction.apply(x_tm, cfg, rng_state, grad_sink, ln_weight, ln_bias, ln_eps, *weights)
 
@@ -349,12 +361,12 @@ def _initial_state(hx, cfg: RNNConfig, x: torch.Tensor):
     if len(states) != (2 if lstm else 1):
         raise RuntimeError(f"b200rnn: LSTM hx must be a pair (h_0, c_0), got {len(states)} tensors")
     batch = x.size(0 if cfg.batch_first else 1) if x.dim() == 3 else None
-    expected = (cfg.num_layers * cfg.num_dirs, batch, cfg.hidden_size)
+    expected = [(cfg.num_layers * cfg.num_dirs, batch, w) for w in (cfg.out_size, cfg.hidden_size)]
     msgs = (("Expected hidden[0] size {}, got {}", "Expected hidden[1] size {}, got {}") if lstm
             else ("Expected hidden size {}, got {}",))
-    for s, msg in zip(states, msgs):
-        if s.size() != expected:
-            raise RuntimeError(msg.format(expected, list(s.size())))
+    for s, msg, want in zip(states, msgs, expected):
+        if s.size() != want:
+            raise RuntimeError(msg.format(want, list(s.size())))
     for s in states:
         if s.device != x.device:
             raise RuntimeError("Input and hidden tensors are not at the same device, found input tensor at "
@@ -412,6 +424,8 @@ def rnn_forward_fused(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNN
     """
     lib = _lib.load()
     _require_cuda_f32(x, "input")
+    if cfg.proj_size:
+        raise NotImplementedError("b200rnn: the fused forward (LayerNorm prologue, time sum) does not take proj_size")
     x_tm = _tm_view(x.transpose(0, 1) if cfg.batch_first else x)
     T, B, _ = x_tm.shape
     H, L, D = cfg.hidden_size, cfg.num_layers, cfg.num_dirs

@@ -12,8 +12,9 @@ default init U(-1/sqrt(H), 1/sqrt(H)) (rnn.py:308-311) and the ``forward`` retur
 
 ``PackedSequence`` input is supported (per-sequence lengths in the kernels), and so are an initial state ``hx``
 (checked as torch checks it, differentiable: streaming inference or truncated BPTT that chains ``h_n`` into the next
-call) and unbatched 2-D input. Unused-by-the-reference features that raise ``NotImplementedError``: proj_size,
-bias=False. A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
+call) and unbatched 2-D input. ``LSTM(..., proj_size=P)`` (LSTMP: ``h_t = W_hr (o_t * tanh c_t)``) runs on its own
+projected kernels for P in {H/4, H/2} and registers ``weight_hr_l{k}[_reverse]`` last, as torch does. Features that
+raise ``NotImplementedError``: bias=False, and other projection sizes. A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
 """
 from __future__ import annotations
 
@@ -41,10 +42,18 @@ class _B200RNNBase(nn.Module):
                  batch_first: bool = False, dropout: float = 0.0, bidirectional: bool = False,
                  proj_size: int = 0, device=None, dtype=None) -> None:
         super().__init__()
+        if proj_size != 0 and self._mode != _lib.LSTM:
+            raise ValueError("proj_size argument is only supported for LSTM, not RNN or GRU")
         if not bias:
             raise NotImplementedError("b200rnn: bias=False is not used by the reference and not implemented")
-        if proj_size != 0:
-            raise NotImplementedError("b200rnn: proj_size is not used by the reference and not implemented")
+        if proj_size < 0:
+            raise ValueError("proj_size should be a positive integer or zero to disable projections")
+        if proj_size >= hidden_size > 0:
+            raise ValueError("proj_size has to be smaller than hidden_size")
+        if proj_size > 0 and (hidden_size not in (128, 256) or proj_size not in (hidden_size // 4, hidden_size // 2)):
+            raise NotImplementedError(
+                f"b200rnn: proj_size={proj_size} with hidden_size={hidden_size} is not implemented; the projected LSTM "
+                "kernels take hidden_size 128 with proj_size 32 or 64, and hidden_size 256 with proj_size 64 or 128")
         if dtype not in (None, torch.float32):
             raise NotImplementedError("b200rnn: float32 only")
         if not isinstance(dropout, (int, float)) or not 0 <= dropout <= 1 or isinstance(dropout, bool):
@@ -62,17 +71,21 @@ class _B200RNNBase(nn.Module):
         self.batch_first = batch_first
         self.dropout = float(dropout)
         self.bidirectional = bidirectional
-        self.proj_size = 0
+        self.proj_size = int(proj_size)
         num_directions = 2 if bidirectional else 1
         gate_size = self._gates * hidden_size
+        real_hidden_size = proj_size if proj_size > 0 else hidden_size
 
         self._flat_weights_names: List[str] = []
         for layer in range(num_layers):
             for direction in range(num_directions):
-                layer_input_size = input_size if layer == 0 else hidden_size * num_directions
+                layer_input_size = input_size if layer == 0 else real_hidden_size * num_directions
                 suffix = "_reverse" if direction == 1 else ""
-                shapes = ((gate_size, layer_input_size), (gate_size, hidden_size), (gate_size,), (gate_size,))
+                shapes = ((gate_size, layer_input_size), (gate_size, real_hidden_size), (gate_size,), (gate_size,))
                 names = ("weight_ih_l{}{}", "weight_hh_l{}{}", "bias_ih_l{}{}", "bias_hh_l{}{}")
+                if proj_size > 0:
+                    shapes += ((proj_size, hidden_size),)
+                    names += ("weight_hr_l{}{}",)
                 for name, shape in zip(names, shapes):
                     pname = name.format(layer, suffix)
                     self.register_parameter(
@@ -106,10 +119,13 @@ class _B200RNNBase(nn.Module):
     @property
     def all_weights(self) -> List[List[nn.Parameter]]:
         fw = self._flat_weights
-        return [fw[i:i + 4] for i in range(0, len(fw), 4)]
+        n = 5 if self.proj_size > 0 else 4
+        return [fw[i:i + n] for i in range(0, len(fw), n)]
 
     def extra_repr(self) -> str:
         s = "{input_size}, {hidden_size}"
+        if self.proj_size != 0:
+            s += ", proj_size={proj_size}"
         if self.num_layers != 1:
             s += ", num_layers={num_layers}"
         if self.batch_first is not False:
@@ -140,7 +156,7 @@ class _B200RNNBase(nn.Module):
         cache is keyed on the parameters' storage addresses and version counters, so ``load_state_dict``, ``.to()`` or
         an in-place edit refresh it; trainable modules never use it (their weights change every step anyway)."""
         ws = self._flat_weights
-        if any(w.requires_grad for w in ws) or not ws[0].is_cuda:
+        if any(w.requires_grad for w in ws) or not ws[0].is_cuda or self.proj_size:
             self._wcache = None
             return None
         key = tuple((w.data_ptr(), w._version) for w in ws)
@@ -156,7 +172,7 @@ class _B200RNNBase(nn.Module):
         return RNNConfig(mode=self._mode, input_size=self.input_size, hidden_size=self.hidden_size,
                          num_layers=self.num_layers, num_dirs=2 if self.bidirectional else 1,
                          dropout=self.dropout, training=self.training, batch_first=self.batch_first,
-                         tf32=tf32_enabled())
+                         tf32=tf32_enabled(), proj_size=self.proj_size)
 
     def _run_packed(self, packed, hx):
         """PackedSequence path (ragged DAIC-style sequences): pad, run with per-sequence lengths, re-pack exactly like
@@ -225,7 +241,7 @@ class _B200RNNBase(nn.Module):
         """
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
-        shape_ok = (input.is_cuda and input.dim() == 3 and
+        shape_ok = (input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and
                                     ln.bias is not None)))
         fusable = not need_grad and shape_ok

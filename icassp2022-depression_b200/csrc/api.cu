@@ -33,9 +33,13 @@ namespace {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// proj_size of a descriptor: the field exists only when B200RNN_FLAG_PROJ says so (a descriptor may end at `flags`)
+inline int desc_proj(const b200rnn_desc* d) { return (d->flags & B200RNN_FLAG_PROJ) ? d->proj_size : 0; }
+
 struct Dims {
   int mode, B, T, I, H, L, D, G;
-  size_t TB, GH, DH;
+  int P, HO, NPAR;  // proj_size (0: none), width of h / the layer output per direction, parameters per (layer, dir)
+  size_t TB, GH, DH;  // DH = D * HO: width of a layer's output
   bool training;
   float p;
 };
@@ -60,6 +64,15 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
               d->hidden_size);
     return B200RNN_ERR_UNSUPPORTED;
   }
+  const int P = desc_proj(d);
+  if (P < 0 || (P > 0 && (d->mode != B200RNN_LSTM || P >= d->hidden_size))) {
+    set_error("proj_size %d invalid: an LSTM takes 0 <= proj_size < hidden_size, a GRU none", P);
+    return B200RNN_ERR_INVALID;
+  }
+  if (P > 0 && P != d->hidden_size / 4 && P != d->hidden_size / 2) {
+    set_error("proj_size %d unsupported: the projected kernels are built for hidden_size/4 and hidden_size/2", P);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   if (!(d->dropout_p >= 0.f && d->dropout_p <= 1.f)) {
     set_error("dropout_p must be in [0,1] (got %f)", (double)d->dropout_p);
     return B200RNN_ERR_INVALID;
@@ -72,9 +85,12 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
   o->L = d->num_layers;
   o->D = d->num_dirs;
   o->G = d->mode == B200RNN_GRU ? 3 : 4;
+  o->P = P;
+  o->HO = P > 0 ? P : d->hidden_size;
+  o->NPAR = P > 0 ? 5 : 4;
   o->TB = (size_t)d->seq_len * d->batch;
   o->GH = (size_t)o->G * o->H;
-  o->DH = (size_t)o->D * o->H;
+  o->DH = (size_t)o->D * o->HO;
   o->training = d->training != 0;
   o->p = d->dropout_p;
   return B200RNN_OK;
@@ -85,6 +101,7 @@ constexpr size_t ALIGN_F = 64;  // floats (256 B)
 // ---- reserve layout (floats) ------------------------------------------------------------------
 struct ReserveLayout {
   size_t gates[8][2], extra[8][2];  // up to 8 layers
+  size_t m[8][2];                   // proj_size > 0: o * tanh(c) of every step, [T,B,H] (operand of dW_hr)
   size_t ylayer[8], ydrop[8];
   size_t xln;  // LayerNorm(x) of the folded prologue, kept for the layer-0 wgrad (B200RNN_FLAG_FUSED_LN)
   size_t total;
@@ -102,6 +119,8 @@ int make_reserve(const Dims& d, ReserveLayout* r, bool fused_ln = false) {
       off += align_up(d.TB * d.GH, ALIGN_F);
       r->extra[l][k] = off;
       off += align_up(d.TB * d.H, ALIGN_F);
+      r->m[l][k] = off;
+      if (d.P > 0) off += align_up(d.TB * d.H, ALIGN_F);
     }
   for (int l = 0; l + 1 < d.L; ++l) {
     r->ylayer[l] = off;
@@ -132,6 +151,7 @@ struct ScratchLayout {
   long long b_ldk;  // leading dimension of the transposed operands: T*B rounded up to a multiple of 4
   size_t b_dxln, b_lnpart;  // fused LayerNorm backward: dense d/dLN(x) [TB][I], per-CTA column partials
   size_t b_h0;              // [B][G*H]: gate gradients of each row's first step, paired with h_0 in dW_hh
+  size_t b_dhp[2];          // proj_size > 0, per direction [T,B,P]: gradient w.r.t. the projected h_t (dW_hr)
   size_t b_total;
   // both passes, past both layouts: int [B], the batch-slot order of a ragged batch (launch_length_order); the forward
   // and the backward each compute it from `lengths`
@@ -179,6 +199,10 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
   size_t g2 = gemm_scratch_bytes((int)d.GH, d.H, K);
   gb = g0 > g1 ? g0 : g1;
   gb = gb > g2 ? gb : g2;
+  if (d.P > 0) {  // dW_hr [P, H]
+    const size_t g3 = gemm_scratch_bytes(d.P, d.H, K);
+    gb = gb > g3 ? gb : g3;
+  }
   s->b_gemm = off;
   s->b_gemm_bytes = gb;
   off += align_up(gb / sizeof(float) + 1, ALIGN_F);
@@ -202,6 +226,10 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
   off += align_up(layernorm_bwd_scratch_floats(d.I), ALIGN_F);
   s->b_h0 = off;
   off += align_up((size_t)d.B * d.GH, ALIGN_F);
+  for (int k = 0; k < 2; ++k) {
+    s->b_dhp[k] = off;
+    if (d.P > 0 && k < d.D) off += align_up(d.TB * (size_t)d.P, ALIGN_F);
+  }
   s->b_total = off;
 
   s->order = s->f_total > s->b_total ? s->f_total : s->b_total;
@@ -298,6 +326,10 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     set_error("forward: null pointer argument");
     return B200RNN_ERR_INVALID;
   }
+  if (d.P > 0 && (y_pool || ln_gamma || wcache || prologue_ev || !y)) {
+    set_error("forward: the model-shell fusions (LayerNorm prologue, y_pool, weight cache) do not take proj_size");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   if (!y && save) {
     set_error("forward: the full output is needed by backward (h_{t-1} of every step): pass y as well as y_pool");
     return B200RNN_ERR_INVALID;
@@ -380,6 +412,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     rp.lengths = lengths;
     rp.order = order;
     rp.tf32 = tf32 ? 1 : 0;
+    rp.P = d.P;
     RecFwdLaunch rec;
     rc = plan_rec_fwd(rp, &rec);
     if (rc) return rc;
@@ -389,7 +422,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     // of the SMs; the GEMM runs as 4-CTA clusters in the cluster slots the recurrence leaves free. Otherwise GEMM and
     // recurrence run one after the other.
     const int gemm_clusters = rec.capacity - rec.nclusters;
-    const bool stream_xproj = d.D == 1 && tc_layer && rec.C == 4 && rec.one_wave() && 2 * rec.ctas() <= sms &&
+    const bool stream_xproj = d.D == 1 && d.P == 0 && tc_layer && rec.C == 4 && rec.one_wave() && 2 * rec.ctas() <= sms &&
                               gemm_clusters > 0;
     // ---- A operand of the tensor-core input projection (fp32, split on chip by the GEMM), shared by the directions:
     // the layer input itself when the GEMM can read it in place, else a dense copy in the GEMM's workspace
@@ -420,9 +453,9 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     if (l == 0 && prologue_ev) B200_CUDA_CHECK(cudaEventRecord(prologue_ev, st));
     ready_zeroed = false;
     for (int k = 0; k < d.D; ++k) {
-      const float* const* pp = params + (size_t)(l * d.D + k) * 4;
+      const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
       const float *w_ih = pp[0], *w_hh = pp[1], *b_ih = pp[2], *b_hh = pp[3];
-      if (!w_ih || !w_hh || !b_ih || !b_hh) {
+      if (!w_ih || !w_hh || !b_ih || !b_hh || (d.P > 0 && !pp[4])) {
         set_error("forward: null parameter pointer (layer %d dir %d)", l, k);
         return B200RNN_ERR_INVALID;
       }
@@ -462,6 +495,10 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       rp.b_hh[k] = b_hh;
       rp.gates[k] = gates;
       rp.extra[k] = save ? R + rl.extra[l][k] : nullptr;
+      if (d.P > 0) {
+        rp.w_hr[k] = pp[4];
+        rp.m[k] = save ? R + rl.m[l][k] : nullptr;
+      }
     }
     float* ylay = nullptr;
     if (l == d.L - 1) {
@@ -472,9 +509,9 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       rp.y = ylay;
       rp.y_st = (long long)d.B * d.DH; rp.y_sb = (long long)d.DH;
     }
-    rp.h_n = h_n + (size_t)l * d.D * d.B * d.H;
+    rp.h_n = h_n + (size_t)l * d.D * d.B * d.HO;
     rp.c_n = c_n ? c_n + (size_t)l * d.D * d.B * d.H : nullptr;
-    rp.h_0 = h_0 ? h_0 + (size_t)l * d.D * d.B * d.H : nullptr;
+    rp.h_0 = h_0 ? h_0 + (size_t)l * d.D * d.B * d.HO : nullptr;
     rp.c_0 = c_0 ? c_0 + (size_t)l * d.D * d.B * d.H : nullptr;
     rp.trace = g_trace;
     // Streamed, this launch directly follows the GEMM in the stream (nothing may be enqueued between them) and never
@@ -512,6 +549,10 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
                                       uint64_t* rng_state, const float* ln_gamma, const float* ln_beta, float ln_eps,
                                       float* y_pool, const int32_t* lengths, const void* wcache,
                                       void* prologue_done, void* stream_) {
+  if (desc && desc_proj(desc) != 0) {
+    set_error("forward_fused: the model-shell entry points do not take proj_size (use b200rnn_forward_hx)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
                       ln_gamma, ln_beta, ln_eps, y_pool, lengths, wcache, prologue_done, nullptr, nullptr, stream_);
 }
@@ -529,7 +570,8 @@ B200RNN_API int b200rnn_forward_hx(const b200rnn_desc* desc, const float* x, int
   if (d.B > 0 && d.T == 0 && h_n && h_0) {  // no step: the final state is the initial one
     cudaStream_t st = static_cast<cudaStream_t>(stream_);
     const size_t bytes = (size_t)d.L * d.D * d.B * d.H * sizeof(float);
-    B200_CUDA_CHECK(cudaMemcpyAsync(h_n, h_0, bytes, cudaMemcpyDeviceToDevice, st));
+    B200_CUDA_CHECK(cudaMemcpyAsync(h_n, h_0, (size_t)d.L * d.D * d.B * d.HO * sizeof(float), cudaMemcpyDeviceToDevice,
+                                    st));
     if (c_n) {
       if (c_0) B200_CUDA_CHECK(cudaMemcpyAsync(c_n, c_0, bytes, cudaMemcpyDeviceToDevice, st));
       else B200_CUDA_CHECK(cudaMemsetAsync(c_n, 0, bytes, st));
@@ -544,8 +586,8 @@ B200RNN_API int b200rnn_forward(const b200rnn_desc* desc, const float* x, int64_
                                 const float* const* params, float* y, int64_t ys_t, int64_t ys_b, float* h_n,
                                 float* c_n, void* reserve, void* scratch, uint64_t seed, uint64_t offset,
                                 uint64_t* rng_state, void* stream_) {
-  return b200rnn_forward_fused(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset,
-                               rng_state, nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr, stream_);
+  return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
+                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream_);
 }
 
 B200RNN_API int b200rnn_wcache_bytes(const b200rnn_desc* desc, size_t* bytes) {
@@ -554,6 +596,10 @@ B200RNN_API int b200rnn_wcache_bytes(const b200rnn_desc* desc, size_t* bytes) {
   if (rc) return rc;
   if (d.L > 8) {
     set_error("num_layers %d > 8 unsupported", d.L);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  if (d.P > 0) {
+    set_error("wcache_bytes: the weight cache of b200rnn_forward_fused does not take proj_size");
     return B200RNN_ERR_UNSUPPORTED;
   }
   WCacheLayout wl;
@@ -570,6 +616,10 @@ B200RNN_API int b200rnn_prepare_weights(const b200rnn_desc* desc, const float* c
   if (!params || !wcache || !aligned_to(wcache, 256) || d.L > 8) {
     set_error("prepare_weights: null / misaligned argument");
     return B200RNN_ERR_INVALID;
+  }
+  if (d.P > 0) {
+    set_error("prepare_weights: the weight cache of b200rnn_forward_fused does not take proj_size");
+    return B200RNN_ERR_UNSUPPORTED;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   WCacheLayout wl;
@@ -613,6 +663,10 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     set_error("backward: B200RNN_FLAG_FUSED_LN and ln_gamma must be given together (as in the forward)");
     return B200RNN_ERR_INVALID;
   }
+  if (d.P > 0 && (fused_ln || dy_pool || !dy)) {
+    set_error("backward: the model-shell fusions (LayerNorm, pooled gradient) do not take proj_size");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   if (fused_ln && (!(d.I == 128 || d.I == 256 || d.I == 512 || d.I == 1024) || !tc_available())) {
     set_error("backward: the fused LayerNorm needs input_size 128, 256, 512 or 1024");
     return B200RNN_ERR_UNSUPPORTED;
@@ -645,6 +699,7 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     RecBwdParams bp;
     memset(&bp, 0, sizeof(bp));
     bp.mode = d.mode; bp.B = d.B; bp.T = d.T; bp.H = d.H; bp.D = d.D;
+    bp.P = d.P;
     if (l == d.L - 1) {
       bp.y = y; bp.y_st = ys_t; bp.y_sb = ys_b;
       bp.dy = dy; bp.dy_st = dys_t; bp.dy_sb = dys_b;
@@ -653,16 +708,17 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
       bp.y = R + rl.ylayer[l]; bp.y_st = (long long)d.B * d.DH; bp.y_sb = (long long)d.DH;
       bp.dy = S + sl.b_dy; bp.dy_st = (long long)d.B * d.DH; bp.dy_sb = (long long)d.DH;
     }
-    const size_t lstate = (size_t)l * d.D * d.B * d.H;  // this layer's [D,B,H] slice of the [L*D,B,H] states
-    bp.dh_n = dh_n ? dh_n + lstate : nullptr;
+    const size_t lstate = (size_t)l * d.D * d.B * d.H;    // this layer's [D,B,H] slice of the [L*D,B,H] cell states
+    const size_t lhstate = (size_t)l * d.D * d.B * d.HO;  // ... and of the [L*D,B,HO] hidden states
+    bp.dh_n = dh_n ? dh_n + lhstate : nullptr;
     bp.dc_n = dc_n ? dc_n + lstate : nullptr;
-    bp.h_0 = h_0 ? h_0 + lstate : nullptr;
+    bp.h_0 = h_0 ? h_0 + lhstate : nullptr;
     bp.c_0 = c_0 ? c_0 + lstate : nullptr;
-    bp.dh_0 = dh_0 ? dh_0 + lstate : nullptr;
+    bp.dh_0 = dh_0 ? dh_0 + lhstate : nullptr;
     bp.dc_0 = dc_0 ? dc_0 + lstate : nullptr;
     for (int k = 0; k < d.D; ++k) {
-      const float* const* pp = params + (size_t)(l * d.D + k) * 4;
-      if (!pp[0] || !pp[1]) {
+      const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
+      if (!pp[0] || !pp[1] || (d.P > 0 && !pp[4])) {
         set_error("backward: null parameter pointer (layer %d dir %d)", l, k);
         return B200RNN_ERR_INVALID;
       }
@@ -673,6 +729,10 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
       bp.dgates[k] = S + sl.b_dgates[k];
       bp.dghn[k] = S + sl.b_dghn[k];
       bp.dbias_part[k] = S + sl.b_bpart[k];
+      if (d.P > 0) {
+        bp.w_hr[k] = pp[4];
+        bp.dhp[k] = S + sl.b_dhp[k];
+      }
     }
     bp.lengths = lengths;
     bp.order = order;
@@ -711,8 +771,8 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     }
     (void)ldk;
     for (int k = 0; k < d.D; ++k) {
-      const float* const* pp = params + (size_t)(l * d.D + k) * 4;
-      float* const* gp = dparams + (size_t)(l * d.D + k) * 4;
+      const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
+      float* const* gp = dparams + (size_t)(l * d.D + k) * d.NPAR;
       float *dw_ih = gp[0], *dw_hh = gp[1], *db_ih = gp[2], *db_hh = gp[3];
       const float* dG = S + sl.b_dgates[k];
       const float* dHN = S + sl.b_dghn[k];
@@ -727,7 +787,7 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
         const TcOperand opX{xS, lo(xS, d.TB * (size_t)Il), (long long)Il, true};
         // the tensor-core path needs 16-byte aligned outputs: a gradient target that is not 16-byte aligned (a view into a caller's
         // flat bucket behind an odd-sized tensor) takes the FFMA GEMM below instead of failing
-        const bool tc_wih = dw_ih && aligned_to(dw_ih, 16), tc_whh = dw_hh && aligned_to(dw_hh, 16) && d.T > 1;
+        const bool tc_wih = dw_ih && aligned_to(dw_ih, 16), tc_whh = dw_hh && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0;
         float* Cx = nullptr;
         RowMap cx_rows = simple_rows(1);
         bool tc_dx = false;
@@ -812,17 +872,17 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
         // forward direction: pairs (dG[t], y[t-1]) for t = 1..T-1 ; reverse: (dG[t], y[t+1]) for t = 0..T-2
         const size_t g_t0 = (k == 0) ? (size_t)d.B : 0;  // first dG row
         const long long y_t0 = (k == 0) ? 0 : bp.y_st;   // first y row offset (elements)
-        const float* hp = bp.y + y_t0 + (long long)k * d.H;
+        const float* hp = bp.y + y_t0 + (long long)k * d.HO;
         RowMap hp_rows = tb_rows(bp.y_st, bp.y_sb, d.B);
         GemmParams g;
         memset(&g, 0, sizeof(g));
         g.B = hp; g.b_rows = hp_rows; g.b_kcontig = 0;
-        g.N = d.H; g.K = Kp;
+        g.N = d.HO; g.K = Kp;
         g.accumulate = accumulate;
         g.a_kcontig = 0;
         if (d.mode == B200RNN_LSTM) {
           g.A = dG + g_t0 * d.GH; g.a_rows = simple_rows((long long)d.GH);
-          g.C = dw_hh; g.c_rows = simple_rows(d.H);
+          g.C = dw_hh; g.c_rows = simple_rows(d.HO);
           g.M = (int)d.GH;
           rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
           if (rc) return rc;
@@ -850,11 +910,22 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
         GemmParams g;
         memset(&g, 0, sizeof(g));
         g.A = rows0; g.a_rows = simple_rows((long long)d.GH); g.a_kcontig = 0;
-        g.B = bp.h_0 + (size_t)k * d.B * d.H; g.b_rows = simple_rows(d.H); g.b_kcontig = 0;
-        g.C = dw_hh; g.c_rows = simple_rows(d.H);
-        g.M = (int)d.GH; g.N = d.H; g.K = d.B;
+        g.B = bp.h_0 + (size_t)k * d.B * d.HO; g.b_rows = simple_rows(d.HO); g.b_kcontig = 0;
+        g.C = dw_hh; g.c_rows = simple_rows(d.HO);
+        g.M = (int)d.GH; g.N = d.HO; g.K = d.B;
         g.accumulate = 1;
         rc = launch_gemm(g, nullptr, 0, st);
+        if (rc) return rc;
+      }
+      if (d.P > 0 && gp[4]) {  // dW_hr[P, H] = sum_tb dh[tb, :]^T m[tb, :] (frozen and skipped steps have dh = 0)
+        GemmParams g;
+        memset(&g, 0, sizeof(g));
+        g.A = S + sl.b_dhp[k]; g.a_rows = simple_rows((long long)d.P); g.a_kcontig = 0;
+        g.B = R + rl.m[l][k]; g.b_rows = simple_rows((long long)d.H); g.b_kcontig = 0;
+        g.C = gp[4]; g.c_rows = simple_rows(d.H);
+        g.M = d.P; g.N = d.H; g.K = (int)d.TB;
+        g.accumulate = accumulate;
+        rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
         if (rc) return rc;
       }
       if (!done_dx) {  // dX_l (+)= dGi * W_ih
@@ -895,6 +966,10 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
                                        void* scratch, float* dx, int64_t dxs_t, int64_t dxs_b, float* const* dparams,
                                        const int32_t* lengths, const float* ln_gamma, float ln_eps, float* dln_gamma,
                                        float* dln_beta, void* stream_) {
+  if (desc && desc_proj(desc) != 0) {
+    set_error("backward_fused: the model-shell entry points do not take proj_size (use b200rnn_backward_hx)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, dy_pool, dy_pool_scale, dh_n,
                        dc_n, reserve, scratch, dx, dxs_t, dxs_b, dparams, lengths, ln_gamma, ln_eps, dln_gamma,
                        dln_beta, nullptr, nullptr, nullptr, nullptr, stream_);
@@ -917,13 +992,13 @@ B200RNN_API int b200rnn_backward_hx(const b200rnn_desc* desc, const float* x, in
   }
   if (d.B > 0 && d.T == 0) {  // no step: the gradients pass from the final state to the initial one
     cudaStream_t st = static_cast<cudaStream_t>(stream_);
-    const size_t bytes = (size_t)d.L * d.D * d.B * d.H * sizeof(float);
+    const size_t bytes[2] = {(size_t)d.L * d.D * d.B * d.HO * sizeof(float), (size_t)d.L * d.D * d.B * d.H * sizeof(float)};
     const float* src[2] = {dh_n, dc_n};
     float* dst[2] = {dh_0, dc_0};
     for (int i = 0; i < 2; ++i) {
       if (!dst[i]) continue;
-      if (src[i]) B200_CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], bytes, cudaMemcpyDeviceToDevice, st));
-      else B200_CUDA_CHECK(cudaMemsetAsync(dst[i], 0, bytes, st));
+      if (src[i]) B200_CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], bytes[i], cudaMemcpyDeviceToDevice, st));
+      else B200_CUDA_CHECK(cudaMemsetAsync(dst[i], 0, bytes[i], st));
     }
     return B200RNN_OK;
   }
@@ -941,9 +1016,9 @@ B200RNN_API int b200rnn_backward(const b200rnn_desc* desc, const float* x, int64
     set_error("backward: null pointer argument");
     return B200RNN_ERR_INVALID;
   }
-  return b200rnn_backward_fused(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, nullptr, 0.f, dh_n, dc_n,
-                                reserve, scratch, dx, dxs_t, dxs_b, dparams, lengths, nullptr, 0.f, nullptr, nullptr,
-                                stream_);
+  return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, nullptr, 0.f, dh_n, dc_n, reserve,
+                       scratch, dx, dxs_t, dxs_b, dparams, lengths, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr,
+                       nullptr, nullptr, stream_);
 }
 
 B200RNN_API int b200rnn_gemm_f32(int M, int N, int K, const float* A, int64_t lda, int a_kcontig, const float* B,

@@ -32,6 +32,11 @@ struct RecFwdParams {
                              // other config is fp32 FFMA and ignores it
   const float* h_0;          // optional [D,B,H] initial state of this layer, caller's row order (NULL: zeros)
   const float* c_0;          // optional [D,B,H] initial cell state (LSTM; NULL: zeros)
+  // LSTM with a projection (rec_fwd_proj_kernel): P = proj_size, 0 = none. Then y, h_n and h_0 are P wide (y column
+  // d*P + p), w_hh is [G*H, P], and m (training) receives o * tanh(c), the operand of the dW_hr GEMM
+  int P;
+  const float* w_hr[2];      // per direction [P, H]
+  float* m[2];               // per direction [T,B,H] (training only)
 };
 
 // A recurrence launch chosen for a shape, before anything is enqueued: `nclusters` clusters of C CTAs, of which
@@ -70,6 +75,11 @@ struct RecBwdParams {
   const float* c_0;          // the forward's initial cell state [D,B,H] or NULL (LSTM)
   float* dh_0;               // out, optional [D,B,H]: gradient w.r.t. h_0 (NULL: the last step's contraction is skipped)
   float* dc_0;               // out, optional [D,B,H]: gradient w.r.t. c_0 (LSTM)
+  // LSTM with a projection (rec_bwd_proj_kernel): P = proj_size, 0 = none. Then dy, dh_n and dh_0 are P wide, w_hh is
+  // read as it lies ([G*H, P]; w_prep unused), and dhp receives dh_t (dy_t plus the recurrent part), dW_hr's operand
+  int P;
+  const float* w_hr[2];      // per direction [P, H]
+  float* dhp[2];             // out: per direction [T,B,P]
 };
 
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)

@@ -998,6 +998,451 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 }
 
 // =================================================================================================
+// LSTM with a projection (proj_size P > 0): forward and BPTT
+// =================================================================================================
+// h_t = W_hr (o_t * tanh c_t), h_t of width P < H. A cluster of C CTAs owns BS batch rows, CTA `rank` owns HS = H/C cell
+// units and keeps on chip, for the whole sequence:
+//   W_s [G*HS][P]: the W_hh rows of its units (row g*HS + u = W_hh[g*H + j0 + u][:]), K = P;
+//   R_s [HS][P]:   the W_hr columns of its units, transposed (R_s[u][p] = W_hr[p][j0 + u]).
+// Rows are padded to P + 4 floats, so that the 8 units a quarter-warp reads with one 16-byte load sit in different banks.
+// One thread per (unit u, batch slot b): NT = HS * BS. Forward step:
+//   1. gate pre-activations W_s h_{t-1} for its 4 rows, cell update, m = o * tanh(c) into m_s[b][u];
+//   2. the CTA's partial projection h^(r)[b][:] = R_s^T m_s[b] (all P outputs from its HS units);
+//   3. the partial goes to every peer's slot [rank] (st.async, one mbarrier per source and buffer, double buffered);
+//   4. next step, every CTA adds the C partials in rank order 0..C-1: all CTAs hold the same bits of h_t, which is the
+//      next contraction's operand; CTA r writes its P/C columns of y and h_n.
+// One exchange per step, as in the unprojected kernels, with P-wide partials instead of HS-wide state slices. BPTT
+// mirrors it: dh_t = dy_t + (the C partials of W_hh^T dgates, in rank order), dm = W_hr[:, units]^T dh_t, the LSTM cell
+// backward from dm, and the CTA's partial W_hh[units]^T dgates goes to the peers. dh_t is written to `dhp` for the
+// dW_hr GEMM. Ragged batches (VL) as in the other kernels: a frozen step keeps (h, c) and emits 0; in BPTT its dh passes
+// through (rank 0 carries it in its partial, the others add zeros, so the sum is exact).
+template <int H, int P, int C, int BS>
+struct ProjCfg {
+  static constexpr int G = 4, HS = H / C, NT = HS * BS;
+  static constexpr int LD = P + 4;  // padded row of W_s / R_s
+  static constexpr int NG = (NT / P < BS) ? NT / P : BS;  // batch groups of the P-wide partial contraction
+  static constexpr int RB = BS / NG;                     // batch rows per thread in it
+  static constexpr size_t W_FLOATS = (size_t)G * HS * LD, R_FLOATS = (size_t)HS * LD;
+  static constexpr size_t V_FLOATS = (size_t)BS * P, SLOT_FLOATS = (size_t)2 * C * BS * P;
+  static constexpr size_t SMEM_F = (W_FLOATS + R_FLOATS + V_FLOATS + SLOT_FLOATS + (size_t)BS * HS) * sizeof(float) +
+                                   2 * C * sizeof(uint64_t) + 2 * BS * sizeof(int);
+  static constexpr size_t SMEM_B = (W_FLOATS + R_FLOATS + V_FLOATS + SLOT_FLOATS + (size_t)BS * G * HS) * sizeof(float) +
+                                   2 * C * sizeof(uint64_t) + 2 * BS * sizeof(int);
+  static_assert(HS * C == H && HS % 8 == 0 && P % (4 * C) == 0 && P % 4 == 0, "bad split");
+  static_assert(NT % 32 == 0 && NT <= 1024 && NG >= 1 && NG * RB == BS && NT >= P, "bad thread count");
+};
+
+// Thread (unit, batch slot) of the projected kernels: 8 consecutive units by 4 batch slots per warp
+template <int BS>
+__device__ __forceinline__ void proj_thread(int tid, int& u, int& b) {
+  u = (tid & 7) + 8 * (tid / (8 * BS));
+  b = (tid >> 3) % BS;
+}
+
+// Stage this CTA's W_hh rows and W_hr columns (once per launch), the row / length of every batch slot
+template <int H, int P, int C, int BS, bool VL>
+__device__ __forceinline__ void proj_prologue(const float* __restrict__ w_hh, const float* __restrict__ w_hr, int j0,
+                                              int b0, int B, int T, const int* lengths, const int* order, float* W_s,
+                                              float* R_s, int* row_s, int* len_s, int tid) {
+  using Cfg = ProjCfg<H, P, C, BS>;
+  constexpr int G = Cfg::G, HS = Cfg::HS, NT = Cfg::NT, LD = Cfg::LD;
+  for (int i = tid; i < G * HS * P / 4; i += NT) {
+    const int r = i / (P / 4), k = (i % (P / 4)) * 4;
+    const int g = r / HS, u = r - g * HS;
+    *reinterpret_cast<float4*>(&W_s[r * LD + k]) =
+        __ldg(reinterpret_cast<const float4*>(w_hh + ((size_t)g * H + j0 + u) * P + k));
+  }
+  for (int i = tid; i < P * HS; i += NT) {
+    const int pp = i / HS, u = i - pp * HS;
+    R_s[u * LD + pp] = __ldg(w_hr + (size_t)pp * H + j0 + u);
+  }
+  if (tid < BS) {
+    const int slot = b0 + tid;
+    const bool valid = slot < B;
+    const int row = (VL && valid) ? order[slot] : slot;
+    row_s[tid] = valid ? row : -1;
+    len_s[tid] = (VL && valid) ? min(max(lengths[row], 0), T) : T;
+  }
+}
+
+// Send this CTA's partial (own slot, written and published by __syncthreads) to the C-1 peers' slot [rank]
+template <int P, int C, int BS, int NT>
+__device__ __forceinline__ void proj_send(float* own, uint64_t* bar, uint32_t rank, int tid) {
+  constexpr int NV = BS * P / 4;
+  const uint32_t bar_addr = ptx::smem_u32(bar);
+  for (int i = tid; i < (C - 1) * NV; i += NT) {
+    const int r = i / NV, v = i - r * NV;
+    const uint32_t peer = (rank + 1 + r) % C;
+    float* src = own + v * 4;
+    ptx::st_async_v4(ptx::mapa(ptx::smem_u32(src), peer), *reinterpret_cast<const float4*>(src),
+                     ptx::mapa(bar_addr, peer));
+  }
+}
+
+// Partial P-wide contraction of the CTA's K values per batch row: out[b][pp] = sum_k A[k * LD + pp] * v[b][k], k in
+// increasing order (one FMA chain per output: deterministic). Threads (pp, batch group) of NG groups of RB rows.
+template <int P, int BS, int NG, int RB, int K>
+__device__ __forceinline__ void proj_partial(const float* __restrict__ A, int ld, const float* __restrict__ v,
+                                             float* __restrict__ out, int tid) {
+  if (tid >= P * NG) return;
+  const int pp = tid % P, bg = tid / P;
+  float acc[RB];
+#pragma unroll
+  for (int r = 0; r < RB; ++r) acc[r] = 0.f;
+#pragma unroll 4
+  for (int k = 0; k < K; k += 4) {
+    const float a0 = A[(k + 0) * ld + pp], a1 = A[(k + 1) * ld + pp], a2 = A[(k + 2) * ld + pp],
+                a3 = A[(k + 3) * ld + pp];
+#pragma unroll
+    for (int r = 0; r < RB; ++r) {
+      const float4 x = *reinterpret_cast<const float4*>(&v[(bg * RB + r) * K + k]);
+      float a = acc[r];
+      a = fmaf(a0, x.x, a);
+      a = fmaf(a1, x.y, a);
+      a = fmaf(a2, x.z, a);
+      a = fmaf(a3, x.w, a);
+      acc[r] = a;
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < RB; ++r) out[(bg * RB + r) * P + pp] = acc[r];
+}
+
+template <int H, int P, int C, int BS, bool VL>
+__global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
+    rec_fwd_proj_kernel(const RecFwdParams p, const int nslices) {
+  using Cfg = ProjCfg<H, P, C, BS>;
+  constexpr int G = Cfg::G, HS = Cfg::HS, NT = Cfg::NT, LD = Cfg::LD, PC = P / C;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  float* W_s = reinterpret_cast<float*>(smem_raw);  // [G*HS][LD]
+  float* R_s = W_s + Cfg::W_FLOATS;                 // [HS][LD]
+  float* h_s = R_s + Cfg::R_FLOATS;                 // [BS][P] h_{t-1}
+  float* slot = h_s + Cfg::V_FLOATS;                // [2][C][BS][P] partial projections
+  float* m_s = slot + Cfg::SLOT_FLOATS;             // [BS][HS]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(m_s + BS * HS);  // [buf * C + src]
+  int* row_s = reinterpret_cast<int*>(bars + 2 * C);            // [BS] batch row of each slot (-1: past the batch)
+  int* len_s = row_s + BS;                                      // [BS] steps of each slot
+
+  const int tid = threadIdx.x;
+  const uint32_t rank = ptx::cluster_ctarank();
+  const int cid = blockIdx.x / C;
+  const int dir = cid / nslices;
+  const int slice = cid - dir * nslices;
+  const int b0 = slice * BS;
+  const int j0 = (int)rank * HS;
+  const int B = p.B;
+  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
+
+  if (tid == 0) {
+    for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], 1u);
+    ptx::fence_mbar_init();
+  }
+  proj_prologue<H, P, C, BS, VL>(p.w_hh[dir], p.w_hr[dir], j0, b0, B, p.T, p.lengths, p.order, W_s, R_s, row_s, len_s,
+                                 tid);
+  __syncthreads();
+  for (int i = tid; i < BS * P; i += NT) {  // h_0 of the cluster's batch slots (zeros past the batch or without h_0)
+    const int q = i / P, k = i - q * P;
+    h_s[i] = (p.h_0 && row_s[q] >= 0) ? p.h_0[((size_t)dir * B + row_s[q]) * P + k] : 0.f;
+  }
+  __syncthreads();
+  ptx::cluster_sync_all();  // peers' barriers are initialised before anyone sends
+
+  int u, b;
+  proj_thread<BS>(tid, u, b);
+  const int j = j0 + u;
+  const int row = row_s[b];
+  const bool valid = row >= 0;
+  const int len = len_s[b];
+  float* gates = p.gates[dir];
+  float c = (p.c_0 && valid) ? p.c_0[((size_t)dir * B + row) * H + j] : 0.f;
+  float gi[G];
+  auto load_gi = [&](int t) {
+#pragma unroll
+    for (int g = 0; g < G; ++g) gi[g] = valid ? gates[((size_t)t * B + row) * (G * H) + g * H + j] : 0.f;
+  };
+  if (T > 0) load_gi(dir ? T - 1 : 0);
+
+  for (int step = 0; step <= T; ++step) {
+    // ---- h of the previous step: the C partials in rank order; this CTA's columns of y --------------------------
+    if (step > 0) {
+      const int cur = step & 1;
+      const int tp = dir ? T - step : step - 1;
+      const uint32_t par = ((step - 1) >> 1) & 1;
+#pragma unroll
+      for (int src = 0; src < C; ++src)
+        if ((uint32_t)src != rank) ptx::mbar_wait(&bars[cur * C + src], par);
+      const float* sl = slot + (size_t)cur * C * BS * P;
+      for (int i = tid; i < BS * P; i += NT) {
+        const int q = i / P, k = i - q * P;
+        float v = sl[i];
+#pragma unroll
+        for (int src = 1; src < C; ++src) v += sl[src * BS * P + i];
+        const bool frozen = VL && tp >= len_s[q];
+        if (!frozen) h_s[i] = v;
+        if (k / PC == (int)rank && row_s[q] >= 0 && p.y)
+          p.y[(long long)tp * p.y_st + (long long)row_s[q] * p.y_sb + dir * P + k] = frozen ? 0.f : v;
+      }
+      __syncthreads();
+    }
+    if (step == T) break;
+    const int t = dir ? T - 1 - step : step;
+    const int nb = (step + 1) & 1;
+    if (tid == 0) {  // this step's partials land in buffer nb; its previous phase was consumed at step - 1
+#pragma unroll
+      for (int src = 0; src < C; ++src)
+        if ((uint32_t)src != rank) ptx::mbar_arrive_expect_tx(&bars[nb * C + src], (uint32_t)(BS * P * sizeof(float)));
+    }
+    // ---- gates, cell, m = o * tanh(c) ----------------------------------------------------------------------------
+    float acc[G];
+#pragma unroll
+    for (int g = 0; g < G; ++g) acc[g] = 0.f;
+#pragma unroll 4
+    for (int k = 0; k < P; k += 4) {
+      const float4 hv = *reinterpret_cast<const float4*>(&h_s[b * P + k]);
+#pragma unroll
+      for (int g = 0; g < G; ++g) {
+        const float4 wv = *reinterpret_cast<const float4*>(&W_s[(g * HS + u) * LD + k]);
+        float a = acc[g];
+        a = fmaf(wv.x, hv.x, a);
+        a = fmaf(wv.y, hv.y, a);
+        a = fmaf(wv.z, hv.z, a);
+        a = fmaf(wv.w, hv.w, a);
+        acc[g] = a;
+      }
+    }
+    const float ig = sigmoid_f(gi[0] + acc[0]);
+    const float fg = sigmoid_f(gi[1] + acc[1]);
+    const float gg = tanh_f(gi[2] + acc[2]);
+    const float og = sigmoid_f(gi[3] + acc[3]);
+    float cnew = fmaf(fg, c, ig * gg);
+    float m = og * tanh_f(cnew);
+    if (VL && t >= len) {
+      cnew = c;
+      m = 0.f;
+    }
+    c = cnew;
+    m_s[b * HS + u] = valid ? m : 0.f;
+    if (valid && p.training) {
+      float* gp = gates + ((size_t)t * B + row) * (G * H) + j;
+      gp[0] = ig; gp[H] = fg; gp[2 * H] = gg; gp[3 * H] = og;
+      p.extra[dir][((size_t)t * B + row) * H + j] = cnew;
+      p.m[dir][((size_t)t * B + row) * H + j] = m;
+    }
+    if (step + 1 < T) load_gi(dir ? T - 2 - step : step + 1);
+    __syncthreads();
+    // ---- this CTA's partial projection into its own slot, then to the peers --------------------------------------
+    float* own = slot + ((size_t)nb * C + rank) * BS * P;
+    proj_partial<P, BS, Cfg::NG, Cfg::RB, HS>(R_s, LD, m_s, own, tid);
+    __syncthreads();
+    proj_send<P, C, BS, NT>(own, &bars[nb * C + rank], rank, tid);
+  }
+  // ---- final state: h_n (this CTA's columns of h_s) and c_n; VL: the steps [T, p.T) the cluster skipped ----------
+  for (int i = tid; i < BS * P; i += NT) {
+    const int q = i / P, k = i - q * P;
+    if (k / PC == (int)rank && row_s[q] >= 0) {
+      p.h_n[((size_t)dir * B + row_s[q]) * P + k] = h_s[i];
+      if (VL && p.y)
+        for (int t = T; t < p.T; ++t) p.y[(long long)t * p.y_st + (long long)row_s[q] * p.y_sb + dir * P + k] = 0.f;
+    }
+  }
+  if (valid) {
+    if (p.c_n) p.c_n[((size_t)dir * B + row) * H + j] = c;
+    if (VL && p.training)  // the dW_hr GEMM reads m of every step
+      for (int t = T; t < p.T; ++t) p.m[dir][((size_t)t * B + row) * H + j] = 0.f;
+  }
+  ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
+}
+
+template <int H, int P, int C, int BS, bool VL>
+__global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
+    rec_bwd_proj_kernel(const RecBwdParams p, const int nslices) {
+  using Cfg = ProjCfg<H, P, C, BS>;
+  constexpr int G = Cfg::G, HS = Cfg::HS, NT = Cfg::NT, LD = Cfg::LD, PC = P / C;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  float* W_s = reinterpret_cast<float*>(smem_raw);  // [G*HS][LD]
+  float* R_s = W_s + Cfg::W_FLOATS;                 // [HS][LD]
+  float* dh_s = R_s + Cfg::R_FLOATS;                // [BS][P] dh_t
+  float* slot = dh_s + Cfg::V_FLOATS;               // [2][C][BS][P] partials of W_hh^T dgates
+  float* dg_s = slot + Cfg::SLOT_FLOATS;            // [BS][G*HS] this CTA's gate gradients
+  uint64_t* bars = reinterpret_cast<uint64_t*>(dg_s + BS * G * HS);
+  int* row_s = reinterpret_cast<int*>(bars + 2 * C);
+  int* len_s = row_s + BS;
+
+  const int tid = threadIdx.x;
+  const uint32_t rank = ptx::cluster_ctarank();
+  const int cid = blockIdx.x / C;
+  const int dir = cid / nslices;
+  const int slice = cid - dir * nslices;
+  const int b0 = slice * BS;
+  const int j0 = (int)rank * HS;
+  const int B = p.B;
+  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;
+
+  if (tid == 0) {
+    for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], 1u);
+    ptx::fence_mbar_init();
+  }
+  proj_prologue<H, P, C, BS, VL>(p.w_hh[dir], p.w_hr[dir], j0, b0, B, p.T, p.lengths, p.order, W_s, R_s, row_s, len_s,
+                                 tid);
+  __syncthreads();
+  ptx::cluster_sync_all();
+
+  int u, b;
+  proj_thread<BS>(tid, u, b);
+  const int j = j0 + u;
+  const int row = row_s[b];
+  const bool valid = row >= 0;
+  const int len = len_s[b];
+  const float* gates = p.gates[dir];
+  const float* extra = p.extra[dir];
+  float* dgates = p.dgates[dir];
+  float* dhp = p.dhp[dir];
+  float dc_carry = (valid && p.dc_n) ? p.dc_n[((size_t)dir * B + row) * H + j] : 0.f;
+  float bsum[G];
+#pragma unroll
+  for (int g = 0; g < G; ++g) bsum[g] = 0.f;
+  float sv[G] = {0.f, 0.f, 0.f, 0.f}, sx = 0.f, cp = 0.f;  // saved gates, c_t, c_{t-1} of the current step (prefetched)
+  auto load_step = [&](int step) {
+    const int t = dir ? step : (T - 1 - step);
+    const int tp = dir ? t + 1 : t - 1;
+    const size_t o = ((size_t)t * B + row) * H + j;
+#pragma unroll
+    for (int g = 0; g < G; ++g) sv[g] = gates[((size_t)t * B + row) * (G * H) + g * H + j];
+    sx = extra[o];
+    if (step < T - 1)
+      cp = extra[((size_t)tp * B + row) * H + j];
+    else
+      cp = p.c_0 ? p.c_0[((size_t)dir * B + row) * H + j] : 0.f;
+  };
+  if (valid && T > 0) load_step(0);
+
+  for (int step = 0; step <= T; ++step) {
+    // ---- dh_t = dy_t + the C partials (rank order); dh_n enters at the first step, dh_0 leaves after the last ----
+    const int cur = step & 1;
+    if (step > 0) {
+      const uint32_t par = ((step - 1) >> 1) & 1;
+#pragma unroll
+      for (int src = 0; src < C; ++src)
+        if ((uint32_t)src != rank) ptx::mbar_wait(&bars[cur * C + src], par);
+    }
+    const int t = dir ? step : (T - 1 - step);
+    const float* sl = slot + (size_t)cur * C * BS * P;
+    for (int i = tid; i < BS * P; i += NT) {
+      const int q = i / P, k = i - q * P;
+      const int r = row_s[q];
+      float rec;
+      if (step == 0) {
+        rec = (p.dh_n && r >= 0) ? p.dh_n[((size_t)dir * B + r) * P + k] : 0.f;
+      } else {
+        rec = sl[i];
+#pragma unroll
+        for (int src = 1; src < C; ++src) rec += sl[src * BS * P + i];
+      }
+      const bool mine = k / PC == (int)rank && r >= 0;
+      if (step < T) {
+        const bool frozen = VL && t >= len_s[q];
+        float v = rec;
+        if (!frozen && r >= 0 && p.dy) v = p.dy[(long long)t * p.dy_st + (long long)r * p.dy_sb + dir * P + k] + rec;
+        dh_s[i] = v;
+        if (mine) dhp[((size_t)t * B + r) * P + k] = frozen ? 0.f : v;
+      } else if (mine && p.dh_0) {
+        p.dh_0[((size_t)dir * B + r) * P + k] = rec;
+      }
+    }
+    __syncthreads();
+    if (step == T) break;
+    const int nb = (step + 1) & 1;
+    if (tid == 0) {
+#pragma unroll
+      for (int src = 0; src < C; ++src)
+        if ((uint32_t)src != rank) ptx::mbar_arrive_expect_tx(&bars[nb * C + src], (uint32_t)(BS * P * sizeof(float)));
+    }
+    // ---- dm = W_hr[:, j]^T dh_t, then the LSTM cell backward from dm ---------------------------------------------
+    float dm = 0.f;
+#pragma unroll 4
+    for (int k = 0; k < P; k += 4) {
+      const float4 wv = *reinterpret_cast<const float4*>(&R_s[u * LD + k]);
+      const float4 dv = *reinterpret_cast<const float4*>(&dh_s[b * P + k]);
+      dm = fmaf(wv.x, dv.x, dm);
+      dm = fmaf(wv.y, dv.y, dm);
+      dm = fmaf(wv.z, dv.z, dm);
+      dm = fmaf(wv.w, dv.w, dm);
+    }
+    const bool frozen = VL && t >= len;
+    float dg[G];
+    {
+      const float ig = sv[0], fg = sv[1], gg = sv[2], og = sv[3];
+      const float tc = tanh_f(sx);
+      const float dout = dm * tc * og * (1.f - og);
+      const float dc = dc_carry + dm * og * (1.f - tc * tc);
+      dg[0] = dc * gg * ig * (1.f - ig);
+      dg[1] = dc * cp * fg * (1.f - fg);
+      dg[2] = dc * ig * (1.f - gg * gg);
+      dg[3] = dout;
+      if (!frozen) dc_carry = dc * fg;  // frozen step: dc passes through
+    }
+    if (frozen || !valid) {
+#pragma unroll
+      for (int g = 0; g < G; ++g) dg[g] = 0.f;
+    }
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      dg_s[b * G * HS + g * HS + u] = dg[g];
+      bsum[g] += dg[g];
+    }
+    if (valid) {
+      float* gp = dgates + ((size_t)t * B + row) * (G * H) + j;
+#pragma unroll
+      for (int g = 0; g < G; ++g) gp[g * H] = dg[g];
+    }
+    if (valid && step + 1 < T) load_step(step + 1);
+    __syncthreads();
+    // ---- partial W_hh[units]^T dgates into the own slot (frozen rows: rank 0 carries dh_t), then to the peers ------
+    float* own = slot + ((size_t)nb * C + rank) * BS * P;
+    proj_partial<P, BS, Cfg::NG, Cfg::RB, G * HS>(W_s, LD, dg_s, own, tid);
+    if constexpr (VL) {
+      __syncthreads();
+      for (int i = tid; i < BS * P; i += NT) {
+        const int q = i / P;
+        if (t >= len_s[q]) own[i] = rank == 0 ? dh_s[i] : 0.f;
+      }
+    }
+    __syncthreads();
+    proj_send<P, C, BS, NT>(own, &bars[nb * C + rank], rank, tid);
+  }
+  if (valid && p.dc_0) p.dc_0[((size_t)dir * B + row) * H + j] = dc_carry;
+  if constexpr (VL) {  // the steps [T, p.T) the cluster skipped: no gate gradient, no dh
+    if (valid)
+      for (int t = T; t < p.T; ++t) {
+        float* gp = dgates + ((size_t)t * B + row) * (G * H) + j;
+#pragma unroll
+        for (int g = 0; g < G; ++g) gp[g * H] = 0.f;
+      }
+    for (int i = tid; i < BS * P; i += NT) {
+      const int q = i / P, k = i - q * P;
+      if (k / PC == (int)rank && row_s[q] >= 0)
+        for (int t = T; t < p.T; ++t) dhp[((size_t)t * B + row_s[q]) * P + k] = 0.f;
+    }
+  }
+  // ---- per-slice bias-gradient partials: sum over the slice's batch slots in slot order -------------------------
+  __syncthreads();
+#pragma unroll
+  for (int g = 0; g < G; ++g) dg_s[b * G * HS + g * HS + u] = bsum[g];
+  __syncthreads();
+  if (b == 0) {
+    float* out = p.dbias_part[dir] + (size_t)slice * (G + 1) * H;
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      float v = 0.f;
+      for (int q = 0; q < BS; ++q) v += dg_s[q * G * HS + g * HS + u];
+      out[g * H + j] = v;
+    }
+    out[G * H + j] = 0.f;
+  }
+  ptx::cluster_sync_all();
+}
+
+// =================================================================================================
 // launchers
 // =================================================================================================
 // Launch config of `nclusters` clusters of C CTAs; `attr` is the storage of the attributes it points to: the cluster
@@ -1128,6 +1573,51 @@ bool try_bwd(RecBwdParams& p, cudaStream_t s, bool force, int* rc) {
   return true;
 }
 
+// LSTM with a projection: one config per (H, P), several waves when its clusters do not all fit
+template <int H, int P, int C, int BS>
+int pick_fwd_proj(const RecFwdParams& p, RecFwdLaunch* L) {
+  using Cfg = ProjCfg<H, P, C, BS>;
+  static_assert(Cfg::SMEM_F <= MAX_SMEM, "projected forward config does not fit an SM");
+  auto k = p.lengths ? rec_fwd_proj_kernel<H, P, C, BS, true> : rec_fwd_proj_kernel<H, P, C, BS, false>;
+  int rc = B200RNN_OK;
+  pick_clustered(k, p, C, BS, Cfg::NT, Cfg::SMEM_F, true, L, &rc, "fwd proj cfg C=%d BS=%d P=%d", C, BS, P);
+  return rc;
+}
+
+template <int H, int P, int C, int BS>
+int launch_bwd_proj(RecBwdParams& p, cudaStream_t s) {
+  using Cfg = ProjCfg<H, P, C, BS>;
+  static_assert(Cfg::SMEM_B <= MAX_SMEM, "projected backward config does not fit an SM");
+  auto k = p.lengths ? rec_bwd_proj_kernel<H, P, C, BS, true> : rec_bwd_proj_kernel<H, P, C, BS, false>;
+  ClusterLaunch<RecBwdParams> L;
+  int rc = B200RNN_OK;
+  pick_clustered(k, p, C, BS, Cfg::NT, Cfg::SMEM_B, true, &L, &rc, "bwd proj cfg C=%d BS=%d P=%d", C, BS, P);
+  if (rc != B200RNN_OK) return rc;
+  p.nslices_out = L.nslices;
+  return launch_clustered(L, p, PROF_REC_BWD, false, s);
+}
+
+// Template arguments <H, P, C, BS>: H = 128 on 2-CTA clusters of 4 batch rows (256 threads), H = 256 on 4-CTA clusters
+// of 8 batch rows (512 threads)
+int plan_rec_fwd_proj(const RecFwdParams& p, RecFwdLaunch* L) {
+  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 32) return pick_fwd_proj<128, 32, 2, 4>(p, L);
+  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 64) return pick_fwd_proj<128, 64, 2, 4>(p, L);
+  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 64) return pick_fwd_proj<256, 64, 4, 8>(p, L);
+  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 128) return pick_fwd_proj<256, 128, 4, 8>(p, L);
+  set_error("recurrence: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d); built for the LSTM with "
+            "proj_size hidden_size/4 or hidden_size/2", p.mode, p.H, p.P);
+  return B200RNN_ERR_UNSUPPORTED;
+}
+
+int launch_rec_bwd_proj(RecBwdParams& p, cudaStream_t s) {
+  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 32) return launch_bwd_proj<128, 32, 2, 4>(p, s);
+  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 64) return launch_bwd_proj<128, 64, 2, 4>(p, s);
+  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 64) return launch_bwd_proj<256, 64, 4, 8>(p, s);
+  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 128) return launch_bwd_proj<256, 128, 4, 8>(p, s);
+  set_error("recurrence backward: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d)", p.mode, p.H, p.P);
+  return B200RNN_ERR_UNSUPPORTED;
+}
+
 }  // namespace
 
 // smallest BS any backward config uses is 2
@@ -1140,6 +1630,7 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
   int rc = B200RNN_OK;
   L->kernel = nullptr;
   if (p.B <= 0 || p.T <= 0) return rc;
+  if (p.P > 0) return plan_rec_fwd_proj(p, L);
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
   if (p.mode == B200RNN_GRU && p.H == 256) {
@@ -1190,6 +1681,7 @@ int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s)
 int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
   int rc = B200RNN_OK;
   if (p.B <= 0 || p.T <= 0) return rc;
+  if (p.P > 0) return launch_rec_bwd_proj(p, s);
   // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
   // (not the weights) dominates the shared-memory traffic of the backward contraction
   if (p.mode == B200RNN_GRU && p.H == 256) {

@@ -55,6 +55,9 @@ enum {
 #define B200RNN_FLAG_FUSED_LN 4u          /* the LayerNorm prologue is part of the differentiated graph: the forward keeps
                                              LN(x) in `reserve`, b200rnn_backward_fused runs the LayerNorm backward.
                                              Must be set identically for workspace_bytes / forward_fused / backward_fused */
+#define B200RNN_FLAG_PROJ 16u             /* the descriptor carries `proj_size` (LSTM with projections). Without this flag the
+                                             library never reads that field, so a descriptor that ends at `flags` (built
+                                             before the field existed) keeps its meaning: no projection. */
 #define B200RNN_FLAG_TF32 8u              /* single-pass TF32 instead of 3xTF32 on the tensor cores: the input-projection,
                                              weight-gradient and input-gradient GEMMs and the GRU-256 tc8 recurrence
                                              round their operands to TF32 (round to nearest, ties away from zero) and
@@ -78,6 +81,13 @@ typedef struct b200rnn_desc {
   int32_t training;    /* 1: module is in train() mode => inter-layer dropout is applied      */
   float dropout_p;     /* inter-layer dropout probability (rnn.py:857-860 / 1233-1236)       */
   uint32_t flags;      /* B200RNN_FLAG_*                                                    */
+  int32_t proj_size;   /* P, read only with B200RNN_FLAG_PROJ: LSTM with projections (rnn.py LSTM proj_size), 0 = none.
+                          Supported: H/4 and H/2.
+                          Then params / dparams hold 5 pointers per (layer, direction), in nn order: weight_ih
+                          [4H, I_l], weight_hh [4H, P], bias_ih, bias_hh, weight_hr [P, H]; I_l = D*P for l > 0;
+                          y is [T, B, D*P], h_0 / h_n / dh_0 / dh_n are [L*D, B, P], c_0 / c_n stay [L*D, B, H].
+                          Only the plain and the _hx entry points take it (the _fused ones and the weight cache
+                          return B200RNN_ERR_UNSUPPORTED).                                                         */
 } b200rnn_desc;
 
 /* ABI version of the loaded library (== B200RNN_ABI_VERSION). */
