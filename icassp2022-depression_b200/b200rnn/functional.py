@@ -92,6 +92,24 @@ def _on(device):
     return torch.cuda.device(device)
 
 
+def _weight_grad_targets(weights, needed, sink, dev):
+    """Where a backward writes the weight gradients, as ``(dptrs, grads_out, accumulate)``: straight into the views
+    ``sink(weights)`` returns (a flat all-reduce bucket; the kernels accumulate into them, ``grads_out`` is all None),
+    or into one fresh flat buffer whose views are returned to autograd. ``needed[i]``: whether ``weights[i]`` wants a
+    gradient (a NULL target otherwise). Each fresh view starts on a 64-float (256-byte) boundary."""
+    if sink is not None:
+        targets = sink(weights)  # list of tensors (same shapes) or None entries
+        dptrs = [t.data_ptr() if (t is not None and n) else None for t, n in zip(targets, needed)]
+        return dptrs, [None] * len(weights), True
+    sizes = [(w.numel() + 63) // 64 * 64 if n else 0 for w, n in zip(weights, needed)]
+    flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
+    grads_out, off = [], 0
+    for w, n, size in zip(weights, needed, sizes):
+        grads_out.append(flat[off:off + w.numel()].view_as(w) if n else None)
+        off += size
+    return [g.data_ptr() if g is not None else None for g in grads_out], grads_out, False
+
+
 class _RNNFunction(torch.autograd.Function):
     """y, h_n[, c_n] = RNN(x, weights, h_0[, c_0]); x is the logical time-major view [T,B,I], h_0 / c_0 are None
     (zeros) or contiguous [L*D,B,HO] / [L*D,B,H] (HO = proj_size, or H without a projection). A projected LSTM always
@@ -189,29 +207,7 @@ class _RNNFunction(torch.autograd.Function):
         if dx is not None and dx.stride(2) != 1 and dx.size(2) != 1:
             dx = torch.empty(x_tm.shape, dtype=torch.float32, device=dev)
 
-        # weight gradients: either straight into caller-provided views (a flat all-reduce bucket) or into one
-        # fresh flat buffer that is returned to autograd as views
-        sink = ctx.grad_sink
-        w_needed = [ctx.needs_input_grad[w0 + i] for i in range(len(weights))]
-        grads_out: list = [None] * len(weights)
-        accumulate = False
-        if sink is not None:
-            targets = sink(weights)  # list of tensors (same shapes) or None entries
-            accumulate = True
-            dptrs = [t.data_ptr() if (t is not None and n) else None for t, n in zip(targets, w_needed)]
-        else:
-            sizes = [w.numel() if n else 0 for w, n in zip(weights, w_needed)]
-            flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
-            dptrs, off = [], 0
-            for i, (w, n) in enumerate(zip(weights, w_needed)):
-                if n:
-                    g = flat[off:off + w.numel()].view_as(w)
-                    off += w.numel()
-                    grads_out[i] = g
-                    dptrs.append(g.data_ptr())
-                else:
-                    dptrs.append(None)
-
+        dptrs, grads_out, accumulate = _weight_grad_targets(weights, ctx.needs_input_grad[w0:], ctx.grad_sink, dev)
         desc = _make_desc(cfg, B, T, True, accumulate)
         _, sbytes = _lib.workspace_bytes(desc)
         scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
@@ -291,26 +287,7 @@ class _LNRNNPoolFunction(torch.autograd.Function):
         dx = torch.empty(T, B, I, dtype=torch.float32, device=dev) if need_dx else None
         dln_w = torch.empty_like(ln_w) if (ctx.fused_ln and ctx.needs_input_grad[4]) else None
         dln_b = torch.empty_like(ln_w) if (ctx.fused_ln and ctx.needs_input_grad[5]) else None
-        sink = ctx.grad_sink
-        w_needed = [ctx.needs_input_grad[7 + i] for i in range(len(weights))]
-        grads_out: list = [None] * len(weights)
-        accumulate = False
-        if sink is not None:
-            targets = sink(weights)
-            accumulate = True
-            dptrs = [t.data_ptr() if (t is not None and n) else None for t, n in zip(targets, w_needed)]
-        else:
-            sizes = [(w.numel() + 63) // 64 * 64 if n else 0 for w, n in zip(weights, w_needed)]
-            flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
-            dptrs, off = [], 0
-            for i, (w, n) in enumerate(zip(weights, w_needed)):
-                if n:
-                    g = flat[off:off + w.numel()].view_as(w)
-                    off += sizes[i]
-                    grads_out[i] = g
-                    dptrs.append(g.data_ptr())
-                else:
-                    dptrs.append(None)
+        dptrs, grads_out, accumulate = _weight_grad_targets(weights, ctx.needs_input_grad[7:], ctx.grad_sink, dev)
         # with a sink the RNN weight gradients accumulate; the LayerNorm gradients are returned to autograd (fresh
         # tensors), so they must be WRITTEN: run them through a zeroed target when accumulating
         if accumulate:

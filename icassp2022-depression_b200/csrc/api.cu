@@ -144,11 +144,9 @@ struct ScratchLayout {
   // backward
   size_t b_dgates[2], b_dghn[2], b_wt[2], b_bpart[2], b_dy, b_gemm;
   size_t b_gemm_bytes;
-  // tensor-core backward GEMMs: dense TF32 hi/lo splits of the operands (hi at the offset, lo right behind it); the names
-  // keep their round-1 "T" although nothing is transposed any more (MN-major operands, gemm_tc.cu)
-  size_t b_tc_dg, b_tc_dgT, b_tc_hnT, b_tc_xT, b_tc_yT, b_tc_wT, b_tc_part;
+  // tensor-core backward GEMMs: dense TF32 hi/lo splits of the operands (hi at the offset, lo right behind it)
+  size_t b_tc_dg, b_tc_hn, b_tc_x, b_tc_y, b_tc_w, b_tc_part;
   size_t b_tc_part_bytes;
-  long long b_ldk;  // leading dimension of the transposed operands: T*B rounded up to a multiple of 4
   size_t b_dxln, b_lnpart;  // fused LayerNorm backward: dense d/dLN(x) [TB][I], per-CTA column partials
   size_t b_h0;              // [B][G*H]: gate gradients of each row's first step, paired with h_0 in dW_hh
   size_t b_dhp[2];          // proj_size > 0, per direction [T,B,P]: gradient w.r.t. the projected h_t (dW_hr)
@@ -208,14 +206,11 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
   off += align_up(gb / sizeof(float) + 1, ALIGN_F);
   {
     const size_t Imax = d.I > (int)d.DH ? (size_t)d.I : d.DH;
-    const size_t ldk = (d.TB + 3) / 4 * 4;
-    s->b_ldk = (long long)ldk;
-    s->b_tc_dg = off;   off += align_up(2 * d.TB * d.GH, ALIGN_F);
-    s->b_tc_dgT = off;  off += align_up(2 * d.GH * ldk, ALIGN_F);
-    s->b_tc_hnT = off;  off += align_up(2 * (size_t)d.H * ldk, ALIGN_F);
-    s->b_tc_xT = off;   off += align_up(2 * Imax * ldk, ALIGN_F);
-    s->b_tc_yT = off;   off += align_up(2 * (size_t)d.H * ldk, ALIGN_F);
-    s->b_tc_wT = off;   off += align_up(2 * Imax * d.GH, ALIGN_F);
+    s->b_tc_dg = off;  off += align_up(2 * d.TB * d.GH, ALIGN_F);
+    s->b_tc_hn = off;  off += align_up(2 * d.TB * d.H, ALIGN_F);
+    s->b_tc_x = off;   off += align_up(2 * d.TB * Imax, ALIGN_F);
+    s->b_tc_y = off;   off += align_up(2 * d.TB * d.H, ALIGN_F);
+    s->b_tc_w = off;   off += align_up(2 * Imax * d.GH, ALIGN_F);
     s->b_tc_part = off;
     s->b_tc_part_bytes = (size_t)160 * 128 * 128 * sizeof(float);  // <= (#SMs / tiles) * M * N
     off += align_up(s->b_tc_part_bytes / sizeof(float), ALIGN_F);
@@ -257,6 +252,65 @@ void make_wcache(const Dims& d, WCacheLayout* w) {
 }
 
 inline bool aligned_to(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
+
+// ---- gradient GEMMs of the backward pass -----------------------------------------------------------------------
+// An fp32 operand [R][C] (row r at p + rows.off(r)) and where the tensor cores take its TF32 split: hi dense [R][C] at
+// `split`, lo right behind it (3xTF32 only). The first tensor-core GEMM that reads the operand writes the split.
+struct GradSrc {
+  const float* p;
+  RowMap rows;
+  int R, C;
+  float* split;
+  bool split_done;
+};
+
+// One operand of a gradient GEMM, read from row `row0` of its source on. kcontig: the source's rows are the GEMM's m
+// (or n) and its columns k; otherwise its rows are k (the operands whose contraction index is the step (t,b)).
+struct GradOperand {
+  GradSrc* src;
+  int row0;
+  bool kcontig;
+};
+
+// C[M,N] (+)= sum_k A(m,k) B(k,n)
+struct GradGemm {
+  GradOperand a, b;
+  int M, N, K;
+  float* C;
+  RowMap c_rows;
+  int accumulate;
+  bool splitk;  // split-K over the long T*B contraction of a wgrad (FFMA: the gemm workspace, tensor cores: b_tc_part)
+  bool tc;      // tensor-core presplit GEMM (3xTF32, or single-pass TF32 with `tf32`); FFMA otherwise
+};
+
+int run_grad_gemm(const GradGemm& g, const ScratchLayout& sl, float* S, bool tf32, cudaStream_t st) {
+  if (!g.tc) {
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    p.A = g.a.src->p + g.a.src->rows.off(g.a.row0); p.a_rows = g.a.src->rows; p.a_kcontig = g.a.kcontig;
+    p.B = g.b.src->p + g.b.src->rows.off(g.b.row0); p.b_rows = g.b.src->rows; p.b_kcontig = g.b.kcontig;
+    p.C = g.C; p.c_rows = g.c_rows;
+    p.M = g.M; p.N = g.N; p.K = g.K;
+    p.accumulate = g.accumulate;
+    const bool ws = g.splitk && sl.b_gemm_bytes;
+    return launch_gemm(p, ws ? S + sl.b_gemm : nullptr, ws ? sl.b_gemm_bytes : 0, st);
+  }
+  TcOperand op[2];
+  for (int i = 0; i < 2; ++i) {
+    const GradOperand& o = i ? g.b : g.a;
+    GradSrc* s = o.src;
+    const size_t n = (size_t)s->R * s->C, at = (size_t)o.row0 * s->C;
+    if (!s->split_done) {
+      const int rc = tc_split(s->p, s->rows, s->R, s->C, s->split, tf32 ? nullptr : s->split + n, st);
+      if (rc) return rc;
+      s->split_done = true;
+    }
+    op[i] = TcOperand{s->split + at, tf32 ? nullptr : s->split + n + at, (long long)s->C, !o.kcontig};
+  }
+  return tc_gemm_presplit(op[0], op[1], g.M, g.N, g.K, g.C, g.c_rows, nullptr, nullptr, 0, g.accumulate,
+                          g.splitk ? S + sl.b_tc_part : nullptr, g.splitk ? sl.b_tc_part_bytes : 0, st, nullptr, 0,
+                          tf32);
+}
 
 }  // namespace
 }  // namespace b200rnn
@@ -686,7 +740,7 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
   const uint64_t* hdr = reinterpret_cast<const uint64_t*>(R);  // dropout seed/offset used by the forward
   const int accumulate = (desc->flags & B200RNN_FLAG_ACCUMULATE_GRADS) ? 1 : 0;
   const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0;  // single-pass TF32 tensor-core GEMMs: hi operands only
-  void* gemm_ws = sl.b_gemm_bytes ? (void*)(S + sl.b_gemm) : nullptr;
+  const int TB = (int)d.TB, GH = (int)d.GH;
   int* order = nullptr;  // the forward's slot order, recomputed from the same lengths (nothing of it is in the reserve)
   if (lengths) {
     order = reinterpret_cast<int*>(S + sl.order);
@@ -739,164 +793,62 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     rc = launch_rec_bwd(bp, st);
     if (rc) return rc;
 
-    // layer input as seen by the forward GEMM
-    const float* in;
-    RowMap in_rows;
+    // The gradient GEMMs of this layer: each runs on the tensor cores when it is eligible, on the FFMA GEMM otherwise.
+    // The tensor cores need 16-byte aligned targets: a gradient view that is not (a caller's flat bucket behind an
+    // odd-sized tensor) takes the FFMA GEMM instead of failing.
+    const bool tc_l = tc_available() && (Il % 128 == 0);
+    // layer input as seen by the forward GEMM; one split serves both directions
+    GradSrc X{nullptr, simple_rows((long long)Il), TB, Il, S + sl.b_tc_x, false};
     if (l == 0 && fused_ln) {  // what the forward GEMM multiplied: LayerNorm(x), saved densely by the prologue
-      in = R + rl.xln;
-      in_rows = simple_rows((long long)d.I);
+      X.p = R + rl.xln;
     } else if (l == 0) {
-      in = x;
-      in_rows = tb_rows(xs_t, xs_b, d.B);
+      X.p = x;
+      X.rows = tb_rows(xs_t, xs_b, d.B);
     } else {
-      in = R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
-      in_rows = simple_rows((long long)d.DH);
+      X.p = R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
     }
-    // with the fused LayerNorm the layer-0 dgrad is d/dLN(x): it goes to scratch and through the LN backward below
+    // dX_l goes to the caller's dx (layer 0) or to the dy of the layer below (scratch). With the fused LayerNorm the
+    // layer-0 dgrad is d/dLN(x): it goes to scratch and through the LN backward below
     const bool ln_l0 = (l == 0) && fused_ln;
     const bool want_dx = (l > 0) || (dx != nullptr) || (ln_l0 && (dln_gamma || dln_beta));
-    // ---- tensor-core 3xTF32 (single-pass TF32) path for the wgrad / dgrad GEMMs (falls back to the FFMA kernel per
-    // GEMM) ---------------------------------------------------------------------------------------------------------
-    const long long ldk = sl.b_ldk;
-    const bool tc_l = tc_available() && (Il % 128 == 0);
-    // Operands whose contraction index (t,b) is their ROW index - X_l, dG, h_prev, dn*r - go to the tensor cores as
-    // MN-major tiles (gemm_tc.cu): they only need the dense TF32 hi/lo split, no transposing pass (round 1 transposed
-    // every one of them: 10 passes, 8 % of the c2 train step).
-    // lo(p): the lo half of a split operand whose hi is at p, or NULL in single-pass TF32 mode (neither written nor read)
-    auto lo = [&](float* hi, size_t n) -> float* { return tf32 ? nullptr : hi + n; };
-    float* xS = S + sl.b_tc_xT;  // [TB][Il] hi, then lo
-    if (tc_l) {  // X_l, shared by both directions
-      rc = tc_split(in, in_rows, (int)d.TB, Il, xS, lo(xS, d.TB * (size_t)Il), st);
-      if (rc) return rc;
+    float* Cx = S + sl.b_dy;
+    RowMap cx_rows = simple_rows((long long)d.DH);
+    if (ln_l0) {
+      Cx = S + sl.b_dxln; cx_rows = simple_rows((long long)d.I);
+    } else if (l == 0) {
+      Cx = dx; cx_rows = tb_rows(dxs_t, dxs_b, d.B);
     }
-    (void)ldk;
+    const bool tc_dx = tc_l && want_dx && aligned_to(Cx, 16) && cx_rows.s_outer % 4 == 0 && cx_rows.s_inner % 4 == 0;
     for (int k = 0; k < d.D; ++k) {
       const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
       float* const* gp = dparams + (size_t)(l * d.D + k) * d.NPAR;
       float *dw_ih = gp[0], *dw_hh = gp[1], *db_ih = gp[2], *db_hh = gp[3];
-      const float* dG = S + sl.b_dgates[k];
-      const float* dHN = S + sl.b_dghn[k];
       if (db_ih || db_hh) {
         rc = launch_bias_reduce(S + sl.b_bpart[k], bp.nslices_out, d.mode, d.H, db_ih, db_hh, accumulate, st);
         if (rc) return rc;
       }
-      bool done_dwih = (dw_ih == nullptr), done_dwhh = (dw_hh == nullptr), done_dx = !want_dx;
-      if (tc_l) {
-        float* dGs = S + sl.b_tc_dg;   // [TB][GH] hi, then lo: MN-major A of the wgrads AND K-major A of the dgrad
-        float* hnS = S + sl.b_tc_hnT;  // [TB][H]   (GRU: dn * r)
-        const TcOperand opX{xS, lo(xS, d.TB * (size_t)Il), (long long)Il, true};
-        // the tensor-core path needs 16-byte aligned outputs: a gradient target that is not 16-byte aligned (a view into a caller's
-        // flat bucket behind an odd-sized tensor) takes the FFMA GEMM below instead of failing
-        const bool tc_wih = dw_ih && aligned_to(dw_ih, 16), tc_whh = dw_hh && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0;
-        float* Cx = nullptr;
-        RowMap cx_rows = simple_rows(1);
-        bool tc_dx = false;
-        if (want_dx) {
-          if (ln_l0) {
-            Cx = S + sl.b_dxln; cx_rows = simple_rows((long long)d.I);
-          } else if (l == 0) {
-            Cx = dx; cx_rows = tb_rows(dxs_t, dxs_b, d.B);
-          } else {
-            Cx = S + sl.b_dy; cx_rows = simple_rows((long long)d.DH);
-          }
-          tc_dx = (reinterpret_cast<uintptr_t>(Cx) % 16 == 0) && cx_rows.s_outer % 4 == 0 && cx_rows.s_inner % 4 == 0;
-        }
-        if (tc_wih || tc_whh || tc_dx) {
-          rc = tc_split(dG, simple_rows((long long)d.GH), (int)d.TB, (int)d.GH, dGs, lo(dGs, d.TB * d.GH), st);
-          if (rc) return rc;
-        }
-        if (tc_wih) {  // dW_ih[GH, Il] = sum_tb dG[tb, :]^T X_l[tb, :]
-          const TcOperand opA{dGs, lo(dGs, d.TB * d.GH), (long long)d.GH, true};
-          rc = tc_gemm_presplit(opA, opX, (int)d.GH, Il, (int)d.TB, dw_ih, simple_rows(Il), nullptr, nullptr, 0,
-                                accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
-          if (rc) return rc;
-          done_dwih = true;
-        }
-        if (tc_whh) {
-          // dW_hh = sum_t dGh[t]^T h_{prev(t)}: rows are (t,b) flattened time-major, so the one-step shift is a ROW
-          // offset of B (forward: dG[t] with y[t-1]; reverse: dG[t] with y[t+1]); rows beyond Kp read as zero (TMA)
-          float* yS = S + sl.b_tc_yT;  // [TB][H]
-          rc = tc_split(bp.y + (long long)k * d.H, tb_rows(bp.y_st, bp.y_sb, d.B), (int)d.TB, d.H, yS,
-                        lo(yS, d.TB * (size_t)d.H), st);
-          if (rc) return rc;
-          const int Kp = (d.T - 1) * d.B;
-          const size_t rowA = (k == 0) ? (size_t)d.B : 0, rowY = (k == 0) ? 0 : (size_t)d.B;
-          const TcOperand opY{yS + rowY * d.H, tf32 ? nullptr : yS + d.TB * (size_t)d.H + rowY * d.H, (long long)d.H, true};
-          if (d.mode == B200RNN_LSTM) {
-            const TcOperand opA{dGs + rowA * d.GH, tf32 ? nullptr : dGs + d.TB * d.GH + rowA * d.GH, (long long)d.GH, true};
-            rc = tc_gemm_presplit(opA, opY, (int)d.GH, d.H, Kp, dw_hh, simple_rows(d.H), nullptr, nullptr, 0,
-                                  accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
-            if (rc) return rc;
-          } else {
-            rc = tc_split(dHN, simple_rows((long long)d.H), (int)d.TB, d.H, hnS, lo(hnS, d.TB * (size_t)d.H), st);
-            if (rc) return rc;
-            // columns [0, 2H) of dG: r and z gates
-            const TcOperand opRZ{dGs + rowA * d.GH, tf32 ? nullptr : dGs + d.TB * d.GH + rowA * d.GH, (long long)d.GH,
-                                 true};
-            rc = tc_gemm_presplit(opRZ, opY, 2 * d.H, d.H, Kp, dw_hh, simple_rows(d.H), nullptr, nullptr, 0,
-                                  accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
-            if (rc) return rc;
-            const TcOperand opN{hnS + rowA * d.H, tf32 ? nullptr : hnS + d.TB * (size_t)d.H + rowA * d.H, (long long)d.H,
-                                true};  // n rows: dn * r
-            rc = tc_gemm_presplit(opN, opY, d.H, d.H, Kp, dw_hh + (size_t)2 * d.H * d.H, simple_rows(d.H), nullptr,
-                                  nullptr, 0, accumulate, S + sl.b_tc_part, sl.b_tc_part_bytes, st, nullptr, 0, tf32);
-            if (rc) return rc;
-          }
-          done_dwhh = true;
-        }
-        if (tc_dx) {  // dX_l (+)= dG[TB, GH] * W_ih[GH, Il]: A K-major (the same split of dG), B = W_ih as it lies (MN-major)
-          float* wS = S + sl.b_tc_wT;   // [GH][Il] hi, then lo
-          rc = tc_split(pp[0], simple_rows(Il), (int)d.GH, Il, wS, lo(wS, d.GH * (size_t)Il), st);
-          if (rc) return rc;
-          const TcOperand opA{dGs, lo(dGs, d.TB * d.GH), (long long)d.GH, false};
-          const TcOperand opB{wS, lo(wS, d.GH * (size_t)Il), (long long)Il, true};
-          rc = tc_gemm_presplit(opA, opB, (int)d.TB, Il, (int)d.GH, Cx, cx_rows, nullptr, nullptr, 0, (k > 0) ? 1 : 0,
-                                nullptr, 0, st, nullptr, 0, tf32);
-          if (rc) return rc;
-          done_dx = true;
-        }
-      }
-      if (!done_dwih) {  // dW_ih = dGi^T * X_l
-        GemmParams g;
-        memset(&g, 0, sizeof(g));
-        g.A = dG; g.a_rows = simple_rows((long long)d.GH); g.a_kcontig = 0;
-        g.B = in; g.b_rows = in_rows; g.b_kcontig = 0;
-        g.C = dw_ih; g.c_rows = simple_rows(Il);
-        g.M = (int)d.GH; g.N = Il; g.K = (int)d.TB;
-        g.accumulate = accumulate;
-        rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
+      // this direction's operands (their split regions are reused by the next direction)
+      GradSrc dG{S + sl.b_dgates[k], simple_rows(GH), TB, GH, S + sl.b_tc_dg, false};
+      GradSrc dnr{S + sl.b_dghn[k], simple_rows(d.H), TB, d.H, S + sl.b_tc_hn, false};  // GRU: dn * r
+      GradSrc h{bp.y + (long long)k * d.HO, tb_rows(bp.y_st, bp.y_sb, d.B), TB, d.HO, S + sl.b_tc_y, false};
+      GradSrc w_ih{pp[0], simple_rows(Il), GH, Il, S + sl.b_tc_w, false};
+      if (dw_ih) {  // dW_ih[GH, Il] = sum_tb dG[tb, :]^T X_l[tb, :]
+        rc = run_grad_gemm({{&dG, 0, false}, {&X, 0, false}, GH, Il, TB, dw_ih, simple_rows(Il), accumulate, true,
+                            tc_l && aligned_to(dw_ih, 16)}, sl, S, tf32, st);
         if (rc) return rc;
       }
-      if (!done_dwhh) {  // dW_hh = sum_t dGh[t]^T * h_{prev(t)}   (the first scanned step's h_0 term follows below)
-        const int Kp = (d.T - 1) * d.B;
-        // forward direction: pairs (dG[t], y[t-1]) for t = 1..T-1 ; reverse: (dG[t], y[t+1]) for t = 0..T-2
-        const size_t g_t0 = (k == 0) ? (size_t)d.B : 0;  // first dG row
-        const long long y_t0 = (k == 0) ? 0 : bp.y_st;   // first y row offset (elements)
-        const float* hp = bp.y + y_t0 + (long long)k * d.HO;
-        RowMap hp_rows = tb_rows(bp.y_st, bp.y_sb, d.B);
-        GemmParams g;
-        memset(&g, 0, sizeof(g));
-        g.B = hp; g.b_rows = hp_rows; g.b_kcontig = 0;
-        g.N = d.HO; g.K = Kp;
-        g.accumulate = accumulate;
-        g.a_kcontig = 0;
-        if (d.mode == B200RNN_LSTM) {
-          g.A = dG + g_t0 * d.GH; g.a_rows = simple_rows((long long)d.GH);
-          g.C = dw_hh; g.c_rows = simple_rows(d.HO);
-          g.M = (int)d.GH;
-          rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
-          if (rc) return rc;
-        } else {
-          // r,z rows share dGi; the n rows use dn*r
-          g.A = dG + g_t0 * d.GH; g.a_rows = simple_rows((long long)d.GH);
-          g.C = dw_hh; g.c_rows = simple_rows(d.H);
-          g.M = 2 * d.H;
-          rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
-          if (rc) return rc;
-          g.A = dHN + g_t0 * d.H; g.a_rows = simple_rows((long long)d.H);
-          g.C = dw_hh + (size_t)2 * d.H * d.H;
-          g.M = d.H;
-          rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
+      if (dw_hh) {
+        // dW_hh = sum_t dGh[t]^T h_{prev(t)}: rows are (t,b) flattened time-major, so the one-step shift is a row
+        // offset of B (forward: dG[t] with h[t-1], t = 1..T-1; reverse: dG[t] with h[t+1], t = 0..T-2). LSTM: one GEMM
+        // over all gates; GRU: the r,z rows from columns [0, 2H) of dG, the n rows from dn*r
+        const int g0 = k == 0 ? d.B : 0, Kp = (d.T - 1) * d.B;
+        const bool gru = d.mode == B200RNN_GRU, tc = tc_l && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0;
+        rc = run_grad_gemm({{&dG, g0, false}, {&h, d.B - g0, false}, gru ? 2 * d.H : GH, d.HO, Kp, dw_hh,
+                            simple_rows(d.HO), accumulate, true, tc}, sl, S, tf32, st);
+        if (rc) return rc;
+        if (gru) {
+          rc = run_grad_gemm({{&dnr, g0, false}, {&h, d.B - g0, false}, d.H, d.HO, Kp, dw_hh + (size_t)2 * d.H * d.HO,
+                              simple_rows(d.HO), accumulate, true, tc}, sl, S, tf32, st);
           if (rc) return rc;
         }
       }
@@ -904,45 +856,24 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
         // the first scanned step's previous state is h_0: dW_hh += sum_b dGh[t_first(b), b]^T h_0[b]. The shifted GEMMs
         // above never pair that step with anything but a zero (T = 1: K = 0; ragged reverse rows: the masked output at
         // len_b), so nothing is counted twice. One fixed-order K = B FFMA GEMM: deterministic.
-        float* rows0 = S + sl.b_h0;  // [B][GH]
-        rc = launch_initial_state_rows(dG, dHN, d.mode, d.B, d.T, d.H, k == 1, lengths, rows0, st);
+        GradSrc rows0{S + sl.b_h0, simple_rows(GH), d.B, GH, nullptr, false};  // [B][GH]
+        GradSrc h0{bp.h_0 + (size_t)k * d.B * d.HO, simple_rows(d.HO), d.B, d.HO, nullptr, false};
+        rc = launch_initial_state_rows(dG.p, dnr.p, d.mode, d.B, d.T, d.H, k == 1, lengths, S + sl.b_h0, st);
         if (rc) return rc;
-        GemmParams g;
-        memset(&g, 0, sizeof(g));
-        g.A = rows0; g.a_rows = simple_rows((long long)d.GH); g.a_kcontig = 0;
-        g.B = bp.h_0 + (size_t)k * d.B * d.HO; g.b_rows = simple_rows(d.HO); g.b_kcontig = 0;
-        g.C = dw_hh; g.c_rows = simple_rows(d.HO);
-        g.M = (int)d.GH; g.N = d.HO; g.K = d.B;
-        g.accumulate = 1;
-        rc = launch_gemm(g, nullptr, 0, st);
+        rc = run_grad_gemm({{&rows0, 0, false}, {&h0, 0, false}, GH, d.HO, d.B, dw_hh, simple_rows(d.HO), 1, false,
+                            false}, sl, S, tf32, st);
         if (rc) return rc;
       }
       if (d.P > 0 && gp[4]) {  // dW_hr[P, H] = sum_tb dh[tb, :]^T m[tb, :] (frozen and skipped steps have dh = 0)
-        GemmParams g;
-        memset(&g, 0, sizeof(g));
-        g.A = S + sl.b_dhp[k]; g.a_rows = simple_rows((long long)d.P); g.a_kcontig = 0;
-        g.B = R + rl.m[l][k]; g.b_rows = simple_rows((long long)d.H); g.b_kcontig = 0;
-        g.C = gp[4]; g.c_rows = simple_rows(d.H);
-        g.M = d.P; g.N = d.H; g.K = (int)d.TB;
-        g.accumulate = accumulate;
-        rc = launch_gemm(g, gemm_ws, sl.b_gemm_bytes, st);
+        GradSrc dhp{S + sl.b_dhp[k], simple_rows(d.P), TB, d.P, nullptr, false};
+        GradSrc m{R + rl.m[l][k], simple_rows(d.H), TB, d.H, nullptr, false};
+        rc = run_grad_gemm({{&dhp, 0, false}, {&m, 0, false}, d.P, d.H, TB, gp[4], simple_rows(d.H), accumulate, true,
+                            false}, sl, S, tf32, st);
         if (rc) return rc;
       }
-      if (!done_dx) {  // dX_l (+)= dGi * W_ih
-        GemmParams g;
-        memset(&g, 0, sizeof(g));
-        g.A = dG; g.a_rows = simple_rows((long long)d.GH); g.a_kcontig = 1;
-        g.B = pp[0]; g.b_rows = simple_rows(Il); g.b_kcontig = 0;
-        if (ln_l0) {
-          g.C = S + sl.b_dxln; g.c_rows = simple_rows((long long)d.I);
-        } else if (l == 0) {
-          g.C = dx; g.c_rows = tb_rows(dxs_t, dxs_b, d.B);
-        } else {
-          g.C = S + sl.b_dy; g.c_rows = simple_rows((long long)d.DH);
-        }
-        g.M = (int)d.TB; g.N = Il; g.K = (int)d.GH;
-        g.accumulate = (k > 0) ? 1 : 0;
-        rc = launch_gemm(g, nullptr, 0, st);
+      if (want_dx) {  // dX_l (+)= dG[TB, GH] W_ih[GH, Il]: dG read K-major, W_ih as it lies
+        rc = run_grad_gemm({{&dG, 0, true}, {&w_ih, 0, false}, TB, Il, GH, Cx, cx_rows, k > 0, false, tc_dx}, sl, S,
+                           tf32, st);
         if (rc) return rc;
       }
     }
