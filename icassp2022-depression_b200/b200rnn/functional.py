@@ -146,20 +146,15 @@ class _RNNFunction(torch.autograd.Function):
         len_ptr = lengths.data_ptr() if lengths is not None else None
         c_n_ptr = c_n.data_ptr() if c_n is not None else None
         if B > 0 and T > 0:
+            # the module forward, with or without hx: the model-shell entry b200rnn_forward_fused is for
+            # rnn_forward_fused / rnn_ln_pool_sum (its no-grad GRU-256 recurrence runs on fp16 pairs)
             with _on(dev):
-                if h_0 is None and not cfg.proj_size:
-                    rc = lib.b200rnn_forward_fused(
-                        ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
-                        y.data_ptr(), ys_t, ys_b, h_n.data_ptr(), c_n_ptr,
-                        reserve.data_ptr() if save else None, scratch.data_ptr(),
-                        0, 0, rng_ptr, None, None, 0.0, None, len_ptr, None, None, _stream_ptr(dev))
-                else:
-                    rc = lib.b200rnn_forward_hx(
-                        ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
-                        y.data_ptr(), ys_t, ys_b, h_0.data_ptr() if h_0 is not None else None,
-                        c_0.data_ptr() if c_0 is not None else None,
-                        h_n.data_ptr(), c_n_ptr, reserve.data_ptr() if save else None, scratch.data_ptr(),
-                        0, 0, rng_ptr, len_ptr, _stream_ptr(dev))
+                rc = lib.b200rnn_forward_hx(
+                    ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+                    y.data_ptr(), ys_t, ys_b, h_0.data_ptr() if h_0 is not None else None,
+                    c_0.data_ptr() if c_0 is not None else None,
+                    h_n.data_ptr(), c_n_ptr, reserve.data_ptr() if save else None, scratch.data_ptr(),
+                    0, 0, rng_ptr, len_ptr, _stream_ptr(dev))
             _lib.check(rc, "b200rnn_forward")
         else:   # no step: the final state is the initial one
             h_n.copy_(h_0) if h_0 is not None else h_n.zero_()

@@ -352,16 +352,22 @@ B200RNN_API int b200rnn_workspace_bytes(const b200rnn_desc* desc, size_t* reserv
   return B200RNN_OK;
 }
 
-// The forward of every entry point; h_0 / c_0 NULL = zeros (b200rnn_forward_hx checked their consistency)
+// The forward of every entry point; h_0 / c_0 NULL = zeros (b200rnn_forward_hx checked their consistency). `shell`:
+// called by b200rnn_forward_fused, the model-shell entry, which never takes an initial state; its no-grad forward runs
+// the GRU-256 tensor-core recurrence on fp16 pairs (RecFwdParams::shell_nograd)
 static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
                         const float* const* params, float* y, int64_t ys_t, int64_t ys_b, float* h_n, float* c_n,
                         void* reserve, void* scratch, uint64_t seed, uint64_t offset, uint64_t* rng_state,
                         const float* ln_gamma, const float* ln_beta, float ln_eps, float* y_pool,
                         const int32_t* lengths, const void* wcache, void* prologue_done, const float* h_0,
-                        const float* c_0, void* stream_) {
+                        const float* c_0, bool shell, void* stream_) {
   Dims d;
   int rc = check_desc(desc, &d);
   if (rc) return rc;
+  if (shell && (h_0 || c_0)) {
+    set_error("forward: the model-shell entry takes no initial state");
+    return B200RNN_ERR_INVALID;
+  }
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   cudaEvent_t prologue_ev = static_cast<cudaEvent_t>(prologue_done);
   if (d.B == 0 || d.T == 0) {
@@ -466,6 +472,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     rp.lengths = lengths;
     rp.order = order;
     rp.tf32 = tf32 ? 1 : 0;
+    rp.shell_nograd = shell && !save ? 1 : 0;
     rp.P = d.P;
     RecFwdLaunch rec;
     rc = plan_rec_fwd(rp, &rec);
@@ -608,7 +615,8 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     return B200RNN_ERR_UNSUPPORTED;
   }
   return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
-                      ln_gamma, ln_beta, ln_eps, y_pool, lengths, wcache, prologue_done, nullptr, nullptr, stream_);
+                      ln_gamma, ln_beta, ln_eps, y_pool, lengths, wcache, prologue_done, nullptr, nullptr, true,
+                      stream_);
 }
 
 B200RNN_API int b200rnn_forward_hx(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
@@ -633,7 +641,7 @@ B200RNN_API int b200rnn_forward_hx(const b200rnn_desc* desc, const float* x, int
     return B200RNN_OK;
   }
   return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
-                      nullptr, nullptr, 0.f, nullptr, lengths, nullptr, nullptr, h_0, c_0, stream_);
+                      nullptr, nullptr, 0.f, nullptr, lengths, nullptr, nullptr, h_0, c_0, false, stream_);
 }
 
 B200RNN_API int b200rnn_forward(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
@@ -641,7 +649,7 @@ B200RNN_API int b200rnn_forward(const b200rnn_desc* desc, const float* x, int64_
                                 float* c_n, void* reserve, void* scratch, uint64_t seed, uint64_t offset,
                                 uint64_t* rng_state, void* stream_) {
   return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
-                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream_);
+                      nullptr, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, false, stream_);
 }
 
 B200RNN_API int b200rnn_wcache_bytes(const b200rnn_desc* desc, size_t* bytes) {

@@ -121,7 +121,7 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-// ---- warp-level tensor-core MMA (SASS: HMMA.1688.F32.TF32) ----------------------------------------
+// ---- warp-level tensor-core MMA (SASS: HMMA.1688.F32.TF32, HMMA.16816.F32) -------------------------
 // x = hi + lo with hi = x truncated to TF32 (its 13 low mantissa bits cleared, in a 32-bit container) and lo = x - hi
 // (exact in fp32, |lo| < 2^-10 |x|). The MMA reads only the TF32 bits of lo, so hi*hi + lo*hi + hi*lo carries ~2^-20
 // relative error per product (3xTF32). Two ops per value: cvt.rna.tf32.f32 (the round-to-nearest split of gemm_tc.cu)
@@ -135,6 +135,16 @@ __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) 
 //   d = {D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]}
 __device__ __forceinline__ void mma_tf32_m16n8k8(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
   asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+// D[16x8] += A[16x16] * B[16x8] in fp16 with fp32 accumulation (SASS: HMMA.16816.F32). Each register is an f16x2,
+// the lower k in the low half; same g, t and the same accumulator fragment d as m16n8k8:
+//   a = {A[g][2t..2t+1], A[g+8][2t..2t+1], A[g][2t+8..2t+9], A[g+8][2t+8..2t+9]},
+//   b = {B[2t..2t+1][g], B[2t+8..2t+9][g]}
+__device__ __forceinline__ void mma_f16_m16n8k16(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
       "{%0, %1, %2, %3};"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));

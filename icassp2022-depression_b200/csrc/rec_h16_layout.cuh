@@ -1,0 +1,74 @@
+// rec_h16_layout.cuh — shared-memory layout of the fp16-pair GRU-256 forward recurrence (rec_fwd_h16_kernel,
+// rnn_rec.cu): where the staging loop puts each weight, where the lane that produces h_t puts each state element, and
+// which 16 bytes a lane reads or hands to the peers. Host and device code: tests/test_h16_layout_cpu.py compiles these
+// helpers into a host program and checks every offset against the regions below and the mma.sync fragment definitions.
+//
+// Geometry (TcFwdCfg, rnn_rec.cu): H = 256 units, C = 4 CTAs per cluster, HS = 64 units per CTA, BS = 8 batch rows,
+// G = 3 gate tiles, 4 unit groups of 16 units, two warps per unit group (k halves). The contraction runs as
+// mma.sync m16n8k16 f16 -> f32 (ptx.cuh mma_f16_m16n8k16) over 16 k-blocks of 16, each operand a (hi, lo) pair of fp16.
+//
+// k order inside a k-block: fragment position p (the k index of the PTX fragments) holds unit kk = h16_perm(p) of the
+// block, bits 2 and 3 swapped. Lane (g, t) of the B fragment then holds units {0,1,4,5} (t = 0), {2,3,6,7} (t = 1),
+// {8,9,12,13} (t = 2), {10,11,14,15} (t = 3): the lanes t < 2 hold the first 8 units of the block, the lanes t >= 2 the
+// last 8. A and B use the same order, so the product is unchanged.
+#pragma once
+#include <math.h>
+
+namespace b200rnn {
+namespace h16 {
+
+constexpr int H = 256, C = 4, HS = H / C, BS = 8, G = 3, NUG = HS / 16, NW = 2 * NUG;
+constexpr int KB = H / 16;    // k-blocks of the contraction
+constexpr int KBC = HS / 16;  // k-blocks per source slice
+// weights: [NUG][G][KB][hi, lo][32 lanes] of 16 bytes (4 f16x2 A-fragment registers): a lane's hi (lo) registers of
+// one (tile, k-block) are one LDS.128, a warp's are 512 contiguous bytes
+constexpr int W_HALVES = NUG * G * KB * 2 * 32 * 8;
+// state: [KB][32 slots] of 16 bytes {hi b0, hi b1, lo b0, lo b1} per buffer
+constexpr int S_HALVES = KB * 32 * 8;
+static_assert(W_HALVES * 2 == G * HS * H * 4, "the fp16 pairs fill exactly the bytes of the fp32 weight tiles");
+static_assert(S_HALVES * 2 == BS * H * 4, "the fp16 pairs fill exactly the bytes of an fp32 state buffer");
+
+// Row scale 2^e of the weight split: max |w| of the row times 2^e lies in [2^14, 2^15), so hi = RN_f16(w 2^e) is normal
+// for every weight within 2^-28 of the row's maximum. e = 0 for a row whose maximum is 0 or not finite: zeros stay exact,
+// and an Inf weight gives hi = Inf, lo = NaN, NaN outputs, as the 3xTF32 split does. e <= 112 keeps 2^e and the unscale
+// 2^-(e + 14) normal fp32 numbers; a row whose maximum is below 2^-98 is scaled less (its hi loses bits, at an absolute
+// error below 2^-120).
+__host__ __device__ inline int scale_exp(float m) {
+  if (!(m > 0.f) || !(m <= 3.40282347e38f)) return 0;
+  int x = 0;
+  frexpf(m, &x);  // m = f 2^x, f in [0.5, 1)
+  return 15 - x < 112 ? 15 - x : 112;
+}
+// the state scale: |h| <= 1 without an initial state, so |h| 2^14 <= 2^14 < 65504
+constexpr float STATE_SCALE = 16384.f;
+
+__host__ __device__ constexpr int perm(int p) { return (p & 3) | ((p >> 3) & 1) << 2 | ((p >> 2) & 1) << 3; }
+
+// A fragment of m16n8k16 (PTX ISA), lane (g, t) = (lane / 4, lane % 4), register r, element e (low half first):
+//   r = 0: A[g][2t + e], 1: A[g + 8][2t + e], 2: A[g][2t + 8 + e], 3: A[g + 8][2t + 8 + e]
+// half index in the weight region of (unit group ug, tile gt, k-block kb, hl = 0 hi / 1 lo, lane, register, element)
+__host__ __device__ constexpr int w_half(int ug, int gt, int kb, int hl, int lane, int r, int e) {
+  return (((((ug * G + gt) * KB + kb) * 2 + hl) * 32 + lane) * 4 + r) * 2 + e;
+}
+// half index of weight row (gate gt, unit u of the CTA's slice), column k, part hl: where the staging loop writes it
+__host__ __device__ constexpr int w_index(int gt, int u, int k, int hl) {
+  return w_half(u / 16, gt, k / 16, hl, (u % 8) * 4 + (perm(k % 16) % 8) / 2, (u % 16) / 8 + 2 * (perm(k % 16) / 8),
+                perm(k % 16) % 2);
+}
+
+// B fragment of m16n8k16 (PTX ISA), lane (g, t): register 0 = {B[2t][g], B[2t + 1][g]}, 1 = {B[2t + 8][g], B[2t + 9][g]}
+// (B[k][n], n = batch row). 16-byte slot of lane `lane` in a k-block: the slots of the lanes holding the first 8 units
+// of the block come first, so that the 8 units a warp finishes are 256 contiguous bytes (see exchange_chunk)
+__host__ __device__ constexpr int state_slot(int lane) { return ((lane & 3) >> 1) * 16 + (lane >> 2) * 2 + (lane & 1); }
+// half index of state element (unit k of the layer, batch row b), part hl, in one state buffer
+__host__ __device__ constexpr int state_index(int k, int b, int hl) {
+  // position of unit kk = k % 16 in the fragment: p = perm(kk); lane t = (p % 8) / 2, register p / 8, element p % 2
+  return ((k / 16 * 32 + state_slot(b * 4 + (perm(k % 16) % 8) / 2)) * 4 + 2 * hl + perm(k % 16) / 8) * 2 +
+         perm(k % 16) % 2;
+}
+// the exchange: after the warp finishing units k0 .. k0 + 7 (k0 % 8 == 0) has written them, lane l < 16 sends the
+// 16-byte chunk with this index (in 16-byte units of the state buffer) to every peer
+__host__ __device__ constexpr int exchange_chunk(int k0, int lane) { return (k0 / 16) * 32 + ((k0 % 16) / 8) * 16 + lane; }
+
+}  // namespace h16
+}  // namespace b200rnn

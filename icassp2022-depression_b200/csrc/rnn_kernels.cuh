@@ -30,6 +30,8 @@ struct RecFwdParams {
   int tiles_n;
   int tf32;                  // single-pass TF32 contraction in the tensor-core config tc8 (B200RNN_FLAG_TF32); every
                              // other config is fp32 FFMA and ignores it
+  int shell_nograd;          // the no-grad forward of b200rnn_forward_fused (nothing saved, no initial state): the GRU-256
+                             // tensor-core config runs on fp16 pairs (rec_fwd_h16_kernel) unless tf32 is set
   const float* h_0;          // optional [D,B,H] initial state of this layer, caller's row order (NULL: zeros)
   const float* c_0;          // optional [D,B,H] initial cell state (LSTM; NULL: zeros)
   // LSTM with a projection (rec_fwd_proj_kernel): P = proj_size, 0 = none. Then y, h_n and h_0 are P wide (y column

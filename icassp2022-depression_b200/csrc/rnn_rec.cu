@@ -22,14 +22,18 @@
 //
 // fp32 FFMA for most configs: the per-step contraction is [BS x H] x [H x G*HS] with BS = 2..8 rows per CTA — far too
 // skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference. The GRU H=256 8-row config runs it
-// on the tensor cores with warp-level mma.sync (N = 8) in 3xTF32 instead (rec_fwd_tc_kernel).
+// on the tensor cores with warp-level mma.sync (N = 8) in 3xTF32 instead (rec_fwd_tc_kernel), or on fp16 pairs split
+// once per launch in the no-grad forward of b200rnn_forward_fused (rec_fwd_h16_kernel).
 #include <map>
 #include <mutex>
 #include <stdlib.h>
 #include <utility>
 
+#include <cuda_fp16.h>
+
 #include "profile.cuh"
 #include "ptx.cuh"
+#include "rec_h16_layout.cuh"
 #include "rnn_core.cuh"
 #include "rnn_kernels.cuh"
 
@@ -516,16 +520,36 @@ __device__ __forceinline__ float round_tf32(float x) {
   return __uint_as_float(r);
 }
 
-template <bool VL, bool TF32>
+// fp16 pairs (rec_fwd_h16_kernel, the no-grad forward of b200rnn_forward_fused; RecFwdParams::shell_nograd): the same
+// cluster, warps, exchange and cell, with every operand an fp16 (hi, lo) pair that fills the 4 bytes of its fp32 value
+// (rec_h16_layout.cuh). An fp16 significand has TF32's 11 bits, so the pair is as precise as the 3xTF32 split, but it is
+// made once: W_hh as it is staged, each row scaled by 2^e_r (h16::scale_exp) so that hi is normal, and h_t by the lane
+// that produces it, scaled by 2^14. The step loop splits and converts nothing: per warp and k-block of 16 it loads the
+// state pair (one LDS.128) and the hi and lo A fragments of two gate tiles (four LDS.128; the third tile, n, stays in
+// registers for the whole launch) and runs nine mma.sync m16n8k16 (hi*hi, lo*hi, hi*lo per tile), with the same chains
+// and restarts as 3xTF32. The pre-activations are unscaled by the exact 2^-(e_r + 14) before the gate math. No initial
+// state: |h_t| <= 1 is what makes the fixed state scale safe.
+enum class TcOp { X3, TF32, F16 };
+
+template <bool VL, TcOp OP>
 __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int nslices) {
   using Cfg = TcFwdCfg;
   constexpr int H = Cfg::H, C = Cfg::C, BS = Cfg::BS, G = Cfg::G, HS = Cfg::HS, NUG = Cfg::NUG, NW = Cfg::NW,
                 NT = Cfg::NT, KS = Cfg::KS, KSC = Cfg::KSC;
+  constexpr bool TF32 = OP == TcOp::TF32, F16 = OP == TcOp::F16;
+  constexpr int KBC = h16::KBC;
+  static_assert(h16::H == H && h16::C == C && h16::BS == BS && h16::G == G && h16::NW == NW, "h16 layout geometry");
+  static_assert(h16::W_HALVES * 2 == (int)Cfg::W_BYTES && h16::S_HALVES * 2 == BS * H * 4, "h16 regions");
+  static_assert(G * HS <= NW * 2 * G * 32, "the row scales fit the swap buffer");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float4* W_f = reinterpret_cast<float4*>(smem_raw);                  // [NUG][G][KS][32 lanes] A fragments
   float* h_s = reinterpret_cast<float*>(smem_raw + Cfg::W_BYTES);     // [2][BS * H] B-fragment order
   float* red = h_s + 2 * BS * H;                                       // [NW][2 * G][32 lanes]
   uint64_t* bars = reinterpret_cast<uint64_t*>(red + NW * 2 * G * 32);  // [buf * C + src] state slices
+  // F16: W_f holds [NUG][G][KB][hi, lo][32 lanes] A fragments and h_s [2][KB][32 slots] state pairs (rec_h16_layout.cuh);
+  // red holds the row scales 2^e_r [G][HS] until the step loop first writes it
+  __half* W_h = reinterpret_cast<__half*>(smem_raw);
+  float* scl = red;
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int ug = w % NUG, kh = w / NUG;
@@ -544,6 +568,21 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], (uint32_t)(i % C) == rank ? (uint32_t)NW : 1u);
     ptx::fence_mbar_init();
   }
+  if constexpr (F16) {  // the row scales: one warp per row
+    for (int rr = w; rr < G * HS; rr += NW) {
+      const float4* row = reinterpret_cast<const float4*>(w_hh + ((size_t)(rr / HS) * H + j0 + rr % HS) * H);
+      float m = 0.f;
+#pragma unroll
+      for (int k = lane; k < H / 4; k += 32) {
+        const float4 v = __ldg(row + k);
+        m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(FULLMASK, m, o));
+      if (lane == 0) scl[rr] = ldexpf(1.f, h16::scale_exp(m));
+    }
+    __syncthreads();
+  }
   // this CTA's rows of the three gate blocks, read as coalesced float4 and scattered into A-fragment order: row u of
   // gate block g goes to unit group u / 16, tile g, fragment row u % 16; k0..k0+3 are the lanes t = 0..3 of one k-step
   // half
@@ -552,14 +591,26 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     const int rr = i / (H / 4), k0 = (i % (H / 4)) * 4;
     const int g = rr / HS, u = rr % HS;
     const float4 v = __ldg(reinterpret_cast<const float4*>(w_hh + ((size_t)g * H + j0 + u) * H + k0));
-    float* dst = reinterpret_cast<float*>(W_f + (((u / 16) * G + g) * KS + k0 / 8) * 32 + (u % 8) * 4) +
-                 (u % 16) / 8 + 2 * ((k0 / 4) & 1);
-    dst[0] = TF32 ? round_tf32(v.x) : v.x;
-    dst[4] = TF32 ? round_tf32(v.y) : v.y;
-    dst[8] = TF32 ? round_tf32(v.z) : v.z;
-    dst[12] = TF32 ? round_tf32(v.w) : v.w;
+    if constexpr (F16) {  // k0, k0 + 1 and k0 + 2, k0 + 3 are the two halves of one f16x2 register each
+      const float s = scl[rr];
+      const float x[4] = {v.x * s, v.y * s, v.z * s, v.w * s};
+#pragma unroll
+      for (int e = 0; e < 4; e += 2) {
+        const __half2 hi = __floats2half2_rn(x[e], x[e + 1]);
+        const __half2 lo = __floats2half2_rn(x[e] - __low2float(hi), x[e + 1] - __high2float(hi));
+        *reinterpret_cast<__half2*>(W_h + h16::w_index(g, u, k0 + e, 0)) = hi;
+        *reinterpret_cast<__half2*>(W_h + h16::w_index(g, u, k0 + e, 1)) = lo;
+      }
+    } else {
+      float* dst = reinterpret_cast<float*>(W_f + (((u / 16) * G + g) * KS + k0 / 8) * 32 + (u % 8) * 4) +
+                   (u % 16) / 8 + 2 * ((k0 / 4) & 1);
+      dst[0] = TF32 ? round_tf32(v.x) : v.x;
+      dst[4] = TF32 ? round_tf32(v.y) : v.y;
+      dst[8] = TF32 ? round_tf32(v.z) : v.z;
+      dst[12] = TF32 ? round_tf32(v.w) : v.w;
+    }
   }
-  if (p.h_0) {  // buffer 0: the initial state in B-fragment order, rounded like the copies the lanes producing h_t hand over
+  if (!F16 && p.h_0) {  // buffer 0: the initial state in B-fragment order, rounded like the copies the lanes producing h_t hand over
     for (int i = tid; i < BS * H; i += NT) {
       const int q = i / H, k = i - q * H;
       const float v = initial_state<VL>(p, dir, b0, q, k);
@@ -570,11 +621,29 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     for (int i = tid; i < 2 * BS * H; i += NT) h_s[i] = 0.f;  // h_0 = 0 (rnn.py:1432-1440)
   }
   __syncthreads();
-  ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
 
   // ---- lane identity: output jb is unit ju, batch row b0 + 2 * ft + jb (accumulator fragment elements 2*kh + jb) ---
   const int fg = lane >> 2, ft = lane & 3;
   const int u0 = ug * 16 + kh * 8;  // first unit (within the CTA's slice) this warp finishes
+  // F16: the n tile's A fragments of this warp's k-blocks in registers, [slice in visiting order][k-block][hi, lo], and
+  // the unscale 2^-(e_r + 14) of the lane's three rows (read before anyone writes `red` in the step loop)
+  uint32_t wreg[F16 ? C : 1][KBC / 2][2][4];
+  float unscale[G];
+  if constexpr (F16) {
+#pragma unroll
+    for (int c = 0; c < C; ++c)
+#pragma unroll
+      for (int kk = 0; kk < KBC / 2; ++kk)
+#pragma unroll
+        for (int hl = 0; hl < 2; ++hl) {
+          const int kb = ((c + (int)rank) % C) * KBC + kh * (KBC / 2) + kk;
+          const uint4 v = *reinterpret_cast<const uint4*>(W_h + h16::w_half(ug, G - 1, kb, hl, lane, 0, 0));
+          wreg[c][kk][hl][0] = v.x; wreg[c][kk][hl][1] = v.y; wreg[c][kk][hl][2] = v.z; wreg[c][kk][hl][3] = v.w;
+        }
+#pragma unroll
+    for (int g = 0; g < G; ++g) unscale[g] = __frcp_rn(scl[g * HS + u0 + fg]) * (1.f / h16::STATE_SCALE);
+  }
+  ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
   const int ju = j0 + u0 + fg;
   FwdCell<B200RNN_GRU, H, VL> cell[2] = {{p, dir, ju, b0 + 2 * ft}, {p, dir, ju, b0 + 2 * ft + 1}};
   GiReady gi_ready;
@@ -612,6 +681,34 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
         for (int m = 0; m < 2; ++m)
 #pragma unroll
           for (int i = 0; i < 4; ++i) d[g][m][i] = 0.f;
+      if constexpr (F16) {  // k-blocks of 16: this warp takes k-blocks kh*2, kh*2 + 1 of every source slice
+        const uint4* h_q = reinterpret_cast<const uint4*>(h_s + cur * BS * H) + h16::state_slot(lane);
+#pragma unroll
+        for (int kk = 0; kk < KBC / 2; ++kk) {
+          const int kb = src * KBC + kh * (KBC / 2) + kk;
+          const uint4 hv = h_q[kb * 32];  // {hi b0, hi b1, lo b0, lo b1}
+          const uint32_t bh[2] = {hv.x, hv.y}, bl[2] = {hv.z, hv.w};
+#pragma unroll
+          for (int g = 0; g < G; ++g) {
+            uint32_t ah[4], al[4];
+            if (g < G - 1) {
+              const uint4* wp = reinterpret_cast<const uint4*>(W_h + h16::w_half(ug, g, kb, 0, lane, 0, 0));
+              const uint4 vh = wp[0], vl = wp[32];  // hi, then lo: 32 lanes x 16 bytes further
+              ah[0] = vh.x; ah[1] = vh.y; ah[2] = vh.z; ah[3] = vh.w;
+              al[0] = vl.x; al[1] = vl.y; al[2] = vl.z; al[3] = vl.w;
+            } else {
+#pragma unroll
+              for (int r = 0; r < 4; ++r) {
+                ah[r] = wreg[c][kk][0][r];
+                al[r] = wreg[c][kk][1][r];
+              }
+            }
+            ptx::mma_f16_m16n8k16(d[g][0], al, bh);
+            ptx::mma_f16_m16n8k16(d[g][0], ah, bl);
+            ptx::mma_f16_m16n8k16(d[g][1], ah, bh);
+          }
+        }
+      } else {
 #pragma unroll
       for (int kk = 0; kk < KSC / 2; ++kk) {
         const int ks = src * KSC + kh * (KSC / 2) + kk;
@@ -643,6 +740,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
           }
         }
       }
+      }
 #pragma unroll
       for (int g = 0; g < G; ++g)
 #pragma unroll
@@ -671,6 +769,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
 #pragma unroll
       for (int jb = 0; jb < 2; ++jb) {
         pre[jb][g] = (kh ? acc[g][2 + jb] : acc[g][jb]) + red_partner[(g * 2 + jb) * 32];
+        if constexpr (F16) pre[jb][g] *= unscale[g];
       }
     float hnew[2];
 #pragma unroll
@@ -680,8 +779,20 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
       // own copy with ordinary stores; after __syncwarp the warp's k-step is 16 contiguous float4 that go to the peers
       // with st.async (ordering of the local path: allgather_units)
       float* h_nxt = h_s + nxt * BS * H;
+      if constexpr (F16) {  // the pair of the scaled state; the cell keeps the fp32 h (h16::exchange_chunk is the
+                            // 16-byte chunk index lane * 4 floats below points at)
+        __half* h_h = reinterpret_cast<__half*>(h_nxt);
 #pragma unroll
-      for (int jb = 0; jb < 2; ++jb) h_nxt[tc_state_index(ju, 2 * ft + jb)] = TF32 ? round_tf32(hnew[jb]) : hnew[jb];
+        for (int jb = 0; jb < 2; ++jb) {
+          const float v = hnew[jb] * h16::STATE_SCALE;
+          const __half hi = __float2half_rn(v);
+          h_h[h16::state_index(ju, 2 * ft + jb, 0)] = hi;
+          h_h[h16::state_index(ju, 2 * ft + jb, 1)] = __float2half_rn(v - __half2float(hi));
+        }
+      } else {
+#pragma unroll
+        for (int jb = 0; jb < 2; ++jb) h_nxt[tc_state_index(ju, 2 * ft + jb)] = TF32 ? round_tf32(hnew[jb]) : hnew[jb];
+      }
       __syncwarp();
       if (lane < 16) {
         float* mine = h_nxt + (j0 + u0) / 8 * 64 + lane * 4;
@@ -715,14 +826,18 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
 }
 
-// 3xTF32 (the default) and single-pass TF32 instantiations, fixed-length and ragged
+// 3xTF32 (the default), single-pass TF32 and fp16-pair instantiations, fixed-length and ragged
 template <bool VL>
 __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFwdParams p, const int nslices) {
-  rec_fwd_tc_body<VL, false>(p, nslices);
+  rec_fwd_tc_body<VL, TcOp::X3>(p, nslices);
 }
 template <bool VL>
 __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tf32_kernel(const RecFwdParams p, const int nslices) {
-  rec_fwd_tc_body<VL, true>(p, nslices);
+  rec_fwd_tc_body<VL, TcOp::TF32>(p, nslices);
+}
+template <bool VL>
+__global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_h16_kernel(const RecFwdParams p, const int nslices) {
+  rec_fwd_tc_body<VL, TcOp::F16>(p, nslices);
 }
 
 // =================================================================================================
@@ -1536,15 +1651,19 @@ bool pick_fwd(const RecFwdParams& p, bool force, RecFwdLaunch* L, int* rc) {
                         "fwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d PB=%d", C, BS, KL, UPL, RG, (int)PB);
 }
 
-// the tensor-core config is the widest-cluster one: it is always taken (several waves when its clusters do not all fit)
+// the tensor-core config is the widest-cluster one: it is always taken (several waves when its clusters do not all fit).
+// Its contraction: single-pass TF32 in TF32 mode, else fp16 pairs for the no-grad forward of b200rnn_forward_fused
+// (no initial state there, see rec_fwd_h16_kernel), else 3xTF32
 int pick_fwd_tc(const RecFwdParams& p, RecFwdLaunch* L) {
   using Cfg = TcFwdCfg;
   static_assert(Cfg::SMEM <= MAX_SMEM, "forward config does not fit an SM");
+  const bool h16 = !p.tf32 && p.shell_nograd;
   auto k = p.tf32 ? (p.lengths ? rec_fwd_tf32_kernel<true> : rec_fwd_tf32_kernel<false>)
+           : h16  ? (p.lengths ? rec_fwd_h16_kernel<true> : rec_fwd_h16_kernel<false>)
                   : (p.lengths ? rec_fwd_tc_kernel<true> : rec_fwd_tc_kernel<false>);
   int rc = B200RNN_OK;
   pick_clustered(k, p, Cfg::C, Cfg::BS, Cfg::NT, Cfg::SMEM, true, L, &rc, "fwd cfg tc8 C=%d BS=%d mma.sync %s",
-                 Cfg::C, Cfg::BS, p.tf32 ? "TF32" : "3xTF32");
+                 Cfg::C, Cfg::BS, p.tf32 ? "TF32" : h16 ? "f16x3" : "3xTF32");
   return rc;
 }
 
@@ -1673,6 +1792,10 @@ int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s)
   if (p.B <= 0 || p.T <= 0) return B200RNN_OK;
   if (p.ready && p.D != 1) {  // GiReady walks the row tiles in increasing t
     set_error("recurrence: a streamed x-projection needs a unidirectional layer");
+    return B200RNN_ERR_INVALID;
+  }
+  if (p.shell_nograd && p.h_0) {  // the fp16-pair state scale assumes |h| <= 1
+    set_error("recurrence: the no-grad fused forward takes no initial state");
     return B200RNN_ERR_INVALID;
   }
   return launch_clustered(L, p, PROF_REC_FWD, p.ready != nullptr, s);
