@@ -83,14 +83,18 @@ struct RecBwdParams {
   const float* w_hr[2];      // per direction [P, H]
   float* dhp[2];             // out: per direction [T,B,P]
 };
+using RecBwdLaunch = ClusterLaunch<RecBwdParams>;
 
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)
 int rec_bwd_max_slices(int B);
 
-// forward: choose the config for p's shape (mode, H, B, D, lengths or not), then launch it; p.ready != NULL launches
+// forward: choose the config for p's shape (mode, H, P, B, D, lengths or not), then launch it; p.ready != NULL launches
 // it with programmatic stream serialization, so that it may start while the GEMM before it still runs
 int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* out);
 int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t stream);
+// backward: the same choice (plan_rec_bwd), then one launch that also prepares W_hh for the unprojected kernels and sets
+// p.nslices_out
+int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* out);
 int launch_rec_bwd(RecBwdParams& p, cudaStream_t stream);
 
 }  // namespace b200rnn

@@ -27,6 +27,7 @@
 #include <map>
 #include <mutex>
 #include <stdlib.h>
+#include <type_traits>
 #include <utility>
 
 #include <cuda_fp16.h>
@@ -43,10 +44,12 @@ namespace {
 
 constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_90
 // The CTA's own state slice is delivered locally (st.shared + mbarrier.arrive per warp). -DB200RNN_SELF_VIA_CLUSTER
-// builds the round-1 behaviour (own slice through st.async like the peers'): compute-sanitizer's racecheck does not
-// model the ordering that inline-PTX mbarrier.arrive / try_wait give to ordinary shared-memory stores and flags every
-// local store / LDS pair of the default build, so the race-free evidence of the REST of the kernel is taken on that
-// build; the ordering argument for the local path is in allgather_units' comment.
+// builds the round-1 behaviour (own slice through st.async like the peers') for the FFMA kernels rec_fwd_kernel and
+// rec_bwd_kernel only: compute-sanitizer's racecheck does not model the ordering that inline-PTX mbarrier.arrive /
+// try_wait give to ordinary shared-memory stores and flags every local store / LDS pair of the default build, so the
+// race-free evidence of the REST of those kernels is taken on that build; the ordering argument for the local path is in
+// allgather_units' comment. The tc8 kernels always deliver the own slice locally (sending it through the cluster would
+// need a staging buffer), and the projected kernels never send to or wait on their own slot.
 #ifdef B200RNN_SELF_VIA_CLUSTER
 constexpr bool kLocalSelf = false;
 #else
@@ -54,9 +57,12 @@ constexpr bool kLocalSelf = true;
 #endif
 constexpr unsigned FULLMASK = 0xffffffffu;
 
+// gate blocks of the cell: GRU r, z, n; LSTM i, f, g, o
+constexpr int gates_of(int mode) { return mode == B200RNN_GRU ? 3 : 4; }
+
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
 struct RecCfg {
-  static constexpr int G = (MODE == B200RNN_GRU) ? 3 : 4;
+  static constexpr int G = gates_of(MODE);
   static constexpr int GH = G * H;
   static constexpr int HS = H / C;
   static constexpr int UPW = (32 / KL) * UPL;  // units per warp
@@ -80,6 +86,95 @@ struct RecCfg {
   static_assert(UPW % 4 == 0, "the exchange packs 4 units per 16-byte store");
   static_assert(NT <= 1024, "too many threads");
 };
+
+// VL: the steps a cluster runs, the length of its first batch slot (the longest: order sorts by descending length)
+__device__ __forceinline__ int slice_steps(const int* lengths, const int* order, int b0, int T) {
+  return min(max(lengths[order[b0]], 0), T);
+}
+
+// What a CTA owns: cluster blockIdx.x / C runs direction `dir` of batch slice `slice` (slots b0 .. b0 + BS - 1), and
+// CTA `rank` of it the HS units from j0. T is the number of steps the cluster runs: p.T, or under VL its longest row's.
+struct ClusterSlice {
+  uint32_t rank;
+  int dir, slice, b0, j0, T;
+};
+
+template <int C, int BS, int HS, bool VL, typename Params>
+__device__ __forceinline__ ClusterSlice cluster_slice(const Params& p, int nslices) {
+  ClusterSlice s;
+  s.rank = ptx::cluster_ctarank();
+  const int cid = blockIdx.x / C;
+  s.dir = cid / nslices;
+  s.slice = cid - s.dir * nslices;
+  s.b0 = s.slice * BS;
+  s.j0 = (int)s.rank * HS;
+  s.T = VL ? slice_steps(p.lengths, p.order, s.b0, p.T) : p.T;
+  return s;
+}
+
+// The [2][C] mbarriers of a double-buffered exchange between the C CTAs of a cluster: bar(buf, src) completes when the
+// slice of source CTA `src` has landed in buffer `buf`. Remote sources complete transaction bytes, one expect_tx per
+// exchange re-armed by thread 0 (arm). LOCAL_SELF: the own slice is delivered locally, with ordinary stores published by
+// plain arrives (the own barrier's arrival count, init), and is never armed.
+// Step s contracts against buffer s & 1, which holds what step s - LAG sent (LAG = 1: the forward kernels and the
+// projected BPTT; LAG = 0: rec_bwd_kernel, which contracts in the step that sends). Each buffer carries every other
+// exchange, so the wait of step s is for phase ((s - LAG) >> 1) & 1. Thread 0 arms a buffer for the next exchange only
+// after its own waits on that buffer's previous phase have passed.
+// The barriers are bars[FIRST + buf * C + src]: FIRST = 1 where bars[0] is the weight barrier of the FFMA kernels.
+template <int C, int LAG, bool LOCAL_SELF, int FIRST = 0>
+struct ExchangeBars {
+  uint64_t* bars;
+  uint32_t rank;
+
+  static __device__ __forceinline__ int buf(int s) { return s & 1; }
+  static __device__ __forceinline__ uint32_t parity(int s) { return ((s - LAG) >> 1) & 1; }
+  __device__ __forceinline__ uint64_t* bar(int b, int src) const { return &bars[FIRST + b * C + src]; }
+
+  // thread 0, before fence_mbar_init
+  __device__ __forceinline__ void init(uint32_t self_arrivals) const {
+    for (int i = 0; i < 2 * C; ++i)
+      ptx::mbar_init(&bars[FIRST + i], (LOCAL_SELF && (uint32_t)(i % C) == rank) ? self_arrivals : 1u);
+  }
+  // thread 0: buffer b expects `bytes` from every source that sends through the cluster
+  __device__ __forceinline__ void arm(int b, uint32_t bytes) const {
+#pragma unroll
+    for (int src = 0; src < C; ++src)
+      if (!LOCAL_SELF || (uint32_t)src != rank) ptx::mbar_arrive_expect_tx(bar(b, src), bytes);
+  }
+  // the slice of source `src` has landed in buffer b = buf(s), phase par = parity(s) (computed once per step)
+  __device__ __forceinline__ void wait(int b, int src, uint32_t par) const { ptx::mbar_wait(bar(b, src), par); }
+};
+
+// The LSTM cell, forward: gate pre-activations gi + pre -> activated gates, c_t and o * tanh(c_t)
+struct LstmStep {
+  float i, f, g, o, c, h;
+};
+
+__device__ __forceinline__ LstmStep lstm_cell_fwd(const float (&gi)[4], const float (&pre)[4], float c) {
+  LstmStep s;
+  s.i = sigmoid_f(gi[0] + pre[0]);
+  s.f = sigmoid_f(gi[1] + pre[1]);
+  s.g = tanh_f(gi[2] + pre[2]);
+  s.o = sigmoid_f(gi[3] + pre[3]);
+  s.c = fmaf(s.f, c, s.i * s.g);  // spelled out: which product is fused must not be left to the compiler
+  s.h = s.o * tanh_f(s.c);
+  return s;
+}
+
+// The LSTM cell, backward: from the saved gates sv = (i, f, g, o), c_t, c_{t-1}, the gradient dh of o * tanh(c_t) and
+// the carried dc, the gate gradients dg; returns the dc carried to step t - 1
+__device__ __forceinline__ float lstm_cell_bwd(const float (&sv)[4], float c_t, float c_prev, float dh, float dc_carry,
+                                               float (&dg)[4]) {
+  const float ig = sv[0], fg = sv[1], gg = sv[2], og = sv[3];
+  const float tc = tanh_f(c_t);
+  const float dout = dh * tc * og * (1.f - og);
+  const float dc = dc_carry + dh * og * (1.f - tc * tc);
+  dg[0] = dc * gg * ig * (1.f - ig);
+  dg[1] = dc * c_prev * fg * (1.f - fg);
+  dg[2] = dc * ig * (1.f - gg * gg);
+  dg[3] = dout;
+  return dc * fg;
+}
 
 // All-gather `val` (owned by lane (unit, batch) of every warp) into vec[b][col0 + unit] of all C CTAs:
 // 4 shuffles gather 4 consecutive units, one 16-byte store per (destination, chunk).
@@ -155,7 +250,7 @@ __device__ __forceinline__ void allgather_units(float val, float* vec_local, int
 // hn = (W_hn h_{t-1})_j + b_hn (GRU) or c_t (LSTM).
 template <int MODE, int H, bool VL>
 struct FwdCell {
-  static constexpr int G = (MODE == B200RNN_GRU) ? 3 : 4;
+  static constexpr int G = gates_of(MODE);
   float* gates;
   float* extra;
   int j, b, len;
@@ -209,12 +304,9 @@ struct FwdCell {
       }
       s[0] = r; s[1] = z; s[2] = n; sx = hn;
     } else {
-      const float ig = sigmoid_f(gi[0] + pre[0]);
-      const float fg = sigmoid_f(gi[1] + pre[1]);
-      const float gg = tanh_f(gi[2] + pre[2]);
-      const float og = sigmoid_f(gi[3] + pre[3]);
-      float cnew = fmaf(fg, c, ig * gg);  // spelled out: which product is fused must not be left to the compiler
-      hnew = og * tanh_f(cnew);
+      const LstmStep st = lstm_cell_fwd(gi, pre, c);
+      float cnew = st.c;
+      hnew = st.h;
       if constexpr (VL) {
         if (t >= len) {
           cnew = c;
@@ -222,7 +314,7 @@ struct FwdCell {
         }
       }
       c = cnew;
-      s[0] = ig; s[1] = fg; s[2] = gg; s[3] = og; sx = cnew;
+      s[0] = st.i; s[1] = st.f; s[2] = st.g; s[3] = st.o; sx = cnew;
     }
     h = hnew;
     float yv = hnew;  // what the caller sees at this step
@@ -268,11 +360,6 @@ struct FwdCell {
   }
 };
 
-// VL: the steps a cluster runs, the length of its first batch slot (the longest: order sorts by descending length)
-__device__ __forceinline__ int slice_steps(const int* lengths, const int* order, int b0, int T) {
-  return min(max(lengths[order[b0]], 0), T);
-}
-
 // Initial value of element (unit k, batch slot q) of the shared state buffer the first step contracts against: h_0 of
 // the row in slot b0 + q (zero past the batch). Every CTA fills its whole buffer from global memory, so step 0 needs no
 // exchange; the caller tests p.h_0 (uniform) and zero-fills without it. Branch-free per lane, like FwdCell's load.
@@ -308,7 +395,7 @@ struct GiReady {
   }
 };
 
-// PB = true: batch-paired contraction and state layout (rnn_core.cuh, dots_chunk2b), see launch_rec_fwd
+// PB = true: batch-paired contraction and state layout (rnn_core.cuh, dots_chunk2b), see plan_rec_fwd
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false, bool PB = false>
 __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     rec_fwd_kernel(const RecFwdParams p, const int nslices) {
@@ -322,20 +409,16 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
   constexpr int NCH = Cfg::NCH, CPS = Cfg::CPS;
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int cid = blockIdx.x / C;
-  const int dir = cid / nslices;
-  const int slice = cid - dir * nslices;
-  const int b0 = slice * BS;
-  const int j0 = (int)rank * HS;
-  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
+  const ClusterSlice cs = cluster_slice<C, BS, HS, VL>(p, nslices);
+  const uint32_t rank = cs.rank;
+  const int dir = cs.dir, b0 = cs.b0, j0 = cs.j0, T = cs.T;
   const float* w_hh = p.w_hh[dir];
+  // step s contracts against the state step s - 1 sent; step 0 against the initial state in buffer 0
+  const ExchangeBars<C, 1, kLocalSelf, 1> xb{bars, rank};
 
   if (tid == 0) {
-    // [0]: weights (tx bytes). [1 + buf*C + src]: slice of source CTA `src` - remote sources complete tx bytes
-    // (one arrive.expect_tx by thread 0 per phase), the CTA's OWN slice is published by one plain arrive per warp
-    for (int i = 0; i < Cfg::NBAR; ++i)
-      ptx::mbar_init(&bars[i], (kLocalSelf && i >= 1 && (uint32_t)((i - 1) % C) == rank) ? (uint32_t)Cfg::NW : 1u);
+    ptx::mbar_init(&bars[0], 1u);  // weights (tx bytes)
+    xb.init((uint32_t)Cfg::NW);    // the own slice: one arrive per warp
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -374,10 +457,10 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 
   for (int step = 0; step < T; ++step) {
     const int t = dir ? (T - 1 - step) : step;
-    const int cur = step & 1, nxt = cur ^ 1;
+    const int cur = xb.buf(step), nxt = cur ^ 1;
     const float* h_cur = h_s + cur * BS * H;
     float* h_nxt = h_s + nxt * BS * H;
-    const uint32_t par = ((step - 1) >> 1) & 1;
+    const uint32_t par = xb.parity(step);
 #ifdef B200RNN_TRACE
     const bool tr = p.trace != nullptr && blockIdx.x == 0 && lane == 0;  // one row of 8 stamps per (step, warp)
 #else
@@ -411,10 +494,10 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       const int ca = (c + rot) % NCH;
       if (step > 0) {
         if (Cfg::ROT) {
-          if (c % CPS == 0) ptx::mbar_wait(&bars[1 + cur * C + ca / CPS], par);
+          if (c % CPS == 0) xb.wait(cur, ca / CPS, par);
         } else {
 #pragma unroll
-          for (int s2 = 0; s2 < Cfg::SPC; ++s2) ptx::mbar_wait(&bars[1 + cur * C + ca * Cfg::SPC + s2], par);
+          for (int s2 = 0; s2 < Cfg::SPC; ++s2) xb.wait(cur, ca * Cfg::SPC + s2, par);
         }
       }
       if (tr && c < 4) trow[1 + c] = clock64();     // slice of chunk c has arrived (this warp passed its wait)
@@ -427,12 +510,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       if (c == 0 && step > 0) cell.flush(p, dir, dir ? (T - step) : (step - 1));  // the previous step's stores
     }
     // every slice of h_step has been consumed by this thread => the barriers of the other buffer are re-armed
-    if (tid == 0 && step + 1 < T) {
-#pragma unroll
-      for (int src = 0; src < C; ++src)
-        if (!kLocalSelf || (uint32_t)src != rank)
-          ptx::mbar_arrive_expect_tx(&bars[1 + nxt * C + src], (uint32_t)(BS * HS * sizeof(float)));
-    }
+    if (tid == 0 && step + 1 < T) xb.arm(nxt, (uint32_t)(BS * HS * sizeof(float)));
     if constexpr (PACKB) {
       float red[G];
       warp_transpose_reduce2b<G, KL, UPL, BS>(acc2b, red, lane);
@@ -451,8 +529,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     if (tr) trow[6] = clock64() + (long long)(hnew == 12345.678f);          // gate math done
 
     if (step + 1 < T)
-      allgather_units<C, KL, UPL, BS, kLocalSelf, PACKB>(hnew, h_nxt, H, j0 + w * UPW, &bars[1 + nxt * C + rank], lane,
-                                                         rank);
+      allgather_units<C, KL, UPL, BS, kLocalSelf, PACKB>(hnew, h_nxt, H, j0 + w * UPW, xb.bar(nxt, rank), lane, rank);
     if (tr) trow[7] = clock64();                                            // exchange issued
 
     if (step == T - 1) {
@@ -553,19 +630,15 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int ug = w % NUG, kh = w / NUG;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int cid = blockIdx.x / C;
-  const int dir = cid / nslices;
-  const int slice = cid - dir * nslices;
-  const int b0 = slice * BS;
-  const int j0 = (int)rank * HS;
-  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
+  const ClusterSlice cs = cluster_slice<C, BS, HS, VL>(p, nslices);
+  const uint32_t rank = cs.rank;
+  const int dir = cs.dir, b0 = cs.b0, j0 = cs.j0, T = cs.T;
   const float* w_hh = p.w_hh[dir];
+  // as in rec_fwd_kernel, but the own slice is always delivered locally
+  const ExchangeBars<C, 1, true> xb{bars, rank};
 
   if (tid == 0) {
-    // remote sources complete tx bytes (one arrive.expect_tx by thread 0 per phase), the own slice is published by one
-    // plain arrive per warp
-    for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], (uint32_t)(i % C) == rank ? (uint32_t)NW : 1u);
+    xb.init((uint32_t)NW);  // the own slice: one arrive per warp
     ptx::fence_mbar_init();
   }
   if constexpr (F16) {  // the row scales: one warp per row
@@ -660,9 +733,9 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   for (int jb = 0; jb < 2; ++jb) cell[jb].start(p, dir);
   for (int step = 0; step < T; ++step) {
     const int t = dir ? (T - 1 - step) : step;
-    const int cur = step & 1, nxt = cur ^ 1;
+    const int cur = xb.buf(step), nxt = cur ^ 1;
     const float2* h_cur = reinterpret_cast<const float2*>(h_s + cur * BS * H) + lane;
-    const uint32_t par = ((step - 1) >> 1) & 1;
+    const uint32_t par = xb.parity(step);
 
     float acc[G][4];
 #pragma unroll
@@ -673,7 +746,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
 #pragma unroll
     for (int c = 0; c < C; ++c) {
       const int src = (c + (int)rank) % C;
-      if (step > 0) ptx::mbar_wait(&bars[cur * C + src], par);
+      if (step > 0) xb.wait(cur, src, par);
       float d[G][2][4];  // [gate tile][lo*hi + hi*lo, hi*hi]; TF32: [gate tile][-, the single product]
 #pragma unroll
       for (int g = 0; g < G; ++g)
@@ -751,11 +824,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
       }
     }
     // every slice of h_step has been consumed by this thread => the barriers of the other buffer are re-armed
-    if (tid == 0 && step + 1 < T) {
-#pragma unroll
-      for (int src = 0; src < C; ++src)
-        if ((uint32_t)src != rank) ptx::mbar_arrive_expect_tx(&bars[nxt * C + src], (uint32_t)(BS * HS * sizeof(float)));
-    }
+    if (tid == 0 && step + 1 < T) xb.arm(nxt, (uint32_t)(BS * HS * sizeof(float)));
     // swap halves with the partner warp: it finishes the other 8 units. WAR on `red`: the partner overwrites it only
     // after its next step's own-slice wait, which needs this warp's arrive below (after the read).
 #pragma unroll
@@ -797,14 +866,14 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
       if (lane < 16) {
         float* mine = h_nxt + (j0 + u0) / 8 * 64 + lane * 4;
         const float4 v = *reinterpret_cast<const float4*>(mine);
-        const uint32_t dst = ptx::smem_u32(mine), bar = ptx::smem_u32(&bars[nxt * C + rank]);
+        const uint32_t dst = ptx::smem_u32(mine), bar = ptx::smem_u32(xb.bar(nxt, rank));
 #pragma unroll
         for (int r = 1; r < C; ++r) {
           const uint32_t peer = (rank + r) % C;
           ptx::st_async_v4(ptx::mapa(dst, peer), v, ptx::mapa(bar, peer));
         }
       }
-      if (lane == 0) ptx::mbar_arrive(&bars[nxt * C + rank]);
+      if (lane == 0) ptx::mbar_arrive(xb.bar(nxt, rank));
     }
 
     if (step == T - 1) {
@@ -879,20 +948,17 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
   constexpr int NCH = Cfg::NCH, CPS = Cfg::CPS, SPC = Cfg::SPC;
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int cid = blockIdx.x / C;
-  const int dir = cid / nslices;
-  const int slice = cid - dir * nslices;
-  const int b0 = slice * BS;
-  const int j0 = (int)rank * HS;
+  const ClusterSlice cs = cluster_slice<C, BS, HS, VL>(p, nslices);
+  const uint32_t rank = cs.rank;
+  const int dir = cs.dir, slice = cs.slice, b0 = cs.b0, j0 = cs.j0, T = cs.T;
   const int B = p.B;
-  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
   const float* w_prep = p.w_prep[dir] + (size_t)rank * G * HS * H;
+  // step s contracts against the gate gradients it sent itself
+  const ExchangeBars<C, 0, kLocalSelf, 1> xb{bars, rank};
 
   if (tid == 0) {
-    // as in the forward: the own slice is delivered locally (G gate-gradient slices x NW warps arrive per phase)
-    for (int i = 0; i < Cfg::NBAR; ++i)
-      ptx::mbar_init(&bars[i], (kLocalSelf && i >= 1 && (uint32_t)((i - 1) % C) == rank) ? (uint32_t)(Cfg::NW * G) : 1u);
+    ptx::mbar_init(&bars[0], 1u);          // weights (tx bytes)
+    xb.init((uint32_t)(Cfg::NW * G));      // the own slice: G gate-gradient slices x NW warps arrive per exchange
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -967,16 +1033,11 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
   const bool want_dh0 = p.dh_0 != nullptr;
   for (int step = 0; step < T; ++step) {
     const int t = dir ? step : (T - 1 - step);
-    const int buf = step & 1;
+    const int buf = xb.buf(step);
     float* d_buf = d_s + buf * BS * GH;
     const bool last = (step == T - 1);
     const bool contract = !last || want_dh0;
-    if (tid == 0 && contract) {
-#pragma unroll
-      for (int src = 0; src < C; ++src)
-        if (!kLocalSelf || (uint32_t)src != rank)
-          ptx::mbar_arrive_expect_tx(&bars[1 + buf * C + src], (uint32_t)(BS * G * HS * sizeof(float)));
-    }
+    if (tid == 0 && contract) xb.arm(buf, (uint32_t)(BS * G * HS * sizeof(float)));
 
     // ---- cell backward for (unit j, batch b) ----------------------------------------------------
     float dh = dh_carry + dyv;
@@ -984,7 +1045,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       if (t >= len_b) dh = dh_carry;  // the output of a frozen step is the constant 0: its dy reaches nothing
     }
     float dg[G], direct, dhn = 0.f;
-    if (MODE == B200RNN_GRU) {
+    if constexpr (MODE == B200RNN_GRU) {
       const float r = sv[0], z = sv[1], n = sv[2], hn = sx;
       const float dn = dh * (1.f - z) * (1.f - n * n);
       const float dz = dh * (hp - n) * z * (1.f - z);
@@ -993,15 +1054,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
       dg[0] = dr; dg[1] = dz; dg[2] = dn;
       direct = dh * z;
     } else {
-      const float ig = sv[0], fg = sv[1], gg = sv[2], og = sv[G - 1];
-      const float tc = tanh_f(sx);
-      const float dout = dh * tc * og * (1.f - og);
-      const float dc = dc_carry + dh * og * (1.f - tc * tc);
-      dg[0] = dc * gg * ig * (1.f - ig);
-      dg[1] = dc * hp * fg * (1.f - fg);
-      dg[2] = dc * ig * (1.f - gg * gg);
-      dg[G - 1] = dout;
-      const float dc_next = dc * fg;
+      const float dc_next = lstm_cell_bwd(sv, sx, hp, dh, dc_carry, dg);
       direct = 0.f;
       if constexpr (VL) {
         if (t >= len_b) direct = dh;  // frozen step: dh and dc pass straight through
@@ -1031,8 +1084,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
         float v = dg[g];
         if (MODE == B200RNN_GRU && g == 2) v = dhn;
         if (!valid) v = 0.f;
-        allgather_units<C, KL, UPL, BS, kLocalSelf>(v, d_buf, GH, g * H + j0 + w * UPW, &bars[1 + buf * C + rank],
-                                                    lane, rank);
+        allgather_units<C, KL, UPL, BS, kLocalSelf>(v, d_buf, GH, g * H + j0 + w * UPW, xb.bar(buf, rank), lane, rank);
       }
     }
 
@@ -1044,7 +1096,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     }
     if (!contract) break;
     if (valid && !last) load_step(step + 1);
-    const uint32_t par = (step >> 1) & 1;
+    const uint32_t par = xb.parity(step);
 
     // ---- dh_{prev}[b][j] = direct + sum_col dgh[b][col] * W_hh[col][j], one gate block of columns at a time ----
     // even-k / odd-k partial sums in one float2 accumulator (two independent FMA chains), folded before the butterfly
@@ -1059,10 +1111,10 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     for (int c = 0; c < NCH; ++c) {
       const int ca = (c + rot) % NCH;
       if (Cfg::ROT) {
-        if (c % CPS == 0) ptx::mbar_wait(&bars[1 + buf * C + ca / CPS], par);
+        if (c % CPS == 0) xb.wait(buf, ca / CPS, par);
       } else {
 #pragma unroll
-        for (int s2 = 0; s2 < SPC; ++s2) ptx::mbar_wait(&bars[1 + buf * C + ca * SPC + s2], par);
+        for (int s2 = 0; s2 < SPC; ++s2) xb.wait(buf, ca * SPC + s2, par);
       }
 #pragma unroll
       for (int g = 0; g < G; ++g) {
@@ -1239,17 +1291,15 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
   int* len_s = row_s + BS;                                      // [BS] steps of each slot
 
   const int tid = threadIdx.x;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int cid = blockIdx.x / C;
-  const int dir = cid / nslices;
-  const int slice = cid - dir * nslices;
-  const int b0 = slice * BS;
-  const int j0 = (int)rank * HS;
+  const ClusterSlice cs = cluster_slice<C, BS, HS, VL>(p, nslices);
+  const uint32_t rank = cs.rank;
+  const int dir = cs.dir, b0 = cs.b0, j0 = cs.j0, T = cs.T;
   const int B = p.B;
-  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;  // steps this cluster runs
+  // step s sums the partials step s - 1 sent; the own slot is never awaited
+  const ExchangeBars<C, 1, true> xb{bars, rank};
 
   if (tid == 0) {
-    for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], 1u);
+    xb.init(1u);
     ptx::fence_mbar_init();
   }
   proj_prologue<H, P, C, BS, VL>(p.w_hh[dir], p.w_hr[dir], j0, b0, B, p.T, p.lengths, p.order, W_s, R_s, row_s, len_s,
@@ -1280,12 +1330,12 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
   for (int step = 0; step <= T; ++step) {
     // ---- h of the previous step: the C partials in rank order; this CTA's columns of y --------------------------
     if (step > 0) {
-      const int cur = step & 1;
+      const int cur = xb.buf(step);
       const int tp = dir ? T - step : step - 1;
-      const uint32_t par = ((step - 1) >> 1) & 1;
+      const uint32_t par = xb.parity(step);
 #pragma unroll
       for (int src = 0; src < C; ++src)
-        if ((uint32_t)src != rank) ptx::mbar_wait(&bars[cur * C + src], par);
+        if ((uint32_t)src != rank) xb.wait(cur, src, par);
       const float* sl = slot + (size_t)cur * C * BS * P;
       for (int i = tid; i < BS * P; i += NT) {
         const int q = i / P, k = i - q * P;
@@ -1301,12 +1351,9 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
     }
     if (step == T) break;
     const int t = dir ? T - 1 - step : step;
-    const int nb = (step + 1) & 1;
-    if (tid == 0) {  // this step's partials land in buffer nb; its previous phase was consumed at step - 1
-#pragma unroll
-      for (int src = 0; src < C; ++src)
-        if ((uint32_t)src != rank) ptx::mbar_arrive_expect_tx(&bars[nb * C + src], (uint32_t)(BS * P * sizeof(float)));
-    }
+    const int nb = xb.buf(step) ^ 1;
+    // this step's partials land in buffer nb; its previous phase was consumed at step - 1
+    if (tid == 0) xb.arm(nb, (uint32_t)(BS * P * sizeof(float)));
     // ---- gates, cell, m = o * tanh(c) ----------------------------------------------------------------------------
     float acc[G];
 #pragma unroll
@@ -1325,12 +1372,9 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
         acc[g] = a;
       }
     }
-    const float ig = sigmoid_f(gi[0] + acc[0]);
-    const float fg = sigmoid_f(gi[1] + acc[1]);
-    const float gg = tanh_f(gi[2] + acc[2]);
-    const float og = sigmoid_f(gi[3] + acc[3]);
-    float cnew = fmaf(fg, c, ig * gg);
-    float m = og * tanh_f(cnew);
+    const LstmStep st = lstm_cell_fwd(gi, acc, c);
+    float cnew = st.c;
+    float m = st.h;
     if (VL && t >= len) {
       cnew = c;
       m = 0.f;
@@ -1339,7 +1383,7 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
     m_s[b * HS + u] = valid ? m : 0.f;
     if (valid && p.training) {
       float* gp = gates + ((size_t)t * B + row) * (G * H) + j;
-      gp[0] = ig; gp[H] = fg; gp[2 * H] = gg; gp[3 * H] = og;
+      gp[0] = st.i; gp[H] = st.f; gp[2 * H] = st.g; gp[3 * H] = st.o;
       p.extra[dir][((size_t)t * B + row) * H + j] = cnew;
       p.m[dir][((size_t)t * B + row) * H + j] = m;
     }
@@ -1349,7 +1393,7 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
     float* own = slot + ((size_t)nb * C + rank) * BS * P;
     proj_partial<P, BS, Cfg::NG, Cfg::RB, HS>(R_s, LD, m_s, own, tid);
     __syncthreads();
-    proj_send<P, C, BS, NT>(own, &bars[nb * C + rank], rank, tid);
+    proj_send<P, C, BS, NT>(own, xb.bar(nb, rank), rank, tid);
   }
   // ---- final state: h_n (this CTA's columns of h_s) and c_n; VL: the steps [T, p.T) the cluster skipped ----------
   for (int i = tid; i < BS * P; i += NT) {
@@ -1384,17 +1428,15 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
   int* len_s = row_s + BS;
 
   const int tid = threadIdx.x;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int cid = blockIdx.x / C;
-  const int dir = cid / nslices;
-  const int slice = cid - dir * nslices;
-  const int b0 = slice * BS;
-  const int j0 = (int)rank * HS;
+  const ClusterSlice cs = cluster_slice<C, BS, HS, VL>(p, nslices);
+  const uint32_t rank = cs.rank;
+  const int dir = cs.dir, slice = cs.slice, b0 = cs.b0, j0 = cs.j0, T = cs.T;
   const int B = p.B;
-  const int T = VL ? slice_steps(p.lengths, p.order, b0, p.T) : p.T;
+  // as in the forward: step s sums the partials step s - 1 sent
+  const ExchangeBars<C, 1, true> xb{bars, rank};
 
   if (tid == 0) {
-    for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], 1u);
+    xb.init(1u);
     ptx::fence_mbar_init();
   }
   proj_prologue<H, P, C, BS, VL>(p.w_hh[dir], p.w_hr[dir], j0, b0, B, p.T, p.lengths, p.order, W_s, R_s, row_s, len_s,
@@ -1433,12 +1475,12 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
 
   for (int step = 0; step <= T; ++step) {
     // ---- dh_t = dy_t + the C partials (rank order); dh_n enters at the first step, dh_0 leaves after the last ----
-    const int cur = step & 1;
+    const int cur = xb.buf(step);
     if (step > 0) {
-      const uint32_t par = ((step - 1) >> 1) & 1;
+      const uint32_t par = xb.parity(step);
 #pragma unroll
       for (int src = 0; src < C; ++src)
-        if ((uint32_t)src != rank) ptx::mbar_wait(&bars[cur * C + src], par);
+        if ((uint32_t)src != rank) xb.wait(cur, src, par);
     }
     const int t = dir ? step : (T - 1 - step);
     const float* sl = slot + (size_t)cur * C * BS * P;
@@ -1466,12 +1508,8 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
     }
     __syncthreads();
     if (step == T) break;
-    const int nb = (step + 1) & 1;
-    if (tid == 0) {
-#pragma unroll
-      for (int src = 0; src < C; ++src)
-        if ((uint32_t)src != rank) ptx::mbar_arrive_expect_tx(&bars[nb * C + src], (uint32_t)(BS * P * sizeof(float)));
-    }
+    const int nb = xb.buf(step) ^ 1;
+    if (tid == 0) xb.arm(nb, (uint32_t)(BS * P * sizeof(float)));
     // ---- dm = W_hr[:, j]^T dh_t, then the LSTM cell backward from dm ---------------------------------------------
     float dm = 0.f;
 #pragma unroll 4
@@ -1485,17 +1523,8 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
     }
     const bool frozen = VL && t >= len;
     float dg[G];
-    {
-      const float ig = sv[0], fg = sv[1], gg = sv[2], og = sv[3];
-      const float tc = tanh_f(sx);
-      const float dout = dm * tc * og * (1.f - og);
-      const float dc = dc_carry + dm * og * (1.f - tc * tc);
-      dg[0] = dc * gg * ig * (1.f - ig);
-      dg[1] = dc * cp * fg * (1.f - fg);
-      dg[2] = dc * ig * (1.f - gg * gg);
-      dg[3] = dout;
-      if (!frozen) dc_carry = dc * fg;  // frozen step: dc passes through
-    }
+    const float dc_next = lstm_cell_bwd(sv, sx, cp, dm, dc_carry, dg);
+    if (!frozen) dc_carry = dc_next;  // frozen step: dc passes through
     if (frozen || !valid) {
 #pragma unroll
       for (int g = 0; g < G; ++g) dg[g] = 0.f;
@@ -1523,7 +1552,7 @@ __global__ void __launch_bounds__(ProjCfg<H, P, C, BS>::NT, 1)
       }
     }
     __syncthreads();
-    proj_send<P, C, BS, NT>(own, &bars[nb * C + rank], rank, tid);
+    proj_send<P, C, BS, NT>(own, xb.bar(nb, rank), rank, tid);
   }
   if (valid && p.dc_0) p.dc_0[((size_t)dir * B + row) * H + j] = dc_carry;
   if constexpr (VL) {  // the steps [T, p.T) the cluster skipped: no gate gradient, no dh
@@ -1668,73 +1697,27 @@ int pick_fwd_tc(const RecFwdParams& p, RecFwdLaunch* L) {
 }
 
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
-bool try_bwd(RecBwdParams& p, cudaStream_t s, bool force, int* rc) {
+bool pick_bwd(const RecBwdParams& p, bool force, RecBwdLaunch* L, int* rc) {
   using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
   static_assert(Cfg::BWD_SMEM <= MAX_SMEM, "backward config does not fit an SM");
   auto k = p.lengths ? rec_bwd_kernel<MODE, H, C, BS, KL, UPL, RG, true> : rec_bwd_kernel<MODE, H, C, BS, KL, UPL, RG, false>;
-  ClusterLaunch<RecBwdParams> L;
-  if (!pick_clustered(k, p, C, BS, Cfg::NT, Cfg::BWD_SMEM, force, &L, rc,
-                      "bwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d", C, BS, KL, UPL, RG))
-    return false;
-  if (*rc != B200RNN_OK) return true;
-  // transposed, per-CTA contiguous copy of W_hh for this cluster width
-  for (int d = 0; d < p.D; ++d) {
-    whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], Cfg::G, H, C);
-    if (cudaGetLastError() != cudaSuccess) {
-      set_error("whh_prep launch failed");
-      *rc = B200RNN_ERR_CUDA;
-      return true;
-    }
-    count_launch();
-  }
-  p.nslices_out = L.nslices;
-  *rc = launch_clustered(L, p, PROF_REC_BWD, false, s);
-  return true;
+  return pick_clustered(k, p, C, BS, Cfg::NT, Cfg::BWD_SMEM, force, L, rc, "bwd cfg C=%d BS=%d KL=%d UPL=%d RG=%d", C,
+                        BS, KL, UPL, RG);
 }
 
-// LSTM with a projection: one config per (H, P), several waves when its clusters do not all fit
-template <int H, int P, int C, int BS>
-int pick_fwd_proj(const RecFwdParams& p, RecFwdLaunch* L) {
+// LSTM with a projection, forward or backward: one config per (H, P), several waves when its clusters do not all fit
+template <int H, int P, int C, int BS, typename Params>
+int pick_proj(const Params& p, ClusterLaunch<Params>* L) {
   using Cfg = ProjCfg<H, P, C, BS>;
-  static_assert(Cfg::SMEM_F <= MAX_SMEM, "projected forward config does not fit an SM");
-  auto k = p.lengths ? rec_fwd_proj_kernel<H, P, C, BS, true> : rec_fwd_proj_kernel<H, P, C, BS, false>;
+  static_assert(Cfg::SMEM_F <= MAX_SMEM && Cfg::SMEM_B <= MAX_SMEM, "projected config does not fit an SM");
   int rc = B200RNN_OK;
-  pick_clustered(k, p, C, BS, Cfg::NT, Cfg::SMEM_F, true, L, &rc, "fwd proj cfg C=%d BS=%d P=%d", C, BS, P);
+  if constexpr (std::is_same<Params, RecFwdParams>::value)
+    pick_clustered(p.lengths ? rec_fwd_proj_kernel<H, P, C, BS, true> : rec_fwd_proj_kernel<H, P, C, BS, false>, p, C,
+                   BS, Cfg::NT, Cfg::SMEM_F, true, L, &rc, "fwd proj cfg C=%d BS=%d P=%d", C, BS, P);
+  else
+    pick_clustered(p.lengths ? rec_bwd_proj_kernel<H, P, C, BS, true> : rec_bwd_proj_kernel<H, P, C, BS, false>, p, C,
+                   BS, Cfg::NT, Cfg::SMEM_B, true, L, &rc, "bwd proj cfg C=%d BS=%d P=%d", C, BS, P);
   return rc;
-}
-
-template <int H, int P, int C, int BS>
-int launch_bwd_proj(RecBwdParams& p, cudaStream_t s) {
-  using Cfg = ProjCfg<H, P, C, BS>;
-  static_assert(Cfg::SMEM_B <= MAX_SMEM, "projected backward config does not fit an SM");
-  auto k = p.lengths ? rec_bwd_proj_kernel<H, P, C, BS, true> : rec_bwd_proj_kernel<H, P, C, BS, false>;
-  ClusterLaunch<RecBwdParams> L;
-  int rc = B200RNN_OK;
-  pick_clustered(k, p, C, BS, Cfg::NT, Cfg::SMEM_B, true, &L, &rc, "bwd proj cfg C=%d BS=%d P=%d", C, BS, P);
-  if (rc != B200RNN_OK) return rc;
-  p.nslices_out = L.nslices;
-  return launch_clustered(L, p, PROF_REC_BWD, false, s);
-}
-
-// Template arguments <H, P, C, BS>: H = 128 on 2-CTA clusters of 4 batch rows (256 threads), H = 256 on 4-CTA clusters
-// of 8 batch rows (512 threads)
-int plan_rec_fwd_proj(const RecFwdParams& p, RecFwdLaunch* L) {
-  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 32) return pick_fwd_proj<128, 32, 2, 4>(p, L);
-  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 64) return pick_fwd_proj<128, 64, 2, 4>(p, L);
-  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 64) return pick_fwd_proj<256, 64, 4, 8>(p, L);
-  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 128) return pick_fwd_proj<256, 128, 4, 8>(p, L);
-  set_error("recurrence: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d); built for the LSTM with "
-            "proj_size hidden_size/4 or hidden_size/2", p.mode, p.H, p.P);
-  return B200RNN_ERR_UNSUPPORTED;
-}
-
-int launch_rec_bwd_proj(RecBwdParams& p, cudaStream_t s) {
-  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 32) return launch_bwd_proj<128, 32, 2, 4>(p, s);
-  if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 64) return launch_bwd_proj<128, 64, 2, 4>(p, s);
-  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 64) return launch_bwd_proj<256, 64, 4, 8>(p, s);
-  if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 128) return launch_bwd_proj<256, 128, 4, 8>(p, s);
-  set_error("recurrence backward: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d)", p.mode, p.H, p.P);
-  return B200RNN_ERR_UNSUPPORTED;
 }
 
 }  // namespace
@@ -1744,12 +1727,21 @@ int rec_bwd_max_slices(int B) { return (B + 1) / 2; }
 
 // Candidates are ordered by batch rows per cluster; the first one whose clusters are all co-resident
 // (one wave => every sequence advances in lock step) wins, else the widest one runs in several waves.
-// Template arguments: <MODE, H, C, BS, KL, UPL, RG>.
+// Template arguments: <MODE, H, C, BS, KL, UPL, RG>; projected: <H, P, C, BS>, H = 128 on 2-CTA clusters of 4 batch rows
+// (256 threads), H = 256 on 4-CTA clusters of 8 batch rows (512 threads).
 int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
   int rc = B200RNN_OK;
   L->kernel = nullptr;
   if (p.B <= 0 || p.T <= 0) return rc;
-  if (p.P > 0) return plan_rec_fwd_proj(p, L);
+  if (p.P > 0) {
+    if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 32) return pick_proj<128, 32, 2, 4>(p, L);
+    if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 64) return pick_proj<128, 64, 2, 4>(p, L);
+    if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 64) return pick_proj<256, 64, 4, 8>(p, L);
+    if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 128) return pick_proj<256, 128, 4, 8>(p, L);
+    set_error("recurrence: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d); built for the LSTM with "
+              "proj_size hidden_size/4 or hidden_size/2", p.mode, p.H, p.P);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
   if (p.mode == B200RNN_GRU && p.H == 256) {
@@ -1788,6 +1780,46 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
   return B200RNN_ERR_UNSUPPORTED;
 }
 
+// The same rule and projected configs as the forward
+int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
+  int rc = B200RNN_OK;
+  L->kernel = nullptr;
+  if (p.B <= 0 || p.T <= 0) return rc;
+  if (p.P > 0) {
+    if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 32) return pick_proj<128, 32, 2, 4>(p, L);
+    if (p.mode == B200RNN_LSTM && p.H == 128 && p.P == 64) return pick_proj<128, 64, 2, 4>(p, L);
+    if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 64) return pick_proj<256, 64, 4, 8>(p, L);
+    if (p.mode == B200RNN_LSTM && p.H == 256 && p.P == 128) return pick_proj<256, 128, 4, 8>(p, L);
+    set_error("recurrence backward: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d)", p.mode, p.H, p.P);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
+  // (not the weights) dominates the shared-memory traffic of the backward contraction
+  if (p.mode == B200RNN_GRU && p.H == 256) {
+    if (pick_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, false, L, &rc)) return rc;
+    if (pick_bwd<B200RNN_GRU, 256, 4, 4, 32, 8, 1>(p, false, L, &rc)) return rc;
+    pick_bwd<B200RNN_GRU, 256, 8, 8, 32, 4, 1>(p, true, L, &rc);
+    return rc;
+  }
+  if (p.mode == B200RNN_GRU && p.H == 128) {
+    if (pick_bwd<B200RNN_GRU, 128, 2, 4, 32, 8, 1>(p, false, L, &rc)) return rc;
+    pick_bwd<B200RNN_GRU, 128, 4, 8, 32, 4, 1>(p, true, L, &rc);
+    return rc;
+  }
+  if (p.mode == B200RNN_LSTM && p.H == 256) {
+    if (pick_bwd<B200RNN_LSTM, 256, 4, 4, 32, 8, 1>(p, false, L, &rc)) return rc;
+    pick_bwd<B200RNN_LSTM, 256, 8, 8, 32, 4, 1>(p, true, L, &rc);
+    return rc;
+  }
+  if (p.mode == B200RNN_LSTM && p.H == 128) {
+    if (pick_bwd<B200RNN_LSTM, 128, 2, 4, 32, 8, 1>(p, false, L, &rc)) return rc;
+    pick_bwd<B200RNN_LSTM, 128, 4, 8, 32, 4, 1>(p, true, L, &rc);
+    return rc;
+  }
+  set_error("recurrence backward: unsupported (mode=%d, hidden_size=%d)", p.mode, p.H);
+  return B200RNN_ERR_UNSUPPORTED;
+}
+
 int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s) {
   if (p.B <= 0 || p.T <= 0) return B200RNN_OK;
   if (p.ready && p.D != 1) {  // GiReady walks the row tiles in increasing t
@@ -1802,35 +1834,21 @@ int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s)
 }
 
 int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
-  int rc = B200RNN_OK;
-  if (p.B <= 0 || p.T <= 0) return rc;
-  if (p.P > 0) return launch_rec_bwd_proj(p, s);
-  // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
-  // (not the weights) dominates the shared-memory traffic of the backward contraction
-  if (p.mode == B200RNN_GRU && p.H == 256) {
-    // as in the forward: a config is taken only when the driver reports all its clusters co-resident
-    if (try_bwd<B200RNN_GRU, 256, 4, 2, 16, 8, 0>(p, s, false, &rc)) return rc;
-    if (try_bwd<B200RNN_GRU, 256, 4, 4, 32, 8, 1>(p, s, false, &rc)) return rc;
-    try_bwd<B200RNN_GRU, 256, 8, 8, 32, 4, 1>(p, s, true, &rc);
-    return rc;
+  RecBwdLaunch L;
+  const int rc = plan_rec_bwd(p, &L);
+  if (rc != B200RNN_OK || L.kernel == nullptr) return rc;
+  if (p.P == 0) {  // transposed, per-CTA contiguous copy of W_hh for the chosen cluster width
+    for (int d = 0; d < p.D; ++d) {
+      whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C);
+      if (cudaGetLastError() != cudaSuccess) {
+        set_error("whh_prep launch failed");
+        return B200RNN_ERR_CUDA;
+      }
+      count_launch();
+    }
   }
-  if (p.mode == B200RNN_GRU && p.H == 128) {
-    if (try_bwd<B200RNN_GRU, 128, 2, 4, 32, 8, 1>(p, s, false, &rc)) return rc;
-    try_bwd<B200RNN_GRU, 128, 4, 8, 32, 4, 1>(p, s, true, &rc);
-    return rc;
-  }
-  if (p.mode == B200RNN_LSTM && p.H == 256) {
-    if (try_bwd<B200RNN_LSTM, 256, 4, 4, 32, 8, 1>(p, s, false, &rc)) return rc;
-    try_bwd<B200RNN_LSTM, 256, 8, 8, 32, 4, 1>(p, s, true, &rc);
-    return rc;
-  }
-  if (p.mode == B200RNN_LSTM && p.H == 128) {
-    if (try_bwd<B200RNN_LSTM, 128, 2, 4, 32, 8, 1>(p, s, false, &rc)) return rc;
-    try_bwd<B200RNN_LSTM, 128, 4, 8, 32, 4, 1>(p, s, true, &rc);
-    return rc;
-  }
-  set_error("recurrence backward: unsupported (mode=%d, hidden_size=%d)", p.mode, p.H);
-  return B200RNN_ERR_UNSUPPORTED;
+  p.nslices_out = L.nslices;
+  return launch_clustered(L, p, PROF_REC_BWD, false, s);
 }
 
 }  // namespace b200rnn

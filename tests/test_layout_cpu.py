@@ -12,7 +12,7 @@ def paired_index(j: int, b: int, KL: int, BS: int) -> int:
     return ((((j // CW) * 4 + (j & 3)) * (BS // 2) + (b >> 1)) * KL + (j % CW) // 4) * 2 + (b & 1)
 
 
-# (H, KL, UPL, BS) of the forward configs dispatched with the batch-paired form (csrc/rnn_rec.cu launch_rec_fwd)
+# (H, KL, UPL, BS) of the forward configs dispatched with the batch-paired form (csrc/rnn_rec.cu plan_rec_fwd)
 CONFIGS = [(256, 16, 4, 4)]
 
 
