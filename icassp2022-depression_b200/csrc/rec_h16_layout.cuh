@@ -70,5 +70,20 @@ __host__ __device__ constexpr int state_index(int k, int b, int hl) {
 // 16-byte chunk with this index (in 16-byte units of the state buffer) to every peer
 __host__ __device__ constexpr int exchange_chunk(int k0, int lane) { return (k0 / 16) * 32 + ((k0 % 16) / 8) * 16 + lane; }
 
+// The x-projection ring (rnn_rec.cu, rec_fwd_tc_body): slot s holds one step's gates of the CTA, [G][BS][RING_ROW]
+// floats, unit u of gate g, batch slot q at ring_index(g, q, u). A row is one 256-byte bulk copy; rows are padded to 68
+// floats so that the rows 2t, 2t + 1 the lanes t = 0..3 of a warp read fall in different banks. In this kernel the
+// n tile's A fragments are read into registers in the prologue, so the n-tile region of unit group s (16 KB, one
+// contiguous block of the weight region) is dead afterwards and holds slot s.
+constexpr int RING_SLOTS = 4, RING_ROW = 68;
+constexpr int RING_SLOT_BYTES = G * BS * RING_ROW * 4;
+__host__ __device__ constexpr int ring_index(int g, int q, int u) { return (g * BS + q) * RING_ROW + u; }
+// byte offset of slot s in the shared-memory block (the weight region starts at 0)
+__host__ __device__ constexpr int ring_byte(int s) { return w_half(s, G - 1, 0, 0, 0, 0, 0) * 2; }
+static_assert(RING_SLOTS <= NUG, "one slot per unit group's n-tile region");
+static_assert(RING_SLOT_BYTES <= KB * 2 * 32 * 8 * 2, "a slot fits the n-tile region of one unit group");
+static_assert((RING_ROW * 4) % 16 == 0 && ring_byte(1) % 128 == 0, "bulk-copy destinations are 16-byte aligned");
+static_assert(HS * 4 == 256, "one ring row is one 256-byte copy");
+
 }  // namespace h16
 }  // namespace b200rnn

@@ -378,7 +378,7 @@ __device__ __forceinline__ float initial_state(const RecFwdParams& p, int dir, i
 // semantics (one broadcast load; a poll loop run by one lane alone made ptxas spill the FFMA configs' registers), and
 // the loads of `gates` that follow stay ordinary loads. `upto`, the last row tile this warp has seen complete, makes a
 // step whose tiles are already known complete cost one compare. Steps are visited in increasing t: only
-// unidirectional layers are streamed.
+// unidirectional layers are streamed. In the tensor-core kernels the producer lane alone polls (rec_fwd_tc_body).
 // The wait always ends: the GEMM never waits on anything, and the programmatic launch starts this kernel only after
 // every GEMM CTA has started. It is bounded all the same (trap after 4M polls, seconds, like the peer exchange in
 // fuse_head.cu), so that a protocol bug is a CUDA error, not a hung GPU.
@@ -549,8 +549,10 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 // forward, GRU H = 256 on the tensor cores (config tc8)
 // =================================================================================================
 // The cluster design of rec_fwd_kernel at C = 4, BS = 8 (weights staged once, per-source mbarriers, double-buffered
-// state, st.async all-gather with the own slice delivered locally, own slice first, deferred global stores, x-projection
-// prefetched one step ahead), but the per-step contraction [192 gate rows of the CTA] x [K = 256] x [8 batch rows] runs
+// state, st.async all-gather with the own slice delivered locally, own slice first, deferred global stores), but the
+// x-projection arrives through a shared-memory ring that a producer warp fills with bulk copies (it alone polls the
+// streamed GEMM's counters, off the compute warps' serial path), and the per-step contraction
+// [192 gate rows of the CTA] x [K = 256] x [8 batch rows] runs
 // on the tensor cores as mma.sync m16n8k8 in 3xTF32 (ptx.cuh split_tf32), at fp32-level error:
 //   * unit group ug (16 units of the CTA's slice) has three gate tiles (r, z, n): three M = 16 tiles of W_hh rows,
 //     N = the 8 batch rows, K in 32 k-steps of 8. Two warps share a unit group and split K: warp (ug, kh) takes k-steps
@@ -576,13 +578,24 @@ struct TcFwdCfg {
   static constexpr int H = 256, C = 4, BS = 8, G = 3, GH = G * H;
   static constexpr int HS = H / C;        // units per CTA
   static constexpr int NUG = HS / 16;     // unit groups
-  static constexpr int NW = 2 * NUG;      // warps: (k half, unit group)
-  static constexpr int NT = NW * 32;
+  static constexpr int NW = 2 * NUG;      // compute warps: (k half, unit group)
+  static constexpr int NTC = NW * 32;     // compute threads
+  static constexpr int NT = NTC + 128;    // and the producer warpgroup
   static constexpr int KS = H / 8;        // k-steps of the contraction
   static constexpr int KSC = HS / 8;      // k-steps per source slice
   static constexpr size_t W_BYTES = (size_t)G * HS * H * sizeof(float);
   static constexpr size_t RED_BYTES = (size_t)NW * 2 * G * 32 * sizeof(float);  // partial sums swapped between halves
-  static constexpr size_t SMEM = W_BYTES + (size_t)2 * BS * H * sizeof(float) + RED_BYTES + 2 * C * sizeof(uint64_t);
+  // x-projection ring of the 3xTF32 and TF32 kernels, behind the swap buffer (the fp16-pair kernel keeps its ring in
+  // dead weight space, rec_h16_layout.cuh)
+  static constexpr int RING_SLOTS = 2;
+  static constexpr size_t RING_BYTES = (size_t)RING_SLOTS * h16::RING_SLOT_BYTES;
+  static constexpr int NBAR = 2 * C + 2 * h16::RING_SLOTS;  // state [buf][src], ring full[slot], ring empty[slot]
+  static constexpr size_t SMEM = W_BYTES + (size_t)2 * BS * H * sizeof(float) + RED_BYTES + RING_BYTES +
+                                 NBAR * sizeof(uint64_t);
+  // setmaxnreg: the producer warpgroup gives its registers to the two compute warpgroups
+  static constexpr int PRODUCER_REGS = 24, COMPUTE_REGS = 240;
+  static_assert(PRODUCER_REGS * 128 + COMPUTE_REGS * NTC <= 65536, "register file");
+  static_assert(RING_SLOTS <= h16::RING_SLOTS, "ring barriers");
 };
 
 // position of state element (k, batch row b) in the B-fragment-ordered buffer: lane (g, t) of k-step ks reads
@@ -622,11 +635,18 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   float4* W_f = reinterpret_cast<float4*>(smem_raw);                  // [NUG][G][KS][32 lanes] A fragments
   float* h_s = reinterpret_cast<float*>(smem_raw + Cfg::W_BYTES);     // [2][BS * H] B-fragment order
   float* red = h_s + 2 * BS * H;                                       // [NW][2 * G][32 lanes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(red + NW * 2 * G * 32);  // [buf * C + src] state slices
+  float* ring_tail = red + NW * 2 * G * 32;                             // X3 / TF32: [RING_SLOTS] x-projection slots
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + Cfg::SMEM - Cfg::NBAR * sizeof(uint64_t));
+  uint64_t* full = bars + 2 * C;                                        // [slot] x-projection of the step has landed
+  uint64_t* empty = full + h16::RING_SLOTS;                             // [slot] every compute warp has read it
   // F16: W_f holds [NUG][G][KB][hi, lo][32 lanes] A fragments and h_s [2][KB][32 slots] state pairs (rec_h16_layout.cuh);
   // red holds the row scales 2^e_r [G][HS] until the step loop first writes it
   __half* W_h = reinterpret_cast<__half*>(smem_raw);
   float* scl = red;
+  constexpr int NSLOT = F16 ? h16::RING_SLOTS : Cfg::RING_SLOTS;
+  auto ring_slot = [&](int s) {
+    return F16 ? reinterpret_cast<float*>(smem_raw + h16::ring_byte(s)) : ring_tail + s * (h16::RING_SLOT_BYTES / 4);
+  };
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int ug = w % NUG, kh = w / NUG;
@@ -638,11 +658,16 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   const ExchangeBars<C, 1, true> xb{bars, rank};
 
   if (tid == 0) {
-    xb.init((uint32_t)NW);  // the own slice: one arrive per warp
+    xb.init((uint32_t)NW);  // the own slice: one arrive per compute warp
+    for (int s = 0; s < NSLOT; ++s) {
+      ptx::mbar_init(&full[s], 1u);           // the producer's expect_tx, then the copies' bytes
+      ptx::mbar_init(&empty[s], (uint32_t)NW);  // one arrive per compute warp
+    }
     ptx::fence_mbar_init();
   }
+  // the prologue is shared by all NT threads, the producer warpgroup included
   if constexpr (F16) {  // the row scales: one warp per row
-    for (int rr = w; rr < G * HS; rr += NW) {
+    for (int rr = w; rr < G * HS; rr += NT / 32) {
       const float4* row = reinterpret_cast<const float4*>(w_hh + ((size_t)(rr / HS) * H + j0 + rr % HS) * H);
       float m = 0.f;
 #pragma unroll
@@ -695,6 +720,37 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   }
   __syncthreads();
 
+  if (w >= NW) {  // the producer warpgroup: one lane fills the x-projection ring, the rest only meets the cluster barriers
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::PRODUCER_REGS));
+    ptx::cluster_sync_all();  // F16: the compute warps have read the n tile (the ring's space) into registers
+    if (w == NW && lane == 0) {
+      const float* gates = p.gates[dir];
+      const int nvalid = min(BS, p.B - b0);  // slots past the batch are never read (FwdCell::valid)
+      GiReady gi_ready;
+      for (int step = 0; step < T; ++step) {
+        const int s = step % NSLOT, t = dir ? (T - 1 - step) : step;
+        if (step >= NSLOT) ptx::mbar_wait(&empty[s], (step / NSLOT - 1) & 1);
+        if (p.ready) {
+          gi_ready.wait(p, t);
+          ptx::fence_proxy_async_global();  // the GEMM's stores, acquired above, are read by the bulk copies below
+        }
+        float* slot = ring_slot(s);
+        ptx::mbar_arrive_expect_tx(&full[s], (uint32_t)(nvalid * G * HS * sizeof(float)));
+        for (int q = 0; q < nvalid; ++q) {
+          const int row = VL ? p.order[b0 + q] : b0 + q;
+          const float* src = gates + ((size_t)t * p.B + row) * (G * H) + j0;
+#pragma unroll
+          for (int g = 0; g < G; ++g)
+            ptx::tma_bulk_g2s(slot + h16::ring_index(g, q, 0), src + g * H, (uint32_t)(HS * sizeof(float)), &full[s]);
+        }
+      }
+    }
+    __syncwarp();
+    ptx::cluster_sync_all();  // the compute warps' final one
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::COMPUTE_REGS));
+
   // ---- lane identity: output jb is unit ju, batch row b0 + 2 * ft + jb (accumulator fragment elements 2*kh + jb) ---
   const int fg = lane >> 2, ft = lane & 3;
   const int u0 = ug * 16 + kh * 8;  // first unit (within the CTA's slice) this warp finishes
@@ -719,12 +775,6 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
   const int ju = j0 + u0 + fg;
   FwdCell<B200RNN_GRU, H, VL> cell[2] = {{p, dir, ju, b0 + 2 * ft}, {p, dir, ju, b0 + 2 * ft + 1}};
-  GiReady gi_ready;
-  if (T > 0) {
-    gi_ready.wait(p, dir ? T - 1 : 0);
-#pragma unroll
-    for (int jb = 0; jb < 2; ++jb) cell[jb].load_gi(p, dir ? T - 1 : 0);
-  }
 
   const float4* W_w = W_f + (size_t)ug * G * KS * 32 + lane;
   float* red_mine = red + w * 2 * G * 32 + lane;                         // written by this warp
@@ -736,6 +786,13 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     const int cur = xb.buf(step), nxt = cur ^ 1;
     const float2* h_cur = reinterpret_cast<const float2*>(h_s + cur * BS * H) + lane;
     const uint32_t par = xb.parity(step);
+#ifdef B200RNN_TRACE
+    const bool tr = p.trace != nullptr && blockIdx.x == 0 && lane == 0;  // one row of 16 stamps per (step, warp)
+#else
+    constexpr bool tr = false;  // build with -DB200RNN_TRACE for the per-phase clock64 timeline (tools/trace_rec.py tc)
+#endif
+    long long* trow = p.trace + ((size_t)step * NW + w) * 16;
+    if (tr) trow[0] = clock64();
 
     float acc[G][4];
 #pragma unroll
@@ -747,6 +804,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     for (int c = 0; c < C; ++c) {
       const int src = (c + (int)rank) % C;
       if (step > 0) xb.wait(cur, src, par);
+      if (tr) trow[1 + c] = clock64();  // slice c (own first) has arrived
       float d[G][2][4];  // [gate tile][lo*hi + hi*lo, hi*hi]; TF32: [gate tile][-, the single product]
 #pragma unroll
       for (int g = 0; g < G; ++g)
@@ -818,13 +876,29 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
       for (int g = 0; g < G; ++g)
 #pragma unroll
         for (int i = 0; i < 4; ++i) acc[g][i] += TF32 ? d[g][1][i] : d[g][0][i] + d[g][1][i];
-      if (c == 0 && step > 0) {  // the previous step's stores
+      if (c == 0) {
+        if (step > 0) {  // the previous step's stores
 #pragma unroll
-        for (int jb = 0; jb < 2; ++jb) cell[jb].flush(p, dir, dir ? (T - step) : (step - 1));
+          for (int jb = 0; jb < 2; ++jb) cell[jb].flush(p, dir, dir ? (T - step) : (step - 1));
+        }
+        // this step's x-projection from its ring slot (already complete in the steady state); the slot is released
+        // to the producer once the whole warp has read it
+        const int s = step % NSLOT;
+        ptx::mbar_wait(&full[s], (step / NSLOT) & 1);
+        const float* slot = ring_slot(s);
+#pragma unroll
+        for (int jb = 0; jb < 2; ++jb)
+          if (cell[jb].valid) {
+#pragma unroll
+            for (int g = 0; g < G; ++g) cell[jb].gi[g] = slot[h16::ring_index(g, 2 * ft + jb, u0 + fg)];
+          }
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty[s]);
       }
     }
     // every slice of h_step has been consumed by this thread => the barriers of the other buffer are re-armed
     if (tid == 0 && step + 1 < T) xb.arm(nxt, (uint32_t)(BS * HS * sizeof(float)));
+    if (tr) trow[5] = clock64() + (long long)(acc[0][0] + acc[1][0] + acc[2][0] == 12345.678f);  // contraction done
     // swap halves with the partner warp: it finishes the other 8 units. WAR on `red`: the partner overwrites it only
     // after its next step's own-slice wait, which needs this warp's arrive below (after the read).
 #pragma unroll
@@ -840,9 +914,11 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
         pre[jb][g] = (kh ? acc[g][2 + jb] : acc[g][jb]) + red_partner[(g * 2 + jb) * 32];
         if constexpr (F16) pre[jb][g] *= unscale[g];
       }
+    if (tr) trow[6] = clock64() + (long long)(pre[0][0] == 12345.678f);  // k-half swap done
     float hnew[2];
 #pragma unroll
     for (int jb = 0; jb < 2; ++jb) hnew[jb] = cell[jb].update(t, pre[jb]);
+    if (tr) trow[7] = clock64() + (long long)(hnew[0] + hnew[1] == 12345.678f);  // update done
 
     if (step + 1 < T) {
       // own copy with ordinary stores; after __syncwarp the warp's k-step is 16 contiguous float4 that go to the peers
@@ -875,17 +951,13 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
       }
       if (lane == 0) ptx::mbar_arrive(xb.bar(nxt, rank));
     }
+    if (tr) trow[8] = clock64();  // slice sent
 
     if (step == T - 1) {
 #pragma unroll
       for (int jb = 0; jb < 2; ++jb) cell[jb].flush(p, dir, t);
 #pragma unroll
       for (int jb = 0; jb < 2; ++jb) cell[jb].finish(p, dir);
-    }
-    if (step + 1 < T) {
-      gi_ready.wait(p, dir ? (T - 2 - step) : (step + 1));
-#pragma unroll
-      for (int jb = 0; jb < 2; ++jb) cell[jb].load_gi(p, dir ? (T - 2 - step) : (step + 1));
     }
   }
   if constexpr (VL) {
