@@ -494,7 +494,8 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       float* a_dense = tc_a_hi(tc_ws);
       if (l == 0 && ln_gamma) {
         float* out = (save && fused_ln) ? R + rl.xln : a_dense;
-        rc = tc_layernorm(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, out, st, ready, tiles_m);
+        // padded rows of a ragged batch are written as 0: the backward's dW_ih GEMM reads this saved operand
+        rc = tc_layernorm(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, out, st, ready, tiles_m, lengths, d.B);
         a_in = out;
         a_rows = simple_rows(Il);
       } else if (!tc_a_f32_in_place(in, in_rows, (int)d.TB, Il)) {
@@ -805,10 +806,16 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     // The tensor cores need 16-byte aligned targets: a gradient view that is not (a caller's flat bucket behind an
     // odd-sized tensor) takes the FFMA GEMM instead of failing.
     const bool tc_l = tc_available() && (Il % 128 == 0);
-    // layer input as seen by the forward GEMM; one split serves both directions
+    // layer input as seen by the forward GEMM; one split serves both directions. The padded steps of a ragged batch
+    // have zero gate gradients, but 0 * NaN is NaN: layer 0's operand must be 0 there, not whatever the caller left in
+    // x (the layers above read the recurrence's outputs, which are 0 past each length)
     GradSrc X{nullptr, simple_rows((long long)Il), TB, Il, S + sl.b_tc_x, false};
-    if (l == 0 && fused_ln) {  // what the forward GEMM multiplied: LayerNorm(x), saved densely by the prologue
+    if (l == 0 && fused_ln) {  // what the forward GEMM multiplied: LayerNorm(x), saved densely by the prologue (padding 0)
       X.p = R + rl.xln;
+    } else if (l == 0 && lengths) {  // x with its padding zeroed, dense in the (unused without LayerNorm) b_dxln region
+      rc = launch_valid_rows(x, tb_rows(xs_t, xs_b, d.B), d.T, d.B, Il, lengths, S + sl.b_dxln, st);
+      if (rc) return rc;
+      X.p = S + sl.b_dxln;
     } else if (l == 0) {
       X.p = x;
       X.rows = tb_rows(xs_t, xs_b, d.B);
@@ -891,7 +898,8 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     }
     if (ln_l0 && want_dx) {  // LayerNorm backward: dx (caller's layout), dgamma, dbeta
       rc = launch_layernorm_bwd(x, tb_rows(xs_t, xs_b, d.B), S + sl.b_dxln, (int)d.TB, d.I, ln_gamma, ln_eps, dx,
-                                tb_rows(dxs_t, dxs_b, d.B), dln_gamma, dln_beta, accumulate, S + sl.b_lnpart, st);
+                                tb_rows(dxs_t, dxs_b, d.B), dln_gamma, dln_beta, accumulate, S + sl.b_lnpart, st,
+                                lengths, d.B);
       if (rc) return rc;
     }
   }

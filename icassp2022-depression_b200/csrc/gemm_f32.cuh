@@ -51,14 +51,16 @@ int tc_gather_rows(const float* src, const RowMap& rows, int R, int Cc, float* d
 // LayerNorm over the last dimension: out[R][Cc] <- LN(src row) * gamma + beta (dense fp32: the A operand of the
 // input projection, and when kept, the layer-0 wgrad operand of the backward pass)
 // `clear` (optional): nclear ints zeroed by the same launch (the ready counters of a streamed GEMM that reads out)
+// `lengths` (optional, ragged batch; rows r = t*B + b): the rows with t >= lengths[b] are written as 0, x is not read
 int tc_layernorm(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta, float eps,
-                 float* out, cudaStream_t stream, int* clear = nullptr, int nclear = 0);
+                 float* out, cudaStream_t stream, int* clear = nullptr, int nclear = 0, const int* lengths = nullptr,
+                 int B = 1);
 // backward of that prologue: dx (strided like x) from dy = d/dLN(x) (dense), dgamma / dbeta (+)=; part = scratch of
-// layernorm_bwd_scratch_floats(Cc) floats
+// layernorm_bwd_scratch_floats(Cc) floats. `lengths` as above: padded rows get dx = 0 and add nothing to dgamma / dbeta
 size_t layernorm_bwd_scratch_floats(int Cc);
 int launch_layernorm_bwd(const float* x, const RowMap& x_rows, const float* dy, int R, int Cc, const float* gamma,
                          float eps, float* dx, const RowMap& dx_rows, float* dgamma, float* dbeta, int accumulate,
-                         float* part, cudaStream_t stream);
+                         float* part, cudaStream_t stream, const int* lengths = nullptr, int B = 1);
 
 // tensor-core (wgmma) 3xTF32 path: C = A[M,K] * B[N,K]^T + biases (both operands k-contiguous, K % 32 == 0, N % 128 == 0)
 size_t gemm_tc_scratch_bytes(int M, int N, int K);

@@ -518,12 +518,19 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, RowMap rows, i
 template <int NV>  // float4 per lane
 __global__ void layernorm_kernel(const float* __restrict__ src, RowMap rows, int R, int Cc,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                                 float* __restrict__ out, int* __restrict__ clear, int nclear) {
+                                 float* __restrict__ out, int* __restrict__ clear, int nclear,
+                                 const int* __restrict__ lengths, int B) {
   if (blockIdx.x == 0)
     for (int i = threadIdx.x; i < nclear; i += blockDim.x) clear[i] = 0;
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
   for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < R; r += gridDim.x * wpb) {
+    if (lengths && r / B >= __ldg(lengths + r % B)) {  // padding of a ragged batch: 0, whatever x holds there
+#pragma unroll
+      for (int i = 0; i < NV; ++i)
+        *reinterpret_cast<float4*>(out + (size_t)r * Cc + i * 128 + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      continue;
+    }
     const float* p = src + rows.off(r);
     float4 x[NV];
     float s = 0.f;
@@ -564,7 +571,8 @@ __global__ void layernorm_kernel(const float* __restrict__ src, RowMap rows, int
 template <int NV>
 __global__ void layernorm_bwd_kernel(const float* __restrict__ x, RowMap x_rows, const float* __restrict__ dy, int R,
                                      int Cc, const float* __restrict__ gamma, float eps, float* __restrict__ dx,
-                                     RowMap dx_rows, float* __restrict__ part /* [grid][2][Cc] */) {
+                                     RowMap dx_rows, float* __restrict__ part /* [grid][2][Cc] */,
+                                     const int* __restrict__ lengths, int B) {
   extern __shared__ float red[];  // [warps][2][Cc]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int wpb = blockDim.x >> 5;
@@ -576,6 +584,14 @@ __global__ void layernorm_bwd_kernel(const float* __restrict__ x, RowMap x_rows,
     gm[i] = __ldg(reinterpret_cast<const float4*>(gamma + i * 128 + lane * 4));
   }
   for (int r = blockIdx.x * wpb + warp; r < R; r += gridDim.x * wpb) {
+    if (lengths && r / B >= __ldg(lengths + r % B)) {  // padding of a ragged batch: dx = 0, nothing to dgamma / dbeta
+      if (dx) {
+#pragma unroll
+        for (int i = 0; i < NV; ++i)
+          *reinterpret_cast<float4*>(dx + dx_rows.off(r) + i * 128 + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      continue;
+    }
     const float* px = x + x_rows.off(r);
     const float* pd = dy + (size_t)r * Cc;
     float4 xv[NV], dv[NV];
@@ -774,7 +790,7 @@ float* tc_a_hi(void* ws) { return reinterpret_cast<float*>((reinterpret_cast<uin
 float* tc_a_lo(void* ws, int M, int K) { return tc_a_hi(ws) + (size_t)M * K; }
 
 int tc_layernorm(const float* src, const RowMap& rows, int R, int Cc, const float* gamma, const float* beta, float eps,
-                 float* out, cudaStream_t stream, int* clear, int nclear) {
+                 float* out, cudaStream_t stream, int* clear, int nclear, const int* lengths, int B) {
   const bool vec = (reinterpret_cast<uintptr_t>(src) & 15u) == 0 && rows.s_outer % 4 == 0 && rows.s_inner % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0 && (reinterpret_cast<uintptr_t>(beta) & 15u) == 0;
   if (!vec || !(Cc == 128 || Cc == 256 || Cc == 512 || Cc == 1024)) {
@@ -786,7 +802,7 @@ int tc_layernorm(const float* src, const RowMap& rows, int R, int Cc, const floa
   ProfScope prof(PROF_MISC, stream);
   if (!clear) nclear = 0;
 #define B200_LNS(NV_) \
-  layernorm_kernel<NV_><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, out, clear, nclear)
+  layernorm_kernel<NV_><<<blocks, 256, 0, stream>>>(src, rows, R, Cc, gamma, beta, eps, out, clear, nclear, lengths, B)
   switch (Cc / 128) {  // instantiated widths: 128, 256, 512, 1024 (the reference normalises 256-d audio features)
     case 1: B200_LNS(1); break;
     case 2: B200_LNS(2); break;
@@ -803,7 +819,7 @@ size_t layernorm_bwd_scratch_floats(int Cc) { return (size_t)LNB_BLOCKS * 2 * Cc
 
 int launch_layernorm_bwd(const float* x, const RowMap& x_rows, const float* dy, int R, int Cc, const float* gamma,
                          float eps, float* dx, const RowMap& dx_rows, float* dgamma, float* dbeta, int accumulate,
-                         float* part, cudaStream_t stream) {
+                         float* part, cudaStream_t stream, const int* lengths, int B) {
   const bool vec = (reinterpret_cast<uintptr_t>(x) & 15u) == 0 && x_rows.s_outer % 4 == 0 && x_rows.s_inner % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(gamma) & 15u) == 0 && (reinterpret_cast<uintptr_t>(dy) & 15u) == 0 &&
                    (!dx || ((reinterpret_cast<uintptr_t>(dx) & 15u) == 0 && dx_rows.s_outer % 4 == 0 &&
@@ -823,7 +839,7 @@ int launch_layernorm_bwd(const float* x, const RowMap& x_rows, const float* dy, 
     attr[current_device()] = true;
   }
 #define B200_LNB(NV_) \
-  layernorm_bwd_kernel<NV_><<<blocks, 256, smem, stream>>>(x, x_rows, dy, R, Cc, gamma, eps, dx, dx_rows, part)
+  layernorm_bwd_kernel<NV_><<<blocks, 256, smem, stream>>>(x, x_rows, dy, R, Cc, gamma, eps, dx, dx_rows, part, lengths, B)
   switch (Cc / 128) {
     case 1: B200_LNB(1); break;
     case 2: B200_LNB(2); break;

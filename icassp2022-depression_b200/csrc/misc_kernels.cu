@@ -90,6 +90,16 @@ __global__ void initial_state_rows_kernel(const float* __restrict__ dgates, cons
   }
 }
 
+__global__ void valid_rows_kernel(const float* __restrict__ src, RowMap rows, int T, int B, int C,
+                                  const int* __restrict__ lengths, float* __restrict__ dst) {
+  const size_t n = (size_t)T * B * C;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int r = (int)(i / C), c = (int)(i % C);
+    const int t = r / B, b = r - t * B;
+    dst[i] = t < lengths[b] ? src[rows.off(r) + c] : 0.f;
+  }
+}
+
 __global__ void bias_reduce_kernel(const float* __restrict__ part, int nslices, int mode, int H, float* db_ih,
                                    float* db_hh, int accumulate) {
   const int G = mode == B200RNN_GRU ? 3 : 4;
@@ -160,6 +170,18 @@ int launch_initial_state_rows(const float* dgates, const float* dghn, int mode, 
   int blocks = (int)((n + 255) / 256);
   if (blocks > NUM_SMS * 4) blocks = NUM_SMS * 4;
   initial_state_rows_kernel<<<blocks, 256, 0, stream>>>(dgates, dghn, mode, B, T, H, reverse ? 1 : 0, lengths, out);
+  B200_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return B200RNN_OK;
+}
+
+int launch_valid_rows(const float* src, const RowMap& rows, int T, int B, int C, const int* lengths, float* dst,
+                      cudaStream_t stream) {
+  const size_t n = (size_t)T * B * C;
+  if (n == 0) return B200RNN_OK;
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > NUM_SMS * 8) blocks = NUM_SMS * 8;
+  valid_rows_kernel<<<blocks, 256, 0, stream>>>(src, rows, T, B, C, lengths, dst);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;

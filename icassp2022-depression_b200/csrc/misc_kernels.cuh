@@ -26,6 +26,12 @@ int launch_length_order(const int* lengths, int B, int* order, cudaStream_t stre
 int launch_initial_state_rows(const float* dgates, const float* dghn, int mode, int B, int T, int H, bool reverse,
                               const int* lengths, float* out, cudaStream_t stream);
 
+// Dense copy dst[T*B][C] of the rows r = t*B + b of src (read through `rows`), with the rows past each sequence's end
+// (t >= lengths[b]) written as 0 instead of read: the layer-0 operand of a ragged backward's dW_ih GEMM, so that
+// whatever the caller left in the padding (NaN, Inf) meets the zero gate gradients of those steps as a 0, not as 0 * NaN.
+int launch_valid_rows(const float* src, const RowMap& rows, int T, int B, int C, const int* lengths, float* dst,
+                      cudaStream_t stream);
+
 // db_ih / db_hh from the per-slice partial sums written by the backward recurrence:
 //   part [nslices][(G+1)*H]  (first G*H: sum of dGi columns; tail H: GRU sum of dn*r)
 //   GRU : db_ih = sum(part[:, :3H]);  db_hh = (sum part[:, :2H], sum part[:, 3H:4H])

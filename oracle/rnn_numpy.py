@@ -143,6 +143,48 @@ def _layer_backward(mode: str, x, w_ih, w_hh, cache, dy, dh_last, dc_last, rever
     return dx, dw_ih, dw_hh, db_ih, db_hh
 
 
+# ---- single steps in float64, with the magnitude each result is computed from ------------------------------------
+# Each returns the next state from a given previous one and, per element of the new state, the componentwise magnitude
+#   S = 1 + sum over the element's gate rows of (|b_ih| + |b_hh| + |W_ih| |x| + |W_hh| |h_prev|)
+# (LSTM: + |f c_prev| + |i g|): the sum of the absolute values of every term the kernel adds up for that element. A
+# floating-point evaluation of the step with unit roundoff u errs by a small multiple of u * S per element (the "1" holds
+# the activations to their absolute accuracy); tests/test_gpu_numerics_f64.py states the multiple.
+
+def _f64(*a):
+    return [np.asarray(v, dtype=np.float64) for v in a]
+
+
+def gru_step(x, h, w_ih, w_hh, b_ih, b_hh):
+    """x [B,I], h [B,H] -> (h' [B,H], S [B,H]); torch gate order r, z, n"""
+    x, h, w_ih, w_hh, b_ih, b_hh = _f64(x, h, w_ih, w_hh, b_ih, b_hh)
+    H = h.shape[1]
+    gi, gh = x @ w_ih.T + b_ih, h @ w_hh.T + b_hh
+    r = _sigmoid(gi[:, :H] + gh[:, :H])
+    z = _sigmoid(gi[:, H:2 * H] + gh[:, H:2 * H])
+    n = np.tanh(gi[:, 2 * H:] + r * gh[:, 2 * H:])
+    mag = np.abs(x) @ np.abs(w_ih).T + np.abs(h) @ np.abs(w_hh).T + np.abs(b_ih) + np.abs(b_hh)  # [B, 3H]
+    S = 1.0 + mag.reshape(-1, 3, H).sum(axis=1) + np.abs(h)
+    return (1.0 - z) * n + z * h, S
+
+
+def lstm_step(x, h, c, w_ih, w_hh, b_ih, b_hh, w_hr=None):
+    """x [B,I], h [B,HO], c [B,H] -> (h' [B,HO], c' [B,H], S_h [B,HO], S_c [B,H]); gate order i, f, g, o.
+    With w_hr [P,H] (proj_size = P) the new state is h' = W_hr (o tanh(c')), and S_h = 1 + |W_hr| S_m with S_m the
+    magnitude of o tanh(c')."""
+    x, h, c, w_ih, w_hh, b_ih, b_hh = _f64(x, h, c, w_ih, w_hh, b_ih, b_hh)
+    H = c.shape[1]
+    a = x @ w_ih.T + h @ w_hh.T + b_ih + b_hh
+    i, f, g, o = _sigmoid(a[:, :H]), _sigmoid(a[:, H:2 * H]), np.tanh(a[:, 2 * H:3 * H]), _sigmoid(a[:, 3 * H:])
+    c_new = f * c + i * g
+    m = o * np.tanh(c_new)
+    mag = np.abs(x) @ np.abs(w_ih).T + np.abs(h) @ np.abs(w_hh).T + np.abs(b_ih) + np.abs(b_hh)  # [B, 4H]
+    S_c = 1.0 + mag.reshape(-1, 4, H).sum(axis=1) + np.abs(f * c) + np.abs(i * g)
+    if w_hr is None:
+        return m, c_new, S_c, S_c
+    w_hr = np.asarray(w_hr, dtype=np.float64)
+    return m @ w_hr.T, c_new, 1.0 + S_c @ np.abs(w_hr).T, S_c
+
+
 class NumpyRNN:
     """Multi-layer (bi)directional GRU/LSTM, time-major [T,B,*], with an explicit backward."""
 

@@ -191,3 +191,67 @@ def test_ref_models_match_reference_live(key, name, cls, regression, shape):
     with torch.no_grad():
         out = mine(params.inputs_for("live:" + key, shape))
     assert np.abs(out.numpy() - arrays["out:" + key]).max() < 1e-6
+
+
+# ---- float64 single steps (oracle.rnn_numpy.gru_step / lstm_step), the per-step reference of the GPU numerics tests --
+
+def _saturating(shape, scale, g):
+    return (scale * torch.randn(shape, generator=g, dtype=torch.float64)).numpy()
+
+
+@pytest.mark.parametrize("scale", [0.3, 4.0])
+def test_gru_step_matches_grucell_f64(scale):
+    from oracle.rnn_numpy import gru_step
+
+    g = torch.Generator().manual_seed(1)
+    I, H, B = 9, 6, 5
+    cell = torch.nn.GRUCell(I, H).double()
+    with torch.no_grad():
+        for p in cell.parameters():
+            p.copy_(torch.from_numpy(_saturating(p.shape, scale, g)))
+    x, h = _saturating((B, I), 2.0, g), np.tanh(_saturating((B, H), 1.0, g))
+    w_ih, w_hh, b_ih, b_hh = [p.detach().numpy() for p in cell.parameters()]
+    h1, S = gru_step(x, h, w_ih, w_hh, b_ih, b_hh)
+    ref = cell(torch.from_numpy(x), torch.from_numpy(h)).detach().numpy()
+    assert np.abs(h1 - ref).max() <= 1e-14
+    # S: 1 + |h| + the absolute terms of the element's three gate rows
+    mag = (np.abs(x) @ np.abs(w_ih).T + np.abs(h) @ np.abs(w_hh).T + np.abs(b_ih) + np.abs(b_hh)).reshape(B, 3, H)
+    assert np.allclose(S, 1.0 + np.abs(h) + mag.sum(axis=1), rtol=1e-14, atol=0)
+    assert (S >= 1.0).all()
+
+
+@pytest.mark.parametrize("proj", [0, 3])
+def test_lstm_step_matches_lstmcell_f64(proj):
+    from oracle.rnn_numpy import lstm_step
+
+    g = torch.Generator().manual_seed(2)
+    I, H, B = 7, 8, 4
+    HO = proj or H
+    cell = torch.nn.LSTMCell(I, H).double()
+    with torch.no_grad():
+        for p in cell.parameters():
+            p.copy_(torch.from_numpy(_saturating(p.shape, 2.0, g)))
+    w_ih, w_hh_full, b_ih, b_hh = [p.detach().numpy() for p in cell.parameters()]
+    x, c = _saturating((B, I), 2.0, g), _saturating((B, H), 5.0, g)
+    h = np.tanh(_saturating((B, HO), 1.0, g))
+    w_hr = _saturating((proj, H), 0.5, g) if proj else None
+    w_hh = w_hh_full[:, :HO]   # a projected cell contracts W_hh [4H, P] with the projected state
+    h1, c1, S_h, S_c = lstm_step(x, h, c, w_ih, w_hh, b_ih, b_hh, w_hr)
+    # stock torch.nn.LSTM with proj_size, one step from (h, c), is the reference for both
+    lstm = torch.nn.LSTM(I, H, proj_size=proj).double()
+    with torch.no_grad():
+        lstm.weight_ih_l0.copy_(torch.from_numpy(w_ih))
+        lstm.weight_hh_l0.copy_(torch.from_numpy(w_hh))
+        lstm.bias_ih_l0.copy_(torch.from_numpy(b_ih))
+        lstm.bias_hh_l0.copy_(torch.from_numpy(b_hh))
+        if proj:
+            lstm.weight_hr_l0.copy_(torch.from_numpy(w_hr))
+        _, (hr, cr) = lstm(torch.from_numpy(x)[None], (torch.from_numpy(h)[None], torch.from_numpy(c)[None]))
+    assert np.abs(h1 - hr[0].numpy()).max() <= 1e-14
+    assert np.abs(c1 - cr[0].numpy()).max() <= 1e-13
+    if not proj:   # the unprojected step is LSTMCell's
+        h2, c2 = cell(torch.from_numpy(x), (torch.from_numpy(h), torch.from_numpy(c)))
+        assert np.abs(h1 - h2.detach().numpy()).max() <= 1e-14
+        assert S_h is S_c
+    assert (S_c >= 1.0 + np.abs(c1) - 1e-12).all()   # |c'| <= |f c| + |i g| < S_c
+    assert S_h.shape == (B, HO) and (S_h >= 1.0).all()
