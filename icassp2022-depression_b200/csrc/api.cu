@@ -8,6 +8,7 @@
 #include <atomic>
 #include <mutex>
 #include <stdarg.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "gemm_f32.cuh"
@@ -156,6 +157,9 @@ struct ScratchLayout {
   size_t order;
 };
 
+// split-K partials of the tensor-core gradient GEMMs: <= (#SMs / tiles) * M * N floats
+constexpr size_t TC_PART_BYTES = (size_t)160 * 128 * 128 * sizeof(float);
+
 void make_scratch(const Dims& d, ScratchLayout* s) {
   size_t off = ALIGN_F;  // header (dropout seed/offset when nothing is saved for backward)
   for (int k = 0; k < d.D; ++k) {
@@ -212,7 +216,7 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
     s->b_tc_y = off;   off += align_up(2 * d.TB * d.H, ALIGN_F);
     s->b_tc_w = off;   off += align_up(2 * Imax * d.GH, ALIGN_F);
     s->b_tc_part = off;
-    s->b_tc_part_bytes = (size_t)160 * 128 * 128 * sizeof(float);  // <= (#SMs / tiles) * M * N
+    s->b_tc_part_bytes = TC_PART_BYTES;
     off += align_up(s->b_tc_part_bytes / sizeof(float), ALIGN_F);
   }
   s->b_dxln = off;
@@ -281,9 +285,42 @@ struct GradGemm {
   int accumulate;
   bool splitk;  // split-K over the long T*B contraction of a wgrad (FFMA: the gemm workspace, tensor cores: b_tc_part)
   bool tc;      // tensor-core presplit GEMM (3xTF32, or single-pass TF32 with `tf32`); FFMA otherwise
+  const char* what = "gemm";  // the product, named in the B200RNN_DEBUG line
 };
 
-int run_grad_gemm(const GradGemm& g, const ScratchLayout& sl, float* S, bool tf32, cudaStream_t st) {
+// The K splits a gradient GEMM runs with, as its launcher chooses them: `splitk` splits of `chunk` k-blocks of 32
+// (tensor cores) or `chunk` K values (FFMA) each; the last split may be shorter
+struct GradPlan {
+  int splitk, chunk;
+};
+
+GradPlan grad_gemm_plan(const GradGemm& g, const ScratchLayout& sl, float* S) {
+  GradPlan p;
+  if (g.tc) {
+    tc_splitk_plan(g.M, g.N, g.K, g.splitk, g.splitk ? sl.b_tc_part_bytes : 0, &p.splitk, &p.chunk);
+  } else {
+    const bool ws = g.splitk && sl.b_gemm_bytes;
+    gemm_splitk_plan(g.M, g.N, g.K, ws ? S + sl.b_gemm : nullptr, ws ? sl.b_gemm_bytes : 0, &p.splitk, &p.chunk);
+  }
+  return p;
+}
+
+// plan (optional): receives the GradPlan the launch runs with. B200RNN_DEBUG: one line per GEMM (host side only)
+int run_grad_gemm(const GradGemm& g, const ScratchLayout& sl, float* S, bool tf32, cudaStream_t st,
+                  GradPlan* plan = nullptr) {
+  static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
+  if (debug || plan) {
+    const GradPlan p = grad_gemm_plan(g, sl, S);
+    if (plan) *plan = p;
+    // the FFMA GEMM is fp32 whatever the TF32 flag says
+    if (debug)
+      fprintf(stderr,
+              "[b200rnn] grad gemm %s: M=%d N=%d K=%d path=%s a=%s b=%s a_row0=%d b_row0=%d splitk=%d %s=%d "
+              "accumulate=%d tf32=%d\n",
+              g.what, g.M, g.N, g.K, g.tc ? "tc" : "ffma", g.a.kcontig ? "k" : "mn", g.b.kcontig ? "k" : "mn",
+              g.a.row0, g.b.row0, p.splitk, g.tc ? "kb_per_split" : "k_chunk", p.chunk, g.accumulate,
+              (g.tc && tf32) ? 1 : 0);
+  }
   if (!g.tc) {
     GemmParams p;
     memset(&p, 0, sizeof(p));
@@ -849,7 +886,7 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
       GradSrc w_ih{pp[0], simple_rows(Il), GH, Il, S + sl.b_tc_w, false};
       if (dw_ih) {  // dW_ih[GH, Il] = sum_tb dG[tb, :]^T X_l[tb, :]
         rc = run_grad_gemm({{&dG, 0, false}, {&X, 0, false}, GH, Il, TB, dw_ih, simple_rows(Il), accumulate, true,
-                            tc_l && aligned_to(dw_ih, 16)}, sl, S, tf32, st);
+                            tc_l && aligned_to(dw_ih, 16), "dW_ih"}, sl, S, tf32, st);
         if (rc) return rc;
       }
       if (dw_hh) {
@@ -859,11 +896,11 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
         const int g0 = k == 0 ? d.B : 0, Kp = (d.T - 1) * d.B;
         const bool gru = d.mode == B200RNN_GRU, tc = tc_l && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0;
         rc = run_grad_gemm({{&dG, g0, false}, {&h, d.B - g0, false}, gru ? 2 * d.H : GH, d.HO, Kp, dw_hh,
-                            simple_rows(d.HO), accumulate, true, tc}, sl, S, tf32, st);
+                            simple_rows(d.HO), accumulate, true, tc, gru ? "dW_hh_rz" : "dW_hh"}, sl, S, tf32, st);
         if (rc) return rc;
         if (gru) {
           rc = run_grad_gemm({{&dnr, g0, false}, {&h, d.B - g0, false}, d.H, d.HO, Kp, dw_hh + (size_t)2 * d.H * d.HO,
-                              simple_rows(d.HO), accumulate, true, tc}, sl, S, tf32, st);
+                              simple_rows(d.HO), accumulate, true, tc, "dW_hh_n"}, sl, S, tf32, st);
           if (rc) return rc;
         }
       }
@@ -876,19 +913,19 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
         rc = launch_initial_state_rows(dG.p, dnr.p, d.mode, d.B, d.T, d.H, k == 1, lengths, S + sl.b_h0, st);
         if (rc) return rc;
         rc = run_grad_gemm({{&rows0, 0, false}, {&h0, 0, false}, GH, d.HO, d.B, dw_hh, simple_rows(d.HO), 1, false,
-                            false}, sl, S, tf32, st);
+                            false, "dW_hh_h0"}, sl, S, tf32, st);
         if (rc) return rc;
       }
       if (d.P > 0 && gp[4]) {  // dW_hr[P, H] = sum_tb dh[tb, :]^T m[tb, :] (frozen and skipped steps have dh = 0)
         GradSrc dhp{S + sl.b_dhp[k], simple_rows(d.P), TB, d.P, nullptr, false};
         GradSrc m{R + rl.m[l][k], simple_rows(d.H), TB, d.H, nullptr, false};
         rc = run_grad_gemm({{&dhp, 0, false}, {&m, 0, false}, d.P, d.H, TB, gp[4], simple_rows(d.H), accumulate, true,
-                            false}, sl, S, tf32, st);
+                            false, "dW_hr"}, sl, S, tf32, st);
         if (rc) return rc;
       }
       if (want_dx) {  // dX_l (+)= dG[TB, GH] W_ih[GH, Il]: dG read K-major, W_ih as it lies
-        rc = run_grad_gemm({{&dG, 0, true}, {&w_ih, 0, false}, TB, Il, GH, Cx, cx_rows, k > 0, false, tc_dx}, sl, S,
-                           tf32, st);
+        rc = run_grad_gemm({{&dG, 0, true}, {&w_ih, 0, false}, TB, Il, GH, Cx, cx_rows, k > 0, false, tc_dx, "dX"}, sl,
+                           S, tf32, st);
         if (rc) return rc;
       }
     }
@@ -1010,6 +1047,99 @@ B200RNN_API int b200rnn_debug_gemm_f32a(int M, int N, int K, const float* A, int
     return B200RNN_ERR_UNSUPPORTED;
   }
   return launch_gemm_tc(g, scratch, scratch_bytes, static_cast<cudaStream_t>(stream_));
+}
+
+/* test only (not declared in the public header): gradient GEMMs as the backward runs them, through run_grad_gemm,
+   in order, over shared sources (a source is split for the tensor cores by the first GEMM that reads it).
+   srcs: nsrc rows of 6 int64 {pointer, s_outer, s_inner, inner_n, R, C}: an fp32 [R][C], row r at pointer +
+   s_outer * (r / inner_n) + s_inner * (r % inner_n) floats.
+   gemms: ngemm rows of 16 int64 {a_src, a_row0, a_kcontig, b_src, b_row0, b_kcontig, M, N, K, C pointer, c_s_outer,
+   c_s_inner, c_inner_n, accumulate, splitk, tc}. tf32: single-pass TF32 tensor-core GEMMs (B200RNN_FLAG_TF32).
+   The scratch is laid out as the backward's: split-K workspaces of the backward's sizes, one split region per source.
+   scratch == NULL: *scratch_bytes receives the size needed. plans (optional): per GEMM the split count and its chunk
+   (k-blocks of 32 on the tensor cores, K values on FFMA) the launch ran with. */
+B200RNN_API int b200rnn_debug_grad_gemm(const int64_t* srcs, int nsrc, const int64_t* gemms, int ngemm, int tf32,
+                                        void* scratch, size_t* scratch_bytes, int* plans, void* stream_) {
+  constexpr int MAX_SRC = 16;
+  if (!srcs || !gemms || !scratch_bytes || nsrc < 1 || nsrc > MAX_SRC || ngemm < 0) {
+    set_error("debug_grad_gemm: bad arguments");
+    return B200RNN_ERR_INVALID;
+  }
+  GradSrc src[MAX_SRC];
+  size_t gb = 0, off = 0;
+  for (int j = 0; j < ngemm; ++j) {  // the FFMA split-K workspace: the backward's formula, largest over the GEMMs
+    const int64_t* q = gemms + (size_t)j * 16;
+    if (q[14] && !q[15]) {
+      const size_t b = gemm_scratch_bytes((int)q[6], (int)q[7], (int)q[8]);
+      gb = b > gb ? b : gb;
+    }
+  }
+  ScratchLayout sl;
+  memset(&sl, 0, sizeof(sl));
+  sl.b_gemm = off;
+  sl.b_gemm_bytes = gb;
+  off += align_up(gb / sizeof(float) + 1, ALIGN_F);
+  size_t split_off[MAX_SRC];
+  for (int i = 0; i < nsrc; ++i) {
+    const int64_t* q = srcs + (size_t)i * 6;
+    if (!q[0] || q[3] < 1 || q[4] < 1 || q[5] < 1) {
+      set_error("debug_grad_gemm: source %d: null pointer or empty shape", i);
+      return B200RNN_ERR_INVALID;
+    }
+    src[i] = GradSrc{reinterpret_cast<const float*>(q[0]), RowMap{q[1], q[2], (int)q[3]}, (int)q[4], (int)q[5],
+                     nullptr, false};
+    split_off[i] = off;
+    off += align_up(2 * (size_t)q[4] * q[5], ALIGN_F);
+  }
+  sl.b_tc_part = off;
+  sl.b_tc_part_bytes = TC_PART_BYTES;
+  off += align_up(TC_PART_BYTES / sizeof(float), ALIGN_F);
+  if (!scratch) {
+    *scratch_bytes = off * sizeof(float);
+    return B200RNN_OK;
+  }
+  if (*scratch_bytes < off * sizeof(float) || !aligned_to(scratch, 256)) {
+    set_error("debug_grad_gemm: the scratch must be 256-byte aligned and hold %zu bytes", off * sizeof(float));
+    return B200RNN_ERR_INVALID;
+  }
+  float* S = static_cast<float*>(scratch);
+  for (int i = 0; i < nsrc; ++i) src[i].split = S + split_off[i];
+  for (int j = 0; j < ngemm; ++j) {
+    const int64_t* q = gemms + (size_t)j * 16;
+    GradGemm g{{nullptr, (int)q[1], q[2] != 0}, {nullptr, (int)q[4], q[5] != 0}, (int)q[6], (int)q[7], (int)q[8],
+               reinterpret_cast<float*>(q[9]), RowMap{q[10], q[11], (int)q[12]}, (int)q[13], q[14] != 0, q[15] != 0,
+               "debug"};
+    // every access stays inside the sources: a kcontig operand reads rows [row0, row0 + M or N) and columns [0, K),
+    // the others rows [row0, row0 + K) and columns [0, M or N); a row offset must keep the row map linear
+    for (int o = 0; o < 2; ++o) {
+      GradOperand& op = o ? g.b : g.a;
+      const int si = (int)(o ? q[3] : q[0]), mn = o ? g.N : g.M;
+      if (si < 0 || si >= nsrc) {
+        set_error("debug_grad_gemm: gemm %d: no source %d", j, si);
+        return B200RNN_ERR_INVALID;
+      }
+      op.src = &src[si];
+      const GradSrc& s = src[si];
+      const int rows = op.kcontig ? mn : g.K, cols = op.kcontig ? g.K : mn;
+      const bool linear = s.rows.inner_n >= s.R || op.row0 % s.rows.inner_n == 0;
+      if (op.row0 < 0 || (long long)op.row0 + rows > s.R || cols > s.C || !linear || (g.tc && s.C % 4 != 0)) {
+        set_error("debug_grad_gemm: gemm %d operand %d does not fit source %d", j, o, si);
+        return B200RNN_ERR_INVALID;
+      }
+    }
+    if (g.M < 1 || g.N < 1 || g.K < 1 || !g.C || g.c_rows.inner_n < 1) {
+      set_error("debug_grad_gemm: gemm %d: bad shape or output", j);
+      return B200RNN_ERR_INVALID;
+    }
+    GradPlan p;
+    const int rc = run_grad_gemm(g, sl, S, tf32 != 0, static_cast<cudaStream_t>(stream_), &p);
+    if (rc) return rc;
+    if (plans) {
+      plans[2 * j] = p.splitk;
+      plans[2 * j + 1] = p.chunk;
+    }
+  }
+  return B200RNN_OK;
 }
 
 }  // extern "C"

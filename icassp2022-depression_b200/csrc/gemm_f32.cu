@@ -252,6 +252,12 @@ void launch_tile(const GemmDev& d, bool a_kc, bool b_kc, dim3 grid, cudaStream_t
 
 }  // namespace
 
+void gemm_splitk_plan(int M, int N, int K, void* scratch, size_t scratch_bytes, int* splitk, int* k_chunk) {
+  const Plan pl = make_plan(M, N, K > 0 ? K : 1, scratch_bytes, scratch != nullptr);
+  *splitk = K > 0 ? pl.splitk : 1;
+  *k_chunk = K > 0 ? pl.k_chunk : BK;
+}
+
 int launch_splitk_reduce(const float* partial, int splitk, int M, int N, float* C, const RowMap& c_rows,
                          const float* bias1, const float* bias2, int bias2_n, int accumulate, cudaStream_t stream) {
   size_t total = (size_t)M * N;

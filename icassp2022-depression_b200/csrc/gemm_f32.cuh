@@ -95,6 +95,10 @@ int launch_splitk_reduce(const float* partial, int splitk, int M, int N, float* 
 
 // bytes of scratch launch_gemm may use for split-K partials for this problem (0 if none wanted)
 size_t gemm_scratch_bytes(int M, int N, int K);
+// the K splits launch_gemm's FFMA path runs with this scratch, and the K range of each (the last may be shorter)
+void gemm_splitk_plan(int M, int N, int K, void* scratch, size_t scratch_bytes, int* splitk, int* k_chunk);
+// the K splits tc_gemm_presplit runs (a workspace of ws_bytes when have_ws), and the k-blocks of 32 in each
+void tc_splitk_plan(int M, int N, int K, bool have_ws, size_t ws_bytes, int* splitk, int* kb_per_split);
 
 // Enqueue on `stream`. `scratch` may be NULL (then no split-K). Returns B200RNN_* code.
 int launch_gemm(const GemmParams& p, void* scratch, size_t scratch_bytes, cudaStream_t stream);

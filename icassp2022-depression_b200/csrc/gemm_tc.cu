@@ -952,6 +952,23 @@ int launch_tc(const CUtensorMap (&m)[4], const TcArgs& a, int stream_clusters, c
 
 }  // namespace
 
+void tc_splitk_plan(int M, int N, int K, bool have_ws, size_t ws_bytes, int* splitk_out, int* kb_per_split) {
+  const int ntiles = ((M + BM - 1) / BM) * (N / BN);
+  const int nkb = (K + BK - 1) / BK;
+  const int sms = num_sms();
+  // split-K when the tile count cannot fill the chip and K is long (the wgrad shapes: K = T*B)
+  int splitk = 1;
+  if (have_ws && ntiles * 2 <= sms && nkb >= 16) {
+    splitk = sms / ntiles;
+    if (splitk > nkb / 8) splitk = nkb / 8;
+    const size_t per = (size_t)M * N * sizeof(float);
+    while (splitk > 1 && per * splitk > ws_bytes) --splitk;
+    if (splitk < 1) splitk = 1;
+  }
+  *kb_per_split = (nkb + splitk - 1) / splitk;
+  *splitk_out = (nkb + *kb_per_split - 1) / *kb_per_split;
+}
+
 // C[M,N] (+)= A[M,K] * B[N,K]^T (+ biases), operands already split into hi/lo matrices (K- or MN-major).
 int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K, float* C, const RowMap& c_rows,
                      const float* bias1, const float* bias2, int bias2_n, int accumulate, void* splitk_ws,
@@ -972,20 +989,7 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
   a.a_hi = A.hi; a.a_lo = A.lo; a.lda = A.ld;
   a.b_hi = B.hi; a.b_lo = B.lo; a.ldb = B.ld;
   a.tf32 = tf32 ? 1 : 0;
-  const int ntiles = a.tiles_m * a.tiles_n;
-  const int nkb = (K + BK - 1) / BK;
-  const int sms = num_sms();
-  // split-K when the tile count cannot fill the chip and K is long (the wgrad shapes: K = T*B)
-  int splitk = 1;
-  if (splitk_ws && ntiles * 2 <= sms && nkb >= 16) {
-    splitk = sms / ntiles;
-    if (splitk > nkb / 8) splitk = nkb / 8;
-    const size_t per = (size_t)M * N * sizeof(float);
-    while (splitk > 1 && per * splitk > splitk_ws_bytes) --splitk;
-    if (splitk < 1) splitk = 1;
-  }
-  a.kb_per_split = (nkb + splitk - 1) / splitk;
-  a.splitk = (nkb + a.kb_per_split - 1) / a.kb_per_split;
+  tc_splitk_plan(M, N, K, splitk_ws != nullptr, splitk_ws_bytes, &a.splitk, &a.kb_per_split);
   a.partial = static_cast<float*>(splitk_ws);
   rc = launch_tc(m, a, stream_clusters, stream);
   if (rc) return rc;

@@ -1,11 +1,16 @@
 """Do the numerics tests bite? Build the library with one small arithmetic mutation at a time and run the tests on it.
 
 Each mutation is one textual edit of csrc/ that changes arithmetic only - no indexing, barrier or memory access - and is
-applied to a copy of the sources in a temporary directory; that copy is built (make, as build() does) and loaded with
-B200RNN_LIB. Against each build the script runs tests/test_gpu_numerics_f64.py and the existing GPU numerics tests, and
-records per mutation which tests fail. A mutation that no new test catches is a hole in the suite.
+applied to a copy of the sources; that copy is built (make, as build() does, reusing the tree's objects so that only
+the mutated file recompiles) and loaded with B200RNN_LIB. Each mutation names the new tests that must catch it and the
+existing tests it is also run against. Against each build the script runs the new tests (stopping after a few
+failures) and then the existing files in order, each until its first failure, stopping at the first file that fails;
+it records per mutation which tests fail. A mutation that no new test catches is a hole in the suite.
 
     python tools/numerics_mutants.py [--only NAME ...] [--out tools/numerics_mutants_results.json]
+    # build where nvcc is, run where the GPU is (the builds are kept under --build-dir and reused):
+    python tools/numerics_mutants.py --build-only --build-dir build/mutants
+    python tools/numerics_mutants.py --build-dir build/mutants
 """
 import argparse
 import json
@@ -20,20 +25,45 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "icassp2022-depression_b200")
 sys.path[:0] = [ROOT, PKG]
 
-# name -> (file under csrc/, text, replacement, what it breaks)
+REC_NEW = ["tests/test_gpu_numerics_f64.py"]
+REC_EXISTING = ["tests/test_gpu_parity.py", "tests/test_gpu_property.py", "tests/test_gpu_coverage.py",
+                "tests/test_gpu_varlen.py", "tests/test_gpu_proj.py", "tests/test_gpu_h16_fwd.py"]
+GEMM_NEW = ["tests/test_gpu_grad_gemm_f64.py"]
+GEMM_EXISTING = ["tests/test_gpu_gemm.py", "tests/test_gpu_gemm_f32a.py", "tests/test_gpu_grad_paths.py",
+                 "tests/test_gpu_parity.py", "tests/test_gpu_tf32_mode.py"]
+
+# name -> (file under csrc/, text, replacement, what it breaks, new tests, existing tests)
 MUTATIONS = {
     "x3_drop_ah_bl": ("rnn_rec.cu", "            ptx::mma_tf32_m16n8k8(d[g][0], ah, bl);\n", "",
-                      "3xTF32 tc8 recurrence: the hi(W) * lo(h) correction mma is lost"),
+                      "3xTF32 tc8 recurrence: the hi(W) * lo(h) correction mma is lost", REC_NEW, REC_EXISTING),
     "f16_drop_ah_bl": ("rnn_rec.cu", "            ptx::mma_f16_m16n8k16(d[g][0], ah, bl);\n", "",
-                       "fp16-pair tc8 recurrence: the hi(W) * lo(h) correction mma is lost"),
+                       "fp16-pair tc8 recurrence: the hi(W) * lo(h) correction mma is lost", REC_NEW, REC_EXISTING),
     "fwdcell_drop_bhn": ("rnn_rec.cu", "const float hn = pre[2] + bhn;", "const float hn = pre[2];",
-                         "every GRU forward config: b_hn left out of the candidate gate"),
+                         "every GRU forward config: b_hn left out of the candidate gate", REC_NEW, REC_EXISTING),
     "bwd_drop_one_minus_r": ("rnn_rec.cu", "const float dr = dn * hn * r * (1.f - r);", "const float dr = dn * hn * r;",
-                             "GRU BPTT: the sigmoid derivative of r loses its (1 - r) factor"),
+                             "GRU BPTT: the sigmoid derivative of r loses its (1 - r) factor", REC_NEW, REC_EXISTING),
+    # the first MMA of a k-step zeroes the accumulator at k = 0: the one that follows takes over that flag
+    "tc_drop_alo_bhi": ("gemm_tc.cu",
+                        "          wgmma_tf32_m64n128k8(acc, a_lo + adv, b_hi + adv, k != 0);\n"
+                        "          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_lo + adv, 1);\n",
+                        "          wgmma_tf32_m64n128k8(acc, a_hi + adv, b_lo + adv, k != 0);\n",
+                        "presplit / MN-major tensor-core GEMM (gradient GEMMs): the lo(A) * hi(B) product is lost",
+                        GEMM_NEW, GEMM_EXISTING),
+    "tc_ra_drop_ah_bl": ("gemm_tc.cu",
+                         "          wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k + 4], b_hi + adv, k != 0);\n"
+                         "          wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k], b_lo + adv, 1);\n",
+                         "          wgmma_tf32_m64n128k8_ra(acc, &fa[8 * k + 4], b_hi + adv, k != 0);\n",
+                         "fp32-A tensor-core GEMM (forward input projection): the hi(A) * lo(W) product is lost",
+                         GEMM_NEW, GEMM_EXISTING),
+    "tc_epilogue_drop_accumulate": ("gemm_tc.cu", "              o.x += old.x; o.y += old.y;\n", "",
+                                    "tensor-core epilogue: accumulate = 1 overwrites C instead of adding to it",
+                                    GEMM_NEW, GEMM_EXISTING),
+    "splitk_reduce_drop_accumulate": ("gemm_f32.cu", "    if (accumulate) s += *dst;\n", "",
+                                      "split-K reduce (both paths): accumulate = 1 overwrites C", GEMM_NEW,
+                                      GEMM_EXISTING),
+    "ffma_epilogue_drop_accumulate": ("gemm_f32.cu", "            if (p.accumulate) o += dst[e];\n", "",
+                                      "FFMA epilogue: accumulate = 1 overwrites C", GEMM_NEW, GEMM_EXISTING),
 }
-NEW = "tests/test_gpu_numerics_f64.py"
-EXISTING = ["tests/test_gpu_parity.py", "tests/test_gpu_property.py", "tests/test_gpu_coverage.py",
-            "tests/test_gpu_varlen.py", "tests/test_gpu_proj.py", "tests/test_gpu_h16_fwd.py"]
 
 
 def gpu_info():
@@ -48,11 +78,18 @@ def gpu_info():
 
 
 def build(tmp, name):
-    """the mutated library: copies of csrc/, the Makefile and include/ under tmp, one edit, make"""
-    src, before, after, _ = MUTATIONS[name]
+    """the mutated library: copies of csrc/, the Makefile, the tree's objects and include/ under tmp, one edit, make;
+    an existing build there is reused"""
+    src, before, after = MUTATIONS[name][:3]
     pkg = os.path.join(tmp, name, "pkg")
+    lib = os.path.join(pkg, "lib", "libb200rnn.so")
+    if os.path.exists(lib):
+        return lib
+    shutil.rmtree(os.path.join(tmp, name), ignore_errors=True)
     shutil.copytree(os.path.join(PKG, "csrc"), os.path.join(pkg, "csrc"))
-    shutil.copy(os.path.join(PKG, "Makefile"), pkg)
+    shutil.copy2(os.path.join(PKG, "Makefile"), pkg)
+    if os.path.isdir(os.path.join(PKG, "build")):   # objects newer than their sources: only the edited file rebuilds
+        shutil.copytree(os.path.join(PKG, "build"), os.path.join(pkg, "build"))
     shutil.copytree(os.path.join(ROOT, "include"), os.path.join(tmp, name, "include"))
     path = os.path.join(pkg, "csrc", src)
     text = open(path).read()
@@ -62,7 +99,7 @@ def build(tmp, name):
         f.write(text.replace(before, after))
     jobs = str(max(1, min(8, os.cpu_count() or 1)))
     subprocess.run(["make", "-C", pkg, "-j", jobs], check=True, capture_output=True)
-    return os.path.join(pkg, "lib", "libb200rnn.so")
+    return lib
 
 
 def failing(lib, paths, maxfail=None):
@@ -79,22 +116,35 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", nargs="*", choices=list(MUTATIONS))
     ap.add_argument("--out", default=os.path.join(ROOT, "tools", "numerics_mutants_results.json"))
+    ap.add_argument("--build-dir", help="keep (and reuse) the mutated builds here instead of a temporary directory")
+    ap.add_argument("--build-only", action="store_true", help="build the mutated libraries, run nothing")
+    ap.add_argument("--new-maxfail", type=int, default=5, help="stop the new tests after this many failures")
     args = ap.parse_args()
-    res = {"mutations": {}}
-    if os.path.exists(args.out):   # a run of some mutations (--only) adds to the results of the others
-        with open(args.out) as f:
-            res = json.load(f)
-    res["device"] = gpu_info()
+    names = args.only or list(MUTATIONS)
     with tempfile.TemporaryDirectory() as tmp:
-        for name in args.only or MUTATIONS:
-            lib = build(tmp, name)
-            new = failing(lib, [NEW])
-            old = {p: failing(lib, [p], maxfail=1) for p in EXISTING}
+        where = os.path.abspath(args.build_dir) if args.build_dir else tmp
+        if args.build_only:
+            for name in names:
+                print(name, build(where, name), flush=True)
+            return 0
+        res = {"mutations": {}}
+        if os.path.exists(args.out):   # a run of some mutations (--only) adds to the results of the others
+            with open(args.out) as f:
+                res = json.load(f)
+        res["device"] = gpu_info()
+        for name in names:
+            src, before, after, breaks, new_paths, old_paths = MUTATIONS[name]
+            lib = build(where, name)
+            new = failing(lib, new_paths, maxfail=args.new_maxfail)
+            old = {}
+            for p in old_paths:   # the first existing file that catches the mutation is enough
+                old[p] = failing(lib, [p], maxfail=1)
+                if old[p]:
+                    break
             res["mutations"][name] = {
-                "file": MUTATIONS[name][0], "replaced": MUTATIONS[name][1].strip(),
-                "with": MUTATIONS[name][2].strip(), "breaks": MUTATIONS[name][3],
-                "new_tests_failing": new, "caught_by_new_tests": bool(new),
-                "existing_first_failure": {p: f[0] for p, f in old.items() if f},
+                "file": src, "replaced": before.strip(), "with": after.strip(), "breaks": breaks,
+                "new_tests": new_paths, "new_tests_failing": new, "caught_by_new_tests": bool(new),
+                "existing_tests_run": list(old), "existing_first_failure": {p: f[0] for p, f in old.items() if f},
                 "caught_by_existing_tests": any(old.values()),
             }
             print(name, "new:", len(new), "existing:", res["mutations"][name]["caught_by_existing_tests"], flush=True)
