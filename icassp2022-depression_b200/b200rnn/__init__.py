@@ -6,7 +6,7 @@ Importing this package does not need a GPU; running any op does, and fails loudl
 """
 from . import _lib
 from ._lib import B200RNNError
-from .modules import GRU, LSTM, from_torch, install, uninstall
+from .modules import GRU, LSTM, GRUCell, LSTMCell, from_torch, install, uninstall
 from .functional import RNNConfig, gemm, rnn_forward
 from .staging import FuseBatch, PinnedStager, bind_host_thread_to_gpu_numa_node, stage_fuse_batch
 from .dp import GradBucket, broadcast_parameters, shard_batch
@@ -17,7 +17,7 @@ from .train_step import FuseFineTuneStep, TrainStep, softmax_cross_entropy
 from .dp import PeerComm
 
 __all__ = [
-    "GRU", "LSTM", "install", "uninstall", "from_torch", "rnn_forward", "gemm", "RNNConfig", "B200RNNError",
+    "GRU", "LSTM", "GRUCell", "LSTMCell", "install", "uninstall", "from_torch", "rnn_forward", "gemm", "RNNConfig", "B200RNNError",
     "AudioBiLSTM", "TextBiLSTM", "fusion_net", "MyLoss", "attention_pool", "FuseBatch", "PinnedStager",
     "stage_fuse_batch", "GradBucket", "broadcast_parameters", "shard_batch", "FusedFuseStep", "FlatAdamW",
     "TrainStep", "FuseFineTuneStep", "softmax_cross_entropy", "PeerComm",

@@ -19,6 +19,7 @@ FLAG_SAVE_FOR_BACKWARD = 2
 FLAG_FUSED_LN = 4
 FLAG_TF32 = 8
 FLAG_PROJ = 16      # the descriptor carries proj_size (read only with this flag)
+FLAG_NO_BIAS = 32   # cells only: bias=False
 ABI_VERSION = 4
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)
@@ -36,6 +37,9 @@ SYMBOLS = (
     "b200rnn_backward_hx",
     "b200rnn_wcache_bytes",
     "b200rnn_prepare_weights",
+    "b200rnn_cell_workspace_bytes",
+    "b200rnn_cell_forward",
+    "b200rnn_cell_backward",
     "b200rnn_gemm_f32",
     "b200rnn_attention_pool",
     "b200rnn_attention_pool_bwd",
@@ -76,6 +80,18 @@ class Desc(ctypes.Structure):
         ("dropout_p", c_float),
         ("flags", c_uint32),
         ("proj_size", c_int32),
+    ]
+
+
+class CellDesc(ctypes.Structure):
+    """``b200rnn_cell_desc`` (include/b200rnn.h): one GRUCell / LSTMCell call."""
+
+    _fields_ = [
+        ("mode", c_int32),
+        ("batch", c_int32),
+        ("input_size", c_int32),
+        ("hidden_size", c_int32),
+        ("flags", c_uint32),
     ]
 
 
@@ -220,6 +236,26 @@ def load() -> ctypes.CDLL:
         c_void_p, c_float, c_void_p, c_void_p,       # ln_gamma, ln_eps, dln_gamma, dln_beta
         c_void_p,                                    # stream
     ]
+    lib.b200rnn_cell_workspace_bytes.restype = c_int
+    lib.b200rnn_cell_workspace_bytes.argtypes = [POINTER(CellDesc), POINTER(c_size_t), POINTER(c_size_t)]
+    lib.b200rnn_cell_forward.restype = c_int
+    lib.b200rnn_cell_forward.argtypes = [
+        POINTER(CellDesc), c_void_p, c_int64,        # desc, x, x_ld
+        c_void_p, c_int64, c_void_p, c_int64,        # h, h_ld, c, c_ld
+        POINTER(c_void_p),                           # params
+        c_void_p, c_void_p, c_void_p,                # h_out, c_out, saved
+        c_void_p,                                    # stream
+    ]
+    lib.b200rnn_cell_backward.restype = c_int
+    lib.b200rnn_cell_backward.argtypes = [
+        POINTER(CellDesc), c_void_p, c_int64,        # desc, x, x_ld
+        c_void_p, c_int64, c_void_p, c_int64,        # h, h_ld, c, c_ld
+        POINTER(c_void_p),                           # params
+        c_void_p, c_void_p, c_void_p,                # dh_out, dc_out, saved
+        c_void_p, c_void_p, c_void_p,                # dx, dh, dc
+        POINTER(c_void_p),                           # dparams
+        c_void_p, c_void_p,                          # scratch, stream
+    ]
     lib.b200rnn_gemm_f32.restype = c_int
     lib.b200rnn_gemm_f32.argtypes = [
         c_int, c_int, c_int, c_void_p, c_int64, c_int, c_void_p, c_int64, c_int, c_void_p, c_int64, c_void_p,
@@ -286,6 +322,14 @@ def workspace_bytes(desc: Desc) -> tuple[int, int]:
     r, s = c_size_t(0), c_size_t(0)
     check(load().b200rnn_workspace_bytes(ctypes.byref(desc), ctypes.byref(r), ctypes.byref(s)), "workspace_bytes")
     return int(r.value), int(s.value)
+
+
+def cell_workspace_bytes(desc: CellDesc) -> tuple[int, int]:
+    """(saved, scratch) bytes of a cell call; raises with the library's message for an invalid descriptor"""
+    sv, s = c_size_t(0), c_size_t(0)
+    check(load().b200rnn_cell_workspace_bytes(ctypes.byref(desc), ctypes.byref(sv), ctypes.byref(s)),
+          "cell_workspace_bytes")
+    return int(sv.value), int(s.value)
 
 
 def ptr_array(ptrs) -> ctypes.Array:

@@ -450,6 +450,134 @@ def prepare_weights(weights: Sequence[torch.Tensor], cfg: RNNConfig) -> torch.Te
     return cache
 
 
+@dataclass
+class CellConfig:
+    mode: int            # _lib.GRU / _lib.LSTM
+    input_size: int
+    hidden_size: int
+    bias: bool
+    tf32: bool = False   # single-pass TF32 contraction and gradient GEMMs (tf32_enabled()), else 3xTF32
+
+
+def _cell_desc(cfg: CellConfig, B: int, save: bool) -> _lib.CellDesc:
+    flags = _lib.FLAG_SAVE_FOR_BACKWARD if save else 0
+    if cfg.tf32:
+        flags |= _lib.FLAG_TF32
+    if not cfg.bias:
+        flags |= _lib.FLAG_NO_BIAS
+    return _lib.CellDesc(cfg.mode, B, cfg.input_size, cfg.hidden_size, flags)
+
+
+def _cell_rows(t: torch.Tensor) -> torch.Tensor:
+    """``t`` [R, C] as the cell entry points take it: feature stride 1 and rows that do not overlap (copy if not)"""
+    if (t.stride(1) != 1 and t.size(1) != 1) or (t.size(0) > 1 and t.stride(0) < t.size(1)):
+        t = t.contiguous()
+    return t
+
+
+class _CellFunction(torch.autograd.Function):
+    """h' (GRU) or (h', c') (LSTM) = cell(x, h, c, weights) for x [B, I]; h / c are None (zeros) or [B, H]. The TF32
+    mode is in ``cfg``, read once per call, and the backward reuses it."""
+
+    # position of the first weight among forward()'s inputs (after ctx)
+    _W0 = 5
+
+    @staticmethod
+    def forward(ctx, x: torch.Tensor, cfg: CellConfig, save: bool, h: Optional[torch.Tensor],
+                c: Optional[torch.Tensor], *weights: torch.Tensor):
+        lib = _lib.load()
+        B, H, dev = x.size(0), cfg.hidden_size, x.device
+        # as in _RNNFunction: the caller decides from grad mode, needs_input_grad confirms
+        save = bool(save) and any(ctx.needs_input_grad)
+        desc = _cell_desc(cfg, B, save)
+        sv_bytes, _ = _lib.cell_workspace_bytes(desc)
+        saved = torch.empty(sv_bytes if save else 0, dtype=torch.uint8, device=dev)
+        h_out = torch.empty(B, H, dtype=torch.float32, device=dev)
+        c_out = torch.empty(B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        ld = lambda t: t.stride(0) if t is not None else 0  # noqa: E731
+        params = _lib.ptr_array([w.data_ptr() for w in weights] + [None] * (4 - len(weights)))
+        with _on(dev):
+            rc = lib.b200rnn_cell_forward(ctypes.byref(desc), x.data_ptr(), x.stride(0), ptr(h), ld(h), ptr(c), ld(c),
+                                          params, h_out.data_ptr(), ptr(c_out), saved.data_ptr() if save else None,
+                                          _stream_ptr(dev))
+        _lib.check(rc, "b200rnn_cell_forward")
+        if save:
+            ctx.cfg = cfg
+            ctx.save_for_backward(x, h, c, saved, *weights)
+        return h_out if c_out is None else (h_out, c_out)
+
+    @staticmethod
+    def backward(ctx, dh_out, dc_out=None):
+        lib = _lib.load()
+        cfg: CellConfig = ctx.cfg
+        x, h, c, saved, *weights = ctx.saved_tensors
+        B, I, H, dev = x.size(0), cfg.input_size, cfg.hidden_size, x.device
+        need = ctx.needs_input_grad
+        w0 = _CellFunction._W0
+        new = lambda n: torch.empty(B, n, dtype=torch.float32, device=dev)  # noqa: E731
+        dx = new(I) if need[0] else None
+        dh = new(H) if h is not None and need[w0 - 2] else None
+        dc = new(H) if c is not None and need[w0 - 1] else None
+        dptrs, grads_out, _ = _weight_grad_targets(weights, need[w0:], None, dev)
+        desc = _cell_desc(cfg, B, True)
+        _, sbytes = _lib.cell_workspace_bytes(desc)
+        scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+        dh_out = dh_out.contiguous() if dh_out is not None else None
+        dc_out = dc_out.contiguous() if dc_out is not None else None
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        ld = lambda t: t.stride(0) if t is not None else 0  # noqa: E731
+        params = _lib.ptr_array([w.data_ptr() for w in weights] + [None] * (4 - len(weights)))
+        dparams = _lib.ptr_array(dptrs + [None] * (4 - len(dptrs)))
+        with _on(dev):
+            rc = lib.b200rnn_cell_backward(ctypes.byref(desc), x.data_ptr(), x.stride(0), ptr(h), ld(h), ptr(c), ld(c),
+                                           params, ptr(dh_out), ptr(dc_out), saved.data_ptr(), ptr(dx), ptr(dh),
+                                           ptr(dc), dparams, scratch.data_ptr(), _stream_ptr(dev))
+        _lib.check(rc, "b200rnn_cell_backward")
+        return (dx, None, None, dh, dc, *grads_out)
+
+
+def cell_forward(x: torch.Tensor, hx, weights: Sequence[torch.Tensor], cfg: CellConfig, name: str):
+    """One GRUCell / LSTMCell step on batched input: ``x`` [B, I], ``hx`` None (zeros), ``h`` (GRU) or ``(h, c)``
+    (LSTM), each [B, H]; ``weights`` = (weight_ih, weight_hh[, bias_ih, bias_hh]). Shapes are checked as torch's
+    ``_VF.gru_cell`` / ``_VF.lstm_cell`` check them (same exception types and messages), before the missing CPU path.
+    Returns ``h'`` or ``(h', c')``."""
+    lstm = cfg.mode == _lib.LSTM
+    states = ()
+    if hx is not None:
+        if lstm and not isinstance(hx, (tuple, list)):
+            raise TypeError(f"lstm_cell(): argument 'hx' (position 2) must be tuple of Tensors, not {type(hx).__name__}")
+        states = tuple(hx) if lstm else (hx,)
+        if lstm and len(states) != 2:
+            raise RuntimeError("lstm_cell expects two hidden states")
+    if x.size(1) != cfg.input_size:
+        raise RuntimeError(f"input has inconsistent input_size: got {x.size(1)} expected {cfg.input_size}")
+    for idx, s in enumerate(states):
+        if s.size(0) != x.size(0):
+            raise RuntimeError(f"Input batch size {x.size(0)} doesn't match hidden{idx} batch size {s.size(0)}")
+        if s.size(1) != cfg.hidden_size:
+            raise RuntimeError(f"hidden{idx} has inconsistent hidden_size: got {s.size(1)}, expected {cfg.hidden_size}")
+    for s in states:
+        if s.device != x.device:
+            raise RuntimeError("Input and hidden tensors are not at the same device, found input tensor at "
+                               f"{x.device} and hidden tensor at {s.device}")
+        if s.dtype != x.dtype:
+            raise RuntimeError("Input and hidden tensors are not the same dtype, found input tensor with "
+                               f"{x.dtype} and hidden tensor with {s.dtype}")
+    _require_cuda_f32(x, "input")
+    for w in weights:
+        _require_cuda_f32(w, f"{name} weight")
+        if not w.is_contiguous():
+            raise _lib.B200RNNError(f"b200rnn: {name} weights must be contiguous")
+        if w.device != x.device:
+            raise _lib.B200RNNError(f"b200rnn: a {name} weight is on {w.device} but the input is on {x.device}")
+    x = _cell_rows(x)
+    states = tuple(_cell_rows(s) for s in states)
+    h, c = (states + (None, None))[:2]
+    save = torch.is_grad_enabled() and (x.requires_grad or any(t.requires_grad for t in (*weights, *states)))
+    return _CellFunction.apply(x, cfg, save, h, c, *weights)
+
+
 def gemm(a: torch.Tensor, b: torch.Tensor, *, a_kcontig: bool = True, b_kcontig: bool = True,
          bias: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, accumulate: bool = False,
          use_splitk: bool = True) -> torch.Tensor:

@@ -26,8 +26,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .functional import (RNNConfig, prepare_weights, rnn_forward, rnn_forward_fused, rnn_ln_pool_sum,
-                         tf32_enabled)
+from .functional import (CellConfig, RNNConfig, cell_forward, prepare_weights, rnn_forward, rnn_forward_fused,
+                         rnn_ln_pool_sum, tf32_enabled)
 
 _TORCH_GRU = nn.GRU
 _TORCH_LSTM = nn.LSTM
@@ -285,8 +285,91 @@ class LSTM(_B200RNNBase):
         return y, (h_n, c_n)
 
 
+class _B200CellBase(nn.Module):
+    """``torch.nn.GRUCell`` / ``LSTMCell`` (RNNCellBase): same constructor, parameters (``weight_ih``, ``weight_hh``,
+    ``bias_ih``, ``bias_hh``, registered as None with ``bias=False``), init, ``extra_repr`` and ``forward``. Any
+    ``input_size`` and ``hidden_size``. One fused launch per forward (csrc/cell.cu). Not rebound by :func:`install`:
+    use them by name or through :func:`from_torch`."""
+
+    _mode: int = -1
+    _gates: int = 0
+
+    def __init__(self, input_size: int, hidden_size: int, bias: bool = True, device=None, dtype=None) -> None:
+        super().__init__()
+        if dtype not in (None, torch.float32):
+            raise NotImplementedError("b200rnn: float32 only")
+        self.input_size = input_size
+        self.hidden_size = hidden_size
+        self.bias = bias
+        kw = dict(dtype=torch.float32, device=device)
+        self.weight_ih = nn.Parameter(torch.empty((self._gates * hidden_size, input_size), **kw))
+        self.weight_hh = nn.Parameter(torch.empty((self._gates * hidden_size, hidden_size), **kw))
+        if bias:
+            self.bias_ih = nn.Parameter(torch.empty(self._gates * hidden_size, **kw))
+            self.bias_hh = nn.Parameter(torch.empty(self._gates * hidden_size, **kw))
+        else:
+            self.register_parameter("bias_ih", None)
+            self.register_parameter("bias_hh", None)
+        self.reset_parameters()
+
+    def reset_parameters(self) -> None:
+        stdv = 1.0 / math.sqrt(self.hidden_size) if self.hidden_size > 0 else 0
+        for weight in self.parameters():
+            nn.init.uniform_(weight, -stdv, stdv)
+
+    def extra_repr(self) -> str:
+        s = "{input_size}, {hidden_size}"
+        if "bias" in self.__dict__ and self.bias is not True:
+            s += ", bias={bias}"
+        return s.format(**self.__dict__)
+
+    def _step(self, x: torch.Tensor, hx):
+        """batched step through functional.cell_forward; the TF32 mode follows torch's setting at this call"""
+        weights = [self.weight_ih, self.weight_hh] + ([self.bias_ih, self.bias_hh] if self.bias else [])
+        cfg = CellConfig(mode=self._mode, input_size=self.input_size, hidden_size=self.hidden_size, bias=self.bias,
+                         tf32=tf32_enabled())
+        return cell_forward(x, hx, weights, cfg, type(self).__name__)
+
+
+class GRUCell(_B200CellBase):
+    """``torch.nn.GRUCell`` (gate order r,z,n) on the sm_90a cell kernels."""
+
+    _mode = _lib.GRU
+    _gates = 3
+
+    def forward(self, input: torch.Tensor, hx: Optional[torch.Tensor] = None) -> torch.Tensor:
+        if input.dim() not in (1, 2):
+            raise ValueError(f"GRUCell: Expected input to be 1D or 2D, got {input.dim()}D instead")
+        if hx is not None and hx.dim() not in (1, 2):
+            raise ValueError(f"GRUCell: Expected hidden to be 1D or 2D, got {hx.dim()}D instead")
+        if input.dim() == 2:
+            return self._step(input, hx)
+        return self._step(input.unsqueeze(0), hx.unsqueeze(0) if hx is not None else None).squeeze(0)
+
+
+class LSTMCell(_B200CellBase):
+    """``torch.nn.LSTMCell`` (gate order i,f,g,o) on the sm_90a cell kernels."""
+
+    _mode = _lib.LSTM
+    _gates = 4
+
+    def forward(self, input: torch.Tensor, hx=None):
+        if input.dim() not in (1, 2):
+            raise ValueError(f"LSTMCell: Expected input to be 1D or 2D, got {input.dim()}D instead")
+        if hx is not None:
+            for idx, value in enumerate(hx):
+                if value.dim() not in (1, 2):
+                    raise ValueError(f"LSTMCell: Expected hx[{idx}] to be 1D or 2D, got {value.dim()}D instead")
+        if input.dim() == 2:
+            return self._step(input, hx)
+        hx = (hx[0].unsqueeze(0), hx[1].unsqueeze(0)) if hx is not None else None
+        h, c = self._step(input.unsqueeze(0), hx)
+        return h.squeeze(0), c.squeeze(0)
+
+
 def install() -> None:
-    """Rebind ``torch.nn.GRU`` / ``torch.nn.LSTM`` so unmodified reference code builds the b200rnn modules."""
+    """Rebind ``torch.nn.GRU`` / ``torch.nn.LSTM`` so unmodified reference code builds the b200rnn modules. The cells
+    are left alone: ``torch.nn.GRUCell`` / ``LSTMCell`` stay stock, so host code using them keeps running."""
     nn.GRU = GRU
     nn.LSTM = LSTM
     torch.nn.modules.GRU = GRU
@@ -300,8 +383,15 @@ def uninstall() -> None:
     torch.nn.modules.LSTM = _TORCH_LSTM
 
 
-def from_torch(module: nn.Module) -> _B200RNNBase:
-    """Build the b200rnn twin of a stock ``nn.GRU`` / ``nn.LSTM`` and copy its parameters."""
+def from_torch(module: nn.Module) -> nn.Module:
+    """Build the b200rnn twin of a stock ``nn.GRU`` / ``nn.LSTM`` / ``nn.GRUCell`` / ``nn.LSTMCell`` and copy its
+    parameters."""
+    if isinstance(module, (nn.GRUCell, nn.LSTMCell)):
+        twin = (GRUCell if isinstance(module, nn.GRUCell) else LSTMCell)(module.input_size, module.hidden_size,
+                                                                         bias=module.bias)
+        twin.load_state_dict(module.state_dict())
+        twin.train(module.training)
+        return twin
     if isinstance(module, _TORCH_GRU):
         cls = GRU
     elif isinstance(module, _TORCH_LSTM):

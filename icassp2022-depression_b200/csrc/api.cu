@@ -11,6 +11,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include "cell_kernels.cuh"
 #include "gemm_f32.cuh"
 #include "misc_kernels.cuh"
 #include "rnn_kernels.cuh"
@@ -347,6 +348,105 @@ int run_grad_gemm(const GradGemm& g, const ScratchLayout& sl, float* S, bool tf3
   return tc_gemm_presplit(op[0], op[1], g.M, g.N, g.K, g.C, g.c_rows, nullptr, nullptr, 0, g.accumulate,
                           g.splitk ? S + sl.b_tc_part : nullptr, g.splitk ? sl.b_tc_part_bytes : 0, st, nullptr, 0,
                           tf32);
+}
+
+// ---- one-step cells ---------------------------------------------------------------------------------------------
+struct CellDims {
+  int mode, B, I, H, G;
+  size_t GH;
+  bool save, tf32, accumulate, bias;
+  // shapes whose gradient GEMMs may take the tensor cores (N % 128 == 0, every source row a multiple of 4 floats):
+  // dx / dW_ih (N = I) and dh / dW_hh (N = H)
+  bool tc_x, tc_h;
+};
+
+constexpr int CELL_MAX_BATCH = 1 << 20;
+
+int check_cell_desc(const b200rnn_cell_desc* d, CellDims* o) {
+  if (!d) {
+    set_error("cell: null descriptor");
+    return B200RNN_ERR_INVALID;
+  }
+  if (d->mode != B200RNN_GRU && d->mode != B200RNN_LSTM) {
+    set_error("cell: mode must be B200RNN_GRU or B200RNN_LSTM (got %d)", d->mode);
+    return B200RNN_ERR_INVALID;
+  }
+  constexpr uint32_t known =
+      B200RNN_FLAG_SAVE_FOR_BACKWARD | B200RNN_FLAG_TF32 | B200RNN_FLAG_ACCUMULATE_GRADS | B200RNN_FLAG_NO_BIAS;
+  if (d->flags & ~known) {
+    set_error("cell: unknown flags 0x%x (a cell takes SAVE_FOR_BACKWARD, TF32, ACCUMULATE_GRADS and NO_BIAS)",
+              d->flags & ~known);
+    return B200RNN_ERR_INVALID;
+  }
+  if (d->batch < 0 || d->input_size < 1 || d->hidden_size < 1) {
+    set_error("cell: bad shape: B=%d I=%d H=%d (B >= 0, I >= 1, H >= 1)", d->batch, d->input_size, d->hidden_size);
+    return B200RNN_ERR_INVALID;
+  }
+  const size_t G = d->mode == B200RNN_GRU ? 3 : 4, GH = G * d->hidden_size;
+  const size_t K = (size_t)(d->input_size > d->hidden_size ? d->input_size : d->hidden_size);
+  if (d->batch > CELL_MAX_BATCH || GH * K > 0x7fffffffu || GH * d->batch > 0x7fffffffu ||
+      K * d->batch > 0x7fffffffu) {
+    set_error("cell: shape too large: B=%d I=%d H=%d (B <= %d, every operand below 2^31 elements)", d->batch,
+              d->input_size, d->hidden_size, CELL_MAX_BATCH);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  o->mode = d->mode;
+  o->B = d->batch;
+  o->I = d->input_size;
+  o->H = d->hidden_size;
+  o->G = (int)G;
+  o->GH = GH;
+  o->save = (d->flags & B200RNN_FLAG_SAVE_FOR_BACKWARD) != 0;
+  o->tf32 = (d->flags & B200RNN_FLAG_TF32) != 0;
+  o->accumulate = (d->flags & B200RNN_FLAG_ACCUMULATE_GRADS) != 0;
+  o->bias = (d->flags & B200RNN_FLAG_NO_BIAS) == 0;
+  o->tc_x = o->I % 128 == 0 && GH % 4 == 0;
+  o->tc_h = o->H % 128 == 0;
+  return B200RNN_OK;
+}
+
+// saved state (floats): the activated gates [B][G*H], then GRU W_hn h + b_hn / LSTM c' [B][H], as the sequence path's
+// reserve holds one step
+struct CellSaved {
+  size_t gates, extra, total;
+};
+
+void make_cell_saved(const CellDims& d, CellSaved* s) {
+  s->gates = 0;
+  s->extra = align_up((size_t)d.B * d.GH, ALIGN_F);
+  s->total = s->extra + align_up((size_t)d.B * d.H, ALIGN_F);
+}
+
+// backward scratch (floats): gate gradients, bias partial sums, and the gradient GEMMs' workspaces laid out as the
+// sequence backward's (split-K partials; a TF32 hi/lo split region per tensor-core source)
+struct CellScratch {
+  size_t dgx, dgh, part;
+  size_t tc_dgx, tc_dgh, tc_x, tc_h, tc_wih, tc_whh;
+  ScratchLayout gemm;  // only b_gemm, b_gemm_bytes, b_tc_part, b_tc_part_bytes are used
+  size_t total;
+};
+
+void make_cell_scratch(const CellDims& d, CellScratch* s) {
+  const size_t B = d.B;
+  size_t off = 0;
+  s->dgx = off;  off += align_up(B * d.GH, ALIGN_F);
+  s->dgh = off;  if (d.mode == B200RNN_GRU) off += align_up(B * d.GH, ALIGN_F);
+  s->part = off; off += align_up((size_t)cell_bwd_slices(d.B) * (d.G + 1) * d.H, ALIGN_F);
+  memset(&s->gemm, 0, sizeof(s->gemm));
+  const size_t g0 = gemm_scratch_bytes((int)d.GH, d.I, d.B), g1 = gemm_scratch_bytes((int)d.GH, d.H, d.B);
+  s->gemm.b_gemm = off;
+  s->gemm.b_gemm_bytes = g0 > g1 ? g0 : g1;
+  off += align_up(s->gemm.b_gemm_bytes / sizeof(float) + 1, ALIGN_F);
+  s->tc_dgx = off;  if (d.tc_x || d.tc_h) off += align_up(2 * B * d.GH, ALIGN_F);
+  s->tc_dgh = off;  if (d.tc_h && d.mode == B200RNN_GRU) off += align_up(2 * B * d.GH, ALIGN_F);
+  s->tc_x = off;    if (d.tc_x) off += align_up(2 * B * d.I, ALIGN_F);
+  s->tc_wih = off;  if (d.tc_x) off += align_up(2 * d.GH * d.I, ALIGN_F);
+  s->tc_h = off;    if (d.tc_h) off += align_up(2 * B * d.H, ALIGN_F);
+  s->tc_whh = off;  if (d.tc_h) off += align_up(2 * d.GH * d.H, ALIGN_F);
+  s->gemm.b_tc_part = off;
+  s->gemm.b_tc_part_bytes = (d.tc_x || d.tc_h) ? TC_PART_BYTES : 0;
+  off += align_up(s->gemm.b_tc_part_bytes / sizeof(float), ALIGN_F);
+  s->total = off;
 }
 
 }  // namespace
@@ -1003,6 +1103,186 @@ B200RNN_API int b200rnn_backward(const b200rnn_desc* desc, const float* x, int64
   return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, nullptr, 0.f, dh_n, dc_n, reserve,
                        scratch, dx, dxs_t, dxs_b, dparams, lengths, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr,
                        nullptr, nullptr, stream_);
+}
+
+B200RNN_API int b200rnn_cell_workspace_bytes(const b200rnn_cell_desc* desc, size_t* saved_bytes, size_t* scratch_bytes) {
+  CellDims d;
+  const int rc = check_cell_desc(desc, &d);
+  if (rc) return rc;
+  CellSaved sv;
+  make_cell_saved(d, &sv);
+  CellScratch sc;
+  make_cell_scratch(d, &sc);
+  if (saved_bytes) *saved_bytes = sv.total * sizeof(float);
+  if (scratch_bytes) *scratch_bytes = sc.total * sizeof(float);
+  return B200RNN_OK;
+}
+
+// x_ld / h_ld / c_ld of a cell call: rows must not overlap (a single row may have any stride)
+static bool cell_rows_ok(int B, int64_t ld, int width) { return B <= 1 || ld >= width; }
+
+// params: 4 pointers (weights required, biases NULL exactly when the descriptor says NO_BIAS)
+static int check_cell_params(const CellDims& d, const float* const* params, const char* what) {
+  if (!params || !params[0] || !params[1]) {
+    set_error("%s: null weight pointer", what);
+    return B200RNN_ERR_INVALID;
+  }
+  if ((params[2] != nullptr) != d.bias || (params[3] != nullptr) != d.bias) {
+    set_error("%s: bias pointers must be both set, or both NULL with B200RNN_FLAG_NO_BIAS", what);
+    return B200RNN_ERR_INVALID;
+  }
+  return B200RNN_OK;
+}
+
+B200RNN_API int b200rnn_cell_forward(const b200rnn_cell_desc* desc, const float* x, int64_t x_ld, const float* h,
+                                     int64_t h_ld, const float* c, int64_t c_ld, const float* const* params,
+                                     float* h_out, float* c_out, void* saved, void* stream_) {
+  CellDims d;
+  int rc = check_cell_desc(desc, &d);
+  if (rc) return rc;
+  const bool lstm = d.mode == B200RNN_LSTM;
+  if (!lstm && (c || c_out)) {
+    set_error("cell_forward: a GRU cell has no cell state (c / c_out must be NULL)");
+    return B200RNN_ERR_INVALID;
+  }
+  if (d.B == 0) return B200RNN_OK;
+  if (!x || !h_out || (lstm && !c_out)) {
+    set_error("cell_forward: null pointer argument");
+    return B200RNN_ERR_INVALID;
+  }
+  rc = check_cell_params(d, params, "cell_forward");
+  if (rc) return rc;
+  if (!cell_rows_ok(d.B, x_ld, d.I) || (h && !cell_rows_ok(d.B, h_ld, d.H)) || (c && !cell_rows_ok(d.B, c_ld, d.H))) {
+    set_error("cell_forward: a row stride is smaller than its row (x_ld=%lld h_ld=%lld c_ld=%lld)", (long long)x_ld,
+              (long long)h_ld, (long long)c_ld);
+    return B200RNN_ERR_INVALID;
+  }
+  if (d.save && (!saved || !aligned_to(saved, 256))) {
+    set_error("cell_forward: B200RNN_FLAG_SAVE_FOR_BACKWARD needs a 256-byte aligned saved-state buffer");
+    return B200RNN_ERR_INVALID;
+  }
+  CellSaved sv;
+  make_cell_saved(d, &sv);
+  float* SV = static_cast<float*>(saved);
+  CellFwdParams p;
+  memset(&p, 0, sizeof(p));
+  p.mode = d.mode; p.B = d.B; p.I = d.I; p.H = d.H;
+  p.tf32 = d.tf32 ? 1 : 0;
+  p.x = x; p.x_ld = x_ld;
+  p.h = h; p.h_ld = h_ld;
+  p.c = c; p.c_ld = c_ld;
+  p.w_ih = params[0]; p.w_hh = params[1]; p.b_ih = params[2]; p.b_hh = params[3];
+  p.h_out = h_out; p.c_out = c_out;
+  p.gates = d.save ? SV + sv.gates : nullptr;
+  p.extra = d.save ? SV + sv.extra : nullptr;
+  return launch_cell_fwd(p, static_cast<cudaStream_t>(stream_));
+}
+
+B200RNN_API int b200rnn_cell_backward(const b200rnn_cell_desc* desc, const float* x, int64_t x_ld, const float* h,
+                                      int64_t h_ld, const float* c, int64_t c_ld, const float* const* params,
+                                      const float* dh_out, const float* dc_out, const void* saved, float* dx,
+                                      float* dh, float* dc, float* const* dparams, void* scratch, void* stream_) {
+  CellDims d;
+  int rc = check_cell_desc(desc, &d);
+  if (rc) return rc;
+  const bool lstm = d.mode == B200RNN_LSTM;
+  if (!lstm && (c || dc_out || dc)) {
+    set_error("cell_backward: a GRU cell has no cell state (c / dc_out / dc must be NULL)");
+    return B200RNN_ERR_INVALID;
+  }
+  if (!dparams) {
+    set_error("cell_backward: null pointer argument");
+    return B200RNN_ERR_INVALID;
+  }
+  if (!d.bias && (dparams[2] || dparams[3])) {
+    set_error("cell_backward: bias gradients requested with B200RNN_FLAG_NO_BIAS");
+    return B200RNN_ERR_INVALID;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const size_t GH = d.GH;
+  const size_t nparam[4] = {GH * d.I, GH * d.H, GH, GH};
+  if (d.B == 0) {  // no row: the parameter gradients are zero
+    if (!d.accumulate)
+      for (int i = 0; i < 4; ++i)
+        if (dparams[i]) B200_CUDA_CHECK(cudaMemsetAsync(dparams[i], 0, nparam[i] * sizeof(float), st));
+    return B200RNN_OK;
+  }
+  if (!x || !saved || !scratch) {
+    set_error("cell_backward: null pointer argument");
+    return B200RNN_ERR_INVALID;
+  }
+  rc = check_cell_params(d, params, "cell_backward");
+  if (rc) return rc;
+  if (!cell_rows_ok(d.B, x_ld, d.I) || (h && !cell_rows_ok(d.B, h_ld, d.H)) || (c && !cell_rows_ok(d.B, c_ld, d.H))) {
+    set_error("cell_backward: a row stride is smaller than its row (x_ld=%lld h_ld=%lld c_ld=%lld)", (long long)x_ld,
+              (long long)h_ld, (long long)c_ld);
+    return B200RNN_ERR_INVALID;
+  }
+  if (!aligned_to(saved, 256) || !aligned_to(scratch, 256)) {
+    set_error("cell_backward: saved / scratch must be 256-byte aligned");
+    return B200RNN_ERR_INVALID;
+  }
+  CellSaved sv;
+  make_cell_saved(d, &sv);
+  CellScratch sc;
+  make_cell_scratch(d, &sc);
+  const float* SV = static_cast<const float*>(saved);
+  float* S = static_cast<float*>(scratch);
+  const int accumulate = d.accumulate ? 1 : 0;
+  const int B = d.B, I = d.I, H = d.H, G = (int)GH;
+
+  // gate gradients; GRU: dh = z * dh' + dG_h W_hh, the direct term goes to dh first; LSTM: dc is final here
+  CellBwdParams bp;
+  memset(&bp, 0, sizeof(bp));
+  bp.mode = d.mode; bp.B = B; bp.H = H;
+  bp.gates = SV + sv.gates; bp.extra = SV + sv.extra;
+  bp.h = h; bp.h_ld = h_ld;
+  bp.c = c; bp.c_ld = c_ld;
+  bp.dh_out = dh_out; bp.dc_out = dc_out;
+  bp.dg_x = S + sc.dgx;
+  bp.dg_h = lstm ? nullptr : S + sc.dgh;
+  bp.direct = lstm ? dc : dh;
+  bp.part = S + sc.part;
+  rc = launch_cell_bwd(bp, st);
+  if (rc) return rc;
+  if (dparams[2] || dparams[3]) {
+    rc = launch_bias_reduce(bp.part, cell_bwd_slices(B), d.mode, H, dparams[2], dparams[3], accumulate, st);
+    if (rc) return rc;
+  }
+
+  // the gradient GEMMs, as the sequence backward runs them (run_grad_gemm: tensor cores where eligible, else FFMA)
+  const bool tc_x = d.tc_x && tc_available(), tc_h = d.tc_h && tc_available();
+  GradSrc DGX{S + sc.dgx, simple_rows(G), B, G, S + sc.tc_dgx, false};
+  GradSrc DGH_gru{S + sc.dgh, simple_rows(G), B, G, S + sc.tc_dgh, false};
+  GradSrc& DGH = lstm ? DGX : DGH_gru;  // the LSTM's h-part gate gradients are its x-part ones
+  GradSrc X{x, simple_rows(x_ld), B, I, S + sc.tc_x, false};
+  GradSrc Hs{h, simple_rows(h_ld), B, H, S + sc.tc_h, false};
+  GradSrc WIH{params[0], simple_rows(I), G, I, S + sc.tc_wih, false};
+  GradSrc WHH{params[1], simple_rows(H), G, H, S + sc.tc_whh, false};
+  const ScratchLayout& sl = sc.gemm;
+  if (dparams[0]) {  // dW_ih [GH, I] = dG_x^T x
+    rc = run_grad_gemm({{&DGX, 0, false}, {&X, 0, false}, G, I, B, dparams[0], simple_rows(I), accumulate, true,
+                        tc_x && aligned_to(dparams[0], 16), "cell dW_ih"}, sl, S, d.tf32, st);
+    if (rc) return rc;
+  }
+  if (dparams[1] && h) {  // dW_hh [GH, H] = dG_h^T h
+    rc = run_grad_gemm({{&DGH, 0, false}, {&Hs, 0, false}, G, H, B, dparams[1], simple_rows(H), accumulate, true,
+                        tc_h && aligned_to(dparams[1], 16), "cell dW_hh"}, sl, S, d.tf32, st);
+    if (rc) return rc;
+  } else if (dparams[1] && !accumulate) {  // h = 0: nothing reaches W_hh
+    B200_CUDA_CHECK(cudaMemsetAsync(dparams[1], 0, nparam[1] * sizeof(float), st));
+  }
+  if (dx) {  // dx [B, I] = dG_x W_ih
+    rc = run_grad_gemm({{&DGX, 0, true}, {&WIH, 0, false}, B, I, G, dx, simple_rows(I), 0, false,
+                        tc_x && aligned_to(dx, 16), "cell dx"}, sl, S, d.tf32, st);
+    if (rc) return rc;
+  }
+  if (dh) {  // dh [B, H] (+)= dG_h W_hh
+    rc = run_grad_gemm({{&DGH, 0, true}, {&WHH, 0, false}, B, H, G, dh, simple_rows(H), lstm ? 0 : 1, false,
+                        tc_h && aligned_to(dh, 16), "cell dh"}, sl, S, d.tf32, st);
+    if (rc) return rc;
+  }
+  return B200RNN_OK;
 }
 
 B200RNN_API int b200rnn_gemm_f32(int M, int N, int K, const float* A, int64_t lda, int a_kcontig, const float* B,

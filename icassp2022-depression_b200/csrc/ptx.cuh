@@ -71,6 +71,26 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
       : "memory");
 }
 
+// ---- cp.async global -> shared (SASS: LDGSTS) -----------------------------------------------------
+// Copies src_bytes (<= the copy size) from src and zero-fills the rest of dst; src_bytes = 0 reads nothing. 16-byte
+// copies need 16-byte aligned dst and src.
+__device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem),
+               "r"(src_bytes)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async4(void* dst_smem, const void* src_gmem, uint32_t src_bytes) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem),
+               "r"(src_bytes)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
 // named CTA barrier `id` (1..15; 0 is __syncthreads) over `nthreads` threads, a multiple of 32
 __device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -35,6 +35,7 @@
 #include "profile.cuh"
 #include "ptx.cuh"
 #include "rec_h16_layout.cuh"
+#include "rnn_cell.cuh"
 #include "rnn_core.cuh"
 #include "rnn_kernels.cuh"
 
@@ -144,37 +145,6 @@ struct ExchangeBars {
   // the slice of source `src` has landed in buffer b = buf(s), phase par = parity(s) (computed once per step)
   __device__ __forceinline__ void wait(int b, int src, uint32_t par) const { ptx::mbar_wait(bar(b, src), par); }
 };
-
-// The LSTM cell, forward: gate pre-activations gi + pre -> activated gates, c_t and o * tanh(c_t)
-struct LstmStep {
-  float i, f, g, o, c, h;
-};
-
-__device__ __forceinline__ LstmStep lstm_cell_fwd(const float (&gi)[4], const float (&pre)[4], float c) {
-  LstmStep s;
-  s.i = sigmoid_f(gi[0] + pre[0]);
-  s.f = sigmoid_f(gi[1] + pre[1]);
-  s.g = tanh_f(gi[2] + pre[2]);
-  s.o = sigmoid_f(gi[3] + pre[3]);
-  s.c = fmaf(s.f, c, s.i * s.g);  // spelled out: which product is fused must not be left to the compiler
-  s.h = s.o * tanh_f(s.c);
-  return s;
-}
-
-// The LSTM cell, backward: from the saved gates sv = (i, f, g, o), c_t, c_{t-1}, the gradient dh of o * tanh(c_t) and
-// the carried dc, the gate gradients dg; returns the dc carried to step t - 1
-__device__ __forceinline__ float lstm_cell_bwd(const float (&sv)[4], float c_t, float c_prev, float dh, float dc_carry,
-                                               float (&dg)[4]) {
-  const float ig = sv[0], fg = sv[1], gg = sv[2], og = sv[3];
-  const float tc = tanh_f(c_t);
-  const float dout = dh * tc * og * (1.f - og);
-  const float dc = dc_carry + dh * og * (1.f - tc * tc);
-  dg[0] = dc * gg * ig * (1.f - ig);
-  dg[1] = dc * c_prev * fg * (1.f - fg);
-  dg[2] = dc * ig * (1.f - gg * gg);
-  dg[3] = dout;
-  return dc * fg;
-}
 
 // All-gather `val` (owned by lane (unit, batch) of every warp) into vec[b][col0 + unit] of all C CTAs:
 // 4 shuffles gather 4 consecutive units, one 16-byte store per (destination, chunk).
@@ -294,15 +264,12 @@ struct FwdCell {
   __device__ __forceinline__ float update(int t, const float (&pre)[G]) {
     float hnew, s[G], sx;
     if constexpr (MODE == B200RNN_GRU) {
-      const float r = sigmoid_f(gi[0] + pre[0]);
-      const float z = sigmoid_f(gi[1] + pre[1]);
-      const float hn = pre[2] + bhn;
-      const float n = tanh_f(gi[2] + r * hn);
-      hnew = n + z * (h - n);
+      const GruStep st = gru_cell_fwd(gi, pre, bhn, h);
+      hnew = st.h;
       if constexpr (VL) {
         if (t >= len) hnew = h;
       }
-      s[0] = r; s[1] = z; s[2] = n; sx = hn;
+      s[0] = st.r; s[1] = st.z; s[2] = st.n; sx = st.hn;
     } else {
       const LstmStep st = lstm_cell_fwd(gi, pre, c);
       float cnew = st.c;
@@ -1118,13 +1085,7 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     }
     float dg[G], direct, dhn = 0.f;
     if constexpr (MODE == B200RNN_GRU) {
-      const float r = sv[0], z = sv[1], n = sv[2], hn = sx;
-      const float dn = dh * (1.f - z) * (1.f - n * n);
-      const float dz = dh * (hp - n) * z * (1.f - z);
-      const float dr = dn * hn * r * (1.f - r);
-      dhn = dn * r;
-      dg[0] = dr; dg[1] = dz; dg[2] = dn;
-      direct = dh * z;
+      direct = gru_cell_bwd(sv, sx, hp, dh, dg, dhn);
     } else {
       const float dc_next = lstm_cell_bwd(sv, sx, hp, dh, dc_carry, dg);
       direct = 0.f;

@@ -246,6 +246,55 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
                                        float* dln_beta, void* stream /* cudaStream_t */);
 
 /*
+ * One-step cells: torch.nn.GRUCell / torch.nn.LSTMCell (rnn.py), any input_size and hidden_size, with or without
+ * biases. A forward is one launch that streams the weights from global memory (L2 after the first call); nothing is
+ * kept on chip between calls. Stream-ordered, no allocation, capturable in a CUDA graph, like the rest of the ABI.
+ */
+#define B200RNN_FLAG_NO_BIAS 32u /* cells only: bias=False, the bias pointers are NULL (and dbias skipped) */
+
+typedef struct b200rnn_cell_desc {
+  int32_t mode;        /* B200RNN_GRU (gate order r,z,n) or B200RNN_LSTM (gate order i,f,g,o) */
+  int32_t batch;       /* B (0 allowed)                                                       */
+  int32_t input_size;  /* I >= 1                                                              */
+  int32_t hidden_size; /* H >= 1                                                              */
+  uint32_t flags;      /* B200RNN_FLAG_SAVE_FOR_BACKWARD, B200RNN_FLAG_TF32, B200RNN_FLAG_ACCUMULATE_GRADS,
+                          B200RNN_FLAG_NO_BIAS; nothing else                                  */
+} b200rnn_cell_desc;
+
+/* Validates the descriptor (message via b200rnn_last_error) and returns the bytes of
+ *   saved   : written by a forward with B200RNN_FLAG_SAVE_FOR_BACKWARD, read by the backward (256-byte aligned)
+ *   scratch : the backward's transient buffer (256-byte aligned); the forward takes none */
+B200RNN_API int b200rnn_cell_workspace_bytes(const b200rnn_cell_desc* desc, size_t* saved_bytes, size_t* scratch_bytes);
+
+/*
+ * Forward of GRUCell / LSTMCell: h' = cell(x W_ih^T + b_ih, h W_hh^T + b_hh) (and c'), one kernel launch.
+ *   x       [B, I], row b at x + b * x_ld (feature stride 1, any alignment)
+ *   h, c    [B, H] at h + b * h_ld / c + b * c_ld, or NULL = zeros; c is LSTM only
+ *   params  4 pointers in nn order: weight_ih [G*H, I], weight_hh [G*H, H] (contiguous, any alignment), bias_ih [G*H],
+ *           bias_hh [G*H] (both NULL with B200RNN_FLAG_NO_BIAS)
+ *   h_out   [B, H] contiguous; c_out [B, H] contiguous, LSTM only (NULL for the GRU)
+ *   saved   required with B200RNN_FLAG_SAVE_FOR_BACKWARD (else ignored): the activated gates and GRU W_hn h + b_hn /
+ *           LSTM c', in the layout of the sequence path's reserve for one step
+ * The output buffers must not overlap the inputs.
+ */
+B200RNN_API int b200rnn_cell_forward(const b200rnn_cell_desc* desc, const float* x, int64_t x_ld, const float* h,
+                                     int64_t h_ld, const float* c, int64_t c_ld, const float* const* params,
+                                     float* h_out, float* c_out, void* saved, void* stream /* cudaStream_t */);
+
+/*
+ * Backward of b200rnn_cell_forward. desc, x, h, c and params as given to that forward (its saved state in `saved`).
+ *   dh_out, dc_out  [B, H] contiguous gradients w.r.t. h' / c' (dc_out LSTM only), or NULL = zeros
+ *   dx [B, I], dh [B, H], dc [B, H] (LSTM only)  contiguous, written (never accumulated), or NULL to skip
+ *   dparams         4 pointers shaped like params, each NULL to skip; written or accumulated per
+ *                   B200RNN_FLAG_ACCUMULATE_GRADS (B = 0: written as zeros, or left as they are)
+ * One elementwise launch, then the gradient GEMMs of the sequence backward (tensor cores or FFMA, deterministic).
+ */
+B200RNN_API int b200rnn_cell_backward(const b200rnn_cell_desc* desc, const float* x, int64_t x_ld, const float* h,
+                                      int64_t h_ld, const float* c, int64_t c_ld, const float* const* params,
+                                      const float* dh_out, const float* dc_out, const void* saved, float* dx, float* dh,
+                                      float* dc, float* const* dparams, void* scratch, void* stream /* cudaStream_t */);
+
+/*
  * Dense helper used by the path (time-parallel input projection, wgrad, dgrad):
  *   C[m,n] (+)= sum_k A(m,k) * B(k,n) + bias[n]
  * exposed so the parity tests can pin the GEMM on its own.

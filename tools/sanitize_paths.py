@@ -3,6 +3,7 @@
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py rnn   # recurrence only
 The GRU H=256 layer also runs at B = 96, which needs the 4-row clusters (bs4: the 2-row ones do not all fit at once).
+    compute-sanitizer --tool memcheck python tools/sanitize_paths.py cells # GRUCell / LSTMCell forward + backward only
 """
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -11,6 +12,21 @@ import torch, b200rnn
 from torch.nn.utils.rnn import pack_padded_sequence
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
+if sys.argv[1:] == ["cells"]:
+    # K and batch tails, unaligned rows (odd offsets into larger buffers), no bias, no state, both contractions
+    for kind, I, H, B, bias in (("gru", 3, 5, 7, True), ("lstm", 257, 129, 9, False), ("gru", 256, 256, 130, False),
+                                ("lstm", 40, 100, 33, True)):
+        cell = (b200rnn.GRUCell if kind == "gru" else b200rnn.LSTMCell)(I, H, bias=bias).to(dev)
+        x = torch.randn(B * I + 1, device=dev)[1:].view(B, I).requires_grad_(True)
+        h = torch.randn(B * H + 1, device=dev)[1:].view(B, H).requires_grad_(True)
+        for prec in ("ieee", "tf32"):
+            torch.backends.cuda.matmul.fp32_precision = prec
+            for hx in (None, h if kind == "gru" else (h, torch.randn(B, H, device=dev))):
+                out = cell(x, hx)
+                (out if kind == "gru" else out[0] + out[1]).sum().backward()
+        torch.cuda.synchronize()
+        print(kind, I, H, B, "ok", flush=True)
+    sys.exit(0)
 for kind, I, H, L, bi in (("gru", 64, 256, 2, False), ("lstm", 64, 128, 2, True), ("gru", 32, 128, 1, True), ("lstm", 32, 256, 1, False)):
     cls = b200rnn.GRU if kind == "gru" else b200rnn.LSTM
     m = cls(I, H, num_layers=L, bidirectional=bi, batch_first=True, dropout=0.3 if L > 1 else 0.0).to(dev).train()
