@@ -13,6 +13,7 @@
 
 #include "cell_kernels.cuh"
 #include "gemm_f32.cuh"
+#include "gemm_h16_layout.cuh"
 #include "misc_kernels.cuh"
 #include "rnn_kernels.cuh"
 
@@ -236,24 +237,22 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
   s->f_total = s->b_total = s->order + align_up((size_t)d.B, ALIGN_F);
 }
 
-// ---- weight cache layout (floats): per (layer, direction) the TF32 hi then lo split of weight_ih [G*H, I_l] -------
+// ---- weight cache layout (floats): per (layer, direction) the TF32 hi then lo split of weight_ih [G*H, I_l], then its
+// fp16-pair split (gemm_h16_layout.cuh, g16::wcache_layout: the byte offsets, all multiples of 256)
 struct WCacheLayout {
-  size_t hi[8][2], lo[8][2];
+  size_t hi[8][2], lo[8][2], h16[8][2];
   size_t total;
 };
 
 void make_wcache(const Dims& d, WCacheLayout* w) {
-  size_t off = 0;
-  for (int l = 0; l < d.L && l < 8; ++l) {
-    const size_t Il = l == 0 ? (size_t)d.I : d.DH;
+  const g16::WCache b = g16::wcache_layout(d.L, d.D, d.I, (int)d.DH, (int)d.GH);
+  for (int l = 0; l < d.L && l < 8; ++l)
     for (int k = 0; k < d.D; ++k) {
-      w->hi[l][k] = off;
-      off += align_up(d.GH * Il, ALIGN_F);
-      w->lo[l][k] = off;
-      off += align_up(d.GH * Il, ALIGN_F);
+      w->hi[l][k] = b.hi[l][k] / sizeof(float);
+      w->lo[l][k] = b.lo[l][k] / sizeof(float);
+      w->h16[l][k] = b.h16[l][k] / sizeof(float);
     }
-  }
-  w->total = off;
+  w->total = b.total / sizeof(float);
 }
 
 inline bool aligned_to(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
@@ -677,9 +676,13 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         g.tc_ws_bytes = sl.f_tc_bytes;
         g.tc_a_f32 = 1;
         g.tc_tf32 = tf32 ? 1 : 0;
+        // the no-grad forward of b200rnn_forward_fused in default precision: fp16 pairs (the rule of the fp16-pair
+        // recurrence, RecFwdParams::shell_nograd)
+        g.tc_h16 = rp.shell_nograd && !tf32 && g16::shape_ok((int)d.GH, Il) ? 1 : 0;
         if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders); TF32 reads only hi
           g.tc_b_hi = WC + wl.hi[l][k];
           g.tc_b_lo = tf32 ? nullptr : WC + wl.lo[l][k];
+          if (g.tc_h16) g.tc_b_h16 = WC + wl.h16[l][k];
         }
         if (stream_xproj && gemm_tc_eligible(g, g.tc_ws_bytes)) {
           g.tc_ready = ready;
@@ -836,6 +839,10 @@ B200RNN_API int b200rnn_prepare_weights(const b200rnn_desc* desc, const float* c
       if (Il % 4 != 0) continue;  // such a layer takes the FFMA projection, which reads the fp32 weights directly
       rc = tc_split(w_ih, simple_rows(Il), (int)d.GH, Il, WC + wl.hi[l][k], WC + wl.lo[l][k], st);
       if (rc) return rc;
+      if (g16::shape_ok((int)d.GH, Il)) {  // the same split the uncached no-grad forward makes per call
+        rc = tc_split_w16(w_ih, simple_rows(Il), (int)d.GH, Il, WC + wl.h16[l][k], st);
+        if (rc) return rc;
+      }
     }
   }
   return B200RNN_OK;
@@ -1324,6 +1331,29 @@ B200RNN_API int b200rnn_debug_gemm_f32a(int M, int N, int K, const float* A, int
   g.tc_stream_clusters = stream_clusters;
   if (!gemm_tc_eligible(g, scratch_bytes) || !tc_a_f32_in_place(A, g.a_rows, M, K)) {
     set_error("debug_gemm_f32a: problem not eligible for the fp32-A tensor-core path");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  return launch_gemm_tc(g, scratch, scratch_bytes, static_cast<cudaStream_t>(stream_));
+}
+
+/* test only (not declared in the public header): the no-grad forward's fp16-pair input projection, arguments as
+   b200rnn_debug_gemm_f32a (W split into fp16 pairs in `scratch` per call); N % 128 == 0 and K % 64 == 0 */
+B200RNN_API int b200rnn_debug_gemm_f16a(int M, int N, int K, const float* A, int64_t a_st, int64_t a_sb, int a_batch,
+                                        const float* W, float* C, const float* bias, int* ready, int stream_clusters,
+                                        void* scratch, size_t scratch_bytes, void* stream_) {
+  GemmParams g;
+  memset(&g, 0, sizeof(g));
+  g.A = A; g.a_rows = a_batch > 0 ? tb_rows(a_st, a_sb, a_batch) : simple_rows(a_st); g.a_kcontig = 1;
+  g.B = W; g.b_rows = simple_rows(K); g.b_kcontig = 1;
+  g.C = C; g.c_rows = simple_rows(N);
+  g.M = M; g.N = N; g.K = K;
+  g.bias1 = bias;
+  g.tc_a_f32 = 1;
+  g.tc_h16 = 1;
+  g.tc_ready = ready;
+  g.tc_stream_clusters = stream_clusters;
+  if (!g16::shape_ok(N, K) || !gemm_tc_eligible(g, scratch_bytes) || !tc_a_f32_in_place(A, g.a_rows, M, K)) {
+    set_error("debug_gemm_f16a: problem not eligible for the fp16-pair tensor-core path");
     return B200RNN_ERR_UNSUPPORTED;
   }
   return launch_gemm_tc(g, scratch, scratch_bytes, static_cast<cudaStream_t>(stream_));

@@ -36,6 +36,11 @@ struct GemmParams {
   // tensor-core path only: single-pass TF32 (one MMA per k-step on operands rounded to TF32; B200RNN_FLAG_TF32)
   // instead of 3xTF32. Only tc_b_hi of a presplit weight is read, and a per-call split writes hi only.
   int tc_tf32;
+  // tensor-core fp32-A path only: fp16 pairs (gemm_f16x3_kernel, the no-grad forward of b200rnn_forward_fused) when the
+  // shape allows (g16::shape_ok), else 3xTF32. tc_b_h16 (optional): W already split into fp16 pairs
+  // (gemm_h16_layout.cuh, b200rnn_prepare_weights); else the call splits W into its workspace.
+  int tc_h16;
+  const void* tc_b_h16;
 };
 
 // where launch_gemm_tc puts the split A operand inside its workspace (tc_a_hi: also room for a dense fp32 [M][K] A)
@@ -89,6 +94,13 @@ int tc_gemm_presplit(const TcOperand& A, const TcOperand& B, int M, int N, int K
 int tc_gemm_f32a(const float* A, const RowMap& a_rows, const TcOperand& B, int M, int N, int K, float* C,
                  const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
                  int* ready = nullptr, int stream_clusters = 0, bool tf32 = false);
+// W[N][K] (rows through `rows`) -> fp16 pairs and row exponents at w16 (256-byte aligned, g16::w16_layout(N, K) bytes)
+int tc_split_w16(const float* W, const RowMap& rows, int N, int K, void* w16, cudaStream_t stream);
+// C = A[M,K] * W[N,K]^T + biases, A fp32 read in place (tc_a_f32_in_place) and split into fp16 pairs on chip, W the
+// fp16 pairs at w16 (tc_split_w16); N % 128 == 0, K % 64 == 0. ready / stream_clusters as above.
+int tc_gemm_f16a(const float* A, const RowMap& a_rows, const void* w16, int M, int N, int K, float* C,
+                 const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
+                 int* ready = nullptr, int stream_clusters = 0);
 // C(m,n) (+)= sum_z partial[z][m][n] (+ biases), fixed order (deterministic)
 int launch_splitk_reduce(const float* partial, int splitk, int M, int N, float* C, const RowMap& c_rows,
                          const float* bias1, const float* bias2, int bias2_n, int accumulate, cudaStream_t stream);

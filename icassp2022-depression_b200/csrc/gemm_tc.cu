@@ -35,13 +35,16 @@
 // written nor loaded (a stage carries 32 KB instead of 48 KB) and a k-block is 4 MMAs; the round-to-nearest flush after
 // every k-block, the streamed publication and the epilogue are those of the 3xTF32 kernel.
 #include <cuda.h>  // CUtensorMap types only; the encoder is fetched through cudaGetDriverEntryPoint
+#include <cuda_fp16.h>
 #include <mutex>
 #include <stdlib.h>
 #include <string.h>
 
 #include "gemm_f32.cuh"
+#include "gemm_h16_layout.cuh"
 #include "profile.cuh"
 #include "ptx.cuh"
+#include "rec_h16_layout.cuh"
 
 namespace b200rnn {
 
@@ -124,6 +127,23 @@ __device__ __forceinline__ void wgmma_tf32_m64n128k8_ra(float (&d)[64], const ui
         B200_ACC8(56)
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
+// D[64x128] (+)= A[64x16] * B[128x16]^T in fp16 with fp32 accumulation, A from registers: a[r] = f16x2 of
+// A(g + 8 (r & 1), 2t + 8 (r >> 1) + {0, 1}) of the warp's 16 rows (low half first), B K-major from shared memory
+__device__ __forceinline__ void wgmma_f16_m64n128k16_ra(float (&d)[64], const uint32_t* a, uint64_t bdesc,
+                                                        int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : B200_ACC8(0), B200_ACC8(8), B200_ACC8(16), B200_ACC8(24), B200_ACC8(32), B200_ACC8(40), B200_ACC8(48),
+        B200_ACC8(56)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
 #undef B200_ACC8
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -153,7 +173,12 @@ struct TcArgs {
   int a_f32;        // A is fp32 (map_a_hi, 3-D), split in registers by the consumers; W K-major presplit
   int a_inner;      // fp32 A: rows per outer index of the 3-D map (tile m0 sits at (m0 % a_inner, m0 / a_inner))
   int tf32;         // single-pass TF32: the lo operands are absent (host side only: selects the kernel instantiation)
+  const int* w_exp; // fp16 pairs: e_n of every W row (gemm_h16_layout.cuh), the epilogue scales column n by 2^-e_n
+  int f16;          // fp16 pairs (gemm_f16x3_kernel; host side only)
 };
+
+// the arithmetic of one instantiation: 3xTF32, single-pass TF32, or fp16 (hi, lo) pairs (fp32 A only)
+enum TcMath { TC_3XTF32, TC_TF32, TC_F16X3 };
 
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64K registers of the SM
 
@@ -195,11 +220,18 @@ __device__ __forceinline__ void load_mn_tile(unsigned char* tile, const float* _
 // the default register budget, so that instantiation has no setmaxnreg; in the K-major one (every operand by TMA, one
 // thread issues) the producer gives registers to the consumers, whose fp32-A path holds the running sum, the wgmma
 // accumulator and two A fragments (4 x 64 registers).
-template <bool MN, bool TF32>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-    gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                       const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-                       const TcArgs args) {
+// fp16 pairs (MATH = TC_F16X3, gemm_f16x3_kernel; fp32 A only): a k-block is 64 k (KB), A arrives as two boxes of 32
+// (ring slots 0 and 1), W as fp16 hi / lo tiles of 128 rows x 128 bytes (slots 2 and 3) with their row exponents in
+// args.w_exp (gemm_h16_layout.cuh). Each consumer scales its rows of the k-block's A by 2^e_m (h16::scale_exp of the
+// row's max |a| over the k-block), splits them into fp16 hi / lo in registers and runs lo*hi, hi*lo, hi*hi as
+// wgmma.m64n128k16 (12 per k-block); the drain unscales with total = fma(acc, 2^-e_m, total), the epilogue multiplies
+// column n by 2^-e_n before the biases.
+template <bool MN, int MATH>
+__device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const CUtensorMap& map_a_lo,
+                                             const CUtensorMap& map_b_hi, const CUtensorMap& map_b_lo,
+                                             const TcArgs args) {
+  constexpr bool TF32 = MATH == TC_TF32, F16 = MATH == TC_F16X3;
+  constexpr int KB = F16 ? g16::BK : BK;  // k per ring stage
   extern __shared__ unsigned char smem_raw[];
   // aligned by offset so that the compiler keeps the shared state space (LDS/STS instead of generic LD/ST)
   unsigned char* base = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -209,7 +241,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   // canonical warp index: the shuffle makes it warp-uniform for the compiler, so the single-thread TMA issue stays on
   // the uniform datapath (no per-instruction R2UR broadcast loop around UTMALDG)
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
-  const int nkb_total = (args.K + BK - 1) / BK;  // the K tail reads as zero
+  const int nkb_total = (args.K + KB - 1) / KB;  // the K tail reads as zero
   const int ntiles = args.tiles_m * args.tiles_n;
   const int nitems = ntiles * args.splitk;
   if (args.ready) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -234,7 +266,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   if (warp < 4) {
     if constexpr (!MN) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
     const int t = threadIdx.x;
-    if (!MN && args.a_f32) {  // one thread issues the fp32 A tile and the W tiles; the consumers split A
+    if (F16 || (!MN && args.a_f32)) {  // one thread issues the fp32 A tile and the W tiles; the consumers split A
       if (warp == 0) {
         int it = 0;  // running k-block counter across items (ring position)
         for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
@@ -244,11 +276,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
             const int s = it % STAGES;
             ptx::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
             unsigned char* st = base + s * STAGE_BYTES;
-            if (ptx::elect_one_sync()) {  // the A_lo slot stays unused: the consumers split A in registers
-              ptx::mbar_arrive_expect_tx(&full[s], (TF32 ? 2u : 3u) * TILE_BYTES);
-              tma_load_3d(st + 0 * TILE_BYTES, &map_a_hi, kb * BK, m0 % args.a_inner, m0 / args.a_inner, &full[s]);
-              tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * BK, n0, &full[s]);
-              if (!TF32) tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * BK, n0, &full[s]);
+            if (ptx::elect_one_sync()) {  // 3xTF32 / TF32: the A_lo slot stays unused (A is split in registers);
+                                          // fp16 pairs: it holds the second 32 k of A
+              ptx::mbar_arrive_expect_tx(&full[s], (F16 ? 4u : TF32 ? 2u : 3u) * TILE_BYTES);
+              tma_load_3d(st + 0 * TILE_BYTES, &map_a_hi, kb * KB, m0 % args.a_inner, m0 / args.a_inner, &full[s]);
+              if (F16)
+                tma_load_3d(st + 1 * TILE_BYTES, &map_a_hi, kb * KB + BK, m0 % args.a_inner, m0 / args.a_inner,
+                            &full[s]);
+              tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * KB, n0, &full[s]);
+              if (!TF32) tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * KB, n0, &full[s]);
             }
             __syncwarp();
           }
@@ -375,6 +411,75 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       }
       wgmma_commit();
     };
+    // fp16 pairs: this thread's A fragment of the 64 k of ring position `pos`, rows g and g + 8, k = 16 s + 8 j + 2 tq
+    // + {0, 1} (float2 loads, conflict-free under the swizzle). Each row is scaled by 2^e, e = h16::scale_exp of its
+    // max |a| over the k-block (quad max: the 4 lanes of a row hold its 64 k), and split; fa[8 s + r] = hi, fa[8 s + 4 +
+    // r] = lo of register r = h + 2 j of k-step s; sc[h] = 2^-e of row g + 8 h
+    const uint32_t a_row16 = (uint32_t)(wg * 64 + wq * 16 + g) * 128u + (tq & 1) * 8u;
+    auto load_a16 = [&](uint32_t (&fa)[32], float (&sc)[2], int pos) {
+      ptx::mbar_wait(&full[pos % STAGES], (pos / STAGES) & 1);
+      const unsigned char* at = base + (pos % STAGES) * STAGE_BYTES + a_row16;
+      float x[2][16];  // [h][4 s + 2 j + e]
+#pragma unroll
+      for (int s4 = 0; s4 < 4; ++s4)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const float2 v = *reinterpret_cast<const float2*>(
+                at + (s4 >> 1) * TILE_BYTES + h * 1024 + (((4 * (s4 & 1) + 2 * j + (tq >> 1)) ^ g) << 4));
+            x[h][4 * s4 + 2 * j] = v.x;
+            x[h][4 * s4 + 2 * j + 1] = v.y;
+          }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float m = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) m = fmaxf(m, fabsf(x[h][i]));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        const int e = g16::scale_exp_bits(m);
+        const float up = g16::exp2i(e);
+        sc[h] = g16::exp2i(-e);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) x[h][i] *= up;
+      }
+#pragma unroll
+      for (int s4 = 0; s4 < 4; ++s4)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float x0 = x[h][4 * s4 + 2 * j], x1 = x[h][4 * s4 + 2 * j + 1];
+            const __half2 hi = __floats2half2_rn(x0, x1);
+            const __half2 lo = __floats2half2_rn(x0 - __low2float(hi), x1 - __high2float(hi));
+            fa[8 * s4 + h + 2 * j] = *reinterpret_cast<const uint32_t*>(&hi);
+            fa[8 * s4 + 4 + h + 2 * j] = *reinterpret_cast<const uint32_t*>(&lo);
+          }
+    };
+    // the 12 fp16 MMAs of a k-block: per k-step of 16 lo*hi, hi*lo, hi*hi, as the 3xTF32 k-block orders them
+    auto issue_ra16 = [&](float (&acc)[64], const uint32_t (&fa)[32], int pos) {
+      const uint32_t st = ptx::smem_u32(base + (pos % STAGES) * STAGE_BYTES);
+      const uint64_t b_hi = make_kmajor_sw128_desc(st + 2 * TILE_BYTES);
+      const uint64_t b_lo = make_kmajor_sw128_desc(st + 3 * TILE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < g16::BK / 16; ++k) {
+        const uint64_t adv = (uint64_t)(k * (32 >> 4));  // K step of 16 f16 = 32 bytes inside the swizzle atom
+        wgmma_f16_m64n128k16_ra(acc, &fa[8 * k + 4], b_hi + adv, k != 0);
+        wgmma_f16_m64n128k16_ra(acc, &fa[8 * k], b_lo + adv, 1);
+        wgmma_f16_m64n128k16_ra(acc, &fa[8 * k], b_hi + adv, 1);
+      }
+      wgmma_commit();
+    };
+    // fp16 pairs: as drain, the k-block's sum unscaled by its rows' 2^-e_m in the same rounding
+    auto drain16 = [&](float (&total)[64], float (&acc)[64], const float (&sc)[2], int pos) {
+      reg_fence(acc);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&empty[pos % STAGES]);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) total[i] = fmaf(acc[i], sc[(i >> 1) & 1], total[i]);
+    };
     int it = 0;
     for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       const int tile = item % ntiles, ks = item / ntiles;
@@ -385,31 +490,56 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 #pragma unroll
       for (int i = 0; i < 64; ++i) total[i] = 0.f;
       float acc[64];
-      if (!MN && args.a_f32) {
+      if (F16 || (!MN && args.a_f32)) {
         // A from registers: the k-block's fp32 fragment is loaded and split here; the next k-block's is loaded while
         // the current MMAs run. Fragments alternate between fa0 and fa1; the loop body is unconditional and the tail
         // peeled, so no branch merges registers a wgmma in flight reads.
         uint32_t fa0[32], fa1[32];
-        load_a(fa0, it);
-        int kb = 0;
-        for (; kb + 2 < nkb; kb += 2) {
+        if constexpr (F16) {  // the same schedule; each fragment carries its rows' unscales
+          float sc0[2], sc1[2];
+          load_a16(fa0, sc0, it);
+          int kb = 0;
+          for (; kb + 2 < nkb; kb += 2) {
+            issue_ra16(acc, fa0, it + kb);
+            load_a16(fa1, sc1, it + kb + 1);
+            wgmma_wait0();
+            drain16(total, acc, sc0, it + kb);
+            issue_ra16(acc, fa1, it + kb + 1);
+            load_a16(fa0, sc0, it + kb + 2);
+            wgmma_wait0();
+            drain16(total, acc, sc1, it + kb + 1);
+          }
+          issue_ra16(acc, fa0, it + kb);
+          if (kb + 1 < nkb) load_a16(fa1, sc1, it + kb + 1);
+          wgmma_wait0();
+          drain16(total, acc, sc0, it + kb);
+          if (kb + 1 < nkb) {
+            issue_ra16(acc, fa1, it + kb + 1);
+            wgmma_wait0();
+            drain16(total, acc, sc1, it + kb + 1);
+          }
+        } else {
+          load_a(fa0, it);
+          int kb = 0;
+          for (; kb + 2 < nkb; kb += 2) {
+            issue_ra(acc, fa0, it + kb);
+            load_a(fa1, it + kb + 1);
+            wgmma_wait0();
+            drain(total, acc, it + kb);
+            issue_ra(acc, fa1, it + kb + 1);
+            load_a(fa0, it + kb + 2);
+            wgmma_wait0();
+            drain(total, acc, it + kb + 1);
+          }
           issue_ra(acc, fa0, it + kb);
-          load_a(fa1, it + kb + 1);
+          if (kb + 1 < nkb) load_a(fa1, it + kb + 1);
           wgmma_wait0();
           drain(total, acc, it + kb);
-          issue_ra(acc, fa1, it + kb + 1);
-          load_a(fa0, it + kb + 2);
-          wgmma_wait0();
-          drain(total, acc, it + kb + 1);
-        }
-        issue_ra(acc, fa0, it + kb);
-        if (kb + 1 < nkb) load_a(fa1, it + kb + 1);
-        wgmma_wait0();
-        drain(total, acc, it + kb);
-        if (kb + 1 < nkb) {
-          issue_ra(acc, fa1, it + kb + 1);
-          wgmma_wait0();
-          drain(total, acc, it + kb + 1);
+          if (kb + 1 < nkb) {
+            issue_ra(acc, fa1, it + kb + 1);
+            wgmma_wait0();
+            drain(total, acc, it + kb + 1);
+          }
         }
       } else {
         for (int kb = 0; kb < nkb; ++kb) {
@@ -423,10 +553,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
       const int r0 = m0 + wg * 64 + wq * 16 + (lane >> 2);
       // the biases of this thread's 32 columns, loaded before the first store: loads placed after a store of C would
       // each wait a full load latency (the compiler cannot move them across a store that might alias)
-      float b1v[32], b2v[32];
+      float b1v[32], b2v[32], wsc[32];  // wsc: fp16 pairs, 2^-e_n of the columns
 #pragma unroll
       for (int q = 0; q < 16; ++q) {
         const int n = n0 + 8 * q + 2 * (lane & 3);
+        if constexpr (F16) {
+          wsc[2 * q] = g16::exp2i(-__ldg(args.w_exp + n));
+          wsc[2 * q + 1] = g16::exp2i(-__ldg(args.w_exp + n + 1));
+        }
         b1v[2 * q] = b1v[2 * q + 1] = b2v[2 * q] = b2v[2 * q + 1] = 0.f;
         if (args.splitk == 1 && args.bias1) { b1v[2 * q] = __ldg(args.bias1 + n); b1v[2 * q + 1] = __ldg(args.bias1 + n + 1); }
         if (args.splitk == 1 && args.bias2) {
@@ -444,6 +578,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         for (int q = 0; q < 16; ++q) {
           const int col = 8 * q + 2 * (lane & 3);
           float2 o = make_float2(total[4 * q + 2 * h], total[4 * q + 2 * h + 1]);
+          if constexpr (F16) {
+            o.x *= wsc[2 * q];
+            o.y *= wsc[2 * q + 1];
+          }
           if (args.splitk == 1) {
             const int n = n0 + col;
             if (args.bias1) { o.x += b1v[2 * q]; o.y += b1v[2 * q + 1]; }
@@ -466,6 +604,46 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
           asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(args.ready + m0 / BM) : "memory");
       }
     }
+  }
+}
+
+template <bool MN, bool TF32>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                       const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
+                       const TcArgs args) {
+  gemm_tc_body<MN, TF32 ? TC_TF32 : TC_3XTF32>(map_a_hi, map_a_lo, map_b_hi, map_b_lo, args);
+}
+
+// fp32 A read in place and split into fp16 pairs on chip, W presplit into fp16 pairs (split_w16_kernel)
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    gemm_f16x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_unused,
+                      const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+                      const TcArgs args) {
+  gemm_tc_body<false, TC_F16X3>(map_a, map_unused, map_w_hi, map_w_lo, args);
+}
+
+// W [N][K] (rows through `rows`) -> fp16 pairs (gemm_h16_layout.cuh): row n scaled by 2^e_n, e_n = h16::scale_exp of
+// its max |w| (rec_h16_layout.cuh: a zero or non-finite row keeps e = 0), hi = RN_f16, lo = RN_f16(w 2^e_n - hi).
+// One warp per row; K even.
+__global__ void split_w16_kernel(const float* __restrict__ src, RowMap rows, int N, int K, __half* __restrict__ hi,
+                                 __half* __restrict__ lo, int* __restrict__ exps) {
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  for (int n = blockIdx.x * wpb + (threadIdx.x >> 5); n < N; n += gridDim.x * wpb) {
+    const float* p = src + rows.off(n);
+    float m = 0.f;
+    for (int k = lane; k < K; k += 32) m = fmaxf(m, fabsf(__ldg(p + k)));
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    const int e = h16::scale_exp(m);
+    const float up = ldexpf(1.f, e);
+    for (int k = 2 * lane; k < K; k += 64) {
+      const float x0 = __ldg(p + k) * up, x1 = __ldg(p + k + 1) * up;
+      const __half2 h = __floats2half2_rn(x0, x1);
+      *reinterpret_cast<__half2*>(hi + (size_t)n * K + k) = h;
+      *reinterpret_cast<__half2*>(lo + (size_t)n * K + k) = __floats2half2_rn(x0 - __low2float(h), x1 - __high2float(h));
+    }
+    if (lane == 0) exps[n] = e;
   }
 }
 
@@ -709,6 +887,20 @@ bool make_map(CUtensorMap* map, const float* ptr, int rows, int K, long long ld 
   return r == CUDA_SUCCESS;
 }
 
+// fp16 pairs of W: dense row-major [rows, K] fp16, box = [128 rows, 64 halves] (128-byte rows), 128-byte swizzle
+bool make_map16(CUtensorMap* map, const void* ptr, int rows, int K) {
+  EncodeTiledFn enc = get_encoder();
+  if (!enc || (reinterpret_cast<uintptr_t>(ptr) & 15u) || K % 8 != 0) return false;
+  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)K * 2};
+  cuuint32_t box[2] = {(cuuint32_t)g16::BK, (cuuint32_t)BN};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS;
+}
+
 // fp32 A operand read in place through its row map: 3-D map {K, inner rows, outer rows} with box {32, bi, 128 / bi},
 // so a 128-row tile is one box. Dense rows (inner_n >= M): {K, M, 1}. Rows r = t * B + b of a [T][B] view (tb_rows):
 // {K, B, T}, which tiles when B divides 128 or is a multiple of it. Strides must be multiples of 16 bytes.
@@ -907,14 +1099,16 @@ int launch_tc(const CUtensorMap (&m)[4], const TcArgs& a, int stream_clusters, c
       B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_f16x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       attr_done[dev] = true;
     }
   }
   const int sms = num_sms();
   const int nitems = a.tiles_m * a.tiles_n * a.splitk;
   const bool mn = a.a_mn || a.b_mn;
-  auto kernel = a.tf32 ? (mn ? gemm_tf32x3_kernel<true, true> : gemm_tf32x3_kernel<false, true>)
-                       : (mn ? gemm_tf32x3_kernel<true, false> : gemm_tf32x3_kernel<false, false>);
+  auto kernel = a.f16    ? gemm_f16x3_kernel
+                : a.tf32 ? (mn ? gemm_tf32x3_kernel<true, true> : gemm_tf32x3_kernel<false, true>)
+                         : (mn ? gemm_tf32x3_kernel<true, false> : gemm_tf32x3_kernel<false, false>);
   dim3 grid(nitems < sms ? nitems : sms, 1, 1);
   if (!a.ready) {
     ProfScope prof(PROF_GEMM, stream);
@@ -1027,6 +1221,56 @@ int tc_gemm_f32a(const float* A, const RowMap& a_rows, const TcOperand& B, int M
   return launch_tc(m, a, stream_clusters, stream);
 }
 
+int tc_split_w16(const float* W, const RowMap& rows, int N, int K, void* w16, cudaStream_t stream) {
+  if (!g16::shape_ok(N, K) || !w16 || (reinterpret_cast<uintptr_t>(w16) % g16::ALIGN)) {
+    set_error("split_w16: needs N %% 128 == 0, K %% 64 == 0 and a 256-byte aligned destination (N=%d K=%d)", N, K);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  const g16::W16 l = g16::w16_layout(N, K);
+  unsigned char* b = static_cast<unsigned char*>(w16);
+  int blocks = (N + 7) / 8;
+  if (blocks > NUM_SMS * 4) blocks = NUM_SMS * 4;
+  ProfScope prof(PROF_MISC, stream);
+  split_w16_kernel<<<blocks, 256, 0, stream>>>(W, rows, N, K, reinterpret_cast<__half*>(b + l.hi),
+                                               reinterpret_cast<__half*>(b + l.lo), reinterpret_cast<int*>(b + l.exp));
+  B200_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return B200RNN_OK;
+}
+
+// C[M,N] = A[M,K] * W[N,K]^T + biases with A in fp32, read in place and split into fp16 pairs on chip; W as fp16 pairs
+// at w16 (tc_split_w16). A tile's result depends on its operands only, not on the grid or on streaming.
+int tc_gemm_f16a(const float* A, const RowMap& a_rows, const void* w16, int M, int N, int K, float* C,
+                 const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
+                 int* ready, int stream_clusters) {
+  int rc = check_tc_shape(M, N, K, C, c_rows, ready, false, stream_clusters);
+  if (rc) return rc;
+  if (!g16::shape_ok(N, K)) {
+    set_error("tc_gemm: the fp16-pair path takes N %% 128 == 0 and K %% 64 == 0 (N=%d K=%d)", N, K);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  CUtensorMap m[4] = {};
+  int inner = 0;
+  if (!make_a_f32_map(&m[0], A, a_rows, M, K, &inner)) {
+    set_error("tc_gemm: the fp32 A operand cannot be read in place (16-byte aligned rows; batch dividing 128 or a "
+              "multiple of it)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  const g16::W16 l = g16::w16_layout(N, K);
+  const unsigned char* b = static_cast<const unsigned char*>(w16);
+  if (!make_map16(&m[2], b + l.hi, N, K) || !make_map16(&m[3], b + l.lo, N, K)) {
+    set_error("tc_gemm: cuTensorMapEncodeTiled failed for the fp16 weight pairs");
+    return B200RNN_ERR_CUDA;
+  }
+  TcArgs a = tc_args(M, N, K, C, c_rows, bias1, bias2, bias2_n, 0, ready);
+  a.a_f32 = 1;
+  a.a_inner = inner;
+  a.kb_per_split = K / g16::BK;
+  a.w_exp = reinterpret_cast<const int*>(b + l.exp);
+  a.f16 = 1;
+  return launch_tc(m, a, stream_clusters, stream);
+}
+
 int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t stream) {
   if (!gemm_tc_eligible(p, ws_bytes)) {
     set_error("gemm_tc: problem not eligible for the tensor-core path");
@@ -1043,6 +1287,25 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
     rc = p.a_kcontig ? tc_split(p.A, p.a_rows, p.M, p.K, a_hi, tf32 ? nullptr : a_lo, stream)
                      : tc_split(p.A, p.a_rows, p.K, p.M, a_hi, tf32 ? nullptr : a_lo, stream);
   if (rc) return rc;
+  static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
+  // fp16 pairs (the no-grad forward of b200rnn_forward_fused): W as split by b200rnn_prepare_weights, else split here
+  // into the room of the TF32 W split; a shape it does not take runs the 3xTF32 fp32-A kernel
+  const bool h16 = p.tc_h16 && p.tc_a_f32 && p.b_kcontig && !tf32 && g16::shape_ok(p.N, p.K);
+  if (debug && p.tc_a_f32)
+    fprintf(stderr, "[b200rnn] forward x-projection: M=%d N=%d K=%d math=%s weights=%s\n", p.M, p.N, p.K,
+            h16 ? "f16x3" : tf32 ? "tf32" : "3xtf32",
+            (h16 ? p.tc_b_h16 != nullptr : b_hi != nullptr) ? "cached" : "split");
+  if (h16) {
+    const void* w16 = p.tc_b_h16;
+    if (!w16) {
+      void* dst = a_lo + (size_t)p.M * p.K;
+      rc = tc_split_w16(p.B, p.b_rows, p.N, p.K, dst, stream);
+      if (rc) return rc;
+      w16 = dst;
+    }
+    return tc_gemm_f16a(p.A, p.a_rows, w16, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, stream,
+                        p.tc_ready, p.tc_stream_clusters);
+  }
   if (!b_hi || (!b_lo && !tf32)) {  // single-pass TF32 reads and writes only hi
     float* w_hi = a_lo + (size_t)p.M * p.K;
     float* w_lo = tf32 ? nullptr : w_hi + (size_t)p.N * p.K;

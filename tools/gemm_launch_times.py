@@ -4,7 +4,8 @@
 For each shape it times, alone on the card:
   * `presplit`: the generic GEMM entry (b200rnn_gemm_f32). The A split pass is a separate launch and is not counted:
     this is the GEMM kernel as the forward ran it before A was split on chip;
-  * `f32a`: the fp32-A GEMM as the forward runs it now (A split in registers), when the loaded library has it.
+  * `f32a`: the fp32-A GEMM (3xTF32, A split in registers), when the loaded library has it;
+  * `f16a`: the fp16-pair fp32-A GEMM of the no-grad fused forward, when the loaded library has it.
 and beside the recurrence: the audio GRU branch (2 streamed layers) at B = 128, as bench.py's roofline pass does.
 The per-tile cost outside the k-loop (epilogue, tile switch) is estimated from the audio shape at K = 256 and K = 512:
 t(K) = waves * (k-blocks * c + e), so e = (2 t(256) - t(512)) / waves.
@@ -84,6 +85,16 @@ def main():
             ms, n = _profiled(run, args.reps)  # includes the per-call W split launch only in PROF_MISC
             res["f32a"] = {"ms": ms, "launches": n, "mma_tflops": flops / ms / 1e9,
                            "bytes": _bytes(M, N, K, 4), "gb_s": _bytes(M, N, K, 4) / ms / 1e6}
+            f16a = getattr(lib, "b200rnn_debug_gemm_f16a", None)
+            if f16a is not None:  # the fp16-pair kernel of the no-grad fused forward (W split per call: PROF_MISC)
+                f16a.restype, f16a.argtypes = f32a.restype, f32a.argtypes
+
+                def run16():
+                    _lib.check(f16a(M, N, K, A.data_ptr(), K, 0, 0, W.data_ptr(), C.data_ptr(), bias.data_ptr(), None,
+                                    0, scratch.data_ptr(), sbytes, stream), "debug_gemm_f16a")
+
+                ms16, n16 = _profiled(run16, args.reps)
+                res["f16a"] = {"ms": ms16, "launches": n16, "vs_f32a": ms16 / ms}
         out["alone"][name] = {"M": M, "N": N, "K": K, **res}
         if f32a is not None and name == "audio_layer":
             t1 = res["f32a"]["ms"]

@@ -6,8 +6,9 @@ the audio branch alone, as CUDA graphs; after a warm-up it profiles `--replays` 
 Every kernel's stream, grid, start and end (µs, relative to its replay's first kernel) go to
 `<out>/step_timeline.json`; the raw chrome traces go beside it.
 
-The audio chain is the stream that runs the GRU recurrence (`rec_fwd_tc_kernel`); every other kernel of the step is
-the text branch or the head. For each audio kernel it prints, as medians over the replays:
+The audio chain is the stream that runs the GRU recurrence (`rec_fwd_tc_kernel`, or `rec_fwd_h16_kernel` in the
+no-grad fused forward); every other kernel of the step is the text branch or the head. For each audio kernel it
+prints, as medians over the replays:
   * `gap`: its start minus the end of its predecessor on the audio stream (negative for a recurrence that starts
     beside its streamed GEMM); for a recurrence also `after_gemm_start`;
   * its duration, beside its duration when the audio branch runs alone.
@@ -35,7 +36,8 @@ from torch.profiler import ProfilerActivity, profile  # noqa: E402
 import b200rnn  # noqa: E402
 import bench  # noqa: E402
 
-REC = "rec_fwd_tc_kernel"
+# the GRU-256 forward recurrence: 3xTF32 tensor cores, or fp16 pairs in the no-grad fused forward
+REC = ("rec_fwd_tc_kernel", "rec_fwd_h16_kernel")
 
 
 def _card():
@@ -103,7 +105,7 @@ def _median(xs):
 def _audio_chain(replay):
     """(audio chain, text branch): the kernels on the recurrence's stream, and the others; the final head kernel after
     the join belongs to neither."""
-    streams = {k["stream"] for k in replay if k["name"] == REC}
+    streams = {k["stream"] for k in replay if k["name"] in REC}
     if len(streams) != 1:
         raise RuntimeError(f"the GRU recurrences ran on streams {sorted(streams)}; expected one audio stream")
     s = streams.pop()
@@ -128,7 +130,7 @@ def _chain_rows(replays):
                "dur_us": round(_median([k["end"] - k["start"] for k in ks]), 1)}
         if i > 0:
             row["gap_us"] = round(_median([a[i]["start"] - a[i - 1]["end"] for a, _ in chains]), 1)
-            if ks[0]["name"] == REC:
+            if ks[0]["name"] in REC:
                 row["after_gemm_start_us"] = round(_median([a[i]["start"] - a[i - 1]["start"] for a, _ in chains]), 1)
         rows.append(row)
     text_end = [max((k["end"] for k in o), default=0.0) - a[-1]["end"] for a, o in chains]
