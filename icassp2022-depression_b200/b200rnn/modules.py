@@ -12,7 +12,9 @@ default init U(-1/sqrt(H), 1/sqrt(H)) (rnn.py:308-311) and the ``forward`` retur
 
 ``PackedSequence`` input is supported (per-sequence lengths in the kernels), and so are an initial state ``hx``
 (checked as torch checks it, differentiable: streaming inference or truncated BPTT that chains ``h_n`` into the next
-call) and unbatched 2-D input. ``LSTM(..., proj_size=P)`` (LSTMP: ``h_t = W_hr (o_t * tanh c_t)``) runs on its own
+call) and unbatched 2-D input. ``hidden_size`` is any multiple of 16 from 16 to 1024: 128 and 256 run the tuned
+fixed-size kernels, every other size the runtime-sized cluster kernels (csrc/rnn_anyh.cu); other sizes raise
+``B200RNNError`` at the first forward. ``LSTM(..., proj_size=P)`` (LSTMP: ``h_t = W_hr (o_t * tanh c_t)``) runs on its own
 projected kernels for P in {H/4, H/2} and registers ``weight_hr_l{k}[_reverse]`` last, as torch does. Features that
 raise ``NotImplementedError``: bias=False, and other projection sizes. A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
 """
@@ -229,7 +231,7 @@ class _B200RNNBase(nn.Module):
                        prologue_done: Optional[torch.cuda.Event] = None) -> torch.Tensor:
         """``self(ln(input))[0].sum(dim=time)`` — the audio branch of fuse_net_whole.py:360-362 / fuse_net.py:338-339.
 
-        For widths the tensor-core projection takes, LayerNorm is folded into the layer-0 operand preparation and the
+        For hidden sizes 128 and 256 and the widths the tensor-core projection takes, LayerNorm is folded into the layer-0 operand preparation and the
         time sum into the last layer's step loop. Without autograd (the reference's fuse scripts run it under
         ``torch.no_grad()``, fuse_net_whole.py:337) the normalised input and the [B,T,H] output never touch HBM; under
         autograd (audio_gru_whole.py:103-108 + loss.backward()) the same fusions run in both directions
@@ -241,7 +243,7 @@ class _B200RNNBase(nn.Module):
         """
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
-        shape_ok = (input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
+        shape_ok = (input.is_cuda and input.dim() == 3 and self.proj_size == 0 and self.hidden_size in (128, 256) and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and
                                     ln.bias is not None)))
         fusable = not need_grad and shape_ok

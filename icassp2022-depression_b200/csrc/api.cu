@@ -39,6 +39,18 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 // proj_size of a descriptor: the field exists only when B200RNN_FLAG_PROJ says so (a descriptor may end at `flags`)
 inline int desc_proj(const b200rnn_desc* d) { return (d->flags & B200RNN_FLAG_PROJ) ? d->proj_size : 0; }
 
+// The model-shell entry points (b200rnn_forward_fused, _backward_fused, _prepare_weights, _wcache_bytes) run only the
+// fixed hidden sizes 128 and 256: their fusions (LayerNorm prologue, pooling, weight cache, the fp16-pair no-grad
+// recurrence) are built for those
+int check_shell_hidden(const b200rnn_desc* d, const char* what) {
+  if (d && d->hidden_size != 128 && d->hidden_size != 256) {
+    set_error("%s: the model-shell entry points take hidden_size 128 and 256 (got %d; use the _hx entry points)", what,
+              d->hidden_size);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  return B200RNN_OK;
+}
+
 struct Dims {
   int mode, B, T, I, H, L, D, G;
   int P, HO, NPAR;  // proj_size (0: none), width of h / the layer output per direction, parameters per (layer, dir)
@@ -62,8 +74,10 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
               d->num_dirs);
     return B200RNN_ERR_INVALID;
   }
-  if (d->hidden_size != 128 && d->hidden_size != 256) {
-    set_error("hidden_size %d unsupported: the sm_90a persistent kernels are built for 128 and 256",
+  // 128 and 256 run the fixed configs of rnn_rec.cu, every other multiple of 16 up to 1024 the runtime-sized kernels
+  // of rnn_anyh.cu
+  if (!anyh_hidden_size(d->hidden_size)) {
+    set_error("hidden_size %d unsupported: the sm_90a recurrence kernels take multiples of 16 from 16 to 1024",
               d->hidden_size);
     return B200RNN_ERR_UNSUPPORTED;
   }
@@ -72,8 +86,10 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
     set_error("proj_size %d invalid: an LSTM takes 0 <= proj_size < hidden_size, a GRU none", P);
     return B200RNN_ERR_INVALID;
   }
-  if (P > 0 && P != d->hidden_size / 4 && P != d->hidden_size / 2) {
-    set_error("proj_size %d unsupported: the projected kernels are built for hidden_size/4 and hidden_size/2", P);
+  if (P > 0 && ((d->hidden_size != 128 && d->hidden_size != 256) ||
+                (P != d->hidden_size / 4 && P != d->hidden_size / 2))) {
+    set_error("proj_size %d unsupported: the projected kernels are built for hidden_size 128 and 256 with "
+              "proj_size hidden_size/4 and hidden_size/2", P);
     return B200RNN_ERR_UNSUPPORTED;
   }
   if (!(d->dropout_p >= 0.f && d->dropout_p <= 1.f)) {
@@ -619,8 +635,9 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     // of the SMs; the GEMM runs as 4-CTA clusters in the cluster slots the recurrence leaves free. Otherwise GEMM and
     // recurrence run one after the other.
     const int gemm_clusters = rec.capacity - rec.nclusters;
-    const bool stream_xproj = d.D == 1 && d.P == 0 && tc_layer && rec.C == 4 && rec.one_wave() && 2 * rec.ctas() <= sms &&
-                              gemm_clusters > 0;
+    // The runtime-sized kernels (rec.anyh) take no streamed x-projection.
+    const bool stream_xproj = !rec.anyh && d.D == 1 && d.P == 0 && tc_layer && rec.C == 4 && rec.one_wave() &&
+                              2 * rec.ctas() <= sms && gemm_clusters > 0;
     // ---- A operand of the tensor-core input projection (fp32, split on chip by the GEMM), shared by the directions:
     // the layer input itself when the GEMM can read it in place, else a dense copy in the GEMM's workspace
     void* tc_ws = S + sl.f_tc;
@@ -755,6 +772,7 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     set_error("forward_fused: the model-shell entry points do not take proj_size (use b200rnn_forward_hx)");
     return B200RNN_ERR_UNSUPPORTED;
   }
+  if (check_shell_hidden(desc, "forward_fused")) return B200RNN_ERR_UNSUPPORTED;
   return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
                       ln_gamma, ln_beta, ln_eps, y_pool, lengths, wcache, prologue_done, nullptr, nullptr, true,
                       stream_);
@@ -805,6 +823,7 @@ B200RNN_API int b200rnn_wcache_bytes(const b200rnn_desc* desc, size_t* bytes) {
     set_error("wcache_bytes: the weight cache of b200rnn_forward_fused does not take proj_size");
     return B200RNN_ERR_UNSUPPORTED;
   }
+  if (check_shell_hidden(desc, "wcache_bytes")) return B200RNN_ERR_UNSUPPORTED;
   WCacheLayout wl;
   make_wcache(d, &wl);
   if (bytes) *bytes = (wl.total + ALIGN_F) * sizeof(float);
@@ -824,6 +843,7 @@ B200RNN_API int b200rnn_prepare_weights(const b200rnn_desc* desc, const float* c
     set_error("prepare_weights: the weight cache of b200rnn_forward_fused does not take proj_size");
     return B200RNN_ERR_UNSUPPORTED;
   }
+  if (check_shell_hidden(desc, "prepare_weights")) return B200RNN_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   WCacheLayout wl;
   make_wcache(d, &wl);
@@ -1001,7 +1021,9 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
         // offset of B (forward: dG[t] with h[t-1], t = 1..T-1; reverse: dG[t] with h[t+1], t = 0..T-2). LSTM: one GEMM
         // over all gates; GRU: the r,z rows from columns [0, 2H) of dG, the n rows from dn*r
         const int g0 = k == 0 ? d.B : 0, Kp = (d.T - 1) * d.B;
-        const bool gru = d.mode == B200RNN_GRU, tc = tc_l && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0;
+        // the tensor-core GEMM needs N = H a multiple of 128 (hidden sizes other than 128 / 256 may not be)
+        const bool gru = d.mode == B200RNN_GRU,
+                   tc = tc_l && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0 && d.HO % 128 == 0;
         rc = run_grad_gemm({{&dG, g0, false}, {&h, d.B - g0, false}, gru ? 2 * d.H : GH, d.HO, Kp, dw_hh,
                             simple_rows(d.HO), accumulate, true, tc, gru ? "dW_hh_rz" : "dW_hh"}, sl, S, tf32, st);
         if (rc) return rc;
@@ -1061,6 +1083,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
     set_error("backward_fused: the model-shell entry points do not take proj_size (use b200rnn_backward_hx)");
     return B200RNN_ERR_UNSUPPORTED;
   }
+  if (check_shell_hidden(desc, "backward_fused")) return B200RNN_ERR_UNSUPPORTED;
   return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, dy_pool, dy_pool_scale, dh_n,
                        dc_n, reserve, scratch, dx, dxs_t, dxs_b, dparams, lengths, ln_gamma, ln_eps, dln_gamma,
                        dln_beta, nullptr, nullptr, nullptr, nullptr, stream_);

@@ -48,6 +48,12 @@ struct ClusterLaunch {
   void (*kernel)(P, int);
   int C, NT, nslices, nclusters, capacity;
   size_t smem;
+  // a runtime-sized kernel of rnn_anyh.cu (hidden sizes other than 128 / 256): it takes no streamed x-projection
+  // (RecFwdParams::ready), and its backward reads W_hh as anyh_prep_kernel lays it out. BS batch rows per cluster;
+  // onchip: W_hh stays in shared memory (else it is read from L2 every step).
+  bool anyh = false;
+  int BS = 0;
+  bool onchip = false;
   int ctas() const { return nclusters * C; }
   bool one_wave() const { return nclusters <= capacity; }
 };
@@ -85,8 +91,17 @@ struct RecBwdParams {
 };
 using RecBwdLaunch = ClusterLaunch<RecBwdParams>;
 
+constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_90
+
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)
 int rec_bwd_max_slices(int B);
+
+// The runtime-sized recurrence (rnn_anyh.cu): the hidden sizes it takes (H % 16 == 0, 16 <= H <= 1024), its config
+// choice for the shapes the fixed configs do not cover, and its W_hh transpose for the backward (any H)
+bool anyh_hidden_size(int H);
+int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* out);
+int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out);
+int launch_anyh_prep(const float* w_hh, float* w_prep, int G, int H, int C, cudaStream_t stream);
 
 // forward: choose the config for p's shape (mode, H, P, B, D, lengths or not), then launch it; p.ready != NULL launches
 // it with programmatic stream serialization, so that it may start while the GEMM before it still runs

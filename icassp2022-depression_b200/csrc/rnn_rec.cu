@@ -43,7 +43,6 @@ namespace b200rnn {
 
 namespace {
 
-constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_90
 // The CTA's own state slice is delivered locally (st.shared + mbarrier.arrive per warp). -DB200RNN_SELF_VIA_CLUSTER
 // builds the round-1 behaviour (own slice through st.async like the peers') for the FFMA kernels rec_fwd_kernel and
 // rec_bwd_kernel only: compute-sanitizer's racecheck does not model the ordering that inline-PTX mbarrier.arrive /
@@ -1808,6 +1807,8 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
     pick_fwd<B200RNN_LSTM, 128, 4, 8, 16, 2, 1>(p, true, L, &rc);
     return rc;
   }
+  // every other hidden size: the runtime-sized kernels of rnn_anyh.cu
+  if (anyh_hidden_size(p.H)) return plan_anyh_fwd(p, L);
   set_error("recurrence: unsupported (mode=%d, hidden_size=%d); built for hidden_size 128 and 256", p.mode,
             p.H);
   return B200RNN_ERR_UNSUPPORTED;
@@ -1849,6 +1850,7 @@ int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
     pick_bwd<B200RNN_LSTM, 128, 4, 8, 32, 4, 1>(p, true, L, &rc);
     return rc;
   }
+  if (anyh_hidden_size(p.H)) return plan_anyh_bwd(p, L);
   set_error("recurrence backward: unsupported (mode=%d, hidden_size=%d)", p.mode, p.H);
   return B200RNN_ERR_UNSUPPORTED;
 }
@@ -1863,6 +1865,10 @@ int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s)
     set_error("recurrence: the no-grad fused forward takes no initial state");
     return B200RNN_ERR_INVALID;
   }
+  if (L.anyh && (p.ready || p.y_pool || p.shell_nograd)) {
+    set_error("recurrence: hidden_size %d takes no streamed x-projection, y_pool or no-grad fused forward", p.H);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   return launch_clustered(L, p, PROF_REC_FWD, p.ready != nullptr, s);
 }
 
@@ -1870,7 +1876,12 @@ int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
   RecBwdLaunch L;
   const int rc = plan_rec_bwd(p, &L);
   if (rc != B200RNN_OK || L.kernel == nullptr) return rc;
-  if (p.P == 0) {  // transposed, per-CTA contiguous copy of W_hh for the chosen cluster width
+  if (L.anyh) {  // the same layout for any H (whh_prep_kernel tiles by 32)
+    for (int d = 0; d < p.D; ++d) {
+      const int prc = launch_anyh_prep(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C, s);
+      if (prc != B200RNN_OK) return prc;
+    }
+  } else if (p.P == 0) {  // transposed, per-CTA contiguous copy of W_hh for the chosen cluster width
     for (int d = 0; d < p.D; ++d) {
       whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C);
       if (cudaGetLastError() != cudaSuccess) {

@@ -4,6 +4,8 @@
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py rnn   # recurrence only
 The GRU H=256 layer also runs at B = 96, which needs the 4-row clusters (bs4: the 2-row ones do not all fit at once).
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py cells # GRUCell / LSTMCell forward + backward only
+    compute-sanitizer --tool racecheck python tools/sanitize_paths.py anyh # runtime-sized recurrence (rnn_anyh.cu) only:
+        GRU H = 192 (W_hh in shared memory) and LSTM H = 768 (W_hh from L2), fixed-length and ragged, with hx and dh_0
 """
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -12,6 +14,21 @@ import torch, b200rnn
 from torch.nn.utils.rnn import pack_padded_sequence
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
+if sys.argv[1:] == ["anyh"]:
+    # B = 5 on clusters planned for more rows: idle threads past the batch, a partial last warp, unequal slices at 464
+    for kind, I, H, B, T in (("gru", 24, 192, 5, 4), ("lstm", 24, 768, 5, 3), ("lstm", 24, 464, 3, 3)):
+        m = (b200rnn.GRU if kind == "gru" else b200rnn.LSTM)(I, H, bidirectional=True).to(dev)
+        x = torch.randn(T, B, I, device=dev, requires_grad=True)
+        h0 = torch.randn(2, B, H, device=dev, requires_grad=True)
+        hx = h0 if kind == "gru" else (h0, torch.randn(2, B, H, device=dev))
+        out = m(x, hx)
+        (out[0].sum() + (out[1] if kind == "gru" else out[1][0]).sum()).backward()
+        xp = pack_padded_sequence(x.detach().requires_grad_(True), torch.tensor([3, 1, 2, 3, 2][:B]),
+                                  enforce_sorted=False)
+        m(xp)[0].data.sum().backward()
+        torch.cuda.synchronize()
+        print(kind, H, "ok", flush=True)
+    sys.exit(0)
 if sys.argv[1:] == ["cells"]:
     # K and batch tails, unaligned rows (odd offsets into larger buffers), no bias, no state, both contractions
     for kind, I, H, B, bias in (("gru", 3, 5, 7, True), ("lstm", 257, 129, 9, False), ("gru", 256, 256, 130, False),
