@@ -105,7 +105,7 @@ def attention_pool_tm(attention_layer: torch.nn.Module, seq_tm: torch.Tensor, h_
     shapes the kernels do not take (T*H beyond one CTA's shared memory) or non-CUDA tensors of the oracle tests."""
     lin = attention_layer[0]
     T, B, H2 = seq_tm.shape
-    fits = (4 * (H2 // 2) + 2 * T + T * (H2 // 2)) * 4 <= 200 * 1024 and (2 * (H2 // 2) + T) * 4 <= 48 * 1024
+    fits = (4 * (H2 // 2) + 2 * T + T * (H2 // 2)) * 4 <= 200 * 1024 and (2 * (H2 // 2) + T) * 4 <= 47 * 1024
     if seq_tm.is_cuda and fits and seq_tm.dtype == torch.float32:
         return _AttentionPoolFunction.apply(seq_tm, h_n, lin.weight, lin.bias)
     from .models import attention_pool as _generic

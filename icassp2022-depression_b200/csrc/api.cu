@@ -1475,4 +1475,51 @@ B200RNN_API int b200rnn_debug_grad_gemm(const int64_t* srcs, int nsrc, const int
   return B200RNN_OK;
 }
 
+/* test only (not declared in the public header): the folded LayerNorm prologue's kernels as a layer runs them.
+   Row r < R of x (and of dx) sits at x + s_outer * (r / inner_n) + s_inner * (r % inner_n) floats; out and dy are dense
+   [R][Cc]. out != NULL: out = LayerNorm(x) * gamma + beta (tc_layernorm). dy != NULL: launch_layernorm_bwd with that
+   dy, dx optional (NULL: only dgamma / dbeta), accumulate into dgamma / dbeta or overwrite them; part holds part_floats
+   >= 2 * 2 * NUM_SMS * Cc floats of per-CTA partials. lengths (optional, B rows per step): rows r with
+   r / B >= lengths[r % B] are padding, as in a ragged batch. */
+B200RNN_API int b200rnn_debug_layernorm(const float* x, int64_t s_outer, int64_t s_inner, int inner_n, int R, int Cc,
+                                        const float* gamma, const float* beta, float eps, float* out, const float* dy,
+                                        float* dx, float* dgamma, float* dbeta, int accumulate, float* part,
+                                        size_t part_floats, const int* lengths, int B, void* stream_) {
+  if (!x || !gamma || R < 1 || inner_n < 1 || (out && !beta) || (dy && (!dgamma || !dbeta || !part)) ||
+      (lengths && B < 1)) {
+    set_error("debug_layernorm: bad arguments");
+    return B200RNN_ERR_INVALID;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const RowMap rows{s_outer, s_inner, inner_n};
+  if (out) {
+    const int rc = tc_layernorm(x, rows, R, Cc, gamma, beta, eps, out, st, nullptr, 0, lengths, B);
+    if (rc != B200RNN_OK) return rc;
+  }
+  if (dy) {
+    if (part_floats < layernorm_bwd_scratch_floats(Cc)) {
+      set_error("debug_layernorm: part holds %zu floats, %zu needed", part_floats, layernorm_bwd_scratch_floats(Cc));
+      return B200RNN_ERR_INVALID;
+    }
+    return launch_layernorm_bwd(x, rows, dy, R, Cc, gamma, eps, dx, rows, dgamma, dbeta, accumulate, part, st, lengths,
+                                B);
+  }
+  return B200RNN_OK;
+}
+
+/* test only (not declared in the public header): the inter-layer dropout as a layer runs it, out[i] = in[i] *
+   keep(i) / (1 - p) over n elements of Philox stream stream_id at {seed, offset}; hdr: 2 uint64 of device memory for
+   the resolved RNG header. Any n and any float alignment (the float4 path and the scalar tail). */
+B200RNN_API int b200rnn_debug_dropout(const float* in, float* out, size_t n, float p, uint64_t seed, uint64_t offset,
+                                      uint32_t stream_id, uint64_t* hdr, void* stream_) {
+  if (!in || !out || !hdr) {
+    set_error("debug_dropout: null pointer");
+    return B200RNN_ERR_INVALID;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const int rc = launch_rng_setup(hdr, seed, offset, nullptr, 0, st);
+  if (rc != B200RNN_OK) return rc;
+  return launch_dropout(in, out, n, p, hdr, stream_id, st);
+}
+
 }  // extern "C"

@@ -162,15 +162,13 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_finish_kernel(const b2
   if (done == sent) return;  // nothing pending (first step, or already flushed)
   peer_wait_sum(a, g, n, done, tid);
   const float t = *a.adam_step + 1.f;
-  const float bc1 = 1.f - powf(a.beta1, t), bc2 = 1.f - powf(a.beta2, t);
-  const float step_size = a.lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
+  const AdamCoef c = adam_coef(t, a.lr, a.beta1, a.beta2, 0.f);
   for (int i = tid; i < n; i += HEAD_THREADS) {
-    const float gi = g[i] * a.grad_scale;
-    const float mi = a.beta1 * a.adam_m[i] + (1.f - a.beta1) * gi;
-    const float vi = a.beta2 * a.adam_v[i] + (1.f - a.beta2) * gi * gi;
+    float w = a.W[i], mi = a.adam_m[i], vi = a.adam_v[i];
+    adam_update(w, mi, vi, g[i] * a.grad_scale, a.beta1, a.beta2, a.eps, c);
     a.adam_m[i] = mi;
     a.adam_v[i] = vi;
-    a.W[i] = a.W[i] - step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + a.eps);
+    a.W[i] = w;
   }
   __syncthreads();
   if (tid == 0) {
@@ -445,15 +443,13 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_kernel(const b200rnn_f
   }
   if (a.do_adam && apply_update) {  // torch.optim.Adam (no weight decay, no amsgrad); grad_scale = 1/world
     const float t = *a.adam_step + 1.f;
-    const float bc1 = 1.f - powf(a.beta1, t), bc2 = 1.f - powf(a.beta2, t);
-    const float step_size = a.lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
+    const AdamCoef c = adam_coef(t, a.lr, a.beta1, a.beta2, 0.f);
     for (int i = tid; i < C * F; i += HEAD_THREADS) {
-      const float g = a.dw[i] * a.grad_scale;
-      const float mi = a.beta1 * a.adam_m[i] + (1.f - a.beta1) * g;
-      const float vi = a.beta2 * a.adam_v[i] + (1.f - a.beta2) * g * g;
+      float w = a.W[i], mi = a.adam_m[i], vi = a.adam_v[i];
+      adam_update(w, mi, vi, a.dw[i] * a.grad_scale, a.beta1, a.beta2, a.eps, c);
       a.adam_m[i] = mi;
       a.adam_v[i] = vi;
-      a.W[i] = a.W[i] - step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + a.eps);
+      a.W[i] = w;
     }
     __syncthreads();
     if (tid == 0) *a.adam_step = t;

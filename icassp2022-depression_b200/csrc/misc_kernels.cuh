@@ -39,4 +39,30 @@ int launch_valid_rows(const float* src, const RowMap& rows, int T, int B, int C,
 int launch_bias_reduce(const float* part, int nslices, int mode, int H, float* db_ih, float* db_hh,
                        int accumulate, cudaStream_t stream);
 
+// ---- one Adam / AdamW rule for every kernel that applies it (adam_kernel, the fuse head and its deferred finish) ----
+// torch.optim.Adam / AdamW without amsgrad at step t (1-based): the same code everywhere, so that the fused head's
+// update and b200rnn_adamw's are bit-identical from the same gradient.
+struct AdamCoef {
+  float step_size;     // lr / (1 - beta1^t)
+  float inv_sqrt_bc2;  // 1 / sqrt(1 - beta2^t)
+  float decay;         // 1 - lr * weight_decay (decoupled, AdamW); exactly 1 for Adam
+};
+// 1 - beta^t = -expm1(t * log1p(-(1 - beta))): 1 - beta is exact in fp32 for beta in [0.5, 1], and no step cancels.
+// 1 - powf(beta, t) loses up to ~110 ulp of bc2 at beta2 = 0.999 and t = 2..5, because beta^t is close to 1 there.
+__device__ __forceinline__ float adam_bias_correction(float beta, float t) {
+  return -expm1f(t * log1pf(-(1.f - beta)));
+}
+__device__ __forceinline__ AdamCoef adam_coef(float t, float lr, float beta1, float beta2, float weight_decay) {
+  return AdamCoef{lr / adam_bias_correction(beta1, t), rsqrtf(adam_bias_correction(beta2, t)), 1.f - lr * weight_decay};
+}
+// g is the already scaled gradient
+__device__ __forceinline__ void adam_update(float& p, float& m, float& v, float g, float beta1, float beta2, float eps,
+                                            const AdamCoef& c) {
+  const float mi = beta1 * m + (1.f - beta1) * g;
+  const float vi = beta2 * v + (1.f - beta2) * g * g;
+  m = mi;
+  v = vi;
+  p = p * c.decay - c.step_size * mi / (sqrtf(vi) * c.inv_sqrt_bc2 + eps);
+}
+
 }  // namespace b200rnn

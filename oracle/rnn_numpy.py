@@ -20,7 +20,9 @@ unpinned" by the reference itself); this restatement is pinned instead against t
 (tests/test_oracle.py compares it with torch.nn.GRU / nn.LSTM on CPU, forward and backward) and, through
 oracle/ref_models.py, against outputs of the reference's own classes recorded in tests/golden/.
 
-Inter-layer dropout is not modelled (compare in eval() / dropout=0, SURVEY.md §8c).
+Inter-layer dropout: ``forward(x, masks=...)`` takes the factor (0 or 1 / (1 - p)) of every element of each
+layer's output but the last, [T, B, D*H] time-major - element (t*B + b)*D*H + j is what the library's dropout reads
+from Philox stream l at the forward's offset (oracle/philox.py). ``backward`` applies the same factors to the gradient.
 
 Ragged batches (``lengths``): PackedSequence semantics of the same modules (packed branch of GRU.forward /
 LSTM.forward, rnn.py:1393-1394,1459-1470 / :1095-1096,1195-1206, fed by torch.nn.utils.rnn.pack_padded_sequence) on the
@@ -202,9 +204,12 @@ class NumpyRNN:
         base = 4 * (l * self.D + d)
         return self.w[base:base + 4]
 
-    def forward(self, x: np.ndarray, lengths=None):
-        """x [T,B,I] (padded); ``lengths`` [B] = valid steps per sequence (PackedSequence semantics) or None."""
+    def forward(self, x: np.ndarray, lengths=None, masks=None):
+        """x [T,B,I] (padded); ``lengths`` [B] = valid steps per sequence (PackedSequence semantics) or None;
+        ``masks``: L - 1 dropout factors [T,B,D*H] multiplied into the output of layers 0..L-2, or None."""
         x = np.asarray(x, dtype=self.dtype)
+        self._masks = None if masks is None else [np.asarray(m, dtype=self.dtype) for m in masks]
+        assert self._masks is None or len(self._masks) == self.L - 1
         self._lengths = None if lengths is None else np.asarray(lengths, dtype=np.int64)
         inp = x
         h_n, c_n, saved = [], [], []
@@ -220,6 +225,8 @@ class NumpyRNN:
                 c_n.append(c)
             saved.append((inp, caches))
             inp = np.concatenate(outs, axis=2) if self.D == 2 else outs[0]
+            if self._masks is not None and l < self.L - 1:
+                inp = inp * self._masks[l]
         self._saved = saved
         h_n = np.stack(h_n)
         if self.mode == "lstm":
@@ -247,7 +254,7 @@ class NumpyRNN:
                                                                  lengths=self._lengths)
                 dinp += dx
                 grads[(l, d)] = (dw_ih, dw_hh, db_ih, db_hh)
-            dy = dinp
+            dy = dinp if (self._masks is None or l == 0) else dinp * self._masks[l - 1]
         flat = []
         for l in range(self.L):
             for d in range(self.D):

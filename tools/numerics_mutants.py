@@ -31,6 +31,9 @@ REC_EXISTING = ["tests/test_gpu_parity.py", "tests/test_gpu_property.py", "tests
 GEMM_NEW = ["tests/test_gpu_grad_gemm_f64.py"]
 GEMM_EXISTING = ["tests/test_gpu_gemm.py", "tests/test_gpu_gemm_f32a.py", "tests/test_gpu_grad_paths.py",
                  "tests/test_gpu_parity.py", "tests/test_gpu_tf32_mode.py"]
+SHELL_NEW = ["tests/test_gpu_shell_f64.py"]
+SHELL_EXISTING = ["tests/test_gpu_head.py", "tests/test_gpu_train_step.py", "tests/test_gpu_fuse_parity.py",
+                  "tests/test_gpu_models.py"]
 
 # name -> (file under csrc/, text, replacement, what it breaks, new tests, existing tests)
 MUTATIONS = {
@@ -63,6 +66,47 @@ MUTATIONS = {
                                       GEMM_EXISTING),
     "ffma_epilogue_drop_accumulate": ("gemm_f32.cu", "            if (p.accumulate) o += dst[e];\n", "",
                                       "FFMA epilogue: accumulate = 1 overwrites C", GEMM_NEW, GEMM_EXISTING),
+    # the three mask mutants: forward and backward (or fused and unfused) make the same mistake
+    "head_keep_word_shift": ("fuse_head.cu", "  return rr[idx & 3] >= thr ? scale : 0.f;",
+                             "  return rr[(idx + 1) & 3] >= thr ? scale : 0.f;",
+                             "fuse head dropout: every element reads the next Philox word", SHELL_NEW, SHELL_EXISTING),
+    "dropout_f4_y_word": ("misc_kernels.cu", "      v.y = rr[1] >= thr ? v.y * scale : 0.f;",
+                          "      v.y = rr[2] >= thr ? v.y * scale : 0.f;",
+                          "inter-layer dropout, float4 path: element 1 of a quad reads word 2", SHELL_NEW,
+                          SHELL_EXISTING),
+    "head_audio_out_stream": ("fuse_head.cu", ": keep_scale(seed, offset, 3, (size_t)b * Ha + (j - Ht), thr, scale);",
+                              ": keep_scale(seed, offset, 2, (size_t)b * Ha + (j - Ht), thr, scale);",
+                              "fuse head: the audio output dropout reuses the input stream 2", SHELL_NEW,
+                              SHELL_EXISTING),
+    "mlp_out_stream": ("head_kernels.cu", "if (drop) v *= keep_scale(hdr, stream_id + 1,",
+                       "if (drop) v *= keep_scale(hdr, stream_id,",
+                       "mlp_dropout: the output dropout reuses the input stream", SHELL_NEW, SHELL_EXISTING),
+    "att_bwd_drop_tanh_deriv": ("head_kernels.cu", "const float dh = score[t] * dcj + ds[t] * q * (1.f - th * th);",
+                                "const float dh = score[t] * dcj + ds[t] * q;",
+                                "attention backward: d tanh loses its (1 - th^2)", SHELL_NEW, SHELL_EXISTING),
+    "sce_dz_p_times_g": ("head_kernels.cu", "dz[(size_t)row * C + lane] = p * (g - dot);",
+                         "dz[(size_t)row * C + lane] = p * g;",
+                         "softmax_ce: dz drops the softmax Jacobian's rank-one term", SHELL_NEW, SHELL_EXISTING),
+    "smoothl1_no_clamp": ("fuse_head.cu", "dt[0] = fminf(fmaxf(d, -1.f), 1.f) * invB;", "dt[0] = d * invB;",
+                          "fuse head SmoothL1: the text head's gradient loses its clamp", SHELL_NEW, SHELL_EXISTING),
+    "regression_no_gate": ("fuse_head.cu", "po = fmaf(gt * v, a.W[j], po);", "po = fmaf(v, a.W[j], po);",
+                           "fuse head regression output: the sigmoid(modal_attn x) gate is dropped", SHELL_NEW,
+                           SHELL_EXISTING),
+    "ln_fwd_drop_eps": ("gemm_tc.cu",
+                        "    const float rstd = rsqrtf(v / (float)Cc + eps);\n#pragma unroll\n    for (int i = 0; i < NV; ++i) {\n"
+                        "      const int k = i * 128 + lane * 4;\n",
+                        "    const float rstd = rsqrtf(v / (float)Cc);\n#pragma unroll\n    for (int i = 0; i < NV; ++i) {\n"
+                        "      const int k = i * 128 + lane * 4;\n",
+                        "LayerNorm forward: eps is left out of rstd", SHELL_NEW, SHELL_EXISTING),
+    "ln_bwd_drop_xhat_mgx": ("gemm_tc.cu", "o4.y = rstd * (dv[i].y - mg - xv[i].y * mgx);", "o4.y = rstd * (dv[i].y - mg);",
+                             "LayerNorm backward: one component of dx loses - xhat mean(g xhat)", SHELL_NEW,
+                             SHELL_EXISTING),
+    "adamw_no_decay": ("misc_kernels.cuh", "  p = p * c.decay - c.step_size", "  p = p - c.step_size",
+                       "AdamW: the decoupled weight decay is lost", SHELL_NEW, SHELL_EXISTING),
+    "adam_pow_bias_correction": ("misc_kernels.cuh", "  return -expm1f(t * log1pf(-(1.f - beta)));",
+                                 "  return 1.f - powf(beta, t);",
+                                 "Adam: the cancelling 1 - powf(beta, t) of the previous code", SHELL_NEW,
+                                 SHELL_EXISTING),
 }
 
 
