@@ -1,4 +1,5 @@
-"""b200rnn — H100-native (sm_90a) GRU / BiLSTM sequence encoders behind the torch.nn.GRU / nn.LSTM API.
+"""b200rnn — H100-native (sm_90a) GRU / BiLSTM sequence encoders behind the torch.nn.GRU / nn.LSTM API (and
+nn.RNN, the cells GRUCell / LSTMCell / RNNCell).
 
 The one hot path of speechandlanguageprocessing/ICASSP2022-Depression (SURVEY.md §8), rebuilt from scratch:
 PyTorch host code -> C-ABI shared library (include/b200rnn.h) -> hand-written CUDA kernels.
@@ -6,7 +7,7 @@ Importing this package does not need a GPU; running any op does, and fails loudl
 """
 from . import _lib
 from ._lib import B200RNNError
-from .modules import GRU, LSTM, GRUCell, LSTMCell, from_torch, install, uninstall
+from .modules import GRU, LSTM, RNN, GRUCell, LSTMCell, RNNCell, from_torch, install, uninstall
 from .functional import RNNConfig, gemm, rnn_forward
 from .staging import FuseBatch, PinnedStager, bind_host_thread_to_gpu_numa_node, stage_fuse_batch
 from .dp import GradBucket, broadcast_parameters, shard_batch
@@ -17,7 +18,7 @@ from .train_step import FuseFineTuneStep, TrainStep, softmax_cross_entropy
 from .dp import PeerComm
 
 __all__ = [
-    "GRU", "LSTM", "GRUCell", "LSTMCell", "install", "uninstall", "from_torch", "rnn_forward", "gemm", "RNNConfig", "B200RNNError",
+    "GRU", "LSTM", "RNN", "GRUCell", "LSTMCell", "RNNCell", "install", "uninstall", "from_torch", "rnn_forward", "gemm", "RNNConfig", "B200RNNError",
     "AudioBiLSTM", "TextBiLSTM", "fusion_net", "MyLoss", "attention_pool", "FuseBatch", "PinnedStager",
     "stage_fuse_batch", "GradBucket", "broadcast_parameters", "shard_batch", "FusedFuseStep", "FlatAdamW",
     "TrainStep", "FuseFineTuneStep", "softmax_cross_entropy", "PeerComm",

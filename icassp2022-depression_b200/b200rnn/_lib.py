@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200RNN_LIB") or os.path.join(os.path.dirname(_HERE), "lib", "libb200rnn.so")
 
 GRU, LSTM = 0, 1
+RNN_TANH, RNN_RELU = 2, 3   # Elman RNN / RNNCell, nonlinearity tanh / relu
 FLAG_ACCUMULATE_GRADS = 1
 FLAG_SAVE_FOR_BACKWARD = 2
 FLAG_FUSED_LN = 4
@@ -84,7 +85,7 @@ class Desc(ctypes.Structure):
 
 
 class CellDesc(ctypes.Structure):
-    """``b200rnn_cell_desc`` (include/b200rnn.h): one GRUCell / LSTMCell call."""
+    """``b200rnn_cell_desc`` (include/b200rnn.h): one GRUCell / LSTMCell / RNNCell call."""
 
     _fields_ = [
         ("mode", c_int32),

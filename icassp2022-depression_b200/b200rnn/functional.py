@@ -353,13 +353,13 @@ def _initial_state(hx, cfg: RNNConfig, x: torch.Tensor):
 def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig,
                 rng_state: Optional[torch.Tensor] = None, grad_sink=None, lengths: Optional[torch.Tensor] = None,
                 hx=None):
-    """Run the multi-layer GRU/LSTM. ``x`` is [T,B,I] (or [B,T,I] if ``cfg.batch_first``), any strides.
+    """Run the multi-layer GRU / LSTM / Elman RNN. ``x`` is [T,B,I] (or [B,T,I] if ``cfg.batch_first``), any strides.
 
-    ``hx`` is the initial state as torch takes it: None (zeros), ``h_0`` (GRU) or ``(h_0, c_0)`` (LSTM), each
+    ``hx`` is the initial state as torch takes it: None (zeros), ``h_0`` (GRU, RNN) or ``(h_0, c_0)`` (LSTM), each
     [L*D, B, H] with the rows in ``x``'s batch order (also with ``lengths``). It is differentiable: ``dh_0`` / ``dc_0``
     are computed only when autograd asks for them.
 
-    Returns ``(y, h_n)`` for GRU and ``(y, h_n, c_n)`` for LSTM, laid out like torch.nn.GRU/LSTM outputs.
+    Returns ``(y, h_n)`` for GRU and RNN and ``(y, h_n, c_n)`` for LSTM, laid out like torch.nn.GRU/LSTM/RNN outputs.
     """
     h_0, c_0 = _initial_state(hx, cfg, x)
     _require_cuda_f32(x, "input")
@@ -452,7 +452,7 @@ def prepare_weights(weights: Sequence[torch.Tensor], cfg: RNNConfig) -> torch.Te
 
 @dataclass
 class CellConfig:
-    mode: int            # _lib.GRU / _lib.LSTM
+    mode: int            # _lib.GRU / _lib.LSTM / _lib.RNN_TANH / _lib.RNN_RELU
     input_size: int
     hidden_size: int
     bias: bool
@@ -538,7 +538,7 @@ class _CellFunction(torch.autograd.Function):
 
 
 def cell_forward(x: torch.Tensor, hx, weights: Sequence[torch.Tensor], cfg: CellConfig, name: str):
-    """One GRUCell / LSTMCell step on batched input: ``x`` [B, I], ``hx`` None (zeros), ``h`` (GRU) or ``(h, c)``
+    """One GRUCell / LSTMCell / RNNCell step on batched input: ``x`` [B, I], ``hx`` None (zeros), ``h`` (GRU, RNN) or ``(h, c)``
     (LSTM), each [B, H]; ``weights`` = (weight_ih, weight_hh[, bias_ih, bias_hh]). Shapes are checked as torch's
     ``_VF.gru_cell`` / ``_VF.lstm_cell`` check them (same exception types and messages), before the missing CPU path.
     Returns ``h'`` or ``(h', c')``."""

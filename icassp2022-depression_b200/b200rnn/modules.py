@@ -1,4 +1,4 @@
-"""Drop-in ``nn.Module`` mirrors of ``torch.nn.GRU`` / ``torch.nn.LSTM`` backed by the sm_90a kernels.
+"""Drop-in ``nn.Module`` mirrors of ``torch.nn.GRU`` / ``torch.nn.LSTM`` / ``torch.nn.RNN`` backed by the sm_90a kernels.
 
 They keep the constructor signature, parameter names / shapes / registration order
 (``weight_ih_l{k}[_reverse]``, ``weight_hh_...``, ``bias_ih_...``, ``bias_hh_...``; torch rnn.py:171-216), the
@@ -17,6 +17,10 @@ fixed-size kernels, every other size the runtime-sized cluster kernels (csrc/rnn
 ``B200RNNError`` at the first forward. ``LSTM(..., proj_size=P)`` (LSTMP: ``h_t = W_hr (o_t * tanh c_t)``) runs on its own
 projected kernels for P in {H/4, H/2} and registers ``weight_hr_l{k}[_reverse]`` last, as torch does. Features that
 raise ``NotImplementedError``: bias=False, and other projection sizes. A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
+
+``RNN(..., nonlinearity='tanh' | 'relu')`` (the Elman network) takes the same inputs and features at every one of
+those hidden sizes on its own runtime-sized kernels (csrc/rnn_elman.cu); it has no model-shell fusion
+(``forward_ln_sum`` computes it unfused, ``frozen_weight_cache`` is None) and no ``proj_size``.
 """
 from __future__ import annotations
 
@@ -33,6 +37,8 @@ from .functional import (CellConfig, RNNConfig, cell_forward, prepare_weights, r
 
 _TORCH_GRU = nn.GRU
 _TORCH_LSTM = nn.LSTM
+_TORCH_RNN = nn.RNN
+_ELMAN_MODES = {"tanh": _lib.RNN_TANH, "relu": _lib.RNN_RELU}
 _module_counter = 0
 
 
@@ -153,12 +159,12 @@ class _B200RNNBase(nn.Module):
     def frozen_weight_cache(self):
         """TF32-split ``weight_ih`` cache for the no-grad fused forward, or None.
 
-        Only while EVERY weight of the module is frozen (``requires_grad=False``, the fuse scripts' encoders:
+        None for an Elman ``RNN``, whose forward has no fused path. Only while EVERY weight of the module is frozen (``requires_grad=False``, the fuse scripts' encoders:
         fuse_net_whole.py:590-593) - nothing this library launches updates such a tensor behind PyTorch's back. The
         cache is keyed on the parameters' storage addresses and version counters, so ``load_state_dict``, ``.to()`` or
         an in-place edit refresh it; trainable modules never use it (their weights change every step anyway)."""
         ws = self._flat_weights
-        if any(w.requires_grad for w in ws) or not ws[0].is_cuda or self.proj_size:
+        if any(w.requires_grad for w in ws) or not ws[0].is_cuda or self.proj_size or self._gates == 1:
             self._wcache = None
             return None
         key = tuple((w.data_ptr(), w._version) for w in ws)
@@ -231,7 +237,7 @@ class _B200RNNBase(nn.Module):
                        prologue_done: Optional[torch.cuda.Event] = None) -> torch.Tensor:
         """``self(ln(input))[0].sum(dim=time)`` — the audio branch of fuse_net_whole.py:360-362 / fuse_net.py:338-339.
 
-        For hidden sizes 128 and 256 and the widths the tensor-core projection takes, LayerNorm is folded into the layer-0 operand preparation and the
+        For a GRU / LSTM with hidden sizes 128 and 256 and the widths the tensor-core projection takes, LayerNorm is folded into the layer-0 operand preparation and the
         time sum into the last layer's step loop. Without autograd (the reference's fuse scripts run it under
         ``torch.no_grad()``, fuse_net_whole.py:337) the normalised input and the [B,T,H] output never touch HBM; under
         autograd (audio_gru_whole.py:103-108 + loss.backward()) the same fusions run in both directions
@@ -243,7 +249,8 @@ class _B200RNNBase(nn.Module):
         """
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
-        shape_ok = (input.is_cuda and input.dim() == 3 and self.proj_size == 0 and self.hidden_size in (128, 256) and
+        shape_ok = (input.is_cuda and input.dim() == 3 and self.proj_size == 0 and self._gates > 1 and
+                    self.hidden_size in (128, 256) and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and
                                     ln.bias is not None)))
         fusable = not need_grad and shape_ok
@@ -287,8 +294,35 @@ class LSTM(_B200RNNBase):
         return y, (h_n, c_n)
 
 
+class RNN(_B200RNNBase):
+    """``torch.nn.RNN``, the Elman network ``h_t = tanh(W_ih x_t + b_ih + W_hh h_{t-1} + b_hh)`` (or relu), on
+    hand-written sm_90a kernels. Same constructor as torch's, ``nonlinearity`` included (also as the fourth
+    positional argument), with its checks and messages; the ``repr`` does not show the nonlinearity, as torch's
+    does not."""
+
+    _gates = 1
+
+    def __init__(self, input_size: int, hidden_size: int, num_layers: int = 1, nonlinearity: str = "tanh",
+                 bias: bool = True, batch_first: bool = False, dropout: float = 0.0, bidirectional: bool = False,
+                 device=None, dtype=None, **kwargs) -> None:
+        if "proj_size" in kwargs:
+            raise ValueError("proj_size argument is only supported for LSTM, not RNN or GRU")
+        if kwargs:
+            raise TypeError(f"RNN.__init__() got an unexpected keyword argument '{next(iter(kwargs))}'")
+        if nonlinearity not in _ELMAN_MODES:
+            raise ValueError(f"Unknown nonlinearity '{nonlinearity}'. Select from 'tanh' or 'relu'.")
+        self.nonlinearity = nonlinearity
+        self._mode = _ELMAN_MODES[nonlinearity]
+        super().__init__(input_size, hidden_size, num_layers=num_layers, bias=bias, batch_first=batch_first,
+                         dropout=dropout, bidirectional=bidirectional, device=device, dtype=dtype)
+
+    def forward(self, input, hx=None):
+        y, h_n = self._run(input, hx)
+        return y, h_n
+
+
 class _B200CellBase(nn.Module):
-    """``torch.nn.GRUCell`` / ``LSTMCell`` (RNNCellBase): same constructor, parameters (``weight_ih``, ``weight_hh``,
+    """``torch.nn.GRUCell`` / ``LSTMCell`` / ``RNNCell`` (RNNCellBase): same constructor, parameters (``weight_ih``, ``weight_hh``,
     ``bias_ih``, ``bias_hh``, registered as None with ``bias=False``), init, ``extra_repr`` and ``forward``. Any
     ``input_size`` and ``hidden_size``. One fused launch per forward (csrc/cell.cu). Not rebound by :func:`install`:
     use them by name or through :func:`from_torch`."""
@@ -323,6 +357,8 @@ class _B200CellBase(nn.Module):
         s = "{input_size}, {hidden_size}"
         if "bias" in self.__dict__ and self.bias is not True:
             s += ", bias={bias}"
+        if "nonlinearity" in self.__dict__ and self.nonlinearity != "tanh":
+            s += ", nonlinearity={nonlinearity}"
         return s.format(**self.__dict__)
 
     def _step(self, x: torch.Tensor, hx):
@@ -369,9 +405,38 @@ class LSTMCell(_B200CellBase):
         return h.squeeze(0), c.squeeze(0)
 
 
+class RNNCell(_B200CellBase):
+    """``torch.nn.RNNCell`` (the Elman cell, tanh or relu) on the sm_90a cell kernels. As in torch, an unknown
+    ``nonlinearity`` is accepted by the constructor and raises at ``forward``."""
+
+    _gates = 1
+
+    def __init__(self, input_size: int, hidden_size: int, bias: bool = True, nonlinearity: str = "tanh", device=None,
+                 dtype=None) -> None:
+        super().__init__(input_size, hidden_size, bias, device=device, dtype=dtype)
+        self.nonlinearity = nonlinearity
+
+    @property
+    def _mode(self) -> int:
+        if self.nonlinearity not in _ELMAN_MODES:
+            raise RuntimeError(f"Unknown nonlinearity: {self.nonlinearity}")
+        return _ELMAN_MODES[self.nonlinearity]
+
+    def forward(self, input: torch.Tensor, hx: Optional[torch.Tensor] = None) -> torch.Tensor:
+        if input.dim() not in (1, 2):
+            raise ValueError(f"RNNCell: Expected input to be 1D or 2D, got {input.dim()}D instead")
+        if hx is not None and hx.dim() not in (1, 2):
+            raise ValueError(f"RNNCell: Expected hidden to be 1D or 2D, got {hx.dim()}D instead")
+        self._mode  # noqa: B018 - the nonlinearity check, before any shape check, as torch orders them
+        if input.dim() == 2:
+            return self._step(input, hx)
+        return self._step(input.unsqueeze(0), hx.unsqueeze(0) if hx is not None else None).squeeze(0)
+
+
 def install() -> None:
     """Rebind ``torch.nn.GRU`` / ``torch.nn.LSTM`` so unmodified reference code builds the b200rnn modules. The cells
-    are left alone: ``torch.nn.GRUCell`` / ``LSTMCell`` stay stock, so host code using them keeps running."""
+    and the Elman RNN are left alone: ``torch.nn.GRUCell`` / ``LSTMCell`` / ``RNNCell`` / ``RNN`` stay stock, so host
+    code using them keeps running."""
     nn.GRU = GRU
     nn.LSTM = LSTM
     torch.nn.modules.GRU = GRU
@@ -386,8 +451,20 @@ def uninstall() -> None:
 
 
 def from_torch(module: nn.Module) -> nn.Module:
-    """Build the b200rnn twin of a stock ``nn.GRU`` / ``nn.LSTM`` / ``nn.GRUCell`` / ``nn.LSTMCell`` and copy its
-    parameters."""
+    """Build the b200rnn twin of a stock ``nn.GRU`` / ``nn.LSTM`` / ``nn.RNN`` / ``nn.GRUCell`` / ``nn.LSTMCell`` /
+    ``nn.RNNCell`` and copy its parameters (and nonlinearity)."""
+    if isinstance(module, nn.RNNCell):
+        twin = RNNCell(module.input_size, module.hidden_size, bias=module.bias, nonlinearity=module.nonlinearity)
+        twin.load_state_dict(module.state_dict())
+        twin.train(module.training)
+        return twin
+    if isinstance(module, _TORCH_RNN):
+        twin = RNN(module.input_size, module.hidden_size, num_layers=module.num_layers,
+                   nonlinearity=module.nonlinearity, bias=module.bias, batch_first=module.batch_first,
+                   dropout=module.dropout, bidirectional=module.bidirectional)
+        twin.load_state_dict(module.state_dict())
+        twin.train(module.training)
+        return twin
     if isinstance(module, (nn.GRUCell, nn.LSTMCell)):
         twin = (GRUCell if isinstance(module, nn.GRUCell) else LSTMCell)(module.input_size, module.hidden_size,
                                                                          bias=module.bias)
@@ -399,7 +476,7 @@ def from_torch(module: nn.Module) -> nn.Module:
     elif isinstance(module, _TORCH_LSTM):
         cls = LSTM
     else:
-        raise TypeError(f"expected torch.nn.GRU or torch.nn.LSTM, got {type(module)}")
+        raise TypeError(f"expected torch.nn.GRU, torch.nn.LSTM or torch.nn.RNN, got {type(module)}")
     twin = cls(module.input_size, module.hidden_size, num_layers=module.num_layers, bias=module.bias,
                batch_first=module.batch_first, dropout=module.dropout, bidirectional=module.bidirectional,
                proj_size=getattr(module, "proj_size", 0))

@@ -40,9 +40,14 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 inline int desc_proj(const b200rnn_desc* d) { return (d->flags & B200RNN_FLAG_PROJ) ? d->proj_size : 0; }
 
 // The model-shell entry points (b200rnn_forward_fused, _backward_fused, _prepare_weights, _wcache_bytes) run only the
-// fixed hidden sizes 128 and 256: their fusions (LayerNorm prologue, pooling, weight cache, the fp16-pair no-grad
-// recurrence) are built for those
-int check_shell_hidden(const b200rnn_desc* d, const char* what) {
+// GRU / LSTM at the fixed hidden sizes 128 and 256: their fusions (LayerNorm prologue, pooling, weight cache, the
+// fp16-pair no-grad recurrence) are built for those
+int check_shell_desc(const b200rnn_desc* d, const char* what) {
+  if (d && is_elman(d->mode)) {
+    set_error("%s: the model-shell entry points take the GRU and the LSTM (got mode %d; use the _hx entry points)",
+              what, d->mode);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   if (d && d->hidden_size != 128 && d->hidden_size != 256) {
     set_error("%s: the model-shell entry points take hidden_size 128 and 256 (got %d; use the _hx entry points)", what,
               d->hidden_size);
@@ -64,8 +69,8 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
     set_error("null descriptor");
     return B200RNN_ERR_INVALID;
   }
-  if (d->mode != B200RNN_GRU && d->mode != B200RNN_LSTM) {
-    set_error("mode must be B200RNN_GRU or B200RNN_LSTM (got %d)", d->mode);
+  if (d->mode != B200RNN_GRU && d->mode != B200RNN_LSTM && !is_elman(d->mode)) {
+    set_error("mode must be B200RNN_GRU, B200RNN_LSTM, B200RNN_RNN_TANH or B200RNN_RNN_RELU (got %d)", d->mode);
     return B200RNN_ERR_INVALID;
   }
   if (d->batch < 0 || d->seq_len < 0 || d->input_size <= 0 || d->num_layers <= 0 ||
@@ -74,8 +79,8 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
               d->num_dirs);
     return B200RNN_ERR_INVALID;
   }
-  // 128 and 256 run the fixed configs of rnn_rec.cu, every other multiple of 16 up to 1024 the runtime-sized kernels
-  // of rnn_anyh.cu
+  // GRU / LSTM 128 and 256 run the fixed configs of rnn_rec.cu, every other multiple of 16 up to 1024 the runtime-sized
+  // kernels of rnn_anyh.cu; the Elman modes run rnn_elman.cu at every one of them
   if (!anyh_hidden_size(d->hidden_size)) {
     set_error("hidden_size %d unsupported: the sm_90a recurrence kernels take multiples of 16 from 16 to 1024",
               d->hidden_size);
@@ -103,7 +108,7 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
   o->H = d->hidden_size;
   o->L = d->num_layers;
   o->D = d->num_dirs;
-  o->G = d->mode == B200RNN_GRU ? 3 : 4;
+  o->G = gates_of(d->mode);
   o->P = P;
   o->HO = P > 0 ? P : d->hidden_size;
   o->NPAR = P > 0 ? 5 : 4;
@@ -119,7 +124,7 @@ constexpr size_t ALIGN_F = 64;  // floats (256 B)
 
 // ---- reserve layout (floats) ------------------------------------------------------------------
 struct ReserveLayout {
-  size_t gates[8][2], extra[8][2];  // up to 8 layers
+  size_t gates[8][2], extra[8][2];  // up to 8 layers; Elman: gates holds h_t, no extra block
   size_t m[8][2];                   // proj_size > 0: o * tanh(c) of every step, [T,B,H] (operand of dW_hr)
   size_t ylayer[8], ydrop[8];
   size_t xln;  // LayerNorm(x) of the folded prologue, kept for the layer-0 wgrad (B200RNN_FLAG_FUSED_LN)
@@ -137,7 +142,7 @@ int make_reserve(const Dims& d, ReserveLayout* r, bool fused_ln = false) {
       r->gates[l][k] = off;
       off += align_up(d.TB * d.GH, ALIGN_F);
       r->extra[l][k] = off;
-      off += align_up(d.TB * d.H, ALIGN_F);
+      if (!is_elman(d.mode)) off += align_up(d.TB * d.H, ALIGN_F);
       r->m[l][k] = off;
       if (d.P > 0) off += align_up(d.TB * d.H, ALIGN_F);
     }
@@ -382,8 +387,8 @@ int check_cell_desc(const b200rnn_cell_desc* d, CellDims* o) {
     set_error("cell: null descriptor");
     return B200RNN_ERR_INVALID;
   }
-  if (d->mode != B200RNN_GRU && d->mode != B200RNN_LSTM) {
-    set_error("cell: mode must be B200RNN_GRU or B200RNN_LSTM (got %d)", d->mode);
+  if (d->mode != B200RNN_GRU && d->mode != B200RNN_LSTM && !is_elman(d->mode)) {
+    set_error("cell: mode must be B200RNN_GRU, B200RNN_LSTM, B200RNN_RNN_TANH or B200RNN_RNN_RELU (got %d)", d->mode);
     return B200RNN_ERR_INVALID;
   }
   constexpr uint32_t known =
@@ -397,7 +402,7 @@ int check_cell_desc(const b200rnn_cell_desc* d, CellDims* o) {
     set_error("cell: bad shape: B=%d I=%d H=%d (B >= 0, I >= 1, H >= 1)", d->batch, d->input_size, d->hidden_size);
     return B200RNN_ERR_INVALID;
   }
-  const size_t G = d->mode == B200RNN_GRU ? 3 : 4, GH = G * d->hidden_size;
+  const size_t G = gates_of(d->mode), GH = G * d->hidden_size;
   const size_t K = (size_t)(d->input_size > d->hidden_size ? d->input_size : d->hidden_size);
   if (d->batch > CELL_MAX_BATCH || GH * K > 0x7fffffffu || GH * d->batch > 0x7fffffffu ||
       K * d->batch > 0x7fffffffu) {
@@ -420,8 +425,8 @@ int check_cell_desc(const b200rnn_cell_desc* d, CellDims* o) {
   return B200RNN_OK;
 }
 
-// saved state (floats): the activated gates [B][G*H], then GRU W_hn h + b_hn / LSTM c' [B][H], as the sequence path's
-// reserve holds one step
+// saved state (floats): the activated gates [B][G*H] (Elman: h'), then GRU W_hn h + b_hn / LSTM c' [B][H] (Elman:
+// none), as the sequence path's reserve holds one step
 struct CellSaved {
   size_t gates, extra, total;
 };
@@ -429,7 +434,7 @@ struct CellSaved {
 void make_cell_saved(const CellDims& d, CellSaved* s) {
   s->gates = 0;
   s->extra = align_up((size_t)d.B * d.GH, ALIGN_F);
-  s->total = s->extra + align_up((size_t)d.B * d.H, ALIGN_F);
+  s->total = s->extra + (is_elman(d.mode) ? 0 : align_up((size_t)d.B * d.H, ALIGN_F));
 }
 
 // backward scratch (floats): gate gradients, bias partial sums, and the gradient GEMMs' workspaces laid out as the
@@ -679,7 +684,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         return B200RNN_ERR_INVALID;
       }
       float* gates = save ? R + rl.gates[l][k] : S + sl.f_gates[k];
-      // K1: x-projection of every time step at once, biases folded (GRU: b_hh only for r,z)
+      // K1: x-projection of every time step at once, biases folded (GRU: b_hh only for r,z; LSTM, Elman: all of it)
       GemmParams g;
       memset(&g, 0, sizeof(g));
       g.A = a_in; g.a_rows = a_rows; g.a_kcontig = 1;
@@ -687,7 +692,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       g.C = gates; g.c_rows = simple_rows((long long)d.GH);
       g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
       g.bias1 = b_ih; g.bias2 = b_hh;
-      g.bias2_n = d.mode == B200RNN_GRU ? 2 * d.H : 4 * d.H;
+      g.bias2_n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
       if (tc_layer) {
         g.tc_ws = tc_ws;
         g.tc_ws_bytes = sl.f_tc_bytes;
@@ -713,7 +718,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       rp.w_hh[k] = w_hh;
       rp.b_hh[k] = b_hh;
       rp.gates[k] = gates;
-      rp.extra[k] = save ? R + rl.extra[l][k] : nullptr;
+      rp.extra[k] = save && !is_elman(d.mode) ? R + rl.extra[l][k] : nullptr;
       if (d.P > 0) {
         rp.w_hr[k] = pp[4];
         rp.m[k] = save ? R + rl.m[l][k] : nullptr;
@@ -751,8 +756,8 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
 // h_0 / c_0 / dh_0 / dc_0 of the hx entry points: c_0 (dc_0) only for the LSTM, and there c_0 only together with h_0
 static int check_initial_state(const b200rnn_desc* desc, const float* h_0, const void* c_0, const void* dc_0,
                                const char* what) {
-  if (desc && desc->mode == B200RNN_GRU && (c_0 || dc_0)) {
-    set_error("%s: a GRU has no cell state (c_0 / dc_0 must be NULL)", what);
+  if (desc && desc->mode != B200RNN_LSTM && (c_0 || dc_0)) {
+    set_error("%s: a %s has no cell state (c_0 / dc_0 must be NULL)", what, mode_name(desc->mode));
     return B200RNN_ERR_INVALID;
   }
   if (c_0 && !h_0) {
@@ -772,7 +777,7 @@ B200RNN_API int b200rnn_forward_fused(const b200rnn_desc* desc, const float* x, 
     set_error("forward_fused: the model-shell entry points do not take proj_size (use b200rnn_forward_hx)");
     return B200RNN_ERR_UNSUPPORTED;
   }
-  if (check_shell_hidden(desc, "forward_fused")) return B200RNN_ERR_UNSUPPORTED;
+  if (check_shell_desc(desc, "forward_fused")) return B200RNN_ERR_UNSUPPORTED;
   return forward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, h_n, c_n, reserve, scratch, seed, offset, rng_state,
                       ln_gamma, ln_beta, ln_eps, y_pool, lengths, wcache, prologue_done, nullptr, nullptr, true,
                       stream_);
@@ -823,7 +828,7 @@ B200RNN_API int b200rnn_wcache_bytes(const b200rnn_desc* desc, size_t* bytes) {
     set_error("wcache_bytes: the weight cache of b200rnn_forward_fused does not take proj_size");
     return B200RNN_ERR_UNSUPPORTED;
   }
-  if (check_shell_hidden(desc, "wcache_bytes")) return B200RNN_ERR_UNSUPPORTED;
+  if (check_shell_desc(desc, "wcache_bytes")) return B200RNN_ERR_UNSUPPORTED;
   WCacheLayout wl;
   make_wcache(d, &wl);
   if (bytes) *bytes = (wl.total + ALIGN_F) * sizeof(float);
@@ -843,7 +848,7 @@ B200RNN_API int b200rnn_prepare_weights(const b200rnn_desc* desc, const float* c
     set_error("prepare_weights: the weight cache of b200rnn_forward_fused does not take proj_size");
     return B200RNN_ERR_UNSUPPORTED;
   }
-  if (check_shell_hidden(desc, "prepare_weights")) return B200RNN_ERR_UNSUPPORTED;
+  if (check_shell_desc(desc, "prepare_weights")) return B200RNN_ERR_UNSUPPORTED;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   WCacheLayout wl;
   make_wcache(d, &wl);
@@ -952,7 +957,7 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
       bp.w_hh[k] = pp[1];
       bp.w_prep[k] = S + sl.b_wt[k];
       bp.gates[k] = R + rl.gates[l][k];
-      bp.extra[k] = R + rl.extra[l][k];
+      bp.extra[k] = is_elman(d.mode) ? nullptr : R + rl.extra[l][k];
       bp.dgates[k] = S + sl.b_dgates[k];
       bp.dghn[k] = S + sl.b_dghn[k];
       bp.dbias_part[k] = S + sl.b_bpart[k];
@@ -1018,8 +1023,8 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
       }
       if (dw_hh) {
         // dW_hh = sum_t dGh[t]^T h_{prev(t)}: rows are (t,b) flattened time-major, so the one-step shift is a row
-        // offset of B (forward: dG[t] with h[t-1], t = 1..T-1; reverse: dG[t] with h[t+1], t = 0..T-2). LSTM: one GEMM
-        // over all gates; GRU: the r,z rows from columns [0, 2H) of dG, the n rows from dn*r
+        // offset of B (forward: dG[t] with h[t-1], t = 1..T-1; reverse: dG[t] with h[t+1], t = 0..T-2). LSTM, Elman:
+        // one GEMM over all gates; GRU: the r,z rows from columns [0, 2H) of dG, the n rows from dn*r
         const int g0 = k == 0 ? d.B : 0, Kp = (d.T - 1) * d.B;
         // the tensor-core GEMM needs N = H a multiple of 128 (hidden sizes other than 128 / 256 may not be)
         const bool gru = d.mode == B200RNN_GRU,
@@ -1083,7 +1088,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
     set_error("backward_fused: the model-shell entry points do not take proj_size (use b200rnn_backward_hx)");
     return B200RNN_ERR_UNSUPPORTED;
   }
-  if (check_shell_hidden(desc, "backward_fused")) return B200RNN_ERR_UNSUPPORTED;
+  if (check_shell_desc(desc, "backward_fused")) return B200RNN_ERR_UNSUPPORTED;
   return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, dy_pool, dy_pool_scale, dh_n,
                        dc_n, reserve, scratch, dx, dxs_t, dxs_b, dparams, lengths, ln_gamma, ln_eps, dln_gamma,
                        dln_beta, nullptr, nullptr, nullptr, nullptr, stream_);
@@ -1172,7 +1177,7 @@ B200RNN_API int b200rnn_cell_forward(const b200rnn_cell_desc* desc, const float*
   if (rc) return rc;
   const bool lstm = d.mode == B200RNN_LSTM;
   if (!lstm && (c || c_out)) {
-    set_error("cell_forward: a GRU cell has no cell state (c / c_out must be NULL)");
+    set_error("cell_forward: a %s cell has no cell state (c / c_out must be NULL)", mode_name(d.mode));
     return B200RNN_ERR_INVALID;
   }
   if (d.B == 0) return B200RNN_OK;
@@ -1204,7 +1209,7 @@ B200RNN_API int b200rnn_cell_forward(const b200rnn_cell_desc* desc, const float*
   p.w_ih = params[0]; p.w_hh = params[1]; p.b_ih = params[2]; p.b_hh = params[3];
   p.h_out = h_out; p.c_out = c_out;
   p.gates = d.save ? SV + sv.gates : nullptr;
-  p.extra = d.save ? SV + sv.extra : nullptr;
+  p.extra = d.save && !is_elman(d.mode) ? SV + sv.extra : nullptr;
   return launch_cell_fwd(p, static_cast<cudaStream_t>(stream_));
 }
 
@@ -1217,7 +1222,7 @@ B200RNN_API int b200rnn_cell_backward(const b200rnn_cell_desc* desc, const float
   if (rc) return rc;
   const bool lstm = d.mode == B200RNN_LSTM;
   if (!lstm && (c || dc_out || dc)) {
-    set_error("cell_backward: a GRU cell has no cell state (c / dc_out / dc must be NULL)");
+    set_error("cell_backward: a %s cell has no cell state (c / dc_out / dc must be NULL)", mode_name(d.mode));
     return B200RNN_ERR_INVALID;
   }
   if (!dparams) {
@@ -1261,17 +1266,19 @@ B200RNN_API int b200rnn_cell_backward(const b200rnn_cell_desc* desc, const float
   const int accumulate = d.accumulate ? 1 : 0;
   const int B = d.B, I = d.I, H = d.H, G = (int)GH;
 
-  // gate gradients; GRU: dh = z * dh' + dG_h W_hh, the direct term goes to dh first; LSTM: dc is final here
+  // gate gradients; GRU: dh = z * dh' + dG_h W_hh, the direct term goes to dh first; LSTM: dc is final here; Elman:
+  // dh = dpre W_hh, no direct term
   CellBwdParams bp;
   memset(&bp, 0, sizeof(bp));
   bp.mode = d.mode; bp.B = B; bp.H = H;
-  bp.gates = SV + sv.gates; bp.extra = SV + sv.extra;
+  const bool elman = is_elman(d.mode);
+  bp.gates = SV + sv.gates; bp.extra = elman ? nullptr : SV + sv.extra;
   bp.h = h; bp.h_ld = h_ld;
   bp.c = c; bp.c_ld = c_ld;
   bp.dh_out = dh_out; bp.dc_out = dc_out;
   bp.dg_x = S + sc.dgx;
-  bp.dg_h = lstm ? nullptr : S + sc.dgh;
-  bp.direct = lstm ? dc : dh;
+  bp.dg_h = d.mode == B200RNN_GRU ? S + sc.dgh : nullptr;
+  bp.direct = lstm ? dc : elman ? nullptr : dh;
   bp.part = S + sc.part;
   rc = launch_cell_bwd(bp, st);
   if (rc) return rc;
@@ -1284,7 +1291,7 @@ B200RNN_API int b200rnn_cell_backward(const b200rnn_cell_desc* desc, const float
   const bool tc_x = d.tc_x && tc_available(), tc_h = d.tc_h && tc_available();
   GradSrc DGX{S + sc.dgx, simple_rows(G), B, G, S + sc.tc_dgx, false};
   GradSrc DGH_gru{S + sc.dgh, simple_rows(G), B, G, S + sc.tc_dgh, false};
-  GradSrc& DGH = lstm ? DGX : DGH_gru;  // the LSTM's h-part gate gradients are its x-part ones
+  GradSrc& DGH = d.mode == B200RNN_GRU ? DGH_gru : DGX;  // LSTM, Elman: the h-part gate gradients are the x-part ones
   GradSrc X{x, simple_rows(x_ld), B, I, S + sc.tc_x, false};
   GradSrc Hs{h, simple_rows(h_ld), B, H, S + sc.tc_h, false};
   GradSrc WIH{params[0], simple_rows(I), G, I, S + sc.tc_wih, false};
@@ -1308,7 +1315,8 @@ B200RNN_API int b200rnn_cell_backward(const b200rnn_cell_desc* desc, const float
     if (rc) return rc;
   }
   if (dh) {  // dh [B, H] (+)= dG_h W_hh
-    rc = run_grad_gemm({{&DGH, 0, true}, {&WHH, 0, false}, B, H, G, dh, simple_rows(H), lstm ? 0 : 1, false,
+    const int acc_dh = d.mode == B200RNN_GRU ? 1 : 0;  // the GRU's direct term z * dh' is in dh already
+    rc = run_grad_gemm({{&DGH, 0, true}, {&WHH, 0, false}, B, H, G, dh, simple_rows(H), acc_dh, false,
                         tc_h && aligned_to(dh, 16), "cell dh"}, sl, S, d.tf32, st);
     if (rc) return rc;
   }

@@ -1,4 +1,4 @@
-// cell.cu — one-step GRUCell / LSTMCell kernels for sm_90a (torch.nn.GRUCell / LSTMCell, rnn.py).
+// cell.cu — one-step GRUCell / LSTMCell / RNNCell kernels for sm_90a (torch.nn.GRUCell / LSTMCell / RNNCell, rnn.py).
 //
 // Forward, cell_fwd_kernel, one launch per call:
 //   * a CTA owns UNITS = 16 hidden units with all G gate rows of them (one m16 tile per gate) and NB = 8 * ntn batch
@@ -16,6 +16,8 @@
 //   * 4 warps: ntn of them own one n-tile each, the other warps split the k-steps of every stage with them (small
 //     batches stream the weights with all 4 warps); their partial sums meet in shared memory in a fixed order.
 // Backward, cell_bwd_kernel: one elementwise pass over the saved gates (the gradient GEMMs run in api.cu).
+// RNNCell: elman_cell_fwd_kernel runs the same step (cell_fwd) with one gate tile and saves h' alone;
+// elman_cell_bwd_kernel is its elementwise backward (dpre from the saved h').
 #include "cell_kernels.cuh"
 #include "profile.cuh"
 #include "ptx.cuh"
@@ -71,9 +73,11 @@ __device__ __forceinline__ bool vec_rows(const float* p, long long ld) {
   return (reinterpret_cast<uintptr_t>(p) & 15u) == 0 && ld % 4 == 0;
 }
 
+// One cell step of the CTA's units and batch rows, the body of cell_fwd_kernel and elman_cell_fwd_kernel. MODE
+// B200RNN_RNN_TANH stands for both Elman modes: the nonlinearity is read from p.mode (warp-uniform).
 template <int MODE, bool TF32>
-__global__ void __launch_bounds__(NT) cell_fwd_kernel(const CellFwdParams p, const int ntn) {
-  constexpr int G = MODE == B200RNN_GRU ? 3 : 4;
+__device__ __forceinline__ void cell_fwd(const CellFwdParams& p, const int ntn) {
+  constexpr int G = gates_of(MODE);
   extern __shared__ __align__(16) float smem[];
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   const int kw = NWARP / ntn;              // warps per n-tile, splitting the k-steps of a stage
@@ -200,7 +204,7 @@ __global__ void __launch_bounds__(NT) cell_fwd_kernel(const CellFwdParams p, con
       const float bi = p.b_ih ? p.b_ih[g * H + j] : 0.f;
       const float bh = p.b_hh ? p.b_hh[g * H + j] : 0.f;
       // as the sequence path's input projection folds them: b_ih, and b_hh except the GRU's n block
-      const bool fold = MODE == B200RNN_LSTM || g < 2;
+      const bool fold = MODE != B200RNN_GRU || g < 2;
       gi[g] = fold ? accx[g][i] + bi + bh : accx[g][i] + bi;
       if (!fold) bhn = bh;
       pre[g] = acch[g][i];
@@ -214,7 +218,7 @@ __global__ void __launch_bounds__(NT) cell_fwd_kernel(const CellFwdParams p, con
         gp[0] = st.r; gp[H] = st.z; gp[2 * H] = st.n;
         p.extra[(size_t)b * H + j] = st.hn;
       }
-    } else {
+    } else if constexpr (MODE == B200RNN_LSTM) {
       const float cp = p.c ? p.c[(long long)b * p.c_ld + j] : 0.f;
       const LstmStep st = lstm_cell_fwd(gi, pre, cp);
       p.h_out[(size_t)b * H + j] = st.h;
@@ -223,8 +227,23 @@ __global__ void __launch_bounds__(NT) cell_fwd_kernel(const CellFwdParams p, con
         gp[0] = st.i; gp[H] = st.f; gp[2 * H] = st.g; gp[3 * H] = st.o;
         p.extra[(size_t)b * H + j] = st.c;
       }
+    } else {  // Elman: h' alone is saved
+      const float h = elman_cell_fwd(gi[0], pre[0], p.mode == B200RNN_RNN_RELU);
+      p.h_out[(size_t)b * H + j] = h;
+      if (gp) gp[0] = h;
     }
   }
+}
+
+template <int MODE, bool TF32>
+__global__ void __launch_bounds__(NT) cell_fwd_kernel(const CellFwdParams p, const int ntn) {
+  cell_fwd<MODE, TF32>(p, ntn);
+}
+
+// RNNCell, tanh or relu (p.mode)
+template <bool TF32>
+__global__ void __launch_bounds__(NT) elman_cell_fwd_kernel(const CellFwdParams p, const int ntn) {
+  cell_fwd<B200RNN_RNN_TANH, TF32>(p, ntn);
 }
 
 // thread = unit j of slice blockIdx.y (BWD_ROWS batch rows), rows in increasing order: the bias partial sums are
@@ -268,6 +287,22 @@ __global__ void __launch_bounds__(128) cell_bwd_kernel(const CellBwdParams p) {
   for (int g = 0; g <= G; ++g) part[g * H] = bsum[g];
 }
 
+// thread = unit j of slice blockIdx.y (BWD_ROWS batch rows), rows in increasing order; part is [slices][H]
+__global__ void __launch_bounds__(128) elman_cell_bwd_kernel(const CellBwdParams p) {
+  const int H = p.H, j = blockIdx.x * 128 + threadIdx.x;
+  if (j >= H) return;
+  const bool relu = p.mode == B200RNN_RNN_RELU;
+  const int slice = blockIdx.y, bend = min(p.B, (slice + 1) * BWD_ROWS);
+  float bsum = 0.f;
+  for (int b = slice * BWD_ROWS; b < bend; ++b) {
+    const float dh = p.dh_out ? p.dh_out[(size_t)b * H + j] : 0.f;
+    const float dg = elman_cell_bwd(p.gates[(size_t)b * H + j], dh, relu);
+    p.dg_x[(size_t)b * H + j] = dg;
+    bsum += dg;
+  }
+  p.part[(size_t)slice * H + j] = bsum;
+}
+
 }  // namespace
 
 int launch_cell_fwd(const CellFwdParams& p, cudaStream_t stream) {
@@ -275,10 +310,10 @@ int launch_cell_fwd(const CellFwdParams& p, cudaStream_t stream) {
   const int ntn = p.B <= 8 ? 1 : p.B <= 16 ? 2 : 4;
   const dim3 grid((p.H + UNITS - 1) / UNITS, (p.B + 8 * ntn - 1) / (8 * ntn));
   const bool gru = p.mode == B200RNN_GRU;
-  void (*k)(const CellFwdParams, int) = gru ? (p.tf32 ? cell_fwd_kernel<B200RNN_GRU, true>
-                                                      : cell_fwd_kernel<B200RNN_GRU, false>)
-                                            : (p.tf32 ? cell_fwd_kernel<B200RNN_LSTM, true>
-                                                      : cell_fwd_kernel<B200RNN_LSTM, false>);
+  void (*k)(const CellFwdParams, int) =
+      is_elman(p.mode) ? (p.tf32 ? elman_cell_fwd_kernel<true> : elman_cell_fwd_kernel<false>)
+      : gru            ? (p.tf32 ? cell_fwd_kernel<B200RNN_GRU, true> : cell_fwd_kernel<B200RNN_GRU, false>)
+                       : (p.tf32 ? cell_fwd_kernel<B200RNN_LSTM, true> : cell_fwd_kernel<B200RNN_LSTM, false>);
   k<<<grid, NT, FWD_SMEM, stream>>>(p, ntn);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
@@ -290,7 +325,9 @@ int cell_bwd_slices(int B) { return (B + BWD_ROWS - 1) / BWD_ROWS; }
 int launch_cell_bwd(const CellBwdParams& p, cudaStream_t stream) {
   ProfScope prof(PROF_MISC, stream);
   const dim3 grid((p.H + 127) / 128, cell_bwd_slices(p.B));
-  if (p.mode == B200RNN_GRU)
+  if (is_elman(p.mode))
+    elman_cell_bwd_kernel<<<grid, 128, 0, stream>>>(p);
+  else if (p.mode == B200RNN_GRU)
     cell_bwd_kernel<B200RNN_GRU><<<grid, 128, 0, stream>>>(p);
   else
     cell_bwd_kernel<B200RNN_LSTM><<<grid, 128, 0, stream>>>(p);

@@ -40,6 +40,14 @@ inline int current_device() {
   return (d < 0 || d >= MAX_DEVICES) ? 0 : d;
 }
 
+// ---- recurrent modes ------------------------------------------------------------------------------
+// gate blocks of the cell: GRU r, z, n; LSTM i, f, g, o; Elman one (the pre-activation)
+constexpr int gates_of(int mode) { return mode == B200RNN_GRU ? 3 : mode == B200RNN_LSTM ? 4 : 1; }
+constexpr bool is_elman(int mode) { return mode == B200RNN_RNN_TANH || mode == B200RNN_RNN_RELU; }
+inline const char* mode_name(int mode) {
+  return mode == B200RNN_GRU ? "GRU" : mode == B200RNN_LSTM ? "LSTM" : mode == B200RNN_RNN_TANH ? "RNN_TANH" : "RNN_RELU";
+}
+
 // ---- two-level row addressing ------------------------------------------------------------------
 // A logical row index r = outer*inner_n + inner maps to element offset
 //   outer*s_outer + inner*s_inner.

@@ -131,6 +131,25 @@ __global__ void bias_reduce_kernel(const float* __restrict__ part, int nslices, 
   if (db_hh) db_hh[c] = accumulate ? db_hh[c] + hh : hh;
 }
 
+// Elman: db_ih = db_hh = the column sums of the per-slice partials [nslices][H] of dpre, in the same fixed order
+__global__ void elman_bias_reduce_kernel(const float* __restrict__ part, int nslices, int H, float* db_ih,
+                                         float* db_hh, int accumulate) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= H) return;
+  float s = 0.f;
+  int k = 0;
+  for (; k + 8 <= nslices; k += 8) {
+    float v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) v[u] = part[(size_t)(k + u) * H + c];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) s += v[u];
+  }
+  for (; k < nslices; ++k) s += part[(size_t)k * H + c];
+  if (db_ih) db_ih[c] = accumulate ? db_ih[c] + s : s;
+  if (db_hh) db_hh[c] = accumulate ? db_hh[c] + s : s;
+}
+
 }  // namespace
 
 int launch_rng_setup(uint64_t* hdr, uint64_t seed, uint64_t offset, uint64_t* state_dev, uint64_t consume,
@@ -165,6 +184,14 @@ int launch_length_order(const int* lengths, int B, int* order, cudaStream_t stre
 
 int launch_initial_state_rows(const float* dgates, const float* dghn, int mode, int B, int T, int H, bool reverse,
                               const int* lengths, float* out, cudaStream_t stream) {
+  if (is_elman(mode)) {  // G*H = H columns and no GRU n block: the LSTM rows of the kernel, H / 4 units per gate
+    if (H % 4) {
+      set_error("initial_state_rows: Elman hidden_size %d is not a multiple of 4", H);
+      return B200RNN_ERR_INVALID;
+    }
+    mode = B200RNN_LSTM;
+    H /= 4;
+  }
   const size_t n = (size_t)B * (mode == B200RNN_GRU ? 3 : 4) * H;
   if (n == 0) return B200RNN_OK;
   int blocks = (int)((n + 255) / 256);
@@ -189,6 +216,12 @@ int launch_valid_rows(const float* src, const RowMap& rows, int T, int B, int C,
 
 int launch_bias_reduce(const float* part, int nslices, int mode, int H, float* db_ih, float* db_hh,
                        int accumulate, cudaStream_t stream) {
+  if (is_elman(mode)) {
+    elman_bias_reduce_kernel<<<(H + 127) / 128, 128, 0, stream>>>(part, nslices, H, db_ih, db_hh, accumulate);
+    B200_CUDA_CHECK(cudaGetLastError());
+    count_launch();
+    return B200RNN_OK;
+  }
   const int G = mode == B200RNN_GRU ? 3 : 4;
   const int GH = G * H;
   bias_reduce_kernel<<<(GH + 127) / 128, 128, 0, stream>>>(part, nslices, mode, H, db_ih, db_hh, accumulate);

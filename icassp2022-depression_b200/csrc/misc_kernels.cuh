@@ -22,7 +22,7 @@ int launch_length_order(const int* lengths, int B, int* order, cudaStream_t stre
 
 // The recurrent-side gate gradient of each row's first scanned step, the rows the initial state's dW_hh term pairs
 // with h_0: out[b][c] = dGh[t_first(b)][b][c] over c < G*H, where dGh is dgates [T,B,G*H] (the GRU's n columns come
-// from dghn [T,B,H] instead). t_first = 0 forward; reverse: T - 1, or lengths[b] - 1 (a row of length 0: zeros).
+// from dghn [T,B,H] instead; an Elman row is its H dpre columns). t_first = 0 forward; reverse: T - 1, or lengths[b] - 1 (a row of length 0: zeros).
 int launch_initial_state_rows(const float* dgates, const float* dghn, int mode, int B, int T, int H, bool reverse,
                               const int* lengths, float* out, cudaStream_t stream);
 
@@ -36,6 +36,7 @@ int launch_valid_rows(const float* src, const RowMap& rows, int T, int B, int C,
 //   part [nslices][(G+1)*H]  (first G*H: sum of dGi columns; tail H: GRU sum of dn*r)
 //   GRU : db_ih = sum(part[:, :3H]);  db_hh = (sum part[:, :2H], sum part[:, 3H:4H])
 //   LSTM: db_ih = db_hh = sum(part[:, :4H])
+//   Elman: part [nslices][H] (sum of dpre); db_ih = db_hh = sum(part)
 int launch_bias_reduce(const float* part, int nslices, int mode, int H, float* db_ih, float* db_hh,
                        int accumulate, cudaStream_t stream);
 

@@ -1,6 +1,6 @@
-// rnn_cell.cuh — the gate math of one GRU / LSTM step, shared by the persistent recurrence kernels (rnn_rec.cu) and
-// the one-step cell kernels (cell.cu), so that a cell and a sequence step apply the same non-linearities in the same
-// order. Gate order as in torch/nn/modules/rnn.py: GRU r, z, n; LSTM i, f, g, o.
+// rnn_cell.cuh — the gate math of one GRU / LSTM / Elman step, shared by the persistent recurrence kernels (rnn_rec.cu,
+// rnn_anyh.cu, rnn_elman.cu) and the one-step cell kernels (cell.cu), so that a cell and a sequence step apply the same
+// non-linearities in the same order. Gate order as in torch/nn/modules/rnn.py: GRU r, z, n; LSTM i, f, g, o.
 #pragma once
 #include "common.cuh"
 
@@ -65,6 +65,19 @@ __device__ __forceinline__ float lstm_cell_bwd(const float (&sv)[4], float c_t, 
   dg[2] = dc * ig * (1.f - gg * gg);
   dg[3] = dout;
   return dc * fg;
+}
+
+// The Elman cell, forward: gi = x-projection with b_ih + b_hh folded in, pre = W_hh h. Returns h = tanh(gi + pre) (the
+// tanh of the GRU n gate) or relu(gi + pre); a NaN pre-activation stays NaN, as torch.relu keeps it
+__device__ __forceinline__ float elman_cell_fwd(float gi, float pre, bool relu) {
+  const float a = gi + pre;
+  return relu ? (a < 0.f ? 0.f : a) : tanh_f(a);
+}
+
+// The Elman cell, backward: from the saved output h and its gradient dh, the gradient of the pre-activation (relu:
+// torch's threshold_backward on the output, dh where h > 0)
+__device__ __forceinline__ float elman_cell_bwd(float h, float dh, bool relu) {
+  return relu ? (h > 0.f ? dh : 0.f) : dh * (1.f - h * h);
 }
 
 }  // namespace b200rnn

@@ -14,7 +14,7 @@ struct RecFwdParams {
   const float* w_hh[2];      // per direction [G*H, H]
   const float* b_hh[2];      // per direction [G*H]  (GRU: only the n third is read; r,z are pre-folded)
   float* gates[2];           // per direction [T,B,G*H]; in: x-projection + folded biases; out: activated gates
-  float* extra[2];           // per direction [T,B,H]; GRU: W_hn h + b_hn ; LSTM: c_t   (training only)
+  float* extra[2];           // per direction [T,B,H]; GRU: W_hn h + b_hn ; LSTM: c_t   (training only; Elman: none)
   float* y;                  // layer output, element (t,b,d*H+j) at t*y_st + b*y_sb + d*H + j (NULL: not written)
   long long y_st, y_sb;
   float* y_pool;             // optional [B, D*H]: sum over t of the layer output (fused pooling epilogue)
@@ -75,7 +75,8 @@ struct RecBwdParams {
   const float* dc_n;         // [D,B,H] or NULL
   float* dgates[2];          // out: [T,B,G*H] gradient w.r.t. the x-projection (dGi)
   float* dghn[2];            // out (GRU only): [T,B,H] gradient w.r.t. (W_hn h + b_hn) = dn * r
-  float* dbias_part[2];      // out: [nslices][(G+1)*H] per-slice column sums (rows 0..G*H: dGi; GRU tail H: dghn)
+  float* dbias_part[2];      // out: [nslices][(G+1)*H] per-slice column sums (rows 0..G*H: dGi; GRU tail H: dghn);
+                             //      Elman: [nslices][H], the sums of dpre
   int nslices_out;           // filled by the launcher
   const int* lengths;        // optional [B], as in the forward
   const int* order;          // with lengths: [B] row of each batch slot, as in the forward
@@ -96,8 +97,9 @@ constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_90
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)
 int rec_bwd_max_slices(int B);
 
-// The runtime-sized recurrence (rnn_anyh.cu): the hidden sizes it takes (H % 16 == 0, 16 <= H <= 1024), its config
-// choice for the shapes the fixed configs do not cover, and its W_hh transpose for the backward (any H)
+// The runtime-sized recurrence (rnn_anyh.cu, rnn_elman.cu): the hidden sizes it takes (H % 16 == 0, 16 <= H <= 1024),
+// its config choice for the GRU / LSTM shapes the fixed configs do not cover and for every Elman shape, and its W_hh
+// transpose for the backward (any H)
 bool anyh_hidden_size(int H);
 int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* out);
 int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out);

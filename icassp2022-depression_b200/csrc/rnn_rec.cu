@@ -57,9 +57,6 @@ constexpr bool kLocalSelf = true;
 #endif
 constexpr unsigned FULLMASK = 0xffffffffu;
 
-// gate blocks of the cell: GRU r, z, n; LSTM i, f, g, o
-constexpr int gates_of(int mode) { return mode == B200RNN_GRU ? 3 : 4; }
-
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
 struct RecCfg {
   static constexpr int G = gates_of(MODE);
@@ -1774,6 +1771,8 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
               "proj_size hidden_size/4 or hidden_size/2", p.mode, p.H, p.P);
     return B200RNN_ERR_UNSUPPORTED;
   }
+  // the Elman modes run the runtime-sized kernels at every hidden size, 128 and 256 included (rnn_elman.cu)
+  if (is_elman(p.mode)) return plan_anyh_fwd(p, L);
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
   if (p.mode == B200RNN_GRU && p.H == 256) {
@@ -1827,6 +1826,7 @@ int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
     set_error("recurrence backward: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d)", p.mode, p.H, p.P);
     return B200RNN_ERR_UNSUPPORTED;
   }
+  if (is_elman(p.mode)) return plan_anyh_bwd(p, L);
   // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
   // (not the weights) dominates the shared-memory traffic of the backward contraction
   if (p.mode == B200RNN_GRU && p.H == 256) {

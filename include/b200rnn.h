@@ -39,7 +39,9 @@ extern "C" {
 #define B200RNN_API
 #endif
 
-enum { B200RNN_GRU = 0, B200RNN_LSTM = 1 };
+/* recurrent cell: GRU, LSTM, or the Elman network h' = act(W_ih x + b_ih + W_hh h + b_hh), act tanh or relu
+ * (torch.nn.RNN / RNNCell nonlinearity='tanh' / 'relu'; one gate block, G = 1) */
+enum { B200RNN_GRU = 0, B200RNN_LSTM = 1, B200RNN_RNN_TANH = 2, B200RNN_RNN_RELU = 3 };
 
 /* error codes */
 enum {
@@ -71,7 +73,9 @@ enum {
  * (rnn.py:1212 / :833) plus the call-time batch shape.
  */
 typedef struct b200rnn_desc {
-  int32_t mode;        /* B200RNN_GRU (gate order r,z,n) or B200RNN_LSTM (gate order i,f,g,o) */
+  int32_t mode;        /* B200RNN_GRU (gate order r,z,n), B200RNN_LSTM (gate order i,f,g,o) or
+                          B200RNN_RNN_TANH / _RELU (one block, G = 1; the _fused entry points and the weight cache
+                          return B200RNN_ERR_UNSUPPORTED for them)                         */
   int32_t batch;       /* B */
   int32_t seq_len;     /* T */
   int32_t input_size;  /* I  (layer-0 feature width)                                        */
@@ -253,7 +257,7 @@ B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x,
 #define B200RNN_FLAG_NO_BIAS 32u /* cells only: bias=False, the bias pointers are NULL (and dbias skipped) */
 
 typedef struct b200rnn_cell_desc {
-  int32_t mode;        /* B200RNN_GRU (gate order r,z,n) or B200RNN_LSTM (gate order i,f,g,o) */
+  int32_t mode;        /* B200RNN_GRU, B200RNN_LSTM, B200RNN_RNN_TANH or B200RNN_RNN_RELU (G = 3, 4, 1) */
   int32_t batch;       /* B (0 allowed)                                                       */
   int32_t input_size;  /* I >= 1                                                              */
   int32_t hidden_size; /* H >= 1                                                              */
