@@ -19,7 +19,7 @@ projected kernels for P in {H/4, H/2} and registers ``weight_hr_l{k}[_reverse]``
 raise ``NotImplementedError``: bias=False, and other projection sizes. A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
 
 ``RNN(..., nonlinearity='tanh' | 'relu')`` (the Elman network) takes the same inputs and features at every one of
-those hidden sizes on its own runtime-sized kernels (csrc/rnn_elman.cu); it has no model-shell fusion
+those hidden sizes on the runtime-sized kernels (csrc/rnn_anyh.cu, one gate block); it has no model-shell fusion
 (``forward_ln_sum`` computes it unfused, ``frozen_weight_cache`` is None) and no ``proj_size``.
 """
 from __future__ import annotations

@@ -80,7 +80,7 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
     return B200RNN_ERR_INVALID;
   }
   // GRU / LSTM 128 and 256 run the fixed configs of rnn_rec.cu, every other multiple of 16 up to 1024 the runtime-sized
-  // kernels of rnn_anyh.cu; the Elman modes run rnn_elman.cu at every one of them
+  // kernels of rnn_anyh.cu; the Elman modes run those at every one of them
   if (!anyh_hidden_size(d->hidden_size)) {
     set_error("hidden_size %d unsupported: the sm_90a recurrence kernels take multiples of 16 from 16 to 1024",
               d->hidden_size);

@@ -1,6 +1,9 @@
-// rnn_anyh.cu — the GRU / LSTM recurrence, forward and BPTT, at every hidden size H % 16 == 0, 16 <= H <= 1024 that the
-// fixed configs of rnn_rec.cu (H = 128, 256) do not cover. H, the cluster width C and the batch rows per cluster BS are
-// known only at run time; the kernels are templated on the mode, ragged batches (VL) and where W_hh lives (ONCHIP).
+// rnn_anyh.cu — the runtime-sized recurrence, forward and BPTT, at every hidden size H % 16 == 0, 16 <= H <= 1024: the
+// GRU / LSTM at the sizes the fixed configs of rnn_rec.cu (H = 128, 256) do not cover, and the Elman RNN
+// (torch.nn.RNN, nonlinearity 'tanh' or 'relu') at all of them. H, the cluster width C and the batch rows per cluster BS
+// are known only at run time; the kernels are templated on the mode, ragged batches (VL) and where W_hh lives (ONCHIP).
+// The Elman kernels are instantiated once, as B200RNN_RNN_TANH, with one gate block (G = 1); the nonlinearity is the
+// warp-uniform runtime flag p.mode.
 //
 // Same launch shape and contract as rec_fwd_kernel / rec_bwd_kernel (rnn_kernels.cuh): grid = D * nslices clusters of C
 // CTAs, cluster = one direction of BS batch slots. The H / 8 groups of 8 units are split as evenly as possible over the
@@ -9,7 +12,7 @@
 // (unit u, batch slot b), 8 consecutive units by BS slots per group of 8 * BS threads (the projected kernels'
 // proj_thread), NT = HS * BS rounded up to whole warps; threads past the CTA's units are idle.
 //   * Weights: ONCHIP, the CTA's G * n rows (forward: W_hh[g*H + j0 + u][:]; backward: W_hh[g*H + :][j0 + u], the
-//     w_prep slice of anyh_prep_kernel) are staged once into shared memory, rows padded to H + 4 floats so that the 8
+//     w_prep slice of whh_prep_kernel) are staged once into shared memory, rows padded to H + 4 floats so that the 8
 //     units a quarter-warp reads with one 16-byte load sit in different banks. Otherwise (the L2 tier) the same rows are
 //     read from global memory every step: weight_hh in place in the forward, w_prep in the backward.
 //   * Step: G fixed-order FFMA chains of length H per thread (k ascending), the cell of rnn_cell.cuh, then the CTA's
@@ -17,18 +20,143 @@
 //     into its own buffer with ordinary stores (published by __syncthreads) and sent to the C - 1 peers with st.async,
 //     which completes transaction bytes on the destination's mbarrier of that source and buffer. Double buffered:
 //     step s contracts against what step s - 1 sent (the ExchangeBars protocol of rnn_rec.cu with LAG = 1).
+//   * Elman: the forward saves the activated h_t as its one gate block and nothing in `extra`; the backward takes
+//     dpre = dh (1 - h^2) for tanh, dh [h > 0] for relu from that saved h_t (elman_cell_bwd).
 //   * The waits are bounded: a protocol bug traps (a CUDA error) instead of hanging the GPU.
-#include <map>
-#include <mutex>
+#include <stdint.h>
 #include <stdlib.h>
-#include <tuple>
 
-#include "anyh_core.cuh"
+#include "ptx.cuh"
 #include "rnn_cell.cuh"
+#include "rnn_kernels.cuh"
 
 namespace b200rnn {
 
 namespace {
+
+constexpr int ANYH_MAX_NT = 512;  // 128 registers per thread: the step keeps G accumulators and G + 1 float4 loads in flight
+
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+  return r;
+}
+
+// mbarrier phase wait that gives up after ~2^24 polls (seconds): a lost exchange becomes a trap, not a hang
+__device__ __forceinline__ void bounded_wait(uint64_t* bar, uint32_t parity) {
+  for (uint32_t n = 0; !ptx::mbar_try_wait(bar, parity); ++n)
+    if (n > (1u << 24)) __trap();
+}
+
+// What a CTA owns, derived from the launch: C from the cluster, its units from anyh_units, BS = ceil(B / nslices) batch
+// slots (at most the BS the host planned with: the shared-memory layout uses this one). Threads whose unit is past the
+// CTA's n units (a partial last warp, or a CTA with fewer units than the widest) are idle: they take unit 0's operands,
+// meet every barrier, and store nothing.
+struct AnyhSlice {
+  int C, HS, BS, NT;  // HS: units of the widest CTA (the row count of W_s)
+  uint32_t rank;
+  int dir, slice, b0, j0, n, T;  // units [j0, j0 + n); T: steps the cluster runs (VL: its longest row's)
+  int u, b;                      // this thread's unit (within the slice; 0 when idle) and batch slot
+  bool active;
+};
+
+template <bool VL, typename Params>
+__device__ __forceinline__ AnyhSlice anyh_slice(const Params& p, int nslices) {
+  AnyhSlice s;
+  s.C = (int)cluster_nctarank();
+  s.HS = anyh_max_units(p.H, s.C);
+  s.NT = (int)blockDim.x;
+  s.BS = (p.B + nslices - 1) / nslices;
+  s.rank = ptx::cluster_ctarank();
+  const int cid = blockIdx.x / s.C;
+  s.dir = cid / nslices;
+  s.slice = cid - s.dir * nslices;
+  s.b0 = s.slice * s.BS;
+  anyh_units(p.H, s.C, (int)s.rank, s.j0, s.n);
+  s.T = VL ? min(max(p.lengths[p.order[s.b0]], 0), p.T) : p.T;
+  const int tid = threadIdx.x;
+  s.u = (tid & 7) + 8 * (tid / (8 * s.BS));
+  s.b = (tid >> 3) % s.BS;
+  s.active = s.u < s.n;
+  if (!s.active) s.u = 0;
+  return s;
+}
+
+// Thread 0: the [2][C] exchange barriers, one arrival (the local arm) per phase
+__device__ __forceinline__ void init_bars(uint64_t* bars, int C) {
+  for (int i = 0; i < 2 * C; ++i) ptx::mbar_init(&bars[i], 1u);
+  ptx::fence_mbar_init();
+}
+
+// Thread 0: buffer `buf` expects from every peer its slice: BS rows of NB blocks of its units
+__device__ __forceinline__ void arm_bars(uint64_t* bars, int buf, const AnyhSlice& s, int H, int NB) {
+  for (int src = 0; src < s.C; ++src) {
+    if ((uint32_t)src == s.rank) continue;
+    int j0, n;
+    anyh_units(H, s.C, src, j0, n);
+    ptx::mbar_arrive_expect_tx(&bars[buf * s.C + src], (uint32_t)(s.BS * NB * n * sizeof(float)));
+  }
+}
+
+// Every thread: the peers' slices of buffer `buf` have landed
+__device__ __forceinline__ void wait_bars(uint64_t* bars, int buf, int C, uint32_t rank, uint32_t parity) {
+  for (int src = 0; src < C; ++src)
+    if ((uint32_t)src != rank) bounded_wait(&bars[buf * C + src], parity);
+}
+
+// Send this CTA's slice of buffer `vec` (BS rows of `width` floats, NB blocks of its n units from column j0 + k * H of
+// each row) to the same place in every peer, completing the bytes on the peer's barrier `bar` (this CTA's source slot)
+__device__ __forceinline__ void send_slice(float* vec, int width, int NB, int H, const AnyhSlice& s, uint64_t* bar) {
+  const int per_row = NB * s.n / 4;  // 16-byte chunks of one row
+  const int n = s.BS * per_row;
+  const uint32_t bar_addr = ptx::smem_u32(bar);
+  for (int i = threadIdx.x; i < (s.C - 1) * n; i += s.NT) {
+    const int r = i / n, v = i - r * n;
+    const int q = v / per_row, c = v - q * per_row;
+    const int blk = c / (s.n / 4), e = c - blk * (s.n / 4);
+    float* src = vec + (size_t)q * width + s.j0 + blk * H + e * 4;
+    const uint32_t peer = (s.rank + 1 + (uint32_t)r) % (uint32_t)s.C;
+    ptx::st_async_v4(ptx::mapa(ptx::smem_u32(src), peer), *reinterpret_cast<const float4*>(src),
+                     ptx::mapa(bar_addr, peer));
+  }
+}
+
+// acc[g] += sum_k w[g * wg + k] * v[g * vg + k], k ascending (one FMA chain per gate: deterministic); vg = 0 in the
+// forward (one state row), H in the backward (gate block g of the gradient row). w from shared memory or, in the L2
+// tier, from global memory (read-only for the whole launch)
+template <int G, bool ONCHIP, bool PER_GATE_V>
+__device__ __forceinline__ void dot_rows(const float* __restrict__ w, size_t wg, const float* __restrict__ v, int vg,
+                                         int K, float (&acc)[G]) {
+  // the backward loads G gradient vectors per k, the L2-tier LSTM forward four global rows: no deeper, or they spill
+  constexpr int UNROLL = PER_GATE_V ? 1 : (G == 4 && !ONCHIP) ? 2 : 4;
+#pragma unroll UNROLL
+  for (int k = 0; k < K; k += 4) {
+    float4 x = *reinterpret_cast<const float4*>(v + k);
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      if (PER_GATE_V && g > 0) x = *reinterpret_cast<const float4*>(v + g * vg + k);
+      const float4 a = ONCHIP ? *reinterpret_cast<const float4*>(w + g * wg + k)
+                              : __ldg(reinterpret_cast<const float4*>(w + g * wg + k));
+      float r = acc[g];
+      r = fmaf(a.x, x.x, r);
+      r = fmaf(a.y, x.y, r);
+      r = fmaf(a.z, x.z, r);
+      r = fmaf(a.w, x.w, r);
+      acc[g] = r;
+    }
+  }
+}
+
+// Stage rows r = 0 .. rows-1 of length H (row r at src + rowoff(r)) into W_s[r][H + 4]
+template <typename RowOff>
+__device__ __forceinline__ void stage_rows(float* W_s, const float* __restrict__ src, int rows, int H, int NT,
+                                           RowOff rowoff) {
+  const int q4 = H / 4, LD = H + 4;
+  for (int i = threadIdx.x; i < rows * q4; i += NT) {
+    const int r = i / q4, k = (i - r * q4) * 4;
+    *reinterpret_cast<float4*>(&W_s[(size_t)r * LD + k]) = __ldg(reinterpret_cast<const float4*>(src + rowoff(r) + k));
+  }
+}
 
 // =================================================================================================
 // forward
@@ -36,8 +164,9 @@ namespace {
 // Shared memory: [W_s: G*n x (H+4), ONCHIP only] [h: 2 x BS x H] [bars: 2 x C]
 template <int MODE, bool VL, bool ONCHIP>
 __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdParams p, const int nslices) {
-  constexpr int G = MODE == B200RNN_GRU ? 3 : 4;
+  constexpr int G = gates_of(MODE);
   const int H = p.H, B = p.B, LD = H + 4;
+  const bool relu = p.mode == B200RNN_RNN_RELU;  // Elman
   const AnyhSlice s = anyh_slice<VL>(p, nslices);
   const int C = s.C, HS = s.HS, BS = s.BS, NT = s.NT, dir = s.dir, b0 = s.b0, j0 = s.j0, n = s.n, T = s.T;
   const uint32_t rank = s.rank;
@@ -49,8 +178,12 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
   const float* w_hh = p.w_hh[dir];
 
   if (tid == 0) init_bars(bars, C);
-  if constexpr (ONCHIP)
-    stage_rows(W_s, w_hh, G * n, H, NT, [&](int r) { return ((size_t)(r / n) * H + j0 + r % n) * H; });
+  if constexpr (ONCHIP) {
+    if constexpr (G == 1)
+      stage_rows(W_s, w_hh, n, H, NT, [&](int r) { return (size_t)(j0 + r) * H; });
+    else
+      stage_rows(W_s, w_hh, G * n, H, NT, [&](int r) { return ((size_t)(r / n) * H + j0 + r % n) * H; });
+  }
   for (int i = tid; i < BS * H; i += NT) {  // buffer 0: h_0 of the cluster's slots (zeros past the batch / without h_0)
     const int q = i / H, k = i - q * H;
     const int slot = b0 + q;
@@ -70,6 +203,8 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
   float c = (MODE == B200RNN_LSTM && p.c_0 && valid) ? p.c_0[((size_t)dir * B + row) * H + j] : 0.f;
   const float bhn = MODE == B200RNN_GRU ? p.b_hh[dir][2 * H + j] : 0.f;
   float gi[G];
+  // Elman: 0 until the first load, the register allocation its timings (tools/elman_steps_results.json) were taken with
+  if constexpr (G == 1) gi[0] = 0.f;
   auto load_gi = [&](int t) {
 #pragma unroll
     for (int g = 0; g < G; ++g) gi[g] = valid ? gates[((size_t)t * B + row) * (G * H) + g * H + j] : 0.f;
@@ -94,20 +229,23 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
       const GruStep st = gru_cell_fwd(gi, acc, bhn, h);
       hnew = frozen ? h : st.h;
       sg[0] = st.r; sg[1] = st.z; sg[2] = st.n; sx = st.hn;
-    } else {
+    } else if constexpr (MODE == B200RNN_LSTM) {
       const LstmStep st = lstm_cell_fwd(gi, acc, c);
       hnew = frozen ? h : st.h;
       c = frozen ? c : st.c;
       sg[0] = st.i; sg[1] = st.f; sg[2] = st.g; sg[3] = st.o; sx = c;
+    } else {
+      sg[0] = elman_cell_fwd(gi[0], acc[0], relu);
+      hnew = frozen ? h : sg[0];
     }
     h = hnew;
     if (valid) {
       if (p.y) p.y[(long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = frozen ? 0.f : hnew;
-      if (p.training) {  // the activated gates over the x-projection, and GRU W_hn h + b_hn / LSTM c_t
+      if (p.training) {  // the activated gates over the x-projection, and GRU W_hn h + b_hn / LSTM c_t (Elman: h_t)
         float* gp = gates + ((size_t)t * B + row) * (G * H) + j;
 #pragma unroll
         for (int g = 0; g < G; ++g) gp[g * H] = sg[g];
-        p.extra[dir][((size_t)t * B + row) * H + j] = sx;
+        if constexpr (G > 1) p.extra[dir][((size_t)t * B + row) * H + j] = sx;
       }
     }
     if (step + 1 < T) {
@@ -130,13 +268,15 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
 // =================================================================================================
 // backward (BPTT)
 // =================================================================================================
-// Shared memory: [W_s: G*n x (H+4), ONCHIP only] [d: 2 x BS x G*H] [red: BS x (G+1) x HS] [bars: 2 x C]
+// Shared memory: [W_s: G*n x (H+4), ONCHIP only] [d: 2 x BS x G*H] [red: BS x NP x HS] [bars: 2 x C]
 // Step s: dh = direct_{s-1} + sum_g W_hh[g-block]^T dgh_{s-1} (the exchange of step s - 1, all G*H columns), the cell
-// backward, then this CTA's dgh (GRU: n-block dn * r) to every CTA. Step T only contracts, for dh_0.
+// backward, then this CTA's dgh (GRU: n-block dn * r; Elman: dpre) to every CTA. Step T only contracts, for dh_0.
 template <int MODE, bool VL, bool ONCHIP>
 __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdParams p, const int nslices) {
-  constexpr int G = MODE == B200RNN_GRU ? 3 : 4;
+  constexpr int G = gates_of(MODE);
+  constexpr int NP = G == 1 ? 1 : G + 1;  // bias-partial blocks per slice: dGi (+ the GRU dghn block, 0 for the LSTM)
   const int H = p.H, B = p.B, LD = H + 4, GH = G * H;
+  const bool relu = p.mode == B200RNN_RNN_RELU;  // Elman
   const AnyhSlice s = anyh_slice<VL>(p, nslices);
   const int C = s.C, HS = s.HS, BS = s.BS, NT = s.NT, dir = s.dir, b0 = s.b0, j0 = s.j0, n = s.n, T = s.T;
   const uint32_t rank = s.rank;
@@ -144,9 +284,9 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
   float* W_s = reinterpret_cast<float*>(smem_raw);  // [G][n][LD]
   float* d_s = W_s + (ONCHIP ? (size_t)G * HS * LD : 0);
   float* red = d_s + (size_t)2 * BS * GH;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(red + (size_t)BS * (G + 1) * HS);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(red + (size_t)BS * NP * HS);
   const int tid = threadIdx.x;
-  // rows (g, u) of this CTA: W_hh[g*H + :][j0 + u], contiguous from G * j0 * H (anyh_prep_kernel)
+  // rows (g, u) of this CTA: W_hh[g*H + :][j0 + u], contiguous from G * j0 * H (whh_prep_kernel)
   const float* w_prep = p.w_prep[dir] + (size_t)G * j0 * H;
 
   if (tid == 0) init_bars(bars, C);
@@ -169,12 +309,9 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
     if (p.dh_n) dh_carry = p.dh_n[((size_t)dir * B + row) * H + j];
     if (MODE == B200RNN_LSTM && p.dc_n) dc_carry = p.dc_n[((size_t)dir * B + row) * H + j];
   }
-  float bsum[G + 1];
-#pragma unroll
-  for (int g = 0; g <= G; ++g) bsum[g] = 0.f;
-  float sv[G], sx = 0.f, hp = 0.f, dyv = 0.f;  // saved gates, hn / c_t, h_{prev} / c_{prev}, dy (prefetched)
-#pragma unroll
-  for (int g = 0; g < G; ++g) sv[g] = 0.f;
+  float bsum[NP] = {};
+  // saved gates (Elman: h_t), hn / c_t, h_{prev} / c_{prev}, dy (prefetched)
+  float sv[G] = {}, sx = 0.f, hp = 0.f, dyv = 0.f;
   const float* s0 = MODE == B200RNN_GRU ? p.h_0 : p.c_0;  // the state before the first step (zeros when NULL)
   auto load_step = [&](int step) {
     const int t = dir ? step : (T - 1 - step);
@@ -183,14 +320,16 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
     const bool has_prev = step < T - 1 && !(MODE == B200RNN_GRU && VL && tp >= len);
 #pragma unroll
     for (int g = 0; g < G; ++g) sv[g] = gates[((size_t)t * B + row) * GH + g * H + j];
-    sx = extra[((size_t)t * B + row) * H + j];
+    if constexpr (G > 1) sx = extra[((size_t)t * B + row) * H + j];
     dyv = p.dy[(long long)t * p.dy_st + (long long)row * p.dy_sb + dir * H + j];
-    if (!has_prev)
-      hp = s0 ? s0[((size_t)dir * B + row) * H + j] : 0.f;
-    else if (MODE == B200RNN_GRU)
-      hp = p.y[(long long)tp * p.y_st + (long long)row * p.y_sb + dir * H + j];
-    else
-      hp = extra[((size_t)tp * B + row) * H + j];
+    if constexpr (G > 1) {
+      if (!has_prev)
+        hp = s0 ? s0[((size_t)dir * B + row) * H + j] : 0.f;
+      else if (MODE == B200RNN_GRU)
+        hp = p.y[(long long)tp * p.y_st + (long long)row * p.y_sb + dir * H + j];
+      else
+        hp = extra[((size_t)tp * B + row) * H + j];
+    }
   };
   if (valid && T > 0) load_step(0);
   const bool want_dh0 = p.dh_0 != nullptr;
@@ -202,7 +341,7 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
       float acc[G];
 #pragma unroll
       for (int g = 0; g < G; ++g) acc[g] = 0.f;
-      dot_rows<G, ONCHIP, true>(wrow, wg, d_s + ((size_t)cur * BS + b) * GH, H, H, acc);
+      dot_rows<G, ONCHIP, (G > 1)>(wrow, wg, d_s + ((size_t)cur * BS + b) * GH, H, H, acc);
       float sum = acc[0];
 #pragma unroll
       for (int g = 1; g < G; ++g) sum += acc[g];
@@ -220,12 +359,15 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
     float dg[G], dhn = 0.f;
     if constexpr (MODE == B200RNN_GRU) {
       direct = gru_cell_bwd(sv, sx, hp, dh, dg, dhn);
-    } else {
+    } else if constexpr (MODE == B200RNN_LSTM) {
       const float dc_next = lstm_cell_bwd(sv, sx, hp, dh, dc_carry, dg);
       direct = 0.f;
       if (!frozen) dc_carry = dc_next;  // frozen: dh and dc pass straight through
+    } else {  // Elman: dpre from the saved h_t; frozen as below
+      dg[0] = frozen ? 0.f : elman_cell_bwd(sv[0], dh, relu);
+      direct = frozen ? dh : 0.f;
     }
-    if (frozen) {
+    if (G > 1 && frozen) {
 #pragma unroll
       for (int g = 0; g < G; ++g) dg[g] = 0.f;
       dhn = 0.f;
@@ -234,7 +376,7 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
     if (valid) {
 #pragma unroll
       for (int g = 0; g < G; ++g) bsum[g] += dg[g];
-      bsum[G] += dhn;
+      if constexpr (NP > G) bsum[G] += dhn;
       float* gp = dgates + ((size_t)t * B + row) * GH + j;
 #pragma unroll
       for (int g = 0; g < G; ++g) gp[g * H] = dg[g];
@@ -264,54 +406,28 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
         if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + row) * H + j] = 0.f;
       }
   }
-  // per-slice bias-gradient partials: the slice's batch slots summed in slot order
+  // per-slice bias-gradient partials [nslices][NP * H] (api.cu reduces them): the slice's batch slots summed in slot
+  // order
   if (s.active) {
 #pragma unroll
-    for (int g = 0; g <= G; ++g) red[((size_t)b * (G + 1) + g) * HS + u] = bsum[g];
+    for (int g = 0; g < NP; ++g) red[((size_t)b * NP + g) * HS + u] = bsum[g];
   }
   __syncthreads();
   if (s.active && b == 0) {
-    float* out = p.dbias_part[dir] + (size_t)s.slice * (G + 1) * H;
-    for (int g = 0; g <= G; ++g) {
+    for (int g = 0; g < NP; ++g) {
       float v = 0.f;
-      for (int q = 0; q < BS; ++q) v += red[((size_t)q * (G + 1) + g) * HS + u];
+      for (int q = 0; q < BS; ++q) v += red[((size_t)q * NP + g) * HS + u];
+      float* out = p.dbias_part[dir] + (size_t)s.slice * NP * H;
       out[g * H + j] = v;
     }
   }
   ptx::cluster_sync_all();
 }
 
-// The backward's W_hh, per CTA of a C-CTA cluster and contiguous: CTA r's block starts at G * j0_r * H and holds
-// out[G*j0_r*H + (g*n_r + u)*H + jj] = W_hh[g*H + jj][j0_r + u] (anyh_units). For even slices this is whh_prep_kernel's
-// layout; that kernel tiles by 32 and takes H / C units per CTA.
-__global__ void anyh_prep_kernel(const float* __restrict__ w_hh, float* __restrict__ out, int G, int H, int C) {
-  __shared__ float tile[32][33];
-  const int nt = (H + 31) / 32;
-  for (int tix = blockIdx.x; tix < G * nt * nt; tix += gridDim.x) {
-    const int g = tix / (nt * nt), rem = tix - g * nt * nt;
-    const int tj = rem / nt, tk = rem - tj * nt;  // row tile of the gate block, column tile
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-      const int r = tj * 32 + i, k = tk * 32 + threadIdx.x;
-      tile[i][threadIdx.x] = (r < H && k < H) ? w_hh[((size_t)g * H + r) * H + k] : 0.f;
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-      const int col = tk * 32 + i, jj = tj * 32 + threadIdx.x;
-      if (col < H && jj < H) {
-        int rk = (col / 8) * C / (H / 8), j0, n;  // the CTA that owns unit col (anyh_units), found from its group
-        anyh_units(H, C, rk, j0, n);
-        while (col >= j0 + n) anyh_units(H, C, ++rk, j0, n);
-        while (col < j0) anyh_units(H, C, --rk, j0, n);
-        out[(size_t)G * j0 * H + ((size_t)g * n + col - j0) * H + jj] = tile[threadIdx.x][i];
-      }
-    }
-    __syncthreads();
-  }
-}
-
 // =================================================================================================
 // config choice
 // =================================================================================================
+// bytes of dynamic shared memory of one launch shape (the Elman backward uses BS x HS floats fewer than this)
 size_t anyh_smem(int G, int H, int C, int BS, bool bwd, bool onchip) {
   const size_t HS = (size_t)anyh_max_units(H, C);
   size_t f = onchip ? (size_t)G * HS * (H + 4) : 0;
@@ -320,37 +436,8 @@ size_t anyh_smem(int G, int H, int C, int BS, bool bwd, bool onchip) {
   return f * sizeof(float) + (size_t)2 * C * sizeof(uint64_t);
 }
 
-// How many clusters of C CTAs of `kernel` (NT threads, smem bytes) can be co-resident, from the driver; cached per
-// (kernel, device, shape). 0 when the query fails or the shape cannot run.
-int anyh_capacity(const void* kernel, int C, int NT, size_t smem) {
-  static std::mutex mu;
-  static std::map<std::tuple<const void*, int, int, int, size_t>, int> cache;
-  const auto key = std::make_tuple(kernel, current_device(), C, NT, smem);
-  std::lock_guard<std::mutex> lk(mu);
-  auto it = cache.find(key);
-  if (it == cache.end()) {
-    int n = 0;
-    // every shape of the kernel may take up to the opt-in limit; 16-CTA clusters are non-portable
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM) == cudaSuccess &&
-        cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = (unsigned)C;
-      attr[0].val.clusterDim.y = 1;
-      attr[0].val.clusterDim.z = 1;
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3((unsigned)(C * NUM_SMS), 1, 1);
-      cfg.blockDim = dim3((unsigned)NT, 1, 1);
-      cfg.dynamicSmemBytes = smem;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) n = 0;
-    }
-    if (n == 0) cudaGetLastError();  // a failed query leaves its error pending: clear that one, not an older one
-    it = cache.emplace(key, n).first;
-  }
-  return it->second;
-}
+template <typename P>
+using AnyhKernel = void (*)(P, int);
 
 template <int MODE>
 AnyhKernel<RecFwdParams> anyh_kernel(const RecFwdParams&, bool vl, bool onchip) {
@@ -371,16 +458,17 @@ AnyhKernel<RecBwdParams> anyh_kernel(const RecBwdParams&, bool vl, bool onchip) 
 //     to 4 warps has one warp per scheduler, so a smaller one shortens no step), ties to the fewest CTAs.
 //   * In the L2 tier a step costs each CTA its G*HS*H weights streamed from L2, whatever BS (a warp's batch slots share
 //     every load): the widest cluster, then the fewest waves, then the fewest batch rows.
-// Capacities come from the driver (anyh_capacity), never from the SM count; clusters that do not fit run in waves.
+// Capacities come from the driver (cluster_capacity), never from the SM count; clusters that do not fit run in waves.
 template <typename P>
 int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L) {
   const int G = gates_of(p.mode), H = p.H;
   const bool vl = p.lengths != nullptr;
   for (int tier = 0; tier < 2; ++tier) {
     const bool onchip = tier == 0;
+    // one Elman instantiation for both nonlinearities
     const AnyhKernel<P> kernel = p.mode == B200RNN_GRU    ? anyh_kernel<B200RNN_GRU>(p, vl, onchip)
                                  : p.mode == B200RNN_LSTM ? anyh_kernel<B200RNN_LSTM>(p, vl, onchip)
-                                                          : elman_kernel(p, vl, onchip);
+                                                          : anyh_kernel<B200RNN_RNN_TANH>(p, vl, onchip);
     bool found = false;
     long long best[3] = {0, 0, 0};
     ClusterLaunch<P> pick{};
@@ -393,7 +481,9 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L) {
         const size_t smem = anyh_smem(G, H, C, BS, bwd, onchip);
         if (smem > (size_t)MAX_SMEM) continue;
         const int nslices = (p.B + BS - 1) / BS, nclusters = nslices * p.D;
-        const int capacity = anyh_capacity((const void*)kernel, C, NT, smem);
+        int capacity = 0;
+        const int rc = cluster_capacity((const void*)kernel, C, NT, smem, &capacity);
+        if (rc != B200RNN_OK) return rc;
         if (capacity <= 0) continue;
         const long long waves = (nclusters + capacity - 1) / capacity;
         long long key[3];
@@ -446,16 +536,6 @@ int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
     return B200RNN_ERR_UNSUPPORTED;
   }
   return plan_anyh(p, true, L);
-}
-
-int launch_anyh_prep(const float* w_hh, float* w_prep, int G, int H, int C, cudaStream_t s) {
-  anyh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(w_hh, w_prep, G, H, C);
-  if (cudaGetLastError() != cudaSuccess) {
-    set_error("anyh_prep launch failed");
-    return B200RNN_ERR_CUDA;
-  }
-  count_launch();
-  return B200RNN_OK;
 }
 
 }  // namespace b200rnn

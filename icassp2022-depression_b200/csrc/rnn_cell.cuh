@@ -1,5 +1,5 @@
 // rnn_cell.cuh — the gate math of one GRU / LSTM / Elman step, shared by the persistent recurrence kernels (rnn_rec.cu,
-// rnn_anyh.cu, rnn_elman.cu) and the one-step cell kernels (cell.cu), so that a cell and a sequence step apply the same
+// rnn_anyh.cu) and the one-step cell kernels (cell.cu), so that a cell and a sequence step apply the same
 // non-linearities in the same order. Gate order as in torch/nn/modules/rnn.py: GRU r, z, n; LSTM i, f, g, o.
 #pragma once
 #include "common.cuh"

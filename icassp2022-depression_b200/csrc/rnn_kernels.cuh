@@ -48,9 +48,9 @@ struct ClusterLaunch {
   void (*kernel)(P, int);
   int C, NT, nslices, nclusters, capacity;
   size_t smem;
-  // a runtime-sized kernel of rnn_anyh.cu (hidden sizes other than 128 / 256): it takes no streamed x-projection
-  // (RecFwdParams::ready), and its backward reads W_hh as anyh_prep_kernel lays it out. BS batch rows per cluster;
-  // onchip: W_hh stays in shared memory (else it is read from L2 every step).
+  // a runtime-sized kernel of rnn_anyh.cu (GRU / LSTM hidden sizes other than 128 / 256, every Elman one): it takes no
+  // streamed x-projection (RecFwdParams::ready). BS batch rows per cluster; onchip: W_hh stays in shared memory (else it
+  // is read from L2 every step).
   bool anyh = false;
   int BS = 0;
   bool onchip = false;
@@ -62,7 +62,8 @@ using RecFwdLaunch = ClusterLaunch<RecFwdParams>;
 struct RecBwdParams {
   int mode, B, T, H, D;
   const float* w_hh[2];      // per direction weight_hh [G*H, H]
-  float* w_prep[2];          // per direction scratch, G*H*H floats: per-CTA transposed slices (filled by the launcher)
+  float* w_prep[2];          // per direction scratch, G*H*H floats: per-CTA transposed slices (whh_prep_kernel, filled
+                             // by the launcher)
   const float* gates[2];     // saved activated gates [T,B,G*H]
   const float* extra[2];     // GRU hn / LSTM c, [T,B,H]
   const float* y;            // this layer's forward output (h_t), strided
@@ -97,13 +98,26 @@ constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_90
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)
 int rec_bwd_max_slices(int B);
 
-// The runtime-sized recurrence (rnn_anyh.cu, rnn_elman.cu): the hidden sizes it takes (H % 16 == 0, 16 <= H <= 1024),
-// its config choice for the GRU / LSTM shapes the fixed configs do not cover and for every Elman shape, and its W_hh
-// transpose for the backward (any H)
+// The units of CTA r of a C-CTA cluster: the H / 8 groups of 8 units split as evenly as possible, [j0, j0 + n). Every
+// CTA owns at least one group when C <= H / 8; a slice of a state row is a whole number of 16-byte chunks. When C
+// divides H / 8 this is the fixed configs' split, H / C units from r * H / C.
+__host__ __device__ __forceinline__ void anyh_units(int H, int C, int r, int& j0, int& n) {
+  const int g = H / 8, a = r * g / C, e = (r + 1) * g / C;
+  j0 = 8 * a;
+  n = 8 * (e - a);
+}
+__host__ __device__ __forceinline__ int anyh_max_units(int H, int C) { return 8 * ((H / 8 + C - 1) / C); }
+
+// How many clusters of C CTAs of `kernel` (NT threads, smem bytes of dynamic shared memory) can be co-resident, from the
+// driver; cached per (kernel, device, C, NT, smem). The first query of a kernel on a device opts it in to MAX_SMEM bytes
+// and to non-portable (16-CTA) clusters; B200RNN_ERR_CUDA when that fails. A failed occupancy query is capacity 0.
+int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capacity);
+
+// The runtime-sized recurrence (rnn_anyh.cu): the hidden sizes it takes (H % 16 == 0, 16 <= H <= 1024) and its config
+// choice for the GRU / LSTM shapes the fixed configs do not cover and for every Elman shape
 bool anyh_hidden_size(int H);
 int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* out);
 int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out);
-int launch_anyh_prep(const float* w_hh, float* w_prep, int G, int H, int C, cudaStream_t stream);
 
 // forward: choose the config for p's shape (mode, H, P, B, D, lengths or not), then launch it; p.ready != NULL launches
 // it with programmatic stream serialization, so that it may start while the GEMM before it still runs

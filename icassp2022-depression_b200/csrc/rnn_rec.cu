@@ -26,7 +26,9 @@
 // once per launch in the no-grad forward of b200rnn_forward_fused (rec_fwd_h16_kernel).
 #include <map>
 #include <mutex>
+#include <set>
 #include <stdlib.h>
+#include <tuple>
 #include <type_traits>
 #include <utility>
 
@@ -950,25 +952,6 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_h16_kernel(const RecF
 // w_prep layout (written by whh_prep_kernel): [C ranks][G][HS][H],
 //   w_prep[rank][g][u][jj] = W_hh[g*H + jj][rank*HS + u]
 // i.e. for every gate block the transposed slice a CTA needs, contiguous per CTA (TMA bulk copyable).
-__global__ void whh_prep_kernel(const float* __restrict__ w_hh, float* __restrict__ out, int G, int H, int C) {
-  __shared__ float tile[32][33];
-  const int HS = H / C;
-  const int tiles_per_g = (H / 32) * (H / 32);
-  for (int tix = blockIdx.x; tix < G * tiles_per_g; tix += gridDim.x) {
-    const int g = tix / tiles_per_g, rem = tix - g * tiles_per_g;
-    const int tj = rem / (H / 32), tk = rem - tj * (H / 32);  // tj: row tile of the gate block, tk: column tile
-    for (int i = threadIdx.y; i < 32; i += blockDim.y)
-      tile[i][threadIdx.x] = w_hh[((size_t)g * H + tj * 32 + i) * H + tk * 32 + threadIdx.x];
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-      const int col = tk * 32 + i;  // column of W_hh = output unit of the backward contraction
-      const int rk = col / HS, u = col - rk * HS;
-      out[(((size_t)rk * G + g) * HS + u) * H + tj * 32 + threadIdx.x] = tile[threadIdx.x][i];
-    }
-    __syncthreads();
-  }
-}
-
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG, bool VL = false>
 __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
     rec_bwd_kernel(const RecBwdParams p, const int nslices) {
@@ -1639,29 +1622,6 @@ cudaLaunchConfig_t cluster_config(int nclusters, int C, int NT, size_t smem, cud
   return cfg;
 }
 
-// Once per (kernel, device): opt the kernel in to `smem` bytes of dynamic shared memory and ask the driver how many of
-// its clusters can be resident at once (0 when the query fails).
-int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capacity) {
-  static std::mutex mu;  // forward and autograd-backward threads both launch
-  static std::map<std::pair<const void*, int>, int> cache;
-  const std::pair<const void*, int> key(kernel, current_device());
-  std::lock_guard<std::mutex> lk(mu);
-  auto it = cache.find(key);
-  if (it == cache.end()) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchAttribute attr[2];
-    const cudaLaunchConfig_t cfg = cluster_config(NUM_SMS, C, NT, smem, 0, attr);
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) {
-      cudaGetLastError();
-      n = 0;
-    }
-    it = cache.emplace(key, n).first;
-  }
-  *capacity = it->second;
-  return B200RNN_OK;
-}
-
 // Chooses `kernel` as D * ceil(B / BS) clusters of C CTAs if the driver reports them all co-resident, or regardless
 // when `force` (then in several waves if they do not fit). Returns false when the config is not taken; true when it is
 // (*L describes it, nothing is enqueued yet) or when the capacity query failed (*rc). B200RNN_DEBUG prints one line per
@@ -1754,6 +1714,33 @@ int pick_proj(const Params& p, ClusterLaunch<Params>* L) {
 // smallest BS any backward config uses is 2
 int rec_bwd_max_slices(int B) { return (B + 1) / 2; }
 
+int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capacity) {
+  static std::mutex mu;  // forward and autograd-backward threads both launch
+  static std::set<std::pair<const void*, int>> opted_in;
+  static std::map<std::tuple<const void*, int, int, int, size_t>, int> cache;
+  const int dev = current_device();
+  const auto key = std::make_tuple(kernel, dev, C, NT, smem);
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = cache.find(key);
+  if (it == cache.end()) {
+    if (!opted_in.count({kernel, dev})) {  // every shape of the kernel may take up to the opt-in limit
+      B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      opted_in.insert({kernel, dev});
+    }
+    cudaLaunchAttribute attr[2];
+    const cudaLaunchConfig_t cfg = cluster_config(NUM_SMS, C, NT, smem, 0, attr);
+    int n = 0;
+    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) {
+      cudaGetLastError();  // a failed query leaves its error pending: clear that one, not an older one
+      n = 0;
+    }
+    it = cache.emplace(key, n).first;
+  }
+  *capacity = it->second;
+  return B200RNN_OK;
+}
+
 // Candidates are ordered by batch rows per cluster; the first one whose clusters are all co-resident
 // (one wave => every sequence advances in lock step) wins, else the widest one runs in several waves.
 // Template arguments: <MODE, H, C, BS, KL, UPL, RG>; projected: <H, P, C, BS>, H = 128 on 2-CTA clusters of 4 batch rows
@@ -1771,7 +1758,7 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
               "proj_size hidden_size/4 or hidden_size/2", p.mode, p.H, p.P);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  // the Elman modes run the runtime-sized kernels at every hidden size, 128 and 256 included (rnn_elman.cu)
+  // the Elman modes run the runtime-sized kernels at every hidden size, 128 and 256 included (rnn_anyh.cu)
   if (is_elman(p.mode)) return plan_anyh_fwd(p, L);
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
@@ -1872,16 +1859,43 @@ int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s)
   return launch_clustered(L, p, PROF_REC_FWD, p.ready != nullptr, s);
 }
 
+namespace {
+
+// The backward's W_hh for a C-CTA cluster, transposed and contiguous per CTA: CTA r's block starts at G * j0_r * H and
+// holds out[G*j0_r*H + (g*n_r + u)*H + jj] = W_hh[g*H + jj][j0_r + u] (anyh_units). For the fixed configs (C divides
+// H / 8) this is the [C ranks][G][H / C][H] layout rec_bwd_kernel copies with TMA.
+__global__ void whh_prep_kernel(const float* __restrict__ w_hh, float* __restrict__ out, int G, int H, int C) {
+  __shared__ float tile[32][33];
+  const int nt = (H + 31) / 32;
+  for (int tix = blockIdx.x; tix < G * nt * nt; tix += gridDim.x) {
+    const int g = tix / (nt * nt), rem = tix - g * nt * nt;
+    const int tj = rem / nt, tk = rem - tj * nt;  // row tile of the gate block, column tile
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+      const int r = tj * 32 + i, k = tk * 32 + threadIdx.x;
+      tile[i][threadIdx.x] = (r < H && k < H) ? w_hh[((size_t)g * H + r) * H + k] : 0.f;
+    }
+    __syncthreads();
+    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+      const int col = tk * 32 + i, jj = tj * 32 + threadIdx.x;
+      if (col < H && jj < H) {
+        int rk = (col / 8) * C / (H / 8), j0, n;  // the CTA that owns unit col (anyh_units), found from its group
+        anyh_units(H, C, rk, j0, n);
+        while (col >= j0 + n) anyh_units(H, C, ++rk, j0, n);
+        while (col < j0) anyh_units(H, C, --rk, j0, n);
+        out[(size_t)G * j0 * H + ((size_t)g * n + col - j0) * H + jj] = tile[threadIdx.x][i];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+}  // namespace
+
 int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
   RecBwdLaunch L;
   const int rc = plan_rec_bwd(p, &L);
   if (rc != B200RNN_OK || L.kernel == nullptr) return rc;
-  if (L.anyh) {  // the same layout for any H (whh_prep_kernel tiles by 32)
-    for (int d = 0; d < p.D; ++d) {
-      const int prc = launch_anyh_prep(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C, s);
-      if (prc != B200RNN_OK) return prc;
-    }
-  } else if (p.P == 0) {  // transposed, per-CTA contiguous copy of W_hh for the chosen cluster width
+  if (p.P == 0) {  // the unprojected kernels read W_hh transposed for the chosen cluster width
     for (int d = 0; d < p.D; ++d) {
       whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C);
       if (cudaGetLastError() != cudaSuccess) {

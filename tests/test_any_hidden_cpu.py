@@ -1,6 +1,6 @@
 """Hidden sizes other than 128 / 256 on the host side: which sizes the descriptor takes, that the model-shell entry
 points refuse them, the modules' parameters and state_dict at those sizes, and that the runtime-sized recurrence
-kernels (csrc/rnn_anyh.cu) compile without stack or local memory."""
+kernels (csrc/rnn_anyh.cu, GRU / LSTM / Elman) compile without stack or local memory."""
 import ctypes
 import os
 import re
@@ -92,9 +92,10 @@ def _anyh_kernels():
     return seen
 
 
-def test_runtime_sized_kernels_use_no_local_memory_and_no_stack():
+def test_gru_lstm_elman_runtime_sized_kernels_use_no_local_memory_and_no_stack():
     seen = _anyh_kernels()
-    # forward and backward x GRU / LSTM x fixed / ragged x shared-memory / L2 weights
-    assert len([n for n in seen if "anyh_fwd_kernel" in n]) == 8, sorted(seen)
-    assert len([n for n in seen if "anyh_bwd_kernel" in n]) == 8, sorted(seen)
+    # forward and backward x GRU / LSTM / Elman (one instantiation for tanh and relu) x fixed / ragged x shared-memory /
+    # L2 weights
+    assert len([n for n in seen if "anyh_fwd_kernel" in n]) == 12, sorted(seen)
+    assert len([n for n in seen if "anyh_bwd_kernel" in n]) == 12, sorted(seen)
     assert all(v == (0, 0) for v in seen.values()), {n: v for n, v in seen.items() if v != (0, 0)}

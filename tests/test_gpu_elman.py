@@ -1,10 +1,11 @@
-"""The Elman RNN on the GPU: ``RNN`` (csrc/rnn_elman.cu) and ``RNNCell`` (cell.cu), nonlinearity tanh and relu.
+"""The Elman RNN on the GPU: ``RNN`` (the Elman instantiations of csrc/rnn_anyh.cu) and ``RNNCell`` (cell.cu),
+nonlinearity tanh and relu.
 
 Reference: stock torch.nn.RNN / RNNCell in float64 on CPU. Tolerances as tests/test_gpu_any_hidden.py: outputs and
 states 1e-5 (absolute for tanh; relative to the largest entry for relu, whose outputs are unbounded), gradients 1e-4
 relative to the largest entry of each tensor (dx, dh_0, every dW and db). The per-step test holds each step of the
 kernel's own trajectory to kappa * u * S away from default init (tests/test_gpu_numerics_f64.py). Which config each
-shape runs is read from the B200RNN_DEBUG lines of a subprocess: every elman_* instantiation and both weight tiers are
+shape runs is read from the B200RNN_DEBUG lines of a subprocess: every Elman instantiation and both weight tiers are
 reached."""
 import contextlib
 import os

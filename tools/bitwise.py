@@ -14,6 +14,8 @@ eight-CTA co-resident clusters (DESIGN.md), GRU-256 runs 2-row clusters at B = 1
 8-CTA ones at B = 128; GRU-128 its 2-CTA config at B = 64 and the 4-CTA fallback at B = 272; the BiLSTM-256 its 4-CTA
 config at B = 32 and the 8-CTA fallback at B = 64; the BiLSTM-128 its 2-CTA config at B = 16 and the 4-CTA fallback at
 B = 136. The projected cases cover the four (H, P), the fused_nograd ones the fp16-pair forward of rnn_forward_fused.
+The anyh_* cases run the runtime-sized kernels (csrc/rnn_anyh.cu) of the GRU, the LSTM and the Elman RNN (tanh and
+relu), with W_hh on chip and read from L2, fixed-length with an initial state and ragged.
 
     # the other build, e.g. of an earlier commit, from a worktree of it:
     #   make -C <worktree>/icassp2022-depression_b200 OBJDIR=<tmp>/obj LIBDIR=$PWD/lib_parent
@@ -52,9 +54,12 @@ def _model(kind, I, H, L=2, bi=False, dropout=0.0, proj=0, seed=0):
     import b200rnn
 
     torch.manual_seed(seed)
-    cls = torch.nn.GRU if kind == "gru" else torch.nn.LSTM
-    ref = cls(I, H, num_layers=L, bidirectional=bi, batch_first=True, dropout=dropout,
-              **({"proj_size": proj} if proj else {}))
+    kw = {"proj_size": proj} if proj else {}
+    if kind in ("rnn_tanh", "rnn_relu"):
+        cls, kw = torch.nn.RNN, {"nonlinearity": kind[4:]}
+    else:
+        cls = torch.nn.GRU if kind == "gru" else torch.nn.LSTM
+    ref = cls(I, H, num_layers=L, bidirectional=bi, batch_first=True, dropout=dropout, **kw)
     return b200rnn.from_torch(ref).to(DEV).train()
 
 
@@ -182,8 +187,8 @@ def _cases():
         lens[0] = T
         return lens
 
-    def cfg_case(kind, I, H, B, bi, proj=0, packed=False, T=24):
-        return lambda: _run(_model(kind, I, H, bi=bi, proj=proj), B, T, hx=proj > 0,
+    def cfg_case(kind, I, H, B, bi, proj=0, packed=False, T=24, hx=None):
+        return lambda: _run(_model(kind, I, H, bi=bi, proj=proj), B, T, hx=proj > 0 if hx is None else hx,
                             lengths=ragged(B, T) if packed else None)
 
     matrix = [("gru", 256, 256, B, False, 0) for B in (16, 64, 128)]
@@ -195,6 +200,17 @@ def _cases():
         for packed in (False, True):
             name = f"cfg_{'bi' if bi else ''}{kind}{H}{f'_p{P}' if P else ''}_i{I}_b{B}_t24{'_ragged' if packed else ''}"
             cases[name] = cfg_case(kind, I, H, B, bi, P, packed)
+
+    # The runtime-sized kernels (csrc/rnn_anyh.cu), each shape fixed-length with an initial state and ragged without:
+    # GRU / LSTM at hidden sizes without a fixed config, W_hh on chip (GRU 64, BiLSTM 192) and read from L2 (GRU 1024,
+    # LSTM 768), and the Elman RNN on chip (tanh 128, relu 512) and from L2 (tanh 1024)
+    anyh = [("gru", 40, 64, 64, False), ("lstm", 40, 192, 16, True), ("gru", 40, 1024, 8, False),
+            ("lstm", 40, 768, 8, False), ("rnn_tanh", 40, 128, 64, False), ("rnn_relu", 40, 512, 64, False),
+            ("rnn_tanh", 40, 1024, 8, False)]
+    for kind, I, H, B, bi in anyh:
+        for packed in (False, True):
+            name = f"anyh_{'bi' if bi else ''}{kind}{H}_i{I}_b{B}_t24{'_ragged' if packed else '_hx'}"
+            cases[name] = cfg_case(kind, I, H, B, bi, packed=packed, hx=not packed)
 
     def fused_nograd(pool_sum):
         from b200rnn import _lib

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""What the Elman recurrence (csrc/rnn_elman.cu) and the RNNCell kernels cost, against stock cuDNN / ATen.
+"""What the Elman recurrence (the Elman kernels of csrc/rnn_anyh.cu) and the RNNCell kernels cost, against stock
+cuDNN / ATen.
 
 Sequence: one unidirectional layer, time-major, T = 120, I = 64, H in {64, 128, 256, 512, 1024}, B in {16, 64, 128},
 nonlinearity tanh and relu:
