@@ -23,7 +23,8 @@
 // fp32 FFMA for most configs: the per-step contraction is [BS x H] x [H x G*HS] with BS = 2..8 rows per CTA — far too
 // skinny for wgmma tiles, and parity is judged at 1e-5 against an fp32 reference. The GRU H=256 8-row config runs it
 // on the tensor cores with warp-level mma.sync (N = 8) in 3xTF32 instead (rec_fwd_tc_kernel), or on fp16 pairs split
-// once per launch in the no-grad forward of b200rnn_forward_fused (rec_fwd_h16_kernel).
+// once per launch in the no-grad forward of b200rnn_forward_fused (rec_fwd_h16_kernel); in that forward the LSTM H=128
+// layers take the same body on 2-CTA clusters of 8 rows (lstm_fwd_h16_kernel).
 #include <map>
 #include <mutex>
 #include <set>
@@ -539,8 +540,15 @@ __global__ void __launch_bounds__(RecCfg<MODE, H, C, BS, KL, UPL, RG>::NT, 1)
 // runs one mma.sync per (gate tile, k-step): 384 per CTA and step instead of 1,152, one accumulator per tile and source
 // slice (4 MMAs). Round-to-nearest, not the truncation of split_tf32: without a lo term a truncated operand would bias
 // every product the same way.
-struct TcFwdCfg {
-  static constexpr int H = 256, C = 4, BS = 8, G = 3, GH = G * H;
+// The geometry is a parameter (TcCfg<MODE, L, RT, TAIL_SLOTS, SCALE_ROWS>, L = h16::Geom): the GRU-256 config TcFwdCfg
+// runs all three contractions, the LSTM-128 one TcLstmCfg (2-CTA clusters of 8 batch rows, 64 units x 4 gates per CTA)
+// only the fp16-pair one. RT gate tiles (the last ones) stay in registers in the fp16-pair kernels; SCALE_ROWS rows'
+// loads are in flight at once in the row-scale pass of the prologue.
+template <int MODE_, typename L_, int RT_, int TAIL_SLOTS, int SCALE_ROWS_>
+struct TcCfg {
+  using L = L_;
+  static constexpr int MODE = MODE_, RT = RT_, SCALE_ROWS = SCALE_ROWS_;
+  static constexpr int H = L::H, C = L::C, BS = L::BS, G = L::G, GH = G * H;
   static constexpr int HS = H / C;        // units per CTA
   static constexpr int NUG = HS / 16;     // unit groups
   static constexpr int NW = 2 * NUG;      // compute warps: (k half, unit group)
@@ -550,10 +558,10 @@ struct TcFwdCfg {
   static constexpr int KSC = HS / 8;      // k-steps per source slice
   static constexpr size_t W_BYTES = (size_t)G * HS * H * sizeof(float);
   static constexpr size_t RED_BYTES = (size_t)NW * 2 * G * 32 * sizeof(float);  // partial sums swapped between halves
-  // x-projection ring of the 3xTF32 and TF32 kernels, behind the swap buffer (the fp16-pair kernel keeps its ring in
-  // dead weight space, rec_h16_layout.cuh)
-  static constexpr int RING_SLOTS = 2;
-  static constexpr size_t RING_BYTES = (size_t)RING_SLOTS * h16::RING_SLOT_BYTES;
+  // x-projection ring behind the swap buffer: the 3xTF32 and TF32 kernels' and the LSTM-128 fp16-pair kernel's (the
+  // GRU-256 fp16-pair kernel keeps its ring in dead weight space, rec_h16_layout.cuh)
+  static constexpr int RING_SLOTS = TAIL_SLOTS;
+  static constexpr size_t RING_BYTES = (size_t)RING_SLOTS * L::RING_SLOT_BYTES;
   static constexpr int NBAR = 2 * C + 2 * h16::RING_SLOTS;  // state [buf][src], ring full[slot], ring empty[slot]
   static constexpr size_t SMEM = W_BYTES + (size_t)2 * BS * H * sizeof(float) + RED_BYTES + RING_BYTES +
                                  NBAR * sizeof(uint64_t);
@@ -561,7 +569,13 @@ struct TcFwdCfg {
   static constexpr int PRODUCER_REGS = 24, COMPUTE_REGS = 240;
   static_assert(PRODUCER_REGS * 128 + COMPUTE_REGS * NTC <= 65536, "register file");
   static_assert(RING_SLOTS <= h16::RING_SLOTS, "ring barriers");
+  static_assert(L::RING_IN_TILE || (h16::RING_SLOTS == RING_SLOTS && (size_t)L::ring_byte(0) == W_BYTES +
+                                    (size_t)2 * BS * H * sizeof(float) + RED_BYTES), "the ring region of the layout");
+  static_assert(L::NW == NW && L::RED_BYTES == (int)RED_BYTES, "h16 layout geometry");
 };
+using TcFwdCfg = TcCfg<B200RNN_GRU, h16::Gru256, 1, 2, 1>;
+// two gate tiles in registers (64 per lane, as the GRU's one tile of four slices) compile with no spill
+using TcLstmCfg = TcCfg<B200RNN_LSTM, h16::Lstm128, 2, 4, 8>;
 
 // position of state element (k, batch row b) in the B-fragment-ordered buffer: lane (g, t) of k-step ks reads
 // {h[g][ks*8 + t], h[g][ks*8 + t + 4]} as the float2 at ks*64 + lane*2
@@ -586,15 +600,17 @@ __device__ __forceinline__ float round_tf32(float x) {
 // state: |h_t| <= 1 is what makes the fixed state scale safe.
 enum class TcOp { X3, TF32, F16 };
 
-template <bool VL, TcOp OP>
+template <typename Cfg, bool VL, TcOp OP>
 __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int nslices) {
-  using Cfg = TcFwdCfg;
+  using L = typename Cfg::L;
   constexpr int H = Cfg::H, C = Cfg::C, BS = Cfg::BS, G = Cfg::G, HS = Cfg::HS, NUG = Cfg::NUG, NW = Cfg::NW,
-                NT = Cfg::NT, KS = Cfg::KS, KSC = Cfg::KSC;
+                NT = Cfg::NT, KS = Cfg::KS, KSC = Cfg::KSC, RT = Cfg::RT;
   constexpr bool TF32 = OP == TcOp::TF32, F16 = OP == TcOp::F16;
-  constexpr int KBC = h16::KBC;
-  static_assert(h16::H == H && h16::C == C && h16::BS == BS && h16::G == G && h16::NW == NW, "h16 layout geometry");
-  static_assert(h16::W_HALVES * 2 == (int)Cfg::W_BYTES && h16::S_HALVES * 2 == BS * H * 4, "h16 regions");
+  constexpr int KBC = L::KBC;
+  static_assert(F16 || Cfg::MODE == B200RNN_GRU, "the 3xTF32 and TF32 contractions are built for the GRU");
+  static_assert(RT >= 1 && RT < G, "register tiles");
+  static_assert(L::H == H && L::C == C && L::BS == BS && L::G == G && L::NW == NW, "h16 layout geometry");
+  static_assert(L::W_HALVES * 2 == (int)Cfg::W_BYTES && L::S_HALVES * 2 == BS * H * 4, "h16 regions");
   static_assert(G * HS <= NW * 2 * G * 32, "the row scales fit the swap buffer");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float4* W_f = reinterpret_cast<float4*>(smem_raw);                  // [NUG][G][KS][32 lanes] A fragments
@@ -610,7 +626,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   float* scl = red;
   constexpr int NSLOT = F16 ? h16::RING_SLOTS : Cfg::RING_SLOTS;
   auto ring_slot = [&](int s) {
-    return F16 ? reinterpret_cast<float*>(smem_raw + h16::ring_byte(s)) : ring_tail + s * (h16::RING_SLOT_BYTES / 4);
+    return F16 ? reinterpret_cast<float*>(smem_raw + L::ring_byte(s)) : ring_tail + s * (L::RING_SLOT_BYTES / 4);
   };
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
@@ -631,18 +647,29 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     ptx::fence_mbar_init();
   }
   // the prologue is shared by all NT threads, the producer warpgroup included
-  if constexpr (F16) {  // the row scales: one warp per row
-    for (int rr = w; rr < G * HS; rr += NT / 32) {
-      const float4* row = reinterpret_cast<const float4*>(w_hh + ((size_t)(rr / HS) * H + j0 + rr % HS) * H);
-      float m = 0.f;
+  if constexpr (F16) {  // the row scales: each warp reduces SR rows at a time, their loads all in flight
+    constexpr int SR = Cfg::SCALE_ROWS, NR = G * HS;
+    for (int r0 = w * SR; r0 < NR; r0 += SR * (NT / 32)) {
+      float m[SR];
 #pragma unroll
-      for (int k = lane; k < H / 4; k += 32) {
-        const float4 v = __ldg(row + k);
-        m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+      for (int i = 0; i < SR; ++i) {
+        const int rr = SR == 1 ? r0 : min(r0 + i, NR - 1);  // past the last row: a repeat, never stored
+        const float4* row = reinterpret_cast<const float4*>(w_hh + ((size_t)(rr / HS) * H + j0 + rr % HS) * H);
+        m[i] = 0.f;
+#pragma unroll
+        for (int k = lane; k < H / 4; k += 32) {
+          const float4 v = __ldg(row + k);
+          m[i] = fmaxf(m[i], fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+        }
       }
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(FULLMASK, m, o));
-      if (lane == 0) scl[rr] = ldexpf(1.f, h16::scale_exp(m));
+      for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+        for (int i = 0; i < SR; ++i) m[i] = fmaxf(m[i], __shfl_xor_sync(FULLMASK, m[i], o));
+      if (lane == 0)
+#pragma unroll
+        for (int i = 0; i < SR; ++i)
+          if (SR == 1 || r0 + i < NR) scl[r0 + i] = ldexpf(1.f, h16::scale_exp(m[i]));
     }
     __syncthreads();
   }
@@ -661,8 +688,8 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
       for (int e = 0; e < 4; e += 2) {
         const __half2 hi = __floats2half2_rn(x[e], x[e + 1]);
         const __half2 lo = __floats2half2_rn(x[e] - __low2float(hi), x[e + 1] - __high2float(hi));
-        *reinterpret_cast<__half2*>(W_h + h16::w_index(g, u, k0 + e, 0)) = hi;
-        *reinterpret_cast<__half2*>(W_h + h16::w_index(g, u, k0 + e, 1)) = lo;
+        *reinterpret_cast<__half2*>(W_h + L::w_index(g, u, k0 + e, 0)) = hi;
+        *reinterpret_cast<__half2*>(W_h + L::w_index(g, u, k0 + e, 1)) = lo;
       }
     } else {
       float* dst = reinterpret_cast<float*>(W_f + (((u / 16) * G + g) * KS + k0 / 8) * 32 + (u % 8) * 4) +
@@ -706,7 +733,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
           const float* src = gates + ((size_t)t * p.B + row) * (G * H) + j0;
 #pragma unroll
           for (int g = 0; g < G; ++g)
-            ptx::tma_bulk_g2s(slot + h16::ring_index(g, q, 0), src + g * H, (uint32_t)(HS * sizeof(float)), &full[s]);
+            ptx::tma_bulk_g2s(slot + L::ring_index(g, q, 0), src + g * H, (uint32_t)(HS * sizeof(float)), &full[s]);
         }
       }
     }
@@ -719,27 +746,31 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   // ---- lane identity: output jb is unit ju, batch row b0 + 2 * ft + jb (accumulator fragment elements 2*kh + jb) ---
   const int fg = lane >> 2, ft = lane & 3;
   const int u0 = ug * 16 + kh * 8;  // first unit (within the CTA's slice) this warp finishes
-  // F16: the n tile's A fragments of this warp's k-blocks in registers, [slice in visiting order][k-block][hi, lo], and
-  // the unscale 2^-(e_r + 14) of the lane's three rows (read before anyone writes `red` in the step loop)
-  uint32_t wreg[F16 ? C : 1][KBC / 2][2][4];
+  // F16: the last RT tiles' A fragments of this warp's k-blocks in registers (GRU: the n tile; LSTM: g and o),
+  // [tile][slice in visiting order][k-block][hi, lo], and the unscale 2^-(e_r + 14) of the lane's G rows (read before
+  // anyone writes `red` in the step loop)
+  uint32_t wreg[F16 ? RT : 1][F16 ? C : 1][KBC / 2][2][4];
   float unscale[G];
   if constexpr (F16) {
 #pragma unroll
-    for (int c = 0; c < C; ++c)
+    for (int rt = 0; rt < RT; ++rt)
 #pragma unroll
-      for (int kk = 0; kk < KBC / 2; ++kk)
+      for (int c = 0; c < C; ++c)
 #pragma unroll
-        for (int hl = 0; hl < 2; ++hl) {
-          const int kb = ((c + (int)rank) % C) * KBC + kh * (KBC / 2) + kk;
-          const uint4 v = *reinterpret_cast<const uint4*>(W_h + h16::w_half(ug, G - 1, kb, hl, lane, 0, 0));
-          wreg[c][kk][hl][0] = v.x; wreg[c][kk][hl][1] = v.y; wreg[c][kk][hl][2] = v.z; wreg[c][kk][hl][3] = v.w;
-        }
+        for (int kk = 0; kk < KBC / 2; ++kk)
+#pragma unroll
+          for (int hl = 0; hl < 2; ++hl) {
+            const int kb = ((c + (int)rank) % C) * KBC + kh * (KBC / 2) + kk;
+            const uint4 v = *reinterpret_cast<const uint4*>(W_h + L::w_half(ug, G - RT + rt, kb, hl, lane, 0, 0));
+            uint32_t* wr = wreg[rt][c][kk][hl];
+            wr[0] = v.x; wr[1] = v.y; wr[2] = v.z; wr[3] = v.w;
+          }
 #pragma unroll
     for (int g = 0; g < G; ++g) unscale[g] = __frcp_rn(scl[g * HS + u0 + fg]) * (1.f / h16::STATE_SCALE);
   }
   ptx::cluster_sync_all();  // peers' barriers and state buffers are initialised before anyone writes into them
   const int ju = j0 + u0 + fg;
-  FwdCell<B200RNN_GRU, H, VL> cell[2] = {{p, dir, ju, b0 + 2 * ft}, {p, dir, ju, b0 + 2 * ft + 1}};
+  FwdCell<Cfg::MODE, H, VL> cell[2] = {{p, dir, ju, b0 + 2 * ft}, {p, dir, ju, b0 + 2 * ft + 1}};
 
   const float4* W_w = W_f + (size_t)ug * G * KS * 32 + lane;
   float* red_mine = red + w * 2 * G * 32 + lane;                         // written by this warp
@@ -787,16 +818,16 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
 #pragma unroll
           for (int g = 0; g < G; ++g) {
             uint32_t ah[4], al[4];
-            if (g < G - 1) {
-              const uint4* wp = reinterpret_cast<const uint4*>(W_h + h16::w_half(ug, g, kb, 0, lane, 0, 0));
+            if (g < G - RT) {
+              const uint4* wp = reinterpret_cast<const uint4*>(W_h + L::w_half(ug, g, kb, 0, lane, 0, 0));
               const uint4 vh = wp[0], vl = wp[32];  // hi, then lo: 32 lanes x 16 bytes further
               ah[0] = vh.x; ah[1] = vh.y; ah[2] = vh.z; ah[3] = vh.w;
               al[0] = vl.x; al[1] = vl.y; al[2] = vl.z; al[3] = vl.w;
             } else {
 #pragma unroll
               for (int r = 0; r < 4; ++r) {
-                ah[r] = wreg[c][kk][0][r];
-                al[r] = wreg[c][kk][1][r];
+                ah[r] = wreg[g - (G - RT)][c][kk][0][r];
+                al[r] = wreg[g - (G - RT)][c][kk][1][r];
               }
             }
             ptx::mma_f16_m16n8k16(d[g][0], al, bh);
@@ -855,7 +886,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
         for (int jb = 0; jb < 2; ++jb)
           if (cell[jb].valid) {
 #pragma unroll
-            for (int g = 0; g < G; ++g) cell[jb].gi[g] = slot[h16::ring_index(g, 2 * ft + jb, u0 + fg)];
+            for (int g = 0; g < G; ++g) cell[jb].gi[g] = slot[L::ring_index(g, 2 * ft + jb, u0 + fg)];
           }
         __syncwarp();
         if (lane == 0) ptx::mbar_arrive(&empty[s]);
@@ -896,8 +927,8 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
         for (int jb = 0; jb < 2; ++jb) {
           const float v = hnew[jb] * h16::STATE_SCALE;
           const __half hi = __float2half_rn(v);
-          h_h[h16::state_index(ju, 2 * ft + jb, 0)] = hi;
-          h_h[h16::state_index(ju, 2 * ft + jb, 1)] = __float2half_rn(v - __half2float(hi));
+          h_h[L::state_index(ju, 2 * ft + jb, 0)] = hi;
+          h_h[L::state_index(ju, 2 * ft + jb, 1)] = __float2half_rn(v - __half2float(hi));
         }
       } else {
 #pragma unroll
@@ -932,18 +963,23 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
 }
 
-// 3xTF32 (the default), single-pass TF32 and fp16-pair instantiations, fixed-length and ragged
+// GRU-256: 3xTF32 (the default), single-pass TF32 and fp16-pair instantiations, fixed-length and ragged
 template <bool VL>
 __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tc_kernel(const RecFwdParams p, const int nslices) {
-  rec_fwd_tc_body<VL, TcOp::X3>(p, nslices);
+  rec_fwd_tc_body<TcFwdCfg, VL, TcOp::X3>(p, nslices);
 }
 template <bool VL>
 __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_tf32_kernel(const RecFwdParams p, const int nslices) {
-  rec_fwd_tc_body<VL, TcOp::TF32>(p, nslices);
+  rec_fwd_tc_body<TcFwdCfg, VL, TcOp::TF32>(p, nslices);
 }
 template <bool VL>
 __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_h16_kernel(const RecFwdParams p, const int nslices) {
-  rec_fwd_tc_body<VL, TcOp::F16>(p, nslices);
+  rec_fwd_tc_body<TcFwdCfg, VL, TcOp::F16>(p, nslices);
+}
+// LSTM-128: fp16 pairs only (the no-grad forward of b200rnn_forward_fused), fixed-length and ragged
+template <bool VL>
+__global__ void __launch_bounds__(TcLstmCfg::NT, 1) lstm_fwd_h16_kernel(const RecFwdParams p, const int nslices) {
+  rec_fwd_tc_body<TcLstmCfg, VL, TcOp::F16>(p, nslices);
 }
 
 // =================================================================================================
@@ -1685,6 +1721,17 @@ int pick_fwd_tc(const RecFwdParams& p, RecFwdLaunch* L) {
   return rc;
 }
 
+// LSTM-128 on fp16 pairs (lstm_fwd_h16_kernel), the no-grad forward of b200rnn_forward_fused only: 2-CTA clusters of 8
+// batch rows, always taken (several waves when its clusters do not all fit)
+int pick_fwd_tcl(const RecFwdParams& p, RecFwdLaunch* L) {
+  using Cfg = TcLstmCfg;
+  static_assert(Cfg::SMEM <= MAX_SMEM, "forward config does not fit an SM");
+  int rc = B200RNN_OK;
+  pick_clustered(p.lengths ? lstm_fwd_h16_kernel<true> : lstm_fwd_h16_kernel<false>, p, Cfg::C, Cfg::BS, Cfg::NT,
+                 Cfg::SMEM, true, L, &rc, "fwd cfg tcl8 C=%d BS=%d mma.sync f16x3", Cfg::C, Cfg::BS);
+  return rc;
+}
+
 template <int MODE, int H, int C, int BS, int KL, int UPL, int RG>
 bool pick_bwd(const RecBwdParams& p, bool force, RecBwdLaunch* L, int* rc) {
   using Cfg = RecCfg<MODE, H, C, BS, KL, UPL, RG>;
@@ -1788,6 +1835,9 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
     return rc;
   }
   if (p.mode == B200RNN_LSTM && p.H == 128) {
+    // the no-grad fused forward (no initial state, default precision): fp16 pairs on the tensor cores, half the CTAs
+    // of the FFMA config below at the same batch
+    if (p.shell_nograd && !p.tf32) return pick_fwd_tcl(p, L);
     // scalar FFMA
     if (pick_fwd<B200RNN_LSTM, 128, 2, 4, 16, 4, 1>(p, false, L, &rc)) return rc;
     pick_fwd<B200RNN_LSTM, 128, 4, 8, 16, 2, 1>(p, true, L, &rc);

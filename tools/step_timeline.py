@@ -13,7 +13,10 @@ prints, as medians over the replays:
     beside its streamed GEMM); for a recurrence also `after_gemm_start`;
   * its duration, beside its duration when the audio branch runs alone.
 and the end of the text branch (with the text half of the head) relative to the end of the audio chain (negative: the
-text branch ends first). The head kernel after the join is counted in neither.
+text branch ends first). The head kernel after the join is counted in neither. The text-branch kernels (every kernel
+off the audio stream before the join) are listed too, in start order: name, grid, median start and duration, so that
+what runs beside rec0's end and rec1's start can be read off, each beside its duration when the text branch runs
+alone.
 
     python tools/step_timeline.py [--replays 20] [--out DIR]      # default DIR: step_timeline/ in the temp directory
 """
@@ -135,7 +138,28 @@ def _chain_rows(replays):
         rows.append(row)
     text_end = [max((k["end"] for k in o), default=0.0) - a[-1]["end"] for a, o in chains]
     step = [max(k["end"] for k in r) for r in replays]
-    return rows, _median(text_end), _median(step)
+    return rows, _median(text_end), _median(step), _text_rows(chains)
+
+
+def _text_rows(chains):
+    """Per position of the text branch (kernels off the audio stream, in start order): name, grid, median start and
+    duration (µs). Empty when the replays disagree on its kernels."""
+    texts = [o for _, o in chains]
+    n = len(texts[0])
+    if any(len(o) != n or [k["name"] for k in o] != [k["name"] for k in texts[0]] for o in texts):
+        return []
+    return [{"kernel": texts[0][i]["name"], "grid": texts[0][i]["grid"],
+             "start_us": round(_median([o[i]["start"] for o in texts]), 1),
+             "dur_us": round(_median([o[i]["end"] - o[i]["start"] for o in texts]), 1)} for i in range(n)]
+
+
+def _alone_rows(replays):
+    """Per position of a replay that runs one branch alone: name, grid, median duration (µs)"""
+    n = len(replays[0])
+    if any(len(r) != n for r in replays):
+        raise RuntimeError("the branch has a different number of kernels in different replays")
+    return [{"kernel": replays[0][i]["name"], "grid": replays[0][i]["grid"],
+             "dur_us": round(_median([r[i]["end"] - r[i]["start"] for r in replays]), 1)} for i in range(n)]
 
 
 def main():
@@ -169,21 +193,28 @@ def main():
         with torch.no_grad():
             fused._audio_branch(b200rnn.FuseBatch(dev_in[i % bench.N_ROTATE][0], dev_in[i % bench.N_ROTATE][1]))
 
-    whole, audio = _capture(step), _capture(audio_branch)
+    def text_branch(i):
+        with torch.no_grad():
+            fused._text_branch(b200rnn.FuseBatch(dev_in[i % bench.N_ROTATE][0], dev_in[i % bench.N_ROTATE][1]))
+
+    whole, audio, text = _capture(step), _capture(audio_branch), _capture(text_branch)
     mode = "graph"
     runs = {"whole_step": _kernels(lambda i: whole[i % len(whole)].replay(), args.replays, args.warmup,
                                    os.path.join(args.out, "trace_whole.json")),
             "audio_alone": _kernels(lambda i: audio[i % len(audio)].replay(), args.replays, args.warmup,
-                                    os.path.join(args.out, "trace_audio.json"))}
+                                    os.path.join(args.out, "trace_audio.json")),
+            "text_alone": _kernels(lambda i: text[i % len(text)].replay(), args.replays, args.warmup,
+                                   os.path.join(args.out, "trace_text.json"))}
     if len({k["stream"] for k in runs["whole_step"][0]}) < 2:
         # the profiler put every kernel of the graph on the launching stream: fall back to eager steps, whose
         # kernels carry the stream they were enqueued on
         mode = "eager"
         runs = {"whole_step": _kernels(step, args.replays, args.warmup, os.path.join(args.out, "trace_whole.json")),
                 "audio_alone": _kernels(audio_branch, args.replays, args.warmup,
-                                        os.path.join(args.out, "trace_audio.json"))}
-    rows, text_end, step = _chain_rows(runs["whole_step"])
-    alone, _, audio_step = _chain_rows(runs["audio_alone"])
+                                        os.path.join(args.out, "trace_audio.json")),
+                "text_alone": _kernels(text_branch, args.replays, args.warmup, os.path.join(args.out, "trace_text.json"))}
+    rows, text_end, step, text_rows = _chain_rows(runs["whole_step"])
+    alone, _, audio_step, _ = _chain_rows(runs["audio_alone"])
     if len(rows) != len(alone):
         raise RuntimeError("the audio chain differs between the whole step and the audio branch alone")
     for r, a in zip(rows, alone):
@@ -192,7 +223,11 @@ def main():
         r["dur_alone_us"] = a["dur_us"]
         if "gap_us" in a:
             r["gap_alone_us"] = a["gap_us"]
-    summary = {"card": card, "mode": mode, "replays": args.replays, "audio_chain": rows,
+    text_alone = _alone_rows(runs["text_alone"])  # the text half of the head is not part of the text branch alone
+    if [r["kernel"] for r in text_rows[:len(text_alone)]] == [a["kernel"] for a in text_alone]:
+        for r, a in zip(text_rows, text_alone):
+            r["dur_alone_us"] = a["dur_us"]
+    summary = {"card": card, "mode": mode, "replays": args.replays, "audio_chain": rows, "text_branch": text_rows,
                "text_end_minus_audio_end_us": round(text_end, 1), "whole_step_us": round(step, 1),
                "audio_alone_us": round(audio_step, 1)}
     with open(os.path.join(args.out, "step_timeline.json"), "w") as f:
@@ -204,6 +239,12 @@ def main():
         print(f"{r['kernel'][:21]:<22}{str(r['grid']):>16}{r['start_us']:>9}{r.get('gap_us', ''):>9}"
               f"{r.get('gap_alone_us', ''):>11}{r['dur_us']:>9}{r['dur_alone_us']:>11}"
               f"{r.get('after_gemm_start_us', ''):>18}")
+    print(f"{'text kernel':<22}{'grid':>16}{'start':>9}{'dur':>9}{'end':>9}{'dur alone':>11}")
+    for r in text_rows:
+        print(f"{r['kernel'][:21]:<22}{str(r['grid']):>16}{r['start_us']:>9}{r['dur_us']:>9}"
+              f"{round(r['start_us'] + r['dur_us'], 1):>9}{r.get('dur_alone_us', ''):>11}")
+    if not text_rows:
+        print("text alone: " + ", ".join(f"{a['kernel']} {a['grid']} {a['dur_us']}" for a in text_alone))
     print(f"text branch ends {text_end:+.1f} µs after the audio chain; step (first to last kernel) {step:.1f} µs, "
           f"audio branch alone {audio_step:.1f} µs")
     print(json.dumps(summary))
