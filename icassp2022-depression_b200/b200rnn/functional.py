@@ -433,8 +433,9 @@ def rnn_forward_fused(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNN
 
 
 def prepare_weights(weights: Sequence[torch.Tensor], cfg: RNNConfig) -> torch.Tensor:
-    """TF32 hi/lo split of every ``weight_ih`` (``b200rnn_prepare_weights``): the weight cache ``rnn_forward_fused``
-    accepts so that frozen encoders split their weights once instead of once per step."""
+    """TF32 hi/lo and fp16-pair splits of every ``weight_ih`` and, for a unidirectional GRU-256, the fp16 pairs of
+    every ``weight_hh`` (``b200rnn_prepare_weights``): the weight cache ``rnn_forward_fused`` accepts so that frozen
+    encoders split their weights once instead of once per step."""
     lib = _lib.load()
     dev = weights[0].device
     for i, w in enumerate(weights):

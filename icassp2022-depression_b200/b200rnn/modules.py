@@ -157,7 +157,9 @@ class _B200RNNBase(nn.Module):
         return d
 
     def frozen_weight_cache(self):
-        """TF32-split ``weight_ih`` cache for the no-grad fused forward, or None.
+        """Weight cache for the no-grad fused forward, or None: the TF32 and fp16-pair splits of every ``weight_ih``
+        and, for a unidirectional GRU with hidden size 256, each layer's ``weight_hh`` as fp16 pairs in the order its
+        recurrence stages them. Cached and uncached calls run the same operands and give bitwise equal results.
 
         None for an Elman ``RNN``, whose forward has no fused path. Only while EVERY weight of the module is frozen (``requires_grad=False``, the fuse scripts' encoders:
         fuse_net_whole.py:590-593) - nothing this library launches updates such a tensor behind PyTorch's back. The

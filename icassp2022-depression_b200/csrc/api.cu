@@ -262,6 +262,8 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
 // fp16-pair split (gemm_h16_layout.cuh, g16::wcache_layout: the byte offsets, all multiples of 256)
 struct WCacheLayout {
   size_t hi[8][2], lo[8][2], h16[8][2];
+  bool has_whh16;  // GRU-256, D = 1: per layer weight_hh as the fp16-pair recurrence stages it (h16::Gru256)
+  size_t whh16[8];
   size_t total;
 };
 
@@ -273,6 +275,8 @@ void make_wcache(const Dims& d, WCacheLayout* w) {
       w->lo[l][k] = b.lo[l][k] / sizeof(float);
       w->h16[l][k] = b.h16[l][k] / sizeof(float);
     }
+  w->has_whh16 = b.has_whh16;
+  for (int l = 0; l < d.L && l < 8; ++l) w->whh16[l] = b.whh16[l] / sizeof(float);
   w->total = b.total / sizeof(float);
 }
 
@@ -631,6 +635,8 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     rp.tf32 = tf32 ? 1 : 0;
     rp.shell_nograd = shell && !save ? 1 : 0;
     rp.P = d.P;
+    // frozen GRU-256 weights: the fp16-pair recurrence copies its W_hh pairs from the cache instead of splitting them
+    if (WC && wl.has_whh16) rp.whh16[0] = WC + wl.whh16[l];
     RecFwdLaunch rec;
     rc = plan_rec_fwd(rp, &rec);
     if (rc) return rc;
@@ -868,6 +874,15 @@ B200RNN_API int b200rnn_prepare_weights(const b200rnn_desc* desc, const float* c
         rc = tc_split_w16(w_ih, simple_rows(Il), (int)d.GH, Il, WC + wl.h16[l][k], st);
         if (rc) return rc;
       }
+    }
+    if (wl.has_whh16) {  // weight_hh: the pairs the fp16-pair recurrence's prologue makes per launch when uncached
+      const float* w_hh = params[(size_t)l * d.D * 4 + 1];
+      if (!w_hh || !aligned_to(w_hh, 16)) {
+        set_error("prepare_weights: null or misaligned weight_hh (layer %d)", l);
+        return B200RNN_ERR_INVALID;
+      }
+      rc = prep_whh_h16(w_hh, WC + wl.whh16[l], st);
+      if (rc) return rc;
     }
   }
   return B200RNN_OK;

@@ -9,9 +9,13 @@
 //   exp [N]    int    e_n = h16::scale_exp(max_k |w[n][k]|)
 // Weight cache, per (layer l, direction k) in this order: the TF32 hi and lo splits of weight_ih as dense fp32 [N][K_l]
 // (read by the autograd / TF32 forwards of a frozen module), then the fp16-pair split above (the no-grad forward).
+// A unidirectional GRU-256 (D = 1, GH = 3 DH, DH = 256) then has, per layer, weight_hh as the fp16-pair recurrence
+// stages it (rec_h16_layout.cuh, h16::Gru256::CACHE_BYTES).
 #pragma once
 #include <stddef.h>
 #include <string.h>
+
+#include "rec_h16_layout.cuh"
 
 namespace b200rnn {
 namespace g16 {
@@ -57,6 +61,8 @@ static_assert(w16_layout(768, 256).lo % ALIGN == 0 && w16_layout(768, 256).exp %
 // size of layer 0, DH = directions x hidden (input size of every later layer)
 struct WCache {
   size_t hi[MAX_LAYERS][2], lo[MAX_LAYERS][2], h16[MAX_LAYERS][2];
+  bool has_whh16;  // the GRU-256 weight_hh images below exist
+  size_t whh16[MAX_LAYERS];
   size_t total;
 };
 inline WCache wcache_layout(int L, int D, int I, int DH, int GH) {
@@ -72,6 +78,11 @@ inline WCache wcache_layout(int L, int D, int I, int DH, int GH) {
       w.h16[l][k] = off;
       if (shape_ok(GH, Il)) off += w16_layout(GH, Il).bytes;
     }
+  }
+  w.has_whh16 = D == 1 && DH == h16::Gru256::H && GH == h16::Gru256::G * DH;
+  for (int l = 0; w.has_whh16 && l < L && l < MAX_LAYERS; ++l) {
+    w.whh16[l] = off;
+    off += align_up((size_t)h16::Gru256::CACHE_BYTES, ALIGN);
   }
   w.total = off;
   return w;

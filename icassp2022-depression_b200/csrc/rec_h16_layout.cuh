@@ -94,6 +94,14 @@ struct Geom {
   __host__ __device__ static constexpr int ring_byte(int s) {
     return RING_IN_TILE ? w_half(s, G - 1, 0, 0, 0, 0, 0) * 2 : W_HALVES * 2 + 2 * S_HALVES * 2 + RED_BYTES + s * RING_SLOT_BYTES;
   }
+  // Weight cache image of W_hh (b200rnn_prepare_weights, prep_whh_h16): per CTA rank, the weight region exactly as the
+  // prologue of the fp16-pair kernel stages it (W_HALVES halves), then the row scales 2^e_r, e_r = scale_exp(max_k
+  // |w_rk|), of its G * HS rows as fp32 [G][HS], padded to 256 bytes
+  static constexpr int CACHE_SCALE_BYTES = (G * HS * 4 + 255) / 256 * 256;
+  static constexpr int CACHE_RANK_BYTES = W_HALVES * 2 + CACHE_SCALE_BYTES;
+  static constexpr int CACHE_BYTES = C * CACHE_RANK_BYTES;
+  __host__ __device__ static constexpr int cache_rank_byte(int rank) { return rank * CACHE_RANK_BYTES; }
+  static_assert(CACHE_RANK_BYTES % 256 == 0 && (G * HS * 4) % 16 == 0, "16-byte copies, 256-byte aligned ranks");
   static_assert(!RING_IN_TILE || RING_SLOTS <= NUG, "one slot per unit group's n-tile region");
   static_assert(!RING_IN_TILE || RING_SLOT_BYTES <= KB * 2 * 32 * 8 * 2, "a slot fits the n-tile region of one unit group");
   static_assert((RING_ROW * 4) % 16 == 0 && ring_byte(0) % 128 == 0 && ring_byte(1) % 128 == 0,

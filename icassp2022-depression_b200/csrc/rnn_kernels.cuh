@@ -39,6 +39,9 @@ struct RecFwdParams {
   int P;
   const float* w_hr[2];      // per direction [P, H]
   float* m[2];               // per direction [T,B,H] (training only)
+  // optional, the GRU-256 fp16-pair kernel only (D = 1): W_hh of direction 0 already split, as the weight cache holds it
+  // (prep_whh_h16, h16::Gru256 cache image; 16-byte aligned). NULL: the prologue splits W_hh itself
+  const void* whh16[2];
 };
 
 // A recurrence launch chosen for a shape, before anything is enqueued: `nclusters` clusters of C CTAs, of which
@@ -123,6 +126,9 @@ int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out);
 // it with programmatic stream serialization, so that it may start while the GEMM before it still runs
 int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* out);
 int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t stream);
+// W_hh [3*256][256] of a GRU-256 layer (16-byte aligned) -> h16::Gru256::CACHE_BYTES at img (256-byte aligned): the
+// fp16 pairs and row scales the prologue of rec_fwd_h16_kernel would make, in its shared-memory order per CTA rank
+int prep_whh_h16(const float* w_hh, void* img, cudaStream_t stream);
 // backward: the same choice (plan_rec_bwd), then one launch that also prepares W_hh for the unprojected kernels and sets
 // p.nslices_out
 int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* out);

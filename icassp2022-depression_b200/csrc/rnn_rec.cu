@@ -647,6 +647,22 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
     ptx::fence_mbar_init();
   }
   // the prologue is shared by all NT threads, the producer warpgroup included
+  // GRU-256 fp16 pairs from the weight cache (RecFwdParams::whh16, frozen weights): the pairs and row scales the two
+  // passes below would make, copied as they lie
+  bool staged = false;
+  if constexpr (F16 && Cfg::MODE == B200RNN_GRU) {
+    if (p.whh16[dir]) {
+      const uint4* img = reinterpret_cast<const uint4*>(static_cast<const unsigned char*>(p.whh16[dir]) +
+                                                        L::cache_rank_byte((int)rank));
+      uint4* dst = reinterpret_cast<uint4*>(smem_raw);
+#pragma unroll 8
+      for (int i = tid; i < L::W_HALVES * 2 / 16; i += NT) dst[i] = __ldg(img + i);
+      for (int i = tid; i < G * HS / 4; i += NT)
+        reinterpret_cast<uint4*>(scl)[i] = __ldg(img + L::W_HALVES * 2 / 16 + i);
+      staged = true;
+    }
+  }
+  if (!staged) {
   if constexpr (F16) {  // the row scales: each warp reduces SR rows at a time, their loads all in flight
     constexpr int SR = Cfg::SCALE_ROWS, NR = G * HS;
     for (int r0 = w * SR; r0 < NR; r0 += SR * (NT / 32)) {
@@ -699,6 +715,7 @@ __device__ __forceinline__ void rec_fwd_tc_body(const RecFwdParams& p, const int
       dst[8] = TF32 ? round_tf32(v.z) : v.z;
       dst[12] = TF32 ? round_tf32(v.w) : v.w;
     }
+  }
   }
   if (!F16 && p.h_0) {  // buffer 0: the initial state in B-fragment order, rounded like the copies the lanes producing h_t hand over
     for (int i = tid; i < BS * H; i += NT) {
@@ -980,6 +997,42 @@ __global__ void __launch_bounds__(TcFwdCfg::NT, 1) rec_fwd_h16_kernel(const RecF
 template <bool VL>
 __global__ void __launch_bounds__(TcLstmCfg::NT, 1) lstm_fwd_h16_kernel(const RecFwdParams p, const int nslices) {
   rec_fwd_tc_body<TcLstmCfg, VL, TcOp::F16>(p, nslices);
+}
+
+// W_hh [G*H][H] of a GRU-256 layer -> its weight cache image (h16::Gru256, prep_whh_h16), one warp per row: the row
+// scale and split of rec_fwd_tc_body's F16 prologue (the same max, scale and roundings, so the staged pairs are
+// bit-identical), written in each rank's A-fragment order
+__global__ void __launch_bounds__(256) whh_h16_prep_kernel(const float* __restrict__ w_hh, unsigned char* __restrict__ img) {
+  using L = h16::Gru256;
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= L::G * L::H) return;
+  const int g = row / L::H, rank = row % L::H / L::HS, u = row % L::HS;
+  const float4* src = reinterpret_cast<const float4*>(w_hh + (size_t)row * L::H);
+  float4 v[L::H / 128];
+  float m = 0.f;
+#pragma unroll
+  for (int i = 0; i < L::H / 128; ++i) {
+    v[i] = __ldg(src + lane + 32 * i);
+    m = fmaxf(m, fmaxf(fmaxf(fabsf(v[i].x), fabsf(v[i].y)), fmaxf(fabsf(v[i].z), fabsf(v[i].w))));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(FULLMASK, m, o));
+  const float s = ldexpf(1.f, h16::scale_exp(m));
+  unsigned char* base = img + L::cache_rank_byte(rank);
+  __half* W = reinterpret_cast<__half*>(base);
+#pragma unroll
+  for (int i = 0; i < L::H / 128; ++i) {
+    const int k0 = (lane + 32 * i) * 4;
+    const float x[4] = {v[i].x * s, v[i].y * s, v[i].z * s, v[i].w * s};
+#pragma unroll
+    for (int e = 0; e < 4; e += 2) {
+      const __half2 hi = __floats2half2_rn(x[e], x[e + 1]);
+      const __half2 lo = __floats2half2_rn(x[e] - __low2float(hi), x[e + 1] - __high2float(hi));
+      *reinterpret_cast<__half2*>(W + L::w_index(g, u, k0 + e, 0)) = hi;
+      *reinterpret_cast<__half2*>(W + L::w_index(g, u, k0 + e, 1)) = lo;
+    }
+  }
+  if (lane == 0) reinterpret_cast<float*>(base + L::W_HALVES * 2)[g * L::HS + u] = s;
 }
 
 // =================================================================================================
@@ -1890,6 +1943,14 @@ int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
   if (anyh_hidden_size(p.H)) return plan_anyh_bwd(p, L);
   set_error("recurrence backward: unsupported (mode=%d, hidden_size=%d)", p.mode, p.H);
   return B200RNN_ERR_UNSUPPORTED;
+}
+
+int prep_whh_h16(const float* w_hh, void* img, cudaStream_t s) {
+  using L = h16::Gru256;
+  whh_h16_prep_kernel<<<L::G * L::H / 8, 256, 0, s>>>(w_hh, static_cast<unsigned char*>(img));
+  B200_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return B200RNN_OK;
 }
 
 int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s) {
