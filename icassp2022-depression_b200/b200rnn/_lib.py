@@ -21,6 +21,8 @@ FLAG_FUSED_LN = 4
 FLAG_TF32 = 8
 FLAG_PROJ = 16      # the descriptor carries proj_size (read only with this flag)
 FLAG_NO_BIAS = 32   # cells only: bias=False
+FLAG_F16 = 64       # x, parameters, states, outputs and gradients are float16 (the reserve and scratch stay fp32)
+FLAG_BF16 = 128     # ... bfloat16
 ABI_VERSION = 4
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)
@@ -311,6 +313,17 @@ def load() -> ctypes.CDLL:
         raise B200RNNError(f"ABI mismatch: library {v}, binding {ABI_VERSION}")
     _lib = lib
     return lib
+
+
+H16_DTYPES = {"torch.float16": FLAG_F16, "torch.bfloat16": FLAG_BF16}
+
+
+def require_fp32_params(params, what: str) -> None:
+    """The model-shell fusions and the flat fp32 optimiser buckets take fp32 parameters only: raise for any other."""
+    for p in params:
+        if p.dtype.is_floating_point and str(p.dtype) != "torch.float32":
+            raise B200RNNError(f"b200rnn: {what} takes float32 parameters (got {p.dtype}); 16-bit modules run through "
+                               "their own forward and autograd, without this fusion")
 
 
 def check(rc: int, what: str) -> None:

@@ -14,6 +14,7 @@ from typing import Iterable, List, Optional
 import torch
 import torch.distributed as dist
 
+from . import _lib
 from .modules import _B200RNNBase
 
 
@@ -45,6 +46,7 @@ class GradBucket:
         self.params: List[torch.nn.Parameter] = [p for p in model.parameters() if p.requires_grad]
         if not self.params:
             raise ValueError("GradBucket: the model has no trainable parameter")
+        _lib.require_fp32_params(self.params, "GradBucket")
         dev = self.params[0].device
         offs, total = _aligned_offsets(self.params)
         self.numel = total

@@ -28,6 +28,7 @@ class RNNConfig:
     batch_first: bool
     tf32: bool = False   # single-pass TF32 tensor-core GEMMs / tc8 recurrence (tf32_enabled()), else 3xTF32
     proj_size: int = 0   # LSTM with projections: width P of h_t (0 = none)
+    dtype: torch.dtype = torch.float32   # of x, the parameters, the states and every output (16-bit: FLAG_F16 / _BF16)
 
     @property
     def out_size(self) -> int:
@@ -56,6 +57,19 @@ def _require_cuda_f32(t: torch.Tensor, name: str) -> None:
         raise _lib.B200RNNError(f"b200rnn: {name} must be float32 (got {t.dtype})")
 
 
+def _require_cuda_dtype(t: torch.Tensor, name: str, dtype: torch.dtype) -> None:
+    """float32 calls: as _require_cuda_f32. 16-bit calls: every tensor has the parameters' dtype"""
+    if dtype == torch.float32:
+        _require_cuda_f32(t, name)
+        return
+    if not t.is_cuda:
+        raise _lib.NoCPUPathError(
+            f"b200rnn: {name} is on {t.device}; this library runs on CUDA (sm_90a) only and has no CPU path"
+        )
+    if t.dtype != dtype:
+        raise _lib.B200RNNError(f"b200rnn: {name} must be {dtype} like the first weight (got {t.dtype})")
+
+
 def _tm_view(x: torch.Tensor) -> torch.Tensor:
     """Return a logical [T,B,F] tensor whose feature stride is 1 (copy only if it is not)."""
     if x.stride(2) != 1 and x.size(2) != 1:
@@ -76,6 +90,7 @@ def _make_desc(cfg: RNNConfig, B: int, T: int, save: bool, accumulate: bool = Fa
         flags |= _lib.FLAG_TF32
     if cfg.proj_size:
         flags |= _lib.FLAG_PROJ
+    flags |= _lib.H16_DTYPES.get(str(cfg.dtype), 0)
     return _lib.Desc(cfg.mode, B, T, cfg.input_size, cfg.hidden_size, cfg.num_layers, cfg.num_dirs,
                      1 if cfg.training else 0, float(cfg.dropout), flags, cfg.proj_size)
 
@@ -95,14 +110,15 @@ def _on(device):
 def _weight_grad_targets(weights, needed, sink, dev):
     """Where a backward writes the weight gradients, as ``(dptrs, grads_out, accumulate)``: straight into the views
     ``sink(weights)`` returns (a flat all-reduce bucket; the kernels accumulate into them, ``grads_out`` is all None),
-    or into one fresh flat buffer whose views are returned to autograd. ``needed[i]``: whether ``weights[i]`` wants a
-    gradient (a NULL target otherwise). Each fresh view starts on a 64-float (256-byte) boundary."""
+    or into one fresh flat buffer (in the weights' dtype) whose views are returned to autograd. ``needed[i]``: whether
+    ``weights[i]`` wants a gradient (a NULL target otherwise). Each fresh view starts on a 256-byte boundary."""
     if sink is not None:
         targets = sink(weights)  # list of tensors (same shapes) or None entries
         dptrs = [t.data_ptr() if (t is not None and n) else None for t, n in zip(targets, needed)]
         return dptrs, [None] * len(weights), True
-    sizes = [(w.numel() + 63) // 64 * 64 if n else 0 for w, n in zip(weights, needed)]
-    flat = torch.empty(sum(sizes), dtype=torch.float32, device=dev)
+    align = 256 // weights[0].element_size()
+    sizes = [(w.numel() + align - 1) // align * align if n else 0 for w, n in zip(weights, needed)]
+    flat = torch.empty(sum(sizes), dtype=weights[0].dtype, device=dev)
     grads_out, off = [], 0
     for w, n, size in zip(weights, needed, sizes):
         grads_out.append(flat[off:off + w.numel()].view_as(w) if n else None)
@@ -133,14 +149,15 @@ class _RNNFunction(torch.autograd.Function):
         rbytes, sbytes = _lib.workspace_bytes(desc)
         reserve = torch.empty(rbytes if save else 0, dtype=torch.uint8, device=dev)
         scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+        dt = cfg.dtype
         if cfg.batch_first:
-            y = torch.empty(B, T, D * HO, dtype=torch.float32, device=dev)
+            y = torch.empty(B, T, D * HO, dtype=dt, device=dev)
             ys_t, ys_b = D * HO, T * D * HO
         else:
-            y = torch.empty(T, B, D * HO, dtype=torch.float32, device=dev)
+            y = torch.empty(T, B, D * HO, dtype=dt, device=dev)
             ys_t, ys_b = B * D * HO, D * HO
-        h_n = torch.empty(L * D, B, HO, dtype=torch.float32, device=dev)
-        c_n = torch.empty(L * D, B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
+        h_n = torch.empty(L * D, B, HO, dtype=dt, device=dev)
+        c_n = torch.empty(L * D, B, H, dtype=dt, device=dev) if cfg.mode == _lib.LSTM else None
         params = _lib.ptr_array([w.data_ptr() for w in weights])
         rng_ptr = rng_state.data_ptr() if rng_state is not None else None
         len_ptr = lengths.data_ptr() if lengths is not None else None
@@ -200,7 +217,7 @@ class _RNNFunction(torch.autograd.Function):
         need_dx = ctx.needs_input_grad[0]
         dx = torch.empty_like(x_tm) if need_dx else None
         if dx is not None and dx.stride(2) != 1 and dx.size(2) != 1:
-            dx = torch.empty(x_tm.shape, dtype=torch.float32, device=dev)
+            dx = torch.empty(x_tm.shape, dtype=x_tm.dtype, device=dev)
 
         dptrs, grads_out, accumulate = _weight_grad_targets(weights, ctx.needs_input_grad[w0:], ctx.grad_sink, dev)
         desc = _make_desc(cfg, B, T, True, accumulate)
@@ -361,12 +378,17 @@ def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig
 
     Returns ``(y, h_n)`` for GRU and RNN and ``(y, h_n, c_n)`` for LSTM, laid out like torch.nn.GRU/LSTM/RNN outputs.
     """
+    if cfg.dtype != torch.float32 and x.dtype != cfg.dtype:   # torch's check_input, before the state checks
+        raise ValueError(f"RNN input dtype ({x.dtype}) does not match weight dtype ({cfg.dtype}). "
+                         f"Convert input: input.to({cfg.dtype}), or convert model: model.to({x.dtype})")
     h_0, c_0 = _initial_state(hx, cfg, x)
-    _require_cuda_f32(x, "input")
+    _require_cuda_dtype(x, "input", cfg.dtype)
     if x.dim() != 3:
         raise NotImplementedError("b200rnn: only batched 3-D input is supported (the reference never uses 2-D)")
+    if cfg.dtype != torch.float32 and cfg.proj_size:
+        raise NotImplementedError("b200rnn: proj_size is float32 only")
     for i, w in enumerate(weights):
-        _require_cuda_f32(w, f"weight[{i}]")
+        _require_cuda_dtype(w, f"weight[{i}]", cfg.dtype)
         if not w.is_contiguous():
             raise _lib.B200RNNError(f"b200rnn: weight[{i}] must be contiguous")
     if x.size(2) != cfg.input_size:

@@ -170,6 +170,7 @@ class FusedFuseStep:
         self.model = model
         self.lr, self.betas, self.eps = float(lr), (float(betas[0]), float(betas[1])), float(eps)
         w = model.fc_final[0].weight
+        _lib.require_fp32_params(model.parameters(), "FusedFuseStep")
         _require_cuda(("model (fc_final.0.weight)", w))
         dev = w.device
         self.w = w

@@ -16,7 +16,13 @@ call) and unbatched 2-D input. ``hidden_size`` is any multiple of 16 from 16 to 
 fixed-size kernels, every other size the runtime-sized cluster kernels (csrc/rnn_anyh.cu); other sizes raise
 ``B200RNNError`` at the first forward. ``LSTM(..., proj_size=P)`` (LSTMP: ``h_t = W_hr (o_t * tanh c_t)``) runs on its own
 projected kernels for P in {H/4, H/2} and registers ``weight_hr_l{k}[_reverse]`` last, as torch does. Features that
-raise ``NotImplementedError``: bias=False, and other projection sizes. A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
+raise ``NotImplementedError``: bias=False, and other projection sizes.
+
+``dtype=torch.float16`` / ``torch.bfloat16`` (or ``.half()``, ``.bfloat16()``, ``.to(dtype)``) gives a 16-bit module:
+input, ``hx``, outputs and gradients in that dtype, the input projection on native 16-bit tensor cores, ``weight_hh``
+kept 16-bit by the runtime-sized recurrence, the state carried in fp32 (DESIGN.md "16-bit modules"). It has every
+feature above except ``proj_size`` and the model-shell fusions (``forward_ln_sum`` computes it unfused,
+``frozen_weight_cache`` is None). A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
 
 ``RNN(..., nonlinearity='tanh' | 'relu')`` (the Elman network) takes the same inputs and features at every one of
 those hidden sizes on the runtime-sized kernels (csrc/rnn_anyh.cu, one gate block); it has no model-shell fusion
@@ -62,8 +68,10 @@ class _B200RNNBase(nn.Module):
             raise NotImplementedError(
                 f"b200rnn: proj_size={proj_size} with hidden_size={hidden_size} is not implemented; the projected LSTM "
                 "kernels take hidden_size 128 with proj_size 32 or 64, and hidden_size 256 with proj_size 64 or 128")
-        if dtype not in (None, torch.float32):
-            raise NotImplementedError("b200rnn: float32 only")
+        if dtype not in (None, torch.float32, torch.float16, torch.bfloat16):
+            raise NotImplementedError("b200rnn: the sequence modules take float32, float16 and bfloat16")
+        if proj_size > 0 and dtype in (torch.float16, torch.bfloat16):
+            raise NotImplementedError("b200rnn: proj_size is float32 only")
         if not isinstance(dropout, (int, float)) or not 0 <= dropout <= 1 or isinstance(dropout, bool):
             raise ValueError("dropout should be a number in range [0, 1] representing the probability of an "
                              "element being zeroed")
@@ -97,7 +105,7 @@ class _B200RNNBase(nn.Module):
                 for name, shape in zip(names, shapes):
                     pname = name.format(layer, suffix)
                     self.register_parameter(
-                        pname, nn.Parameter(torch.empty(shape, dtype=torch.float32, device=device)))
+                        pname, nn.Parameter(torch.empty(shape, dtype=dtype or torch.float32, device=device)))
                     self._flat_weights_names.append(pname)
         # device-resident Philox state {seed, offset} of the inter-layer dropout; advanced by the kernels so a
         # captured CUDA graph draws a new mask per replay. Not part of the state_dict.
@@ -166,7 +174,8 @@ class _B200RNNBase(nn.Module):
         cache is keyed on the parameters' storage addresses and version counters, so ``load_state_dict``, ``.to()`` or
         an in-place edit refresh it; trainable modules never use it (their weights change every step anyway)."""
         ws = self._flat_weights
-        if any(w.requires_grad for w in ws) or not ws[0].is_cuda or self.proj_size or self._gates == 1:
+        if (any(w.requires_grad for w in ws) or not ws[0].is_cuda or self.proj_size or self._gates == 1 or
+                ws[0].dtype != torch.float32):
             self._wcache = None
             return None
         key = tuple((w.data_ptr(), w._version) for w in ws)
@@ -182,7 +191,7 @@ class _B200RNNBase(nn.Module):
         return RNNConfig(mode=self._mode, input_size=self.input_size, hidden_size=self.hidden_size,
                          num_layers=self.num_layers, num_dirs=2 if self.bidirectional else 1,
                          dropout=self.dropout, training=self.training, batch_first=self.batch_first,
-                         tf32=tf32_enabled(), proj_size=self.proj_size)
+                         tf32=tf32_enabled(), proj_size=self.proj_size, dtype=self._flat_weights[0].dtype)
 
     def _run_packed(self, packed, hx):
         """PackedSequence path (ragged DAIC-style sequences): pad, run with per-sequence lengths, re-pack exactly like
@@ -252,6 +261,7 @@ class _B200RNNBase(nn.Module):
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
         shape_ok = (input.is_cuda and input.dim() == 3 and self.proj_size == 0 and self._gates > 1 and
+                    self._flat_weights[0].dtype == torch.float32 and
                     self.hidden_size in (128, 256) and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and
                                     ln.bias is not None)))

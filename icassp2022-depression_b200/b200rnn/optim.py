@@ -51,6 +51,7 @@ class FlatAdamW:
         self.lr, self.betas, self.eps = float(lr), (float(betas[0]), float(betas[1])), float(eps)
         plist = [([p for p in g["params"] if p.requires_grad], g.get("weight_decay", 0.0))
                  for g in groups if any(p.requires_grad for p in g["params"])]
+        _lib.require_fp32_params([p for ps, _ in plist for p in ps], "FlatAdamW")
         dev = plist[0][0][0].device
         sizes = [(_aligned_offsets(ps)[1] + 63) // 64 * 64 for ps, _ in plist]
         # every group's gradients live in ONE contiguous bucket: the data-parallel step all-reduces it with a single

@@ -80,6 +80,7 @@ class TrainStep:
                  loss: Union[str, Callable] = "softmax_ce", y_dtype=torch.int64, use_graph: bool = True,
                  input_requires_grad: bool = True):
         p0 = next(model.parameters())
+        _lib.require_fp32_params(model.parameters(), "TrainStep")
         if not p0.is_cuda:
             raise _lib.B200RNNError("b200rnn.TrainStep: the model is not on a CUDA device - no CPU path")
         self.model, self.opt, self.loss_kind = model, optimizer, loss

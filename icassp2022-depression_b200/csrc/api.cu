@@ -14,6 +14,7 @@
 #include "cell_kernels.cuh"
 #include "gemm_f32.cuh"
 #include "gemm_h16_layout.cuh"
+#include "h16.cuh"
 #include "misc_kernels.cuh"
 #include "rnn_kernels.cuh"
 
@@ -43,6 +44,11 @@ inline int desc_proj(const b200rnn_desc* d) { return (d->flags & B200RNN_FLAG_PR
 // GRU / LSTM at the fixed hidden sizes 128 and 256: their fusions (LayerNorm prologue, pooling, weight cache, the
 // fp16-pair no-grad recurrence) are built for those
 int check_shell_desc(const b200rnn_desc* d, const char* what) {
+  if (d && (d->flags & (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16))) {
+    set_error("%s: the model-shell entry points and the weight cache are float32 only (use the _hx entry points for "
+              "16-bit tensors)", what);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   if (d && is_elman(d->mode)) {
     set_error("%s: the model-shell entry points take the GRU and the LSTM (got mode %d; use the _hx entry points)",
               what, d->mode);
@@ -62,6 +68,7 @@ struct Dims {
   size_t TB, GH, DH;  // DH = D * HO: width of a layer's output
   bool training;
   float p;
+  int dt;  // DT_F32, or DT_F16 / DT_BF16: the caller's tensors are 16-bit (B200RNN_FLAG_F16 / _BF16)
 };
 
 int check_desc(const b200rnn_desc* d, Dims* o) {
@@ -97,6 +104,15 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
               "proj_size hidden_size/4 and hidden_size/2", P);
     return B200RNN_ERR_UNSUPPORTED;
   }
+  const uint32_t h16 = d->flags & (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16);
+  if (h16 == (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16)) {
+    set_error("B200RNN_FLAG_F16 and B200RNN_FLAG_BF16 exclude each other");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  if (h16 && P > 0) {
+    set_error("proj_size is float32 only (B200RNN_FLAG_F16 / _BF16 with B200RNN_FLAG_PROJ)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   if (!(d->dropout_p >= 0.f && d->dropout_p <= 1.f)) {
     set_error("dropout_p must be in [0,1] (got %f)", (double)d->dropout_p);
     return B200RNN_ERR_INVALID;
@@ -117,6 +133,7 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
   o->DH = (size_t)o->D * o->HO;
   o->training = d->training != 0;
   o->p = d->dropout_p;
+  o->dt = h16 == B200RNN_FLAG_F16 ? DT_F16 : h16 == B200RNN_FLAG_BF16 ? DT_BF16 : DT_F32;
   return B200RNN_OK;
 }
 
@@ -128,6 +145,9 @@ struct ReserveLayout {
   size_t m[8][2];                   // proj_size > 0: o * tanh(c) of every step, [T,B,H] (operand of dW_hr)
   size_t ylayer[8], ydrop[8];
   size_t xln;  // LayerNorm(x) of the folded prologue, kept for the layer-0 wgrad (B200RNN_FLAG_FUSED_LN)
+  // 16-bit calls, behind the fp32 layout: the input of layer l + 1 as its GEMM read it (rounded, dropped, rounded
+  // again; widened), and the top layer's fp32 output (the BPTT's h_{t-1}; the caller's y is rounded)
+  size_t xin[8], ytop;
   size_t total;
 };
 
@@ -154,6 +174,12 @@ int make_reserve(const Dims& d, ReserveLayout* r, bool fused_ln = false) {
   }
   r->xln = off;
   if (fused_ln) off += align_up(d.TB * (size_t)d.I, ALIGN_F);
+  for (int l = 0; l + 1 < d.L; ++l) {
+    r->xin[l] = off;
+    if (d.dt) off += align_up(d.TB * d.DH, ALIGN_F);
+  }
+  r->ytop = off;
+  if (d.dt) off += align_up(d.TB * d.DH, ALIGN_F);
   r->total = off;
   return B200RNN_OK;
 }
@@ -179,6 +205,40 @@ struct ScratchLayout {
   // and the backward each compute it from `lengths`
   size_t order;
 };
+
+// ---- 16-bit calls: fp32 copies behind the scratch layout (floats, from `base`) ---------------------------------------
+// forward: the widened biases of every (layer, direction) and the W_hh of one layer's directions (fixed configs), the
+//          widened h_0 / c_0, the fp32 h_n / c_n, the 16-bit input of the next layer (a16), and without a reserve the
+//          rounded inputs and the top layer's fp32 output
+// backward: x, dy, the states and their gradients, every parameter and gradient, dx, all fp32
+struct H16Scratch {
+  size_t bias[8][2], whh, h0, c0, hn, cn, a16, xin, ytop;
+  size_t x32, dy32, dhn, dcn, bh0, bc0, dh0, dc0, w32[8][2], dw32[8][2], dx32;
+  size_t total;
+};
+
+void make_h16_scratch(const Dims& d, size_t base, H16Scratch* h) {
+  size_t off = base;
+  auto take = [&](size_t n) { const size_t at = off; off += align_up(n, ALIGN_F); return at; };
+  const size_t st = (size_t)d.L * d.D * d.B * d.H;
+  for (int l = 0; l < d.L && l < 8; ++l)
+    for (int k = 0; k < d.D; ++k) h->bias[l][k] = take(2 * d.GH);
+  h->whh = take((size_t)d.D * d.GH * d.H);
+  h->h0 = take(st); h->c0 = take(st); h->hn = take(st); h->cn = take(st);
+  h->a16 = take((d.TB * (d.I > (int)d.DH ? (size_t)d.I : d.DH) + 1) / 2);
+  h->xin = take(d.TB * d.DH);
+  h->ytop = take(d.TB * d.DH);
+  h->x32 = take(d.TB * d.I); h->dy32 = take(d.TB * d.DH);
+  h->dhn = take(st); h->dcn = take(st); h->bh0 = take(st); h->bc0 = take(st); h->dh0 = take(st); h->dc0 = take(st);
+  for (int l = 0; l < d.L && l < 8; ++l)
+    for (int k = 0; k < d.D; ++k) {
+      const size_t n = d.GH * (l == 0 ? (size_t)d.I : d.DH) + d.GH * d.H + 2 * d.GH;
+      h->w32[l][k] = take(n);
+      h->dw32[l][k] = take(n);
+    }
+  h->dx32 = take(d.TB * d.I);
+  h->total = off;
+}
 
 // split-K partials of the tensor-core gradient GEMMs: <= (#SMs / tiles) * M * N floats
 constexpr size_t TC_PART_BYTES = (size_t)160 * 128 * 128 * sizeof(float);
@@ -508,8 +568,14 @@ B200RNN_API int b200rnn_workspace_bytes(const b200rnn_desc* desc, size_t* reserv
   if (rc) return rc;
   ScratchLayout s;
   make_scratch(d, &s);
+  size_t stotal = s.f_total > s.b_total ? s.f_total : s.b_total;
+  if (d.dt) {
+    H16Scratch h;
+    make_h16_scratch(d, stotal, &h);
+    stotal = h.total;
+  }
   if (reserve_bytes) *reserve_bytes = (r.total + ALIGN_F) * sizeof(float);
-  if (scratch_bytes) *scratch_bytes = ((s.f_total > s.b_total ? s.f_total : s.b_total) + ALIGN_F) * sizeof(float);
+  if (scratch_bytes) *scratch_bytes = (stotal + ALIGN_F) * sizeof(float);
   return B200RNN_OK;
 }
 
@@ -595,6 +661,41 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     rc = launch_length_order(lengths, d.B, order, st);
     if (rc) return rc;
   }
+  // 16-bit call: the fp32 kernels read exact fp32 copies of the biases and states; h_n / c_n (and y) are produced in
+  // fp32 and rounded once at the end, the input projection reads the 16-bit operands natively
+  const int dt = d.dt;
+  H16Scratch hs;
+  void* const y16 = y;
+  void* const hn16 = h_n;
+  void* const cn16 = c_n;
+  if (dt) {
+    make_h16_scratch(d, sl.b_total, &hs);
+    for (int l = 0; l < d.L; ++l)
+      for (int k = 0; k < d.D; ++k) {
+        const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
+        if (!pp[2] || !pp[3]) {
+          set_error("forward: null parameter pointer (layer %d dir %d)", l, k);
+          return B200RNN_ERR_INVALID;
+        }
+        for (int i = 0; i < 2; ++i) {
+          rc = launch_widen16(pp[2 + i], simple_rows(d.GH), 1, (int)d.GH, dt, S + hs.bias[l][k] + i * d.GH, st);
+          if (rc) return rc;
+        }
+      }
+    const int nst = d.L * d.D * d.B;
+    if (h_0) {
+      rc = launch_widen16(h_0, simple_rows(d.H), nst, d.H, dt, S + hs.h0, st);
+      if (rc) return rc;
+      h_0 = S + hs.h0;
+    }
+    if (c_0) {
+      rc = launch_widen16(c_0, simple_rows(d.H), nst, d.H, dt, S + hs.c0, st);
+      if (rc) return rc;
+      c_0 = S + hs.c0;
+    }
+    h_n = S + hs.hn;
+    if (c_n) c_n = S + hs.cn;
+  }
 
   const bool tc = tc_available();
   const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0;  // single-pass TF32 GEMMs and tc8 recurrence
@@ -624,7 +725,21 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         in = S + sl.f_y[(l - 1) & 1];
       in_rows = simple_rows((long long)d.DH);
     }
-    const bool tc_layer = tc && (Il % 32 == 0) && (d.GH % 128 == 0);
+    const bool tc_layer = !dt && tc && (Il % 32 == 0) && (d.GH % 128 == 0);
+    // 16-bit: the A operand of the native input projection, read in place when the TMA can (else a dense copy)
+    const void* a16 = l == 0 ? static_cast<const void*>(x) : S + hs.a16;
+    RowMap a16_rows = l == 0 ? tb_rows(xs_t, xs_b, d.B) : simple_rows((long long)d.DH);
+    bool n16 = false;
+    if (dt) {
+      n16 = tc && tc_gemm_n16_ok(a16, a16_rows, params[(size_t)l * d.D * d.NPAR], (int)d.TB, (int)d.GH, Il);
+      if (!n16 && l == 0 && tc && tc_gemm_n16_ok(S + hs.a16, simple_rows(Il), params[0], (int)d.TB, (int)d.GH, Il)) {
+        rc = launch_copy16(x, a16_rows, (int)d.TB, Il, S + hs.a16, st);
+        if (rc) return rc;
+        a16 = S + hs.a16;
+        a16_rows = simple_rows(Il);
+        n16 = true;
+      }
+    }
     // ---- the recurrence config, chosen before anything of the layer is enqueued
     RecFwdParams rp;
     memset(&rp, 0, sizeof(rp));
@@ -638,7 +753,8 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     // frozen GRU-256 weights: the fp16-pair recurrence copies its W_hh pairs from the cache instead of splitting them
     if (WC && wl.has_whh16) rp.whh16[0] = WC + wl.whh16[l];
     RecFwdLaunch rec;
-    rc = plan_rec_fwd(rp, &rec);
+    // 16-bit: the runtime-sized kernels read weight_hh as it lies; the fixed configs get fp32 copies below
+    rc = plan_rec_fwd(rp, &rec, dt);
     if (rc) return rc;
     // Stream the input projection into the recurrence (DESIGN.md §4): the GEMM runs beside the recurrence and publishes
     // its row tiles in time order, the recurrence starts while it runs and waits per step for the tiles it reads. Only
@@ -690,39 +806,73 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         return B200RNN_ERR_INVALID;
       }
       float* gates = save ? R + rl.gates[l][k] : S + sl.f_gates[k];
-      // K1: x-projection of every time step at once, biases folded (GRU: b_hh only for r,z; LSTM, Elman: all of it)
-      GemmParams g;
-      memset(&g, 0, sizeof(g));
-      g.A = a_in; g.a_rows = a_rows; g.a_kcontig = 1;
-      g.B = w_ih; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
-      g.C = gates; g.c_rows = simple_rows((long long)d.GH);
-      g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
-      g.bias1 = b_ih; g.bias2 = b_hh;
-      g.bias2_n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
-      if (tc_layer) {
-        g.tc_ws = tc_ws;
-        g.tc_ws_bytes = sl.f_tc_bytes;
-        g.tc_a_f32 = 1;
-        g.tc_tf32 = tf32 ? 1 : 0;
-        // the no-grad forward of b200rnn_forward_fused in default precision: fp16 pairs (the rule of the fp16-pair
-        // recurrence, RecFwdParams::shell_nograd)
-        g.tc_h16 = rp.shell_nograd && !tf32 && g16::shape_ok((int)d.GH, Il) ? 1 : 0;
-        if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders); TF32 reads only hi
-          g.tc_b_hi = WC + wl.hi[l][k];
-          g.tc_b_lo = tf32 ? nullptr : WC + wl.lo[l][k];
-          if (g.tc_h16) g.tc_b_h16 = WC + wl.h16[l][k];
+      if (dt) {  // K1 on 16-bit operands: native f16 / bf16 wgmma, else the FFMA GEMM on exact fp32 copies
+        const float* b32 = S + hs.bias[l][k];
+        const int b2n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
+        // each direction's weight_ih checked on its own: one the TMA cannot read takes the FFMA GEMM
+        if (n16 && tc_gemm_n16_ok(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il)) {
+          rc = tc_gemm_n16(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il, dt, gates, simple_rows((long long)d.GH), b32,
+                           b32 + d.GH, b2n, st);
+        } else {
+          float* aw = S + sl.f_tc;
+          float* ww = aw + align_up(d.TB * Il, ALIGN_F);
+          rc = launch_widen16(a16, a16_rows, (int)d.TB, Il, dt, aw, st);
+          if (!rc) rc = launch_widen16(w_ih, simple_rows(Il), (int)d.GH, Il, dt, ww, st);
+          if (rc) return rc;
+          GemmParams g;
+          memset(&g, 0, sizeof(g));
+          g.A = aw; g.a_rows = simple_rows(Il); g.a_kcontig = 1;
+          g.B = ww; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
+          g.C = gates; g.c_rows = simple_rows((long long)d.GH);
+          g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
+          g.bias1 = b32; g.bias2 = b32 + d.GH; g.bias2_n = b2n;
+          rc = launch_gemm(g, nullptr, 0, st);
         }
-        if (stream_xproj && gemm_tc_eligible(g, g.tc_ws_bytes)) {
-          g.tc_ready = ready;
-          g.tc_stream_clusters = gemm_clusters;
-          rp.ready = ready;
-          rp.tiles_n = (int)d.GH / TC_TILE_N;
+        if (rc) return rc;
+      } else {
+        // K1: x-projection of every time step at once, biases folded (GRU: b_hh only for r,z; LSTM, Elman: all of it)
+        GemmParams g;
+        memset(&g, 0, sizeof(g));
+        g.A = a_in; g.a_rows = a_rows; g.a_kcontig = 1;
+        g.B = w_ih; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
+        g.C = gates; g.c_rows = simple_rows((long long)d.GH);
+        g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
+        g.bias1 = b_ih; g.bias2 = b_hh;
+        g.bias2_n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
+        if (tc_layer) {
+          g.tc_ws = tc_ws;
+          g.tc_ws_bytes = sl.f_tc_bytes;
+          g.tc_a_f32 = 1;
+          g.tc_tf32 = tf32 ? 1 : 0;
+          // the no-grad forward of b200rnn_forward_fused in default precision: fp16 pairs (the rule of the fp16-pair
+          // recurrence, RecFwdParams::shell_nograd)
+          g.tc_h16 = rp.shell_nograd && !tf32 && g16::shape_ok((int)d.GH, Il) ? 1 : 0;
+          if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders); TF32 reads only hi
+            g.tc_b_hi = WC + wl.hi[l][k];
+            g.tc_b_lo = tf32 ? nullptr : WC + wl.lo[l][k];
+            if (g.tc_h16) g.tc_b_h16 = WC + wl.h16[l][k];
+          }
+          if (stream_xproj && gemm_tc_eligible(g, g.tc_ws_bytes)) {
+            g.tc_ready = ready;
+            g.tc_stream_clusters = gemm_clusters;
+            rp.ready = ready;
+            rp.tiles_n = (int)d.GH / TC_TILE_N;
+          }
         }
+        rc = launch_gemm(g, nullptr, 0, st);
+        if (rc) return rc;
       }
-      rc = launch_gemm(g, nullptr, 0, st);
-      if (rc) return rc;
       rp.w_hh[k] = w_hh;
       rp.b_hh[k] = b_hh;
+      if (dt) {
+        rp.b_hh[k] = S + hs.bias[l][k] + d.GH;
+        if (!rec.anyh) {  // the fixed configs read fp32: an exact copy per direction
+          float* w32 = S + hs.whh + (size_t)k * d.GH * d.H;
+          rc = launch_widen16(w_hh, simple_rows(d.H), (int)d.GH, d.H, dt, w32, st);
+          if (rc) return rc;
+          rp.w_hh[k] = w32;
+        }
+      }
       rp.gates[k] = gates;
       rp.extra[k] = save && !is_elman(d.mode) ? R + rl.extra[l][k] : nullptr;
       if (d.P > 0) {
@@ -731,7 +881,10 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       }
     }
     float* ylay = nullptr;
-    if (l == d.L - 1) {
+    if (l == d.L - 1 && dt) {  // fp32, kept for the backward; rounded into the caller's y below
+      rp.y = save ? R + rl.ytop : S + hs.ytop;
+      rp.y_st = (long long)d.B * d.DH; rp.y_sb = (long long)d.DH;
+    } else if (l == d.L - 1) {
       rp.y = y; rp.y_st = ys_t; rp.y_sb = ys_b;
       rp.y_pool = y_pool;
     } else {
@@ -748,13 +901,39 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     // comes first: launched after the GEMM, the recurrence waits only on a kernel whose CTAs have all started.
     rc = launch_rec_fwd(rec, rp, st);
     if (rc) return rc;
-    if (drop && l + 1 < d.L) {  // K7; keeps the raw output when it is needed by backward, else in place
+    if (dt) {
+      // 16-bit: the output is rounded once; an inner layer's output is rounded before the dropout and again after it,
+      // as stock torch materialises it, and becomes the next layer's 16-bit A operand (its fp32 widening is kept for
+      // the backward's dW_ih)
+      const RowMap dense = simple_rows((long long)d.DH);
+      const int TB = (int)d.TB, DH = (int)d.DH;
+      if (l + 1 < d.L) {
+        float* xin = save ? R + rl.xin[l] : S + hs.xin;
+        void* next = S + hs.a16;
+        if (drop) {
+          rc = launch_narrow16(ylay, dense, TB, DH, dt, next, dense, false, xin, st);
+          if (!rc) rc = launch_dropout(xin, xin, d.TB * d.DH, d.p, hdr, (uint32_t)l, st);
+          if (!rc) rc = launch_narrow16(xin, dense, TB, DH, dt, next, dense, false, xin, st);
+        } else {
+          rc = launch_narrow16(ylay, dense, TB, DH, dt, next, dense, false, save ? xin : nullptr, st);
+        }
+      } else {
+        rc = launch_narrow16(rp.y, dense, TB, DH, dt, y16, tb_rows(ys_t, ys_b, d.B), false, nullptr, st);
+      }
+      if (rc) return rc;
+    } else if (drop && l + 1 < d.L) {  // K7; keeps the raw output when it is needed by backward, else in place
       float* dropped = save ? R + rl.ydrop[l] : ylay;
       // the next layer's GEMM reads `dropped` in place; the same launch zeroes its ready counters
       rc = launch_dropout(ylay, dropped, d.TB * d.DH, d.p, hdr, (uint32_t)l, st, ready, tiles_m);
       ready_zeroed = true;
       if (rc) return rc;
     }
+  }
+  if (dt) {
+    const int nst = d.L * d.D * d.B;
+    rc = launch_narrow16(h_n, simple_rows(d.H), nst, d.H, dt, hn16, simple_rows(d.H), false, nullptr, st);
+    if (!rc && cn16) rc = launch_narrow16(c_n, simple_rows(d.H), nst, d.H, dt, cn16, simple_rows(d.H), false, nullptr, st);
+    if (rc) return rc;
   }
   return B200RNN_OK;
 }
@@ -801,8 +980,9 @@ B200RNN_API int b200rnn_forward_hx(const b200rnn_desc* desc, const float* x, int
   if (rc) return rc;
   if (d.B > 0 && d.T == 0 && h_n && h_0) {  // no step: the final state is the initial one
     cudaStream_t st = static_cast<cudaStream_t>(stream_);
-    const size_t bytes = (size_t)d.L * d.D * d.B * d.H * sizeof(float);
-    B200_CUDA_CHECK(cudaMemcpyAsync(h_n, h_0, (size_t)d.L * d.D * d.B * d.HO * sizeof(float), cudaMemcpyDeviceToDevice,
+    const size_t es = d.dt ? 2 : sizeof(float);
+    const size_t bytes = (size_t)d.L * d.D * d.B * d.H * es;
+    B200_CUDA_CHECK(cudaMemcpyAsync(h_n, h_0, (size_t)d.L * d.D * d.B * d.HO * es, cudaMemcpyDeviceToDevice,
                                     st));
     if (c_n) {
       if (c_0) B200_CUDA_CHECK(cudaMemcpyAsync(c_n, c_0, bytes, cudaMemcpyDeviceToDevice, st));
@@ -895,7 +1075,8 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
                          const float* dc_n, const void* reserve, void* scratch, float* dx, int64_t dxs_t,
                          int64_t dxs_b, float* const* dparams, const int32_t* lengths, const float* ln_gamma,
                          float ln_eps, float* dln_gamma, float* dln_beta, const float* h_0, const float* c_0,
-                         float* dh_0, float* dc_0, void* stream_) {
+                         float* dh_0, float* dc_0, void* stream_, const float* const* layer_in = nullptr,
+                         int w16 = 0, const void* const* whh16 = nullptr) {
   Dims d;
   int rc = check_desc(desc, &d);
   if (rc) return rc;
@@ -983,7 +1164,9 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     }
     bp.lengths = lengths;
     bp.order = order;
-    rc = launch_rec_bwd(bp, st);
+    // 16-bit: whh16 holds each (layer, direction)'s weight_hh as the caller passed it, staged in 16 bits by the
+    // runtime-sized BPTT
+    rc = launch_rec_bwd(bp, st, w16, whh16 ? whh16 + (size_t)l * d.D : nullptr);
     if (rc) return rc;
 
     // The gradient GEMMs of this layer: each runs on the tensor cores when it is eligible, on the FFMA GEMM otherwise.
@@ -1004,7 +1187,7 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
       X.p = x;
       X.rows = tb_rows(xs_t, xs_b, d.B);
     } else {
-      X.p = R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
+      X.p = layer_in ? layer_in[l - 1] : R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
     }
     // dX_l goes to the caller's dx (layer 0) or to the dy of the layer below (scratch). With the fused LayerNorm the
     // layer-0 dgrad is d/dLN(x): it goes to scratch and through the LN backward below
@@ -1092,6 +1275,100 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
   return B200RNN_OK;
 }
 
+// The backward of a 16-bit call: exact fp32 copies of every operand into the scratch behind the fp32 layout, the fp32
+// backward on them (with the forward's fp32 top-layer output and rounded layer inputs from the reserve), then every
+// gradient rounded once into the caller's 16-bit tensors (added to them with B200RNN_FLAG_ACCUMULATE_GRADS).
+static int backward_h16(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b, const float* const* params,
+                        const float* dy, int64_t dys_t, int64_t dys_b, const float* dh_n, const float* dc_n,
+                        const float* h_0, const float* c_0, float* dh_0, float* dc_0, const void* reserve,
+                        void* scratch, float* dx, int64_t dxs_t, int64_t dxs_b, float* const* dparams,
+                        const int32_t* lengths, void* stream_) {
+  Dims d;
+  int rc = check_desc(desc, &d);
+  if (rc) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  if (d.B == 0 || d.T == 0) return B200RNN_OK;
+  if (!x || !params || !dy || !reserve || !scratch || !dparams) {
+    set_error("backward: null pointer argument");
+    return B200RNN_ERR_INVALID;
+  }
+  if (!aligned_to(reserve, 256) || !aligned_to(scratch, 256)) {
+    set_error("backward: reserve/scratch must be 256-byte aligned");
+    return B200RNN_ERR_INVALID;
+  }
+  ReserveLayout rl;
+  rc = make_reserve(d, &rl);
+  if (rc) return rc;
+  ScratchLayout sl;
+  make_scratch(d, &sl);
+  H16Scratch hs;
+  make_h16_scratch(d, sl.b_total, &hs);
+  const float* R = static_cast<const float*>(reserve);
+  float* S = static_cast<float*>(scratch);
+  const int dt = d.dt, TB = (int)d.TB, DH = (int)d.DH, nst = d.L * d.D * d.B;
+  const RowMap hrows = simple_rows(d.H);
+  rc = launch_widen16(x, tb_rows(xs_t, xs_b, d.B), TB, d.I, dt, S + hs.x32, st);
+  if (!rc) rc = launch_widen16(dy, tb_rows(dys_t, dys_b, d.B), TB, DH, dt, S + hs.dy32, st);
+  const float* src[4] = {dh_n, dc_n, h_0, c_0};
+  const size_t at[4] = {hs.dhn, hs.dcn, hs.bh0, hs.bc0};
+  const float* w[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (int i = 0; i < 4 && !rc; ++i)
+    if (src[i]) {
+      rc = launch_widen16(src[i], hrows, nst, d.H, dt, S + at[i], st);
+      w[i] = S + at[i];
+    }
+  if (rc) return rc;
+  const float* p32[8 * 2 * 4];
+  float* dp32[8 * 2 * 4];
+  for (int l = 0; l < d.L; ++l)
+    for (int k = 0; k < d.D; ++k) {
+      const int Il = l == 0 ? d.I : DH;
+      const size_t n[4] = {d.GH * (size_t)Il, d.GH * (size_t)d.H, d.GH, d.GH};
+      size_t off = 0;
+      for (int i = 0; i < 4; ++i) {
+        const size_t j = (size_t)(l * d.D + k) * 4 + i;
+        if (!params[j]) {
+          set_error("backward: null parameter pointer (layer %d dir %d)", l, k);
+          return B200RNN_ERR_INVALID;
+        }
+        float* p = S + hs.w32[l][k] + off;
+        rc = launch_widen16(params[j], simple_rows((long long)n[i]), 1, (int)n[i], dt, p, st);
+        if (rc) return rc;
+        p32[j] = p;
+        dp32[j] = dparams[j] ? S + hs.dw32[l][k] + off : nullptr;
+        off += n[i];
+      }
+    }
+  const float* layer_in[8];
+  for (int l = 0; l + 1 < d.L; ++l) layer_in[l] = R + rl.xin[l];
+  const void* whh16[8 * 2];
+  for (int i = 0; i < d.L * d.D; ++i) whh16[i] = params[(size_t)i * 4 + 1];
+  b200rnn_desc d32 = *desc;
+  d32.flags &= ~(B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_ACCUMULATE_GRADS);
+  rc = backward_impl(&d32, S + hs.x32, (int64_t)d.B * d.I, d.I, p32, R + rl.ytop, (int64_t)d.B * DH, DH, S + hs.dy32,
+                     (int64_t)d.B * DH, DH, nullptr, 0.f, w[0], w[1], reserve, scratch, dx ? S + hs.dx32 : nullptr,
+                     (int64_t)d.B * d.I, d.I, dp32, lengths, nullptr, 0.f, nullptr, nullptr, w[2], w[3],
+                     dh_0 ? S + hs.dh0 : nullptr, dc_0 ? S + hs.dc0 : nullptr, stream_, layer_in, dt, whh16);
+  if (rc) return rc;
+  const bool acc = (desc->flags & B200RNN_FLAG_ACCUMULATE_GRADS) != 0;
+  if (dx) rc = launch_narrow16(S + hs.dx32, simple_rows(d.I), TB, d.I, dt, dx, tb_rows(dxs_t, dxs_b, d.B), false,
+                               nullptr, st);
+  if (!rc && dh_0) rc = launch_narrow16(S + hs.dh0, hrows, nst, d.H, dt, dh_0, hrows, false, nullptr, st);
+  if (!rc && dc_0) rc = launch_narrow16(S + hs.dc0, hrows, nst, d.H, dt, dc_0, hrows, false, nullptr, st);
+  for (int l = 0; l < d.L && !rc; ++l)
+    for (int k = 0; k < d.D && !rc; ++k) {
+      const int Il = l == 0 ? d.I : DH;
+      const size_t n[4] = {d.GH * (size_t)Il, d.GH * (size_t)d.H, d.GH, d.GH};
+      for (int i = 0; i < 4 && !rc; ++i) {
+        const size_t j = (size_t)(l * d.D + k) * 4 + i;
+        if (dparams[j])
+          rc = launch_narrow16(dp32[j], simple_rows((long long)n[i]), 1, (int)n[i], dt, dparams[j],
+                               simple_rows((long long)n[i]), acc, nullptr, st);
+      }
+    }
+  return rc;
+}
+
 B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
                                        const float* const* params, const float* y, int64_t ys_t, int64_t ys_b,
                                        const float* dy, int64_t dys_t, int64_t dys_b, const float* dy_pool,
@@ -1126,7 +1403,8 @@ B200RNN_API int b200rnn_backward_hx(const b200rnn_desc* desc, const float* x, in
   }
   if (d.B > 0 && d.T == 0) {  // no step: the gradients pass from the final state to the initial one
     cudaStream_t st = static_cast<cudaStream_t>(stream_);
-    const size_t bytes[2] = {(size_t)d.L * d.D * d.B * d.HO * sizeof(float), (size_t)d.L * d.D * d.B * d.H * sizeof(float)};
+    const size_t es = d.dt ? 2 : sizeof(float);
+    const size_t bytes[2] = {(size_t)d.L * d.D * d.B * d.HO * es, (size_t)d.L * d.D * d.B * d.H * es};
     const float* src[2] = {dh_n, dc_n};
     float* dst[2] = {dh_0, dc_0};
     for (int i = 0; i < 2; ++i) {
@@ -1136,6 +1414,9 @@ B200RNN_API int b200rnn_backward_hx(const b200rnn_desc* desc, const float* x, in
     }
     return B200RNN_OK;
   }
+  if (d.dt)
+    return backward_h16(desc, x, xs_t, xs_b, params, dy, dys_t, dys_b, dh_n, dc_n, h_0, c_0, dh_0, dc_0, reserve,
+                        scratch, dx, dxs_t, dxs_b, dparams, lengths, stream_);
   return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, nullptr, 0.f, dh_n, dc_n, reserve,
                        scratch, dx, dxs_t, dxs_b, dparams, lengths, nullptr, 0.f, nullptr, nullptr, h_0, c_0, dh_0, dc_0,
                        stream_);
@@ -1150,6 +1431,9 @@ B200RNN_API int b200rnn_backward(const b200rnn_desc* desc, const float* x, int64
     set_error("backward: null pointer argument");
     return B200RNN_ERR_INVALID;
   }
+  if (desc && (desc->flags & (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16)))
+    return backward_h16(desc, x, xs_t, xs_b, params, dy, dys_t, dys_b, dh_n, dc_n, nullptr, nullptr, nullptr, nullptr,
+                        reserve, scratch, dx, dxs_t, dxs_b, dparams, lengths, stream_);
   return backward_impl(desc, x, xs_t, xs_b, params, y, ys_t, ys_b, dy, dys_t, dys_b, nullptr, 0.f, dh_n, dc_n, reserve,
                        scratch, dx, dxs_t, dxs_b, dparams, lengths, nullptr, 0.f, nullptr, nullptr, nullptr, nullptr,
                        nullptr, nullptr, stream_);
@@ -1533,6 +1817,12 @@ B200RNN_API int b200rnn_debug_layernorm(const float* x, int64_t s_outer, int64_t
 /* test only (not declared in the public header): the inter-layer dropout as a layer runs it, out[i] = in[i] *
    keep(i) / (1 - p) over n elements of Philox stream stream_id at {seed, offset}; hdr: 2 uint64 of device memory for
    the resolved RNG header. Any n and any float alignment (the float4 path and the scalar tail). */
+/* debug only (not declared in the public header): bytes of dynamic shared memory of one runtime-sized recurrence
+ * launch shape (anyh_smem), so that tests derive the on-chip tier bounds from the function the planner uses */
+B200RNN_API size_t b200rnn_debug_anyh_smem(int G, int H, int C, int BS, int bwd, int onchip, int wbytes) {
+  return anyh_smem(G, H, C, BS, bwd != 0, onchip != 0, wbytes);
+}
+
 B200RNN_API int b200rnn_debug_dropout(const float* in, float* out, size_t n, float p, uint64_t seed, uint64_t offset,
                                       uint32_t stream_id, uint64_t* hdr, void* stream_) {
   if (!in || !out || !hdr) {

@@ -42,6 +42,7 @@
 
 #include "gemm_f32.cuh"
 #include "gemm_h16_layout.cuh"
+#include "h16.cuh"
 #include "profile.cuh"
 #include "ptx.cuh"
 #include "rec_h16_layout.cuh"
@@ -81,6 +82,13 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(ptx::smem_u32(bar)), "r"(bytes)
                : "memory");
+}
+
+// mbarrier phase wait that gives up after ~2^24 polls (seconds): in the native 16-bit kernel a TMA transaction that never
+// completes (a map that disagrees with the expected bytes) becomes a trap, not a hang
+__device__ __forceinline__ void bounded_wait(uint64_t* bar, uint32_t parity) {
+  for (uint32_t n = 0; !ptx::mbar_try_wait(bar, parity); ++n)
+    if (n > (1u << 24)) __trap();
 }
 
 // shared-memory matrix descriptor (sm_90): K-major tile, 128-byte swizzle, rows of 128 B, 8-row groups 1024 B apart
@@ -144,6 +152,27 @@ __device__ __forceinline__ void wgmma_f16_m64n128k16_ra(float (&d)[64], const ui
         B200_ACC8(56)
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
+// the same in f16 (BF = false) or bf16 (BF = true) with both the A fragment (layout of wgmma_f16_m64n128k16_ra) and
+// B from 16-bit data as it lies: the native 16-bit input projection (gemm_n16_kernel)
+template <bool BF>
+__device__ __forceinline__ void wgmma_n16_m64n128k16_ra(float (&d)[64], const uint32_t* a, uint64_t bdesc,
+                                                        int accumulate) {
+  if constexpr (BF)
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : B200_ACC8(0), B200_ACC8(8), B200_ACC8(16), B200_ACC8(24), B200_ACC8(32), B200_ACC8(40), B200_ACC8(48),
+          B200_ACC8(56)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+  else
+    wgmma_f16_m64n128k16_ra(d, a, bdesc, accumulate);
+}
 #undef B200_ACC8
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -175,10 +204,12 @@ struct TcArgs {
   int tf32;         // single-pass TF32: the lo operands are absent (host side only: selects the kernel instantiation)
   const int* w_exp; // fp16 pairs: e_n of every W row (gemm_h16_layout.cuh), the epilogue scales column n by 2^-e_n
   int f16;          // fp16 pairs (gemm_f16x3_kernel; host side only)
+  int n16;          // native 16-bit operands: TC_F16 or TC_BF16 (gemm_n16_kernel; host side only), else 0
 };
 
-// the arithmetic of one instantiation: 3xTF32, single-pass TF32, or fp16 (hi, lo) pairs (fp32 A only)
-enum TcMath { TC_3XTF32, TC_TF32, TC_F16X3 };
+// the arithmetic of one instantiation: 3xTF32, single-pass TF32, fp16 (hi, lo) pairs (fp32 A only), or native f16 /
+// bf16 operands (16-bit A and W, one MMA per k-step)
+enum TcMath { TC_3XTF32, TC_TF32, TC_F16X3, TC_F16, TC_BF16 };
 
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64K registers of the SM
 
@@ -226,12 +257,18 @@ __device__ __forceinline__ void load_mn_tile(unsigned char* tile, const float* _
 // row's max |a| over the k-block), splits them into fp16 hi / lo in registers and runs lo*hi, hi*lo, hi*hi as
 // wgmma.m64n128k16 (12 per k-block); the drain unscales with total = fma(acc, 2^-e_m, total), the epilogue multiplies
 // column n by 2^-e_n before the biases.
+// Native 16-bit (MATH = TC_F16 / TC_BF16, gemm_n16_kernel; args.a_f32 = 1 for the single TMA issuer): a k-block is 64 k,
+// A (128 rows x 128 bytes, 3-D map read in place) in slot 0 and W in slot 2, both K-major under the 128-byte swizzle;
+// each consumer loads its A fragment of the k-block as it lies (the fp32-A kernel's addressing, 16 registers) and runs
+// 4 wgmma.m64n128k16 with W from shared memory, then the round-to-nearest drain of the 3xTF32 kernel. No split, no
+// scale: the products are exact in fp32.
 template <bool MN, int MATH>
 __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const CUtensorMap& map_a_lo,
                                              const CUtensorMap& map_b_hi, const CUtensorMap& map_b_lo,
                                              const TcArgs args) {
   constexpr bool TF32 = MATH == TC_TF32, F16 = MATH == TC_F16X3;
-  constexpr int KB = F16 ? g16::BK : BK;  // k per ring stage
+  constexpr bool NAT = MATH == TC_F16 || MATH == TC_BF16;
+  constexpr int KB = (F16 || NAT) ? g16::BK : BK;  // k per ring stage
   extern __shared__ unsigned char smem_raw[];
   // aligned by offset so that the compiler keeps the shared state space (LDS/STS instead of generic LD/ST)
   unsigned char* base = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -258,7 +295,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
     }
     if (!args.b_mn) {
       prefetch_tmap(&map_b_hi);
-      if (!TF32) prefetch_tmap(&map_b_lo);
+      if (!TF32 && !NAT) prefetch_tmap(&map_b_lo);
     }
   }
   __syncthreads();
@@ -274,17 +311,20 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
           tile_origin(args, item % ntiles, m0, n0);
           for (int kb = 0; kb < nkb_total; ++kb, ++it) {
             const int s = it % STAGES;
-            ptx::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+            if constexpr (NAT)
+              bounded_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+            else
+              ptx::mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
             unsigned char* st = base + s * STAGE_BYTES;
             if (ptx::elect_one_sync()) {  // 3xTF32 / TF32: the A_lo slot stays unused (A is split in registers);
                                           // fp16 pairs: it holds the second 32 k of A
-              ptx::mbar_arrive_expect_tx(&full[s], (F16 ? 4u : TF32 ? 2u : 3u) * TILE_BYTES);
+              ptx::mbar_arrive_expect_tx(&full[s], (NAT ? 2u : F16 ? 4u : TF32 ? 2u : 3u) * TILE_BYTES);
               tma_load_3d(st + 0 * TILE_BYTES, &map_a_hi, kb * KB, m0 % args.a_inner, m0 / args.a_inner, &full[s]);
               if (F16)
                 tma_load_3d(st + 1 * TILE_BYTES, &map_a_hi, kb * KB + BK, m0 % args.a_inner, m0 / args.a_inner,
                             &full[s]);
               tma_load_2d(st + 2 * TILE_BYTES, &map_b_hi, kb * KB, n0, &full[s]);
-              if (!TF32) tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * KB, n0, &full[s]);
+              if (!TF32 && !NAT) tma_load_2d(st + 3 * TILE_BYTES, &map_b_lo, kb * KB, n0, &full[s]);
             }
             __syncwarp();
           }
@@ -472,6 +512,26 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
       }
       wgmma_commit();
     };
+    // native 16-bit: the 4 MMAs of a k-block of 64. Register 4 s + i of the A fragment holds the pair at row g + 8 (i & 1),
+    // k = 16 s + 8 (i >> 1) + 2 tq: 16-byte chunk 2 s + (i >> 1) of the row, swizzled by g, 4 tq bytes in (a_row)
+    auto issue_n16 = [&](float (&acc)[64], int pos) {
+      bounded_wait(&full[pos % STAGES], (pos / STAGES) & 1);
+      const unsigned char* at = base + (pos % STAGES) * STAGE_BYTES + a_row;
+      uint32_t fa[16];
+#pragma unroll
+      for (int s4 = 0; s4 < 4; ++s4)
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          fa[4 * s4 + i] = *reinterpret_cast<const uint32_t*>(at + (i & 1) * 1024 + (((2 * s4 + (i >> 1)) ^ g) << 4));
+      const uint64_t b = make_kmajor_sw128_desc(ptx::smem_u32(base + (pos % STAGES) * STAGE_BYTES) + 2 * TILE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < g16::BK / 16; ++k) {
+        const uint64_t adv = (uint64_t)(k * (32 >> 4));  // K step of 16 halves = 32 bytes inside the swizzle atom
+        wgmma_n16_m64n128k16_ra<MATH == TC_BF16>(acc, &fa[4 * k], b + adv, k != 0);
+      }
+      wgmma_commit();
+    };
     // fp16 pairs: as drain, the k-block's sum unscaled by its rows' 2^-e_m in the same rounding
     auto drain16 = [&](float (&total)[64], float (&acc)[64], const float (&sc)[2], int pos) {
       reg_fence(acc);
@@ -490,7 +550,13 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& map_a_hi, const 
 #pragma unroll
       for (int i = 0; i < 64; ++i) total[i] = 0.f;
       float acc[64];
-      if (F16 || (!MN && args.a_f32)) {
+      if constexpr (NAT) {
+        for (int kb = 0; kb < nkb; ++kb) {
+          issue_n16(acc, it + kb);
+          wgmma_wait0();
+          drain(total, acc, it + kb);
+        }
+      } else if (F16 || (!MN && args.a_f32)) {
         // A from registers: the k-block's fp32 fragment is loaded and split here; the next k-block's is loaded while
         // the current MMAs run. Fragments alternate between fa0 and fa1; the loop body is unconditional and the tail
         // peeled, so no branch merges registers a wgmma in flight reads.
@@ -621,6 +687,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
                       const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
                       const TcArgs args) {
   gemm_tc_body<false, TC_F16X3>(map_a, map_unused, map_w_hi, map_w_lo, args);
+}
+
+// 16-bit A read in place and 16-bit W, both straight into wgmma (MATH = TC_F16 or TC_BF16)
+template <int MATH>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+    gemm_n16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_unused,
+                    const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_unused2,
+                    const TcArgs args) {
+  gemm_tc_body<false, MATH>(map_a, map_unused, map_w, map_unused2, args);
 }
 
 // W [N][K] (rows through `rows`) -> fp16 pairs (gemm_h16_layout.cuh): row n scaled by 2^e_n, e_n = h16::scale_exp of
@@ -901,6 +976,29 @@ bool make_map16(CUtensorMap* map, const void* ptr, int rows, int K) {
   return r == CUDA_SUCCESS;
 }
 
+// 16-bit A operand read in place through its row map: make_a_f32_map's 3-D map with 2-byte elements and boxes of 64 k
+// (128 bytes). TMA only moves the elements, so fp16 and bf16 share the FLOAT16 map type (the zero fill is +0 in both).
+bool make_a16_map(CUtensorMap* map, const void* ptr, const RowMap& rows, int M, int K, int* inner) {
+  EncodeTiledFn enc = get_encoder();
+  if (!enc || (reinterpret_cast<uintptr_t>(ptr) & 15u) || K % 8 != 0) return false;
+  const bool dense = rows.inner_n >= M;
+  const long long ni = dense ? M : rows.inner_n;
+  const long long no = dense ? 1 : (M + ni - 1) / ni;
+  const long long si = rows.s_inner, so = dense ? (long long)M * rows.s_inner : rows.s_outer;
+  if (!dense && (M % ni != 0 || !(ni % BM == 0 || BM % ni == 0))) return false;
+  if (si < K || si % 8 != 0 || so < 1 || so % 8 != 0) return false;
+  const cuuint32_t bi = (cuuint32_t)(dense || ni >= BM ? BM : ni);
+  cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)ni, (cuuint64_t)no};
+  cuuint64_t strides[2] = {(cuuint64_t)si * 2, (cuuint64_t)so * 2};
+  cuuint32_t box[3] = {(cuuint32_t)g16::BK, bi, (cuuint32_t)BM / bi};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  *inner = (int)ni;
+  return r == CUDA_SUCCESS;
+}
+
 // fp32 A operand read in place through its row map: 3-D map {K, inner rows, outer rows} with box {32, bi, 128 / bi},
 // so a 128-row tile is one box. Dense rows (inner_n >= M): {K, M, 1}. Rows r = t * B + b of a [T][B] view (tb_rows):
 // {K, B, T}, which tiles when B divides 128 or is a multiple of it. Strides must be multiples of 16 bytes.
@@ -1100,13 +1198,17 @@ int launch_tc(const CUtensorMap (&m)[4], const TcArgs& a, int stream_clusters, c
       B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_f16x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_n16_kernel<TC_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+      B200_CUDA_CHECK(cudaFuncSetAttribute(gemm_n16_kernel<TC_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
       attr_done[dev] = true;
     }
   }
   const int sms = num_sms();
   const int nitems = a.tiles_m * a.tiles_n * a.splitk;
   const bool mn = a.a_mn || a.b_mn;
-  auto kernel = a.f16    ? gemm_f16x3_kernel
+  auto kernel = a.n16 == TC_BF16 ? gemm_n16_kernel<TC_BF16>
+                : a.n16        ? gemm_n16_kernel<TC_F16>
+                : a.f16        ? gemm_f16x3_kernel
                 : a.tf32 ? (mn ? gemm_tf32x3_kernel<true, true> : gemm_tf32x3_kernel<false, true>)
                          : (mn ? gemm_tf32x3_kernel<true, false> : gemm_tf32x3_kernel<false, false>);
   dim3 grid(nitems < sms ? nitems : sms, 1, 1);
@@ -1322,6 +1424,36 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
   TcOperand A{a_hi, a_lo, p.a_kcontig ? p.K : p.M, !p.a_kcontig};
   return tc_gemm_presplit(A, B, p.M, p.N, p.K, p.C, p.c_rows, p.bias1, p.bias2, p.bias2_n, 0, nullptr, 0, stream,
                           p.tc_ready, p.tc_stream_clusters, tf32);
+}
+
+bool tc_gemm_n16_ok(const void* A, const RowMap& a_rows, const void* W, int M, int N, int K) {
+  CUtensorMap m;
+  int inner = 0;
+  return M >= 1 && N % BN == 0 && N > 0 && K % 8 == 0 && K > 0 && (reinterpret_cast<uintptr_t>(W) & 15u) == 0 &&
+         make_a16_map(&m, A, a_rows, M, K, &inner);
+}
+
+int tc_gemm_n16(const void* A, const RowMap& a_rows, const void* W, int M, int N, int K, int dt, float* C,
+                const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream) {
+  int rc = check_tc_shape(M, N, K, C, c_rows, nullptr, false, 0);
+  if (rc) return rc;
+  CUtensorMap m[4] = {};
+  int inner = 0;
+  if (!make_a16_map(&m[0], A, a_rows, M, K, &inner) || !make_map16(&m[2], W, N, K)) {
+    set_error("tc_gemm: the 16-bit operands cannot be read by TMA (16-byte aligned rows, K %% 8 == 0, batch dividing "
+              "128 or a multiple of it)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
+  if (debug)
+    fprintf(stderr, "[b200rnn] forward x-projection: M=%d N=%d K=%d math=%s weights=native\n", M, N, K,
+            dt == DT_BF16 ? "bf16" : "f16");
+  TcArgs a = tc_args(M, N, K, C, c_rows, bias1, bias2, bias2_n, 0, nullptr);
+  a.a_f32 = 1;  // one thread issues the A and W boxes
+  a.a_inner = inner;
+  a.kb_per_split = (K + g16::BK - 1) / g16::BK;
+  a.n16 = dt == DT_BF16 ? TC_BF16 : TC_F16;
+  return launch_tc(m, a, 0, stream);
 }
 
 }  // namespace b200rnn

@@ -23,9 +23,12 @@
 //   * Elman: the forward saves the activated h_t as its one gate block and nothing in `extra`; the backward takes
 //     dpre = dh (1 - h^2) for tanh, dh [h > 0] for relu from that saved h_t (elman_cell_bwd).
 //   * The waits are bounded: a protocol bug traps (a CUDA error) instead of hanging the GPU.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdlib.h>
 
+#include "h16.cuh"
 #include "ptx.cuh"
 #include "rnn_cell.cuh"
 #include "rnn_kernels.cuh"
@@ -123,7 +126,19 @@ __device__ __forceinline__ void send_slice(float* vec, int width, int NB, int H,
 
 // acc[g] += sum_k w[g * wg + k] * v[g * vg + k], k ascending (one FMA chain per gate: deterministic); vg = 0 in the
 // forward (one state row), H in the backward (gate block g of the gradient row). w from shared memory or, in the L2
-// tier, from global memory (read-only for the whole launch)
+// tier, from global memory (read-only for the whole launch). WT: the storage of w, float or 16-bit (__half /
+// __nv_bfloat16, widened exactly in registers: the same chains)
+template <typename WT>
+__device__ __forceinline__ float4 widen4(uint2 u) {
+  if constexpr (__is_same(WT, __nv_bfloat16)) {
+    return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                       __uint_as_float(u.y & 0xffff0000u));
+  } else {
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+  }
+}
 template <int G, bool ONCHIP, bool PER_GATE_V>
 __device__ __forceinline__ void dot_rows(const float* __restrict__ w, size_t wg, const float* __restrict__ v, int vg,
                                          int K, float (&acc)[G]) {
@@ -146,7 +161,28 @@ __device__ __forceinline__ void dot_rows(const float* __restrict__ w, size_t wg,
     }
   }
 }
-
+// The same chains over 16-bit weights, widened exactly in registers (8-byte loads of 4 weights)
+template <int G, bool ONCHIP, bool PER_GATE_V, typename WT>
+__device__ __forceinline__ void dot_rows16(const WT* __restrict__ w, size_t wg, const float* __restrict__ v, int vg,
+                                           int K, float (&acc)[G]) {
+  constexpr int UNROLL = PER_GATE_V ? 1 : (G == 4 && !ONCHIP) ? 2 : 4;
+#pragma unroll UNROLL
+  for (int k = 0; k < K; k += 4) {
+    float4 x = *reinterpret_cast<const float4*>(v + k);
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      if (PER_GATE_V && g > 0) x = *reinterpret_cast<const float4*>(v + g * vg + k);
+      const float4 a = widen4<WT>(ONCHIP ? *reinterpret_cast<const uint2*>(w + g * wg + k)
+                                         : __ldg(reinterpret_cast<const uint2*>(w + g * wg + k)));
+      float r = acc[g];
+      r = fmaf(a.x, x.x, r);
+      r = fmaf(a.y, x.y, r);
+      r = fmaf(a.z, x.z, r);
+      r = fmaf(a.w, x.w, r);
+      acc[g] = r;
+    }
+  }
+}
 // Stage rows r = 0 .. rows-1 of length H (row r at src + rowoff(r)) into W_s[r][H + 4]
 template <typename RowOff>
 __device__ __forceinline__ void stage_rows(float* W_s, const float* __restrict__ src, int rows, int H, int NT,
@@ -155,6 +191,16 @@ __device__ __forceinline__ void stage_rows(float* W_s, const float* __restrict__
   for (int i = threadIdx.x; i < rows * q4; i += NT) {
     const int r = i / q4, k = (i - r * q4) * 4;
     *reinterpret_cast<float4*>(&W_s[(size_t)r * LD + k]) = __ldg(reinterpret_cast<const float4*>(src + rowoff(r) + k));
+  }
+}
+
+// The same with 16-bit rows: W_s[r][H + 8], 16-byte chunks of 8 elements (the pad keeps 16 bytes, as above)
+template <typename WT, typename RowOff>
+__device__ __forceinline__ void stage_rows16(WT* W_s, const WT* __restrict__ src, int rows, int H, int NT, RowOff rowoff) {
+  const int q8 = H / 8, LD = H + 8;
+  for (int i = threadIdx.x; i < rows * q8; i += NT) {
+    const int r = i / q8, k = (i - r * q8) * 8;
+    *reinterpret_cast<uint4*>(&W_s[(size_t)r * LD + k]) = __ldg(reinterpret_cast<const uint4*>(src + rowoff(r) + k));
   }
 }
 
@@ -263,6 +309,120 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
       for (int t = T; t < p.T; ++t) p.y[(long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = 0.f;
   }
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
+}
+
+// The forward over a 16-bit weight_hh (WT = __half / __nv_bfloat16), anyh16_fwd_kernel: anyh_fwd_kernel's step with
+// rows of H + 8 elements on chip and the weights widened in registers (dot_rows16). anyh_fwd_kernel keeps its own
+// text so that the fp32 instantiations compile exactly as before.
+// Shared memory: [W_s: G*n x (H+8) WT, ONCHIP only] [h: 2 x BS x H] [bars: 2 x C]
+template <int MODE, bool VL, bool ONCHIP, typename WT>
+__device__ __forceinline__ void anyh_fwd_body(const RecFwdParams p, const int nslices) {
+  constexpr int G = gates_of(MODE);
+  const int H = p.H, B = p.B, LD = H + 8;
+  const bool relu = p.mode == B200RNN_RNN_RELU;  // Elman
+  const AnyhSlice s = anyh_slice<VL>(p, nslices);
+  const int C = s.C, HS = s.HS, BS = s.BS, NT = s.NT, dir = s.dir, b0 = s.b0, j0 = s.j0, n = s.n, T = s.T;
+  const uint32_t rank = s.rank;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  WT* W_s = reinterpret_cast<WT*>(smem_raw);  // [G][n][LD]
+  float* h_s = reinterpret_cast<float*>(W_s + (ONCHIP ? (size_t)G * HS * LD : 0));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(h_s + (size_t)2 * BS * H);
+  const int tid = threadIdx.x;
+  const WT* w_hh = reinterpret_cast<const WT*>(p.w_hh[dir]);
+
+  if (tid == 0) init_bars(bars, C);
+  if constexpr (ONCHIP) {
+    if constexpr (G == 1)
+      stage_rows16(W_s, w_hh, n, H, NT, [&](int r) { return (size_t)(j0 + r) * H; });
+    else
+      stage_rows16(W_s, w_hh, G * n, H, NT, [&](int r) { return ((size_t)(r / n) * H + j0 + r % n) * H; });
+  }
+  for (int i = tid; i < BS * H; i += NT) {  // buffer 0: h_0 of the cluster's slots (zeros past the batch / without h_0)
+    const int q = i / H, k = i - q * H;
+    const int slot = b0 + q;
+    float v = 0.f;
+    if (p.h_0 && slot < B) v = p.h_0[((size_t)dir * B + (VL ? p.order[slot] : slot)) * H + k];
+    h_s[i] = v;
+  }
+  __syncthreads();
+  ptx::cluster_sync_all();  // peers' barriers are initialised before anyone sends
+
+  const int u = s.u, b = s.b, j = j0 + u, slot = b0 + b;
+  const bool valid = s.active && slot < B;
+  const int row = valid ? (VL ? p.order[slot] : slot) : 0;
+  const int len = (VL && valid) ? p.lengths[row] : p.T;
+  float* gates = p.gates[dir];
+  float h = (p.h_0 && valid) ? p.h_0[((size_t)dir * B + row) * H + j] : 0.f;
+  float c = (MODE == B200RNN_LSTM && p.c_0 && valid) ? p.c_0[((size_t)dir * B + row) * H + j] : 0.f;
+  const float bhn = MODE == B200RNN_GRU ? p.b_hh[dir][2 * H + j] : 0.f;
+  float gi[G];
+  // Elman: 0 until the first load, the register allocation its timings (tools/elman_steps_results.json) were taken with
+  if constexpr (G == 1) gi[0] = 0.f;
+  auto load_gi = [&](int t) {
+#pragma unroll
+    for (int g = 0; g < G; ++g) gi[g] = valid ? gates[((size_t)t * B + row) * (G * H) + g * H + j] : 0.f;
+  };
+  if (T > 0) load_gi(dir ? T - 1 : 0);
+  const WT* wrow = ONCHIP ? W_s + (size_t)u * LD : w_hh + (size_t)(j0 + u) * H;
+  const size_t wg = ONCHIP ? (size_t)n * LD : (size_t)H * H;
+
+  for (int step = 0; step < T; ++step) {
+    const int t = dir ? T - 1 - step : step;
+    const int cur = step & 1, nxt = cur ^ 1;
+    if (step > 0) wait_bars(bars, cur, C, rank, ((step - 1) >> 1) & 1);
+    if (tid == 0 && step + 1 < T) arm_bars(bars, nxt, s, H, 1);
+    float acc[G];
+#pragma unroll
+    for (int g = 0; g < G; ++g) acc[g] = 0.f;
+    dot_rows16<G, ONCHIP, false, WT>(wrow, wg, h_s + ((size_t)cur * BS + b) * H, 0, H, acc);
+
+    float hnew, sg[G], sx;
+    const bool frozen = VL && t >= len;  // past its length a row keeps its state and emits 0
+    if constexpr (MODE == B200RNN_GRU) {
+      const GruStep st = gru_cell_fwd(gi, acc, bhn, h);
+      hnew = frozen ? h : st.h;
+      sg[0] = st.r; sg[1] = st.z; sg[2] = st.n; sx = st.hn;
+    } else if constexpr (MODE == B200RNN_LSTM) {
+      const LstmStep st = lstm_cell_fwd(gi, acc, c);
+      hnew = frozen ? h : st.h;
+      c = frozen ? c : st.c;
+      sg[0] = st.i; sg[1] = st.f; sg[2] = st.g; sg[3] = st.o; sx = c;
+    } else {
+      sg[0] = elman_cell_fwd(gi[0], acc[0], relu);
+      hnew = frozen ? h : sg[0];
+    }
+    h = hnew;
+    if (valid) {
+      if (p.y) p.y[(long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = frozen ? 0.f : hnew;
+      if (p.training) {  // the activated gates over the x-projection, and GRU W_hn h + b_hn / LSTM c_t (Elman: h_t)
+        float* gp = gates + ((size_t)t * B + row) * (G * H) + j;
+#pragma unroll
+        for (int g = 0; g < G; ++g) gp[g * H] = sg[g];
+        if constexpr (G > 1) p.extra[dir][((size_t)t * B + row) * H + j] = sx;
+      }
+    }
+    if (step + 1 < T) {
+      float* h_nxt = h_s + (size_t)nxt * BS * H;
+      if (s.active) h_nxt[(size_t)b * H + j] = hnew;
+      __syncthreads();  // the own slice is complete (and every thread is past step - 1's reads of buffer nxt)
+      send_slice(h_nxt, H, 1, H, s, &bars[nxt * C + rank]);
+      load_gi(dir ? T - 2 - step : step + 1);
+    }
+  }
+  if (valid) {
+    p.h_n[((size_t)dir * B + row) * H + j] = h;
+    if (MODE == B200RNN_LSTM && p.c_n) p.c_n[((size_t)dir * B + row) * H + j] = c;
+    if (VL && p.y)  // the steps [T, p.T) the cluster skipped emit 0, as past any sequence's length
+      for (int t = T; t < p.T; ++t) p.y[(long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = 0.f;
+  }
+  ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
+}
+
+
+// 16-bit weight_hh (__half or __nv_bfloat16): half the shared memory per weight row, so more hidden sizes stay on chip
+template <int MODE, bool VL, bool ONCHIP, typename WT>
+__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_fwd_kernel(const RecFwdParams p, const int nslices) {
+  anyh_fwd_body<MODE, VL, ONCHIP, WT>(p, nslices);
 }
 
 // =================================================================================================
@@ -424,30 +584,213 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
   ptx::cluster_sync_all();
 }
 
+// The BPTT over the 16-bit transposed weight_hh (whh_prep16_kernel's output), anyh16_bwd_kernel: as anyh_bwd_kernel,
+// whose text is kept for the fp32 instantiations
+template <int MODE, bool VL, bool ONCHIP, typename WT>
+__device__ __forceinline__ void anyh_bwd_body(const RecBwdParams& p, const int nslices) {
+  constexpr int G = gates_of(MODE);
+  constexpr int NP = G == 1 ? 1 : G + 1;  // bias-partial blocks per slice: dGi (+ the GRU dghn block, 0 for the LSTM)
+  const int H = p.H, B = p.B, LD = H + 8, GH = G * H;
+  const bool relu = p.mode == B200RNN_RNN_RELU;  // Elman
+  const AnyhSlice s = anyh_slice<VL>(p, nslices);
+  const int C = s.C, HS = s.HS, BS = s.BS, NT = s.NT, dir = s.dir, b0 = s.b0, j0 = s.j0, n = s.n, T = s.T;
+  const uint32_t rank = s.rank;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  WT* W_s = reinterpret_cast<WT*>(smem_raw);  // [G][n][LD]
+  float* d_s = reinterpret_cast<float*>(W_s + (ONCHIP ? (size_t)G * HS * LD : 0));
+  float* red = d_s + (size_t)2 * BS * GH;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(red + (size_t)BS * NP * HS);
+  const int tid = threadIdx.x;
+  // rows (g, u) of this CTA: W_hh[g*H + :][j0 + u], contiguous from G * j0 * H (whh_prep_kernel)
+  const WT* w_prep = reinterpret_cast<const WT*>(p.w_prep[dir]) + (size_t)G * j0 * H;
+
+  if (tid == 0) init_bars(bars, C);
+  if constexpr (ONCHIP) stage_rows16(W_s, w_prep, G * n, H, NT, [&](int r) { return (size_t)r * H; });
+  __syncthreads();
+  ptx::cluster_sync_all();
+
+  const int u = s.u, b = s.b, j = j0 + u, slot = b0 + b;
+  const bool valid = s.active && slot < B;
+  const int row = valid ? (VL ? p.order[slot] : slot) : 0;
+  const int len = (VL && valid) ? p.lengths[row] : T;
+  const float* gates = p.gates[dir];
+  const float* extra = p.extra[dir];
+  float* dgates = p.dgates[dir];
+  const WT* wrow = ONCHIP ? W_s + (size_t)u * LD : w_prep + (size_t)u * H;
+  const size_t wg = ONCHIP ? (size_t)n * LD : (size_t)n * H;
+
+  float dh_carry = 0.f, dc_carry = 0.f, direct = 0.f;
+  if (valid) {
+    if (p.dh_n) dh_carry = p.dh_n[((size_t)dir * B + row) * H + j];
+    if (MODE == B200RNN_LSTM && p.dc_n) dc_carry = p.dc_n[((size_t)dir * B + row) * H + j];
+  }
+  float bsum[NP] = {};
+  // saved gates (Elman: h_t), hn / c_t, h_{prev} / c_{prev}, dy (prefetched)
+  float sv[G] = {}, sx = 0.f, hp = 0.f, dyv = 0.f;
+  const float* s0 = MODE == B200RNN_GRU ? p.h_0 : p.c_0;  // the state before the first step (zeros when NULL)
+  auto load_step = [&](int step) {
+    const int t = dir ? step : (T - 1 - step);
+    const int tp = dir ? t + 1 : t - 1;
+    // GRU, VL: the output at tp >= len is the masked 0, not the kept state; the LSTM reads the kept c from `extra`
+    const bool has_prev = step < T - 1 && !(MODE == B200RNN_GRU && VL && tp >= len);
+#pragma unroll
+    for (int g = 0; g < G; ++g) sv[g] = gates[((size_t)t * B + row) * GH + g * H + j];
+    if constexpr (G > 1) sx = extra[((size_t)t * B + row) * H + j];
+    dyv = p.dy[(long long)t * p.dy_st + (long long)row * p.dy_sb + dir * H + j];
+    if constexpr (G > 1) {
+      if (!has_prev)
+        hp = s0 ? s0[((size_t)dir * B + row) * H + j] : 0.f;
+      else if (MODE == B200RNN_GRU)
+        hp = p.y[(long long)tp * p.y_st + (long long)row * p.y_sb + dir * H + j];
+      else
+        hp = extra[((size_t)tp * B + row) * H + j];
+    }
+  };
+  if (valid && T > 0) load_step(0);
+  const bool want_dh0 = p.dh_0 != nullptr;
+
+  for (int step = 0; step <= T; ++step) {
+    if (step > 0) {  // dh of this step from the gate gradients step - 1 sent
+      const int cur = step & 1;
+      wait_bars(bars, cur, C, rank, ((step - 1) >> 1) & 1);
+      float acc[G];
+#pragma unroll
+      for (int g = 0; g < G; ++g) acc[g] = 0.f;
+      dot_rows16<G, ONCHIP, (G > 1), WT>(wrow, wg, d_s + ((size_t)cur * BS + b) * GH, H, H, acc);
+      float sum = acc[0];
+#pragma unroll
+      for (int g = 1; g < G; ++g) sum += acc[g];
+      dh_carry = direct + sum;
+    }
+    if (step == T) break;
+    const int t = dir ? step : (T - 1 - step);
+    const bool last = step == T - 1;
+    const bool send = !last || want_dh0;
+    const int nxt = (step + 1) & 1;
+    if (tid == 0 && send) arm_bars(bars, nxt, s, H, G);
+
+    const bool frozen = VL && t >= len;  // the output of a frozen step is the constant 0: its dy reaches nothing
+    const float dh = frozen ? dh_carry : dh_carry + dyv;
+    float dg[G], dhn = 0.f;
+    if constexpr (MODE == B200RNN_GRU) {
+      direct = gru_cell_bwd(sv, sx, hp, dh, dg, dhn);
+    } else if constexpr (MODE == B200RNN_LSTM) {
+      const float dc_next = lstm_cell_bwd(sv, sx, hp, dh, dc_carry, dg);
+      direct = 0.f;
+      if (!frozen) dc_carry = dc_next;  // frozen: dh and dc pass straight through
+    } else {  // Elman: dpre from the saved h_t; frozen as below
+      dg[0] = frozen ? 0.f : elman_cell_bwd(sv[0], dh, relu);
+      direct = frozen ? dh : 0.f;
+    }
+    if (G > 1 && frozen) {
+#pragma unroll
+      for (int g = 0; g < G; ++g) dg[g] = 0.f;
+      dhn = 0.f;
+      direct = dh;
+    }
+    if (valid) {
+#pragma unroll
+      for (int g = 0; g < G; ++g) bsum[g] += dg[g];
+      if constexpr (NP > G) bsum[G] += dhn;
+      float* gp = dgates + ((size_t)t * B + row) * GH + j;
+#pragma unroll
+      for (int g = 0; g < G; ++g) gp[g * H] = dg[g];
+      if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + row) * H + j] = dhn;
+    }
+    if (!send) break;
+    float* d_nxt = d_s + (size_t)nxt * BS * GH;
+#pragma unroll
+    for (int g = 0; g < G; ++g) {  // the recurrent-side gate gradient (GRU n block: dn * r)
+      const float v = (MODE == B200RNN_GRU && g == 2) ? dhn : dg[g];
+      if (s.active) d_nxt[(size_t)b * GH + g * H + j] = valid ? v : 0.f;
+    }
+    __syncthreads();  // the own slice is complete (and every thread is past step - 1's reads of buffer nxt)
+    send_slice(d_nxt, GH, G, H, s, &bars[nxt * C + rank]);
+    if (valid && !last) load_step(step + 1);
+  }
+  // gradients w.r.t. the initial state: what the scan carried past its first step (a cluster that ran no step passes
+  // dh_n / dc_n on)
+  if (valid) {
+    if (want_dh0) p.dh_0[((size_t)dir * B + row) * H + j] = dh_carry;
+    if (MODE == B200RNN_LSTM && p.dc_0) p.dc_0[((size_t)dir * B + row) * H + j] = dc_carry;
+    if (VL)  // the steps [T, p.T) the cluster skipped: their gate gradients are 0
+      for (int t = T; t < p.T; ++t) {
+        float* gp = dgates + ((size_t)t * B + row) * GH + j;
+#pragma unroll
+        for (int g = 0; g < G; ++g) gp[g * H] = 0.f;
+        if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + row) * H + j] = 0.f;
+      }
+  }
+  // per-slice bias-gradient partials [nslices][NP * H] (api.cu reduces them): the slice's batch slots summed in slot
+  // order
+  if (s.active) {
+#pragma unroll
+    for (int g = 0; g < NP; ++g) red[((size_t)b * NP + g) * HS + u] = bsum[g];
+  }
+  __syncthreads();
+  if (s.active && b == 0) {
+    for (int g = 0; g < NP; ++g) {
+      float v = 0.f;
+      for (int q = 0; q < BS; ++q) v += red[((size_t)q * NP + g) * HS + u];
+      float* out = p.dbias_part[dir] + (size_t)s.slice * NP * H;
+      out[g * H + j] = v;
+    }
+  }
+  ptx::cluster_sync_all();
+}
+
+
+// 16-bit transposed weight_hh: half the shared memory per weight row, as in the forward
+template <int MODE, bool VL, bool ONCHIP, typename WT>
+__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_bwd_kernel(const RecBwdParams p, const int nslices) {
+  anyh_bwd_body<MODE, VL, ONCHIP, WT>(p, nslices);
+}
+
 // =================================================================================================
 // config choice
 // =================================================================================================
-// bytes of dynamic shared memory of one launch shape (the Elman backward uses BS x HS floats fewer than this)
-size_t anyh_smem(int G, int H, int C, int BS, bool bwd, bool onchip) {
+}  // namespace
+
+// the Elman backward uses BS x HS floats fewer than this; each staged weight row is padded by 16 bytes
+size_t anyh_smem(int G, int H, int C, int BS, bool bwd, bool onchip, int wbytes) {
   const size_t HS = (size_t)anyh_max_units(H, C);
-  size_t f = onchip ? (size_t)G * HS * (H + 4) : 0;
-  f += (size_t)2 * BS * (bwd ? G * H : H);
+  const size_t w = onchip ? (size_t)G * HS * (H + 16 / wbytes) * wbytes : 0;
+  size_t f = (size_t)2 * BS * (bwd ? G * H : H);
   if (bwd) f += (size_t)BS * (G + 1) * HS;
-  return f * sizeof(float) + (size_t)2 * C * sizeof(uint64_t);
+  return w + f * sizeof(float) + (size_t)2 * C * sizeof(uint64_t);
 }
+
+namespace {
 
 template <typename P>
 using AnyhKernel = void (*)(P, int);
 
-template <int MODE>
-AnyhKernel<RecFwdParams> anyh_kernel(const RecFwdParams&, bool vl, bool onchip) {
-  return vl ? (onchip ? anyh_fwd_kernel<MODE, true, true> : anyh_fwd_kernel<MODE, true, false>)
-            : (onchip ? anyh_fwd_kernel<MODE, false, true> : anyh_fwd_kernel<MODE, false, false>);
+template <int MODE, typename WT>
+AnyhKernel<RecFwdParams> anyh16_kernel(const RecFwdParams&, bool vl, bool onchip) {
+  return vl ? (onchip ? anyh16_fwd_kernel<MODE, true, true, WT> : anyh16_fwd_kernel<MODE, true, false, WT>)
+            : (onchip ? anyh16_fwd_kernel<MODE, false, true, WT> : anyh16_fwd_kernel<MODE, false, false, WT>);
+}
+template <int MODE, typename WT>
+AnyhKernel<RecBwdParams> anyh16_kernel(const RecBwdParams&, bool vl, bool onchip) {
+  return vl ? (onchip ? anyh16_bwd_kernel<MODE, true, true, WT> : anyh16_bwd_kernel<MODE, true, false, WT>)
+            : (onchip ? anyh16_bwd_kernel<MODE, false, true, WT> : anyh16_bwd_kernel<MODE, false, false, WT>);
 }
 template <int MODE>
 AnyhKernel<RecBwdParams> anyh_kernel(const RecBwdParams&, bool vl, bool onchip) {
   return vl ? (onchip ? anyh_bwd_kernel<MODE, true, true> : anyh_bwd_kernel<MODE, true, false>)
             : (onchip ? anyh_bwd_kernel<MODE, false, true> : anyh_bwd_kernel<MODE, false, false>);
+}
+template <int MODE>
+AnyhKernel<RecFwdParams> anyh_kernel(const RecFwdParams&, bool vl, bool onchip) {
+  return vl ? (onchip ? anyh_fwd_kernel<MODE, true, true> : anyh_fwd_kernel<MODE, true, false>)
+            : (onchip ? anyh_fwd_kernel<MODE, false, true> : anyh_fwd_kernel<MODE, false, false>);
+}
+// w16: the storage of weight_hh, DT_F32 or DT_F16 / DT_BF16 (h16.cuh)
+template <int MODE, typename P>
+AnyhKernel<P> anyh_kernel_w(const P& p, bool vl, bool onchip, int w16) {
+  if (w16 == DT_F16) return anyh16_kernel<MODE, __half>(p, vl, onchip);
+  if (w16 == DT_BF16) return anyh16_kernel<MODE, __nv_bfloat16>(p, vl, onchip);
+  return anyh_kernel<MODE>(p, vl, onchip);
 }
 
 // The cluster shape of one launch. Candidates: C in {2, 4, 8, 16} with at least one group of 8 units per CTA
@@ -460,15 +803,16 @@ AnyhKernel<RecBwdParams> anyh_kernel(const RecBwdParams&, bool vl, bool onchip) 
 //     every load): the widest cluster, then the fewest waves, then the fewest batch rows.
 // Capacities come from the driver (cluster_capacity), never from the SM count; clusters that do not fit run in waves.
 template <typename P>
-int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L) {
+int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L, int w16) {
+  const int wbytes = w16 ? 2 : 4;
   const int G = gates_of(p.mode), H = p.H;
   const bool vl = p.lengths != nullptr;
   for (int tier = 0; tier < 2; ++tier) {
     const bool onchip = tier == 0;
     // one Elman instantiation for both nonlinearities
-    const AnyhKernel<P> kernel = p.mode == B200RNN_GRU    ? anyh_kernel<B200RNN_GRU>(p, vl, onchip)
-                                 : p.mode == B200RNN_LSTM ? anyh_kernel<B200RNN_LSTM>(p, vl, onchip)
-                                                          : anyh_kernel<B200RNN_RNN_TANH>(p, vl, onchip);
+    const AnyhKernel<P> kernel = p.mode == B200RNN_GRU    ? anyh_kernel_w<B200RNN_GRU>(p, vl, onchip, w16)
+                                 : p.mode == B200RNN_LSTM ? anyh_kernel_w<B200RNN_LSTM>(p, vl, onchip, w16)
+                                                          : anyh_kernel_w<B200RNN_RNN_TANH>(p, vl, onchip, w16);
     bool found = false;
     long long best[3] = {0, 0, 0};
     ClusterLaunch<P> pick{};
@@ -478,7 +822,7 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L) {
       for (int BS = 2; BS <= 64; BS *= 2) {
         const int NT = (HS * BS + 31) / 32 * 32;
         if (NT > ANYH_MAX_NT) continue;
-        const size_t smem = anyh_smem(G, H, C, BS, bwd, onchip);
+        const size_t smem = anyh_smem(G, H, C, BS, bwd, onchip, wbytes);
         if (smem > (size_t)MAX_SMEM) continue;
         const int nslices = (p.B + BS - 1) / BS, nclusters = nslices * p.D;
         int capacity = 0;
@@ -506,9 +850,10 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L) {
     if (found) {
       static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
       if (debug)
-        fprintf(stderr, "[b200rnn] %s %s cfg %s VL=%d H=%d C=%d BS=%d tier=%s: need %d clusters, capacity %d, smem %zu\n",
+        fprintf(stderr, "[b200rnn] %s %s cfg %s VL=%d H=%d C=%d BS=%d tier=%s%s: need %d clusters, capacity %d, smem %zu\n",
                 bwd ? "bwd" : "fwd", G == 1 ? "elman" : "anyh", mode_name(p.mode), (int)vl, H, pick.C, pick.BS,
-                onchip ? "smem" : "l2", pick.nclusters, pick.capacity, pick.smem);
+                onchip ? "smem" : "l2", wbytes == 2 ? " w_hh=16bit" : "", pick.nclusters, pick.capacity,
+                pick.smem);
       *L = pick;
       return B200RNN_OK;
     }
@@ -521,21 +866,21 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L) {
 
 bool anyh_hidden_size(int H) { return H >= 16 && H <= 1024 && H % 16 == 0; }
 
-int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
+int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16) {
   if (p.y_pool || p.ready || p.shell_nograd || p.P > 0) {
     set_error("recurrence: hidden_size %d runs without the model-shell fusions (y_pool, streamed x-projection, "
               "no-grad fused forward) and without proj_size", p.H);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  return plan_anyh(p, false, L);
+  return plan_anyh(p, false, L, w16);
 }
 
-int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
+int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16) {
   if (!p.dy || p.P > 0) {
     set_error("recurrence backward: hidden_size %d takes the full output gradient dy and no proj_size", p.H);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  return plan_anyh(p, true, L);
+  return plan_anyh(p, true, L, w16);
 }
 
 }  // namespace b200rnn

@@ -119,19 +119,26 @@ int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capaci
 // The runtime-sized recurrence (rnn_anyh.cu): the hidden sizes it takes (H % 16 == 0, 16 <= H <= 1024) and its config
 // choice for the GRU / LSTM shapes the fixed configs do not cover and for every Elman shape
 bool anyh_hidden_size(int H);
-int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* out);
-int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out);
+// bytes of dynamic shared memory of one runtime-sized launch shape: G gate blocks, C-CTA clusters of BS batch rows,
+// backward or forward, weight_hh on chip (onchip) in wbytes per weight (4: fp32, 2: 16-bit)
+size_t anyh_smem(int G, int H, int C, int BS, bool bwd, bool onchip, int wbytes);
+// w16: the storage of weight_hh, 0 (fp32) or DT_F16 / DT_BF16 (h16.cuh): the 16-bit kernels stage half the bytes
+int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* out, int w16 = 0);
+int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out, int w16 = 0);
 
 // forward: choose the config for p's shape (mode, H, P, B, D, lengths or not), then launch it; p.ready != NULL launches
 // it with programmatic stream serialization, so that it may start while the GEMM before it still runs
-int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* out);
+// w16: the storage of p.w_hh (see plan_anyh_fwd), taken by the runtime-sized kernels; the fixed configs read fp32
+int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* out, int w16 = 0);
 int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t stream);
 // W_hh [3*256][256] of a GRU-256 layer (16-byte aligned) -> h16::Gru256::CACHE_BYTES at img (256-byte aligned): the
 // fp16 pairs and row scales the prologue of rec_fwd_h16_kernel would make, in its shared-memory order per CTA rank
 int prep_whh_h16(const float* w_hh, void* img, cudaStream_t stream);
 // backward: the same choice (plan_rec_bwd), then one launch that also prepares W_hh for the unprojected kernels and sets
 // p.nslices_out
-int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* out);
-int launch_rec_bwd(RecBwdParams& p, cudaStream_t stream);
+// whh16 (optional, with w16 != 0): per direction the 16-bit weight_hh; when the runtime-sized kernels run, W_hh is
+// transposed from it in 16 bits and staged as such (p.w_prep then holds 16-bit data); otherwise p.w_hh (fp32) is used
+int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* out, int w16 = 0);
+int launch_rec_bwd(RecBwdParams& p, cudaStream_t stream, int w16 = 0, const void* const* whh16 = nullptr);
 
 }  // namespace b200rnn

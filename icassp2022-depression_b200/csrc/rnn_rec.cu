@@ -1845,7 +1845,7 @@ int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capaci
 // (one wave => every sequence advances in lock step) wins, else the widest one runs in several waves.
 // Template arguments: <MODE, H, C, BS, KL, UPL, RG>; projected: <H, P, C, BS>, H = 128 on 2-CTA clusters of 4 batch rows
 // (256 threads), H = 256 on 4-CTA clusters of 8 batch rows (512 threads).
-int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
+int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16) {
   int rc = B200RNN_OK;
   L->kernel = nullptr;
   if (p.B <= 0 || p.T <= 0) return rc;
@@ -1859,7 +1859,7 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
     return B200RNN_ERR_UNSUPPORTED;
   }
   // the Elman modes run the runtime-sized kernels at every hidden size, 128 and 256 included (rnn_anyh.cu)
-  if (is_elman(p.mode)) return plan_anyh_fwd(p, L);
+  if (is_elman(p.mode)) return plan_anyh_fwd(p, L, w16);
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
   if (p.mode == B200RNN_GRU && p.H == 256) {
@@ -1897,14 +1897,14 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L) {
     return rc;
   }
   // every other hidden size: the runtime-sized kernels of rnn_anyh.cu
-  if (anyh_hidden_size(p.H)) return plan_anyh_fwd(p, L);
+  if (anyh_hidden_size(p.H)) return plan_anyh_fwd(p, L, w16);
   set_error("recurrence: unsupported (mode=%d, hidden_size=%d); built for hidden_size 128 and 256", p.mode,
             p.H);
   return B200RNN_ERR_UNSUPPORTED;
 }
 
 // The same rule and projected configs as the forward
-int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
+int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16) {
   int rc = B200RNN_OK;
   L->kernel = nullptr;
   if (p.B <= 0 || p.T <= 0) return rc;
@@ -1916,7 +1916,7 @@ int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
     set_error("recurrence backward: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d)", p.mode, p.H, p.P);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  if (is_elman(p.mode)) return plan_anyh_bwd(p, L);
+  if (is_elman(p.mode)) return plan_anyh_bwd(p, L, w16);
   // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
   // (not the weights) dominates the shared-memory traffic of the backward contraction
   if (p.mode == B200RNN_GRU && p.H == 256) {
@@ -1940,7 +1940,7 @@ int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L) {
     pick_bwd<B200RNN_LSTM, 128, 4, 8, 32, 4, 1>(p, true, L, &rc);
     return rc;
   }
-  if (anyh_hidden_size(p.H)) return plan_anyh_bwd(p, L);
+  if (anyh_hidden_size(p.H)) return plan_anyh_bwd(p, L, w16);
   set_error("recurrence backward: unsupported (mode=%d, hidden_size=%d)", p.mode, p.H);
   return B200RNN_ERR_UNSUPPORTED;
 }
@@ -1975,15 +1975,16 @@ namespace {
 // The backward's W_hh for a C-CTA cluster, transposed and contiguous per CTA: CTA r's block starts at G * j0_r * H and
 // holds out[G*j0_r*H + (g*n_r + u)*H + jj] = W_hh[g*H + jj][j0_r + u] (anyh_units). For the fixed configs (C divides
 // H / 8) this is the [C ranks][G][H / C][H] layout rec_bwd_kernel copies with TMA.
-__global__ void whh_prep_kernel(const float* __restrict__ w_hh, float* __restrict__ out, int G, int H, int C) {
-  __shared__ float tile[32][33];
+template <typename T>
+__device__ __forceinline__ void whh_prep_body(const T* __restrict__ w_hh, T* __restrict__ out, int G, int H, int C) {
+  __shared__ T tile[32][33];
   const int nt = (H + 31) / 32;
   for (int tix = blockIdx.x; tix < G * nt * nt; tix += gridDim.x) {
     const int g = tix / (nt * nt), rem = tix - g * nt * nt;
     const int tj = rem / nt, tk = rem - tj * nt;  // row tile of the gate block, column tile
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {
       const int r = tj * 32 + i, k = tk * 32 + threadIdx.x;
-      tile[i][threadIdx.x] = (r < H && k < H) ? w_hh[((size_t)g * H + r) * H + k] : 0.f;
+      tile[i][threadIdx.x] = (r < H && k < H) ? w_hh[((size_t)g * H + r) * H + k] : T(0);
     }
     __syncthreads();
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {
@@ -2000,15 +2001,30 @@ __global__ void whh_prep_kernel(const float* __restrict__ w_hh, float* __restric
   }
 }
 
+__global__ void whh_prep_kernel(const float* __restrict__ w_hh, float* __restrict__ out, int G, int H, int C) {
+  whh_prep_body<float>(w_hh, out, G, H, C);
+}
+
+// the same transpose of a 16-bit weight_hh, bit for bit (the 16-bit runtime-sized backward stages it as it lies)
+__global__ void whh_prep16_kernel(const uint16_t* __restrict__ w_hh, uint16_t* __restrict__ out, int G, int H, int C) {
+  whh_prep_body<uint16_t>(w_hh, out, G, H, C);
+}
+
 }  // namespace
 
-int launch_rec_bwd(RecBwdParams& p, cudaStream_t s) {
+int launch_rec_bwd(RecBwdParams& p, cudaStream_t s, int w16, const void* const* whh16) {
   RecBwdLaunch L;
-  const int rc = plan_rec_bwd(p, &L);
+  if (!whh16) w16 = 0;
+  const int rc = plan_rec_bwd(p, &L, w16);
   if (rc != B200RNN_OK || L.kernel == nullptr) return rc;
   if (p.P == 0) {  // the unprojected kernels read W_hh transposed for the chosen cluster width
     for (int d = 0; d < p.D; ++d) {
-      whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C);
+      if (L.anyh && w16)
+        whh_prep16_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(static_cast<const uint16_t*>(whh16[d]),
+                                                          reinterpret_cast<uint16_t*>(p.w_prep[d]), gates_of(p.mode),
+                                                          p.H, L.C);
+      else
+        whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C);
       if (cudaGetLastError() != cudaSuccess) {
         set_error("whh_prep launch failed");
         return B200RNN_ERR_CUDA;

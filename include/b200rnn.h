@@ -19,7 +19,7 @@
  *   - purely stream-ordered: all work is enqueued on `stream`, no host synchronisation, no hidden
  *     allocation on the hot path, capturable in a CUDA graph;
  *   - int return: 0 = ok, <0 = error (message via b200rnn_last_error(), thread-local);
- *   - fp32 everywhere ("dtype": "f32").
+ *   - fp32 everywhere ("dtype": "f32"), except the sequence calls with B200RNN_FLAG_F16 / B200RNN_FLAG_BF16.
  */
 #ifndef B200RNN_H_
 #define B200RNN_H_
@@ -67,6 +67,17 @@ enum {
                                              forward / forward_fused / backward / backward_fused (set it identically for
                                              a forward and its backward); workspace_bytes and prepare_weights accept it.
                                              b200rnn_gemm_f32 is always 3xTF32. */
+#define B200RNN_FLAG_F16 64u              /* 16-bit tensors (torch.float16 modules): x, every parameter, h_0 / c_0, y, h_n /
+                                             c_n, dy, dh_n / dc_n and every gradient output of b200rnn_forward(_hx) /
+                                             b200rnn_backward(_hx) are IEEE fp16 (the pointers keep their float types).
+                                             The input projection multiplies the 16-bit operands on the tensor cores
+                                             (exact products, fp32 sums), the state is carried in fp32, each output is
+                                             rounded to nearest even once; an inner layer's output is rounded before
+                                             the dropout and after it. The reserve and the scratch stay fp32 and internal
+                                             (b200rnn_workspace_bytes sizes them for the flag). Not with
+                                             B200RNN_FLAG_PROJ; the _fused entry points and the weight cache return
+                                             B200RNN_ERR_UNSUPPORTED. */
+#define B200RNN_FLAG_BF16 128u            /* the same with bfloat16 tensors; excludes B200RNN_FLAG_F16 */
 
 /*
  * Problem descriptor. Mirrors the constructor arguments of torch.nn.GRU / torch.nn.LSTM
