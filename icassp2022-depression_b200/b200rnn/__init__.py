@@ -6,6 +6,7 @@ PyTorch host code -> C-ABI shared library (include/b200rnn.h) -> hand-written CU
 Importing this package does not need a GPU; running any op does, and fails loudly without one.
 """
 from . import _lib
+from . import ops  # registers the b200rnn:: custom ops (torch.export / torch.compile)
 from ._lib import B200RNNError
 from .modules import GRU, LSTM, RNN, GRUCell, LSTMCell, RNNCell, from_torch, install, uninstall
 from .functional import RNNConfig, gemm, rnn_forward

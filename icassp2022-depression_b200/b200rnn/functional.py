@@ -36,6 +36,7 @@ class RNNConfig:
         return self.proj_size if self.proj_size > 0 else self.hidden_size
 
 
+@torch.compiler.assume_constant_result   # dynamo cannot read the setting: a compiled graph keeps the value it traced
 def tf32_enabled() -> bool:
     """Whether torch's fp32 matmul precision asks for TF32: ``torch.backends.cuda.matmul.fp32_precision``, or, while
     that is ``"none"``, the global ``torch.backends.fp32_precision``. ``torch.set_float32_matmul_precision("high")``
@@ -107,15 +108,19 @@ def _on(device):
     return torch.cuda.device(device)
 
 
-def _weight_grad_targets(weights, needed, sink, dev):
+def _weight_grad_targets(weights, needed, sink, dev, separate: bool = False):
     """Where a backward writes the weight gradients, as ``(dptrs, grads_out, accumulate)``: straight into the views
     ``sink(weights)`` returns (a flat all-reduce bucket; the kernels accumulate into them, ``grads_out`` is all None),
     or into one fresh flat buffer (in the weights' dtype) whose views are returned to autograd. ``needed[i]``: whether
-    ``weights[i]`` wants a gradient (a NULL target otherwise). Each fresh view starts on a 256-byte boundary."""
+    ``weights[i]`` wants a gradient (a NULL target otherwise). Each fresh view starts on a 256-byte boundary.
+    ``separate``: one fresh tensor per gradient instead (the custom ops, whose outputs may not alias each other)."""
     if sink is not None:
         targets = sink(weights)  # list of tensors (same shapes) or None entries
         dptrs = [t.data_ptr() if (t is not None and n) else None for t, n in zip(targets, needed)]
         return dptrs, [None] * len(weights), True
+    if separate:
+        grads_out = _weight_grad_buffers(weights, needed)
+        return [g.data_ptr() if g is not None else None for g in grads_out], grads_out, False
     align = 256 // weights[0].element_size()
     sizes = [(w.numel() + align - 1) // align * align if n else 0 for w, n in zip(weights, needed)]
     flat = torch.empty(sum(sizes), dtype=weights[0].dtype, device=dev)
@@ -124,6 +129,134 @@ def _weight_grad_targets(weights, needed, sink, dev):
         grads_out.append(flat[off:off + w.numel()].view_as(w) if n else None)
         off += size
     return [g.data_ptr() if g is not None else None for g in grads_out], grads_out, False
+
+
+def _weight_grad_buffers(weights, needed):
+    """one fresh gradient tensor per weight that wants one (None otherwise); the weights are contiguous"""
+    return [torch.empty_like(w) if n else None for w, n in zip(weights, needed)]
+
+
+def _forward_buffers(x_tm: torch.Tensor, cfg: RNNConfig, save: bool, with_scratch: bool = True):
+    """Descriptor and the buffers of one sequence forward, as ``(desc, reserve, scratch, y, (ys_t, ys_b), h_n, c_n)``:
+    ``y`` batch-first or time-major as ``cfg`` says, ``c_n`` None but for the LSTM, the reserve empty without ``save``.
+    Host arithmetic only (``b200rnn_workspace_bytes``), so the custom ops' fake implementations call it too, without
+    the scratch."""
+    T, B, _ = x_tm.shape
+    H, L, D, HO = cfg.hidden_size, cfg.num_layers, cfg.num_dirs, cfg.out_size
+    dev = x_tm.device
+    desc = _make_desc(cfg, B, T, save)
+    rbytes, sbytes = _lib.workspace_bytes(desc)
+    reserve = torch.empty(rbytes if save else 0, dtype=torch.uint8, device=dev)
+    scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev) if with_scratch else None
+    dt = cfg.dtype
+    if cfg.batch_first:
+        y = torch.empty(B, T, D * HO, dtype=dt, device=dev)
+        ys = (D * HO, T * D * HO)
+    else:
+        y = torch.empty(T, B, D * HO, dtype=dt, device=dev)
+        ys = (B * D * HO, D * HO)
+    h_n = torch.empty(L * D, B, HO, dtype=dt, device=dev)
+    c_n = torch.empty(L * D, B, H, dtype=dt, device=dev) if cfg.mode == _lib.LSTM else None
+    return desc, reserve, scratch, y, ys, h_n, c_n
+
+
+def _rnn_forward_impl(x_tm: torch.Tensor, cfg: RNNConfig, rng_state: Optional[torch.Tensor],
+                      lengths: Optional[torch.Tensor], save: bool, h_0: Optional[torch.Tensor],
+                      c_0: Optional[torch.Tensor], weights: Sequence[torch.Tensor]):
+    """The sequence forward (one ``b200rnn_forward_hx`` call) shared by :class:`_RNNFunction` and the
+    ``b200rnn::rnn_forward`` op: returns ``(y, h_n, c_n, reserve)``, ``c_n`` None but for the LSTM."""
+    lib = _lib.load()
+    T, B, _ = x_tm.shape
+    dev = x_tm.device
+    desc, reserve, scratch, y, (ys_t, ys_b), h_n, c_n = _forward_buffers(x_tm, cfg, save)
+    params = _lib.ptr_array([w.data_ptr() for w in weights])
+    rng_ptr = rng_state.data_ptr() if rng_state is not None else None
+    len_ptr = lengths.data_ptr() if lengths is not None else None
+    c_n_ptr = c_n.data_ptr() if c_n is not None else None
+    if B > 0 and T > 0:
+        # the module forward, with or without hx: the model-shell entry b200rnn_forward_fused is for
+        # rnn_forward_fused / rnn_ln_pool_sum (its no-grad GRU-256 recurrence runs on fp16 pairs)
+        with _on(dev):
+            rc = lib.b200rnn_forward_hx(
+                ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+                y.data_ptr(), ys_t, ys_b, h_0.data_ptr() if h_0 is not None else None,
+                c_0.data_ptr() if c_0 is not None else None,
+                h_n.data_ptr(), c_n_ptr, reserve.data_ptr() if save else None, scratch.data_ptr(),
+                0, 0, rng_ptr, len_ptr, _stream_ptr(dev))
+        _lib.check(rc, "b200rnn_forward")
+    else:   # no step: the final state is the initial one
+        h_n.copy_(h_0) if h_0 is not None else h_n.zero_()
+        if c_n is not None:
+            c_n.copy_(c_0) if c_0 is not None else c_n.zero_()
+    return y, h_n, c_n, reserve
+
+
+def _dx_buffer(x_tm: torch.Tensor) -> torch.Tensor:
+    """the input gradient: laid out like ``x_tm`` when its feature stride is 1, else dense time-major"""
+    dx = torch.empty_like(x_tm)
+    if dx.stride(2) != 1 and dx.size(2) != 1:
+        dx = torch.empty(x_tm.shape, dtype=x_tm.dtype, device=x_tm.device)
+    return dx
+
+
+def _rnn_backward_impl(cfg: RNNConfig, x_tm, y, reserve, h_0, c_0, weights, dy, dh_n, dc_n, lengths,
+                       need_dx: bool, need_dh_0: bool, need_dc_0: bool, need_w, grad_sink, separate: bool = False):
+    """BPTT (``b200rnn_backward`` / ``_hx``) shared by :class:`_RNNFunction` and the ``b200rnn::rnn_backward`` op:
+    returns ``(dx, dh_0, dc_0, weight grads)``, None for every gradient that is not wanted (a NULL pointer to the
+    library). ``grad_sink`` / ``separate``: see :func:`_weight_grad_targets`."""
+    lib = _lib.load()
+    T, B, _ = x_tm.shape
+    dev = x_tm.device
+    if cfg.batch_first:
+        ys_t, ys_b = cfg.num_dirs * cfg.out_size, T * cfg.num_dirs * cfg.out_size
+    else:
+        ys_t, ys_b = B * cfg.num_dirs * cfg.out_size, cfg.num_dirs * cfg.out_size
+    # gradients w.r.t. the initial state only when autograd asks: dh_0 costs the last step's contraction
+    dh_0 = torch.empty_like(h_0) if h_0 is not None and need_dh_0 else None
+    dc_0 = torch.empty_like(c_0) if c_0 is not None and need_dc_0 else None
+
+    if dy is None:
+        dy = torch.zeros_like(y)
+    if dy.stride(2) != 1 and dy.size(2) != 1:
+        dy = dy.contiguous()
+    if cfg.batch_first:
+        dys_t, dys_b = dy.stride(1), dy.stride(0)
+    else:
+        dys_t, dys_b = dy.stride(0), dy.stride(1)
+    if dh_n is not None:
+        dh_n = dh_n.contiguous()
+    if dc_n is not None:
+        dc_n = dc_n.contiguous()
+
+    dx = _dx_buffer(x_tm) if need_dx else None
+
+    dptrs, grads_out, accumulate = _weight_grad_targets(weights, need_w, grad_sink, dev, separate)
+    desc = _make_desc(cfg, B, T, True, accumulate)
+    _, sbytes = _lib.workspace_bytes(desc)
+    scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+    params = _lib.ptr_array([w.data_ptr() for w in weights])
+    dparams = _lib.ptr_array(dptrs)
+    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    if B > 0 and T > 0:
+        with _on(dev):
+            head = (ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+                    y.data_ptr(), ys_t, ys_b, dy.data_ptr(), dys_t, dys_b, ptr(dh_n), ptr(dc_n))
+            tail = (reserve.data_ptr(), scratch.data_ptr(), ptr(dx),
+                    dx.stride(0) if dx is not None else 0, dx.stride(1) if dx is not None else 0,
+                    dparams, ptr(lengths), _stream_ptr(dev))
+            if h_0 is None and not cfg.proj_size:
+                rc = lib.b200rnn_backward(*head, *tail)
+            else:
+                rc = lib.b200rnn_backward_hx(*head, ptr(h_0), ptr(c_0), ptr(dh_0), ptr(dc_0), *tail)
+        _lib.check(rc, "b200rnn_backward")
+    else:   # no step: parameters get nothing, the state gradients pass through
+        for g in grads_out:
+            if g is not None:
+                g.zero_()
+        for d0, dn in ((dh_0, dh_n), (dc_0, dc_n)):
+            if d0 is not None:
+                d0.copy_(dn) if dn is not None else d0.zero_()
+    return dx, dh_0, dc_0, grads_out
 
 
 class _RNNFunction(torch.autograd.Function):
@@ -138,49 +271,13 @@ class _RNNFunction(torch.autograd.Function):
     def forward(ctx, x_tm: torch.Tensor, cfg: RNNConfig, rng_state: Optional[torch.Tensor], grad_sink,
                 lengths: Optional[torch.Tensor], save: bool, h_0: Optional[torch.Tensor], c_0: Optional[torch.Tensor],
                 *weights: torch.Tensor):
-        lib = _lib.load()
-        T, B, _ = x_tm.shape
-        H, L, D, HO = cfg.hidden_size, cfg.num_layers, cfg.num_dirs, cfg.out_size
-        dev = x_tm.device
         # `save` is decided by the caller: grad mode is always off in here, and needs_input_grad is True for
         # requires_grad weights even under torch.no_grad() (it would allocate the reserve and store gates for nothing)
         save = bool(save) and any(ctx.needs_input_grad)
-        desc = _make_desc(cfg, B, T, save)
-        rbytes, sbytes = _lib.workspace_bytes(desc)
-        reserve = torch.empty(rbytes if save else 0, dtype=torch.uint8, device=dev)
-        scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
-        dt = cfg.dtype
-        if cfg.batch_first:
-            y = torch.empty(B, T, D * HO, dtype=dt, device=dev)
-            ys_t, ys_b = D * HO, T * D * HO
-        else:
-            y = torch.empty(T, B, D * HO, dtype=dt, device=dev)
-            ys_t, ys_b = B * D * HO, D * HO
-        h_n = torch.empty(L * D, B, HO, dtype=dt, device=dev)
-        c_n = torch.empty(L * D, B, H, dtype=dt, device=dev) if cfg.mode == _lib.LSTM else None
-        params = _lib.ptr_array([w.data_ptr() for w in weights])
-        rng_ptr = rng_state.data_ptr() if rng_state is not None else None
-        len_ptr = lengths.data_ptr() if lengths is not None else None
-        c_n_ptr = c_n.data_ptr() if c_n is not None else None
-        if B > 0 and T > 0:
-            # the module forward, with or without hx: the model-shell entry b200rnn_forward_fused is for
-            # rnn_forward_fused / rnn_ln_pool_sum (its no-grad GRU-256 recurrence runs on fp16 pairs)
-            with _on(dev):
-                rc = lib.b200rnn_forward_hx(
-                    ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
-                    y.data_ptr(), ys_t, ys_b, h_0.data_ptr() if h_0 is not None else None,
-                    c_0.data_ptr() if c_0 is not None else None,
-                    h_n.data_ptr(), c_n_ptr, reserve.data_ptr() if save else None, scratch.data_ptr(),
-                    0, 0, rng_ptr, len_ptr, _stream_ptr(dev))
-            _lib.check(rc, "b200rnn_forward")
-        else:   # no step: the final state is the initial one
-            h_n.copy_(h_0) if h_0 is not None else h_n.zero_()
-            if c_n is not None:
-                c_n.copy_(c_0) if c_0 is not None else c_n.zero_()
+        y, h_n, c_n, reserve = _rnn_forward_impl(x_tm, cfg, rng_state, lengths, save, h_0, c_0, weights)
         if save:
             ctx.cfg = cfg
             ctx.grad_sink = grad_sink
-            ctx.ys = (ys_t, ys_b)
             ctx.lengths = lengths
             ctx.save_for_backward(x_tm, y, reserve, h_0, c_0, *weights)
         if c_n is None:
@@ -189,62 +286,12 @@ class _RNNFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy, dh_n, dc_n=None):
-        lib = _lib.load()
-        cfg: RNNConfig = ctx.cfg
         x_tm, y, reserve, h_0, c_0, *weights = ctx.saved_tensors
-        T, B, _ = x_tm.shape
-        H, L, D = cfg.hidden_size, cfg.num_layers, cfg.num_dirs
-        dev = x_tm.device
-        ys_t, ys_b = ctx.ys
         w0 = _RNNFunction._W0
-        # gradients w.r.t. the initial state only when autograd asks: dh_0 costs the last step's contraction
-        dh_0 = torch.empty_like(h_0) if h_0 is not None and ctx.needs_input_grad[w0 - 2] else None
-        dc_0 = torch.empty_like(c_0) if c_0 is not None and ctx.needs_input_grad[w0 - 1] else None
-
-        if dy is None:
-            dy = torch.zeros_like(y)
-        if dy.stride(2) != 1 and dy.size(2) != 1:
-            dy = dy.contiguous()
-        if cfg.batch_first:
-            dys_t, dys_b = dy.stride(1), dy.stride(0)
-        else:
-            dys_t, dys_b = dy.stride(0), dy.stride(1)
-        if dh_n is not None:
-            dh_n = dh_n.contiguous()
-        if dc_n is not None:
-            dc_n = dc_n.contiguous()
-
-        need_dx = ctx.needs_input_grad[0]
-        dx = torch.empty_like(x_tm) if need_dx else None
-        if dx is not None and dx.stride(2) != 1 and dx.size(2) != 1:
-            dx = torch.empty(x_tm.shape, dtype=x_tm.dtype, device=dev)
-
-        dptrs, grads_out, accumulate = _weight_grad_targets(weights, ctx.needs_input_grad[w0:], ctx.grad_sink, dev)
-        desc = _make_desc(cfg, B, T, True, accumulate)
-        _, sbytes = _lib.workspace_bytes(desc)
-        scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
-        params = _lib.ptr_array([w.data_ptr() for w in weights])
-        dparams = _lib.ptr_array(dptrs)
-        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-        if B > 0 and T > 0:
-            with _on(dev):
-                head = (ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
-                        y.data_ptr(), ys_t, ys_b, dy.data_ptr(), dys_t, dys_b, ptr(dh_n), ptr(dc_n))
-                tail = (reserve.data_ptr(), scratch.data_ptr(), ptr(dx),
-                        dx.stride(0) if dx is not None else 0, dx.stride(1) if dx is not None else 0,
-                        dparams, ptr(ctx.lengths), _stream_ptr(dev))
-                if h_0 is None and not cfg.proj_size:
-                    rc = lib.b200rnn_backward(*head, *tail)
-                else:
-                    rc = lib.b200rnn_backward_hx(*head, ptr(h_0), ptr(c_0), ptr(dh_0), ptr(dc_0), *tail)
-            _lib.check(rc, "b200rnn_backward")
-        else:   # no step: parameters get nothing, the state gradients pass through
-            for g in grads_out:
-                if g is not None:
-                    g.zero_()
-            for d0, dn in ((dh_0, dh_n), (dc_0, dc_n)):
-                if d0 is not None:
-                    d0.copy_(dn) if dn is not None else d0.zero_()
+        need = ctx.needs_input_grad
+        dx, dh_0, dc_0, grads_out = _rnn_backward_impl(ctx.cfg, x_tm, y, reserve, h_0, c_0, weights, dy, dh_n, dc_n,
+                                                       ctx.lengths, need[0], need[w0 - 2], need[w0 - 1], need[w0:],
+                                                       ctx.grad_sink)
         return (dx, None, None, None, None, None, dh_0, dc_0, *grads_out)
 
 
@@ -367,6 +414,13 @@ def _initial_state(hx, cfg: RNNConfig, x: torch.Tensor):
     return states[0], (states[1] if lstm else None)
 
 
+@torch.compiler.disable   # raised outside the trace, so that torch.compile hands the caller this error itself
+def _grad_sink_untraceable():
+    raise _lib.B200RNNError(
+        "b200rnn: a module with a gradient sink (GradBucket / FlatAdamW) writes its gradients into the flat bucket "
+        "behind autograd's back, which torch.compile and torch.export cannot trace; run it eagerly")
+
+
 def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig,
                 rng_state: Optional[torch.Tensor] = None, grad_sink=None, lengths: Optional[torch.Tensor] = None,
                 hx=None):
@@ -402,6 +456,10 @@ def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig
             raise _lib.B200RNNError(f"b200rnn: weight[{i}] is on {w.device} but the input is on {x.device}")
     states = [s for s in (h_0, c_0) if s is not None]
     save = torch.is_grad_enabled() and (x.requires_grad or any(t.requires_grad for t in (*weights, *states)))
+    if torch.compiler.is_compiling():   # dynamo / export: the custom op, which traces without a pointer
+        if grad_sink is not None:
+            _grad_sink_untraceable()
+        return _ops.rnn_forward_traced(x_tm, cfg, rng_state, lengths, save, h_0, c_0, weights)
     return _RNNFunction.apply(x_tm, cfg, rng_state, grad_sink, lengths, save, h_0, c_0, *weights)
 
 
@@ -498,6 +556,70 @@ def _cell_rows(t: torch.Tensor) -> torch.Tensor:
     return t
 
 
+def _cell_forward_buffers(x: torch.Tensor, cfg: CellConfig, save: bool):
+    """``(desc, saved, h_out, c_out)`` of one cell forward (``c_out`` None but for the LSTM, ``saved`` empty without
+    ``save``): host arithmetic only, shared with the ``b200rnn::cell_forward`` op's fake implementation"""
+    B, H, dev = x.size(0), cfg.hidden_size, x.device
+    desc = _cell_desc(cfg, B, save)
+    sv_bytes, _ = _lib.cell_workspace_bytes(desc)
+    saved = torch.empty(sv_bytes if save else 0, dtype=torch.uint8, device=dev)
+    h_out = torch.empty(B, H, dtype=torch.float32, device=dev)
+    c_out = torch.empty(B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
+    return desc, saved, h_out, c_out
+
+
+def _cell_forward_impl(x, cfg: CellConfig, save: bool, h, c, weights):
+    """one ``b200rnn_cell_forward`` call, shared by :class:`_CellFunction` and the ``b200rnn::cell_forward`` op:
+    returns ``(h_out, c_out, saved)``"""
+    lib = _lib.load()
+    dev = x.device
+    desc, saved, h_out, c_out = _cell_forward_buffers(x, cfg, save)
+    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    ld = lambda t: t.stride(0) if t is not None else 0  # noqa: E731
+    params = _lib.ptr_array([w.data_ptr() for w in weights] + [None] * (4 - len(weights)))
+    with _on(dev):
+        rc = lib.b200rnn_cell_forward(ctypes.byref(desc), x.data_ptr(), x.stride(0), ptr(h), ld(h), ptr(c), ld(c),
+                                      params, h_out.data_ptr(), ptr(c_out), saved.data_ptr() if save else None,
+                                      _stream_ptr(dev))
+    _lib.check(rc, "b200rnn_cell_forward")
+    return h_out, c_out, saved
+
+
+def _cell_grad_buffers(x, cfg: CellConfig, h, c, need_dx: bool, need_dh: bool, need_dc: bool):
+    """``(dx, dh, dc)`` of a cell backward, None where not wanted"""
+    B, I, H, dev = x.size(0), cfg.input_size, cfg.hidden_size, x.device
+    new = lambda n: torch.empty(B, n, dtype=torch.float32, device=dev)  # noqa: E731
+    dx = new(I) if need_dx else None
+    dh = new(H) if h is not None and need_dh else None
+    dc = new(H) if c is not None and need_dc else None
+    return dx, dh, dc
+
+
+def _cell_backward_impl(cfg: CellConfig, x, h, c, saved, weights, dh_out, dc_out, need_dx: bool, need_dh: bool,
+                        need_dc: bool, need_w, separate: bool = False):
+    """one ``b200rnn_cell_backward`` call, shared by :class:`_CellFunction` and the ``b200rnn::cell_backward`` op:
+    returns ``(dx, dh, dc, weight grads)``, None for every gradient that is not wanted"""
+    lib = _lib.load()
+    B, dev = x.size(0), x.device
+    dx, dh, dc = _cell_grad_buffers(x, cfg, h, c, need_dx, need_dh, need_dc)
+    dptrs, grads_out, _ = _weight_grad_targets(weights, need_w, None, dev, separate)
+    desc = _cell_desc(cfg, B, True)
+    _, sbytes = _lib.cell_workspace_bytes(desc)
+    scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+    dh_out = dh_out.contiguous() if dh_out is not None else None
+    dc_out = dc_out.contiguous() if dc_out is not None else None
+    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    ld = lambda t: t.stride(0) if t is not None else 0  # noqa: E731
+    params = _lib.ptr_array([w.data_ptr() for w in weights] + [None] * (4 - len(weights)))
+    dparams = _lib.ptr_array(dptrs + [None] * (4 - len(dptrs)))
+    with _on(dev):
+        rc = lib.b200rnn_cell_backward(ctypes.byref(desc), x.data_ptr(), x.stride(0), ptr(h), ld(h), ptr(c), ld(c),
+                                       params, ptr(dh_out), ptr(dc_out), saved.data_ptr(), ptr(dx), ptr(dh),
+                                       ptr(dc), dparams, scratch.data_ptr(), _stream_ptr(dev))
+    _lib.check(rc, "b200rnn_cell_backward")
+    return dx, dh, dc, grads_out
+
+
 class _CellFunction(torch.autograd.Function):
     """h' (GRU) or (h', c') (LSTM) = cell(x, h, c, weights) for x [B, I]; h / c are None (zeros) or [B, H]. The TF32
     mode is in ``cfg``, read once per call, and the backward reuses it."""
@@ -508,23 +630,9 @@ class _CellFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x: torch.Tensor, cfg: CellConfig, save: bool, h: Optional[torch.Tensor],
                 c: Optional[torch.Tensor], *weights: torch.Tensor):
-        lib = _lib.load()
-        B, H, dev = x.size(0), cfg.hidden_size, x.device
         # as in _RNNFunction: the caller decides from grad mode, needs_input_grad confirms
         save = bool(save) and any(ctx.needs_input_grad)
-        desc = _cell_desc(cfg, B, save)
-        sv_bytes, _ = _lib.cell_workspace_bytes(desc)
-        saved = torch.empty(sv_bytes if save else 0, dtype=torch.uint8, device=dev)
-        h_out = torch.empty(B, H, dtype=torch.float32, device=dev)
-        c_out = torch.empty(B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
-        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-        ld = lambda t: t.stride(0) if t is not None else 0  # noqa: E731
-        params = _lib.ptr_array([w.data_ptr() for w in weights] + [None] * (4 - len(weights)))
-        with _on(dev):
-            rc = lib.b200rnn_cell_forward(ctypes.byref(desc), x.data_ptr(), x.stride(0), ptr(h), ld(h), ptr(c), ld(c),
-                                          params, h_out.data_ptr(), ptr(c_out), saved.data_ptr() if save else None,
-                                          _stream_ptr(dev))
-        _lib.check(rc, "b200rnn_cell_forward")
+        h_out, c_out, saved = _cell_forward_impl(x, cfg, save, h, c, weights)
         if save:
             ctx.cfg = cfg
             ctx.save_for_backward(x, h, c, saved, *weights)
@@ -532,31 +640,11 @@ class _CellFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dh_out, dc_out=None):
-        lib = _lib.load()
-        cfg: CellConfig = ctx.cfg
         x, h, c, saved, *weights = ctx.saved_tensors
-        B, I, H, dev = x.size(0), cfg.input_size, cfg.hidden_size, x.device
         need = ctx.needs_input_grad
         w0 = _CellFunction._W0
-        new = lambda n: torch.empty(B, n, dtype=torch.float32, device=dev)  # noqa: E731
-        dx = new(I) if need[0] else None
-        dh = new(H) if h is not None and need[w0 - 2] else None
-        dc = new(H) if c is not None and need[w0 - 1] else None
-        dptrs, grads_out, _ = _weight_grad_targets(weights, need[w0:], None, dev)
-        desc = _cell_desc(cfg, B, True)
-        _, sbytes = _lib.cell_workspace_bytes(desc)
-        scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
-        dh_out = dh_out.contiguous() if dh_out is not None else None
-        dc_out = dc_out.contiguous() if dc_out is not None else None
-        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-        ld = lambda t: t.stride(0) if t is not None else 0  # noqa: E731
-        params = _lib.ptr_array([w.data_ptr() for w in weights] + [None] * (4 - len(weights)))
-        dparams = _lib.ptr_array(dptrs + [None] * (4 - len(dptrs)))
-        with _on(dev):
-            rc = lib.b200rnn_cell_backward(ctypes.byref(desc), x.data_ptr(), x.stride(0), ptr(h), ld(h), ptr(c), ld(c),
-                                           params, ptr(dh_out), ptr(dc_out), saved.data_ptr(), ptr(dx), ptr(dh),
-                                           ptr(dc), dparams, scratch.data_ptr(), _stream_ptr(dev))
-        _lib.check(rc, "b200rnn_cell_backward")
+        dx, dh, dc, grads_out = _cell_backward_impl(ctx.cfg, x, h, c, saved, weights, dh_out, dc_out, need[0],
+                                                    need[w0 - 2], need[w0 - 1], need[w0:])
         return (dx, None, None, dh, dc, *grads_out)
 
 
@@ -598,6 +686,8 @@ def cell_forward(x: torch.Tensor, hx, weights: Sequence[torch.Tensor], cfg: Cell
     states = tuple(_cell_rows(s) for s in states)
     h, c = (states + (None, None))[:2]
     save = torch.is_grad_enabled() and (x.requires_grad or any(t.requires_grad for t in (*weights, *states)))
+    if torch.compiler.is_compiling():
+        return _ops.cell_forward_traced(x, cfg, save, h, c, weights)
     return _CellFunction.apply(x, cfg, save, h, c, *weights)
 
 
@@ -630,3 +720,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_kcontig: bool = True, b_kcontig:
                                   scratch.data_ptr() if scratch is not None else None, sbytes, _stream_ptr(a.device))
     _lib.check(rc, "b200rnn_gemm_f32")
     return out
+
+
+# the custom ops (b200rnn/ops.py) wrap the helpers above; imported last because they import this module
+from . import ops as _ops  # noqa: E402

@@ -102,11 +102,12 @@ class _AttentionPoolFunction(torch.autograd.Function):
 def attention_pool_tm(attention_layer: torch.nn.Module, seq_tm: torch.Tensor, h_n: torch.Tensor) -> torch.Tensor:
     """``attention_net_with_w`` (text_bilstm_whole.py:74-99) on the TIME-MAJOR LSTM output ``seq_tm`` [T,B,2H] and
     ``h_n`` [L*D,B,H] -> [B,H]; differentiable (one kernel each way). Falls back to the PyTorch expression only for
-    shapes the kernels do not take (T*H beyond one CTA's shared memory) or non-CUDA tensors of the oracle tests."""
+    shapes the kernels do not take (T*H beyond one CTA's shared memory), non-CUDA tensors of the oracle tests, and under
+    torch.compile / torch.export, which have no custom op for these kernels."""
     lin = attention_layer[0]
     T, B, H2 = seq_tm.shape
     fits = (4 * (H2 // 2) + 2 * T + T * (H2 // 2)) * 4 <= 200 * 1024 and (2 * (H2 // 2) + T) * 4 <= 47 * 1024
-    if seq_tm.is_cuda and fits and seq_tm.dtype == torch.float32:
+    if seq_tm.is_cuda and fits and seq_tm.dtype == torch.float32 and not torch.compiler.is_compiling():
         return _AttentionPoolFunction.apply(seq_tm, h_n, lin.weight, lin.bias)
     from .models import attention_pool as _generic
 

@@ -173,6 +173,8 @@ class _B200RNNBase(nn.Module):
         fuse_net_whole.py:590-593) - nothing this library launches updates such a tensor behind PyTorch's back. The
         cache is keyed on the parameters' storage addresses and version counters, so ``load_state_dict``, ``.to()`` or
         an in-place edit refresh it; trainable modules never use it (their weights change every step anyway)."""
+        if torch.compiler.is_compiling():
+            return None   # keyed on storage addresses and version counters, which a traced graph does not have
         ws = self._flat_weights
         if (any(w.requires_grad for w in ws) or not ws[0].is_cuda or self.proj_size or self._gates == 1 or
                 ws[0].dtype != torch.float32):
@@ -260,8 +262,9 @@ class _B200RNNBase(nn.Module):
         """
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
-        shape_ok = (input.is_cuda and input.dim() == 3 and self.proj_size == 0 and self._gates > 1 and
-                    self._flat_weights[0].dtype == torch.float32 and
+        # torch.compile / torch.export trace the unfused expression through the custom ops (b200rnn/ops.py)
+        shape_ok = (not torch.compiler.is_compiling() and input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
+                    self._gates > 1 and self._flat_weights[0].dtype == torch.float32 and
                     self.hidden_size in (128, 256) and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and
                                     ln.bias is not None)))
