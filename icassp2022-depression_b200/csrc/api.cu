@@ -698,7 +698,9 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
   }
 
   const bool tc = tc_available();
-  const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0;  // single-pass TF32 GEMMs and tc8 recurrence
+  // single-pass TF32 GEMMs and tc8 recurrence; fp32 calls only: 16-bit modules keep their numerics whatever torch's fp32
+  // matmul precision says, as cuDNN's 16-bit RNNs do
+  const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0 && !dt;
   int sms = NUM_SMS;
   {
     int dev = 0;
@@ -1344,7 +1346,8 @@ static int backward_h16(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
   const void* whh16[8 * 2];
   for (int i = 0; i < d.L * d.D; ++i) whh16[i] = params[(size_t)i * 4 + 1];
   b200rnn_desc d32 = *desc;
-  d32.flags &= ~(B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_ACCUMULATE_GRADS);
+  // TF32 applies to fp32 calls only (forward_impl): the fp32 backward of a 16-bit call runs its 3xTF32 GEMMs
+  d32.flags &= ~(B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_ACCUMULATE_GRADS | B200RNN_FLAG_TF32);
   rc = backward_impl(&d32, S + hs.x32, (int64_t)d.B * d.I, d.I, p32, R + rl.ytop, (int64_t)d.B * DH, DH, S + hs.dy32,
                      (int64_t)d.B * DH, DH, nullptr, 0.f, w[0], w[1], reserve, scratch, dx ? S + hs.dx32 : nullptr,
                      (int64_t)d.B * d.I, d.I, dp32, lengths, nullptr, 0.f, nullptr, nullptr, w[2], w[3],

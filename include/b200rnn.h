@@ -66,7 +66,8 @@ enum {
                                              issue one MMA per product; every other kernel stays fp32. Honoured by
                                              forward / forward_fused / backward / backward_fused (set it identically for
                                              a forward and its backward); workspace_bytes and prepare_weights accept it.
-                                             b200rnn_gemm_f32 is always 3xTF32. */
+                                             b200rnn_gemm_f32 is always 3xTF32. Ignored with B200RNN_FLAG_F16 / _BF16:
+                                             16-bit calls compute as they do without it. */
 #define B200RNN_FLAG_F16 64u              /* 16-bit tensors (torch.float16 modules): x, every parameter, h_0 / c_0, y, h_n /
                                              c_n, dy, dh_n / dc_n and every gradient output of b200rnn_forward(_hx) /
                                              b200rnn_backward(_hx) are IEEE fp16 (the pointers keep their float types).

@@ -187,6 +187,17 @@ def lstm_step(x, h, c, w_ih, w_hh, b_ih, b_hh, w_hr=None):
     return m @ w_hr.T, c_new, 1.0 + S_c @ np.abs(w_hr).T, S_c
 
 
+def elman_step(x, h, w_ih, w_hh, b_ih, b_hh, nonlinearity="tanh"):
+    """x [B,I], h [B,H] -> (h' [B,H], S [B,H]); h' = act(W_ih x + b_ih + W_hh h + b_hh) (torch.nn.RNN,
+    rnn.py:496-505). relu is exact, so its S has no activation term: S is the magnitude of the pre-activation's terms."""
+    x, h, w_ih, w_hh, b_ih, b_hh = _f64(x, h, w_ih, w_hh, b_ih, b_hh)
+    a = x @ w_ih.T + b_ih + h @ w_hh.T + b_hh
+    mag = np.abs(x) @ np.abs(w_ih).T + np.abs(h) @ np.abs(w_hh).T + np.abs(b_ih) + np.abs(b_hh)
+    if nonlinearity == "relu":
+        return np.maximum(a, 0.0), mag
+    return np.tanh(a), 1.0 + mag
+
+
 class NumpyRNN:
     """Multi-layer (bi)directional GRU/LSTM, time-major [T,B,*], with an explicit backward."""
 

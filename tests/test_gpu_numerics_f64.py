@@ -73,6 +73,7 @@ CONFIGS = {
     "bilstmp_h128_p64": ("lstm", 256, 128, 16, True, 64, "fp32"),
     "bilstmp_h256_p64": ("lstm", 256, 256, 16, True, 64, "fp32"),
     "bilstmp_h256_p128": ("lstm", 256, 256, 16, True, 128, "fp32"),
+    "bilstm128_tcl8_f16pair": ("lstm", 256, 128, 128, True, 0, "f16"),
 }
 # the config line each entry must run (B200RNN_DEBUG), forward and backward
 FWD_LINE = {
@@ -91,6 +92,7 @@ FWD_LINE = {
     "bilstmp_h128_p64": "fwd proj cfg C=2 BS=4 P=64",
     "bilstmp_h256_p64": "fwd proj cfg C=4 BS=8 P=64",
     "bilstmp_h256_p128": "fwd proj cfg C=4 BS=8 P=128",
+    "bilstm128_tcl8_f16pair": "fwd cfg tcl8 C=2 BS=8 mma.sync f16x3",
 }
 BWD_LINE = {
     "gru256_bs2": "bwd cfg C=4 BS=2 KL=16 UPL=8 RG=0",
@@ -108,8 +110,9 @@ BWD_LINE = {
     "bilstmp_h256_p64": "bwd proj cfg C=4 BS=8 P=64",
     "bilstmp_h256_p128": "bwd proj cfg C=4 BS=8 P=128",
 }
-# plan_rec_fwd: 5 GRU-256 contractions, 2 GRU-128, 2 LSTM-256, 2 LSTM-128, 4 projected; plan_rec_bwd: 3 + 2 + 2 + 2 + 4
-N_FWD_ENTRIES, N_BWD_ENTRIES = 15, 13
+# plan_rec_fwd: 5 GRU-256 contractions, 2 GRU-128, 2 LSTM-256, 3 LSTM-128 (FFMA narrow and wide, fp16-pair tcl8),
+# 4 projected; plan_rec_bwd: 3 + 2 + 2 + 2 + 4
+N_FWD_ENTRIES, N_BWD_ENTRIES = 16, 13
 REGIMES = ("default", "saturated", "large_input", "small_signal")
 
 
@@ -198,7 +201,8 @@ def _per_step(name, regime, ragged, T):
 
     kind, I, H, B, bi, P, mode = _shape(name, regime)
     if mode == "f16" and ragged:
-        pytest.skip("the fp16-pair forward is the no-grad fused entry; its ragged form runs in test_gpu_h16_fwd.py")
+        pytest.skip("the fp16-pair forward is the no-grad fused entry; its ragged form runs in test_gpu_h16_fwd.py and "
+                    "test_gpu_lstm_h16_fwd.py")
     ref = _torch_model(kind, I, H, bi, P, regime)
     mine = from_torch(ref).to(DEV)
     x = _input(regime, T, B, I)
@@ -218,6 +222,24 @@ def _per_step(name, regime, ragged, T):
             worst = max(worst, (err / (KAPPA * u * S[live])).max(initial=0.0))
             assert (y[t][~live] == 0).all(), (name, t)
             h_prev = np.where(live[:, None], y[t], h_prev)
+    elif mode == "f16":   # the no-grad fused entry takes no initial state: each step's state from a prefix run
+        # (forward direction: x[:t]) and a suffix run (reverse direction: x[T-t:]), whose outputs must be bitwise the
+        # full run's
+        y_full = _forward(mine, mode, x.to(DEV))[0].cpu()
+        ws = [_f64_weights(ref, d) for d in range(D)]
+        prev = [(np.zeros((B, H)), np.zeros((B, H))) for _ in range(D)]
+        for t in range(1, T + 1):
+            runs = [_forward(mine, mode, x[:t].to(DEV))] + ([_forward(mine, mode, x[T - t:].to(DEV))] if bi else [])
+            assert torch.equal(runs[0][0].cpu()[:, :, :H], y_full[:t, :, :H]), (name, t)
+            if bi:
+                assert torch.equal(runs[1][0].cpu()[:, :, H:], y_full[T - t:, :, H:]), (name, t)
+            for d in range(D):
+                hn, cn = (a[d].cpu().double().numpy() for a in runs[d][1:3])
+                hp, cp = prev[d]
+                h64, c64, S_h, S_c = lstm_step(x64[t - 1] if d == 0 else x64[T - t], hp, cp, *ws[d][:4])
+                for got, want, S in ((hn, h64, S_h), (cn, c64, S_c)):
+                    worst = max(worst, (np.abs(got - want) / (KAPPA * u * S)).max())
+                prev[d] = (hn, cn)
     else:   # LSTM / LSTMP: chained one-step calls through hx, which return the cell state as well
         h = torch.zeros(D, B, HO, device=DEV)
         c = torch.zeros(D, B, H, device=DEV)

@@ -34,6 +34,8 @@ GEMM_EXISTING = ["tests/test_gpu_gemm.py", "tests/test_gpu_gemm_f32a.py", "tests
 SHELL_NEW = ["tests/test_gpu_shell_f64.py"]
 SHELL_EXISTING = ["tests/test_gpu_head.py", "tests/test_gpu_train_step.py", "tests/test_gpu_fuse_parity.py",
                   "tests/test_gpu_models.py"]
+H16_NEW = ["tests/test_gpu_h16_numerics_f64.py"]
+H16_EXISTING = ["tests/test_gpu_h16_modules.py"]
 
 # name -> (file under csrc/, text, replacement, what it breaks, new tests, existing tests)
 MUTATIONS = {
@@ -107,6 +109,23 @@ MUTATIONS = {
                                  "  return 1.f - powf(beta, t);",
                                  "Adam: the cancelling 1 - powf(beta, t) of the previous code", SHELL_NEW,
                                  SHELL_EXISTING),
+    "h16_narrow_toward_zero": ("h16.cu", "__half_as_ushort(__float2half_rn(v))", "__half_as_ushort(__float2half_rz(v))",
+                               "16-bit outputs: fp16 narrowing rounds toward zero instead of to nearest", H16_NEW,
+                               H16_EXISTING),
+    "h16_bwd_skip_valid_rows": ("api.cu", "    } else if (l == 0 && lengths) {  // x with its padding zeroed",
+                                "    } else if (l == 0 && lengths && !layer_in) {  // x with its padding zeroed",
+                                "16-bit backward: dW_ih reads the caller's padded rows of x (0 * NaN)", H16_NEW,
+                                H16_EXISTING),
+    "h16_widen_bf16_flush_subnormals": ("h16.cu", "return dt == DT_BF16 ? __uint_as_float((uint32_t)v << 16)",
+                                        "return dt == DT_BF16 ? ((v & 0x7f80u) ? __uint_as_float((uint32_t)v << 16) : 0.f)",
+                                        "bf16 widening flushes subnormals to zero", H16_NEW, H16_EXISTING),
+    "h16_accumulate_two_roundings": ("h16.cu", "      if (accumulate) v += widen(d[c], dt);\n",
+                                     "      if (accumulate) v = widen(narrow(v, dt), dt) + widen(d[c], dt);\n",
+                                     "ACCUMULATE_GRADS, row path: the gradient is rounded before it is added",
+                                     H16_NEW, H16_EXISTING),
+    "tcl8_drop_al_bh": ("rnn_rec.cu", "            ptx::mma_f16_m16n8k16(d[g][0], al, bh);\n", "",
+                        "fp16-pair tc8 / tcl8 recurrence: the lo(W) * hi(h) correction mma is lost", REC_NEW,
+                        ["tests/test_gpu_lstm_h16_fwd.py"]),
 }
 
 
