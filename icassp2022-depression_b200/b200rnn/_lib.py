@@ -124,6 +124,7 @@ class FuseHeadArgs(ctypes.Structure):
         ("adam_m", c_void_p), ("adam_v", c_void_p), ("adam_step", c_void_p),
         ("comm_step", c_void_p), ("comm_done", c_void_p),
         ("comm_buf", c_void_p * 8),
+        ("halves", c_void_p),
     ]
 
     def __init__(self, **kw):

@@ -139,6 +139,10 @@ class FusedFuseStep:
     output, the two-head loss, ``d fc_final.0.weight``, the data-parallel gradient sum and the Adam update - is ONE
     launch of ``b200rnn_fuse_head``. Both flavours are covered: the 2-class classification ``fusion_net`` (Softmax
     output, cross entropy) and the regression one (sigmoid ``modal_attn`` gate + ReLU output, SmoothL1, one output).
+    With ``concurrent_branches`` the text half of that launch runs on the text stream before the join; for the
+    classification flavour (``split_loss``, every exchange but "peer_async") the audio half also runs before the join,
+    on the audio stream, and each half emits its logit halves, so that after the join one single-CTA launch is left:
+    loss, gradient, exchange and Adam. Logits, loss and update are bit-identical either way.
 
     Data parallel (``torch.distributed`` initialised, world > 1): ``exchange="peer"`` (default when CUDA IPC peer
     mapping works) sums the 3 KB gradient inside the same kernel through peer-mapped buffers over NVLink
@@ -218,6 +222,11 @@ class FusedFuseStep:
                     if self.comm is not None:
                         self.comm.close()
                     self.comm, self.exchange = None, "nccl"
+        # Classification with the split head: each branch launch also writes its halves of the row logits (which read
+        # fc_final.0.weight, so not under "peer_async", where the previous update lands on another stream), and after
+        # the join only the single-CTA loss launch remains.
+        self.split_loss = self.split_head and not self.regression and self.exchange != "peer_async"
+        self._halves = None
 
     def _finish_args(self) -> "_lib.FuseHeadArgs":
         m = self.model
@@ -259,7 +268,7 @@ class FusedFuseStep:
         m = self.model
         return m.lstm_net_audio.forward_ln_sum(batch.audio, None if self.regression else m.ln, prologue_done)
 
-    def _encoders(self, batch: FuseBatch, text_stage=None):
+    def _encoders(self, batch: FuseBatch, text_stage=None, audio_stage=None):
         """The two independent encoder branches (fuse_net_whole.py:347 text BiLSTM, :361 audio GRU). With
         ``concurrent_branches`` the audio branch - the critical path, 2 x 120 serial steps - is enqueued on a second,
         high-priority stream (fork / join by events, captured as parallel branches of the CUDA graph): its persistent
@@ -268,7 +277,8 @@ class FusedFuseStep:
         text GEMM CTAs that are pending while the LayerNorm runs take the SMs it frees and hold them for tens of µs,
         so the audio GEMM and recurrence would start late. Gated, the audio kernels become pending no later than the
         text ones, at higher priority. ``text_stage(seq, h_n)`` (the text half of the head kernel) runs on the text
-        stream before the join, i.e. off the critical path."""
+        stream before the join, i.e. off the critical path; ``audio_stage(pooled)`` (the audio half) runs on the audio
+        stream right behind the recurrence."""
         dev = batch.text.device
         if not self.concurrent_branches:
             seq, h_n = self._text_branch(batch)
@@ -281,6 +291,8 @@ class FusedFuseStep:
         self._side.wait_stream(main)
         with torch.cuda.stream(self._side):
             pooled = self._audio_branch(batch, self._prologue_done)
+            if audio_stage is not None:
+                audio_stage(pooled)
         main.wait_event(self._prologue_done)
         seq, h_n = self._text_branch(batch)
         extra = text_stage(seq, h_n) if text_stage is not None else None
@@ -348,16 +360,6 @@ class FusedFuseStep:
             with torch.cuda.stream(self._aux), _on(dev):
                 _lib.check(lib.b200rnn_fuse_head_finish(ctypes.byref(fa), _stream(dev)), "b200rnn_fuse_head_finish")
 
-        def text_stage(seq, h_n):
-            # the text half of the head (attention pooling + fc_out) on the text branch's stream, while the audio
-            # recurrence is still running; reads the same {seed, offset} the final launch will read and then advance
-            a0 = self._args(seq, h_n, None, tf, None)
-            a0.rng_state = self.rng_state.data_ptr()
-            with _on(dev):
-                _lib.check(lib.b200rnn_fuse_head(ctypes.byref(a0), _stream(dev)), "b200rnn_fuse_head (text stage)")
-            return True
-
-        seq, h_n, pooled, _ = self._encoders(batch, text_stage if self.split_head else None)
         # the kernel reads `const int64_t labels[B]` (classification) / `const float labels[B]` (regression): anything
         # else (int32 from numpy, a strided view) would be silently misread, so it is converted here; class indices
         # outside {0,1} poison the loss with NaN on the device
@@ -372,7 +374,37 @@ class FusedFuseStep:
                                                         int(self.regression)))
         if self._dw_part is None or self._dw_part.numel() < need:
             self._dw_part = torch.empty(need, device=dev)
-        a = self._args(seq, h_n, pooled, tf, af, tf_in=tf if self.split_head else None)
+        if self.split_loss and (self._halves is None or self._halves.numel() < 4 * B):
+            self._halves = torch.empty(4 * B, device=dev)
+
+        def stage(a0, what):
+            # a branch's half of the head on that branch's stream; reads the same {seed, offset} the final launch
+            # will read and then advance
+            a0.rng_state = self.rng_state.data_ptr()
+            if self.split_loss:
+                a0.W, a0.halves, a0.dw_part = self.w.data_ptr(), self._halves.data_ptr(), self._dw_part.data_ptr()
+            with _on(dev):
+                _lib.check(lib.b200rnn_fuse_head(ctypes.byref(a0), _stream(dev)), f"b200rnn_fuse_head ({what} stage)")
+
+        def text_stage(seq, h_n):
+            # attention pooling + fc_out on the text branch's stream, while the audio recurrence is still running
+            stage(self._args(seq, h_n, None, tf, None), "text")
+            return True
+
+        def audio_stage(pooled):
+            # fc_audio on the audio stream right behind the recurrence, before the join
+            a0 = _lib.FuseHeadArgs(B=B, Ht=m.text_hidden_dims, Ha=m.audio_hidden_dims, training=int(m.training),
+                                   p=float(m.dropout), pooled=pooled.data_ptr(), w_a=m.fc_audio[1].weight.data_ptr(),
+                                   b_a=m.fc_audio[1].bias.data_ptr(), audio_feature=af.data_ptr())
+            stage(a0, "audio")
+
+        seq, h_n, pooled, _ = self._encoders(batch, text_stage if self.split_head else None,
+                                             audio_stage if self.split_loss else None)
+        if self.split_loss:   # both halves are done: loss, dW, exchange and Adam only
+            a = _lib.FuseHeadArgs(B=B, Ht=m.text_hidden_dims, Ha=m.audio_hidden_dims, training=int(m.training),
+                                  p=float(m.dropout), halves=self._halves.data_ptr())
+        else:
+            a = self._args(seq, h_n, pooled, tf, af, tf_in=tf if self.split_head else None)
         a.W = self.w.data_ptr()
         a.w_modal = m.modal_attn.weight.data_ptr() if self.regression else None
         a.labels = labels.data_ptr()

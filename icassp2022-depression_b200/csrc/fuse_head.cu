@@ -8,6 +8,11 @@
 //   [data parallel] sum of that gradient over the ranks: one-shot NVLink exchange, peer stores + flags (below)
 //   torch.optim.Adam step on fc_final.0.weight                                          :416, 456
 //
+// Split head (classification, args.halves): the text launch also writes each row's text logit halves and text feature
+// columns, an audio launch on the audio stream right after the GRU does the same for the audio half, and only the loss,
+// dW, the exchange and Adam are left for one single-CTA launch after the join (fuse_loss_kernel). Every sum keeps its
+// order, so the split step computes bit-identical logits, loss and update.
+//
 // As separate kernels this is 7 launches (attention_pool, rng_next, 2x mlp_dropout, fuse_loss_grad, adam, adam_step)
 // plus a 3 KB ncclAllReduce and a 1/world scaling launch between the loss and Adam, all latency-bound. Here a CTA owns
 // ROWS batch rows from the LSTM output to its rows' loss and gradient contribution; the last CTA to finish (ticket counter) reduces the
@@ -31,6 +36,7 @@ namespace {
 
 constexpr int HEAD_THREADS = 256;
 constexpr int HEAD_ROWS = 1;        // batch rows per CTA: B CTAs, the chip is covered at B = 128 (latency-bound work)
+constexpr int LOSS_THREADS = 512;   // split head, loss launch: one thread per dW column up to F = 512
 constexpr int ROWSTAT = 8;          // floats per batch row handed to the last CTA: dt[2], da[2], row loss (padded)
 constexpr int COMM_MAX_WORLD = B200RNN_COMM_MAX_WORLD;
 constexpr int COMM_PAYLOAD = 1024;  // floats per slot (fc_final.0.weight is 2 x 384 = 768; + loss)
@@ -113,11 +119,36 @@ __device__ __forceinline__ void matvec_rows(const float* __restrict__ W, const f
   }
 }
 
+// two-head cross entropy of one row from its logit halves pt (text) and pa (audio): d loss / d logits and the row loss
+__device__ __forceinline__ float ce_row(const float pt[2], const float pa[2], long long y, float invB, float dt[2],
+                                        float da[2]) {
+  float lrow = 0.f;
+  float m = fmaxf(pt[0], pt[1]), e0 = expf(pt[0] - m), e1 = expf(pt[1] - m), z = e0 + e1;
+  lrow += (m + logf(z)) - (y == 0 ? pt[0] : pt[1]);
+  dt[0] = (e0 / z - (y == 0 ? 1.f : 0.f)) * invB;
+  dt[1] = (e1 / z - (y == 1 ? 1.f : 0.f)) * invB;
+  m = fmaxf(pa[0], pa[1]); e0 = expf(pa[0] - m); e1 = expf(pa[1] - m); z = e0 + e1;
+  lrow += (m + logf(z)) - (y == 0 ? pa[0] : pa[1]);
+  da[0] = (e0 / z - (y == 0 ? 1.f : 0.f)) * invB;
+  da[1] = (e1 / z - (y == 1 ? 1.f : 0.f)) * invB;
+  if (y != 0 && y != 1) lrow = __int_as_float(0x7fc00000);  // a label outside {0,1} poisons the loss (NaN)
+  return lrow;
+}
+
+// Softmax(fc_final(concat)) of one row - accuracy only in the reference
+__device__ __forceinline__ void softmax_row(const float pt[2], const float pa[2], float* out_row) {
+  const float l0 = pt[0] + pa[0], l1 = pt[1] + pa[1], mm = fmaxf(l0, l1);
+  const float x0 = expf(l0 - mm), x1 = expf(l1 - mm);
+  out_row[0] = x0 / (x0 + x1);
+  out_row[1] = x1 / (x0 + x1);
+}
+
 // ---- one-shot peer exchange, two halves (see the file header) -------------------------------------------------------
 // send: g[0..n) -> slot [parity][rank] of every rank's buffer, then the step tag into flag [parity][rank] there
-__device__ __forceinline__ void peer_send(const b200rnn_fuse_head_args& a, const float* g, int n, uint32_t step, int tid) {
+__device__ __forceinline__ void peer_send(const b200rnn_fuse_head_args& a, const float* g, int n, uint32_t step, int tid,
+                                          int nt) {
   const uint32_t par = step & 1u, tag = step + 1u;
-  for (int idx = tid; idx < a.world * n; idx += HEAD_THREADS) {
+  for (int idx = tid; idx < a.world * n; idx += nt) {
     const int dst = idx / n, i = idx - dst * n;
     float* slot = reinterpret_cast<float*>(static_cast<unsigned char*>(a.comm_buf[dst]) + COMM_DATA_OFF) +
                   ((size_t)par * COMM_MAX_WORLD + a.rank) * COMM_PAYLOAD;
@@ -132,7 +163,8 @@ __device__ __forceinline__ void peer_send(const b200rnn_fuse_head_args& a, const
   }
 }
 // wait for every peer's slot of `step`, then out[i] = sum over ranks in rank order (identical on every rank)
-__device__ __forceinline__ void peer_wait_sum(const b200rnn_fuse_head_args& a, float* out, int n, uint32_t step, int tid) {
+__device__ __forceinline__ void peer_wait_sum(const b200rnn_fuse_head_args& a, float* out, int n, uint32_t step, int tid,
+                                              int nt) {
   const uint32_t par = step & 1u, tag = step + 1u;
   if (tid < a.world) {
     const uint32_t* mine = reinterpret_cast<const uint32_t*>(static_cast<unsigned char*>(a.comm_buf[a.rank]) + COMM_FLAG_OFF) +
@@ -145,7 +177,7 @@ __device__ __forceinline__ void peer_wait_sum(const b200rnn_fuse_head_args& a, f
   __syncthreads();
   const float* slots = reinterpret_cast<const float*>(static_cast<unsigned char*>(a.comm_buf[a.rank]) + COMM_DATA_OFF) +
                        (size_t)par * COMM_MAX_WORLD * COMM_PAYLOAD;
-  for (int i = tid; i < n; i += HEAD_THREADS) {
+  for (int i = tid; i < n; i += nt) {
     float s = 0.f;
     for (int r = 0; r < a.world; ++r) s += __ldcv(slots + (size_t)r * COMM_PAYLOAD + i);  // rank order on every rank
     out[i] = s;
@@ -160,7 +192,7 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_finish_kernel(const b2
   const int n = (a.regression ? 1 : 2) * (a.Ht + a.Ha);
   const uint32_t done = *a.comm_done, sent = *a.comm_step;
   if (done == sent) return;  // nothing pending (first step, or already flushed)
-  peer_wait_sum(a, g, n, done, tid);
+  peer_wait_sum(a, g, n, done, tid, HEAD_THREADS);
   const float t = *a.adam_step + 1.f;
   const AdamCoef c = adam_coef(t, a.lr, a.beta1, a.beta2, 0.f);
   for (int i = tid; i < n; i += HEAD_THREADS) {
@@ -174,6 +206,74 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_finish_kernel(const b2
   if (tid == 0) {
     *a.adam_step = t;
     *a.comm_done = done + 1u;
+  }
+}
+
+// Per-row scalars rst[B][ROWSTAT] (in shared memory) and the feature matrix feat_ws[B][F] -> dW (fixed batch order),
+// the loss (fixed order), the peer exchange, the Philox offset advance and Adam. Run by all NT threads of ONE CTA.
+template <int NT>
+__device__ __forceinline__ void loss_tail(const b200rnn_fuse_head_args& a, const float* rst, const float* feat_ws,
+                                          bool drop, uint64_t offset, int tid, int lane, int warp) {
+  const int Ht = a.Ht, F = a.Ht + a.Ha, B = a.B, C = a.regression ? 1 : 2;
+  for (int j = tid; j < F; j += NT) {
+    float g0 = 0.f, g1 = 0.f;
+    const int so = (j < Ht) ? 0 : 2;
+    int b = 0;
+    for (; b + 16 <= B; b += 16) {  // 16 independent coalesced loads in flight per thread, then the ordered adds
+      float fv[16];
+#pragma unroll
+      for (int u = 0; u < 16; ++u) fv[u] = __ldcg(feat_ws + (size_t)(b + u) * F + j);
+#pragma unroll
+      for (int u = 0; u < 16; ++u) {
+        g0 = fmaf(rst[(b + u) * ROWSTAT + so], fv[u], g0);
+        g1 = fmaf(rst[(b + u) * ROWSTAT + so + 1], fv[u], g1);
+      }
+    }
+    for (; b < B; ++b) {
+      const float fv = __ldcg(feat_ws + (size_t)b * F + j);
+      g0 = fmaf(rst[b * ROWSTAT + so], fv, g0);
+      g1 = fmaf(rst[b * ROWSTAT + so + 1], fv, g1);
+    }
+    a.dw[j] = a.accumulate ? a.dw[j] + g0 : g0;
+    if (C == 2) a.dw[F + j] = a.accumulate ? a.dw[F + j] + g1 : g1;
+  }
+  if (warp == 0) {  // loss = sum of the row losses, fixed order
+    float l = 0.f;
+    for (int b = lane; b < B; b += 32) l += rst[b * ROWSTAT + 4];
+    l = warp_sum(l);
+    if (lane == 0) a.dw[C * F] = l;
+  }
+  __syncthreads();
+  bool apply_update = true;
+  if (a.world > 1) {
+    const uint32_t step = *a.comm_step;  // device-resident: a captured graph advances it at every replay
+    const int NX = C * F;  // the loss stays local (each rank reports its own shard's loss, like the reference would)
+    peer_send(a, a.dw, NX, step, tid, NT);
+    if (a.defer_exchange) {
+      apply_update = false;  // b200rnn_fuse_head_finish waits, sums and applies Adam (next step, beside the encoders)
+    } else {
+      peer_wait_sum(a, a.dw, NX, step, tid, NT);
+    }
+    if (tid == 0) *a.comm_step = step + 1u;
+    __syncthreads();
+  }
+  if (tid == 0) {
+    *a.loss = a.dw[C * F];
+    *a.ticket = 0u;  // re-armed for the next launch (graph replay)
+    if (drop && a.rng_state) a.rng_state[1] = offset + a.rng_consume;
+  }
+  if (a.do_adam && apply_update) {  // torch.optim.Adam (no weight decay, no amsgrad); grad_scale = 1/world
+    const float t = *a.adam_step + 1.f;
+    const AdamCoef c = adam_coef(t, a.lr, a.beta1, a.beta2, 0.f);
+    for (int i = tid; i < C * F; i += NT) {
+      float w = a.W[i], mi = a.adam_m[i], vi = a.adam_v[i];
+      adam_update(w, mi, vi, a.dw[i] * a.grad_scale, a.beta1, a.beta2, a.eps, c);
+      a.adam_m[i] = mi;
+      a.adam_v[i] = vi;
+      a.W[i] = w;
+    }
+    __syncthreads();
+    if (tid == 0) *a.adam_step = t;
   }
 }
 
@@ -195,6 +295,15 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_kernel(const b200rnn_f
   __shared__ int s_last;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = HEAD_THREADS / 32;
   const int b0 = blockIdx.x * R;
+  const bool text = !a.tf_in && (a.seq || a.ctx_in);  // this launch computes the text half
+
+  // fc_audio.1.weight into L2 before the wait. The GRU before it never triggers its dependents early, so a programmatic
+  // launch only overlaps this with the GRU's last CTAs draining and its memory flush, not with its steps
+  if (a.pooled) {
+    const size_t line = (size_t)blockIdx.x * HEAD_THREADS + tid, lines = (size_t)Ha * Ha * sizeof(float) / 128;
+    if (line < lines) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.w_a + line * 32));
+  }
+  asm volatile("griddepcontrol.wait;" ::: "memory");  // no-op unless launched programmatically
 
   float* feat_ws = a.dw_part ? a.dw_part + (size_t)B * ROWSTAT : nullptr;  // [B][F] features for the gradient pass
   const bool drop = a.training && a.p > 0.f;
@@ -269,7 +378,7 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_kernel(const b200rnn_f
       }
       ctx[idx] = acc;
     }
-  } else {  // attention context given (features computed elsewhere)
+  } else if (a.ctx_in) {  // attention context given (features computed elsewhere)
     for (int idx = tid; idx < R * Ht; idx += HEAD_THREADS) {
       const int r = idx / Ht, j = idx - r * Ht, b = b0 + r;
       float v = (b < B) ? a.ctx_in[(size_t)b * Ht + j] : 0.f;
@@ -287,12 +396,12 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_kernel(const b200rnn_f
     }
   __syncthreads();
   // ---------------- the two Linear+ReLU heads, then their output Dropout ------------------------------------------
-  if (!a.tf_in) matvec_rows<R, true>(a.w_t, a.b_t, ctx, Ht, feat, F, Ht, Ht, warp, nw, lane);
+  if (text) matvec_rows<R, true>(a.w_t, a.b_t, ctx, Ht, feat, F, Ht, Ht, warp, nw, lane);
   if (a.pooled) matvec_rows<R, true>(a.w_a, a.b_a, xa, Ha, feat + Ht, F, Ha, Ha, warp, nw, lane);
   __syncthreads();
   for (int idx = tid; idx < R * F; idx += HEAD_THREADS) {
     const int r = idx / F, j = idx - r * F, b = b0 + r;
-    if ((j < Ht) ? (a.tf_in != nullptr) : (a.pooled == nullptr)) continue;  // half not produced by this launch
+    if ((j < Ht) ? !text : (a.pooled == nullptr)) continue;  // half not produced by this launch
     float v = feat[idx];
     if (b < B) {
       if (drop)
@@ -309,6 +418,31 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_kernel(const b200rnn_f
     feat[idx] = v;
   }
   __syncthreads();
+  if (a.halves) {  // split head: this half's logits and feature columns of the row; fuse_loss_kernel does the rest
+    if (warp < R && b0 + warp < B) {
+      const int r = warp, b = b0 + r;
+      const float* f = feat + r * F;
+      float h[2] = {0.f, 0.f};
+      for (int j = lane; j < F; j += 32) {  // the lane-strided chains of the whole-row loop below, one half of them
+        if ((j < Ht) != text) continue;
+        const float v = f[j];
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+          if (c < C) h[c] = fmaf(v, a.W[(size_t)c * F + j], h[c]);
+      }
+      h[0] = warp_sum(h[0]);
+      if (C == 2) h[1] = warp_sum(h[1]);
+      if (lane == 0) {
+        a.halves[(size_t)b * 4 + (text ? 0 : 2)] = h[0];
+        a.halves[(size_t)b * 4 + (text ? 1 : 3)] = h[1];
+      }
+    }
+    for (int idx = tid; idx < R * F; idx += HEAD_THREADS) {
+      const int r = idx / F, j = idx - r * F, b = b0 + r;
+      if (b < B && (j < Ht) == text) feat_ws[(size_t)b * F + j] = feat[idx];
+    }
+    return;
+  }
   if (!a.W) return;  // features only
 
   // ---------------- model output + two-head loss + per-row gradient contribution ---------------------------------
@@ -340,22 +474,8 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_kernel(const b200rnn_f
       if (C == 2) { pt[1] = warp_sum(pt[1]); pa[1] = warp_sum(pa[1]); }
       float dt[2] = {0.f, 0.f}, da[2] = {0.f, 0.f}, lrow = 0.f;
       if (!a.regression) {
-        const long long y = reinterpret_cast<const long long*>(a.labels)[b];
-        float m = fmaxf(pt[0], pt[1]), e0 = expf(pt[0] - m), e1 = expf(pt[1] - m), z = e0 + e1;
-        lrow += (m + logf(z)) - (y == 0 ? pt[0] : pt[1]);
-        dt[0] = (e0 / z - (y == 0 ? 1.f : 0.f)) * invB;
-        dt[1] = (e1 / z - (y == 1 ? 1.f : 0.f)) * invB;
-        m = fmaxf(pa[0], pa[1]); e0 = expf(pa[0] - m); e1 = expf(pa[1] - m); z = e0 + e1;
-        lrow += (m + logf(z)) - (y == 0 ? pa[0] : pa[1]);
-        da[0] = (e0 / z - (y == 0 ? 1.f : 0.f)) * invB;
-        da[1] = (e1 / z - (y == 1 ? 1.f : 0.f)) * invB;
-        if (y != 0 && y != 1) lrow = __int_as_float(0x7fc00000);  // a label outside {0,1} poisons the loss (NaN)
-        if (a.out && lane == 0) {  // Softmax(fc_final(concat)) - accuracy only in the reference
-          const float l0 = pt[0] + pa[0], l1 = pt[1] + pa[1], mm = fmaxf(l0, l1);
-          const float x0 = expf(l0 - mm), x1 = expf(l1 - mm);
-          a.out[(size_t)b * 2 + 0] = x0 / (x0 + x1);
-          a.out[(size_t)b * 2 + 1] = x1 / (x0 + x1);
-        }
+        lrow = ce_row(pt, pa, reinterpret_cast<const long long*>(a.labels)[b], invB, dt, da);
+        if (a.out && lane == 0) softmax_row(pt, pa, a.out + (size_t)b * 2);
       } else {  // SmoothL1 (beta = 1, mean over the B x 1 predictions), fuse_net.py:357-366
         const float y = reinterpret_cast<const float*>(a.labels)[b];
         float d = pt[0] - y;
@@ -394,66 +514,29 @@ __global__ void __launch_bounds__(HEAD_THREADS) fuse_head_kernel(const b200rnn_f
   float* rst = sm;  // [B][ROWSTAT] : B * 8 floats <= the R*(3Ht+2F+Ha+T) floats carved above? checked on the host
   for (int idx = tid; idx < B * ROWSTAT; idx += HEAD_THREADS) rst[idx] = __ldcg(a.dw_part + idx);
   __syncthreads();
-  for (int j = tid; j < F; j += HEAD_THREADS) {
-    float g0 = 0.f, g1 = 0.f;
-    const int so = (j < Ht) ? 0 : 2;
-    int b = 0;
-    for (; b + 16 <= B; b += 16) {  // 16 independent coalesced loads in flight per thread, then the ordered adds
-      float fv[16];
-#pragma unroll
-      for (int u = 0; u < 16; ++u) fv[u] = __ldcg(feat_ws + (size_t)(b + u) * F + j);
-#pragma unroll
-      for (int u = 0; u < 16; ++u) {
-        g0 = fmaf(rst[(b + u) * ROWSTAT + so], fv[u], g0);
-        g1 = fmaf(rst[(b + u) * ROWSTAT + so + 1], fv[u], g1);
-      }
-    }
-    for (; b < B; ++b) {
-      const float fv = __ldcg(feat_ws + (size_t)b * F + j);
-      g0 = fmaf(rst[b * ROWSTAT + so], fv, g0);
-      g1 = fmaf(rst[b * ROWSTAT + so + 1], fv, g1);
-    }
-    a.dw[j] = a.accumulate ? a.dw[j] + g0 : g0;
-    if (C == 2) a.dw[F + j] = a.accumulate ? a.dw[F + j] + g1 : g1;
-  }
-  if (warp == 0) {  // loss = sum of the row losses, fixed order
-    float l = 0.f;
-    for (int b = lane; b < B; b += 32) l += rst[b * ROWSTAT + 4];
-    l = warp_sum(l);
-    if (lane == 0) a.dw[C * F] = l;
+  loss_tail<HEAD_THREADS>(a, rst, feat_ws, drop, offset, tid, lane, warp);
+}
+
+// Split head, after the join: the loss of every row from the halves the two branch launches wrote, then loss_tail.
+// One CTA: one thread per row, then the same fixed-order reductions as the last CTA of fuse_head_kernel, with one
+// thread per dW column.
+__global__ void __launch_bounds__(LOSS_THREADS) fuse_loss_kernel(const b200rnn_fuse_head_args a) {
+  extern __shared__ __align__(16) float rst[];  // [B][ROWSTAT]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, B = a.B;
+  const float invB = 1.f / (float)B;
+  const bool drop = a.training && a.p > 0.f;
+  const uint64_t offset = drop ? a.rng_state[1] : 0;
+  for (int b = tid; b < B; b += LOSS_THREADS) {
+    const float4 h = __ldcg(reinterpret_cast<const float4*>(a.halves) + b);
+    const float pt[2] = {h.x, h.y}, pa[2] = {h.z, h.w};
+    float dt[2], da[2];
+    const float lrow = ce_row(pt, pa, reinterpret_cast<const long long*>(a.labels)[b], invB, dt, da);
+    if (a.out) softmax_row(pt, pa, a.out + (size_t)b * 2);
+    float* st = rst + b * ROWSTAT;
+    st[0] = dt[0]; st[1] = dt[1]; st[2] = da[0]; st[3] = da[1]; st[4] = lrow * invB;
   }
   __syncthreads();
-  bool apply_update = true;
-  if (a.world > 1) {
-    const uint32_t step = *a.comm_step;  // device-resident: a captured graph advances it at every replay
-    const int NX = C * F;  // the loss stays local (each rank reports its own shard's loss, like the reference would)
-    peer_send(a, a.dw, NX, step, tid);
-    if (a.defer_exchange) {
-      apply_update = false;  // b200rnn_fuse_head_finish waits, sums and applies Adam (next step, beside the encoders)
-    } else {
-      peer_wait_sum(a, a.dw, NX, step, tid);
-    }
-    if (tid == 0) *a.comm_step = step + 1u;
-    __syncthreads();
-  }
-  if (tid == 0) {
-    *a.loss = a.dw[C * F];
-    *a.ticket = 0u;  // re-armed for the next launch (graph replay)
-    if (drop && a.rng_state) a.rng_state[1] = offset + a.rng_consume;
-  }
-  if (a.do_adam && apply_update) {  // torch.optim.Adam (no weight decay, no amsgrad); grad_scale = 1/world
-    const float t = *a.adam_step + 1.f;
-    const AdamCoef c = adam_coef(t, a.lr, a.beta1, a.beta2, 0.f);
-    for (int i = tid; i < C * F; i += HEAD_THREADS) {
-      float w = a.W[i], mi = a.adam_m[i], vi = a.adam_v[i];
-      adam_update(w, mi, vi, a.dw[i] * a.grad_scale, a.beta1, a.beta2, a.eps, c);
-      a.adam_m[i] = mi;
-      a.adam_v[i] = vi;
-      a.W[i] = w;
-    }
-    __syncthreads();
-    if (tid == 0) *a.adam_step = t;
-  }
+  loss_tail<LOSS_THREADS>(a, rst, a.dw_part + (size_t)B * ROWSTAT, drop, offset, tid, lane, warp);
 }
 
 size_t head_smem_floats(int B, int Ht, int Ha, int T, bool loss_stage) {
@@ -487,9 +570,20 @@ B200RNN_API int b200rnn_fuse_head(const b200rnn_fuse_head_args* args, void* stre
     return B200RNN_ERR_UNSUPPORTED;
   }
   if (a.B == 0) return B200RNN_OK;
+  const bool text_in = a.tf_in || a.seq || a.ctx_in;
   const bool have_text = a.tf_in ? true
                          : (a.seq ? (a.h_n && a.w_att && a.b_att && a.T >= 1 && a.n_states >= 1) : (a.ctx_in != nullptr));
-  if (!have_text || (!a.tf_in && (!a.w_t || !a.b_t)) || (a.pooled && (!a.w_a || !a.b_a)) || (!a.pooled && a.W)) {
+  // split head: one branch per launch (its halves), or neither (the loss launch)
+  const bool loss_launch = a.halves && !text_in && !a.pooled;
+  if (a.halves && (a.regression || !a.W || !a.dw_part || (text_in && a.pooled) ||
+                   (reinterpret_cast<uintptr_t>(a.halves) & 15u))) {
+    set_error("fuse_head: halves: classification only, 16-byte aligned, needs W and dw_part, and one branch (or none) "
+              "per launch");
+    return B200RNN_ERR_INVALID;
+  }
+  const bool branch_ok = a.halves ? (loss_launch || a.pooled || (have_text && !a.tf_in)) : have_text;
+  if (!branch_ok || (text_in && !a.tf_in && (!a.w_t || !a.b_t)) || (a.pooled && (!a.w_a || !a.b_a)) ||
+      (!a.pooled && a.W && !a.halves)) {
     set_error("fuse_head: null pointer argument (or the loss stage without the audio stage)");
     return B200RNN_ERR_INVALID;
   }
@@ -497,7 +591,7 @@ B200RNN_API int b200rnn_fuse_head(const b200rnn_fuse_head_args* args, void* stre
     set_error("fuse_head: train-mode dropout needs rng_state");
     return B200RNN_ERR_INVALID;
   }
-  if (a.W) {
+  if (a.W && (!a.halves || loss_launch)) {
     if (!a.labels || !a.dw_part || !a.dw || !a.loss || !a.ticket) {
       set_error("fuse_head: loss stage needs labels, dw_part, dw, loss and ticket");
       return B200RNN_ERR_INVALID;
@@ -520,7 +614,25 @@ B200RNN_API int b200rnn_fuse_head(const b200rnn_fuse_head_args* args, void* stre
         }
     }
   }
-  const size_t smem = head_smem_floats(a.B, a.Ht, a.Ha, (a.seq && !a.tf_in) ? a.T : 0, a.W != nullptr) * sizeof(float);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (loss_launch) {
+    const size_t smem = (size_t)a.B * ROWSTAT * sizeof(float);
+    if (smem > 200 * 1024) {
+      set_error("fuse_head: batch too large for the single-CTA loss launch");
+      return B200RNN_ERR_UNSUPPORTED;
+    }
+    static bool loss_attr[MAX_DEVICES] = {false};
+    if (!loss_attr[current_device()]) {
+      B200_CUDA_CHECK(cudaFuncSetAttribute(fuse_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      loss_attr[current_device()] = true;
+    }
+    fuse_loss_kernel<<<1, LOSS_THREADS, smem, stream>>>(a);
+    B200_CUDA_CHECK(cudaGetLastError());
+    count_launch();
+    return B200RNN_OK;
+  }
+  const bool stage_only = a.halves || !a.W;
+  const size_t smem = head_smem_floats(a.B, a.Ht, a.Ha, (a.seq && !a.tf_in) ? a.T : 0, !stage_only) * sizeof(float);
   if (smem > 200 * 1024) {
     set_error("fuse_head: widths too large for one CTA");
     return B200RNN_ERR_UNSUPPORTED;
@@ -531,7 +643,23 @@ B200RNN_API int b200rnn_fuse_head(const b200rnn_fuse_head_args* args, void* stre
     attr[current_device()] = true;
   }
   const int grid = (a.B + HEAD_ROWS - 1) / HEAD_ROWS;
-  fuse_head_kernel<<<grid, HEAD_THREADS, smem, static_cast<cudaStream_t>(stream_)>>>(a);
+  if (a.halves && a.pooled) {
+    // the audio launch follows the GRU on its stream: launched programmatically, its CTAs start (and prefetch
+    // fc_audio.1.weight) as the recurrence's CTAs exit; griddepcontrol.wait holds every read of the GRU's output
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(HEAD_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr1[1];
+    attr1[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr1[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr1;
+    cfg.numAttrs = 1;
+    B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, fuse_head_kernel, a));
+  } else {
+    fuse_head_kernel<<<grid, HEAD_THREADS, smem, stream>>>(a);
+  }
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;

@@ -382,6 +382,7 @@ B200RNN_API int b200rnn_adamw(float* p, const float* g, float* m, float* v, floa
  *                            while the audio encoder is still busy, the final launch then takes tf_in
  *   W   != NULL            : output + loss + gradient (+ exchange when world > 1) (+ Adam when do_adam); W == NULL
  *                            stops after text_feature / audio_feature
+ *   halves != NULL         : the split head, see the field
  * Dropout: Philox streams 0,1 (text head in/out) and 2,3 (audio head in/out) keyed by rng_state = {seed, offset}
  * (read on the device; with the loss stage the offset is advanced by rng_consume at the end, so a captured CUDA graph
  * draws fresh masks per replay) - the same streams b200rnn_mlp_dropout uses.
@@ -434,6 +435,12 @@ typedef struct b200rnn_fuse_head_args {
   uint32_t* comm_step;    /* world > 1: device uint32 step counter of the exchange (zero-initialised)           */
   uint32_t* comm_done;    /* defer_exchange: device uint32 count of steps whose update has been applied (zero-init.) */
   void* comm_buf[B200RNN_COMM_MAX_WORLD]; /* world > 1: every rank's exchange buffer as mapped in THIS process    */
+  float* halves;          /* split head (classification): [B][4] per-row fc_final logit halves {text c0, c1, audio c0, c1},
+                             16-byte aligned (read as float4; an unaligned pointer is rejected).
+                             With halves set, a text launch (pooled == NULL) or an audio launch (seq, ctx_in, tf_in
+                             NULL) writes its half of each row's logits and of the feature matrix in dw_part (W and
+                             dw_part required) and stops; a launch with neither branch then runs only the loss, dW,
+                             the exchange and Adam, in one CTA. The result is bit-identical to the one-launch tail.  */
 } b200rnn_fuse_head_args;
 
 B200RNN_API size_t b200rnn_fuse_head_scratch_floats(int B, int Ht, int Ha, int regression);

@@ -13,7 +13,9 @@ prints, as medians over the replays:
     beside its streamed GEMM); for a recurrence also `after_gemm_start`;
   * its duration, beside its duration when the audio branch runs alone.
 and the end of the text branch (with the text half of the head) relative to the end of the audio chain (negative: the
-text branch ends first). The head kernel after the join is counted in neither. The text-branch kernels (every kernel
+text branch ends first). The head launch after the join (the step's last kernel) is counted in neither: it is
+listed on its own, with the join gap (its start minus the end of everything before it) and the time from the audio
+chain's end to the step's end. The text-branch kernels (every kernel
 off the audio stream before the join) are listed too, in start order: name, grid, median start and duration, so that
 what runs beside rec0's end and rec1's start can be read off, each beside its duration when the text branch runs
 alone.
@@ -41,6 +43,8 @@ import bench  # noqa: E402
 
 # the GRU-256 forward recurrence: 3xTF32 tensor cores, or fp16 pairs in the no-grad fused forward
 REC = ("rec_fwd_tc_kernel", "rec_fwd_h16_kernel")
+# the head launch after the join: the whole head, or only the loss / dW / Adam of the split classification head
+AFTER_JOIN = ("fuse_head_kernel", "fuse_loss_kernel")
 
 
 def _card():
@@ -105,18 +109,39 @@ def _median(xs):
     return xs[len(xs) // 2] if len(xs) % 2 else 0.5 * (xs[len(xs) // 2 - 1] + xs[len(xs) // 2])
 
 
-def _audio_chain(replay):
-    """(audio chain, text branch): the kernels on the recurrence's stream, and the others; the final head kernel after
-    the join belongs to neither."""
+def _split(replay):
+    """(audio chain, text branch, after the join): the kernels on the recurrence's stream; the others; the step's last
+    launch, the head kernel that runs once both branches have ended. A replayed graph may report that kernel on either
+    branch's stream, so it is told apart by its place, not its stream."""
     streams = {k["stream"] for k in replay if k["name"] in REC}
     if len(streams) != 1:
         raise RuntimeError(f"the GRU recurrences ran on streams {sorted(streams)}; expected one audio stream")
     s = streams.pop()
-    if replay[-1]["name"] == "fuse_head_kernel":
-        replay = replay[:-1]
-    audio = [k for k in replay if k["stream"] == s]
-    other = [k for k in replay if k["stream"] != s]
+    before, post = (replay[:-1], replay[-1:]) if replay[-1]["name"] in AFTER_JOIN else (replay, [])
+    return [k for k in before if k["stream"] == s], [k for k in before if k["stream"] != s], post
+
+
+def _audio_chain(replay):
+    """(audio chain, text branch): the kernels on the recurrence's stream, and the others; the kernels after the join
+    belong to neither."""
+    audio, other, _ = _split(replay)
     return audio, other
+
+
+def _post_join(replays):
+    """The kernels after the join (name, grid, median start and duration, µs), the median join gap (first post-join
+    start minus the end of every kernel before it) and the median time from the audio chain's end to the step's end."""
+    parts = [_split(r) for r in replays]
+    names = [k["name"] for k in parts[0][2]]
+    if any([k["name"] for k in p[2]] != names for p in parts):
+        raise RuntimeError("the kernels after the join differ between replays")
+    rows = [{"kernel": n, "grid": parts[0][2][i]["grid"],
+             "start_us": round(_median([p[2][i]["start"] for p in parts]), 1),
+             "dur_us": round(_median([p[2][i]["end"] - p[2][i]["start"] for p in parts]), 1)}
+            for i, n in enumerate(names)]
+    gap = _median([p[2][0]["start"] - max(k["end"] for k in p[0] + p[1]) for p in parts]) if names else 0.0
+    tail = _median([max(k["end"] for k in r) - max(k["end"] for k in p[0]) for r, p in zip(replays, parts)])
+    return rows, round(gap, 1), round(tail, 1)
 
 
 def _chain_rows(replays):
@@ -215,9 +240,9 @@ def main():
                 "text_alone": _kernels(text_branch, args.replays, args.warmup, os.path.join(args.out, "trace_text.json"))}
     rows, text_end, step, text_rows = _chain_rows(runs["whole_step"])
     alone, _, audio_step, _ = _chain_rows(runs["audio_alone"])
-    if len(rows) != len(alone):
+    if len(rows) < len(alone):
         raise RuntimeError("the audio chain differs between the whole step and the audio branch alone")
-    for r, a in zip(rows, alone):
+    for r, a in zip(rows, alone):  # kernels past the audio branch alone (the head's audio stage) have no alone value
         if r["kernel"] != a["kernel"]:
             raise RuntimeError("the audio chain differs between the whole step and the audio branch alone")
         r["dur_alone_us"] = a["dur_us"]
@@ -227,8 +252,10 @@ def main():
     if [r["kernel"] for r in text_rows[:len(text_alone)]] == [a["kernel"] for a in text_alone]:
         for r, a in zip(text_rows, text_alone):
             r["dur_alone_us"] = a["dur_us"]
+    post, join_gap, tail = _post_join(runs["whole_step"])
     summary = {"card": card, "mode": mode, "replays": args.replays, "audio_chain": rows, "text_branch": text_rows,
-               "text_end_minus_audio_end_us": round(text_end, 1), "whole_step_us": round(step, 1),
+               "text_end_minus_audio_end_us": round(text_end, 1), "post_join": post, "join_gap_us": join_gap,
+               "audio_end_to_step_end_us": tail, "whole_step_us": round(step, 1),
                "audio_alone_us": round(audio_step, 1)}
     with open(os.path.join(args.out, "step_timeline.json"), "w") as f:
         json.dump({"summary": summary, "kernels": runs}, f, indent=1)
@@ -237,7 +264,7 @@ def main():
           f"{'after GEMM start':>18}   (µs, median of {args.replays} replays)")
     for r in rows:
         print(f"{r['kernel'][:21]:<22}{str(r['grid']):>16}{r['start_us']:>9}{r.get('gap_us', ''):>9}"
-              f"{r.get('gap_alone_us', ''):>11}{r['dur_us']:>9}{r['dur_alone_us']:>11}"
+              f"{r.get('gap_alone_us', ''):>11}{r['dur_us']:>9}{r.get('dur_alone_us', ''):>11}"
               f"{r.get('after_gemm_start_us', ''):>18}")
     print(f"{'text kernel':<22}{'grid':>16}{'start':>9}{'dur':>9}{'end':>9}{'dur alone':>11}")
     for r in text_rows:
@@ -245,6 +272,10 @@ def main():
               f"{round(r['start_us'] + r['dur_us'], 1):>9}{r.get('dur_alone_us', ''):>11}")
     if not text_rows:
         print("text alone: " + ", ".join(f"{a['kernel']} {a['grid']} {a['dur_us']}" for a in text_alone))
+    print(f"{'after the join':<22}{'grid':>16}{'start':>9}{'dur':>9}")
+    for r in post:
+        print(f"{r['kernel'][:21]:<22}{str(r['grid']):>16}{r['start_us']:>9}{r['dur_us']:>9}")
+    print(f"join gap {join_gap} µs; audio chain end to step end {tail} µs")
     print(f"text branch ends {text_end:+.1f} µs after the audio chain; step (first to last kernel) {step:.1f} µs, "
           f"audio branch alone {audio_step:.1f} µs")
     print(json.dumps(summary))
