@@ -23,6 +23,7 @@ FLAG_PROJ = 16      # the descriptor carries proj_size (read only with this flag
 FLAG_NO_BIAS = 32   # cells only: bias=False
 FLAG_F16 = 64       # x, parameters, states, outputs and gradients are float16 (the reserve and scratch stay fp32)
 FLAG_BF16 = 128     # ... bfloat16
+FLAG_F32_PARAMS = 256  # with FLAG_F16 / _BF16: the parameters and their gradient targets are fp32 (autocast)
 ABI_VERSION = 4
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)

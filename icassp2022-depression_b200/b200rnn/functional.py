@@ -29,6 +29,9 @@ class RNNConfig:
     tf32: bool = False   # single-pass TF32 tensor-core GEMMs / tc8 recurrence (tf32_enabled()), else 3xTF32
     proj_size: int = 0   # LSTM with projections: width P of h_t (0 = none)
     dtype: torch.dtype = torch.float32   # of x, the parameters, the states and every output (16-bit: FLAG_F16 / _BF16)
+    # fp32 master parameters of a 16-bit call (torch.autocast, FLAG_F32_PARAMS): the parameters and their gradients
+    # are float32, everything else is ``dtype``; computes what the 16-bit module computes on the rounded parameters
+    master_f32: bool = False
 
     @property
     def out_size(self) -> int:
@@ -59,7 +62,8 @@ def _require_cuda_f32(t: torch.Tensor, name: str) -> None:
 
 
 def _require_cuda_dtype(t: torch.Tensor, name: str, dtype: torch.dtype) -> None:
-    """float32 calls: as _require_cuda_f32. 16-bit calls: every tensor has the parameters' dtype"""
+    """float32 calls: as _require_cuda_f32. 16-bit calls: every tensor has the call's dtype (the parameters' dtype, or
+    float32 for the parameters of a master-weight call)"""
     if dtype == torch.float32:
         _require_cuda_f32(t, name)
         return
@@ -92,6 +96,8 @@ def _make_desc(cfg: RNNConfig, B: int, T: int, save: bool, accumulate: bool = Fa
     if cfg.proj_size:
         flags |= _lib.FLAG_PROJ
     flags |= _lib.H16_DTYPES.get(str(cfg.dtype), 0)
+    if cfg.master_f32:
+        flags |= _lib.FLAG_F32_PARAMS
     return _lib.Desc(cfg.mode, B, T, cfg.input_size, cfg.hidden_size, cfg.num_layers, cfg.num_dirs,
                      1 if cfg.training else 0, float(cfg.dropout), flags, cfg.proj_size)
 
@@ -442,7 +448,7 @@ def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig
     if cfg.dtype != torch.float32 and cfg.proj_size:
         raise NotImplementedError("b200rnn: proj_size is float32 only")
     for i, w in enumerate(weights):
-        _require_cuda_dtype(w, f"weight[{i}]", cfg.dtype)
+        _require_cuda_dtype(w, f"weight[{i}]", torch.float32 if cfg.master_f32 else cfg.dtype)
         if not w.is_contiguous():
             raise _lib.B200RNNError(f"b200rnn: weight[{i}] must be contiguous")
     if x.size(2) != cfg.input_size:

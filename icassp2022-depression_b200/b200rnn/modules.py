@@ -24,6 +24,9 @@ kept 16-bit by the runtime-sized recurrence, the state carried in fp32 (DESIGN.m
 feature above except ``proj_size`` and the model-shell fusions (``forward_ln_sum`` computes it unfused,
 ``frozen_weight_cache`` is None). A host (CPU) tensor raises ``B200RNNError`` that is also a ``NotImplementedError``: there is no CPU path.
 
+Under ``torch.autocast("cuda")`` an fp32 module without ``proj_size`` runs as its float16 twin would, on the fp32
+parameters as masters (fp32 gradients; DESIGN.md "Mixed precision"); 16-bit modules keep their dtype.
+
 ``RNN(..., nonlinearity='tanh' | 'relu')`` (the Elman network) takes the same inputs and features at every one of
 those hidden sizes on the runtime-sized kernels (csrc/rnn_anyh.cu, one gate block); it has no model-shell fusion
 (``forward_ln_sum`` computes it unfused, ``frozen_weight_cache`` is None) and no ``proj_size``.
@@ -45,6 +48,10 @@ _TORCH_GRU = nn.GRU
 _TORCH_LSTM = nn.LSTM
 _TORCH_RNN = nn.RNN
 _ELMAN_MODES = {"tanh": _lib.RNN_TANH, "relu": _lib.RNN_RELU}
+# The dtype stock nn.GRU / LSTM / RNN run in under torch.autocast("cuda", dtype=...): the AutocastCUDA wrapper of
+# aten::_cudnn_rnn casts the input, the states and the weights to float16 whatever the region's dtype is, bfloat16
+# included (measured on the H100, pinned by tests/test_gpu_autocast.py). An fp32 module here follows it.
+_AUTOCAST_DTYPE = torch.float16
 _module_counter = 0
 
 
@@ -187,22 +194,33 @@ class _B200RNNBase(nn.Module):
             self._wcache = (key, prepare_weights(ws, self._config()))
         return self._wcache[1]
 
-    def _config(self) -> RNNConfig:
+    def _config(self, autocast_dtype: Optional[torch.dtype] = None) -> RNNConfig:
         """The call's configuration, built per forward call: the TF32 mode follows torch's fp32 matmul precision at
-        that moment (``functional.tf32_enabled``), and the backward of the call reuses it."""
+        that moment (``functional.tf32_enabled``), and the backward of the call reuses it. ``autocast_dtype``: the
+        call runs in that 16-bit dtype on the fp32 parameters as masters (:meth:`_autocast_dtype`)."""
         return RNNConfig(mode=self._mode, input_size=self.input_size, hidden_size=self.hidden_size,
                          num_layers=self.num_layers, num_dirs=2 if self.bidirectional else 1,
                          dropout=self.dropout, training=self.training, batch_first=self.batch_first,
-                         tf32=tf32_enabled(), proj_size=self.proj_size, dtype=self._flat_weights[0].dtype)
+                         tf32=tf32_enabled(), proj_size=self.proj_size,
+                         dtype=autocast_dtype or self._flat_weights[0].dtype, master_f32=autocast_dtype is not None)
 
-    def _run_packed(self, packed, hx):
+    def _autocast_dtype(self) -> Optional[torch.dtype]:
+        """The 16-bit dtype this call runs in under ``torch.autocast("cuda")``, or None (the module's own dtype). An fp32
+        module without ``proj_size`` inside an enabled CUDA autocast region runs as its 16-bit twin would on its
+        parameters rounded to nearest even, with the fp32 parameters as masters: their gradients come back in fp32
+        (``B200RNN_FLAG_F32_PARAMS``), as through the casts of stock torch's autocast wrapper. 16-bit modules keep
+        their dtype; ``proj_size`` has no 16-bit kernels and stays fp32."""
+        if self.proj_size or self._flat_weights[0].dtype != torch.float32 or not torch.is_autocast_enabled("cuda"):
+            return None
+        return _AUTOCAST_DTYPE
+
+    def _run_packed(self, packed, hx, cfg: RNNConfig):
         """PackedSequence path (ragged DAIC-style sequences): pad, run with per-sequence lengths, re-pack exactly like
         torch (same batch_sizes / sorted_indices; hx, h_n and c_n in the caller's original batch order: the padded
         batch is in that order already)."""
         rnn_utils = nn.utils.rnn
         padded, lengths = rnn_utils.pad_packed_sequence(packed, batch_first=self.batch_first)
-        out = rnn_forward(padded, self._flat_weights, self._config(), self._rng_state, self._grad_sink, lengths=lengths,
-                          hx=hx)
+        out = rnn_forward(padded, self._flat_weights, cfg, self._rng_state, self._grad_sink, lengths=lengths, hx=hx)
         y = out[0]
         bdim = 0 if self.batch_first else 1
         if packed.sorted_indices is not None:
@@ -227,8 +245,14 @@ class _B200RNNBase(nn.Module):
         return None
 
     def _run(self, input, hx):
+        dt = self._autocast_dtype()
+        cfg = self._config(dt)
+        if dt is not None:   # autograd casts: the caller's input and states get their gradients in their own dtypes
+            input = input.to(dt)
+            if hx is not None:
+                hx = tuple(s.to(dt) for s in hx) if isinstance(hx, (tuple, list)) else hx.to(dt)
         if isinstance(input, nn.utils.rnn.PackedSequence):
-            return self._run_packed(input, hx)
+            return self._run_packed(input, hx, cfg)
         if input.dim() not in (2, 3):
             raise ValueError(f"{type(self).__name__}: Expected input to be 2D or 3D, got {input.dim()}D instead")
         batched = input.dim() == 3
@@ -237,13 +261,13 @@ class _B200RNNBase(nn.Module):
             if msg:
                 raise RuntimeError(msg)
         if batched:
-            return rnn_forward(input, self._flat_weights, self._config(), self._rng_state, self._grad_sink, hx=hx)
+            return rnn_forward(input, self._flat_weights, cfg, self._rng_state, self._grad_sink, hx=hx)
         # unbatched [T, I] (and [L*D, H] states): one batch row, whatever batch_first says, as torch runs it
         batch_dim = 0 if self.batch_first else 1
         if hx is not None:
             hx = tuple(s.unsqueeze(1) for s in hx) if self._mode == _lib.LSTM else hx.unsqueeze(1)
-        out = rnn_forward(input.unsqueeze(batch_dim), self._flat_weights, self._config(), self._rng_state,
-                          self._grad_sink, hx=hx)
+        out = rnn_forward(input.unsqueeze(batch_dim), self._flat_weights, cfg, self._rng_state, self._grad_sink,
+                          hx=hx)
         return (out[0].squeeze(batch_dim), *(s.squeeze(1) for s in out[1:]))
 
     def forward_ln_sum(self, input: torch.Tensor, ln: Optional[nn.LayerNorm] = None,
@@ -262,8 +286,9 @@ class _B200RNNBase(nn.Module):
         """
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
-        # torch.compile / torch.export trace the unfused expression through the custom ops (b200rnn/ops.py)
-        shape_ok = (not torch.compiler.is_compiling() and input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
+        # torch.compile / torch.export trace the unfused expression through the custom ops (b200rnn/ops.py), and so does
+        # a call under torch.autocast (the fusions are fp32 only)
+        shape_ok = (not torch.compiler.is_compiling() and self._autocast_dtype() is None and input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
                     self._gates > 1 and self._flat_weights[0].dtype == torch.float32 and
                     self.hidden_size in (128, 256) and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and

@@ -27,10 +27,13 @@ from . import functional as F
 
 
 def _rnn_config(kind, input_size, hidden_size, num_layers, num_dirs, proj_size, dropout, training, batch_first, tf32,
-                dtype) -> F.RNNConfig:
+                dtype, weights) -> F.RNNConfig:
+    """``master_f32`` (fp32 master parameters of a 16-bit call, ``torch.autocast``) is not an attribute of the ops: it
+    is what fp32 ``weights`` beside a 16-bit ``dtype`` mean, so the schemas stay as they were"""
+    master_f32 = dtype != torch.float32 and len(weights) > 0 and weights[0].dtype == torch.float32
     return F.RNNConfig(mode=kind, input_size=input_size, hidden_size=hidden_size, num_layers=num_layers,
                        num_dirs=num_dirs, dropout=dropout, training=training, batch_first=batch_first, tf32=tf32,
-                       proj_size=proj_size, dtype=dtype)
+                       proj_size=proj_size, dtype=dtype, master_f32=master_f32)
 
 
 def _rnn_attrs(cfg: F.RNNConfig) -> tuple:
@@ -65,7 +68,7 @@ def _rnn_forward_cuda(x, weights, h_0, c_0, lengths, rng_state, kind, input_size
     """``(y, h_n, c_n, reserve)`` of the RNN over the time-major view ``x`` [T, B, I]; the reserve (uint8) holds what
     the backward reads and is empty without ``save``."""
     cfg = _rnn_config(kind, input_size, hidden_size, num_layers, num_dirs, proj_size, dropout, training, batch_first,
-                      tf32, dtype)
+                      tf32, dtype, weights)
     y, h_n, c_n, reserve = F._rnn_forward_impl(x, cfg, rng_state, lengths, save, h_0, c_0, weights)
     return y, h_n, _none(c_n, y), reserve
 
@@ -73,7 +76,7 @@ def _rnn_forward_cuda(x, weights, h_0, c_0, lengths, rng_state, kind, input_size
 def _rnn_forward_fake(x, weights, h_0, c_0, lengths, rng_state, kind, input_size, hidden_size, num_layers, num_dirs,
                       proj_size, dropout, training, batch_first, tf32, dtype, save):
     cfg = _rnn_config(kind, input_size, hidden_size, num_layers, num_dirs, proj_size, dropout, training, batch_first,
-                      tf32, dtype)
+                      tf32, dtype, weights)
     _, reserve, _, y, _, h_n, c_n = F._forward_buffers(x, cfg, save, with_scratch=False)
     return y, h_n, _none(c_n, y), reserve
 
@@ -123,7 +126,7 @@ def rnn_backward(x: Tensor, y: Tensor, reserve: Tensor, h_0: Optional[Tensor], c
     """``(dx, dh_0, dc_0, weight grads)``. ``needs`` = [dx, dh_0, dc_0, one per weight]: what is not needed is not
     computed (a NULL pointer to the library) and comes back as an empty ``[0]`` tensor."""
     cfg = _rnn_config(kind, input_size, hidden_size, num_layers, num_dirs, proj_size, dropout, training, batch_first,
-                      tf32, dtype)
+                      tf32, dtype, weights)
     dx, dh_0, dc_0, dws = F._rnn_backward_impl(cfg, x, y, reserve, h_0, c_0, weights, dy, dh_n, dc_n, lengths,
                                                needs[0], needs[1], needs[2], needs[3:], None, separate=True)
     return _none(dx, x), _none(dh_0, x), _none(dc_0, x), [_none(g, w) for g, w in zip(dws, weights)]

@@ -44,7 +44,7 @@ inline int desc_proj(const b200rnn_desc* d) { return (d->flags & B200RNN_FLAG_PR
 // GRU / LSTM at the fixed hidden sizes 128 and 256: their fusions (LayerNorm prologue, pooling, weight cache, the
 // fp16-pair no-grad recurrence) are built for those
 int check_shell_desc(const b200rnn_desc* d, const char* what) {
-  if (d && (d->flags & (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16))) {
+  if (d && (d->flags & (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_F32_PARAMS))) {
     set_error("%s: the model-shell entry points and the weight cache are float32 only (use the _hx entry points for "
               "16-bit tensors)", what);
     return B200RNN_ERR_UNSUPPORTED;
@@ -69,6 +69,7 @@ struct Dims {
   bool training;
   float p;
   int dt;  // DT_F32, or DT_F16 / DT_BF16: the caller's tensors are 16-bit (B200RNN_FLAG_F16 / _BF16)
+  bool master;  // B200RNN_FLAG_F32_PARAMS: the parameters and their gradients are fp32 (the rest is 16-bit)
 };
 
 int check_desc(const b200rnn_desc* d, Dims* o) {
@@ -109,6 +110,11 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
     set_error("B200RNN_FLAG_F16 and B200RNN_FLAG_BF16 exclude each other");
     return B200RNN_ERR_UNSUPPORTED;
   }
+  const bool master = (d->flags & B200RNN_FLAG_F32_PARAMS) != 0;
+  if (master && !h16) {
+    set_error("B200RNN_FLAG_F32_PARAMS needs B200RNN_FLAG_F16 or B200RNN_FLAG_BF16 (the dtype of the other tensors)");
+    return B200RNN_ERR_INVALID;
+  }
   if (h16 && P > 0) {
     set_error("proj_size is float32 only (B200RNN_FLAG_F16 / _BF16 with B200RNN_FLAG_PROJ)");
     return B200RNN_ERR_UNSUPPORTED;
@@ -134,6 +140,7 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
   o->training = d->training != 0;
   o->p = d->dropout_p;
   o->dt = h16 == B200RNN_FLAG_F16 ? DT_F16 : h16 == B200RNN_FLAG_BF16 ? DT_BF16 : DT_F32;
+  o->master = master;
   return B200RNN_OK;
 }
 
@@ -211,9 +218,12 @@ struct ScratchLayout {
 //          widened h_0 / c_0, the fp32 h_n / c_n, the 16-bit input of the next layer (a16), and without a reserve the
 //          rounded inputs and the top layer's fp32 output
 // backward: x, dy, the states and their gradients, every parameter and gradient, dx, all fp32
+// fp32 master parameters (B200RNN_FLAG_F32_PARAMS), behind the rest: the 16-bit images of every weight_ih and weight_hh,
+//          which the 16-bit kernels read in place of the caller's 16-bit parameters
 struct H16Scratch {
   size_t bias[8][2], whh, h0, c0, hn, cn, a16, xin, ytop;
   size_t x32, dy32, dhn, dcn, bh0, bc0, dh0, dc0, w32[8][2], dw32[8][2], dx32;
+  size_t ih16[8][2], hh16[8][2];
   size_t total;
 };
 
@@ -237,6 +247,12 @@ void make_h16_scratch(const Dims& d, size_t base, H16Scratch* h) {
       h->dw32[l][k] = take(n);
     }
   h->dx32 = take(d.TB * d.I);
+  for (int l = 0; l < d.L && l < 8; ++l)
+    for (int k = 0; k < d.D; ++k) {
+      const size_t Il = l == 0 ? (size_t)d.I : d.DH;
+      h->ih16[l][k] = take(d.master ? (d.GH * Il + 1) / 2 : 0);
+      h->hh16[l][k] = take(d.master ? (d.GH * d.H + 1) / 2 : 0);
+    }
   h->total = off;
 }
 
@@ -579,6 +595,48 @@ B200RNN_API int b200rnn_workspace_bytes(const b200rnn_desc* desc, size_t* reserv
   return B200RNN_OK;
 }
 
+// B200RNN_FLAG_F32_PARAMS: one round16_multi launch over the call's L * D * 4 fp32 parameters. Every parameter is
+// rounded to the 16-bit dtype once; what the 16-bit call reads from the caller's 16-bit parameters is written from it:
+//   forward:  the 16-bit images of weight_ih (hs.ih16) and weight_hh (hs.hh16), the fp32 biases (hs.bias) and, for the
+//             fixed configs (whh32), the fp32 weight_hh at its place in hs.w32;
+//   backward: every parameter in fp32 (hs.w32, the fp32 BPTT's operands) and the 16-bit weight_hh images.
+// img: the parameter table of the rest of the call (images of the weights; biases and fp32 weight_hh read elsewhere)
+static int round_master_params(const Dims& d, const float* const* params, float* S, const H16Scratch& hs, bool bwd,
+                               bool whh32, const float** img, cudaStream_t st) {
+  if (!params) {
+    set_error("null parameter table");
+    return B200RNN_ERR_INVALID;
+  }
+  Round16Seg seg[ROUND16_MAX_SEGS];
+  int n = 0;
+  for (int l = 0; l < d.L; ++l)
+    for (int k = 0; k < d.D; ++k) {
+      const size_t j = (size_t)(l * d.D + k) * 4;
+      const size_t Il = l == 0 ? (size_t)d.I : d.DH;
+      for (int i = 0; i < 4; ++i)
+        if (!params[j + i]) {
+          set_error("null parameter pointer (layer %d dir %d)", l, k);
+          return B200RNN_ERR_INVALID;
+        }
+      uint16_t* ih16 = reinterpret_cast<uint16_t*>(S + hs.ih16[l][k]);
+      uint16_t* hh16 = reinterpret_cast<uint16_t*>(S + hs.hh16[l][k]);
+      float* w32 = S + hs.w32[l][k];
+      const long long nih = (long long)(d.GH * Il), nhh = (long long)(d.GH * d.H), nb = (long long)d.GH;
+      float* b32 = bwd ? w32 + nih + nhh : S + hs.bias[l][k];
+      seg[n++] = Round16Seg{params[j], bwd ? nullptr : ih16, bwd ? w32 : nullptr, nih};
+      // the fixed configs' forward reads weight_hh in fp32 only, everything else the 16-bit image
+      const bool hh32 = bwd || whh32;
+      seg[n++] = Round16Seg{params[j + 1], (bwd || !whh32) ? hh16 : nullptr, hh32 ? w32 + nih : nullptr, nhh};
+      seg[n++] = Round16Seg{params[j + 2], nullptr, b32, nb};
+      seg[n++] = Round16Seg{params[j + 3], nullptr, b32 + nb, nb};
+      img[j] = reinterpret_cast<const float*>(ih16);
+      img[j + 1] = reinterpret_cast<const float*>(hh16);
+      img[j + 2] = params[j + 2];
+      img[j + 3] = params[j + 3];
+    }
+  return launch_round16_multi(seg, n, d.dt, ROUND16_IMAGES, st);
+}
+
 // The forward of every entry point; h_0 / c_0 NULL = zeros (b200rnn_forward_hx checked their consistency). `shell`:
 // called by b200rnn_forward_fused, the model-shell entry, which never takes an initial state; its no-grad forward runs
 // the GRU-256 tensor-core recurrence on fp16 pairs (RecFwdParams::shell_nograd)
@@ -668,9 +726,18 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
   void* const y16 = y;
   void* const hn16 = h_n;
   void* const cn16 = c_n;
+  // fp32 master parameters: one launch rounds them into what the 16-bit call reads (16-bit images of weight_ih and
+  // weight_hh, the fp32 biases, the fixed configs' fp32 weight_hh), and the rest of the call runs on the images
+  const float* img[8 * 2 * 4];
+  const bool fixed_whh = !is_elman(d.mode) && (d.H == 128 || d.H == 256);
   if (dt) {
     make_h16_scratch(d, sl.b_total, &hs);
-    for (int l = 0; l < d.L; ++l)
+    if (d.master) {
+      rc = round_master_params(d, params, S, hs, false, fixed_whh, img, st);
+      if (rc) return rc;
+      params = img;
+    }
+    for (int l = 0; l < d.L && !d.master; ++l)
       for (int k = 0; k < d.D; ++k) {
         const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
         if (!pp[2] || !pp[3]) {
@@ -868,7 +935,13 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       rp.b_hh[k] = b_hh;
       if (dt) {
         rp.b_hh[k] = S + hs.bias[l][k] + d.GH;
-        if (!rec.anyh) {  // the fixed configs read fp32: an exact copy per direction
+        if (!rec.anyh && d.master) {  // rounded into hs.w32 by round_master_params
+          if (!fixed_whh) {
+            set_error("forward: no fp32 weight_hh for the recurrence config (mode %d, hidden_size %d)", d.mode, d.H);
+            return B200RNN_ERR_UNSUPPORTED;
+          }
+          rp.w_hh[k] = S + hs.w32[l][k] + d.GH * (size_t)Il;
+        } else if (!rec.anyh) {  // the fixed configs read fp32: an exact copy per direction
           float* w32 = S + hs.whh + (size_t)k * d.GH * d.H;
           rc = launch_widen16(w_hh, simple_rows(d.H), (int)d.GH, d.H, dt, w32, st);
           if (rc) return rc;
@@ -1322,6 +1395,12 @@ static int backward_h16(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
   if (rc) return rc;
   const float* p32[8 * 2 * 4];
   float* dp32[8 * 2 * 4];
+  // fp32 master parameters: one launch rounds them into hs.w32 and the 16-bit weight_hh images
+  const float* img[8 * 2 * 4];
+  if (d.master) {
+    rc = round_master_params(d, params, S, hs, true, true, img, st);
+    if (rc) return rc;
+  }
   for (int l = 0; l < d.L; ++l)
     for (int k = 0; k < d.D; ++k) {
       const int Il = l == 0 ? d.I : DH;
@@ -1334,7 +1413,7 @@ static int backward_h16(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
           return B200RNN_ERR_INVALID;
         }
         float* p = S + hs.w32[l][k] + off;
-        rc = launch_widen16(params[j], simple_rows((long long)n[i]), 1, (int)n[i], dt, p, st);
+        if (!d.master) rc = launch_widen16(params[j], simple_rows((long long)n[i]), 1, (int)n[i], dt, p, st);
         if (rc) return rc;
         p32[j] = p;
         dp32[j] = dparams[j] ? S + hs.dw32[l][k] + off : nullptr;
@@ -1344,10 +1423,11 @@ static int backward_h16(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
   const float* layer_in[8];
   for (int l = 0; l + 1 < d.L; ++l) layer_in[l] = R + rl.xin[l];
   const void* whh16[8 * 2];
-  for (int i = 0; i < d.L * d.D; ++i) whh16[i] = params[(size_t)i * 4 + 1];
+  for (int i = 0; i < d.L * d.D; ++i) whh16[i] = (d.master ? img : params)[(size_t)i * 4 + 1];
   b200rnn_desc d32 = *desc;
   // TF32 applies to fp32 calls only (forward_impl): the fp32 backward of a 16-bit call runs its 3xTF32 GEMMs
-  d32.flags &= ~(B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_ACCUMULATE_GRADS | B200RNN_FLAG_TF32);
+  d32.flags &= ~(B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_ACCUMULATE_GRADS | B200RNN_FLAG_TF32 |
+                 B200RNN_FLAG_F32_PARAMS);
   rc = backward_impl(&d32, S + hs.x32, (int64_t)d.B * d.I, d.I, p32, R + rl.ytop, (int64_t)d.B * DH, DH, S + hs.dy32,
                      (int64_t)d.B * DH, DH, nullptr, 0.f, w[0], w[1], reserve, scratch, dx ? S + hs.dx32 : nullptr,
                      (int64_t)d.B * d.I, d.I, dp32, lengths, nullptr, 0.f, nullptr, nullptr, w[2], w[3],
@@ -1358,6 +1438,20 @@ static int backward_h16(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
                                nullptr, st);
   if (!rc && dh_0) rc = launch_narrow16(S + hs.dh0, hrows, nst, d.H, dt, dh_0, hrows, false, nullptr, st);
   if (!rc && dc_0) rc = launch_narrow16(S + hs.dc0, hrows, nst, d.H, dt, dc_0, hrows, false, nullptr, st);
+  if (!rc && d.master) {  // one launch: every gradient rounded to the 16-bit dtype and widened into its fp32 target
+    Round16Seg seg[ROUND16_MAX_SEGS];
+    int ns = 0;
+    for (int l = 0; l < d.L; ++l)
+      for (int k = 0; k < d.D; ++k) {
+        const int Il = l == 0 ? d.I : DH;
+        const size_t n[4] = {d.GH * (size_t)Il, d.GH * (size_t)d.H, d.GH, d.GH};
+        for (int i = 0; i < 4; ++i) {
+          const size_t j = (size_t)(l * d.D + k) * 4 + i;
+          seg[ns++] = Round16Seg{dp32[j], nullptr, dparams[j], dparams[j] ? (long long)n[i] : 0};
+        }
+      }
+    return launch_round16_multi(seg, ns, dt, acc ? ROUND16_GRAD_ADD : ROUND16_GRAD_SET, st);
+  }
   for (int l = 0; l < d.L && !rc; ++l)
     for (int k = 0; k < d.D && !rc; ++k) {
       const int Il = l == 0 ? d.I : DH;

@@ -2,6 +2,7 @@
 // round-to-nearest-even narrowing of every output. Element-wise and HBM-bound.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <string.h>
 
 #include "h16.cuh"
 
@@ -74,6 +75,31 @@ __global__ void copy16_kernel(const uint16_t* __restrict__ src, RowMap rows, int
   }
 }
 
+// The segments of one launch_round16_multi call: each takes ceil(n / ROUND16_CHUNK) consecutive blocks from blk0[s]
+constexpr int ROUND16_CHUNK = 4096;
+struct Round16Table {
+  Round16Seg seg[ROUND16_MAX_SEGS];
+  int blk0[ROUND16_MAX_SEGS + 1];
+  int nseg;
+};
+
+__global__ void __launch_bounds__(256) round16_multi_kernel(const __grid_constant__ Round16Table t, int dt, int mode) {
+  int s = 0;
+  while (s + 1 < t.nseg && (int)blockIdx.x >= t.blk0[s + 1]) ++s;
+  const float* src = t.seg[s].src;
+  uint16_t* d16 = t.seg[s].d16;
+  float* d32 = t.seg[s].d32;
+  const long long base = (long long)(blockIdx.x - t.blk0[s]) * ROUND16_CHUNK;
+  const long long n = t.seg[s].n - base < ROUND16_CHUNK ? t.seg[s].n - base : ROUND16_CHUNK;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const long long j = base + i;
+    const uint16_t r = narrow(src[j], dt);
+    const float w = widen(r, dt);
+    if (d16) d16[j] = r;
+    if (d32) d32[j] = mode == ROUND16_GRAD_ADD ? d32[j] + w : w;
+  }
+}
+
 // dense rows (row r at r * C) on both sides, whole 4-element vectors, aligned for them
 bool dense_vec(const RowMap& a, const RowMap& b, int R, int C, const void* p16, const void* p32, const void* wb) {
   auto dense = [&](const RowMap& m) { return R == 1 || (m.s_inner == C && (m.inner_n >= R || m.s_outer == (long long)m.inner_n * C)); };
@@ -108,6 +134,28 @@ int launch_narrow16(const float* src, const RowMap& src_rows, int R, int C, int 
   const bool vec = dense_vec(dst_rows, src_rows, R, C, dst, src, wb);
   narrow16_kernel<<<vec ? blocks_for((size_t)R * C / 4) : rows_blocks(R), 256, 0, stream>>>(
       src, src_rows, R, C, dt, static_cast<uint16_t*>(dst), dst_rows, accumulate ? 1 : 0, wb, vec ? 1 : 0);
+  B200_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return B200RNN_OK;
+}
+
+int launch_round16_multi(const Round16Seg* segs, int nseg, int dt, int mode, cudaStream_t stream) {
+  if (nseg > ROUND16_MAX_SEGS) {
+    set_error("round16: %d parameter tensors, at most %d", nseg, ROUND16_MAX_SEGS);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  Round16Table t;
+  memset(&t, 0, sizeof(t));
+  long long blocks = 0;
+  for (int s = 0; s < nseg; ++s) {  // empty segments (a gradient not asked for) take no block
+    if (segs[s].n <= 0 || (!segs[s].d16 && !segs[s].d32)) continue;
+    t.seg[t.nseg] = segs[s];
+    t.blk0[t.nseg++] = (int)blocks;
+    blocks += (segs[s].n + ROUND16_CHUNK - 1) / ROUND16_CHUNK;
+  }
+  t.blk0[t.nseg] = (int)blocks;
+  if (blocks == 0) return B200RNN_OK;
+  round16_multi_kernel<<<(unsigned)blocks, 256, 0, stream>>>(t, dt, mode);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;

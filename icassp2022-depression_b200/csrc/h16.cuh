@@ -18,6 +18,21 @@ int launch_widen16(const void* src, const RowMap& rows, int R, int C, int dt, fl
 int launch_narrow16(const float* src, const RowMap& src_rows, int R, int C, int dt, void* dst, const RowMap& dst_rows,
                     bool accumulate, float* wb, cudaStream_t stream);
 
+// ---- fp32 master parameters (B200RNN_FLAG_F32_PARAMS): one launch over every parameter tensor of a call ----------------
+// Per segment, element i: r = round_dt(src[i]) (nearest even, as narrow16 rounds), then
+//   ROUND16_IMAGES:   d16[i] = r, d32[i] = widen(r)      (either target may be NULL)
+//   ROUND16_GRAD_SET: d32[i] = widen(r)                  (a gradient into its fp32 target)
+//   ROUND16_GRAD_ADD: d32[i] = d32[i] + widen(r)         (the same, accumulated in fp32)
+enum : int { ROUND16_IMAGES = 0, ROUND16_GRAD_SET = 1, ROUND16_GRAD_ADD = 2 };
+constexpr int ROUND16_MAX_SEGS = 8 * 2 * 4;  // L * D * 4 parameters, L <= 8, D <= 2
+struct Round16Seg {
+  const float* src;
+  uint16_t* d16;
+  float* d32;
+  long long n;
+};
+int launch_round16_multi(const Round16Seg* segs, int nseg, int dt, int mode, cudaStream_t stream);
+
 // 16-bit rows gathered into a dense [R][C] 16-bit copy (an A operand the TMA cannot read in place)
 int launch_copy16(const void* src, const RowMap& rows, int R, int C, void* dst, cudaStream_t stream);
 

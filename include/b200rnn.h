@@ -79,6 +79,15 @@ enum {
                                              B200RNN_FLAG_PROJ; the _fused entry points and the weight cache return
                                              B200RNN_ERR_UNSUPPORTED. */
 #define B200RNN_FLAG_BF16 128u            /* the same with bfloat16 tensors; excludes B200RNN_FLAG_F16 */
+#define B200RNN_FLAG_F32_PARAMS 256u      /* mixed precision (fp32 master weights), only together with B200RNN_FLAG_F16 or
+                                             _BF16: the parameter pointers and every dparams target are fp32, everything
+                                             else is 16-bit as with the dtype flag alone. The call computes exactly what
+                                             the 16-bit call computes on the parameters rounded to nearest even: one
+                                             launch rounds them at the start of the forward and of the backward, and one
+                                             launch writes each gradient as widen(round(g)) into its fp32 target (added
+                                             to it with B200RNN_FLAG_ACCUMULATE_GRADS). Alone: B200RNN_ERR_INVALID. With
+                                             B200RNN_FLAG_PROJ, in the _fused entry points and the weight cache:
+                                             B200RNN_ERR_UNSUPPORTED. b200rnn_workspace_bytes sizes the rounded images. */
 
 /*
  * Problem descriptor. Mirrors the constructor arguments of torch.nn.GRU / torch.nn.LSTM
