@@ -1,8 +1,8 @@
 """Do the numerics tests bite? Build the library with one small arithmetic mutation at a time and run the tests on it.
 
-Each mutation is one textual edit of csrc/ that changes arithmetic only - no indexing, barrier or memory access - and is
-applied to a copy of the sources; that copy is built (make, as build() does, reusing the tree's objects so that only
-the mutated file recompiles) and loaded with B200RNN_LIB. Each mutation names the new tests that must catch it and the
+Each mutation is one textual edit of csrc/ that changes arithmetic only or removes a data store - never an index, a
+barrier, a flag or a counter, so that no mutated build can fault or hang - and is applied to a copy of the sources; that
+copy is built (make, as build() does, reusing the tree's objects so that only the mutated file recompiles) and loaded with B200RNN_LIB. Each mutation names the new tests that must catch it and the
 existing tests it is also run against. Against each build the script runs the new tests (stopping after a few
 failures) and then the existing files in order, each until its first failure, stopping at the first file that fails;
 it records per mutation which tests fail. A mutation that no new test catches is a hole in the suite.
@@ -37,7 +37,16 @@ SHELL_EXISTING = ["tests/test_gpu_head.py", "tests/test_gpu_train_step.py", "tes
 H16_NEW = ["tests/test_gpu_h16_numerics_f64.py"]
 H16_EXISTING = ["tests/test_gpu_h16_modules.py"]
 
-# name -> (file under csrc/, text, replacement, what it breaks, new tests, existing tests)
+ANYH_NEW = ["tests/test_gpu_anyh_numerics_f64.py", "tests/test_gpu_poisoned_buffers.py"]
+ANYH_EXISTING = ["tests/test_gpu_any_hidden.py", "tests/test_gpu_elman.py", "tests/test_gpu_varlen_sorted.py"]
+CELL_NEW = ["tests/test_gpu_anyh_numerics_f64.py::test_cell_backward_off_default_init_vs_f64"]
+CELL_EXISTING = ["tests/test_gpu_cells.py", "tests/test_gpu_elman.py"]
+# tf32(v): v with its 13 low mantissa bits cleared, the operand precision of a single-pass TF32 product
+_TF32 = "__uint_as_float(__float_as_uint({}) & 0xffffe000u)"
+
+# name -> (file under csrc/, text, replacement, what it breaks, new tests, existing tests[, occurrence]). Without an
+# occurrence the text must occur exactly once; with one, the occurrence-th (from 0) of several is edited: the fp32 and
+# the 16-bit bodies of rnn_anyh.cu share their text, and the fp32 kernels come first in the file.
 MUTATIONS = {
     "x3_drop_ah_bl": ("rnn_rec.cu", "            ptx::mma_tf32_m16n8k8(d[g][0], ah, bl);\n", "",
                       "3xTF32 tc8 recurrence: the hi(W) * lo(h) correction mma is lost", REC_NEW, REC_EXISTING),
@@ -126,6 +135,47 @@ MUTATIONS = {
     "tcl8_drop_al_bh": ("rnn_rec.cu", "            ptx::mma_f16_m16n8k16(d[g][0], al, bh);\n", "",
                         "fp16-pair tc8 / tcl8 recurrence: the lo(W) * hi(h) correction mma is lost", REC_NEW,
                         ["tests/test_gpu_lstm_h16_fwd.py"]),
+    # the fp32 runtime-sized BPTT (anyh_bwd_kernel): arithmetic edits, or the removal of a data store
+    "anyh_bwd_dh_tf32": ("rnn_anyh.cu", "      dh_carry = direct + sum;\n",
+                         "      dh_carry = direct + " + _TF32.format("sum") + ";\n",
+                         "fp32 anyh BPTT: the recurrent contraction dh = W_hh^T dg is truncated to TF32", ANYH_NEW,
+                         ANYH_EXISTING, 0),
+    "anyh_bwd_send_bf16": ("rnn_anyh.cu", "      const float v = (MODE == B200RNN_GRU && g == 2) ? dhn : dg[g];\n",
+                           "      const float v = __bfloat162float(__float2bfloat16((MODE == B200RNN_GRU && g == 2) ? dhn "
+                           ": dg[g]));\n",
+                           "fp32 anyh BPTT: the gate gradient sent to the cluster is rounded to bf16", ANYH_NEW,
+                           ANYH_EXISTING, 0),
+    "anyh_bwd_frozen_dy": ("rnn_anyh.cu", "    const float dh = frozen ? dh_carry : dh_carry + dyv;\n",
+                           "    const float dh = dh_carry + dyv;\n",
+                           "fp32 anyh BPTT: dy past a row's length is added into the carried gradient", ANYH_NEW,
+                           ANYH_EXISTING, 0),
+    "anyh_bwd_skip_tail_zero": ("rnn_anyh.cu",
+                                "#pragma unroll\n        for (int g = 0; g < G; ++g) gp[g * H] = 0.f;\n"
+                                "        if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + row) * H + j] = 0.f;\n",
+                                "        (void)gp;\n",
+                                "fp32 anyh BPTT, ragged: the gate gradients of the steps [T, p.T) a cluster skipped "
+                                "are not written", ANYH_NEW, ANYH_EXISTING, 0),
+    "anyh_bwd_lstm_frozen_dc": ("rnn_anyh.cu",
+                                "      if (!frozen) dc_carry = dc_next;  // frozen: dh and dc pass straight through\n",
+                                "      dc_carry = dc_next;\n",
+                                "fp32 anyh LSTM BPTT, ragged: dc is carried through a frozen step's cell backward",
+                                ANYH_NEW, ANYH_EXISTING, 0),
+    "anyh_bwd_gru_vl_prev": ("rnn_anyh.cu",
+                             "    const bool has_prev = step < T - 1 && !(MODE == B200RNN_GRU && VL && tp >= len);\n",
+                             "    const bool has_prev = step < T - 1;\n",
+                             "fp32 anyh GRU BPTT, ragged reverse half: the last valid step reads the masked 0 as its "
+                             "previous state instead of h_0", ANYH_NEW, ANYH_EXISTING, 0),
+    "cell_bwd_gru_dh_drop8": ("cell.cu", "      direct = gru_cell_bwd(sv, sx, hp, dh, dg, dhn);\n",
+                              "      direct = gru_cell_bwd(sv, sx, hp, __uint_as_float(__float_as_uint(dh) & 0xffffff00u), "
+                              "dg, dhn);\n",
+                              "GRUCell backward: the output gradient loses its 8 low mantissa bits", CELL_NEW,
+                              CELL_EXISTING),
+    "cell_bwd_elman_dh_drop8": ("cell.cu",
+                                "    const float dg = elman_cell_bwd(p.gates[(size_t)b * H + j], dh, relu);\n",
+                                "    const float dg = elman_cell_bwd(p.gates[(size_t)b * H + j], "
+                                "__uint_as_float(__float_as_uint(dh) & 0xffffff00u), relu);\n",
+                                "RNNCell backward: the output gradient loses its 8 low mantissa bits", CELL_NEW,
+                                CELL_EXISTING[1:]),
 }
 
 
@@ -144,6 +194,7 @@ def build(tmp, name):
     """the mutated library: copies of csrc/, the Makefile, the tree's objects and include/ under tmp, one edit, make;
     an existing build there is reused"""
     src, before, after = MUTATIONS[name][:3]
+    occurrence = MUTATIONS[name][6] if len(MUTATIONS[name]) > 6 else None
     pkg = os.path.join(tmp, name, "pkg")
     lib = os.path.join(pkg, "lib", "libb200rnn.so")
     if os.path.exists(lib):
@@ -156,10 +207,15 @@ def build(tmp, name):
     shutil.copytree(os.path.join(ROOT, "include"), os.path.join(tmp, name, "include"))
     path = os.path.join(pkg, "csrc", src)
     text = open(path).read()
-    if text.count(before) != 1:
+    if occurrence is None and text.count(before) != 1:
         raise SystemExit(f"{name}: the text to mutate occurs {text.count(before)} times in {src}")
+    if occurrence is not None and text.count(before) <= occurrence:
+        raise SystemExit(f"{name}: the text to mutate occurs {text.count(before)} times in {src}, not {occurrence + 1}")
+    at = -1
+    for _ in range((occurrence or 0) + 1):
+        at = text.index(before, at + 1)
     with open(path, "w") as f:
-        f.write(text.replace(before, after))
+        f.write(text[:at] + after + text[at + len(before):])
     jobs = str(max(1, min(8, os.cpu_count() or 1)))
     subprocess.run(["make", "-C", pkg, "-j", jobs], check=True, capture_output=True)
     return lib
@@ -196,7 +252,7 @@ def main():
                 res = json.load(f)
         res["device"] = gpu_info()
         for name in names:
-            src, before, after, breaks, new_paths, old_paths = MUTATIONS[name]
+            src, before, after, breaks, new_paths, old_paths = MUTATIONS[name][:6]
             lib = build(where, name)
             new = failing(lib, new_paths, maxfail=args.new_maxfail)
             old = {}
@@ -206,6 +262,7 @@ def main():
                     break
             res["mutations"][name] = {
                 "file": src, "replaced": before.strip(), "with": after.strip(), "breaks": breaks,
+                **({"occurrence": MUTATIONS[name][6]} if len(MUTATIONS[name]) > 6 else {}),
                 "new_tests": new_paths, "new_tests_failing": new, "caught_by_new_tests": bool(new),
                 "existing_tests_run": list(old), "existing_first_failure": {p: f[0] for p, f in old.items() if f},
                 "caught_by_existing_tests": any(old.values()),
