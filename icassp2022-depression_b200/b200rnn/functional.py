@@ -82,6 +82,27 @@ def _tm_view(x: torch.Tensor) -> torch.Tensor:
     return x
 
 
+def _ln_operand_ok(x_tm: torch.Tensor, ln_w: Optional[torch.Tensor], ln_b: Optional[torch.Tensor]) -> bool:
+    """Whether the fused LayerNorm prologue and its backward can read ``x_tm`` [T,B,I] as it lies: a 16-byte aligned
+    base, time and batch strides that are multiples of 4 floats, and 16-byte aligned gamma and beta. The C ABI returns
+    ``B200RNN_ERR_UNSUPPORTED`` for any other x; the Python entries run on a dense copy instead."""
+    def aligned(t):
+        return t is None or t.data_ptr() % 16 == 0
+    return aligned(x_tm) and x_tm.stride(0) % 4 == 0 and x_tm.stride(1) % 4 == 0 and aligned(ln_w) and aligned(ln_b)
+
+
+def _ln_operands(x_tm: torch.Tensor, ln_w: Optional[torch.Tensor], ln_b: Optional[torch.Tensor]):
+    """``(x_tm, ln_w, ln_b)`` as the fused LayerNorm reads them: each tensor :func:`_ln_operand_ok` rejects is replaced
+    by a fresh (aligned; for x, dense time-major) copy, the others are passed as they are. The copies are
+    differentiable: autograd carries dx, dgamma and dbeta back to the caller's tensors."""
+    if ln_w is None or _ln_operand_ok(x_tm, ln_w, ln_b):
+        return x_tm, ln_w, ln_b
+    fresh = lambda t: t if t is None or t.data_ptr() % 16 == 0 else t.clone()  # noqa: E731
+    if not _ln_operand_ok(x_tm, None, None):
+        x_tm = x_tm.clone(memory_format=torch.contiguous_format)
+    return x_tm, fresh(ln_w), fresh(ln_b)
+
+
 def _make_desc(cfg: RNNConfig, B: int, T: int, save: bool, accumulate: bool = False,
                fused_ln: bool = False) -> _lib.Desc:
     flags = 0
@@ -389,6 +410,7 @@ def rnn_ln_pool_sum(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNCo
     if cfg.proj_size:
         raise NotImplementedError("b200rnn: the fused LayerNorm / time-sum path does not take proj_size")
     x_tm = _tm_view(x.transpose(0, 1) if cfg.batch_first else x)
+    x_tm, ln_weight, ln_bias = _ln_operands(x_tm, ln_weight, ln_bias)
     return _LNRNNPoolFunction.apply(x_tm, cfg, rng_state, grad_sink, ln_weight, ln_bias, ln_eps, *weights)
 
 
@@ -485,6 +507,7 @@ def rnn_forward_fused(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNN
     if cfg.proj_size:
         raise NotImplementedError("b200rnn: the fused forward (LayerNorm prologue, time sum) does not take proj_size")
     x_tm = _tm_view(x.transpose(0, 1) if cfg.batch_first else x)
+    x_tm, ln_weight, ln_bias = _ln_operands(x_tm, ln_weight, ln_bias)
     T, B, _ = x_tm.shape
     H, L, D = cfg.hidden_size, cfg.num_layers, cfg.num_dirs
     dev = x.device

@@ -799,6 +799,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     const void* a16 = l == 0 ? static_cast<const void*>(x) : S + hs.a16;
     RowMap a16_rows = l == 0 ? tb_rows(xs_t, xs_b, d.B) : simple_rows((long long)d.DH);
     bool n16 = false;
+    const char* a16_route = "tma";  // B200RNN_DEBUG: where the 16-bit A operand comes from
     if (dt) {
       n16 = tc && tc_gemm_n16_ok(a16, a16_rows, params[(size_t)l * d.D * d.NPAR], (int)d.TB, (int)d.GH, Il);
       if (!n16 && l == 0 && tc && tc_gemm_n16_ok(S + hs.a16, simple_rows(Il), params[0], (int)d.TB, (int)d.GH, Il)) {
@@ -806,6 +807,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         if (rc) return rc;
         a16 = S + hs.a16;
         a16_rows = simple_rows(Il);
+        a16_route = "copy16";
         n16 = true;
       }
     }
@@ -839,6 +841,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     void* tc_ws = S + sl.f_tc;
     const float* a_in = in;
     RowMap a_rows = in_rows;
+    const char* a_route = "tma";  // B200RNN_DEBUG: where the fp32 A operand comes from
     if (tc_layer) {
       float* a_dense = tc_a_hi(tc_ws);
       if (l == 0 && ln_gamma) {
@@ -847,10 +850,12 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         rc = tc_layernorm(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, out, st, ready, tiles_m, lengths, d.B);
         a_in = out;
         a_rows = simple_rows(Il);
+        a_route = "ln";
       } else if (!tc_a_f32_in_place(in, in_rows, (int)d.TB, Il)) {
         rc = tc_gather_rows(in, in_rows, (int)d.TB, Il, a_dense, st, ready, tiles_m);
         a_in = a_dense;
         a_rows = simple_rows(Il);
+        a_route = "gather";
       } else if (stream_xproj && !ready_zeroed) {
         B200_CUDA_CHECK(cudaMemsetAsync(ready, 0, tiles_m * sizeof(int), st));
       }
@@ -881,7 +886,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         // each direction's weight_ih checked on its own: one the TMA cannot read takes the FFMA GEMM
         if (n16 && tc_gemm_n16_ok(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il)) {
           rc = tc_gemm_n16(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il, dt, gates, simple_rows((long long)d.GH), b32,
-                           b32 + d.GH, b2n, st);
+                           b32 + d.GH, b2n, st, a16_route);
         } else {
           float* aw = S + sl.f_tc;
           float* ww = aw + align_up(d.TB * Il, ALIGN_F);
@@ -895,6 +900,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
           g.C = gates; g.c_rows = simple_rows((long long)d.GH);
           g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
           g.bias1 = b32; g.bias2 = b32 + d.GH; g.bias2_n = b2n;
+          g.a_route = "widen";
           rc = launch_gemm(g, nullptr, 0, st);
         }
         if (rc) return rc;
@@ -908,6 +914,7 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
         g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
         g.bias1 = b_ih; g.bias2 = b_hh;
         g.bias2_n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
+        g.a_route = a_route;
         if (tc_layer) {
           g.tc_ws = tc_ws;
           g.tc_ws_bytes = sl.f_tc_bytes;

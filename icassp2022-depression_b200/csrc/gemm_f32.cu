@@ -5,6 +5,9 @@
 // Rows may be two-level strided (RowMap) so batch_first / permuted inputs are read in place.
 // fp32 FFMA on purpose: the reference path is fp32 (torch rnn.py:1221-1224, :842-847) and parity is
 // judged at 1e-5; the dense shapes go to the 3xTF32 tensor-core kernel (gemm_tc.cu), this one takes the rest.
+#include <stdlib.h>
+#include <string.h>
+
 #include "gemm_f32.cuh"
 #include "profile.cuh"
 
@@ -301,6 +304,12 @@ int launch_gemm(const GemmParams& p, void* scratch, size_t scratch_bytes, cudaSt
   d.accumulate = p.accumulate;
   d.a_vec = rows_vec_ok(p.A, p.a_rows);
   d.b_vec = rows_vec_ok(p.B, p.b_rows);
+  static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
+  // the forward input projection on this GEMM: A read through its row map ("rows"), or a dense copy of it. Its own
+  // line: "forward x-projection" names the tensor-core projections
+  if (debug && p.a_route)
+    fprintf(stderr, "[b200rnn] ffma x-projection: M=%d N=%d K=%d a=%s loads=%s\n", p.M, p.N, p.K,
+            strcmp(p.a_route, "tma") ? p.a_route : "rows", d.a_vec ? "vec4" : "scalar");
   Plan pl = make_plan(p.M, p.N, p.K > 0 ? p.K : 1, scratch_bytes, scratch != nullptr);
   d.splitk = pl.splitk;
   d.k_chunk = pl.k_chunk;

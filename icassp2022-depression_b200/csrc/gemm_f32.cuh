@@ -41,6 +41,10 @@ struct GemmParams {
   // (gemm_h16_layout.cuh, b200rnn_prepare_weights); else the call splits W into its workspace.
   int tc_h16;
   const void* tc_b_h16;
+  // the forward input projection only (else NULL): where its A operand comes from, named on the B200RNN_DEBUG line.
+  // "tma" (read in place through a_rows), "gather" (dense copy), "ln" (the LayerNorm prologue's output), "widen" (fp32
+  // copy of a 16-bit operand). Host side only.
+  const char* a_route;
 };
 
 // where launch_gemm_tc puts the split A operand inside its workspace (tc_a_hi: also room for a dense fp32 [M][K] A)

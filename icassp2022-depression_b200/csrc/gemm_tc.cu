@@ -1394,9 +1394,9 @@ int launch_gemm_tc(const GemmParams& p, void* ws, size_t ws_bytes, cudaStream_t 
   // into the room of the TF32 W split; a shape it does not take runs the 3xTF32 fp32-A kernel
   const bool h16 = p.tc_h16 && p.tc_a_f32 && p.b_kcontig && !tf32 && g16::shape_ok(p.N, p.K);
   if (debug && p.tc_a_f32)
-    fprintf(stderr, "[b200rnn] forward x-projection: M=%d N=%d K=%d math=%s weights=%s\n", p.M, p.N, p.K,
+    fprintf(stderr, "[b200rnn] forward x-projection: M=%d N=%d K=%d math=%s weights=%s a=%s\n", p.M, p.N, p.K,
             h16 ? "f16x3" : tf32 ? "tf32" : "3xtf32",
-            (h16 ? p.tc_b_h16 != nullptr : b_hi != nullptr) ? "cached" : "split");
+            (h16 ? p.tc_b_h16 != nullptr : b_hi != nullptr) ? "cached" : "split", p.a_route ? p.a_route : "tma");
   if (h16) {
     const void* w16 = p.tc_b_h16;
     if (!w16) {
@@ -1434,7 +1434,8 @@ bool tc_gemm_n16_ok(const void* A, const RowMap& a_rows, const void* W, int M, i
 }
 
 int tc_gemm_n16(const void* A, const RowMap& a_rows, const void* W, int M, int N, int K, int dt, float* C,
-                const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream) {
+                const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
+                const char* a_route) {
   int rc = check_tc_shape(M, N, K, C, c_rows, nullptr, false, 0);
   if (rc) return rc;
   CUtensorMap m[4] = {};
@@ -1446,8 +1447,8 @@ int tc_gemm_n16(const void* A, const RowMap& a_rows, const void* W, int M, int N
   }
   static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
   if (debug)
-    fprintf(stderr, "[b200rnn] forward x-projection: M=%d N=%d K=%d math=%s weights=native\n", M, N, K,
-            dt == DT_BF16 ? "bf16" : "f16");
+    fprintf(stderr, "[b200rnn] forward x-projection: M=%d N=%d K=%d math=%s weights=native a=%s\n", M, N, K,
+            dt == DT_BF16 ? "bf16" : "f16", a_route ? a_route : "tma");
   TcArgs a = tc_args(M, N, K, C, c_rows, bias1, bias2, bias2_n, 0, nullptr);
   a.a_f32 = 1;  // one thread issues the A and W boxes
   a.a_inner = inner;

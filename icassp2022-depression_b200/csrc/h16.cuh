@@ -42,7 +42,10 @@ int launch_copy16(const void* src, const RowMap& rows, int R, int C, void* dst, 
 // the operands' alignment allow it (N % 128 == 0, K % 8 == 0, 16-byte aligned rows; A's rows as tc_a_f32_in_place
 // requires of an fp32 A).
 bool tc_gemm_n16_ok(const void* A, const RowMap& a_rows, const void* W, int M, int N, int K);
+// a_route: where A comes from ("tma": the caller's tensor or the previous layer's output, "copy16": a dense copy of x),
+// named on the B200RNN_DEBUG line
 int tc_gemm_n16(const void* A, const RowMap& a_rows, const void* W, int M, int N, int K, int dt, float* C,
-                const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream);
+                const RowMap& c_rows, const float* bias1, const float* bias2, int bias2_n, cudaStream_t stream,
+                const char* a_route = "tma");
 
 }  // namespace b200rnn

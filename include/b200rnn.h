@@ -166,7 +166,10 @@ B200RNN_API int b200rnn_forward(const b200rnn_desc* desc, const float* x, int64_
  * Forward with the model-shell fusions around the encoder (SURVEY.md 8f rank 1), used by the audio branch
  * `x = self.ln(x); x, _ = self.lstm_net_audio(x); x = x.sum(dim=1)` of fuse_net_whole.py:360-362:
  *   ln_gamma/ln_beta/ln_eps : LayerNorm over the feature dimension applied to x on the fly (folded into the operand
- *                             preparation of the layer-0 input projection); NULL = no LayerNorm
+ *                             preparation of the layer-0 input projection); NULL = no LayerNorm. It reads x in place
+ *                             and needs x, ln_gamma and ln_beta 16-byte aligned and x_stride_t, x_stride_b multiples of
+ *                             4: any other x returns B200RNN_ERR_UNSUPPORTED ("needs 16-byte aligned rows"); pass a
+ *                             dense copy of such an x (b200rnn.functional does)
  *   y_pool                  : optional [B, D*H] = sum over time of the top layer's output; with y == NULL the
  *                             [T,B,D*H] output is never written (only allowed without B200RNN_FLAG_SAVE_FOR_BACKWARD)
  *   lengths                 : optional DEVICE array [B] of valid step counts (torch PackedSequence semantics on the
@@ -260,6 +263,9 @@ B200RNN_API int b200rnn_backward_hx(const b200rnn_desc* desc, const float* x, in
  *   ln_gamma / ln_eps       : with B200RNN_FLAG_FUSED_LN: the layer-0 input gradient is d/dLN(x); it is pushed through
  *                             the LayerNorm backward (statistics recomputed from x) into dx, and
  *   dln_gamma / dln_beta    : (+)= the LayerNorm parameter gradients (NULL to skip), per B200RNN_FLAG_ACCUMULATE_GRADS
+ * The LayerNorm backward reads x and writes dx in place with 16-byte accesses: x, dx and ln_gamma must be 16-byte
+ * aligned and x_stride_t, x_stride_b, dx_stride_t and dx_stride_b multiples of 4, else the call returns
+ * B200RNN_ERR_UNSUPPORTED.
  */
 B200RNN_API int b200rnn_backward_fused(const b200rnn_desc* desc, const float* x, int64_t x_stride_t,
                                        int64_t x_stride_b, const float* const* params, const float* y,

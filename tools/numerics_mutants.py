@@ -1,7 +1,8 @@
 """Do the numerics tests bite? Build the library with one small arithmetic mutation at a time and run the tests on it.
 
-Each mutation is one textual edit of csrc/ that changes arithmetic only or removes a data store - never an index, a
-barrier, a flag or a counter, so that no mutated build can fault or hang - and is applied to a copy of the sources; that
+Each mutation is one textual edit of csrc/ that changes arithmetic only or removes a data store - never a barrier, a
+flag or a counter, and an index only where no test it runs can then reach outside its allocation (the strided-layout
+mutations, each with its reason), so that no mutated build can fault or hang - and is applied to a copy of the sources; that
 copy is built (make, as build() does, reusing the tree's objects so that only the mutated file recompiles) and loaded with B200RNN_LIB. Each mutation names the new tests that must catch it and the
 existing tests it is also run against. Against each build the script runs the new tests (stopping after a few
 failures) and then the existing files in order, each until its first failure, stopping at the first file that fails;
@@ -41,6 +42,11 @@ ANYH_NEW = ["tests/test_gpu_anyh_numerics_f64.py", "tests/test_gpu_poisoned_buff
 ANYH_EXISTING = ["tests/test_gpu_any_hidden.py", "tests/test_gpu_elman.py", "tests/test_gpu_varlen_sorted.py"]
 CELL_NEW = ["tests/test_gpu_anyh_numerics_f64.py::test_cell_backward_off_default_init_vs_f64"]
 CELL_EXISTING = ["tests/test_gpu_cells.py", "tests/test_gpu_elman.py"]
+# caller-laid-out sequence tensors. These mutations change which element an access reaches, never whether it is a
+# vector or a scalar access. Each note says why the mutated access stays inside the caller's allocation for every test
+# in its lists (five of them inside the span of any view, whatever holds it), not only for the tests a run with
+# --new-maxfail happens to reach
+STRIDED_NEW = ["tests/test_gpu_strided_io.py"]
 # tf32(v): v with its 13 low mantissa bits cleared, the operand precision of a single-pass TF32 product
 _TF32 = "__uint_as_float(__float_as_uint({}) & 0xffffe000u)"
 
@@ -176,6 +182,56 @@ MUTATIONS = {
                                 "__uint_as_float(__float_as_uint(dh) & 0xffffff00u), relu);\n",
                                 "RNNCell backward: the output gradient loses its 8 low mantissa bits", CELL_NEW,
                                 CELL_EXISTING[1:]),
+    # make_a16_map has the same line first. In bounds: the outer stride only ever gets smaller, so every box starts
+    # inside the view's footprint
+    "a_f32_map_drop_time_gap": ("gemm_tc.cu",
+                                "  const long long si = rows.s_inner, so = dense ? (long long)M * rows.s_inner : "
+                                "rows.s_outer;\n",
+                                "  const long long si = rows.s_inner, so = dense ? (long long)M * rows.s_inner : "
+                                "(rows.s_outer < ni * rows.s_inner ? rows.s_outer : ni * rows.s_inner);\n",
+                                "fp32 input projection read in place: the 3-D map's outer (time) stride ignores a gap "
+                                "between steps", STRIDED_NEW, ["tests/test_gpu_gemm_f32a.py", "tests/test_gpu_parity.py"],
+                                1),
+    # dense_vec's s_outer == inner_n * C term loosened to >=, on the widening's source: a time gap is taken for dense.
+    # In bounds for any view without overlapping rows: the vector path reads R * C elements from its base, and such a
+    # view spans at least that many
+    "widen16_src_outer_ignored": ("h16.cu",
+                                  "  const bool vec = dense_vec(rows, simple_rows(C), R, C, src, dst, nullptr);\n",
+                                  "  const bool vec = dense_vec(rows.s_outer >= (long long)rows.inner_n * C ? "
+                                  "RowMap{0, rows.s_inner, 0x7fffffff} : rows, simple_rows(C), R, C, src, dst, "
+                                  "nullptr);\n",
+                                  "widen16: a 16-bit x / dy with gaps between its steps is taken for dense", STRIDED_NEW,
+                                  ["tests/test_gpu_h16_modules.py"]),
+    # the same on the narrowing's destination: R * C elements written from the base of a y / dx that spans them
+    "narrow16_dst_outer_ignored": ("h16.cu",
+                                   "  const bool vec = dense_vec(dst_rows, src_rows, R, C, dst, src, wb);\n",
+                                   "  const bool vec = dense_vec(dst_rows.s_outer >= (long long)dst_rows.inner_n * C ? "
+                                   "RowMap{0, dst_rows.s_inner, 0x7fffffff} : dst_rows, src_rows, R, C, dst, src, "
+                                   "wb);\n",
+                                   "narrow16: a 16-bit y / dx with gaps between its steps is written as dense",
+                                   STRIDED_NEW, ["tests/test_gpu_h16_modules.py"]),
+    # The two below clamp a stride to at most its true value, so each access lands at or below the address the correct
+    # code reaches in the same view: in bounds for any caller's tensor, whatever its storage.
+    "rec_fwd_y_dense_rows": ("rnn_rec.cu",
+                             "      if (p.y) p.y[(long long)t * p.y_st + (long long)b * p.y_sb + dir * H + j] = pend_y;\n",
+                             "      if (p.y) p.y[(long long)t * p.y_st + (long long)b * (p.y_sb < p.D * H ? p.y_sb : p.D * H) "
+                             "+ dir * H + j] = pend_y;\n",
+                             "fixed-config forward recurrence: y's batch stride clamped to D * H (dense rows)", STRIDED_NEW,
+                             ["tests/test_gpu_parity.py"]),
+    "rec_bwd_dy_dense_rows": ("rnn_rec.cu",
+                              "    dyv = p.dy ? p.dy[(long long)t * p.dy_st + (long long)b * p.dy_sb + dir * H + j] : "
+                              "dy_pooled;\n",
+                              "    dyv = p.dy ? p.dy[(long long)t * p.dy_st + (long long)b * (p.dy_sb < p.D * H ? p.dy_sb : "
+                              "p.D * H) + dir * H + j] : dy_pooled;\n",
+                              "fixed-config BPTT: dy's batch stride clamped to D * H (dense rows)", STRIDED_NEW,
+                              ["tests/test_gpu_parity.py"]),
+    # Reads the T * B * C elements from x's base, which not every tensor holds (an expanded x does not). Safe for the
+    # tests it runs: the only ragged x of test_gpu_strided_io.py are compare(..., ragged=True)'s backed views, whose
+    # buffers cover that dense footprint (backing), and test_gpu_varlen.py passes dense padded tensors only.
+    "valid_rows_dense_src": ("misc_kernels.cu", "    dst[i] = t < lengths[b] ? src[rows.off(r) + c] : 0.f;\n",
+                             "    dst[i] = t < lengths[b] ? src[(size_t)r * C + c] : 0.f;\n",
+                             "ragged backward: the padding-zeroed copy of x reads row r at r * C, ignoring x's strides",
+                             STRIDED_NEW, ["tests/test_gpu_varlen.py"]),
 }
 
 

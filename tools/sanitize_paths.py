@@ -4,6 +4,7 @@
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py rnn   # recurrence only
 The GRU H=256 layer also runs at B = 96, which needs the 4-row clusters (bs4: the 2-row ones do not all fit at once).
     compute-sanitizer --tool memcheck python tools/sanitize_paths.py cells # GRUCell / LSTMCell forward + backward only
+    compute-sanitizer --tool memcheck python tools/sanitize_paths.py strided # caller-laid-out x / dy / y / dx
     compute-sanitizer --tool racecheck python tools/sanitize_paths.py anyh # runtime-sized recurrence (rnn_anyh.cu) only:
         GRU H = 192 (W_hh in shared memory) and LSTM H = 768 (W_hh from L2), fixed-length and ragged, with hx and dh_0
 """
@@ -29,6 +30,13 @@ if sys.argv[1:] == ["anyh"]:
         torch.cuda.synchronize()
         print(kind, H, "ok", flush=True)
     sys.exit(0)
+if sys.argv[1:] == ["strided"]:
+    # the whole layout matrix of tests/test_gpu_strided_io.py (offset, gapped, broadcast and size-1 x, dy, y and dx;
+    # both batch_first settings, the _hx and _fused C ABI pairs, autocast, hx, ragged, the LayerNorm fold), in this
+    # process; test_routes only re-runs the catalogue's forwards in a child process to read their debug lines
+    import pytest
+    sys.exit(pytest.main(["-q", "-p", "no:cacheprovider", "-x", os.path.join(ROOT, "tests", "test_gpu_strided_io.py"),
+                          "-k", "not test_routes"]))
 if sys.argv[1:] == ["cells"]:
     # K and batch tails, unaligned rows (odd offsets into larger buffers), no bias, no state, both contractions
     for kind, I, H, B, bias in (("gru", 3, 5, 7, True), ("lstm", 257, 129, 9, False), ("gru", 256, 256, 130, False),
