@@ -24,6 +24,7 @@ FLAG_NO_BIAS = 32   # cells only: bias=False
 FLAG_F16 = 64       # x, parameters, states, outputs and gradients are float16 (the reserve and scratch stay fp32)
 FLAG_BF16 = 128     # ... bfloat16
 FLAG_F32_PARAMS = 256  # with FLAG_F16 / _BF16: the parameters and their gradient targets are fp32 (autocast)
+FLAG_MODELS = 512   # the descriptor carries models / model_strides: M models of one shape in one call (torch.func.vmap)
 ABI_VERSION = 4
 
 # every symbol include/b200rnn.h declares (tests check the .so exports exactly these)
@@ -69,8 +70,9 @@ IPC_HANDLE_BYTES = 64
 
 
 class Desc(ctypes.Structure):
-    """``b200rnn_desc`` (include/b200rnn.h). ``proj_size`` is last and read only with ``FLAG_PROJ``: positional
-    construction with the first ten fields means "no projection"."""
+    """``b200rnn_desc`` (include/b200rnn.h). ``proj_size`` is read only with ``FLAG_PROJ``, ``models`` and
+    ``model_strides`` only with ``FLAG_MODELS``: positional construction with the first ten fields means "no projection,
+    one model"."""
 
     _fields_ = [
         ("mode", c_int32),
@@ -84,6 +86,8 @@ class Desc(ctypes.Structure):
         ("dropout_p", c_float),
         ("flags", c_uint32),
         ("proj_size", c_int32),
+        ("models", c_int32),                          # read only with FLAG_MODELS
+        ("model_strides", POINTER(c_int64)),  # ... [x, rng_state, params...] in elements, 0 = shared
     ]
 
 

@@ -32,6 +32,12 @@ class RNNConfig:
     # fp32 master parameters of a 16-bit call (torch.autocast, FLAG_F32_PARAMS): the parameters and their gradients
     # are float32, everything else is ``dtype``; computes what the 16-bit module computes on the rounded parameters
     master_f32: bool = False
+    # M > 1: one call runs M models (torch.func.vmap, b200rnn.func): x [M,T,B,I] (or [M,B,T,I]), every parameter
+    # [M, ...] (model stride 0 = shared), h_0 / c_0 and every output and gradient dense [M, ...]
+    models: int = 1
+    # with models > 1, the model stride of rng_state: 2 = one row per model, 0 = one state and one mask for every
+    # model, -1 = one state drawn by the models as consecutive calls would draw it
+    rng_stride: int = 0
 
     @property
     def out_size(self) -> int:
@@ -104,7 +110,9 @@ def _ln_operands(x_tm: torch.Tensor, ln_w: Optional[torch.Tensor], ln_b: Optiona
 
 
 def _make_desc(cfg: RNNConfig, B: int, T: int, save: bool, accumulate: bool = False,
-               fused_ln: bool = False) -> _lib.Desc:
+               fused_ln: bool = False, model_strides: Optional[Sequence[int]] = None) -> _lib.Desc:
+    """``model_strides`` (``cfg.models > 1``): of x, rng_state and each parameter, in elements (zeros when None: the
+    workspace sizes do not depend on them)"""
     flags = 0
     if save:
         flags |= _lib.FLAG_SAVE_FOR_BACKWARD
@@ -119,8 +127,23 @@ def _make_desc(cfg: RNNConfig, B: int, T: int, save: bool, accumulate: bool = Fa
     flags |= _lib.H16_DTYPES.get(str(cfg.dtype), 0)
     if cfg.master_f32:
         flags |= _lib.FLAG_F32_PARAMS
-    return _lib.Desc(cfg.mode, B, T, cfg.input_size, cfg.hidden_size, cfg.num_layers, cfg.num_dirs,
+    desc = _lib.Desc(cfg.mode, B, T, cfg.input_size, cfg.hidden_size, cfg.num_layers, cfg.num_dirs,
                      1 if cfg.training else 0, float(cfg.dropout), flags, cfg.proj_size)
+    if cfg.models > 1:
+        n = 2 + 4 * cfg.num_layers * cfg.num_dirs
+        strides = (ctypes.c_int64 * n)(*(model_strides if model_strides is not None else [0] * n))
+        desc.flags |= _lib.FLAG_MODELS
+        desc.models = cfg.models
+        desc.model_strides = ctypes.cast(strides, ctypes.POINTER(ctypes.c_int64))
+        desc.keepalive = strides   # the library reads the array during the call
+    return desc
+
+
+def _model_strides(cfg: RNNConfig, x_tm: torch.Tensor, weights: Sequence[torch.Tensor]) -> Optional[list]:
+    """the model strides of a ``cfg.models > 1`` call: x, rng_state, each parameter (None for one model)"""
+    if cfg.models == 1:
+        return None
+    return [x_tm.stride(0), cfg.rng_stride, *(w.stride(0) for w in weights)]
 
 
 def _stream_ptr(device=None) -> int:
@@ -159,31 +182,34 @@ def _weight_grad_targets(weights, needed, sink, dev, separate: bool = False):
 
 
 def _weight_grad_buffers(weights, needed):
-    """one fresh gradient tensor per weight that wants one (None otherwise); the weights are contiguous"""
-    return [torch.empty_like(w) if n else None for w, n in zip(weights, needed)]
+    """one fresh dense gradient tensor per weight that wants one (None otherwise)"""
+    return [torch.empty(w.shape, dtype=w.dtype, device=w.device) if n else None for w, n in zip(weights, needed)]
 
 
-def _forward_buffers(x_tm: torch.Tensor, cfg: RNNConfig, save: bool, with_scratch: bool = True):
+def _forward_buffers(x_tm: torch.Tensor, cfg: RNNConfig, save: bool, with_scratch: bool = True,
+                     model_strides: Optional[Sequence[int]] = None):
     """Descriptor and the buffers of one sequence forward, as ``(desc, reserve, scratch, y, (ys_t, ys_b), h_n, c_n)``:
     ``y`` batch-first or time-major as ``cfg`` says, ``c_n`` None but for the LSTM, the reserve empty without ``save``.
     Host arithmetic only (``b200rnn_workspace_bytes``), so the custom ops' fake implementations call it too, without
-    the scratch."""
-    T, B, _ = x_tm.shape
+    the scratch. With ``cfg.models`` = M > 1 every buffer has a leading [M] dimension (the reserve: M one-model blocks)."""
+    T, B = x_tm.shape[-3], x_tm.shape[-2]
     H, L, D, HO = cfg.hidden_size, cfg.num_layers, cfg.num_dirs, cfg.out_size
     dev = x_tm.device
-    desc = _make_desc(cfg, B, T, save)
+    M = cfg.models
+    lead = (M,) if M > 1 else ()
+    desc = _make_desc(cfg, B, T, save, model_strides=model_strides)
     rbytes, sbytes = _lib.workspace_bytes(desc)
-    reserve = torch.empty(rbytes if save else 0, dtype=torch.uint8, device=dev)
+    reserve = torch.empty(*lead, rbytes // M if save else 0, dtype=torch.uint8, device=dev)
     scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev) if with_scratch else None
     dt = cfg.dtype
     if cfg.batch_first:
-        y = torch.empty(B, T, D * HO, dtype=dt, device=dev)
+        y = torch.empty(*lead, B, T, D * HO, dtype=dt, device=dev)
         ys = (D * HO, T * D * HO)
     else:
-        y = torch.empty(T, B, D * HO, dtype=dt, device=dev)
+        y = torch.empty(*lead, T, B, D * HO, dtype=dt, device=dev)
         ys = (B * D * HO, D * HO)
-    h_n = torch.empty(L * D, B, HO, dtype=dt, device=dev)
-    c_n = torch.empty(L * D, B, H, dtype=dt, device=dev) if cfg.mode == _lib.LSTM else None
+    h_n = torch.empty(*lead, L * D, B, HO, dtype=dt, device=dev)
+    c_n = torch.empty(*lead, L * D, B, H, dtype=dt, device=dev) if cfg.mode == _lib.LSTM else None
     return desc, reserve, scratch, y, ys, h_n, c_n
 
 
@@ -193,9 +219,10 @@ def _rnn_forward_impl(x_tm: torch.Tensor, cfg: RNNConfig, rng_state: Optional[to
     """The sequence forward (one ``b200rnn_forward_hx`` call) shared by :class:`_RNNFunction` and the
     ``b200rnn::rnn_forward`` op: returns ``(y, h_n, c_n, reserve)``, ``c_n`` None but for the LSTM."""
     lib = _lib.load()
-    T, B, _ = x_tm.shape
+    T, B = x_tm.shape[-3], x_tm.shape[-2]
     dev = x_tm.device
-    desc, reserve, scratch, y, (ys_t, ys_b), h_n, c_n = _forward_buffers(x_tm, cfg, save)
+    desc, reserve, scratch, y, (ys_t, ys_b), h_n, c_n = _forward_buffers(x_tm, cfg, save,
+                                                                         model_strides=_model_strides(cfg, x_tm, weights))
     params = _lib.ptr_array([w.data_ptr() for w in weights])
     rng_ptr = rng_state.data_ptr() if rng_state is not None else None
     len_ptr = lengths.data_ptr() if lengths is not None else None
@@ -205,7 +232,7 @@ def _rnn_forward_impl(x_tm: torch.Tensor, cfg: RNNConfig, rng_state: Optional[to
         # rnn_forward_fused / rnn_ln_pool_sum (its no-grad GRU-256 recurrence runs on fp16 pairs)
         with _on(dev):
             rc = lib.b200rnn_forward_hx(
-                ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+                ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(-3), x_tm.stride(-2), params,
                 y.data_ptr(), ys_t, ys_b, h_0.data_ptr() if h_0 is not None else None,
                 c_0.data_ptr() if c_0 is not None else None,
                 h_n.data_ptr(), c_n_ptr, reserve.data_ptr() if save else None, scratch.data_ptr(),
@@ -219,7 +246,10 @@ def _rnn_forward_impl(x_tm: torch.Tensor, cfg: RNNConfig, rng_state: Optional[to
 
 
 def _dx_buffer(x_tm: torch.Tensor) -> torch.Tensor:
-    """the input gradient: laid out like ``x_tm`` when its feature stride is 1, else dense time-major"""
+    """the input gradient: laid out like ``x_tm`` when its feature stride is 1, else dense time-major; several models
+    ([M,T,B,I]): dense"""
+    if x_tm.dim() == 4:
+        return torch.empty(x_tm.shape, dtype=x_tm.dtype, device=x_tm.device)
     dx = torch.empty_like(x_tm)
     if dx.stride(2) != 1 and dx.size(2) != 1:
         dx = torch.empty(x_tm.shape, dtype=x_tm.dtype, device=x_tm.device)
@@ -232,7 +262,7 @@ def _rnn_backward_impl(cfg: RNNConfig, x_tm, y, reserve, h_0, c_0, weights, dy, 
     returns ``(dx, dh_0, dc_0, weight grads)``, None for every gradient that is not wanted (a NULL pointer to the
     library). ``grad_sink`` / ``separate``: see :func:`_weight_grad_targets`."""
     lib = _lib.load()
-    T, B, _ = x_tm.shape
+    T, B = x_tm.shape[-3], x_tm.shape[-2]
     dev = x_tm.device
     if cfg.batch_first:
         ys_t, ys_b = cfg.num_dirs * cfg.out_size, T * cfg.num_dirs * cfg.out_size
@@ -244,12 +274,12 @@ def _rnn_backward_impl(cfg: RNNConfig, x_tm, y, reserve, h_0, c_0, weights, dy, 
 
     if dy is None:
         dy = torch.zeros_like(y)
-    if dy.stride(2) != 1 and dy.size(2) != 1:
+    if (dy.stride(-1) != 1 and dy.size(-1) != 1) or cfg.models > 1:   # several models: dense per model
         dy = dy.contiguous()
     if cfg.batch_first:
-        dys_t, dys_b = dy.stride(1), dy.stride(0)
+        dys_t, dys_b = dy.stride(-2), dy.stride(-3)
     else:
-        dys_t, dys_b = dy.stride(0), dy.stride(1)
+        dys_t, dys_b = dy.stride(-3), dy.stride(-2)
     if dh_n is not None:
         dh_n = dh_n.contiguous()
     if dc_n is not None:
@@ -258,7 +288,7 @@ def _rnn_backward_impl(cfg: RNNConfig, x_tm, y, reserve, h_0, c_0, weights, dy, 
     dx = _dx_buffer(x_tm) if need_dx else None
 
     dptrs, grads_out, accumulate = _weight_grad_targets(weights, need_w, grad_sink, dev, separate)
-    desc = _make_desc(cfg, B, T, True, accumulate)
+    desc = _make_desc(cfg, B, T, True, accumulate, model_strides=_model_strides(cfg, x_tm, weights))
     _, sbytes = _lib.workspace_bytes(desc)
     scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
     params = _lib.ptr_array([w.data_ptr() for w in weights])
@@ -266,10 +296,10 @@ def _rnn_backward_impl(cfg: RNNConfig, x_tm, y, reserve, h_0, c_0, weights, dy, 
     ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
     if B > 0 and T > 0:
         with _on(dev):
-            head = (ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params,
+            head = (ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(-3), x_tm.stride(-2), params,
                     y.data_ptr(), ys_t, ys_b, dy.data_ptr(), dys_t, dys_b, ptr(dh_n), ptr(dc_n))
             tail = (reserve.data_ptr(), scratch.data_ptr(), ptr(dx),
-                    dx.stride(0) if dx is not None else 0, dx.stride(1) if dx is not None else 0,
+                    dx.stride(-3) if dx is not None else 0, dx.stride(-2) if dx is not None else 0,
                     dparams, ptr(lengths), _stream_ptr(dev))
             if h_0 is None and not cfg.proj_size:
                 rc = lib.b200rnn_backward(*head, *tail)
@@ -488,7 +518,16 @@ def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig
         if grad_sink is not None:
             _grad_sink_untraceable()
         return _ops.rnn_forward_traced(x_tm, cfg, rng_state, lengths, save, h_0, c_0, weights)
+    if functorch_active():   # torch.func.grad / vmap: wrapped tensors have no pointer (b200rnn/func.py)
+        _func.check_supported(cfg, lengths, grad_sink)
+        return _func.rnn_forward(x_tm, cfg, rng_state, save, h_0, c_0, weights)
     return _RNNFunction.apply(x_tm, cfg, rng_state, grad_sink, lengths, save, h_0, c_0, *weights)
+
+
+def functorch_active() -> bool:
+    """Whether a torch.func transform (vmap, grad, ...) is running: its tensors have no data pointer, so the fused
+    model-shell paths, which hand pointers to the library directly, are not taken"""
+    return torch._C._are_functorch_transforms_active()
 
 
 @torch.no_grad()
@@ -751,5 +790,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_kcontig: bool = True, b_kcontig:
     return out
 
 
-# the custom ops (b200rnn/ops.py) wrap the helpers above; imported last because they import this module
+# the custom ops (b200rnn/ops.py) and the torch.func path (b200rnn/func.py) wrap the helpers above; imported last
+# because they import this module
+from . import func as _func  # noqa: E402
 from . import ops as _ops  # noqa: E402

@@ -41,8 +41,9 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .functional import (CellConfig, RNNConfig, cell_forward, prepare_weights, rnn_forward, rnn_forward_fused,
-                         rnn_ln_pool_sum, tf32_enabled)
+from .func import check_supported
+from .functional import (CellConfig, RNNConfig, cell_forward, functorch_active, prepare_weights, rnn_forward,
+                         rnn_forward_fused, rnn_ln_pool_sum, tf32_enabled)
 
 _TORCH_GRU = nn.GRU
 _TORCH_LSTM = nn.LSTM
@@ -218,6 +219,8 @@ class _B200RNNBase(nn.Module):
         """PackedSequence path (ragged DAIC-style sequences): pad, run with per-sequence lengths, re-pack exactly like
         torch (same batch_sizes / sorted_indices; hx, h_n and c_n in the caller's original batch order: the padded
         batch is in that order already)."""
+        if functorch_active():   # raised before torch's unpacking, which cannot run under torch.func either
+            check_supported(cfg, packed.batch_sizes, self._grad_sink)
         rnn_utils = nn.utils.rnn
         padded, lengths = rnn_utils.pad_packed_sequence(packed, batch_first=self.batch_first)
         out = rnn_forward(padded, self._flat_weights, cfg, self._rng_state, self._grad_sink, lengths=lengths, hx=hx)
@@ -287,8 +290,9 @@ class _B200RNNBase(nn.Module):
         need_grad = torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
         # torch.compile / torch.export trace the unfused expression through the custom ops (b200rnn/ops.py), and so does
-        # a call under torch.autocast (the fusions are fp32 only)
-        shape_ok = (not torch.compiler.is_compiling() and self._autocast_dtype() is None and input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
+        # a call under torch.autocast (the fusions are fp32 only); torch.func transforms compute it through b200rnn/func.py
+        shape_ok = (not torch.compiler.is_compiling() and not functorch_active() and self._autocast_dtype() is None and
+                    input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
                     self._gates > 1 and self._flat_weights[0].dtype == torch.float32 and
                     self.hidden_size in (128, 256) and
                     (ln is None or (self.input_size in (128, 256, 512, 1024) and ln.elementwise_affine and

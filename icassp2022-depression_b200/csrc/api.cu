@@ -39,11 +39,17 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 // proj_size of a descriptor: the field exists only when B200RNN_FLAG_PROJ says so (a descriptor may end at `flags`)
 inline int desc_proj(const b200rnn_desc* d) { return (d->flags & B200RNN_FLAG_PROJ) ? d->proj_size : 0; }
+// the model count, read only under B200RNN_FLAG_MODELS
+inline int desc_models(const b200rnn_desc* d) { return (d->flags & B200RNN_FLAG_MODELS) ? d->models : 1; }
 
 // The model-shell entry points (b200rnn_forward_fused, _backward_fused, _prepare_weights, _wcache_bytes) run only the
 // GRU / LSTM at the fixed hidden sizes 128 and 256: their fusions (LayerNorm prologue, pooling, weight cache, the
 // fp16-pair no-grad recurrence) are built for those
 int check_shell_desc(const b200rnn_desc* d, const char* what) {
+  if (d && desc_models(d) != 1) {
+    set_error("%s: the model-shell entry points run one model (use the _hx entry points for several)", what);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   if (d && (d->flags & (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_F32_PARAMS))) {
     set_error("%s: the model-shell entry points and the weight cache are float32 only (use the _hx entry points for "
               "16-bit tensors)", what);
@@ -70,6 +76,8 @@ struct Dims {
   float p;
   int dt;  // DT_F32, or DT_F16 / DT_BF16: the caller's tensors are 16-bit (B200RNN_FLAG_F16 / _BF16)
   bool master;  // B200RNN_FLAG_F32_PARAMS: the parameters and their gradients are fp32 (the rest is 16-bit)
+  int M;        // models (B200RNN_FLAG_MODELS), 1 without the flag
+  const int64_t* ms;  // with M > 1: the caller's model strides (x, rng_state, params[i])
 };
 
 int check_desc(const b200rnn_desc* d, Dims* o) {
@@ -123,6 +131,21 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
     set_error("dropout_p must be in [0,1] (got %f)", (double)d->dropout_p);
     return B200RNN_ERR_INVALID;
   }
+  const int M = desc_models(d);
+  if (M < 1) {
+    set_error("models must be >= 1 (got %d)", M);
+    return B200RNN_ERR_INVALID;
+  }
+  if (M > 1 && !d->model_strides) {
+    set_error("models %d without model_strides", M);
+    return B200RNN_ERR_INVALID;
+  }
+  if (M > 1 && (P > 0 || h16 || master ||
+                (d->flags & (B200RNN_FLAG_FUSED_LN | B200RNN_FLAG_ACCUMULATE_GRADS)))) {
+    set_error("models %d: several models in one call are float32 only, without proj_size, the fused LayerNorm or "
+              "B200RNN_FLAG_ACCUMULATE_GRADS", M);
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   o->mode = d->mode;
   o->B = d->batch;
   o->T = d->seq_len;
@@ -141,6 +164,8 @@ int check_desc(const b200rnn_desc* d, Dims* o) {
   o->p = d->dropout_p;
   o->dt = h16 == B200RNN_FLAG_F16 ? DT_F16 : h16 == B200RNN_FLAG_BF16 ? DT_BF16 : DT_F32;
   o->master = master;
+  o->M = M;
+  o->ms = M > 1 ? d->model_strides : nullptr;
   return B200RNN_OK;
 }
 
@@ -332,6 +357,29 @@ void make_scratch(const Dims& d, ScratchLayout* s) {
 
   s->order = s->f_total > s->b_total ? s->f_total : s->b_total;
   s->f_total = s->b_total = s->order + align_up((size_t)d.B, ALIGN_F);
+}
+
+// One model's reserve and scratch blocks (floats, multiples of ALIGN_F): what b200rnn_workspace_bytes returns for one
+// model; model m's blocks start at m times them
+void model_blocks(const Dims& d, bool fused_ln, size_t* rs, size_t* ss) {
+  ReserveLayout r;
+  make_reserve(d, &r, fused_ln);
+  ScratchLayout s;
+  make_scratch(d, &s);
+  size_t stotal = s.f_total > s.b_total ? s.f_total : s.b_total;
+  if (d.dt) {
+    H16Scratch h;
+    make_h16_scratch(d, stotal, &h);
+    stotal = h.total;
+  }
+  *rs = r.total + ALIGN_F;
+  *ss = stotal + ALIGN_F;
+}
+
+// Model m's parameter table: params[i] offset by m times its model stride (NULL stays NULL)
+void model_params(const Dims& d, const float* const* params, int m, const float** out) {
+  const int n = d.L * d.D * d.NPAR;
+  for (int i = 0; i < n; ++i) out[i] = params[i] ? params[i] + (m ? m * d.ms[2 + i] : 0) : nullptr;
 }
 
 // ---- weight cache layout (floats): per (layer, direction) the TF32 hi then lo split of weight_ih [G*H, I_l], then its
@@ -582,16 +630,10 @@ B200RNN_API int b200rnn_workspace_bytes(const b200rnn_desc* desc, size_t* reserv
   ReserveLayout r;
   rc = make_reserve(d, &r, (desc->flags & B200RNN_FLAG_FUSED_LN) != 0);
   if (rc) return rc;
-  ScratchLayout s;
-  make_scratch(d, &s);
-  size_t stotal = s.f_total > s.b_total ? s.f_total : s.b_total;
-  if (d.dt) {
-    H16Scratch h;
-    make_h16_scratch(d, stotal, &h);
-    stotal = h.total;
-  }
-  if (reserve_bytes) *reserve_bytes = (r.total + ALIGN_F) * sizeof(float);
-  if (scratch_bytes) *scratch_bytes = (stotal + ALIGN_F) * sizeof(float);
+  size_t rs, ss;
+  model_blocks(d, (desc->flags & B200RNN_FLAG_FUSED_LN) != 0, &rs, &ss);
+  if (reserve_bytes) *reserve_bytes = (size_t)d.M * rs * sizeof(float);
+  if (scratch_bytes) *scratch_bytes = (size_t)d.M * ss * sizeof(float);
   return B200RNN_OK;
 }
 
@@ -653,6 +695,10 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     set_error("forward: the model-shell entry takes no initial state");
     return B200RNN_ERR_INVALID;
   }
+  if (d.M > 1 && lengths) {
+    set_error("forward: several models in one call take no lengths (ragged batches run one model per call)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   cudaEvent_t prologue_ev = static_cast<cudaEvent_t>(prologue_done);
   if (d.B == 0 || d.T == 0) {
@@ -705,13 +751,29 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
   if (rc) return rc;
   ScratchLayout sl;
   make_scratch(d, &sl);
-  float* R = static_cast<float*>(reserve);
-  float* S = static_cast<float*>(scratch);
+  // model m's reserve and scratch blocks start at m * RS and m * SS (one model: R0 and S0 are the whole buffers)
+  float* const R0 = static_cast<float*>(reserve);
+  float* const S0 = static_cast<float*>(scratch);
+  size_t RS, SS;
+  model_blocks(d, fused_ln, &RS, &SS);
+  float* R = R0;
+  float* S = S0;
   const bool drop = d.training && d.p > 0.f && d.L > 1;
-  uint64_t* hdr = reinterpret_cast<uint64_t*>(save ? R : S);
+  // each model's dropout header {seed, offset} at the start of its block
+  auto model_hdr = [&](int m) { return reinterpret_cast<uint64_t*>(save ? R0 + m * RS : S0 + m * SS); };
+  uint64_t* hdr = model_hdr(0);
   if (drop || save) {
-    rc = launch_rng_setup(hdr, seed, offset, rng_state, drop ? (uint64_t)((d.TB * d.DH + 3) / 4) : 0, st);
-    if (rc) return rc;
+    // rng_state per model (stride > 0), or one shared state read by every model and advanced by model 0, which comes
+    // last: once (stride 0: every model draws the same masks) or M times (stride -1: model m draws what the m-th of M
+    // consecutive one-model calls would)
+    const int64_t rng_ms = d.M > 1 ? d.ms[1] : 0;
+    const uint64_t draw = drop ? (uint64_t)((d.TB * d.DH + 3) / 4) : 0;
+    for (int m = d.M - 1; m >= 0; --m) {
+      const uint64_t consume = rng_ms > 0 ? draw : m > 0 ? 0 : rng_ms < 0 ? d.M * draw : draw;
+      rc = launch_rng_setup(model_hdr(m), seed, offset, rng_state ? rng_state + m * (rng_ms > 0 ? rng_ms : 0) : nullptr,
+                            consume, st, rng_ms < 0 ? m * draw : 0);
+      if (rc) return rc;
+    }
   }
   int* order = nullptr;  // ragged batch: rows sorted into batch slots by length, shared by every layer
   if (lengths) {
@@ -779,38 +841,9 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
   int* ready = reinterpret_cast<int*>(S + sl.f_ready);
   const int tiles_m = (int)((d.TB + TC_TILE_M - 1) / TC_TILE_M);
   bool ready_zeroed = false;  // this layer's dropout pass zeroed the counters for the next layer
+  const float* pm[8 * 2 * 5];  // model m's parameter table
   for (int l = 0; l < d.L; ++l) {
     const int Il = l == 0 ? d.I : (int)d.DH;
-    // ---- layer input ---------------------------------------------------------------------------
-    const float* in;
-    RowMap in_rows;
-    if (l == 0) {
-      in = x;
-      in_rows = tb_rows(xs_t, xs_b, d.B);
-    } else {
-      if (save)
-        in = R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
-      else
-        in = S + sl.f_y[(l - 1) & 1];
-      in_rows = simple_rows((long long)d.DH);
-    }
-    const bool tc_layer = !dt && tc && (Il % 32 == 0) && (d.GH % 128 == 0);
-    // 16-bit: the A operand of the native input projection, read in place when the TMA can (else a dense copy)
-    const void* a16 = l == 0 ? static_cast<const void*>(x) : S + hs.a16;
-    RowMap a16_rows = l == 0 ? tb_rows(xs_t, xs_b, d.B) : simple_rows((long long)d.DH);
-    bool n16 = false;
-    const char* a16_route = "tma";  // B200RNN_DEBUG: where the 16-bit A operand comes from
-    if (dt) {
-      n16 = tc && tc_gemm_n16_ok(a16, a16_rows, params[(size_t)l * d.D * d.NPAR], (int)d.TB, (int)d.GH, Il);
-      if (!n16 && l == 0 && tc && tc_gemm_n16_ok(S + hs.a16, simple_rows(Il), params[0], (int)d.TB, (int)d.GH, Il)) {
-        rc = launch_copy16(x, a16_rows, (int)d.TB, Il, S + hs.a16, st);
-        if (rc) return rc;
-        a16 = S + hs.a16;
-        a16_rows = simple_rows(Il);
-        a16_route = "copy16";
-        n16 = true;
-      }
-    }
     // ---- the recurrence config, chosen before anything of the layer is enqueued
     RecFwdParams rp;
     memset(&rp, 0, sizeof(rp));
@@ -825,8 +858,9 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     if (WC && wl.has_whh16) rp.whh16[0] = WC + wl.whh16[l];
     RecFwdLaunch rec;
     // 16-bit: the runtime-sized kernels read weight_hh as it lies; the fixed configs get fp32 copies below
-    rc = plan_rec_fwd(rp, &rec, dt);
+    rc = plan_rec_fwd(rp, &rec, dt, d.M);
     if (rc) return rc;
+    const bool tc_layer = !dt && tc && (Il % 32 == 0) && (d.GH % 128 == 0);
     // Stream the input projection into the recurrence (DESIGN.md §4): the GEMM runs beside the recurrence and publishes
     // its row tiles in time order, the recurrence starts while it runs and waits per step for the tiles it reads. Only
     // when the recurrence is unidirectional (it walks t upwards), fits one wave of 4-CTA clusters and takes at most half
@@ -836,131 +870,185 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
     // The runtime-sized kernels (rec.anyh) take no streamed x-projection.
     const bool stream_xproj = !rec.anyh && d.D == 1 && d.P == 0 && tc_layer && rec.C == 4 && rec.one_wave() &&
                               2 * rec.ctas() <= sms && gemm_clusters > 0;
-    // ---- A operand of the tensor-core input projection (fp32, split on chip by the GEMM), shared by the directions:
-    // the layer input itself when the GEMM can read it in place, else a dense copy in the GEMM's workspace
-    void* tc_ws = S + sl.f_tc;
-    const float* a_in = in;
-    RowMap a_rows = in_rows;
-    const char* a_route = "tma";  // B200RNN_DEBUG: where the fp32 A operand comes from
-    if (tc_layer) {
-      float* a_dense = tc_a_hi(tc_ws);
-      if (l == 0 && ln_gamma) {
-        float* out = (save && fused_ln) ? R + rl.xln : a_dense;
-        // padded rows of a ragged batch are written as 0: the backward's dW_ih GEMM reads this saved operand
-        rc = tc_layernorm(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, out, st, ready, tiles_m, lengths, d.B);
-        a_in = out;
-        a_rows = simple_rows(Il);
-        a_route = "ln";
-      } else if (!tc_a_f32_in_place(in, in_rows, (int)d.TB, Il)) {
-        rc = tc_gather_rows(in, in_rows, (int)d.TB, Il, a_dense, st, ready, tiles_m);
-        a_in = a_dense;
-        a_rows = simple_rows(Il);
-        a_route = "gather";
-      } else if (stream_xproj && !ready_zeroed) {
-        B200_CUDA_CHECK(cudaMemsetAsync(ready, 0, tiles_m * sizeof(int), st));
+    // Several models: each model's layer input and input projection in turn, into its own blocks; the recurrence
+    // below runs them all
+    for (int m = 0; m < d.M; ++m) {
+      R = R0 + m * RS;
+      S = S0 + m * SS;
+      const float* const xm = m ? x + m * d.ms[0] : x;
+      if (m) {
+        model_params(d, params, m, pm);
       }
-      if (rc) return rc;
-    } else if (l == 0 && ln_gamma) {
-      set_error("forward: the fused LayerNorm prologue needs the tensor-core input projection (input_size %% 32 == 0)");
-      return B200RNN_ERR_UNSUPPORTED;
-    }
-    // everything before the first GEMM is enqueued: kernels of a stream gated on this event become pending no earlier
-    // than the layer-0 GEMM, which then wins the SMs on this stream's priority
-    if (l == 0 && prologue_ev) B200_CUDA_CHECK(cudaEventRecord(prologue_ev, st));
-    ready_zeroed = false;
-    for (int k = 0; k < d.D; ++k) {
-      const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
-      const float *w_ih = pp[0], *w_hh = pp[1], *b_ih = pp[2], *b_hh = pp[3];
-      if (!w_ih || !w_hh || !b_ih || !b_hh || (d.P > 0 && !pp[4])) {
-        set_error("forward: null parameter pointer (layer %d dir %d)", l, k);
-        return B200RNN_ERR_INVALID;
+      const float* const* const params_m = m ? pm : params;
+      // ---- layer input ---------------------------------------------------------------------------
+      const float* in;
+      RowMap in_rows;
+      if (l == 0) {
+        in = xm;
+        in_rows = tb_rows(xs_t, xs_b, d.B);
+      } else {
+        if (save)
+          in = R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
+        else
+          in = S + sl.f_y[(l - 1) & 1];
+        in_rows = simple_rows((long long)d.DH);
       }
-      if (!aligned_to(w_hh, 16)) {
-        set_error("forward: weight_hh must be 16-byte aligned for the TMA bulk copy (layer %d dir %d)", l, k);
-        return B200RNN_ERR_INVALID;
-      }
-      float* gates = save ? R + rl.gates[l][k] : S + sl.f_gates[k];
-      if (dt) {  // K1 on 16-bit operands: native f16 / bf16 wgmma, else the FFMA GEMM on exact fp32 copies
-        const float* b32 = S + hs.bias[l][k];
-        const int b2n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
-        // each direction's weight_ih checked on its own: one the TMA cannot read takes the FFMA GEMM
-        if (n16 && tc_gemm_n16_ok(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il)) {
-          rc = tc_gemm_n16(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il, dt, gates, simple_rows((long long)d.GH), b32,
-                           b32 + d.GH, b2n, st, a16_route);
-        } else {
-          float* aw = S + sl.f_tc;
-          float* ww = aw + align_up(d.TB * Il, ALIGN_F);
-          rc = launch_widen16(a16, a16_rows, (int)d.TB, Il, dt, aw, st);
-          if (!rc) rc = launch_widen16(w_ih, simple_rows(Il), (int)d.GH, Il, dt, ww, st);
+      // 16-bit: the A operand of the native input projection, read in place when the TMA can (else a dense copy)
+      const void* a16 = l == 0 ? static_cast<const void*>(x) : S + hs.a16;
+      RowMap a16_rows = l == 0 ? tb_rows(xs_t, xs_b, d.B) : simple_rows((long long)d.DH);
+      bool n16 = false;
+      const char* a16_route = "tma";  // B200RNN_DEBUG: where the 16-bit A operand comes from
+      if (dt) {
+        n16 = tc && tc_gemm_n16_ok(a16, a16_rows, params[(size_t)l * d.D * d.NPAR], (int)d.TB, (int)d.GH, Il);
+        if (!n16 && l == 0 && tc && tc_gemm_n16_ok(S + hs.a16, simple_rows(Il), params[0], (int)d.TB, (int)d.GH, Il)) {
+          rc = launch_copy16(x, a16_rows, (int)d.TB, Il, S + hs.a16, st);
           if (rc) return rc;
+          a16 = S + hs.a16;
+          a16_rows = simple_rows(Il);
+          a16_route = "copy16";
+          n16 = true;
+        }
+      }
+      // ---- A operand of the tensor-core input projection (fp32, split on chip by the GEMM), shared by the directions:
+      // the layer input itself when the GEMM can read it in place, else a dense copy in the GEMM's workspace
+      void* tc_ws = S + sl.f_tc;
+      const float* a_in = in;
+      RowMap a_rows = in_rows;
+      const char* a_route = "tma";  // B200RNN_DEBUG: where the fp32 A operand comes from
+      if (tc_layer) {
+        float* a_dense = tc_a_hi(tc_ws);
+        if (l == 0 && ln_gamma) {
+          float* out = (save && fused_ln) ? R + rl.xln : a_dense;
+          // padded rows of a ragged batch are written as 0: the backward's dW_ih GEMM reads this saved operand
+          rc = tc_layernorm(in, in_rows, (int)d.TB, Il, ln_gamma, ln_beta, ln_eps, out, st, ready, tiles_m, lengths, d.B);
+          a_in = out;
+          a_rows = simple_rows(Il);
+          a_route = "ln";
+        } else if (!tc_a_f32_in_place(in, in_rows, (int)d.TB, Il)) {
+          rc = tc_gather_rows(in, in_rows, (int)d.TB, Il, a_dense, st, ready, tiles_m);
+          a_in = a_dense;
+          a_rows = simple_rows(Il);
+          a_route = "gather";
+        } else if (stream_xproj && !ready_zeroed) {
+          B200_CUDA_CHECK(cudaMemsetAsync(ready, 0, tiles_m * sizeof(int), st));
+        }
+        if (rc) return rc;
+      } else if (l == 0 && ln_gamma) {
+        set_error("forward: the fused LayerNorm prologue needs the tensor-core input projection (input_size %% 32 == 0)");
+        return B200RNN_ERR_UNSUPPORTED;
+      }
+      // everything before the first GEMM is enqueued: kernels of a stream gated on this event become pending no earlier
+      // than the layer-0 GEMM, which then wins the SMs on this stream's priority
+      if (l == 0 && prologue_ev) B200_CUDA_CHECK(cudaEventRecord(prologue_ev, st));
+      ready_zeroed = false;
+      for (int k = 0; k < d.D; ++k) {
+        const float* const* pp = params_m + (size_t)(l * d.D + k) * d.NPAR;
+        const float *w_ih = pp[0], *w_hh = pp[1], *b_ih = pp[2], *b_hh = pp[3];
+        if (!w_ih || !w_hh || !b_ih || !b_hh || (d.P > 0 && !pp[4])) {
+          set_error("forward: null parameter pointer (layer %d dir %d)", l, k);
+          return B200RNN_ERR_INVALID;
+        }
+        if (!aligned_to(w_hh, 16)) {
+          set_error("forward: weight_hh must be 16-byte aligned for the TMA bulk copy (layer %d dir %d)", l, k);
+          return B200RNN_ERR_INVALID;
+        }
+        float* gates = save ? R + rl.gates[l][k] : S + sl.f_gates[k];
+        if (dt) {  // K1 on 16-bit operands: native f16 / bf16 wgmma, else the FFMA GEMM on exact fp32 copies
+          const float* b32 = S + hs.bias[l][k];
+          const int b2n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
+          // each direction's weight_ih checked on its own: one the TMA cannot read takes the FFMA GEMM
+          if (n16 && tc_gemm_n16_ok(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il)) {
+            rc = tc_gemm_n16(a16, a16_rows, w_ih, (int)d.TB, (int)d.GH, Il, dt, gates, simple_rows((long long)d.GH), b32,
+                             b32 + d.GH, b2n, st, a16_route);
+          } else {
+            float* aw = S + sl.f_tc;
+            float* ww = aw + align_up(d.TB * Il, ALIGN_F);
+            rc = launch_widen16(a16, a16_rows, (int)d.TB, Il, dt, aw, st);
+            if (!rc) rc = launch_widen16(w_ih, simple_rows(Il), (int)d.GH, Il, dt, ww, st);
+            if (rc) return rc;
+            GemmParams g;
+            memset(&g, 0, sizeof(g));
+            g.A = aw; g.a_rows = simple_rows(Il); g.a_kcontig = 1;
+            g.B = ww; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
+            g.C = gates; g.c_rows = simple_rows((long long)d.GH);
+            g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
+            g.bias1 = b32; g.bias2 = b32 + d.GH; g.bias2_n = b2n;
+            g.a_route = "widen";
+            rc = launch_gemm(g, nullptr, 0, st);
+          }
+          if (rc) return rc;
+        } else {
+          // K1: x-projection of every time step at once, biases folded (GRU: b_hh only for r,z; LSTM, Elman: all of it)
           GemmParams g;
           memset(&g, 0, sizeof(g));
-          g.A = aw; g.a_rows = simple_rows(Il); g.a_kcontig = 1;
-          g.B = ww; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
+          g.A = a_in; g.a_rows = a_rows; g.a_kcontig = 1;
+          g.B = w_ih; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
           g.C = gates; g.c_rows = simple_rows((long long)d.GH);
           g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
-          g.bias1 = b32; g.bias2 = b32 + d.GH; g.bias2_n = b2n;
-          g.a_route = "widen";
+          g.bias1 = b_ih; g.bias2 = b_hh;
+          g.bias2_n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
+          g.a_route = a_route;
+          if (tc_layer) {
+            g.tc_ws = tc_ws;
+            g.tc_ws_bytes = sl.f_tc_bytes;
+            g.tc_a_f32 = 1;
+            g.tc_tf32 = tf32 ? 1 : 0;
+            // the no-grad forward of b200rnn_forward_fused in default precision: fp16 pairs (the rule of the fp16-pair
+            // recurrence, RecFwdParams::shell_nograd)
+            g.tc_h16 = rp.shell_nograd && !tf32 && g16::shape_ok((int)d.GH, Il) ? 1 : 0;
+            if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders); TF32 reads only hi
+              g.tc_b_hi = WC + wl.hi[l][k];
+              g.tc_b_lo = tf32 ? nullptr : WC + wl.lo[l][k];
+              if (g.tc_h16) g.tc_b_h16 = WC + wl.h16[l][k];
+            }
+            if (stream_xproj && gemm_tc_eligible(g, g.tc_ws_bytes)) {
+              g.tc_ready = ready;
+              g.tc_stream_clusters = gemm_clusters;
+              rp.ready = ready;
+              rp.tiles_n = (int)d.GH / TC_TILE_N;
+            }
+          }
           rc = launch_gemm(g, nullptr, 0, st);
-        }
-        if (rc) return rc;
-      } else {
-        // K1: x-projection of every time step at once, biases folded (GRU: b_hh only for r,z; LSTM, Elman: all of it)
-        GemmParams g;
-        memset(&g, 0, sizeof(g));
-        g.A = a_in; g.a_rows = a_rows; g.a_kcontig = 1;
-        g.B = w_ih; g.b_rows = simple_rows(Il); g.b_kcontig = 1;
-        g.C = gates; g.c_rows = simple_rows((long long)d.GH);
-        g.M = (int)d.TB; g.N = (int)d.GH; g.K = Il;
-        g.bias1 = b_ih; g.bias2 = b_hh;
-        g.bias2_n = d.mode == B200RNN_GRU ? 2 * d.H : (int)d.GH;
-        g.a_route = a_route;
-        if (tc_layer) {
-          g.tc_ws = tc_ws;
-          g.tc_ws_bytes = sl.f_tc_bytes;
-          g.tc_a_f32 = 1;
-          g.tc_tf32 = tf32 ? 1 : 0;
-          // the no-grad forward of b200rnn_forward_fused in default precision: fp16 pairs (the rule of the fp16-pair
-          // recurrence, RecFwdParams::shell_nograd)
-          g.tc_h16 = rp.shell_nograd && !tf32 && g16::shape_ok((int)d.GH, Il) ? 1 : 0;
-          if (WC) {  // weight_ih was split once by b200rnn_prepare_weights (frozen encoders); TF32 reads only hi
-            g.tc_b_hi = WC + wl.hi[l][k];
-            g.tc_b_lo = tf32 ? nullptr : WC + wl.lo[l][k];
-            if (g.tc_h16) g.tc_b_h16 = WC + wl.h16[l][k];
-          }
-          if (stream_xproj && gemm_tc_eligible(g, g.tc_ws_bytes)) {
-            g.tc_ready = ready;
-            g.tc_stream_clusters = gemm_clusters;
-            rp.ready = ready;
-            rp.tiles_n = (int)d.GH / TC_TILE_N;
-          }
-        }
-        rc = launch_gemm(g, nullptr, 0, st);
-        if (rc) return rc;
-      }
-      rp.w_hh[k] = w_hh;
-      rp.b_hh[k] = b_hh;
-      if (dt) {
-        rp.b_hh[k] = S + hs.bias[l][k] + d.GH;
-        if (!rec.anyh && d.master) {  // rounded into hs.w32 by round_master_params
-          if (!fixed_whh) {
-            set_error("forward: no fp32 weight_hh for the recurrence config (mode %d, hidden_size %d)", d.mode, d.H);
-            return B200RNN_ERR_UNSUPPORTED;
-          }
-          rp.w_hh[k] = S + hs.w32[l][k] + d.GH * (size_t)Il;
-        } else if (!rec.anyh) {  // the fixed configs read fp32: an exact copy per direction
-          float* w32 = S + hs.whh + (size_t)k * d.GH * d.H;
-          rc = launch_widen16(w_hh, simple_rows(d.H), (int)d.GH, d.H, dt, w32, st);
           if (rc) return rc;
-          rp.w_hh[k] = w32;
+        }
+        if (m > 0) continue;  // the recurrence takes model 0's pointers and the model strides
+        rp.w_hh[k] = w_hh;
+        rp.b_hh[k] = b_hh;
+        if (dt) {
+          rp.b_hh[k] = S + hs.bias[l][k] + d.GH;
+          if (!rec.anyh && d.master) {  // rounded into hs.w32 by round_master_params
+            if (!fixed_whh) {
+              set_error("forward: no fp32 weight_hh for the recurrence config (mode %d, hidden_size %d)", d.mode, d.H);
+              return B200RNN_ERR_UNSUPPORTED;
+            }
+            rp.w_hh[k] = S + hs.w32[l][k] + d.GH * (size_t)Il;
+          } else if (!rec.anyh) {  // the fixed configs read fp32: an exact copy per direction
+            float* w32 = S + hs.whh + (size_t)k * d.GH * d.H;
+            rc = launch_widen16(w_hh, simple_rows(d.H), (int)d.GH, d.H, dt, w32, st);
+            if (rc) return rc;
+            rp.w_hh[k] = w32;
+          }
+        }
+        rp.gates[k] = gates;
+        rp.extra[k] = save && !is_elman(d.mode) ? R + rl.extra[l][k] : nullptr;
+        if (d.P > 0) {
+          rp.w_hr[k] = pp[4];
+          rp.m[k] = save ? R + rl.m[l][k] : nullptr;
         }
       }
-      rp.gates[k] = gates;
-      rp.extra[k] = save && !is_elman(d.mode) ? R + rl.extra[l][k] : nullptr;
-      if (d.P > 0) {
-        rp.w_hr[k] = pp[4];
-        rp.m[k] = save ? R + rl.m[l][k] : nullptr;
+    }
+    R = R0;
+    S = S0;
+    if (d.M > 1) {
+      RecModels& mo = rec.models;
+      for (int k = 0; k < d.D; ++k) {
+        const int64_t* msp = d.ms + 2 + (size_t)(l * d.D + k) * d.NPAR;
+        mo.whh[k] = msp[1];
+        mo.bhh[k] = msp[3];
       }
+      mo.saved = (long long)(save ? RS : SS);
+      mo.y = l == d.L - 1 ? (long long)(d.TB * d.DH) : mo.saved;
+      mo.state = (long long)d.L * d.D * d.B * d.H;
     }
     float* ylay = nullptr;
     if (l == d.L - 1 && dt) {  // fp32, kept for the backward; rounded into the caller's y below
@@ -1004,11 +1092,15 @@ static int forward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t, 
       }
       if (rc) return rc;
     } else if (drop && l + 1 < d.L) {  // K7; keeps the raw output when it is needed by backward, else in place
-      float* dropped = save ? R + rl.ydrop[l] : ylay;
-      // the next layer's GEMM reads `dropped` in place; the same launch zeroes its ready counters
-      rc = launch_dropout(ylay, dropped, d.TB * d.DH, d.p, hdr, (uint32_t)l, st, ready, tiles_m);
+      for (int m = 0; m < d.M; ++m) {  // each model with its own header
+        const size_t at = m * (save ? RS : SS);
+        float* dropped = save ? R + at + rl.ydrop[l] : ylay + at;
+        // the next layer's GEMM reads `dropped` in place; the same launch zeroes its ready counters
+        rc = launch_dropout(ylay + at, dropped, d.TB * d.DH, d.p, model_hdr(m), (uint32_t)l, st, m ? nullptr : ready,
+                            tiles_m);
+        if (rc) return rc;
+      }
       ready_zeroed = true;
-      if (rc) return rc;
     }
   }
   if (dt) {
@@ -1190,10 +1282,18 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
   if (rc) return rc;
   ScratchLayout sl;
   make_scratch(d, &sl);
-  const float* R = static_cast<const float*>(reserve);
-  float* S = static_cast<float*>(scratch);
+  if (d.M > 1 && lengths) {
+    set_error("backward: several models in one call take no lengths (ragged batches run one model per call)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  // model m's reserve and scratch blocks start at m * RS and m * SS (one model: R0 and S0 are the whole buffers)
+  const float* const R0 = static_cast<const float*>(reserve);
+  float* const S0 = static_cast<float*>(scratch);
+  size_t RS, SS;
+  model_blocks(d, fused_ln, &RS, &SS);
+  const float* R = R0;
+  float* S = S0;
   const bool drop = d.training && d.p > 0.f && d.L > 1;
-  const uint64_t* hdr = reinterpret_cast<const uint64_t*>(R);  // dropout seed/offset used by the forward
   const int accumulate = (desc->flags & B200RNN_FLAG_ACCUMULATE_GRADS) ? 1 : 0;
   const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0;  // single-pass TF32 tensor-core GEMMs: hi operands only
   const int TB = (int)d.TB, GH = (int)d.GH;
@@ -1204,6 +1304,8 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     if (rc) return rc;
   }
 
+  const float* pm[8 * 2 * 5];  // model m's parameter table
+  float* dpm[8 * 2 * 5];       // ... and gradient targets
   for (int l = d.L - 1; l >= 0; --l) {
     const int Il = l == 0 ? d.I : (int)d.DH;
     RecBwdParams bp;
@@ -1246,113 +1348,149 @@ static int backward_impl(const b200rnn_desc* desc, const float* x, int64_t xs_t,
     }
     bp.lengths = lengths;
     bp.order = order;
+    RecModels mo;  // the caller's tensors are dense per model but for x and the parameters (desc->model_strides)
+    if (d.M > 1) {
+      mo.M = d.M;
+      for (int k = 0; k < d.D; ++k) {
+        mo.whh[k] = d.ms[2 + (size_t)(l * d.D + k) * d.NPAR + 1];
+        mo.wprep[k] = mo.whh[k] ? (long long)SS : 0;  // a shared weight_hh is transposed once, into model 0's scratch
+      }
+      mo.saved = (long long)RS;
+      mo.y = l == d.L - 1 ? (long long)(d.TB * d.DH) : (long long)RS;
+      mo.dy = l == d.L - 1 ? (long long)(d.TB * d.DH) : (long long)SS;
+      mo.scr = (long long)SS;
+      mo.state = (long long)d.L * d.D * d.B * d.H;
+    }
     // 16-bit: whh16 holds each (layer, direction)'s weight_hh as the caller passed it, staged in 16 bits by the
     // runtime-sized BPTT
-    rc = launch_rec_bwd(bp, st, w16, whh16 ? whh16 + (size_t)l * d.D : nullptr);
+    rc = launch_rec_bwd(bp, st, w16, whh16 ? whh16 + (size_t)l * d.D : nullptr, d.M > 1 ? &mo : nullptr);
     if (rc) return rc;
 
-    // The gradient GEMMs of this layer: each runs on the tensor cores when it is eligible, on the FFMA GEMM otherwise.
-    // The tensor cores need 16-byte aligned targets: a gradient view that is not (a caller's flat bucket behind an
-    // odd-sized tensor) takes the FFMA GEMM instead of failing.
-    const bool tc_l = tc_available() && (Il % 128 == 0);
-    // layer input as seen by the forward GEMM; one split serves both directions. The padded steps of a ragged batch
-    // have zero gate gradients, but 0 * NaN is NaN: layer 0's operand must be 0 there, not whatever the caller left in
-    // x (the layers above read the recurrence's outputs, which are 0 past each length)
-    GradSrc X{nullptr, simple_rows((long long)Il), TB, Il, S + sl.b_tc_x, false};
-    if (l == 0 && fused_ln) {  // what the forward GEMM multiplied: LayerNorm(x), saved densely by the prologue (padding 0)
-      X.p = R + rl.xln;
-    } else if (l == 0 && lengths) {  // x with its padding zeroed, dense in the (unused without LayerNorm) b_dxln region
-      rc = launch_valid_rows(x, tb_rows(xs_t, xs_b, d.B), d.T, d.B, Il, lengths, S + sl.b_dxln, st);
-      if (rc) return rc;
-      X.p = S + sl.b_dxln;
-    } else if (l == 0) {
-      X.p = x;
-      X.rows = tb_rows(xs_t, xs_b, d.B);
-    } else {
-      X.p = layer_in ? layer_in[l - 1] : R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
-    }
-    // dX_l goes to the caller's dx (layer 0) or to the dy of the layer below (scratch). With the fused LayerNorm the
-    // layer-0 dgrad is d/dLN(x): it goes to scratch and through the LN backward below
-    const bool ln_l0 = (l == 0) && fused_ln;
-    const bool want_dx = (l > 0) || (dx != nullptr) || (ln_l0 && (dln_gamma || dln_beta));
-    float* Cx = S + sl.b_dy;
-    RowMap cx_rows = simple_rows((long long)d.DH);
-    if (ln_l0) {
-      Cx = S + sl.b_dxln; cx_rows = simple_rows((long long)d.I);
-    } else if (l == 0) {
-      Cx = dx; cx_rows = tb_rows(dxs_t, dxs_b, d.B);
-    }
-    const bool tc_dx = tc_l && want_dx && aligned_to(Cx, 16) && cx_rows.s_outer % 4 == 0 && cx_rows.s_inner % 4 == 0;
-    for (int k = 0; k < d.D; ++k) {
-      const float* const* pp = params + (size_t)(l * d.D + k) * d.NPAR;
-      float* const* gp = dparams + (size_t)(l * d.D + k) * d.NPAR;
-      float *dw_ih = gp[0], *dw_hh = gp[1], *db_ih = gp[2], *db_hh = gp[3];
-      if (db_ih || db_hh) {
-        rc = launch_bias_reduce(S + sl.b_bpart[k], bp.nslices_out, d.mode, d.H, db_ih, db_hh, accumulate, st);
-        if (rc) return rc;
+    // Several models: the gradient GEMMs of each model in turn, on its own blocks
+    for (int m = 0; m < d.M; ++m) {
+      R = R0 + m * RS;
+      S = S0 + m * SS;
+      const float* const xm = m ? x + m * d.ms[0] : x;
+      if (m) {
+        model_params(d, params, m, pm);
+        for (int i = 0; i < d.L * d.D * d.NPAR; ++i) {  // the gradient targets: dense per model, m parameter sizes on
+          const int li = i / (d.D * d.NPAR), pi = i % d.NPAR;
+          const size_t n = pi == 0 ? d.GH * (li == 0 ? (size_t)d.I : d.DH) : pi == 1 ? d.GH * d.H : d.GH;
+          dpm[i] = dparams[i] ? dparams[i] + m * n : nullptr;
+        }
       }
-      // this direction's operands (their split regions are reused by the next direction)
-      GradSrc dG{S + sl.b_dgates[k], simple_rows(GH), TB, GH, S + sl.b_tc_dg, false};
-      GradSrc dnr{S + sl.b_dghn[k], simple_rows(d.H), TB, d.H, S + sl.b_tc_hn, false};  // GRU: dn * r
-      GradSrc h{bp.y + (long long)k * d.HO, tb_rows(bp.y_st, bp.y_sb, d.B), TB, d.HO, S + sl.b_tc_y, false};
-      GradSrc w_ih{pp[0], simple_rows(Il), GH, Il, S + sl.b_tc_w, false};
-      if (dw_ih) {  // dW_ih[GH, Il] = sum_tb dG[tb, :]^T X_l[tb, :]
-        rc = run_grad_gemm({{&dG, 0, false}, {&X, 0, false}, GH, Il, TB, dw_ih, simple_rows(Il), accumulate, true,
-                            tc_l && aligned_to(dw_ih, 16), "dW_ih"}, sl, S, tf32, st);
+      const float* const* const params_m = m ? pm : params;
+      float* const* const dparams_m = m ? dpm : dparams;
+      float* const dxm = dx && m ? dx + m * d.TB * d.I : dx;
+      const float* const ym = bp.y + m * mo.y;
+      const float* const h0m = bp.h_0 ? bp.h_0 + m * mo.state : nullptr;
+      const uint64_t* hdr = reinterpret_cast<const uint64_t*>(R);  // dropout seed/offset used by the forward
+
+      // The gradient GEMMs of this layer: each runs on the tensor cores when it is eligible, on the FFMA GEMM otherwise.
+      // The tensor cores need 16-byte aligned targets: a gradient view that is not (a caller's flat bucket behind an
+      // odd-sized tensor) takes the FFMA GEMM instead of failing.
+      const bool tc_l = tc_available() && (Il % 128 == 0);
+      // layer input as seen by the forward GEMM; one split serves both directions. The padded steps of a ragged batch
+      // have zero gate gradients, but 0 * NaN is NaN: layer 0's operand must be 0 there, not whatever the caller left in
+      // x (the layers above read the recurrence's outputs, which are 0 past each length)
+      GradSrc X{nullptr, simple_rows((long long)Il), TB, Il, S + sl.b_tc_x, false};
+      if (l == 0 && fused_ln) {  // what the forward GEMM multiplied: LayerNorm(x), saved densely by the prologue (padding 0)
+        X.p = R + rl.xln;
+      } else if (l == 0 && lengths) {  // x with its padding zeroed, dense in the (unused without LayerNorm) b_dxln region
+        rc = launch_valid_rows(xm, tb_rows(xs_t, xs_b, d.B), d.T, d.B, Il, lengths, S + sl.b_dxln, st);
         if (rc) return rc;
+        X.p = S + sl.b_dxln;
+      } else if (l == 0) {
+        X.p = xm;
+        X.rows = tb_rows(xs_t, xs_b, d.B);
+      } else {
+        X.p = layer_in ? layer_in[l - 1] : R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
       }
-      if (dw_hh) {
-        // dW_hh = sum_t dGh[t]^T h_{prev(t)}: rows are (t,b) flattened time-major, so the one-step shift is a row
-        // offset of B (forward: dG[t] with h[t-1], t = 1..T-1; reverse: dG[t] with h[t+1], t = 0..T-2). LSTM, Elman:
-        // one GEMM over all gates; GRU: the r,z rows from columns [0, 2H) of dG, the n rows from dn*r
-        const int g0 = k == 0 ? d.B : 0, Kp = (d.T - 1) * d.B;
-        // the tensor-core GEMM needs N = H a multiple of 128 (hidden sizes other than 128 / 256 may not be)
-        const bool gru = d.mode == B200RNN_GRU,
-                   tc = tc_l && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0 && d.HO % 128 == 0;
-        rc = run_grad_gemm({{&dG, g0, false}, {&h, d.B - g0, false}, gru ? 2 * d.H : GH, d.HO, Kp, dw_hh,
-                            simple_rows(d.HO), accumulate, true, tc, gru ? "dW_hh_rz" : "dW_hh"}, sl, S, tf32, st);
-        if (rc) return rc;
-        if (gru) {
-          rc = run_grad_gemm({{&dnr, g0, false}, {&h, d.B - g0, false}, d.H, d.HO, Kp, dw_hh + (size_t)2 * d.H * d.HO,
-                              simple_rows(d.HO), accumulate, true, tc, "dW_hh_n"}, sl, S, tf32, st);
+      // dX_l goes to the caller's dx (layer 0) or to the dy of the layer below (scratch). With the fused LayerNorm the
+      // layer-0 dgrad is d/dLN(x): it goes to scratch and through the LN backward below
+      const bool ln_l0 = (l == 0) && fused_ln;
+      const bool want_dx = (l > 0) || (dxm != nullptr) || (ln_l0 && (dln_gamma || dln_beta));
+      float* Cx = S + sl.b_dy;
+      RowMap cx_rows = simple_rows((long long)d.DH);
+      if (ln_l0) {
+        Cx = S + sl.b_dxln; cx_rows = simple_rows((long long)d.I);
+      } else if (l == 0) {
+        Cx = dxm; cx_rows = tb_rows(dxs_t, dxs_b, d.B);
+      }
+      const bool tc_dx = tc_l && want_dx && aligned_to(Cx, 16) && cx_rows.s_outer % 4 == 0 && cx_rows.s_inner % 4 == 0;
+      for (int k = 0; k < d.D; ++k) {
+        const float* const* pp = params_m + (size_t)(l * d.D + k) * d.NPAR;
+        float* const* gp = dparams_m + (size_t)(l * d.D + k) * d.NPAR;
+        float *dw_ih = gp[0], *dw_hh = gp[1], *db_ih = gp[2], *db_hh = gp[3];
+        if (db_ih || db_hh) {
+          rc = launch_bias_reduce(S + sl.b_bpart[k], bp.nslices_out, d.mode, d.H, db_ih, db_hh, accumulate, st);
+          if (rc) return rc;
+        }
+        // this direction's operands (their split regions are reused by the next direction)
+        GradSrc dG{S + sl.b_dgates[k], simple_rows(GH), TB, GH, S + sl.b_tc_dg, false};
+        GradSrc dnr{S + sl.b_dghn[k], simple_rows(d.H), TB, d.H, S + sl.b_tc_hn, false};  // GRU: dn * r
+        GradSrc h{ym + (long long)k * d.HO, tb_rows(bp.y_st, bp.y_sb, d.B), TB, d.HO, S + sl.b_tc_y, false};
+        GradSrc w_ih{pp[0], simple_rows(Il), GH, Il, S + sl.b_tc_w, false};
+        if (dw_ih) {  // dW_ih[GH, Il] = sum_tb dG[tb, :]^T X_l[tb, :]
+          rc = run_grad_gemm({{&dG, 0, false}, {&X, 0, false}, GH, Il, TB, dw_ih, simple_rows(Il), accumulate, true,
+                              tc_l && aligned_to(dw_ih, 16), "dW_ih"}, sl, S, tf32, st);
+          if (rc) return rc;
+        }
+        if (dw_hh) {
+          // dW_hh = sum_t dGh[t]^T h_{prev(t)}: rows are (t,b) flattened time-major, so the one-step shift is a row
+          // offset of B (forward: dG[t] with h[t-1], t = 1..T-1; reverse: dG[t] with h[t+1], t = 0..T-2). LSTM, Elman:
+          // one GEMM over all gates; GRU: the r,z rows from columns [0, 2H) of dG, the n rows from dn*r
+          const int g0 = k == 0 ? d.B : 0, Kp = (d.T - 1) * d.B;
+          // the tensor-core GEMM needs N = H a multiple of 128 (hidden sizes other than 128 / 256 may not be)
+          const bool gru = d.mode == B200RNN_GRU,
+                     tc = tc_l && aligned_to(dw_hh, 16) && d.T > 1 && d.P == 0 && d.HO % 128 == 0;
+          rc = run_grad_gemm({{&dG, g0, false}, {&h, d.B - g0, false}, gru ? 2 * d.H : GH, d.HO, Kp, dw_hh,
+                              simple_rows(d.HO), accumulate, true, tc, gru ? "dW_hh_rz" : "dW_hh"}, sl, S, tf32, st);
+          if (rc) return rc;
+          if (gru) {
+            rc = run_grad_gemm({{&dnr, g0, false}, {&h, d.B - g0, false}, d.H, d.HO, Kp, dw_hh + (size_t)2 * d.H * d.HO,
+                                simple_rows(d.HO), accumulate, true, tc, "dW_hh_n"}, sl, S, tf32, st);
+            if (rc) return rc;
+          }
+        }
+        if (dw_hh && h0m) {
+          // the first scanned step's previous state is h_0: dW_hh += sum_b dGh[t_first(b), b]^T h_0[b]. The shifted GEMMs
+          // above never pair that step with anything but a zero (T = 1: K = 0; ragged reverse rows: the masked output at
+          // len_b), so nothing is counted twice. One fixed-order K = B FFMA GEMM: deterministic.
+          GradSrc rows0{S + sl.b_h0, simple_rows(GH), d.B, GH, nullptr, false};  // [B][GH]
+          GradSrc h0{h0m + (size_t)k * d.B * d.HO, simple_rows(d.HO), d.B, d.HO, nullptr, false};
+          rc = launch_initial_state_rows(dG.p, dnr.p, d.mode, d.B, d.T, d.H, k == 1, lengths, S + sl.b_h0, st);
+          if (rc) return rc;
+          rc = run_grad_gemm({{&rows0, 0, false}, {&h0, 0, false}, GH, d.HO, d.B, dw_hh, simple_rows(d.HO), 1, false,
+                              false, "dW_hh_h0"}, sl, S, tf32, st);
+          if (rc) return rc;
+        }
+        if (d.P > 0 && gp[4]) {  // dW_hr[P, H] = sum_tb dh[tb, :]^T m[tb, :] (frozen and skipped steps have dh = 0)
+          GradSrc dhp{S + sl.b_dhp[k], simple_rows(d.P), TB, d.P, nullptr, false};
+          GradSrc m{R + rl.m[l][k], simple_rows(d.H), TB, d.H, nullptr, false};
+          rc = run_grad_gemm({{&dhp, 0, false}, {&m, 0, false}, d.P, d.H, TB, gp[4], simple_rows(d.H), accumulate, true,
+                              false, "dW_hr"}, sl, S, tf32, st);
+          if (rc) return rc;
+        }
+        if (want_dx) {  // dX_l (+)= dG[TB, GH] W_ih[GH, Il]: dG read K-major, W_ih as it lies
+          rc = run_grad_gemm({{&dG, 0, true}, {&w_ih, 0, false}, TB, Il, GH, Cx, cx_rows, k > 0, false, tc_dx, "dX"}, sl,
+                             S, tf32, st);
           if (rc) return rc;
         }
       }
-      if (dw_hh && bp.h_0) {
-        // the first scanned step's previous state is h_0: dW_hh += sum_b dGh[t_first(b), b]^T h_0[b]. The shifted GEMMs
-        // above never pair that step with anything but a zero (T = 1: K = 0; ragged reverse rows: the masked output at
-        // len_b), so nothing is counted twice. One fixed-order K = B FFMA GEMM: deterministic.
-        GradSrc rows0{S + sl.b_h0, simple_rows(GH), d.B, GH, nullptr, false};  // [B][GH]
-        GradSrc h0{bp.h_0 + (size_t)k * d.B * d.HO, simple_rows(d.HO), d.B, d.HO, nullptr, false};
-        rc = launch_initial_state_rows(dG.p, dnr.p, d.mode, d.B, d.T, d.H, k == 1, lengths, S + sl.b_h0, st);
-        if (rc) return rc;
-        rc = run_grad_gemm({{&rows0, 0, false}, {&h0, 0, false}, GH, d.HO, d.B, dw_hh, simple_rows(d.HO), 1, false,
-                            false, "dW_hh_h0"}, sl, S, tf32, st);
+      if (l > 0 && drop) {  // gradient through the inter-layer dropout of layer l-1's output (same mask)
+        rc = launch_dropout(S + sl.b_dy, S + sl.b_dy, d.TB * d.DH, d.p, hdr, (uint32_t)(l - 1), st);
         if (rc) return rc;
       }
-      if (d.P > 0 && gp[4]) {  // dW_hr[P, H] = sum_tb dh[tb, :]^T m[tb, :] (frozen and skipped steps have dh = 0)
-        GradSrc dhp{S + sl.b_dhp[k], simple_rows(d.P), TB, d.P, nullptr, false};
-        GradSrc m{R + rl.m[l][k], simple_rows(d.H), TB, d.H, nullptr, false};
-        rc = run_grad_gemm({{&dhp, 0, false}, {&m, 0, false}, d.P, d.H, TB, gp[4], simple_rows(d.H), accumulate, true,
-                            false, "dW_hr"}, sl, S, tf32, st);
-        if (rc) return rc;
-      }
-      if (want_dx) {  // dX_l (+)= dG[TB, GH] W_ih[GH, Il]: dG read K-major, W_ih as it lies
-        rc = run_grad_gemm({{&dG, 0, true}, {&w_ih, 0, false}, TB, Il, GH, Cx, cx_rows, k > 0, false, tc_dx, "dX"}, sl,
-                           S, tf32, st);
+      if (ln_l0 && want_dx) {  // LayerNorm backward: dx (caller's layout), dgamma, dbeta
+        rc = launch_layernorm_bwd(xm, tb_rows(xs_t, xs_b, d.B), S + sl.b_dxln, (int)d.TB, d.I, ln_gamma, ln_eps, dxm,
+                                  tb_rows(dxs_t, dxs_b, d.B), dln_gamma, dln_beta, accumulate, S + sl.b_lnpart, st,
+                                  lengths, d.B);
         if (rc) return rc;
       }
     }
-    if (l > 0 && drop) {  // gradient through the inter-layer dropout of layer l-1's output (same mask)
-      rc = launch_dropout(S + sl.b_dy, S + sl.b_dy, d.TB * d.DH, d.p, hdr, (uint32_t)(l - 1), st);
-      if (rc) return rc;
-    }
-    if (ln_l0 && want_dx) {  // LayerNorm backward: dx (caller's layout), dgamma, dbeta
-      rc = launch_layernorm_bwd(x, tb_rows(xs_t, xs_b, d.B), S + sl.b_dxln, (int)d.TB, d.I, ln_gamma, ln_eps, dx,
-                                tb_rows(dxs_t, dxs_b, d.B), dln_gamma, dln_beta, accumulate, S + sl.b_lnpart, st,
-                                lengths, d.B);
-      if (rc) return rc;
-    }
+    R = R0;
+    S = S0;
   }
   return B200RNN_OK;
 }

@@ -10,7 +10,7 @@ namespace {
 // Inter-layer dropout, nn.GRU/nn.LSTM semantics (rnn.py:857-860, :1233-1236): Bernoulli(1-p) keep mask,
 // kept values scaled by 1/(1-p). One Philox call yields the mask of 4 consecutive elements.
 __global__ void rng_setup_kernel(uint64_t* hdr, uint64_t seed, uint64_t offset, uint64_t* state_dev,
-                                 uint64_t consume) {
+                                 uint64_t consume, uint64_t skip) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     if (state_dev) {
       seed = state_dev[0];
@@ -18,7 +18,7 @@ __global__ void rng_setup_kernel(uint64_t* hdr, uint64_t seed, uint64_t offset, 
       state_dev[1] = offset + consume;
     }
     hdr[0] = seed;
-    hdr[1] = offset;
+    hdr[1] = offset + skip;
   }
 }
 
@@ -153,8 +153,8 @@ __global__ void elman_bias_reduce_kernel(const float* __restrict__ part, int nsl
 }  // namespace
 
 int launch_rng_setup(uint64_t* hdr, uint64_t seed, uint64_t offset, uint64_t* state_dev, uint64_t consume,
-                     cudaStream_t stream) {
-  rng_setup_kernel<<<1, 32, 0, stream>>>(hdr, seed, offset, state_dev, consume);
+                     cudaStream_t stream, uint64_t skip) {
+  rng_setup_kernel<<<1, 32, 0, stream>>>(hdr, seed, offset, state_dev, consume, skip);
   B200_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return B200RNN_OK;

@@ -6,9 +6,10 @@ namespace b200rnn {
 
 // Resolve the dropout RNG state of one forward call on the device, so the call is CUDA-graph replayable:
 //   hdr[0] = seed, hdr[1] = offset   taken from `state_dev` ([seed, offset], then offset += consume) if it is
-//   non-NULL, else from the by-value arguments.
+//   non-NULL, else from the by-value arguments. skip: hdr[1] = offset + skip (one of several models drawing from
+//   one state as consecutive calls would)
 int launch_rng_setup(uint64_t* hdr, uint64_t seed, uint64_t offset, uint64_t* state_dev, uint64_t consume,
-                     cudaStream_t stream);
+                     cudaStream_t stream, uint64_t skip = 0);
 
 // out[i] = in[i] * mask(i) / (1-p) over n dense elements; mask is Philox4x32-10 keyed by hdr = {seed, offset}
 // and the per-layer stream id; in == out is allowed (in place).

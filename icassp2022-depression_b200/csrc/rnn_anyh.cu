@@ -71,7 +71,7 @@ __device__ __forceinline__ AnyhSlice anyh_slice(const Params& p, int nslices) {
   s.NT = (int)blockDim.x;
   s.BS = (p.B + nslices - 1) / nslices;
   s.rank = ptx::cluster_ctarank();
-  const int cid = blockIdx.x / s.C;
+  const int cid = (blockIdx.x / s.C) % (p.D * nslices);  // clusters: model-major (anyh_model), direction, slice
   s.dir = cid / nslices;
   s.slice = cid - s.dir * nslices;
   s.b0 = s.slice * s.BS;
@@ -83,6 +83,12 @@ __device__ __forceinline__ AnyhSlice anyh_slice(const Params& p, int nslices) {
   s.active = s.u < s.n;
   if (!s.active) s.u = 0;
   return s;
+}
+
+// The model of this CTA's cluster when one launch runs several (RecModels): clusters are model-major
+template <typename Params>
+__device__ __forceinline__ int anyh_model(const Params& p, int nslices) {
+  return (int)(blockIdx.x / (cluster_nctarank() * p.D * nslices));
 }
 
 // Thread 0: the [2][C] exchange barriers, one arrival (the local arm) per phase
@@ -209,7 +215,7 @@ __device__ __forceinline__ void stage_rows16(WT* W_s, const WT* __restrict__ src
 // =================================================================================================
 // Shared memory: [W_s: G*n x (H+4), ONCHIP only] [h: 2 x BS x H] [bars: 2 x C]
 template <int MODE, bool VL, bool ONCHIP>
-__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdParams p, const int nslices) {
+__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdParams p, const int nslices, const RecModels mdl) {
   constexpr int G = gates_of(MODE);
   const int H = p.H, B = p.B, LD = H + 4;
   const bool relu = p.mode == B200RNN_RNN_RELU;  // Elman
@@ -221,7 +227,17 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
   float* h_s = W_s + (ONCHIP ? (size_t)G * HS * LD : 0);
   uint64_t* bars = reinterpret_cast<uint64_t*>(h_s + (size_t)2 * BS * H);
   const int tid = threadIdx.x;
-  const float* w_hh = p.w_hh[dir];
+  // this cluster's model: every pointer offset by the model's block (0 for model 0, or for a shared tensor). The GRU's
+  // L2 tier, which has no register to spare in its step loop, reads the index again from the launch registers each time
+  constexpr bool REMAT = !ONCHIP && MODE == B200RNN_GRU;
+  const int m = mdl.M > 1 ? anyh_model(p, nslices) : 0;
+  auto moff = [&](long long stride) {
+    if constexpr (!REMAT) return (long long)m * stride;
+    return mdl.M > 1 ? (long long)anyh_model(p, nslices) * stride : 0ll;
+  };
+  const float* w_hh = p.w_hh[dir] + m * (dir ? mdl.whh[1] : mdl.whh[0]);
+  const float* h_0 = p.h_0 ? p.h_0 + m * mdl.state : nullptr;
+  const float* c_0 = p.c_0 ? p.c_0 + m * mdl.state : nullptr;
 
   if (tid == 0) init_bars(bars, C);
   if constexpr (ONCHIP) {
@@ -234,7 +250,7 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
     const int q = i / H, k = i - q * H;
     const int slot = b0 + q;
     float v = 0.f;
-    if (p.h_0 && slot < B) v = p.h_0[((size_t)dir * B + (VL ? p.order[slot] : slot)) * H + k];
+    if (h_0 && slot < B) v = h_0[((size_t)dir * B + (VL ? p.order[slot] : slot)) * H + k];
     h_s[i] = v;
   }
   __syncthreads();
@@ -245,18 +261,17 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
   const int row = valid ? (VL ? p.order[slot] : slot) : 0;
   const int len = (VL && valid) ? p.lengths[row] : p.T;
   float* gates = p.gates[dir];
-  float h = (p.h_0 && valid) ? p.h_0[((size_t)dir * B + row) * H + j] : 0.f;
-  float c = (MODE == B200RNN_LSTM && p.c_0 && valid) ? p.c_0[((size_t)dir * B + row) * H + j] : 0.f;
-  const float bhn = MODE == B200RNN_GRU ? p.b_hh[dir][2 * H + j] : 0.f;
+  float h = (h_0 && valid) ? h_0[((size_t)dir * B + row) * H + j] : 0.f;
+  float c = (MODE == B200RNN_LSTM && c_0 && valid) ? c_0[((size_t)dir * B + row) * H + j] : 0.f;
+  const float bhn = MODE == B200RNN_GRU ? p.b_hh[dir][m * (dir ? mdl.bhh[1] : mdl.bhh[0]) + 2 * H + j] : 0.f;
   float gi[G];
   // Elman: 0 until the first load, the register allocation its timings (tools/elman_steps_results.json) were taken with
   if constexpr (G == 1) gi[0] = 0.f;
   auto load_gi = [&](int t) {
 #pragma unroll
-    for (int g = 0; g < G; ++g) gi[g] = valid ? gates[((size_t)t * B + row) * (G * H) + g * H + j] : 0.f;
+    for (int g = 0; g < G; ++g) gi[g] = valid ? gates[moff(mdl.saved) + ((size_t)t * B + row) * (G * H) + g * H + j] : 0.f;
   };
   if (T > 0) load_gi(dir ? T - 1 : 0);
-  const float* wrow = ONCHIP ? W_s + (size_t)u * LD : w_hh + (size_t)(j0 + u) * H;
   const size_t wg = ONCHIP ? (size_t)n * LD : (size_t)H * H;
 
   for (int step = 0; step < T; ++step) {
@@ -267,6 +282,9 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
     float acc[G];
 #pragma unroll
     for (int g = 0; g < G; ++g) acc[g] = 0.f;
+    // the L2 tier reads this model's weight_hh in place (its address formed per step where REMAT)
+    const float* wrow = ONCHIP ? W_s + (size_t)u * LD
+                               : p.w_hh[dir] + moff(dir ? mdl.whh[1] : mdl.whh[0]) + (size_t)(j0 + u) * H;
     dot_rows<G, ONCHIP, false>(wrow, wg, h_s + ((size_t)cur * BS + b) * H, 0, H, acc);
 
     float hnew, sg[G], sx;
@@ -286,12 +304,12 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
     }
     h = hnew;
     if (valid) {
-      if (p.y) p.y[(long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = frozen ? 0.f : hnew;
+      if (p.y) p.y[moff(mdl.y) + (long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = frozen ? 0.f : hnew;
       if (p.training) {  // the activated gates over the x-projection, and GRU W_hn h + b_hn / LSTM c_t (Elman: h_t)
-        float* gp = gates + ((size_t)t * B + row) * (G * H) + j;
+        float* gp = gates + moff(mdl.saved) + ((size_t)t * B + row) * (G * H) + j;
 #pragma unroll
         for (int g = 0; g < G; ++g) gp[g * H] = sg[g];
-        if constexpr (G > 1) p.extra[dir][((size_t)t * B + row) * H + j] = sx;
+        if constexpr (G > 1) p.extra[dir][moff(mdl.saved) + ((size_t)t * B + row) * H + j] = sx;
       }
     }
     if (step + 1 < T) {
@@ -303,10 +321,10 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_fwd_kernel(const RecFwdPa
     }
   }
   if (valid) {
-    p.h_n[((size_t)dir * B + row) * H + j] = h;
-    if (MODE == B200RNN_LSTM && p.c_n) p.c_n[((size_t)dir * B + row) * H + j] = c;
+    p.h_n[moff(mdl.state) + ((size_t)dir * B + row) * H + j] = h;
+    if (MODE == B200RNN_LSTM && p.c_n) p.c_n[moff(mdl.state) + ((size_t)dir * B + row) * H + j] = c;
     if (VL && p.y)  // the steps [T, p.T) the cluster skipped emit 0, as past any sequence's length
-      for (int t = T; t < p.T; ++t) p.y[(long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = 0.f;
+      for (int t = T; t < p.T; ++t) p.y[moff(mdl.y) + (long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] = 0.f;
   }
   ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
 }
@@ -421,7 +439,7 @@ __device__ __forceinline__ void anyh_fwd_body(const RecFwdParams p, const int ns
 
 // 16-bit weight_hh (__half or __nv_bfloat16): half the shared memory per weight row, so more hidden sizes stay on chip
 template <int MODE, bool VL, bool ONCHIP, typename WT>
-__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_fwd_kernel(const RecFwdParams p, const int nslices) {
+__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_fwd_kernel(const RecFwdParams p, const int nslices, const RecModels) {
   anyh_fwd_body<MODE, VL, ONCHIP, WT>(p, nslices);
 }
 
@@ -432,7 +450,7 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_fwd_kernel(const RecFwd
 // Step s: dh = direct_{s-1} + sum_g W_hh[g-block]^T dgh_{s-1} (the exchange of step s - 1, all G*H columns), the cell
 // backward, then this CTA's dgh (GRU: n-block dn * r; Elman: dpre) to every CTA. Step T only contracts, for dh_0.
 template <int MODE, bool VL, bool ONCHIP>
-__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdParams p, const int nslices) {
+__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdParams p, const int nslices, const RecModels mdl) {
   constexpr int G = gates_of(MODE);
   constexpr int NP = G == 1 ? 1 : G + 1;  // bias-partial blocks per slice: dGi (+ the GRU dghn block, 0 for the LSTM)
   const int H = p.H, B = p.B, LD = H + 4, GH = G * H;
@@ -447,7 +465,9 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
   uint64_t* bars = reinterpret_cast<uint64_t*>(red + (size_t)BS * NP * HS);
   const int tid = threadIdx.x;
   // rows (g, u) of this CTA: W_hh[g*H + :][j0 + u], contiguous from G * j0 * H (whh_prep_kernel)
-  const float* w_prep = p.w_prep[dir] + (size_t)G * j0 * H;
+  // this cluster's model: every pointer offset by the model's block (0 for model 0, or for a shared tensor)
+  const long long m = mdl.M > 1 ? anyh_model(p, nslices) : 0;
+  const float* w_prep = p.w_prep[dir] + m * (dir ? mdl.wprep[1] : mdl.wprep[0]) + (size_t)G * j0 * H;
 
   if (tid == 0) init_bars(bars, C);
   if constexpr (ONCHIP) stage_rows(W_s, w_prep, G * n, H, NT, [&](int r) { return (size_t)r * H; });
@@ -458,21 +478,29 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
   const bool valid = s.active && slot < B;
   const int row = valid ? (VL ? p.order[slot] : slot) : 0;
   const int len = (VL && valid) ? p.lengths[row] : T;
-  const float* gates = p.gates[dir];
-  const float* extra = p.extra[dir];
-  float* dgates = p.dgates[dir];
+  const float* gates = p.gates[dir] + m * mdl.saved;
+  const float* extra = p.extra[dir] ? p.extra[dir] + m * mdl.saved : nullptr;
+  float* dgates = p.dgates[dir] + m * mdl.scr;
+  float* dghn = p.dghn[dir] ? p.dghn[dir] + m * mdl.scr : nullptr;
+  const float* y = p.y + m * mdl.y;
+  const float* dy = p.dy + m * mdl.dy;
+  const float* dh_n = p.dh_n ? p.dh_n + m * mdl.state : nullptr;
+  const float* dc_n = p.dc_n ? p.dc_n + m * mdl.state : nullptr;
+  float* dh_0 = p.dh_0 ? p.dh_0 + m * mdl.state : nullptr;
+  float* dc_0 = p.dc_0 ? p.dc_0 + m * mdl.state : nullptr;
   const float* wrow = ONCHIP ? W_s + (size_t)u * LD : w_prep + (size_t)u * H;
   const size_t wg = ONCHIP ? (size_t)n * LD : (size_t)n * H;
 
   float dh_carry = 0.f, dc_carry = 0.f, direct = 0.f;
   if (valid) {
-    if (p.dh_n) dh_carry = p.dh_n[((size_t)dir * B + row) * H + j];
-    if (MODE == B200RNN_LSTM && p.dc_n) dc_carry = p.dc_n[((size_t)dir * B + row) * H + j];
+    if (dh_n) dh_carry = dh_n[((size_t)dir * B + row) * H + j];
+    if (MODE == B200RNN_LSTM && dc_n) dc_carry = dc_n[((size_t)dir * B + row) * H + j];
   }
   float bsum[NP] = {};
   // saved gates (Elman: h_t), hn / c_t, h_{prev} / c_{prev}, dy (prefetched)
   float sv[G] = {}, sx = 0.f, hp = 0.f, dyv = 0.f;
   const float* s0 = MODE == B200RNN_GRU ? p.h_0 : p.c_0;  // the state before the first step (zeros when NULL)
+  if (s0) s0 += m * mdl.state;
   auto load_step = [&](int step) {
     const int t = dir ? step : (T - 1 - step);
     const int tp = dir ? t + 1 : t - 1;
@@ -481,18 +509,18 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
 #pragma unroll
     for (int g = 0; g < G; ++g) sv[g] = gates[((size_t)t * B + row) * GH + g * H + j];
     if constexpr (G > 1) sx = extra[((size_t)t * B + row) * H + j];
-    dyv = p.dy[(long long)t * p.dy_st + (long long)row * p.dy_sb + dir * H + j];
+    dyv = dy[(long long)t * p.dy_st + (long long)row * p.dy_sb + dir * H + j];
     if constexpr (G > 1) {
       if (!has_prev)
         hp = s0 ? s0[((size_t)dir * B + row) * H + j] : 0.f;
       else if (MODE == B200RNN_GRU)
-        hp = p.y[(long long)tp * p.y_st + (long long)row * p.y_sb + dir * H + j];
+        hp = y[(long long)tp * p.y_st + (long long)row * p.y_sb + dir * H + j];
       else
         hp = extra[((size_t)tp * B + row) * H + j];
     }
   };
   if (valid && T > 0) load_step(0);
-  const bool want_dh0 = p.dh_0 != nullptr;
+  const bool want_dh0 = dh_0 != nullptr;
 
   for (int step = 0; step <= T; ++step) {
     if (step > 0) {  // dh of this step from the gate gradients step - 1 sent
@@ -540,7 +568,7 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
       float* gp = dgates + ((size_t)t * B + row) * GH + j;
 #pragma unroll
       for (int g = 0; g < G; ++g) gp[g * H] = dg[g];
-      if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + row) * H + j] = dhn;
+      if (MODE == B200RNN_GRU) dghn[((size_t)t * B + row) * H + j] = dhn;
     }
     if (!send) break;
     float* d_nxt = d_s + (size_t)nxt * BS * GH;
@@ -556,14 +584,14 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
   // gradients w.r.t. the initial state: what the scan carried past its first step (a cluster that ran no step passes
   // dh_n / dc_n on)
   if (valid) {
-    if (want_dh0) p.dh_0[((size_t)dir * B + row) * H + j] = dh_carry;
-    if (MODE == B200RNN_LSTM && p.dc_0) p.dc_0[((size_t)dir * B + row) * H + j] = dc_carry;
+    if (want_dh0) dh_0[((size_t)dir * B + row) * H + j] = dh_carry;
+    if (MODE == B200RNN_LSTM && dc_0) dc_0[((size_t)dir * B + row) * H + j] = dc_carry;
     if (VL)  // the steps [T, p.T) the cluster skipped: their gate gradients are 0
       for (int t = T; t < p.T; ++t) {
         float* gp = dgates + ((size_t)t * B + row) * GH + j;
 #pragma unroll
         for (int g = 0; g < G; ++g) gp[g * H] = 0.f;
-        if (MODE == B200RNN_GRU) p.dghn[dir][((size_t)t * B + row) * H + j] = 0.f;
+        if (MODE == B200RNN_GRU) dghn[((size_t)t * B + row) * H + j] = 0.f;
       }
   }
   // per-slice bias-gradient partials [nslices][NP * H] (api.cu reduces them): the slice's batch slots summed in slot
@@ -577,7 +605,7 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_bwd_kernel(const RecBwdPa
     for (int g = 0; g < NP; ++g) {
       float v = 0.f;
       for (int q = 0; q < BS; ++q) v += red[((size_t)q * NP + g) * HS + u];
-      float* out = p.dbias_part[dir] + (size_t)s.slice * NP * H;
+      float* out = p.dbias_part[dir] + m * mdl.scr + (size_t)s.slice * NP * H;
       out[g * H + j] = v;
     }
   }
@@ -742,7 +770,7 @@ __device__ __forceinline__ void anyh_bwd_body(const RecBwdParams& p, const int n
 
 // 16-bit transposed weight_hh: half the shared memory per weight row, as in the forward
 template <int MODE, bool VL, bool ONCHIP, typename WT>
-__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_bwd_kernel(const RecBwdParams p, const int nslices) {
+__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_bwd_kernel(const RecBwdParams p, const int nslices, const RecModels) {
   anyh_bwd_body<MODE, VL, ONCHIP, WT>(p, nslices);
 }
 
@@ -763,7 +791,7 @@ size_t anyh_smem(int G, int H, int C, int BS, bool bwd, bool onchip, int wbytes)
 namespace {
 
 template <typename P>
-using AnyhKernel = void (*)(P, int);
+using AnyhKernel = void (*)(P, int, RecModels);
 
 template <int MODE, typename WT>
 AnyhKernel<RecFwdParams> anyh16_kernel(const RecFwdParams&, bool vl, bool onchip) {
@@ -803,7 +831,7 @@ AnyhKernel<P> anyh_kernel_w(const P& p, bool vl, bool onchip, int w16) {
 //     every load): the widest cluster, then the fewest waves, then the fewest batch rows.
 // Capacities come from the driver (cluster_capacity), never from the SM count; clusters that do not fit run in waves.
 template <typename P>
-int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L, int w16) {
+int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L, int w16, int models) {
   const int wbytes = w16 ? 2 : 4;
   const int G = gates_of(p.mode), H = p.H;
   const bool vl = p.lengths != nullptr;
@@ -824,6 +852,8 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L, int w16) {
         if (NT > ANYH_MAX_NT) continue;
         const size_t smem = anyh_smem(G, H, C, BS, bwd, onchip, wbytes);
         if (smem > (size_t)MAX_SMEM) continue;
+        // the shape is chosen as for one model, so that each model computes what it computes alone (the bias
+        // gradient's slice sums included); several models add clusters, in waves when they do not all fit
         const int nslices = (p.B + BS - 1) / BS, nclusters = nslices * p.D;
         int capacity = 0;
         const int rc = cluster_capacity((const void*)kernel, C, NT, smem, &capacity);
@@ -840,10 +870,11 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L, int w16) {
                                                                   (key[1] == best[1] && key[2] < best[2])))) {
           found = true;
           best[0] = key[0]; best[1] = key[1]; best[2] = key[2];
-          pick = ClusterLaunch<P>{kernel, C, NT, nslices, nclusters, capacity, smem};
+          pick = ClusterLaunch<P>{(const void*)kernel, C, NT, nslices, nclusters * models, capacity, smem};
           pick.anyh = true;
           pick.BS = BS;
           pick.onchip = onchip;
+          pick.models.M = models;
         }
       }
     }
@@ -866,21 +897,21 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L, int w16) {
 
 bool anyh_hidden_size(int H) { return H >= 16 && H <= 1024 && H % 16 == 0; }
 
-int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16) {
+int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16, int models) {
   if (p.y_pool || p.ready || p.shell_nograd || p.P > 0) {
     set_error("recurrence: hidden_size %d runs without the model-shell fusions (y_pool, streamed x-projection, "
               "no-grad fused forward) and without proj_size", p.H);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  return plan_anyh(p, false, L, w16);
+  return plan_anyh(p, false, L, w16, models);
 }
 
-int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16) {
+int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16, int models) {
   if (!p.dy || p.P > 0) {
     set_error("recurrence backward: hidden_size %d takes the full output gradient dy and no proj_size", p.H);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  return plan_anyh(p, true, L, w16);
+  return plan_anyh(p, true, L, w16, models);
 }
 
 }  // namespace b200rnn

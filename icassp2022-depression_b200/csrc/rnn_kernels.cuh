@@ -44,11 +44,26 @@ struct RecFwdParams {
   const void* whh16[2];
 };
 
+// Several models in one launch of the runtime-sized kernels (b200rnn_desc::models): model m's clusters follow model
+// m - 1's, and each pointer of the launch's params is offset by m times its model stride here (elements; 0 = shared).
+// The kernels take it beside their params, which keep the layout the fixed configs are compiled against.
+struct RecModels {
+  int M = 1;
+  long long whh[2] = {0, 0};    // weight_hh per direction (backward: for the launcher's transposes, one per distinct one)
+  long long bhh[2] = {0, 0};    // forward: bias_hh per direction
+  long long wprep[2] = {0, 0};  // backward: w_prep per direction
+  long long saved = 0;          // gates and extra (forward: the reserve, or the scratch without save)
+  long long y = 0, dy = 0;      // y; backward: dy
+  long long scr = 0;            // backward: dgates, dghn, dbias_part
+  long long state = 0;          // h_0, c_0, h_n, c_n; backward: dh_n, dc_n, h_0, c_0, dh_0, dc_0
+};
+
 // A recurrence launch chosen for a shape, before anything is enqueued: `nclusters` clusters of C CTAs, of which
-// `capacity` can be co-resident (cudaOccupancyMaxActiveClusters).
+// `capacity` can be co-resident (cudaOccupancyMaxActiveClusters). `kernel` takes (P, int nslices) or, the runtime-sized
+// kernels, (P, int nslices, RecModels).
 template <typename P>
 struct ClusterLaunch {
-  void (*kernel)(P, int);
+  const void* kernel;
   int C, NT, nslices, nclusters, capacity;
   size_t smem;
   // a runtime-sized kernel of rnn_anyh.cu (GRU / LSTM hidden sizes other than 128 / 256, every Elman one): it takes no
@@ -57,6 +72,7 @@ struct ClusterLaunch {
   bool anyh = false;
   int BS = 0;
   bool onchip = false;
+  RecModels models;  // the runtime-sized kernels: the models of the launch (nclusters counts them all)
   int ctas() const { return nclusters * C; }
   bool one_wave() const { return nclusters <= capacity; }
 };
@@ -123,13 +139,15 @@ bool anyh_hidden_size(int H);
 // backward or forward, weight_hh on chip (onchip) in wbytes per weight (4: fp32, 2: 16-bit)
 size_t anyh_smem(int G, int H, int C, int BS, bool bwd, bool onchip, int wbytes);
 // w16: the storage of weight_hh, 0 (fp32) or DT_F16 / DT_BF16 (h16.cuh): the 16-bit kernels stage half the bytes
-int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* out, int w16 = 0);
-int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out, int w16 = 0);
+// models: M > 1 runs M models in one launch
+int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* out, int w16 = 0, int models = 1);
+int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* out, int w16 = 0, int models = 1);
 
 // forward: choose the config for p's shape (mode, H, P, B, D, lengths or not), then launch it; p.ready != NULL launches
 // it with programmatic stream serialization, so that it may start while the GEMM before it still runs
 // w16: the storage of p.w_hh (see plan_anyh_fwd), taken by the runtime-sized kernels; the fixed configs read fp32
-int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* out, int w16 = 0);
+// models > 1: that many models in one launch of the runtime-sized kernels (the caller fills out->models' strides)
+int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* out, int w16 = 0, int models = 1);
 int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t stream);
 // W_hh [3*256][256] of a GRU-256 layer (16-byte aligned) -> h16::Gru256::CACHE_BYTES at img (256-byte aligned): the
 // fp16 pairs and row scales the prologue of rec_fwd_h16_kernel would make, in its shared-memory order per CTA rank
@@ -138,7 +156,9 @@ int prep_whh_h16(const float* w_hh, void* img, cudaStream_t stream);
 // p.nslices_out
 // whh16 (optional, with w16 != 0): per direction the 16-bit weight_hh; when the runtime-sized kernels run, W_hh is
 // transposed from it in 16 bits and staged as such (p.w_prep then holds 16-bit data); otherwise p.w_hh (fp32) is used
-int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* out, int w16 = 0);
-int launch_rec_bwd(RecBwdParams& p, cudaStream_t stream, int w16 = 0, const void* const* whh16 = nullptr);
+// models (optional): several models in one launch, as in plan_rec_fwd
+int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* out, int w16 = 0, int models = 1);
+int launch_rec_bwd(RecBwdParams& p, cudaStream_t stream, int w16 = 0, const void* const* whh16 = nullptr,
+                   const RecModels* models = nullptr);
 
 }  // namespace b200rnn

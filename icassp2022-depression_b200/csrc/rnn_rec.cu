@@ -1730,7 +1730,7 @@ bool pick_clustered(void (*kernel)(P, int), const P& p, int C, int BS, int NT, s
     fprintf(stderr, "[b200rnn] %s: need %d clusters, capacity %d, smem %zu\n", what, nclusters, capacity, smem);
   }
   if (!force && nclusters > capacity) return false;
-  *L = ClusterLaunch<P>{kernel, C, NT, nslices, nclusters, capacity, smem};
+  *L = ClusterLaunch<P>{(const void*)kernel, C, NT, nslices, nclusters, capacity, smem};
   return true;
 }
 
@@ -1739,7 +1739,11 @@ int launch_clustered(const ClusterLaunch<P>& L, const P& p, int prof_kind, bool 
   ProfScope prof(prof_kind, s);
   cudaLaunchAttribute attr[2];
   const cudaLaunchConfig_t cfg = cluster_config(L.nclusters, L.C, L.NT, L.smem, s, attr, programmatic);
-  const cudaError_t e = cudaLaunchKernelEx(&cfg, L.kernel, p, L.nslices);
+  // (P, int) kernels read the first two arguments, the runtime-sized ones all three
+  int nslices = L.nslices;
+  RecModels models = L.models;
+  void* args[3] = {const_cast<P*>(&p), &nslices, &models};
+  const cudaError_t e = cudaLaunchKernelExC(&cfg, L.kernel, args);
   if (e != cudaSuccess) {
     set_error("cudaLaunchKernelEx of a recurrence kernel failed: %s", cudaGetErrorString(e));
     return B200RNN_ERR_CUDA;
@@ -1845,7 +1849,7 @@ int cluster_capacity(const void* kernel, int C, int NT, size_t smem, int* capaci
 // (one wave => every sequence advances in lock step) wins, else the widest one runs in several waves.
 // Template arguments: <MODE, H, C, BS, KL, UPL, RG>; projected: <H, P, C, BS>, H = 128 on 2-CTA clusters of 4 batch rows
 // (256 threads), H = 256 on 4-CTA clusters of 8 batch rows (512 threads).
-int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16) {
+int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16, int models) {
   int rc = B200RNN_OK;
   L->kernel = nullptr;
   if (p.B <= 0 || p.T <= 0) return rc;
@@ -1858,8 +1862,9 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16) {
               "proj_size hidden_size/4 or hidden_size/2", p.mode, p.H, p.P);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  // the Elman modes run the runtime-sized kernels at every hidden size, 128 and 256 included (rnn_anyh.cu)
-  if (is_elman(p.mode)) return plan_anyh_fwd(p, L, w16);
+  // the Elman modes and several models in one launch run the runtime-sized kernels at every hidden size, 128 and 256
+  // included (rnn_anyh.cu)
+  if (is_elman(p.mode) || models > 1) return plan_anyh_fwd(p, L, w16, models);
   // One config per shape plus a wider-batch fallback that runs in several waves when the batch needs more clusters
   // than fit the chip.
   if (p.mode == B200RNN_GRU && p.H == 256) {
@@ -1904,7 +1909,7 @@ int plan_rec_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16) {
 }
 
 // The same rule and projected configs as the forward
-int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16) {
+int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16, int models) {
   int rc = B200RNN_OK;
   L->kernel = nullptr;
   if (p.B <= 0 || p.T <= 0) return rc;
@@ -1916,7 +1921,7 @@ int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16) {
     set_error("recurrence backward: unsupported projection (mode=%d, hidden_size=%d, proj_size=%d)", p.mode, p.H, p.P);
     return B200RNN_ERR_UNSUPPORTED;
   }
-  if (is_elman(p.mode)) return plan_anyh_bwd(p, L, w16);
+  if (is_elman(p.mode) || models > 1) return plan_anyh_bwd(p, L, w16, models);
   // K across all 32 lanes with 8 units per lane halves the redundant reads of the [BS][G*H] gradient vector, which
   // (not the weights) dominates the shared-memory traffic of the backward contraction
   if (p.mode == B200RNN_GRU && p.H == 256) {
@@ -2012,25 +2017,30 @@ __global__ void whh_prep16_kernel(const uint16_t* __restrict__ w_hh, uint16_t* _
 
 }  // namespace
 
-int launch_rec_bwd(RecBwdParams& p, cudaStream_t s, int w16, const void* const* whh16) {
+int launch_rec_bwd(RecBwdParams& p, cudaStream_t s, int w16, const void* const* whh16, const RecModels* models) {
   RecBwdLaunch L;
   if (!whh16) w16 = 0;
-  const int rc = plan_rec_bwd(p, &L, w16);
+  const int rc = plan_rec_bwd(p, &L, w16, models ? models->M : 1);
   if (rc != B200RNN_OK || L.kernel == nullptr) return rc;
+  if (models) L.models = *models;
+  const RecModels& ms = L.models;
   if (p.P == 0) {  // the unprojected kernels read W_hh transposed for the chosen cluster width
-    for (int d = 0; d < p.D; ++d) {
-      if (L.anyh && w16)
-        whh_prep16_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(static_cast<const uint16_t*>(whh16[d]),
-                                                          reinterpret_cast<uint16_t*>(p.w_prep[d]), gates_of(p.mode),
-                                                          p.H, L.C);
-      else
-        whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d], p.w_prep[d], gates_of(p.mode), p.H, L.C);
-      if (cudaGetLastError() != cudaSuccess) {
-        set_error("whh_prep launch failed");
-        return B200RNN_ERR_CUDA;
+    for (int d = 0; d < p.D; ++d)
+      for (int m = 0; m < ms.M; ++m) {  // once per distinct weight_hh: a shared one once
+        if (m > 0 && ms.whh[d] == 0) break;
+        if (L.anyh && w16)
+          whh_prep16_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(static_cast<const uint16_t*>(whh16[d]),
+                                                            reinterpret_cast<uint16_t*>(p.w_prep[d]), gates_of(p.mode),
+                                                            p.H, L.C);
+        else
+          whh_prep_kernel<<<NUM_SMS, dim3(32, 8), 0, s>>>(p.w_hh[d] + m * ms.whh[d], p.w_prep[d] + m * ms.wprep[d],
+                                                          gates_of(p.mode), p.H, L.C);
+        if (cudaGetLastError() != cudaSuccess) {
+          set_error("whh_prep launch failed");
+          return B200RNN_ERR_CUDA;
+        }
+        count_launch();
       }
-      count_launch();
-    }
   }
   p.nslices_out = L.nslices;
   return launch_clustered(L, p, PROF_REC_BWD, false, s);

@@ -88,6 +88,9 @@ enum {
                                              to it with B200RNN_FLAG_ACCUMULATE_GRADS). Alone: B200RNN_ERR_INVALID. With
                                              B200RNN_FLAG_PROJ, in the _fused entry points and the weight cache:
                                              B200RNN_ERR_UNSUPPORTED. b200rnn_workspace_bytes sizes the rounded images. */
+#define B200RNN_FLAG_MODELS 512u          /* the descriptor carries `models` and `model_strides`: one call runs M independent
+                                             models of the same shape (an ensemble, or per-sample gradients). Without this
+                                             flag neither field is read. See `models` below. */
 
 /*
  * Problem descriptor. Mirrors the constructor arguments of torch.nn.GRU / torch.nn.LSTM
@@ -113,6 +116,19 @@ typedef struct b200rnn_desc {
                           y is [T, B, D*P], h_0 / h_n / dh_0 / dh_n are [L*D, B, P], c_0 / c_n stay [L*D, B, H].
                           Only the plain and the _hx entry points take it (the _fused ones and the weight cache
                           return B200RNN_ERR_UNSUPPORTED).                                                         */
+  int32_t models;      /* M >= 1, read only with B200RNN_FLAG_MODELS (1 without it). Model m's tensors follow model 0's:
+                            x, every parameter and rng_state at m * model_strides[i] elements (0 = shared by all
+                            models); everything else at m times its one-model size: y and dy [T,B,D*H] (the per-model
+                            strides as given), dx [T,B,I] (strides as given), h_0 / c_0 / h_n / c_n / dh_n / dc_n /
+                            dh_0 / dc_0 [L*D,B,H], each dparams target its parameter's element count, and reserve /
+                            scratch M blocks of the one-model size (b200rnn_workspace_bytes returns M times it).
+                            Each recurrence layer runs all models in one launch (runtime-sized kernels at every
+                            hidden size); the GEMMs and the dropout run per model. M > 1 is fp32 only, without
+                            proj_size, lengths, the model-shell entry points or B200RNN_FLAG_ACCUMULATE_GRADS. */
+  const int64_t* model_strides; /* host array, read only with B200RNN_FLAG_MODELS: [0] x, [2 + i] params[i], in
+                            elements; [1] rng_state in uint64 elements: > 0 one state per model; 0 one shared state,
+                            advanced once, every model drawing the same masks; -1 one shared state, advanced M times,
+                            model m drawing the masks the m-th of M consecutive one-model calls would */
 } b200rnn_desc;
 
 /* ABI version of the loaded library (== B200RNN_ABI_VERSION). */
