@@ -40,6 +40,8 @@ SYMBOLS = (
     "b200rnn_backward",
     "b200rnn_backward_fused",
     "b200rnn_backward_hx",
+    "b200rnn_tangent_workspace_bytes",
+    "b200rnn_forward_tangent",
     "b200rnn_wcache_bytes",
     "b200rnn_prepare_weights",
     "b200rnn_cell_workspace_bytes",
@@ -230,6 +232,22 @@ def load() -> ctypes.CDLL:
         c_void_p,                                    # lengths
         c_void_p,                                    # stream
     ]
+    lib.b200rnn_tangent_workspace_bytes.restype = c_int
+    lib.b200rnn_tangent_workspace_bytes.argtypes = [POINTER(Desc), POINTER(c_size_t)]
+    lib.b200rnn_forward_tangent.restype = c_int
+    lib.b200rnn_forward_tangent.argtypes = [
+        POINTER(Desc), c_void_p, c_int64, c_int64,   # desc, x, strides
+        POINTER(c_void_p),                           # params
+        c_void_p, c_int64, c_int64,                  # y
+        c_void_p, c_void_p,                          # h_0, c_0
+        c_void_p, c_void_p,                          # reserve, lengths
+        c_void_p, POINTER(c_void_p),                 # x_dot, params_dot
+        c_void_p, c_void_p,                          # h_0_dot, c_0_dot
+        c_void_p, c_int64, c_int64,                  # y_dot
+        c_void_p, c_void_p,                          # h_n_dot, c_n_dot
+        c_void_p,                                    # scratch
+        c_void_p,                                    # stream
+    ]
     lib.b200rnn_backward_fused.restype = c_int
     lib.b200rnn_backward_fused.argtypes = [
         POINTER(Desc), c_void_p, c_int64, c_int64,   # desc, x, strides
@@ -342,6 +360,13 @@ def workspace_bytes(desc: Desc) -> tuple[int, int]:
     r, s = c_size_t(0), c_size_t(0)
     check(load().b200rnn_workspace_bytes(ctypes.byref(desc), ctypes.byref(r), ctypes.byref(s)), "workspace_bytes")
     return int(r.value), int(s.value)
+
+
+def tangent_workspace_bytes(desc: Desc) -> int:
+    """scratch bytes of a b200rnn_forward_tangent call; raises with the library's message for a refused descriptor"""
+    s = c_size_t(0)
+    check(load().b200rnn_tangent_workspace_bytes(ctypes.byref(desc), ctypes.byref(s)), "tangent_workspace_bytes")
+    return int(s.value)
 
 
 def cell_workspace_bytes(desc: CellDesc) -> tuple[int, int]:

@@ -15,6 +15,13 @@ expanded into a dense block. Inter-layer dropout follows vmap's ``randomness``: 
 from an unbatched one, the mask the m-th of M consecutive one-model calls would draw; ``'same'`` applies one mask to
 every model and needs an unbatched state. Each state advances as the Python loop over the models would advance it.
 
+Forward mode: ``torch.func.jvp`` / ``jacfwd`` (and eager ``torch.autograd.forward_ad`` dual tensors, through
+``functional._RNNFunction.jvp``) compute the tangent with :class:`_Tangent`, one ``b200rnn_forward_tangent`` call over the
+reserve the forward kept: the tangent pre-activations by the time-parallel GEMMs, then one tangent recurrence launch per
+layer. ``jacfwd`` vmaps the jvp over M tangent directions: :meth:`_Tangent.vmap` passes them to the library as one call,
+each recurrence layer running all M in one launch, the primal shared. Second-order products (``hessian``,
+``jvp(grad(f))``, the gradient of a tangent) raise ``B200RNNError``.
+
 The one call is not always the faster one (README, tools/ensemble_steps_results.json): it wins for small batches from a
 handful of models on and for per-sample gradients, and loses for one model (the transform's host cost) and for large
 batches at hidden sizes 128 / 256, where a loop runs the fixed configs tuned for them and the ensemble the
@@ -94,6 +101,7 @@ class _Forward(torch.autograd.Function):
         ctx.cfg = cfg
         if save:
             ctx.save_for_backward(x_tm, y, reserve, h_0, c_0, *weights)
+            ctx.save_for_forward(x_tm, y, reserve, h_0, c_0, *weights)
 
     @staticmethod
     def backward(ctx, dy, dh_n, dc_n, _dreserve):
@@ -107,6 +115,12 @@ class _Forward(torch.autograd.Function):
         keep = lambda g, n: g if n else None  # noqa: E731
         return (keep(dx, needs[0]), None, None, None, keep(dh_0, needs[1]), keep(dc_0, needs[2]),
                 *(keep(g, n) for g, n in zip(dws, needs[3:])))
+
+    @staticmethod
+    def jvp(ctx, x_dot, _cfg, _rng, _save, h0_dot, c0_dot, *w_dots):
+        x_tm, y, reserve, h_0, c_0, *weights = ctx.saved_tensors
+        y_dot, h_n_dot, c_n_dot = tangent(ctx.cfg, x_tm, y, reserve, h_0, c_0, x_dot, h0_dot, c0_dot, weights, w_dots)
+        return y_dot, h_n_dot, c_n_dot if c_n_dot is not None else None, None
 
     @staticmethod
     def vmap(info, in_dims, x_tm, cfg, rng_state, save, h_0, c_0, *weights):
@@ -169,11 +183,20 @@ class _Backward(torch.autograd.Function):
         raise _lib.B200RNNError("b200rnn: the recurrence's backward is not differentiable (no double backward)")
 
     @staticmethod
+    def jvp(ctx, *tangents):
+        raise _lib.B200RNNError("b200rnn: forward-over-reverse (hessian, jvp of grad) is not supported: the "
+                                "recurrence's backward has no forward-mode derivative")
+
+    @staticmethod
     def vmap(info, in_dims, cfg, needs, x_tm, y, reserve, h_0, c_0, dy, dh_n, dc_n, *weights):
         M = info.batch_size
         if cfg.models > 1:
             raise _lib.B200RNNError("b200rnn: nested vmap over a recurrent module is not supported")
         _, _, x_dim, y_dim, r_dim, h_dim, c_dim, dy_dim, dhn_dim, dcn_dim, *w_dims = in_dims
+        # still wrapped below this vmap: a jvp (hessian = jacfwd(jacrev)) differentiates the backward in forward mode
+        if any(torch._C._functorch.is_functorch_wrapped_tensor(t) for t in (x_tm, y, dy, *weights) if t is not None):
+            raise _lib.B200RNNError("b200rnn: forward-over-reverse (hessian, jvp of grad) is not supported: the "
+                                    "recurrence's backward has no forward-mode derivative")
         cfg_m = dataclasses.replace(cfg, models=M) if M > 1 else cfg
         x_m = _to_models(x_tm, x_dim, M, dense=False)
         if x_m.stride(-1) != 1 and x_m.size(-1) != 1:
@@ -186,6 +209,53 @@ class _Backward(torch.autograd.Function):
         wanted = (needs[0], needs[1] and h_0 is not None, needs[2] and c_0 is not None, *needs[3:])
         out_dims = tuple(0 if n else None for n in wanted)
         return _with_model_dim(out, out_dims, M), out_dims
+
+
+class _Tangent(torch.autograd.Function):
+    """``(y', h_n', c_n')`` of :class:`_Forward` (``c_n'`` an empty stand-in but for the LSTM) from the primal's
+    ``x_tm``, ``y``, ``reserve`` and states and the tangents of ``x_tm``, ``h_0``, ``c_0`` and each weight (None = 0;
+    ``weights_and_dots`` is the weights, then one tangent per weight). Not differentiable."""
+
+    @staticmethod
+    def forward(cfg, x_tm, y, reserve, h_0, c_0, x_dot, h0_dot, c0_dot, *weights_and_dots):
+        n = len(weights_and_dots) // 2
+        y_dot, h_n_dot, c_n_dot = F._rnn_tangent_impl(cfg, x_tm, y, reserve, h_0, c_0, weights_and_dots[:n], x_dot,
+                                                      h0_dot, c0_dot, weights_and_dots[n:])
+        return y_dot, h_n_dot, c_n_dot if c_n_dot is not None else y_dot.new_empty(0)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise _lib.B200RNNError("b200rnn: reverse-over-forward (the gradient of a jvp tangent) is not supported")
+
+    @staticmethod
+    def vmap(info, in_dims, cfg, x_tm, y, reserve, h_0, c_0, x_dot, h0_dot, c0_dot, *weights_and_dots):
+        """M tangent directions over one primal (``jacfwd``): one library call, each tangent a dense [M, ...] block"""
+        M = info.batch_size
+        n = len(weights_and_dots) // 2
+        _, x_dim, y_dim, r_dim, h_dim, c_dim, xd_dim, hd_dim, cd_dim, *wd = in_dims
+        if any(d is not None for d in (x_dim, y_dim, r_dim, h_dim, c_dim, *wd[:n])):
+            raise _lib.B200RNNError("b200rnn: forward-mode AD over a vmap-batched primal (a jvp inside vmap over "
+                                    "models or samples) is not supported; vmap over the tangents only (jacfwd)")
+        dense = lambda t, d: _to_models(t, d, M, True)  # noqa: E731
+        dots = [dense(t, d) for t, d in zip(weights_and_dots[n:], wd[n:])]
+        y_dot, h_n_dot, c_n_dot = F._rnn_tangent_impl(cfg, x_tm, y, reserve, h_0, c_0, weights_and_dots[:n],
+                                                      dense(x_dot, xd_dim), dense(h0_dot, hd_dim),
+                                                      dense(c0_dot, cd_dim), dots, directions=M)
+        lstm = cfg.mode == _lib.LSTM
+        out = (y_dot, h_n_dot, c_n_dot if lstm else y_dot.new_empty(0))
+        out_dims = (0, 0, 0 if lstm else None)
+        return _with_model_dim(out, out_dims, M), out_dims
+
+
+def tangent(cfg: F.RNNConfig, x_tm, y, reserve, h_0, c_0, x_dot, h0_dot, c0_dot, weights, w_dots):
+    """``(y', h_n', c_n')`` through :class:`_Tangent`, ``c_n'`` None but for the LSTM"""
+    y_dot, h_n_dot, c_n_dot = _Tangent.apply(cfg, x_tm, y, reserve, h_0, c_0, x_dot, h0_dot, c0_dot, *weights,
+                                             *w_dots)
+    return y_dot, h_n_dot, c_n_dot if cfg.mode == _lib.LSTM else None
 
 
 def rnn_forward(x_tm: torch.Tensor, cfg: F.RNNConfig, rng_state: Optional[torch.Tensor], save: bool,

@@ -8,12 +8,17 @@ happens in ``lib/libb200rnn.so``. CPU tensors are rejected — there is no fallb
 from __future__ import annotations
 
 import ctypes
+import dataclasses
 from dataclasses import dataclass
 from typing import Optional, Sequence
 
 import torch
+import torch.autograd.forward_ad as fwAD
 
 from . import _lib
+
+# rnn_forward's `save` when forward-mode AD may ask for a tangent: the forward keeps its reserve whatever autograd needs
+SAVE_FOR_TANGENT = 2
 
 
 @dataclass
@@ -316,6 +321,63 @@ def _rnn_backward_impl(cfg: RNNConfig, x_tm, y, reserve, h_0, c_0, weights, dy, 
     return dx, dh_0, dc_0, grads_out
 
 
+def _rnn_tangent_impl(cfg: RNNConfig, x_tm, y, reserve, h_0, c_0, weights, x_dot, h0_dot, c0_dot, w_dots,
+                      directions: int = 1):
+    """Forward-mode AD of a saving forward (one ``b200rnn_forward_tangent`` call): ``(y', h_n', c_n')`` from the
+    tangents of x (time-major), h_0, c_0 and each weight, each None = 0. ``y'`` is laid out like ``y``, ``c_n'`` None but
+    for the LSTM. ``directions`` = M > 1: every tangent (and output) carries a leading [M] dimension of tangent
+    directions over the one primal, which the library runs in one recurrence launch per layer."""
+    lib = _lib.load()
+    T, B = x_tm.shape[0], x_tm.shape[1]
+    H, L, D = cfg.hidden_size, cfg.num_layers, cfg.num_dirs
+    dev = x_tm.device
+    M = directions
+    lead = (M,) if M > 1 else ()
+    desc = _make_desc(dataclasses.replace(cfg, models=M), B, T, True)
+    sbytes = _lib.tangent_workspace_bytes(desc)
+    scratch = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+    y_dot = torch.empty(*lead, *y.shape, dtype=torch.float32, device=dev)
+    if cfg.batch_first:
+        ys, yds = (D * H, T * D * H), (D * H, T * D * H)
+    else:
+        ys, yds = (B * D * H, D * H), (B * D * H, D * H)
+    h_n_dot = torch.empty(*lead, L * D, B, H, dtype=torch.float32, device=dev)
+    c_n_dot = torch.empty(*lead, L * D, B, H, dtype=torch.float32, device=dev) if cfg.mode == _lib.LSTM else None
+    dense = lambda t: t.contiguous() if t is not None else None  # noqa: E731
+    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    x_dot, h0_dot, c0_dot = dense(x_dot), dense(h0_dot), dense(c0_dot)
+    w_dots = [dense(w) for w in w_dots]
+    params = _lib.ptr_array([w.data_ptr() for w in weights])
+    params_dot = _lib.ptr_array([ptr(w) for w in w_dots]) if any(w is not None for w in w_dots) else None
+    with _on(dev):
+        rc = lib.b200rnn_forward_tangent(
+            ctypes.byref(desc), x_tm.data_ptr(), x_tm.stride(0), x_tm.stride(1), params, y.data_ptr(), *ys,
+            ptr(h_0), ptr(c_0), reserve.data_ptr(), None, ptr(x_dot), params_dot, ptr(h0_dot), ptr(c0_dot),
+            y_dot.data_ptr(), *yds, h_n_dot.data_ptr(), ptr(c_n_dot), scratch.data_ptr(), _stream_ptr(dev))
+    _lib.check(rc, "b200rnn_forward_tangent")
+    return y_dot, h_n_dot, c_n_dot
+
+
+def forward_ad_active(*tensors) -> bool:
+    """Whether any of ``tensors`` is a dual tensor of the current ``torch.autograd.forward_ad`` level, whose tangent
+    forward-mode AD will ask for (the model-shell fusions do not compute one, so they take their unfused expressions)"""
+    if fwAD._current_level < 0:
+        return False
+    return any(t is not None and fwAD.unpack_dual(t).tangent is not None for t in tensors)
+
+
+def check_forward_ad(cfg: RNNConfig, lengths) -> None:
+    """The parts of the sequence path that have no forward mode raise here, before any launch"""
+    if cfg.proj_size:
+        raise _lib.B200RNNError("b200rnn: forward-mode AD (jvp / jacfwd / dual tensors) does not take proj_size")
+    if cfg.dtype != torch.float32 or cfg.master_f32:
+        raise _lib.B200RNNError("b200rnn: forward-mode AD (jvp / jacfwd / dual tensors) runs float32 modules outside "
+                                "torch.autocast only")
+    if lengths is not None:
+        raise _lib.B200RNNError("b200rnn: forward-mode AD (jvp / jacfwd / dual tensors) does not take PackedSequence "
+                                "input")
+
+
 class _RNNFunction(torch.autograd.Function):
     """y, h_n[, c_n] = RNN(x, weights, h_0[, c_0]); x is the logical time-major view [T,B,I], h_0 / c_0 are None
     (zeros) or contiguous [L*D,B,HO] / [L*D,B,H] (HO = proj_size, or H without a projection). A projected LSTM always
@@ -329,14 +391,18 @@ class _RNNFunction(torch.autograd.Function):
                 lengths: Optional[torch.Tensor], save: bool, h_0: Optional[torch.Tensor], c_0: Optional[torch.Tensor],
                 *weights: torch.Tensor):
         # `save` is decided by the caller: grad mode is always off in here, and needs_input_grad is True for
-        # requires_grad weights even under torch.no_grad() (it would allocate the reserve and store gates for nothing)
-        save = bool(save) and any(ctx.needs_input_grad)
+        # requires_grad weights even under torch.no_grad() (it would allocate the reserve and store gates for nothing).
+        # SAVE_FOR_TANGENT: a dual input, whose tangent the jvp below computes from the reserve
+        tangent = save == SAVE_FOR_TANGENT
+        save = tangent or (bool(save) and any(ctx.needs_input_grad))
         y, h_n, c_n, reserve = _rnn_forward_impl(x_tm, cfg, rng_state, lengths, save, h_0, c_0, weights)
         if save:
             ctx.cfg = cfg
             ctx.grad_sink = grad_sink
             ctx.lengths = lengths
             ctx.save_for_backward(x_tm, y, reserve, h_0, c_0, *weights)
+            if tangent:
+                ctx.save_for_forward(x_tm, y, reserve, h_0, c_0, *weights)
         if c_n is None:
             return y, h_n
         return y, h_n, c_n
@@ -344,12 +410,25 @@ class _RNNFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy, dh_n, dc_n=None):
         x_tm, y, reserve, h_0, c_0, *weights = ctx.saved_tensors
+        # under a dual level, a dual output gradient or a dual saved input (x, a weight, h_0 / c_0) asks for the
+        # gradient's own tangent, which the raw-pointer BPTT does not compute: refuse rather than drop it
+        if forward_ad_active(dy, dh_n, dc_n, x_tm, h_0, c_0, *weights):
+            raise _lib.B200RNNError("b200rnn: forward-over-reverse (a jvp of the recurrence's backward, e.g. a "
+                                    "Hessian-vector product) is not supported")
         w0 = _RNNFunction._W0
         need = ctx.needs_input_grad
         dx, dh_0, dc_0, grads_out = _rnn_backward_impl(ctx.cfg, x_tm, y, reserve, h_0, c_0, weights, dy, dh_n, dc_n,
                                                        ctx.lengths, need[0], need[w0 - 2], need[w0 - 1], need[w0:],
                                                        ctx.grad_sink)
         return (dx, None, None, None, None, None, dh_0, dc_0, *grads_out)
+
+    @staticmethod
+    def jvp(ctx, x_dot, _cfg, _rng, _sink, _lengths, _save, h0_dot, c0_dot, *w_dots):
+        """eager ``torch.autograd.forward_ad``: the tangent recurrence over the reserve the forward kept"""
+        x_tm, y, reserve, h_0, c_0, *weights = ctx.saved_tensors
+        y_dot, h_n_dot, c_n_dot = _func.tangent(ctx.cfg, x_tm, y, reserve, h_0, c_0, x_dot, h0_dot, c0_dot, weights,
+                                                w_dots)
+        return (y_dot, h_n_dot) if ctx.cfg.mode != _lib.LSTM else (y_dot, h_n_dot, c_n_dot)
 
 
 class _LNRNNPoolFunction(torch.autograd.Function):
@@ -514,13 +593,16 @@ def rnn_forward(x: torch.Tensor, weights: Sequence[torch.Tensor], cfg: RNNConfig
             raise _lib.B200RNNError(f"b200rnn: weight[{i}] is on {w.device} but the input is on {x.device}")
     states = [s for s in (h_0, c_0) if s is not None]
     save = torch.is_grad_enabled() and (x.requires_grad or any(t.requires_grad for t in (*weights, *states)))
+    if forward_ad_active(x, *weights, *states):   # a dual tensor: keep the reserve for the tangent recurrence
+        check_forward_ad(cfg, lengths)
+        save = SAVE_FOR_TANGENT
     if torch.compiler.is_compiling():   # dynamo / export: the custom op, which traces without a pointer
         if grad_sink is not None:
             _grad_sink_untraceable()
         return _ops.rnn_forward_traced(x_tm, cfg, rng_state, lengths, save, h_0, c_0, weights)
-    if functorch_active():   # torch.func.grad / vmap: wrapped tensors have no pointer (b200rnn/func.py)
+    if functorch_active():   # torch.func.grad / vmap / jvp: wrapped tensors have no pointer (b200rnn/func.py)
         _func.check_supported(cfg, lengths, grad_sink)
-        return _func.rnn_forward(x_tm, cfg, rng_state, save, h_0, c_0, weights)
+        return _func.rnn_forward(x_tm, cfg, rng_state, True, h_0, c_0, weights)
     return _RNNFunction.apply(x_tm, cfg, rng_state, grad_sink, lengths, save, h_0, c_0, *weights)
 
 

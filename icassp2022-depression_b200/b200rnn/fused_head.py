@@ -15,7 +15,7 @@ from typing import Optional
 import torch
 
 from . import _lib
-from .functional import _on, functorch_active, rnn_forward_fused
+from .functional import _on, forward_ad_active, functorch_active, rnn_forward_fused
 from .staging import FuseBatch
 
 
@@ -103,12 +103,12 @@ def attention_pool_tm(attention_layer: torch.nn.Module, seq_tm: torch.Tensor, h_
     """``attention_net_with_w`` (text_bilstm_whole.py:74-99) on the TIME-MAJOR LSTM output ``seq_tm`` [T,B,2H] and
     ``h_n`` [L*D,B,H] -> [B,H]; differentiable (one kernel each way). Falls back to the PyTorch expression only for
     shapes the kernels do not take (T*H beyond one CTA's shared memory), non-CUDA tensors of the oracle tests, and under
-    torch.compile / torch.export, which have no custom op for these kernels, and torch.func transforms."""
+    torch.compile / torch.export, which have no custom op for these kernels, torch.func transforms and forward-mode AD."""
     lin = attention_layer[0]
     T, B, H2 = seq_tm.shape
     fits = (4 * (H2 // 2) + 2 * T + T * (H2 // 2)) * 4 <= 200 * 1024 and (2 * (H2 // 2) + T) * 4 <= 47 * 1024
     if (seq_tm.is_cuda and fits and seq_tm.dtype == torch.float32 and not torch.compiler.is_compiling() and
-            not functorch_active()):
+            not functorch_active() and not forward_ad_active(seq_tm, h_n, lin.weight, lin.bias)):
         return _AttentionPoolFunction.apply(seq_tm, h_n, lin.weight, lin.bias)
     from .models import attention_pool as _generic
 

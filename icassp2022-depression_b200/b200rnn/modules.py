@@ -42,8 +42,8 @@ import torch.nn as nn
 
 from . import _lib
 from .func import check_supported
-from .functional import (CellConfig, RNNConfig, cell_forward, functorch_active, prepare_weights, rnn_forward,
-                         rnn_forward_fused, rnn_ln_pool_sum, tf32_enabled)
+from .functional import (CellConfig, RNNConfig, cell_forward, check_forward_ad, forward_ad_active, functorch_active,
+                         prepare_weights, rnn_forward, rnn_forward_fused, rnn_ln_pool_sum, tf32_enabled)
 
 _TORCH_GRU = nn.GRU
 _TORCH_LSTM = nn.LSTM
@@ -221,6 +221,8 @@ class _B200RNNBase(nn.Module):
         batch is in that order already)."""
         if functorch_active():   # raised before torch's unpacking, which cannot run under torch.func either
             check_supported(cfg, packed.batch_sizes, self._grad_sink)
+        if forward_ad_active(packed.data):   # stock pack_padded_sequence refuses forward AD too
+            check_forward_ad(cfg, packed.batch_sizes)
         rnn_utils = nn.utils.rnn
         padded, lengths = rnn_utils.pad_packed_sequence(packed, batch_first=self.batch_first)
         out = rnn_forward(padded, self._flat_weights, cfg, self._rng_state, self._grad_sink, lengths=lengths, hx=hx)
@@ -291,7 +293,9 @@ class _B200RNNBase(nn.Module):
                                                  or (ln is not None and any(p.requires_grad for p in ln.parameters())))
         # torch.compile / torch.export trace the unfused expression through the custom ops (b200rnn/ops.py), and so does
         # a call under torch.autocast (the fusions are fp32 only); torch.func transforms compute it through b200rnn/func.py
+        # and so does forward-mode AD (a dual input or parameter)
         shape_ok = (not torch.compiler.is_compiling() and not functorch_active() and self._autocast_dtype() is None and
+                    not forward_ad_active(input, *self.parameters(), *(ln.parameters() if ln is not None else ())) and
                     input.is_cuda and input.dim() == 3 and self.proj_size == 0 and
                     self._gates > 1 and self._flat_weights[0].dtype == torch.float32 and
                     self.hidden_size in (128, 256) and

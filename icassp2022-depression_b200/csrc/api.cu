@@ -1681,6 +1681,236 @@ B200RNN_API int b200rnn_backward(const b200rnn_desc* desc, const float* x, int64
                        nullptr, nullptr, stream_);
 }
 
+// The descriptor of a tangent call: what forward mode does not run is refused before anything else
+static int check_tangent_desc(const b200rnn_desc* desc, Dims* d) {
+  if (desc && desc_proj(desc) != 0) {
+    set_error("forward_tangent: proj_size is not supported in forward mode");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  if (desc && (desc->flags & (B200RNN_FLAG_F16 | B200RNN_FLAG_BF16 | B200RNN_FLAG_F32_PARAMS))) {
+    set_error("forward_tangent: forward mode is float32 only (no B200RNN_FLAG_F16 / _BF16 / _F32_PARAMS)");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  if (desc && (desc->flags & B200RNN_FLAG_FUSED_LN)) {
+    set_error("forward_tangent: the model-shell fusions (B200RNN_FLAG_FUSED_LN) are not supported in forward mode");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  return check_desc(desc, d);
+}
+
+// Scratch of b200rnn_forward_tangent (floats): one tensor-core GEMM workspace shared by every GEMM of the call (they run
+// one after the other on the stream), then per tangent direction its pre-activations (per layer direction [T,B,G*H]),
+// the GRU's n-block h side ([T,B,H]) and the two buffers of an inner layer's tangent output ([T,B,D*H])
+struct TangentLayout {
+  size_t tc_ws, tc_ws_bytes;
+  size_t pre[2], preh[2], ybuf[2];  // offsets within a direction's block
+  size_t block, total;
+};
+
+static void make_tangent_layout(const Dims& d, TangentLayout* t) {
+  const size_t g0 = gemm_tc_scratch_bytes((int)d.TB, (int)d.GH, d.I);
+  const size_t g1 = gemm_tc_scratch_bytes((int)d.TB, (int)d.GH, (int)d.DH);
+  t->tc_ws_bytes = g0 > g1 ? g0 : g1;
+  t->tc_ws = 0;
+  size_t off = 0;
+  for (int k = 0; k < 2; ++k) {
+    t->pre[k] = off;
+    if (k < d.D) off += align_up(d.TB * d.GH, ALIGN_F);
+  }
+  for (int k = 0; k < 2; ++k) {
+    t->preh[k] = off;
+    if (k < d.D && d.mode == B200RNN_GRU) off += align_up(d.TB * (size_t)d.H, ALIGN_F);
+  }
+  for (int k = 0; k < 2; ++k) {
+    t->ybuf[k] = off;
+    if (d.L > 1) off += align_up(d.TB * d.DH, ALIGN_F);
+  }
+  t->block = off;
+  t->total = align_up(t->tc_ws_bytes / sizeof(float) + 1, ALIGN_F) + (size_t)d.M * t->block;
+}
+
+B200RNN_API int b200rnn_tangent_workspace_bytes(const b200rnn_desc* desc, size_t* scratch_bytes) {
+  Dims d;
+  const int rc = check_tangent_desc(desc, &d);
+  if (rc) return rc;
+  TangentLayout tl;
+  make_tangent_layout(d, &tl);
+  if (scratch_bytes) *scratch_bytes = tl.total * sizeof(float);
+  return B200RNN_OK;
+}
+
+// Forward-mode AD of a saving forward (include/b200rnn.h). Per layer and direction: the tangent pre-activations by the
+// time-parallel GEMMs, W_ih x' + W_ih' x (+ W_hh' h_{t-1}, the primal output shifted by one step and h_0 for the first
+// step), then one tangent recurrence launch for every direction of the layer and every tangent direction, then the
+// primal's dropout mask on an inner layer's tangent output, which is the next layer's x'.
+B200RNN_API int b200rnn_forward_tangent(const b200rnn_desc* desc, const float* x, int64_t xs_t, int64_t xs_b,
+                                        const float* const* params, const float* y, int64_t ys_t, int64_t ys_b,
+                                        const float* h_0, const float* c_0, const void* reserve,
+                                        const int32_t* lengths, const float* x_dot, const float* const* params_dot,
+                                        const float* h_0_dot, const float* c_0_dot, float* y_dot, int64_t yds_t,
+                                        int64_t yds_b, float* h_n_dot, float* c_n_dot, void* scratch, void* stream_) {
+  if (lengths) {
+    set_error("forward_tangent: ragged batches (lengths) are not supported in forward mode");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  Dims d;
+  int rc = check_tangent_desc(desc, &d);
+  if (rc) return rc;
+  rc = check_initial_state(desc, h_0, c_0, c_0_dot, "forward_tangent");
+  if (rc) return rc;
+  if (!h_n_dot || !y_dot || (d.mode == B200RNN_LSTM && !c_n_dot) || (d.mode != B200RNN_LSTM && c_n_dot)) {
+    set_error("forward_tangent: y_dot and h_n_dot (and, for the LSTM only, c_n_dot) are required");
+    return B200RNN_ERR_INVALID;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const int M = d.M;  // tangent directions
+  const size_t nstate = (size_t)d.L * d.D * d.B * d.H;
+  if (d.B == 0 || d.T == 0) {  // no step: the final state's tangent is the initial one's
+    if (h_0_dot) B200_CUDA_CHECK(cudaMemcpyAsync(h_n_dot, h_0_dot, M * nstate * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    else B200_CUDA_CHECK(cudaMemsetAsync(h_n_dot, 0, M * nstate * sizeof(float), st));
+    if (c_n_dot) {
+      if (c_0_dot) B200_CUDA_CHECK(cudaMemcpyAsync(c_n_dot, c_0_dot, M * nstate * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      else B200_CUDA_CHECK(cudaMemsetAsync(c_n_dot, 0, M * nstate * sizeof(float), st));
+    }
+    return B200RNN_OK;
+  }
+  if (!x || !params || !y || !reserve || !scratch) {
+    set_error("forward_tangent: null pointer argument");
+    return B200RNN_ERR_INVALID;
+  }
+  if (!aligned_to(reserve, 256) || !aligned_to(scratch, 256)) {
+    set_error("forward_tangent: reserve/scratch must be 256-byte aligned");
+    return B200RNN_ERR_INVALID;
+  }
+  for (int i = 0; i < d.L * d.D * 4; ++i)
+    if (!params[i]) {
+      set_error("forward_tangent: null parameter pointer (index %d)", i);
+      return B200RNN_ERR_INVALID;
+    }
+  ReserveLayout rl;
+  rc = make_reserve(d, &rl);
+  if (rc) return rc;
+  TangentLayout tl;
+  make_tangent_layout(d, &tl);
+  const float* R = static_cast<const float*>(reserve);
+  float* const tc_ws = static_cast<float*>(scratch);
+  float* const S0 = tc_ws + align_up(tl.tc_ws_bytes / sizeof(float) + 1, ALIGN_F);  // direction 0's block
+  const size_t SS = tl.block;
+  const uint64_t* hdr = reinterpret_cast<const uint64_t*>(R);  // the primal's dropout seed / offset
+  const bool drop = d.training && d.p > 0.f && d.L > 1;
+  const bool tf32 = (desc->flags & B200RNN_FLAG_TF32) != 0;
+  const int TB = (int)d.TB, GH = (int)d.GH, H = d.H;
+  const bool gru = d.mode == B200RNN_GRU;
+  // an inner layer's tangent output, per tangent direction: two buffers of its block, layer l writing l & 1
+  const size_t* ybuf = tl.ybuf;
+  // C (+)= A W^T over the FFMA GEMM; `tc_ok`: the first (writing) GEMM of a buffer may take the tensor cores
+  auto gemm = [&](const float* A, RowMap a_rows, const float* W, float* C, int Mr, int N, int K, RowMap c_rows, int acc,
+                  bool tc_ok) {
+    GemmParams g;
+    memset(&g, 0, sizeof(g));
+    g.A = A; g.a_rows = a_rows; g.a_kcontig = 1;
+    g.B = W; g.b_rows = simple_rows(K); g.b_kcontig = 1;
+    g.C = C; g.c_rows = c_rows;
+    g.M = Mr; g.N = N; g.K = K;
+    g.accumulate = acc;
+    if (tc_ok && tc_available()) {
+      g.tc_ws = tc_ws;
+      g.tc_ws_bytes = tl.tc_ws_bytes;
+      g.tc_tf32 = tf32 ? 1 : 0;
+    }
+    return launch_gemm(g, nullptr, 0, st);
+  };
+  for (int l = 0; l < d.L; ++l) {
+    const int Il = l == 0 ? d.I : (int)d.DH;
+    const bool top = l == d.L - 1;
+    // the primal layer input and output, as the forward read and wrote them
+    const float* in = l == 0 ? x : R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);
+    const RowMap in_rows = l == 0 ? tb_rows(xs_t, xs_b, d.B) : simple_rows((long long)d.DH);
+    const float* out = top ? y : R + rl.ylayer[l];
+    const long long out_st = top ? ys_t : (long long)d.B * d.DH, out_sb = top ? ys_b : (long long)d.DH;
+    RecTanParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.mode = d.mode; rp.B = d.B; rp.T = d.T; rp.H = H; rp.D = d.D;
+    rp.y = out; rp.y_st = out_st; rp.y_sb = out_sb;
+    rp.h_0 = h_0 ? h_0 + (size_t)l * d.D * d.B * H : nullptr;
+    rp.c_0 = c_0 ? c_0 + (size_t)l * d.D * d.B * H : nullptr;
+    for (int m = 0; m < M; ++m) {
+      float* const S = S0 + m * SS;
+      // the tangent layer input x' (layer 0: the caller's dense [T,B,I] block, NULL = 0)
+      const float* in_dot = l == 0 ? (x_dot ? x_dot + (size_t)m * TB * d.I : nullptr) : S + ybuf[(l - 1) & 1];
+      for (int k = 0; k < d.D; ++k) {
+        const size_t pi = (size_t)(l * d.D + k) * 4;
+        const float* const* pp = params + pi;
+        const float* wih_d = params_dot && params_dot[pi] ? params_dot[pi] + (size_t)m * GH * Il : nullptr;
+        const float* whh_d = params_dot && params_dot[pi + 1] ? params_dot[pi + 1] + (size_t)m * GH * H : nullptr;
+        float* pre = S + tl.pre[k];
+        float* preh = S + tl.preh[k];
+        bool pre_init = false;
+        if (in_dot) {  // W_ih x'
+          rc = gemm(in_dot, simple_rows(Il), pp[0], pre, TB, GH, Il, simple_rows(GH), 0, true);
+          if (rc) return rc;
+          pre_init = true;
+        }
+        if (wih_d) {  // W_ih' x
+          rc = gemm(in, in_rows, wih_d, pre, TB, GH, Il, simple_rows(GH), pre_init, !pre_init);
+          if (rc) return rc;
+          pre_init = true;
+        }
+        if (whh_d) {
+          // W_hh' h_{t-1}: the primal output one step back (reverse: one step ahead) for every step but the first, h_0
+          // (or nothing) for the first. GRU: the r, z blocks into pre, the n block into preh (r multiplies it)
+          if (!pre_init) B200_CUDA_CHECK(cudaMemsetAsync(pre, 0, d.TB * d.GH * sizeof(float), st));
+          if (gru) B200_CUDA_CHECK(cudaMemsetAsync(preh, 0, d.TB * H * sizeof(float), st));
+          pre_init = true;
+          const float* hp = out + (long long)k * H + (k == 0 ? 0 : out_st);
+          const size_t c_row0 = k == 0 ? (size_t)d.B : 0;  // first C row the shifted GEMM writes
+          const int Mr = (d.T - 1) * d.B, nrz = gru ? 2 * H : GH;
+          const RowMap hp_rows = tb_rows(out_st, out_sb, d.B);
+          const float* h0k = rp.h_0 ? rp.h_0 + (size_t)k * d.B * H : nullptr;
+          const size_t first = (size_t)(k == 0 ? 0 : d.T - 1) * d.B;  // rows of the first scanned step
+          rc = gemm(hp, hp_rows, whh_d, pre + c_row0 * GH, Mr, nrz, H, simple_rows(GH), 1, false);
+          if (!rc && h0k) rc = gemm(h0k, simple_rows(H), whh_d, pre + first * GH, d.B, nrz, H, simple_rows(GH), 1, false);
+          if (!rc && gru) {
+            rc = gemm(hp, hp_rows, whh_d + (size_t)2 * H * H, preh + c_row0 * H, Mr, H, H, simple_rows(H), 1, false);
+            if (!rc && h0k)
+              rc = gemm(h0k, simple_rows(H), whh_d + (size_t)2 * H * H, preh + first * H, d.B, H, H, simple_rows(H), 1, false);
+          }
+          if (rc) return rc;
+        }
+        if (m > 0) continue;  // the launch takes direction 0's pointers and the strides below
+        rp.w_hh[k] = pp[1];
+        rp.gates[k] = R + rl.gates[l][k];
+        rp.extra[k] = is_elman(d.mode) ? nullptr : R + rl.extra[l][k];
+        rp.pre[k] = pre_init ? pre : nullptr;
+        rp.preh[k] = gru && whh_d ? preh : nullptr;
+        rp.bih_dot[k] = params_dot ? params_dot[pi + 2] : nullptr;
+        rp.bhh_dot[k] = params_dot ? params_dot[pi + 3] : nullptr;
+      }
+    }
+    rp.h0_dot = h_0_dot ? h_0_dot + (size_t)l * d.D * d.B * H : nullptr;
+    rp.c0_dot = c_0_dot ? c_0_dot + (size_t)l * d.D * d.B * H : nullptr;
+    if (top) {
+      rp.ydot = y_dot; rp.yd_st = yds_t; rp.yd_sb = yds_b; rp.m_ydot = (long long)(d.TB * d.DH);
+    } else {
+      rp.ydot = S0 + ybuf[l & 1]; rp.yd_st = (long long)d.B * d.DH; rp.yd_sb = (long long)d.DH; rp.m_ydot = (long long)SS;
+    }
+    rp.hn_dot = h_n_dot + (size_t)l * d.D * d.B * H;
+    rp.cn_dot = c_n_dot ? c_n_dot + (size_t)l * d.D * d.B * H : nullptr;
+    rp.m_pre = rp.m_preh = (long long)SS;
+    rp.m_bdot = GH;
+    rp.m_state = (long long)nstate;
+    rc = launch_rec_tangent(rp, M, st);
+    if (rc) return rc;
+    if (drop && !top)  // the primal's mask (same header, same stream id) on the tangent: the next layer's x'
+      for (int m = 0; m < M; ++m) {
+        float* yd = S0 + m * SS + ybuf[l & 1];
+        rc = launch_dropout(yd, yd, d.TB * d.DH, d.p, hdr, (uint32_t)l, st);
+        if (rc) return rc;
+      }
+  }
+  return B200RNN_OK;
+}
+
 B200RNN_API int b200rnn_cell_workspace_bytes(const b200rnn_cell_desc* desc, size_t* saved_bytes, size_t* scratch_bytes) {
   CellDims d;
   const int rc = check_cell_desc(desc, &d);

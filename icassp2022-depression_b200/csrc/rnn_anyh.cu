@@ -775,6 +775,129 @@ __global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh16_bwd_kernel(const RecBwd
 }
 
 // =================================================================================================
+// tangent (forward-mode AD)
+// =================================================================================================
+// The linearised forward: the same slice, staged W_hh rows, contraction and exchange as anyh_fwd_kernel, applied to the
+// tangent state h'_{t-1}; the cell is the linearised cell of rnn_cell.cuh at the primal's saved activations. Step t:
+// a = pre_t + b' + W_hh h'_{t-1} (GRU n block: pre_t is the x side, preh_t + b_hn' + W_hn h'_{t-1} the h side).
+// Cluster m / (D * nslices) is tangent direction m (mdl.M of them); the primal tensors are shared by all.
+// Shared memory: [W_s: G*n x (H+4), ONCHIP only] [h': 2 x BS x H] [bars: 2 x C]
+template <int MODE, bool ONCHIP>
+__global__ void __launch_bounds__(ANYH_MAX_NT, 1) anyh_tangent_kernel(const RecTanParams p, const int nslices, const RecModels mdl) {
+  constexpr int G = gates_of(MODE);
+  const int H = p.H, B = p.B, LD = H + 4, GH = G * H;
+  const bool relu = p.mode == B200RNN_RNN_RELU;  // Elman
+  const AnyhSlice s = anyh_slice<false>(p, nslices);
+  const int C = s.C, HS = s.HS, BS = s.BS, NT = s.NT, dir = s.dir, b0 = s.b0, j0 = s.j0, n = s.n, T = s.T;
+  const uint32_t rank = s.rank;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  float* W_s = reinterpret_cast<float*>(smem_raw);  // [G][n][LD]
+  float* h_s = W_s + (ONCHIP ? (size_t)G * HS * LD : 0);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(h_s + (size_t)2 * BS * H);
+  const int tid = threadIdx.x;
+  // the tangent direction of this cluster, and the offset of its block of a tangent tensor. The L2 tier, which has no
+  // register to spare in its step loop, forms the pointers from the launch registers at each use
+  const long long m = mdl.M > 1 ? anyh_model(p, nslices) : 0;
+  auto tan_ptr = [&](const float* base, long long stride) -> const float* {
+    if (!base) return nullptr;
+    if constexpr (ONCHIP) return base + m * stride;
+    return base + (mdl.M > 1 ? (long long)anyh_model(p, nslices) : 0ll) * stride;
+  };
+  const float* w_hh = p.w_hh[dir];
+  const float* h0_dot = p.h0_dot ? p.h0_dot + m * p.m_state : nullptr;
+  const float* c0_dot = p.c0_dot ? p.c0_dot + m * p.m_state : nullptr;
+
+  if (tid == 0) init_bars(bars, C);
+  if constexpr (ONCHIP) {
+    if constexpr (G == 1)
+      stage_rows(W_s, w_hh, n, H, NT, [&](int r) { return (size_t)(j0 + r) * H; });
+    else
+      stage_rows(W_s, w_hh, G * n, H, NT, [&](int r) { return ((size_t)(r / n) * H + j0 + r % n) * H; });
+  }
+  for (int i = tid; i < BS * H; i += NT) {  // buffer 0: h'_0 of the cluster's slots (zeros past the batch / without it)
+    const int q = i / H, k = i - q * H;
+    const int slot = b0 + q;
+    h_s[i] = (h0_dot && slot < B) ? h0_dot[((size_t)dir * B + slot) * H + k] : 0.f;
+  }
+  __syncthreads();
+  ptx::cluster_sync_all();  // peers' barriers are initialised before anyone sends
+
+  const int u = s.u, b = s.b, j = j0 + u, row = b0 + b;
+  const bool valid = s.active && row < B;
+  const size_t st0 = ((size_t)dir * B + row) * H + j;  // this thread's element of a [D,B,H] state
+  float hd = (h0_dot && valid) ? h0_dot[st0] : 0.f;
+  float cd = (MODE == B200RNN_LSTM && c0_dot && valid) ? c0_dot[st0] : 0.f;
+  // the primal state before the step: GRU h_{t-1}, LSTM c_{t-1}
+  const float* s0 = MODE == B200RNN_GRU ? p.h_0 : p.c_0;
+  float sp = (G > 1 && s0 && valid) ? s0[st0] : 0.f;
+  const size_t wg = ONCHIP ? (size_t)n * LD : (size_t)H * H;
+  const float* wrow = ONCHIP ? W_s + (size_t)u * LD : w_hh + (size_t)(j0 + u) * H;
+
+  for (int step = 0; step < T; ++step) {
+    const int t = dir ? T - 1 - step : step;
+    const int cur = step & 1, nxt = cur ^ 1;
+    // this step's saved activations and tangent pre-activations: loaded before the exchange wait, but in the
+    // L2 tier, which has no register to keep them through the contraction
+    float sv[G], sx = 0.f, a[G], ah = 0.f;
+    auto load_step = [&]() {
+      const size_t tb = (size_t)t * B + row;
+      const float* gates = p.gates[dir];
+      const float* pre = tan_ptr(p.pre[dir], p.m_pre);
+      const float* bih = tan_ptr(p.bih_dot[dir], p.m_bdot);
+      const float* bhh = tan_ptr(p.bhh_dot[dir], p.m_bdot);
+#pragma unroll
+      for (int g = 0; g < G; ++g) {
+        sv[g] = valid ? gates[tb * GH + g * H + j] : 0.f;
+        a[g] = (valid && pre) ? pre[tb * GH + g * H + j] : 0.f;
+        // the bias tangents, folded as the forward folds the biases (GRU: b_hn' on the h side); re-read every step
+        // from L1 rather than held in registers through the contraction
+        if (bih) a[g] += bih[g * H + j];
+        if (bhh && !(MODE == B200RNN_GRU && g == 2)) a[g] += bhh[g * H + j];
+      }
+      if constexpr (G > 1) sx = valid ? p.extra[dir][tb * H + j] : 0.f;
+      const float* preh = MODE == B200RNN_GRU ? tan_ptr(p.preh[dir], p.m_preh) : nullptr;
+      if (valid && preh) ah = preh[tb * H + j];
+      if (MODE == B200RNN_GRU && bhh) ah += bhh[2 * H + j];
+    };
+    constexpr bool LATE = !ONCHIP;
+    if constexpr (!LATE) load_step();
+    if (step > 0) wait_bars(bars, cur, C, rank, ((step - 1) >> 1) & 1);
+    if (tid == 0 && step + 1 < T) arm_bars(bars, nxt, s, H, 1);
+    float acc[G];
+#pragma unroll
+    for (int g = 0; g < G; ++g) acc[g] = 0.f;
+    dot_rows<G, ONCHIP, false>(wrow, wg, h_s + ((size_t)cur * BS + b) * H, 0, H, acc);
+    if constexpr (LATE) load_step();
+
+    float hdn;
+    if constexpr (MODE == B200RNN_GRU) {
+      const float ar[3] = {a[0] + acc[0], a[1] + acc[1], a[2]};
+      hdn = gru_cell_jvp(sv, sx, sp, ar, ah + acc[2], hd);
+      sp = valid ? p.y[(long long)t * p.y_st + (long long)row * p.y_sb + dir * H + j] : 0.f;  // h_t
+    } else if constexpr (MODE == B200RNN_LSTM) {
+      const float ar[4] = {a[0] + acc[0], a[1] + acc[1], a[2] + acc[2], a[3] + acc[3]};
+      hdn = lstm_cell_jvp(sv, sx, sp, ar, cd);
+      sp = sx;  // c_t
+    } else {
+      hdn = elman_cell_jvp(sv[0], a[0] + acc[0], relu);
+    }
+    hd = hdn;
+    if (valid) const_cast<float*>(tan_ptr(p.ydot, p.m_ydot))[(long long)t * p.yd_st + (long long)row * p.yd_sb + dir * H + j] = hdn;
+    if (step + 1 < T) {
+      float* h_nxt = h_s + (size_t)nxt * BS * H;
+      if (s.active) h_nxt[(size_t)b * H + j] = valid ? hdn : 0.f;
+      __syncthreads();  // the own slice is complete (and every thread is past step - 1's reads of buffer nxt)
+      send_slice(h_nxt, H, 1, H, s, &bars[nxt * C + rank]);
+    }
+  }
+  if (valid) {
+    p.hn_dot[m * p.m_state + st0] = hd;
+    if (MODE == B200RNN_LSTM && p.cn_dot) p.cn_dot[m * p.m_state + st0] = cd;
+  }
+  ptx::cluster_sync_all();  // nobody exits while a peer could still address its shared memory
+}
+
+// =================================================================================================
 // config choice
 // =================================================================================================
 }  // namespace
@@ -812,6 +935,15 @@ template <int MODE>
 AnyhKernel<RecFwdParams> anyh_kernel(const RecFwdParams&, bool vl, bool onchip) {
   return vl ? (onchip ? anyh_fwd_kernel<MODE, true, true> : anyh_fwd_kernel<MODE, true, false>)
             : (onchip ? anyh_fwd_kernel<MODE, false, true> : anyh_fwd_kernel<MODE, false, false>);
+}
+// the tangent recurrence: fp32 weight_hh and full-length rows only
+template <int MODE, typename WT>
+AnyhKernel<RecTanParams> anyh16_kernel(const RecTanParams&, bool, bool) {
+  return nullptr;
+}
+template <int MODE>
+AnyhKernel<RecTanParams> anyh_kernel(const RecTanParams&, bool, bool onchip) {
+  return onchip ? anyh_tangent_kernel<MODE, true> : anyh_tangent_kernel<MODE, false>;
 }
 // w16: the storage of weight_hh, DT_F32 or DT_F16 / DT_BF16 (h16.cuh)
 template <int MODE, typename P>
@@ -882,7 +1014,7 @@ int plan_anyh(const P& p, bool bwd, ClusterLaunch<P>* L, int w16, int models) {
       static const bool debug = getenv("B200RNN_DEBUG") != nullptr;
       if (debug)
         fprintf(stderr, "[b200rnn] %s %s cfg %s VL=%d H=%d C=%d BS=%d tier=%s%s: need %d clusters, capacity %d, smem %zu\n",
-                bwd ? "bwd" : "fwd", G == 1 ? "elman" : "anyh", mode_name(p.mode), (int)vl, H, pick.C, pick.BS,
+                __is_same(P, RecTanParams) ? "tan" : bwd ? "bwd" : "fwd", G == 1 ? "elman" : "anyh", mode_name(p.mode), (int)vl, H, pick.C, pick.BS,
                 onchip ? "smem" : "l2", wbytes == 2 ? " w_hh=16bit" : "", pick.nclusters, pick.capacity,
                 pick.smem);
       *L = pick;
@@ -904,6 +1036,14 @@ int plan_anyh_fwd(const RecFwdParams& p, RecFwdLaunch* L, int w16, int models) {
     return B200RNN_ERR_UNSUPPORTED;
   }
   return plan_anyh(p, false, L, w16, models);
+}
+
+int plan_anyh_tangent(const RecTanParams& p, RecTanLaunch* L, int directions) {
+  if (p.lengths) {
+    set_error("tangent recurrence: ragged batches (lengths) are not supported");
+    return B200RNN_ERR_UNSUPPORTED;
+  }
+  return plan_anyh(p, false, L, 0, directions);
 }
 
 int plan_anyh_bwd(const RecBwdParams& p, RecBwdLaunch* L, int w16, int models) {

@@ -80,4 +80,37 @@ __device__ __forceinline__ float elman_cell_bwd(float h, float dh, bool relu) {
   return relu ? (h > 0.f ? dh : 0.f) : dh * (1.f - h * h);
 }
 
+// ---- linearised cells (forward-mode AD): the tangent of a step from the saved activations, sigma' = s (1 - s),
+// tanh' = 1 - t^2, relu' = [h > 0]
+
+// The GRU cell: sv = (r, z, n), hn = W_hn h + b_hn, h_prev = h_{t-1}; a[0..1] the r, z pre-activation tangents, a[2] the
+// n block's x-side tangent, ahn the tangent of W_hn h + b_hn, hd the tangent of h_{t-1}. Returns the tangent of h_t.
+__device__ __forceinline__ float gru_cell_jvp(const float (&sv)[3], float hn, float h_prev, const float (&a)[3], float ahn,
+                                              float hd) {
+  const float r = sv[0], z = sv[1], n = sv[2];
+  const float dr = r * (1.f - r) * a[0];
+  const float dz = z * (1.f - z) * a[1];
+  const float dn = (1.f - n * n) * (a[2] + dr * hn + r * ahn);
+  return (1.f - z) * dn + z * hd + dz * (h_prev - n);
+}
+
+// The LSTM cell: sv = (i, f, g, o), c_t, c_prev = c_{t-1}; a the pre-activation tangents, cd the tangent of c_{t-1}.
+// Returns the tangent of h_t; cd becomes the tangent of c_t.
+__device__ __forceinline__ float lstm_cell_jvp(const float (&sv)[4], float c_t, float c_prev, const float (&a)[4],
+                                               float& cd) {
+  const float ig = sv[0], fg = sv[1], gg = sv[2], og = sv[3];
+  const float di = ig * (1.f - ig) * a[0];
+  const float df = fg * (1.f - fg) * a[1];
+  const float dg = (1.f - gg * gg) * a[2];
+  const float dout = og * (1.f - og) * a[3];
+  cd = df * c_prev + fg * cd + di * gg + ig * dg;
+  const float tc = tanh_f(c_t);
+  return dout * tc + og * (1.f - tc * tc) * cd;
+}
+
+// The Elman cell: from the saved output h and the pre-activation tangent a, the tangent of h
+__device__ __forceinline__ float elman_cell_jvp(float h, float a, bool relu) {
+  return relu ? (h > 0.f ? a : 0.f) : a * (1.f - h * h);
+}
+
 }  // namespace b200rnn

@@ -112,6 +112,36 @@ struct RecBwdParams {
 };
 using RecBwdLaunch = ClusterLaunch<RecBwdParams>;
 
+// The tangent recurrence of one layer (forward-mode AD, anyh_tangent_kernel): from the primal's saved gates, the tangent
+// pre-activations and the tangent initial state, the tangent output. Launched like the runtime-sized forward (plan_anyh's
+// shapes, W_hh rows staged or read from L2); M tangent directions run in one launch, clusters direction-major, each
+// direction's tangent tensors at m times their stride below while every primal tensor is shared.
+struct RecTanParams {
+  int mode, B, T, H, D;
+  const int* lengths;        // always NULL (forward mode takes no ragged batch): the slice code reads them
+  const int* order;
+  const float* w_hh[2];      // primal weight_hh per direction [G*H, H]
+  const float* gates[2];     // the primal's saved activated gates [T,B,G*H] (Elman: h_t)
+  const float* extra[2];     // ... and GRU W_hn h + b_hn / LSTM c_t [T,B,H] (Elman: NULL)
+  const float* y;            // the primal layer output h_t (GRU: h_{t-1} of the next step), strided
+  long long y_st, y_sb;
+  const float* h_0;          // primal initial states [D,B,H] or NULL (zeros)
+  const float* c_0;
+  const float* pre[2];       // per direction [T,B,G*H] or NULL (0): W_ih x' + W_ih' x (+ W_hh' h_{t-1}, GRU r,z only)
+  const float* preh[2];      // GRU, per direction [T,B,H] or NULL (0): W_hn' h_{t-1}
+  const float* bih_dot[2];   // per direction [G*H] or NULL: tangents of bias_ih / bias_hh
+  const float* bhh_dot[2];
+  const float* h0_dot;       // [D,B,H] or NULL: tangents of the initial states
+  const float* c0_dot;
+  float* ydot;               // tangent output, element (t,b,d*H+j) at t*yd_st + b*yd_sb + d*H + j
+  long long yd_st, yd_sb;
+  float* hn_dot;             // [D,B,H]
+  float* cn_dot;             // [D,B,H] (LSTM) or NULL
+  // the stride of tangent direction m's block of each tangent tensor (elements); every primal tensor is shared
+  long long m_pre, m_preh, m_bdot, m_ydot, m_state;
+};
+using RecTanLaunch = ClusterLaunch<RecTanParams>;
+
 constexpr int MAX_SMEM = 232448;  // 227 KB opt-in limit per CTA on sm_90
 
 // number of batch slices the launcher will use for this shape (needed to size dbias_part)
@@ -160,5 +190,9 @@ int prep_whh_h16(const float* w_hh, void* img, cudaStream_t stream);
 int plan_rec_bwd(const RecBwdParams& p, RecBwdLaunch* out, int w16 = 0, int models = 1);
 int launch_rec_bwd(RecBwdParams& p, cudaStream_t stream, int w16 = 0, const void* const* whh16 = nullptr,
                    const RecModels* models = nullptr);
+// the tangent recurrence (rnn_anyh.cu) at every hidden size anyh_hidden_size takes, for `directions` tangent directions
+// in one launch: plan, then launch
+int plan_anyh_tangent(const RecTanParams& p, RecTanLaunch* out, int directions);
+int launch_rec_tangent(const RecTanParams& p, int directions, cudaStream_t stream);
 
 }  // namespace b200rnn

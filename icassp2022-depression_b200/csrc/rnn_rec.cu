@@ -1975,6 +1975,14 @@ int launch_rec_fwd(const RecFwdLaunch& L, const RecFwdParams& p, cudaStream_t s)
   return launch_clustered(L, p, PROF_REC_FWD, p.ready != nullptr, s);
 }
 
+int launch_rec_tangent(const RecTanParams& p, int directions, cudaStream_t s) {
+  if (p.B <= 0 || p.T <= 0) return B200RNN_OK;
+  RecTanLaunch L;
+  const int rc = plan_anyh_tangent(p, &L, directions);
+  if (rc != B200RNN_OK) return rc;
+  return launch_clustered(L, p, PROF_REC_FWD, false, s);
+}
+
 namespace {
 
 // The backward's W_hh for a C-CTA cluster, transposed and contiguous per CTA: CTA r's block starts at G * j0_r * H and

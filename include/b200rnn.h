@@ -270,6 +270,34 @@ B200RNN_API int b200rnn_backward_hx(const b200rnn_desc* desc, const float* x, in
                                     const int32_t* lengths, void* stream /* cudaStream_t */);
 
 /*
+ * Forward-mode AD (a Jacobian-vector product) of a forward that saved for backward: what torch.func.jvp and
+ * torch.autograd.forward_ad compute through nn.GRU / nn.LSTM / nn.RNN. desc, x, params, y, h_0 / c_0 and reserve are
+ * those of a b200rnn_forward_hx call made with B200RNN_FLAG_SAVE_FOR_BACKWARD (desc without B200RNN_FLAG_MODELS; same
+ * dropout mask: the reserve holds it). The tangents, each NULL = zero (its GEMM is skipped):
+ *   x_dot       [T,B,I] dense
+ *   params_dot  NULL, or 4*L*D pointers shaped like params, each NULL or the parameter's tangent
+ *   h_0_dot, c_0_dot  [L*D,B,H] (c_0_dot LSTM only)
+ * and the outputs:
+ *   y_dot       [T,B,D*H] addressed as y_dot[t*y_dot_stride_t + b*y_dot_stride_b + c]
+ *   h_n_dot, c_n_dot  [L*D,B,H] contiguous (c_n_dot LSTM only, else NULL)
+ * Several tangent directions over one primal (torch.func.jacfwd): desc with B200RNN_FLAG_MODELS and models = M
+ * (model_strides is required but not read); every tangent input and output is then M dense blocks of its one-direction
+ * size (y_dot's block T*B*D*H, strided inside as given), and each recurrence layer runs all of them in one launch.
+ * scratch: b200rnn_tangent_workspace_bytes(desc) bytes, 256-byte aligned (one GEMM workspace shared by the call, then
+ * per tangent direction its tangent pre-activations and inner-layer outputs). Returns B200RNN_ERR_UNSUPPORTED, before
+ * any launch, for proj_size, B200RNN_FLAG_F16 / _BF16 / _F32_PARAMS, B200RNN_FLAG_FUSED_LN and lengths (which must be
+ * NULL).
+ */
+B200RNN_API int b200rnn_tangent_workspace_bytes(const b200rnn_desc* desc, size_t* scratch_bytes);
+B200RNN_API int b200rnn_forward_tangent(const b200rnn_desc* desc, const float* x, int64_t x_stride_t,
+                                        int64_t x_stride_b, const float* const* params, const float* y,
+                                        int64_t y_stride_t, int64_t y_stride_b, const float* h_0, const float* c_0,
+                                        const void* reserve, const int32_t* lengths, const float* x_dot,
+                                        const float* const* params_dot, const float* h_0_dot, const float* c_0_dot,
+                                        float* y_dot, int64_t y_dot_stride_t, int64_t y_dot_stride_b, float* h_n_dot,
+                                        float* c_n_dot, void* scratch, void* stream /* cudaStream_t */);
+
+/*
  * Backward with the model-shell fusions of the TRAINING path (SURVEY.md 8f rank 1; audio_gru_whole.py:103-108 with
  * loss.backward() at :190): b200rnn_backward plus
  *   dy_pool / dy_pool_scale : when dy == NULL the top layer's output gradient is dy_pool[b, c] * dy_pool_scale for
