@@ -1758,14 +1758,18 @@ B200RNN_API int b200rnn_forward_tangent(const b200rnn_desc* desc, const float* x
   if (rc) return rc;
   rc = check_initial_state(desc, h_0, c_0, c_0_dot, "forward_tangent");
   if (rc) return rc;
-  if (!h_n_dot || !y_dot || (d.mode == B200RNN_LSTM && !c_n_dot) || (d.mode != B200RNN_LSTM && c_n_dot)) {
+  // an output with no element may be NULL (an empty tensor's data pointer): y_dot when B == 0 or T == 0, the states'
+  // tangents when B == 0
+  const bool empty = d.B == 0 || d.T == 0, lstm = d.mode == B200RNN_LSTM;
+  if ((!empty && !y_dot) || (d.B > 0 && (!h_n_dot || (lstm && !c_n_dot))) || (!lstm && c_n_dot)) {
     set_error("forward_tangent: y_dot and h_n_dot (and, for the LSTM only, c_n_dot) are required");
     return B200RNN_ERR_INVALID;
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const int M = d.M;  // tangent directions
   const size_t nstate = (size_t)d.L * d.D * d.B * d.H;
-  if (d.B == 0 || d.T == 0) {  // no step: the final state's tangent is the initial one's
+  if (empty) {  // no step: the final state's tangent is the initial one's
+    if (nstate == 0) return B200RNN_OK;
     if (h_0_dot) B200_CUDA_CHECK(cudaMemcpyAsync(h_n_dot, h_0_dot, M * nstate * sizeof(float), cudaMemcpyDeviceToDevice, st));
     else B200_CUDA_CHECK(cudaMemsetAsync(h_n_dot, 0, M * nstate * sizeof(float), st));
     if (c_n_dot) {

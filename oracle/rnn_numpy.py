@@ -198,6 +198,105 @@ def elman_step(x, h, w_ih, w_hh, b_ih, b_hh, nonlinearity="tanh"):
     return np.tanh(a), 1.0 + mag
 
 
+# ---- linearised single steps (forward-mode AD) in float64, with the magnitude each tangent is computed from ---------
+# Each takes the primal (x, h[, c], W_ih, W_hh, b_ih, b_hh) and the tangents (x', h'[, c'], W_ih', W_hh', b_ih', b_hh'),
+# any tangent None = 0, and returns the tangent of the new state and, per element, a magnitude S' for the bound
+#   |h'_kernel - h'_64| <= KAPPA_T u S'        (tests/test_gpu_jvp_numerics_f64.py derives KAPPA_T)
+# S' = R + S Q covers both error sources of a kernel that applies the linearised cell at its own saved activations:
+#   R  the rounding of the tangent itself: per gate row the magnitude M of the tangent pre-activation
+#      |W_ih| |x'| + |W_ih'| |x| + |W_hh| |h'| + |W_hh'| |h| + |b_ih'| + |b_hh'| (the GRU's n block: x side and h side
+#      separately), each row weighted by max(1, |d state' / d row|) - the r row of the GRU is scaled by r (1 - r) |hn|,
+#      the f row of the LSTM by f (1 - f) |c_prev|, either of which can exceed 1 - plus the products the linearised
+#      cell adds up (GRU |(1 - z) dn|, |z h'|, |dz (h - n)|, |dr hn|, |(1 - z) (n's tangent pre-activation)|; LSTM
+#      |df c|, |f c'|, |di g|, |i dg|, |do tanh c|, |o c'_t|);
+#   S Q the primal's own error: the saved activations (gates, GRU hn, LSTM c_t) lie within the primal step's bound
+#      KAPPA u S (gru_step / lstm_step / elman_step) of float64, and Q is the sum over those saved values of the
+#      magnitude of the tangent's partial derivative with respect to each, so S Q bounds what that error moves the
+#      tangent by (KAPPA <= KAPPA_T, so KAPPA_T u S' covers KAPPA u S Q).
+
+def _dots(tangents, like):
+    return [np.zeros_like(v) if t is None else np.asarray(t, dtype=np.float64) for t, v in zip(tangents, like)]
+
+
+def _pre_jvp(x, h, w_ih, w_hh, xd, hd, wid, whd, bid, bhd):
+    """the x-side and h-side tangent pre-activations [B, G*H] and their magnitudes"""
+    ai = xd @ w_ih.T + x @ wid.T + bid
+    ah = hd @ w_hh.T + h @ whd.T + bhd
+    mi = np.abs(xd) @ np.abs(w_ih).T + np.abs(x) @ np.abs(wid).T + np.abs(bid)
+    mh = np.abs(hd) @ np.abs(w_hh).T + np.abs(h) @ np.abs(whd).T + np.abs(bhd)
+    return ai, ah, mi, mh
+
+
+def gru_step_jvp(x, h, w_ih, w_hh, b_ih, b_hh, xd=None, hd=None, w_ihd=None, w_hhd=None, b_ihd=None, b_hhd=None):
+    """x [B,I], h [B,H] and their tangents -> (h'_t [B,H], S' [B,H])"""
+    x, h, w_ih, w_hh, b_ih, b_hh = _f64(x, h, w_ih, w_hh, b_ih, b_hh)
+    xd, hd, wid, whd, bid, bhd = _dots((xd, hd, w_ihd, w_hhd, b_ihd, b_hhd), (x, h, w_ih, w_hh, b_ih, b_hh))
+    H = h.shape[1]
+    gi, gh = x @ w_ih.T + b_ih, h @ w_hh.T + b_hh
+    r = _sigmoid(gi[:, :H] + gh[:, :H])
+    z = _sigmoid(gi[:, H:2 * H] + gh[:, H:2 * H])
+    hn = gh[:, 2 * H:]
+    n = np.tanh(gi[:, 2 * H:] + r * hn)
+    _, S = gru_step(x, h, w_ih, w_hh, b_ih, b_hh)
+    ai, ah, mi, mh = _pre_jvp(x, h, w_ih, w_hh, xd, hd, wid, whd, bid, bhd)
+    a_r, a_z = ai[:, :H] + ah[:, :H], ai[:, H:2 * H] + ah[:, H:2 * H]
+    a_n, a_hn = ai[:, 2 * H:], ah[:, 2 * H:]
+    dr, dz = r * (1 - r) * a_r, z * (1 - z) * a_z
+    inner = a_n + dr * hn + r * a_hn
+    dn = (1 - n * n) * inner
+    hdot = (1 - z) * dn + z * hd + dz * (h - n)
+    m = mi + mh
+    R = (m[:, :H] * np.maximum(1.0, r * (1 - r) * np.abs(hn)) + m[:, H:2 * H] + mi[:, 2 * H:] + mh[:, 2 * H:]
+         + np.abs((1 - z) * dn) + np.abs(z * hd) + np.abs(dz * (h - n)) + np.abs(dr * hn) + np.abs((1 - z) * inner))
+    Q = (np.abs(a_r) * np.abs(hn) + np.abs(a_hn)                          # r
+         + np.abs(dn) + np.abs(hd) + np.abs(a_z) * np.abs(h - n)           # z
+         + 2 * np.abs(inner) + np.abs(dz)                                   # n
+         + np.abs(dr))                                                      # hn
+    return hdot, R + S * Q
+
+
+def lstm_step_jvp(x, h, c, w_ih, w_hh, b_ih, b_hh, xd=None, hd=None, cd=None, w_ihd=None, w_hhd=None, b_ihd=None,
+                  b_hhd=None):
+    """x [B,I], h [B,H], c [B,H] and their tangents -> (h'_t, c'_t, S'_h, S'_c), each [B,H]"""
+    x, h, c, w_ih, w_hh, b_ih, b_hh = _f64(x, h, c, w_ih, w_hh, b_ih, b_hh)
+    xd, hd, cd, wid, whd, bid, bhd = _dots((xd, hd, cd, w_ihd, w_hhd, b_ihd, b_hhd), (x, h, c, w_ih, w_hh, b_ih, b_hh))
+    H = c.shape[1]
+    a = x @ w_ih.T + h @ w_hh.T + b_ih + b_hh
+    i, f, g, o = _sigmoid(a[:, :H]), _sigmoid(a[:, H:2 * H]), np.tanh(a[:, 2 * H:3 * H]), _sigmoid(a[:, 3 * H:])
+    c_new = f * c + i * g
+    tc = np.tanh(c_new)
+    _, _, _, S = lstm_step(x, h, c, w_ih, w_hh, b_ih, b_hh)
+    ai, ah, mi, mh = _pre_jvp(x, h, w_ih, w_hh, xd, hd, wid, whd, bid, bhd)
+    ad, m = ai + ah, mi + mh
+    di, df = i * (1 - i) * ad[:, :H], f * (1 - f) * ad[:, H:2 * H]
+    dg, do = (1 - g * g) * ad[:, 2 * H:3 * H], o * (1 - o) * ad[:, 3 * H:]
+    cdot = df * c + f * cd + di * g + i * dg
+    hdot = do * tc + o * (1 - tc * tc) * cdot
+    rows = (m[:, :H] + m[:, H:2 * H] * np.maximum(1.0, f * (1 - f) * np.abs(c)) + m[:, 2 * H:3 * H] + m[:, 3 * H:])
+    R_c = rows + np.abs(df * c) + np.abs(f * cd) + np.abs(di * g) + np.abs(i * dg)
+    R_h = R_c + np.abs(do * tc) + np.abs(o * cdot)
+    Q_c = (np.abs(ad[:, :H] * g) + np.abs(dg)                               # i
+           + np.abs(ad[:, H:2 * H] * c) + np.abs(cd)                        # f
+           + np.abs(di) + 2 * np.abs(i * g * ad[:, 2 * H:3 * H]))           # g
+    Q_h = (Q_c + np.abs(ad[:, 3 * H:] * tc) + np.abs(cdot)                  # o
+           + np.abs(do) + 2 * np.abs(o * cdot))                             # c_t
+    return hdot, cdot, R_h + S * Q_h, R_c + S * Q_c
+
+
+def elman_step_jvp(x, h, w_ih, w_hh, b_ih, b_hh, xd=None, hd=None, w_ihd=None, w_hhd=None, b_ihd=None, b_hhd=None,
+                   nonlinearity="tanh"):
+    """x [B,I], h [B,H] and their tangents -> (h'_t [B,H], S' [B,H]). relu: the tangent is a' where a > 0, exact
+    there, so S' carries no primal term (the branch is the precondition the caller checks)."""
+    x, h, w_ih, w_hh, b_ih, b_hh = _f64(x, h, w_ih, w_hh, b_ih, b_hh)
+    xd, hd, wid, whd, bid, bhd = _dots((xd, hd, w_ihd, w_hhd, b_ihd, b_hhd), (x, h, w_ih, w_hh, b_ih, b_hh))
+    h_new, S = elman_step(x, h, w_ih, w_hh, b_ih, b_hh, nonlinearity)
+    ai, ah, mi, mh = _pre_jvp(x, h, w_ih, w_hh, xd, hd, wid, whd, bid, bhd)
+    ad, m = ai + ah, mi + mh
+    if nonlinearity == "relu":
+        return np.where(h_new > 0, ad, 0.0), m
+    return (1 - h_new * h_new) * ad, m + S * 2 * np.abs(ad)
+
+
 class NumpyRNN:
     """Multi-layer (bi)directional GRU/LSTM, time-major [T,B,*], with an explicit backward."""
 

@@ -47,6 +47,9 @@ CELL_EXISTING = ["tests/test_gpu_cells.py", "tests/test_gpu_elman.py"]
 # in its lists (five of them inside the span of any view, whatever holds it), not only for the tests a run with
 # --new-maxfail happens to reach
 STRIDED_NEW = ["tests/test_gpu_strided_io.py"]
+# forward-mode AD: the tangent GEMMs (api.cu b200rnn_forward_tangent), anyh_tangent_kernel and the linearised cells
+JVP_NEW = ["tests/test_gpu_jvp_numerics_f64.py"]
+JVP_EXISTING = ["tests/test_gpu_jvp.py"]
 # tf32(v): v with its 13 low mantissa bits cleared, the operand precision of a single-pass TF32 product
 _TF32 = "__uint_as_float(__float_as_uint({}) & 0xffffe000u)"
 
@@ -232,6 +235,37 @@ MUTATIONS = {
                              "    dst[i] = t < lengths[b] ? src[(size_t)r * C + c] : 0.f;\n",
                              "ragged backward: the padding-zeroed copy of x reads row r at r * C, ignoring x's strides",
                              STRIDED_NEW, ["tests/test_gpu_varlen.py"]),
+    # forward-mode AD. The stride mutations make every tangent direction read (or, in the L2 tier, also write) direction
+    # 0's block of a tangent tensor: in bounds, since direction 0's block is the first of each allocation
+    "jvp_gru_drop_dr_hn": ("rnn_cell.cuh", "const float dn = (1.f - n * n) * (a[2] + dr * hn + r * ahn);",
+                           "const float dn = (1.f - n * n) * (a[2] + r * ahn);",
+                           "GRU tangent: the candidate gate loses the dr * hn term", JVP_NEW, JVP_EXISTING),
+    "jvp_lstm_drop_df_c": ("rnn_cell.cuh", "  cd = df * c_prev + fg * cd + di * gg + ig * dg;\n",
+                           "  cd = fg * cd + di * gg + ig * dg;\n",
+                           "LSTM tangent: the cell tangent loses df * c_prev", JVP_NEW, JVP_EXISTING),
+    "jvp_drop_bhn_h_side": ("rnn_anyh.cu", "      if (MODE == B200RNN_GRU && bhh) ah += bhh[2 * H + j];\n", "",
+                            "GRU tangent: b_hn' is left off the h side", JVP_NEW, JVP_EXISTING),
+    "jvp_send_tf32": ("rnn_anyh.cu", "      if (s.active) h_nxt[(size_t)b * H + j] = valid ? hdn : 0.f;\n",
+                      "      if (s.active) h_nxt[(size_t)b * H + j] = valid ? " + _TF32.format("hdn") + " : 0.f;\n",
+                      "tangent recurrence: the tangent state sent to the cluster is rounded to TF32", JVP_NEW,
+                      JVP_EXISTING),
+    # the first occurrence is the backward's gradient-GEMM descriptor
+    "jvp_gemm_tf32": ("api.cu", "      g.tc_tf32 = tf32 ? 1 : 0;\n", "      g.tc_tf32 = 1;\n",
+                      "tangent GEMMs: single-pass TF32 whatever torch's setting", JVP_NEW, JVP_EXISTING, 1),
+    "jvp_m_bdot_zero": ("api.cu", "    rp.m_bdot = GH;\n", "    rp.m_bdot = 0;\n",
+                        "batched tangents: every direction reads direction 0's bias tangents", JVP_NEW, JVP_EXISTING),
+    "jvp_m_preh_zero": ("api.cu", "    rp.m_pre = rp.m_preh = (long long)SS;\n",
+                        "    rp.m_pre = (long long)SS;\n    rp.m_preh = 0;\n",
+                        "batched tangents: every direction reads direction 0's GRU W_hn' h side", JVP_NEW, JVP_EXISTING),
+    "jvp_h0_dot_direction0": ("rnn_anyh.cu",
+                              "  const float* h0_dot = p.h0_dot ? p.h0_dot + m * p.m_state : nullptr;\n",
+                              "  const float* h0_dot = p.h0_dot ? p.h0_dot : nullptr;\n",
+                              "batched tangents: every direction starts from direction 0's h_0'", JVP_NEW, JVP_EXISTING),
+    "jvp_l2_tan_ptr_direction0": ("rnn_anyh.cu",
+                                  "    return base + (mdl.M > 1 ? (long long)anyh_model(p, nslices) : 0ll) * stride;\n",
+                                  "    return base;\n",
+                                  "batched tangents, L2 tier: every direction reads and writes direction 0's blocks",
+                                  JVP_NEW, JVP_EXISTING),
 }
 
 
