@@ -50,6 +50,11 @@ STRIDED_NEW = ["tests/test_gpu_strided_io.py"]
 # forward-mode AD: the tangent GEMMs (api.cu b200rnn_forward_tangent), anyh_tangent_kernel and the linearised cells
 JVP_NEW = ["tests/test_gpu_jvp_numerics_f64.py"]
 JVP_EXISTING = ["tests/test_gpu_jvp.py"]
+# stacked calls: what only layers l > 0 run (api.cu forward and backward layer loops)
+STACK_NEW = ["tests/test_gpu_stacked_f64.py"]
+STACK_EXISTING = ["tests/test_gpu_parity.py", "tests/test_gpu_proj.py", "tests/test_gpu_any_hidden.py",
+                  "tests/test_gpu_elman.py", "tests/test_gpu_initial_state.py", "tests/test_gpu_shell_f64.py",
+                  "tests/test_gpu_h16_modules.py"]
 # tf32(v): v with its 13 low mantissa bits cleared, the operand precision of a single-pass TF32 product
 _TF32 = "__uint_as_float(__float_as_uint({}) & 0xffffe000u)"
 
@@ -266,6 +271,32 @@ MUTATIONS = {
                                   "    return base;\n",
                                   "batched tangents, L2 tier: every direction reads and writes direction 0's blocks",
                                   JVP_NEW, JVP_EXISTING),
+    # stacked calls. The edits change a precision flag, drop a launch, pick the other of two reserve regions of the
+    # same size, or overwrite instead of accumulate: every access stays where the unmutated one goes
+    "stack_inner_dx_tf32": ("api.cu", '"dX"}, sl,\n                             S, tf32, st);',
+                            '"dX"}, sl,\n                             S, tf32 || l > 0, st);',
+                            "backward of layers l > 0: the dX GEMM (the dy of the layer below) runs single-pass TF32 "
+                            "in 3xTF32 mode", STACK_NEW, STACK_EXISTING),
+    "stack_inner_xproj_tf32": ("api.cu", "            g.tc_tf32 = tf32 ? 1 : 0;\n",
+                               "            g.tc_tf32 = (tf32 || l > 0) ? 1 : 0;\n",
+                               "forward of layers l > 0: the tensor-core x-projection runs single-pass TF32 in 3xTF32 "
+                               "mode", STACK_NEW, STACK_EXISTING),
+    "stack_no_inner_dropout_bwd": ("api.cu",
+                                   "        rc = launch_dropout(S + sl.b_dy, S + sl.b_dy, d.TB * d.DH, d.p, hdr, "
+                                   "(uint32_t)(l - 1), st);\n",
+                                   "        (void)hdr;\n",
+                                   "backward: the gradient through the inter-layer dropout is not masked", STACK_NEW,
+                                   STACK_EXISTING),
+    "stack_dw_ih_undropped": ("api.cu",
+                              "X.p = layer_in ? layer_in[l - 1] : R + (drop ? rl.ydrop[l - 1] : rl.ylayer[l - 1]);",
+                              "X.p = layer_in ? layer_in[l - 1] : R + rl.ylayer[l - 1];",
+                              "backward: dW_ih of layer l reads layer l - 1's output before its dropout", STACK_NEW,
+                              STACK_EXISTING),
+    "stack_inner_dx_second_dir_overwrites": ("api.cu",
+                                             "TB, Il, GH, Cx, cx_rows, k > 0, false, tc_dx, \"dX\"}",
+                                             "TB, Il, GH, Cx, cx_rows, k > 0 && l == 0, false, tc_dx, \"dX\"}",
+                                             "backward of layers l > 0: the reverse direction's dX overwrites the dy of "
+                                             "the layer below instead of adding to it", STACK_NEW, STACK_EXISTING),
 }
 
 
